@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — sequences/sec for ESM-2 650M bulk embedding extraction at L=1024 (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a (H100) path
     python bench.py --impl reference --steps K --warmup W     # the reference algorithm on the host CPU cores
 
 A "step" is one pass of the hot path (embed -> 33 x TransformerLayer -> final LayerNorm -> per-sequence mean, and for
@@ -16,14 +16,17 @@ padding, generator seed 1234), seeded random-init weights (checkpoints are unrea
            in pinned HOST memory, per-token [B,T,E] fp32 and per-sequence mean representations end in pinned HOST
            memory; H2D and D2H copies are inside the timed region.
 `kernels` / `roofline`: a separate pass of the same step with every launch bracketed by CUDA events on the launch
-           stream (esmb200_profile_enable); the dominant kernel against the measured cuBLAS bf16 peak in
-           MEASURED_PEAKS.json.
+           stream (esmb200_profile_enable); the dominant kernel against the bf16 peak in MEASURED_PEAKS.json when that
+           file is present, else the H100 SXM data-sheet figures (dense bf16, HBM3).
+`--dump-outputs DIR`: after the timed steps, the per-sequence mean representations the last timed step returned are
+           written as DIR/mean.npy (float32 [batch, 1280]; above 64 MB a fixed seeded sample of the rows); tokens and
+           weights are seeded, so two builds can be compared output for output.
 `configs`: BASELINE.json configs[3] (3B, L=512, contacts) and configs[4] (MSA Transformer, 128 x 512 MSA), N=1 only.
-`gpu_eager_baseline`: the UNMODIFIED reference (baseline/_ref, else the oracle port: same ATen ops) in eager fp32 on
+`gpu_eager_baseline`: the UNMODIFIED reference (oracle/_ref, else the oracle port: same ATen ops) in eager fp32 on
            the same GPU — what scripts/extract.py:70-72 gives a user today.
 `cpu_baseline`: the reference on the box's host cores, on a bounded sample (N=1, rank 0 only): the unmodified
-           reference when baseline/_ref is present (kind "reference"), else the oracle port (kind "port").
-Only the baseline legs and --impl reference import oracle/ or baseline/_ref; the product path never does.
+           reference when oracle/_ref is present (kind "reference"), else the oracle port (kind "port").
+Only the baseline legs and --impl reference import oracle/ (and oracle/_ref); the product path never does.
 """
 from __future__ import annotations
 
@@ -45,6 +48,7 @@ sys.path.insert(0, ROOT)
 MODEL = "esm2_t33_650M_UR50D"
 L_LAYERS, E, H, F = 33, 1280, 20, 5120
 GLOBAL_BATCH, SEQ_LEN = 256, 1024
+DUMP_LIMIT_BYTES = 64 << 20  # --dump-outputs writes at most this much
 TAGS = ["ln1_f16", "gemm_qkv_rope", "attention", "gemm_out_residual", "ln2_f16", "gemm_fc1_gelu", "gemm_fc2_residual",
         "key_bits", "embed", "layernorm_f32", "attention_probs", "convert", "gemm_other", "mean_pool",
         "tied_row_logits", "tied_row_softmax", "tied_row_update"]
@@ -69,11 +73,12 @@ def measured_peaks():
         d = json.load(open(path))
         return {"tensor_burst": d["bf16_tflops"], "tensor_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "hbm": d["hbm_gbs"], "source": "MEASURED_PEAKS.json (of measured)"}
-    return {"tensor_burst": 1590.0, "tensor_sustained": 1400.0, "hbm": 6650.0, "source": "B200_PROFILING.md (of fallback)"}
+    return {"tensor_burst": 989.0, "tensor_sustained": 989.0, "hbm": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense bf16, HBM3; not measured)"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -105,8 +110,8 @@ class ClockSampler(threading.Thread):
 
 
 def import_reference():
-    """The unmodified reference package from baseline/_ref (offline `pip install --target`, DESIGN.md §6) or None."""
-    ref = os.path.join(ROOT, "baseline", "_ref")
+    """The unmodified reference package from oracle/_ref (made by build(), oracle/reference.py) or None."""
+    ref = os.path.join(ROOT, "oracle", "_ref")
     if not os.path.isdir(os.path.join(ref, "esm")):
         return None
     if ref not in sys.path:
@@ -154,7 +159,7 @@ class RefRunner:
 
 def pick_cpu_threads(runner, T=SEQ_LEN):
     """All host threads are available to the CPU arm; PyTorch's intra-op scaling is not monotonic on many-core hosts
-    (on the 128-thread B200 host 128 threads run this model SLOWER than 32), so time one TransformerLayer per candidate
+    (on large hosts all threads can run this model SLOWER than 32), so time one TransformerLayer per candidate
     count and keep the fastest — the reference gets its best configuration."""
     ncpu = os.cpu_count() or 1
     cands = sorted({c for c in (8, 16, 32, 64, ncpu // 2, ncpu) if 1 <= c <= ncpu})
@@ -209,7 +214,7 @@ def gpu_eager_reference(state_dict, dev, n_seq=8, reps=2, T=SEQ_LEN):
         torch.cuda.empty_cache()
         return {"value": round(n_seq / ms * 1e3, 3), "unit": "sequences/s", "kind": "reference" if import_reference() else "port",
                 "dtype": "f32 (TF32 off)", "sample": f"{n_seq} of the {GLOBAL_BATCH} sequences (L={T}) per pass, eager "
-                f"PyTorch {torch.__version__} on the same B200, {ms:.1f} ms per pass"}
+                f"PyTorch {torch.__version__} on the same GPU, {ms:.1f} ms per pass"}
     finally:
         torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
 
@@ -223,7 +228,7 @@ def run_reference(args):
     sd = {k: v.detach() for k, v in model.state_dict().items()}
     n_seq = args.ref_seqs
     v, ms, cores, kind = cpu_reference_seq_per_s(sd, n_seq, args.steps, args.warmup)
-    impl = "the unmodified reference (baseline/_ref)" if kind == "reference" else "the oracle port of the reference"
+    impl = "the unmodified reference (oracle/_ref)" if kind == "reference" else "the oracle port of the reference"
     sample = (f"{n_seq} of the {GLOBAL_BATCH} sequences (L={SEQ_LEN}) per step, {impl}, fp32, torch {torch.__version__} "
               f"CPU, {cores} threads (fastest of the counts tried on {os.cpu_count()} logical cores)")
     print(json.dumps({
@@ -304,13 +309,14 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--batch", type=int, default=GLOBAL_BATCH)
     ap.add_argument("--micro-batch", type=int, default=128)
     ap.add_argument("--ref-seqs", type=int, default=2, help="sequences per step of the CPU reference arm")
     ap.add_argument("--cpu-baseline-seqs", type=int, default=4)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip configs[3]/[4] and the GPU eager baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -359,13 +365,24 @@ def main():
     sampler = ClockSampler(local_rank)
     sampler.start()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    last = None
     ev0.record()
     for _ in range(args.steps):
-        step_device()
+        last = step_device()
     ev1.record()
     torch.cuda.synchronize()
     barrier()
     ms_total = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0 and last is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        mean = last.float().cpu()
+        max_rows = DUMP_LIMIT_BYTES // (mean.shape[1] * 4)
+        if mean.shape[0] > max_rows:  # a fixed, seeded sample of the rows (sorted), the same for every run of this batch
+            rows = torch.randperm(mean.shape[0], generator=torch.Generator().manual_seed(0))[:max_rows].sort().values
+            mean = mean[rows]
+        np.save(os.path.join(args.dump_outputs, "mean.npy"), mean.numpy())
+    del last
     launches = lib.esmb200_launch_count() - launches0
 
     # ---- per-kernel pass: the same step with every launch bracketed by events (breaks PDL overlap, so it is separate)
@@ -449,17 +466,8 @@ def main():
             ach, peak, unit = amount / avg / 1e9, peaks["tensor_sustained"], "TFLOP/s"
         else:
             ach, peak, unit = amount / avg / 1e6, peaks["hbm"], "GB/s"
-        traffic, traffic_src = None, None
-        for fname in ("r02_traffic.json", "r01_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", fname)
-            if os.path.exists(tpath):  # DRAM bytes per token of this kernel from a committed ncu --set full capture
-                bpt = json.load(open(tpath))["bytes_per_token"].get(dom)
-                if bpt:
-                    traffic = round(bpt * M)
-                    traffic_src = f"static: profiles/{fname} (ncu --set full dram__bytes of this kernel per token x {M} tokens)"
-                    break
         roofline = {"kernel": dom, "bound": kind, "achieved": round(ach, 1), "peak": peak, "unit": unit,
-                    "frac": round(ach / peak, 4), "traffic": traffic, "traffic_source": traffic_src,
+                    "frac": round(ach / peak, 4),
                     "peak_source": peaks["source"] + (", sustained (kernel timed inside a long step)" if kind == "tensor" else ""),
                     "avg_launch_ms": round(avg, 4), "algorithmic_per_launch": amount}
 
@@ -473,7 +481,7 @@ def main():
                    "global_batch": args.batch, "seq_len": SEQ_LEN, "per_gpu_batch": n_local,
                    "parallelism": f"dp{world} (sequence sharding, one all-gather of [B,E] means)",
                    "weights": "seeded random init (no checkpoints offline)", "repr_layers": [L_LAYERS],
-                   "l2": "activations per step (>1 GB/GPU) exceed the 126 MB L2; no explicit flush"},
+                   "l2": "activations per step (>1 GB/GPU) exceed the 50 MB L2; no explicit flush"},
         "model_tflops": round(value * flops_per_seq() / 1e12, 1),
         "tensor_frac_whole_step": round(value * flops_per_seq() / 1e12 / world / peaks["tensor_sustained"], 4),
         "e2e": {"value": round(e2e_value, 2), "unit": "sequences/s", "h2d_bytes_per_step": emb.h2d_bytes * world,
@@ -503,7 +511,7 @@ def main():
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         n = args.cpu_baseline_seqs
         v, ms, cores, kind = cpu_reference_seq_per_s(model_cpu_sd, n, steps=1, warmup=0)
-        impl = "the unmodified reference (baseline/_ref)" if kind == "reference" else "fp32 oracle port of the reference"
+        impl = "the unmodified reference (oracle/_ref)" if kind == "reference" else "fp32 oracle port of the reference"
         out["cpu_baseline"] = {"value": round(v, 4), "unit": "sequences/s", "cores": cores, "kind": kind,
                                "sample": f"one pass over {n} of the {args.batch} sequences (L={SEQ_LEN}), {impl} on the "
                                          f"host CPU, fp32, {ms / 1e3:.1f} s"}

@@ -1,4 +1,4 @@
-"""esm_b200 — B200-native (sm_100a) ESM-2 transformer-layer forward behind the reference's Python API.
+"""esm_b200 — H100-native (sm_90a) ESM-2 transformer-layer forward behind the reference's Python API.
 
     from esm_b200 import pretrained
     model, alphabet = pretrained.esm2_t33_650M_UR50D()      # same call as esm.pretrained.*

@@ -190,7 +190,7 @@ def load():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise Esmb200Error(
-                f"{LIB_PATH} not found: build it with `python -m esm_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} not found: build it with `python -m esm_b200.build` (nvcc, sm_90a). "
                 "esm_b200 has no CPU or PyTorch fallback for the transformer-layer path."
             )
         lib = ctypes.CDLL(LIB_PATH)

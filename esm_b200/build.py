@@ -1,4 +1,4 @@
-"""In-tree build of libesmb200.so with nvcc for sm_100a (no JIT cache: the .so travels with the repo snapshot).
+"""In-tree build of libesmb200.so with nvcc for sm_90a (H100) (no JIT cache: the .so travels with the repo snapshot).
 
     python -m esm_b200.build [--force]
 """
@@ -16,7 +16,7 @@ SOURCES = ["api.cu"]
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [os.path.join("..", "..", "include", "esmb200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]
@@ -31,13 +31,13 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, defines=(), out: str = OUT) -> str:
-    """Build libesmb200.so.  `defines` / `out` produce developer variants (e.g. -DESMB200_EXPERIMENTS for the
-    profiling-only GEMM epilogues) that are loaded through ESMB200_LIB_PATH; the product library takes neither."""
+    """Build libesmb200.so.  `defines` / `out` produce developer variants that are loaded through ESMB200_LIB_PATH;
+    the product library takes neither."""
     if not force and out == OUT and not _stale():
         return OUT
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
-        raise RuntimeError("nvcc not found: libesmb200.so must be built with the CUDA 12.9 toolkit (sm_100a)")
+        raise RuntimeError("nvcc not found: libesmb200.so must be built with a CUDA 12 toolkit (sm_90a)")
     cmd = ([nvcc] + NVCC_FLAGS + [f"-D{d}" for d in defines] + (["-Xptxas", "-v"] if verbose else []) +
            ["-o", out] + SOURCES)
     r = subprocess.run(cmd, cwd=CSRC, capture_output=True, text=True)

@@ -1,4 +1,4 @@
-// esm_b200 — C ABI (include/esmb200.h): host-side orchestration of the sm_100a kernels.
+// esm_b200 — C ABI (include/esmb200.h): host-side orchestration of the sm_90a kernels.
 //
 // Everything here is plain C-callable: device pointers in, launches on the caller's stream, no torch types.
 // Host work per call is limited to encoding a handful of TMA descriptors (cuTensorMapEncodeTiled) and
@@ -18,9 +18,6 @@
 
 #include <mutex>
 
-#ifdef ESMB200_EXPERIMENTS
-#include "attention7.cuh"  // round-1 kernel, A/B only
-#endif
 #include "attention8.cuh"
 #include "attention_contact.cuh"
 #include "attention_probs.cuh"
@@ -132,55 +129,8 @@ int make_tmap_f16(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t col
   return make_tmap_2d(map, ptr, 2, rows, cols, ld_elems, box_rows);
 }
 
-// attention implementation: 8 = attention8.cuh (4 CTAs/SM, default), 7 = attention7.cuh (2 CTAs/SM, two MMA issuing
-// threads; kept for A/B runs).  ESMB200_ATTN_POLY = n sends every n-th pair of exponentials of v8 to the FMA pipe.
-int g_attn_version = -1, g_attn_poly = -1;  // -1: take the environment / default on first use
-
-int attn_version() {
-  if (g_attn_version < 0) {
-    const char* e = getenv("ESMB200_ATTN");
-#ifdef ESMB200_EXPERIMENTS
-    g_attn_version = (e && e[0] == '7') ? 7 : 8;
-#else
-    g_attn_version = 8;
-#endif
-  }
-  return g_attn_version;
-}
-
-int attn_poly() {
-  if (g_attn_poly < 0) {
-    const char* e = getenv("ESMB200_ATTN_POLY");
-    g_attn_poly = (e && (e[0] == '0' || e[0] == '2' || e[0] == '3' || e[0] == '4')) ? (e[0] - '0') : 4;
-  }
-  return g_attn_poly;
-}
-
-cudaError_t launch_attention_fwd(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnParams& ap, int sms,
-                                 cudaStream_t st) {
-  if (ap.lo_off > 0) return launch_attention_v8_poly<0, true>(tq, tkv, ap, sms, st);  // fp32x3: all exponentials on MUFU
-  if (ap.slots == 2) return launch_attention_v8_poly<4, false, 2>(tq, tkv, ap, sms, st);  // head_dim <= 128 (15B)
-#ifdef ESMB200_EXPERIMENTS
-  if (attn_version() == 7) return launch_attention_v7(tq, tkv, ap, sms, st);
-#endif
-  switch (attn_poly()) {
-    case 0: return launch_attention_v8_poly<0>(tq, tkv, ap, sms, st);
-    case 2: return launch_attention_v8_poly<2>(tq, tkv, ap, sms, st);
-    case 3: return launch_attention_v8_poly<3>(tq, tkv, ap, sms, st);
-    default: return launch_attention_v8_poly<4>(tq, tkv, ap, sms, st);
-  }
-}
-
 // 64-wide column slots per head on the attention side: 1 for head_dim <= 64, 2 up to 128 (elementwise.cuh head_slot)
 inline int head_slots(int E, int H) { return (H > 0 && E / H > 64) ? 2 : 1; }
-
-int qkv_chunked() {  // tile walk of the QKV GEMM (gemm2.cuh): 1 = one contiguous run of tiles per cluster (default)
-  static const int v = [] {
-    const char* e = getenv("ESMB200_QKV_CHUNKED");
-    return (e && e[0] == '0') ? 0 : 1;
-  }();
-  return v;
-}
 
 constexpr int kMaxDevices = 64;
 
@@ -194,55 +144,45 @@ int num_sms() {  // per device: one process may drive several GPUs
 }
 
 int check_device() {
-  static int ok[kMaxDevices] = {};  // 0 unknown, 1 sm_100, -1 other
+  static int ok[kMaxDevices] = {};  // 0 unknown, 1 sm_90, -1 other
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return fail(ESMB200_ECUDA, "no CUDA device");
   if (dev < 0 || dev >= kMaxDevices) return fail(ESMB200_ECUDA, "device ordinal out of range");
   if (ok[dev] == 0) {
     int major = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-    ok[dev] = (major == 10) ? 1 : -1;
+    ok[dev] = (major == 9) ? 1 : -1;
   }
   if (ok[dev] < 0)
-    return fail(ESMB200_ECUDA, "esmb200 requires an sm_100a (Blackwell B200) device; there is no fallback path");
+    return fail(ESMB200_ECUDA, "esmb200 requires an sm_90a (Hopper H100) device; there is no fallback path");
   return ESMB200_OK;
 }
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const GemmParams& p,
-                cudaStream_t st, int tag = T_GEMM_OTHER, bool split = false) {
+int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st,
+                int tag = T_GEMM_OTHER, bool split = false) {
   ProfScope ps(tag, st);
   cudaError_t e;
   if (split) {  // fp32x3 precision: operands stored as fp16 hi | lo along K (gemm2.cuh)
     if (p.K % 64 != 0) return fail(ESMB200_EINVAL, "fp32x3 precision needs K % 64 == 0");
     switch (epi) {
-      case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE, true>(ta, tb, tout, p, num_sms(), st); break;
-      case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL, true>(ta, tb, tout, p, num_sms(), st); break;
-      case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU, true>(ta, tb, tout, p, num_sms(), st); break;
-      case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32, true>(ta, tb, tout, p, num_sms(), st); break;
-      case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32, true>(ta, tb, tout, p, num_sms(), st); break;
+      case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE, true>(ta, tb, p, num_sms(), st); break;
+      case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL, true>(ta, tb, p, num_sms(), st); break;
+      case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU, true>(ta, tb, p, num_sms(), st); break;
+      case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32, true>(ta, tb, p, num_sms(), st); break;
+      case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32, true>(ta, tb, p, num_sms(), st); break;
       default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
     }
     if (e != cudaSuccess) return fail_cuda(e, "gemm launch (fp32x3)");
     return ESMB200_OK;
   }
   switch (epi) {
-    case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32>(ta, tb, tout, p, num_sms(), st); break;
-#ifdef ESMB200_EXPERIMENTS  // profiling-only epilogues (profiles/r01_epilogue_experiments.txt)
-    case EPI_NONE: e = launch_gemm2_epi<EPI_NONE>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_LDONLY: e = launch_gemm2_epi<EPI_LDONLY>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_LD_X16: e = launch_gemm2_epi<EPI_LD_X16>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_LD_4WARPS: e = launch_gemm2_epi<EPI_LD_4WARPS>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_LD_BATCH: e = launch_gemm2_epi<EPI_LD_BATCH>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_GELU_MATHONLY: e = launch_gemm2_epi<EPI_GELU_MATHONLY>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_F16_STOREONLY: e = launch_gemm2_epi<EPI_F16_STOREONLY>(ta, tb, tout, p, num_sms(), st); break;
-    case EPI_FMA_MATHONLY: e = launch_gemm2_epi<EPI_FMA_MATHONLY>(ta, tb, tout, p, num_sms(), st); break;
-#endif
+    case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE>(ta, tb, p, num_sms(), st); break;
+    case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL>(ta, tb, p, num_sms(), st); break;
+    case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU>(ta, tb, p, num_sms(), st); break;
+    case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32>(ta, tb, p, num_sms(), st); break;
+    case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32>(ta, tb, p, num_sms(), st); break;
     default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
   }
   if (e != cudaSuccess) return fail_cuda(e, "gemm launch");
@@ -318,7 +258,7 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
     rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * T, qcols, qcols, attn8_cfg::BLOCK_KV);
     if (rc) return rc;
     ProfScope ps(T_ATTN, st);
-    e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
+    e = launch_attention_fwd(tq, tkv, ap, st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "attention launch");
   if (probs && contact && !split) {
@@ -392,7 +332,7 @@ int esmb200_convert_f16(const float* src, void* dst, size_t n, void* stream) {
   if (n == 0) return ESMB200_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   size_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
   ProfScope ps(T_CONVERT, st);
   convert_f32_f16_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), n);
   CK(cudaGetLastError());
@@ -464,7 +404,7 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   auto convert = [&](const float* src, __half* dst, size_t rows, int K) -> int {  // [rows,K] fp32 -> fp16 (hi | lo)
     if (!split) return esmb200_convert_f16(src, dst, rows * (size_t)K, stream);
     size_t blocks = (rows * (size_t)K + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
     ProfScope ps(T_CONVERT, st);
     convert_f32_split_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, dst, rows, K);
     cudaError_t ce = cudaGetLastError();
@@ -557,8 +497,7 @@ int carve_workspace(Workspace* ws, void* workspace, size_t bytes, int E, int H, 
 }
 
 struct ActMaps {
-  CUtensorMap xn, ctx, h;       // A operands (fp16, box {64,128}); h doubles as fc1's output map
-  CUtensorMap qkv_out, x_out;   // epilogue outputs: qkv fp16 [M,3E] box {64,128}; x fp32 [M,E] box {32,128}
+  CUtensorMap xn, ctx, h;       // A operands (fp16, box {64,128})
 };
 
 int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* rope_cos, const float* rope_sin,
@@ -579,10 +518,10 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   GemmParams g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = 3 * Ea; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * Ea;
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = Ea; g.q_scale = L->q_scale; g.chunked = qkv_chunked();
+  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = Ea; g.q_scale = L->q_scale;
   g.lo_col_off = 3 * Ea;
   g.rope_ld = 32 * L->slots;
-  int rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_out, g, st, T_QKV, split);
+  int rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV, split);
   if (rc) return rc;
   // attention (multihead_attention.py:357-394)
   rc = run_attention(ws.qkv, ws.ctx, attn_probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split, contact,
@@ -591,7 +530,7 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   // out_proj + residual (multihead_attention.py:395, modules.py:134)
   memset(&g, 0, sizeof g);
   g.M = M; g.N = E; g.K = Ea; g.bias = L->out_b; g.out = x; g.ldo = E;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_out, g, st, T_OUT, split);
+  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT, split);
   if (rc) return rc;
   // LN2 -> fp16 (modules.py:137)
   {
@@ -603,22 +542,20 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   // fc1 + GELU (modules.py:138)
   memset(&g, 0, sizeof g);
   g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.out = ws.h; g.ldo = F; g.lo_col_off = F;
-  rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h, g, st, T_FC1, split);
+  rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, g, st, T_FC1, split);
   if (rc) return rc;
   // fc2 + residual (modules.py:139-140)
   memset(&g, 0, sizeof g);
   g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b; g.out = x; g.ldo = E;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_out, g, st, T_FC2, split);
+  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, g, st, T_FC2, split);
   return rc;
 }
 
-int make_act_maps(ActMaps* am, const Workspace& ws, const float* x, int E, int H, int F, int M, int split = 0) {
+int make_act_maps(ActMaps* am, const Workspace& ws, int E, int H, int F, int M, int split = 0) {
   const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;  // fp32x3: activations are [rows, 2 * width]
   int rc = make_tmap_f16(&am->xn, ws.xn, M, pf * E, pf * E, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&am->ctx, ws.ctx, M, pf * Ea, pf * Ea, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&am->h, ws.h, M, pf * F, pf * F, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&am->qkv_out, ws.qkv, M, pf * 3 * Ea, pf * 3 * Ea, 128);
-  if (!rc) rc = make_tmap_2d(&am->x_out, x, 4, M, E, E, 128);
   return rc;
 }
 }  // namespace
@@ -653,7 +590,7 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
   rc = carve_workspace(&ws, workspace, workspace_bytes, E, H, F, B, T, split);
   if (rc) return rc;
   ActMaps am;
-  rc = make_act_maps(&am, ws, x, E, H, F, B * T, split);
+  rc = make_act_maps(&am, ws, E, H, F, B * T, split);
   if (rc) return rc;
   rc = run_key_bits(pad_mask, ws.as, B, T, st);
   if (rc) return rc;
@@ -729,18 +666,15 @@ int esmb200_gemm_f16(int32_t epilogue, const void* a, const void* w, const float
   if (rc) return rc;
   if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
     return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb, tout;
-  const bool out_f16 = (epilogue == EPI_QKV_ROPE || epilogue == EPI_BIAS_GELU || epilogue == EPI_F16_STOREONLY ||
-                        epilogue == EPI_GELU_MATHONLY || epilogue == EPI_FMA_MATHONLY);
+  CUtensorMap ta, tb;
   rc = make_tmap_f16(&ta, a, M, K, K, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, N, K, K, gemm2_cfg::HALF_N);
-  if (!rc) rc = make_tmap_2d(&tout, out, out_f16 ? 2 : 4, M, N, N, 128);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = N; g.K = K; g.bias = bias; g.out = out; g.ldo = N;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, tout, g, static_cast<cudaStream_t>(stream));
+  return launch_gemm(epilogue, ta, tb, g, static_cast<cudaStream_t>(stream));
 }
 
 // ---- fp32x3 precision building blocks (hi | lo fp16 operands): used by the LM head and the kernel-level parity tests
@@ -758,7 +692,7 @@ int esmb200_convert_split(const float* src, void* dst, int64_t rows, int32_t K, 
   if (rows <= 0 || K <= 0) return ESMB200_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   size_t blocks = ((size_t)rows * K + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
   ProfScope ps(T_CONVERT, st);
   convert_f32_split_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), (size_t)rows, K);
   CK(cudaGetLastError());
@@ -777,17 +711,15 @@ int esmb200_gemm_split(int32_t epilogue, const void* a, const void* w, const flo
   if (rc) return rc;
   if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
     return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb, tout;
+  CUtensorMap ta, tb;
   rc = make_tmap_f16(&ta, a, M, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, N, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::HALF_N);
-  if (!rc) rc = f16_out ? make_tmap_2d(&tout, out, 2, M, 2 * (uint64_t)N, 2 * (uint64_t)N, 128)
-                        : make_tmap_2d(&tout, out, 4, M, N, N, 128);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = N; g.K = K; g.bias = bias; g.out = out; g.ldo = N; g.lo_col_off = N;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, tout, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, true);
+  return launch_gemm(epilogue, ta, tb, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, true);
 }
 
 int esmb200_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
@@ -811,16 +743,15 @@ int esmb200_gemm_qkv_f16(const void* a, const void* w, const float* bias, void* 
     return fail(ESMB200_EINVAL, "rope tables must be given together with T, or not at all");
   int rc = check_device();
   if (rc) return rc;
-  CUtensorMap ta, tb, tout;
+  CUtensorMap ta, tb;
   rc = make_tmap_f16(&ta, a, M, E, E, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, 3 * (uint64_t)E, E, E, gemm2_cfg::HALF_N);
-  if (!rc) rc = make_tmap_2d(&tout, out, 2, M, 3 * (uint64_t)E, 3 * (uint64_t)E, 128);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
   g.M = M; g.N = 3 * E; g.K = E; g.bias = bias; g.out = out; g.ldo = 3 * E;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T > 0 ? T : 1; g.E = E; g.q_scale = q_scale;
-  return launch_gemm(EPI_QKV_ROPE, ta, tb, tout, g, static_cast<cudaStream_t>(stream));
+  return launch_gemm(EPI_QKV_ROPE, ta, tb, g, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
@@ -933,7 +864,7 @@ int esmb200_column_attention(const void* qkv, const uint8_t* pad_mask, void* ctx
   cudaError_t e;
   {
     ProfScope ps(T_ATTN, st);
-    e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
+    e = launch_attention_fwd(tq, tkv, ap, st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
   return ESMB200_OK;
@@ -977,7 +908,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   uint8_t* tied_scratch = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024)) + base_bytes;
   const size_t tied_bytes = esmb200_tied_row_attention_scratch_bytes(B, C, H);
   ActMaps am;
-  rc = make_act_maps(&am, ws, x, E, H, F, M);
+  rc = make_act_maps(&am, ws, E, H, F, M);
   if (rc) return rc;
   rc = run_key_bits(col_pad_mask, ws.as, B * C, R, st);  // column attention: B*C sequences of R keys
   if (rc) return rc;
@@ -999,7 +930,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     memset(&g, 0, sizeof g);
     g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * E;
     g.T = 1; g.E = E; g.q_scale = row_scale;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_out, g, st, T_QKV);
+    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV);
     if (rc) return rc;
     if (pad_mask) {
       ProfScope ps(T_KEYBITS, st);
@@ -1011,7 +942,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     if (rc) return rc;
     memset(&g, 0, sizeof g);
     g.M = M; g.N = E; g.K = E; g.bias = L->out_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_out, g, st, T_OUT);
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT);
     if (rc) return rc;
     // ---------------- column attention (modules.py:208-212; axial_attention.py:182-239) ----------------
     L = col_layers[i];
@@ -1023,7 +954,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     memset(&g, 0, sizeof g);
     g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * E;
     g.T = 1; g.E = E; g.q_scale = 0.125f;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_out, g, st, T_QKV);
+    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV);
     if (rc) return rc;
     {
       AttnParams ap;
@@ -1031,12 +962,12 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
       ap.keybits = ws.as.keybits; ap.kvlen = ws.as.kvlen; ap.words = ws.as.words;
       ap.ctx = ws.ctx; ap.row_max = nullptr; ap.row_sum = nullptr; ap.cols = C;
       ProfScope ps(T_ATTN, st);
-      e = launch_attention_fwd(tcq, tckv, ap, num_sms(), st);
+      e = launch_attention_fwd(tcq, tckv, ap, st);
     }
     if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
     memset(&g, 0, sizeof g);
     g.M = M; g.N = E; g.K = E; g.bias = L->out_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_out, g, st, T_OUT);
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT);
     if (rc) return rc;
     // ---------------- feed-forward (modules.py:213-214, 413-418) ----------------
     {
@@ -1046,11 +977,11 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     if (e != cudaSuccess) return fail_cuda(e, "ffn layernorm");
     memset(&g, 0, sizeof g);
     g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.out = ws.h; g.ldo = F;
-    rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h, g, st, T_FC1);
+    rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, g, st, T_FC1);
     if (rc) return rc;
     memset(&g, 0, sizeof g);
     g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_out, g, st, T_FC2);
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, g, st, T_FC2);
     if (rc) return rc;
   }
   return ESMB200_OK;
@@ -1130,24 +1061,9 @@ int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_
   return ESMB200_OK;
 }
 
-#ifdef ESMB200_TRACE
-int esmb200_debug_read_attn_trace(long long* out, int32_t n) {
-  CK(cudaMemcpyFromSymbol(out, esmb200::g_attn_trace, sizeof(long long) * (size_t)n));
-  return ESMB200_OK;
-}
-#endif
 
 int esmb200_set_option(const char* name, int32_t value) {
   if (!name) return fail(ESMB200_EINVAL, "null option name");
-#ifdef ESMB200_EXPERIMENTS
-  if (!strcmp(name, "attn") && (value == 7 || value == 8)) { g_attn_version = value; return ESMB200_OK; }
-#else
-  if (!strcmp(name, "attn") && value == 8) { g_attn_version = value; return ESMB200_OK; }
-#endif
-  if (!strcmp(name, "attn_poly") && (value == 0 || value == 2 || value == 3 || value == 4)) {
-    g_attn_poly = value;
-    return ESMB200_OK;
-  }
   if (!strcmp(name, "pdl") && (value == 0 || value == 1)) { pdl_flag() = value; return ESMB200_OK; }
   return fail(ESMB200_EINVAL, std::string("unknown option or value: ") + name);
 }

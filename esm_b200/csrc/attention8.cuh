@@ -1,39 +1,15 @@
-// esm_b200 — attention forward v8 (sm_100a, head_dim 64): FOUR small persistent CTAs per SM.
+// esm_b200 — attention forward (sm_90a): flash attention with TMA-fed K/V stages and warp-level tensor-core MMAs.
 //
-// Replaces /root/reference/esm/multihead_attention.py:357-394 (same contract as attention7.cuh).
+// Replaces esm/multihead_attention.py:357-394.  One CTA per (sequence, head, 128-query tile), eight warps of 16 query
+// rows each.  Thread 0 loads the Q tile once and streams 64-key K/V blocks through a two-stage TMA ring (mbarrier
+// completion); every warp computes S = Q K^T for its rows (mma.sync m16n8k16 from ldmatrix reads of the 128B-swizzled
+// tiles), applies the key-padding mask, keeps the online-softmax statistics in registers (exact running maximum, fp32
+// row sums), rescales O, and multiplies P (fp16, straight from the S registers) with V (ldmatrix.trans).
+// Exactness: P is rounded to fp16 relative to the running maximum (values <= 1), row sums and O are fp32.
 //
-// Why (profiles/r01_ncu_attention_v7_and_tied.txt, VERDICT r1 weak #5): v7 (2 CTAs/SM, S triple buffered, two MMA
-// issuing threads) leaves every unit idle — tensor pipe 26 %, MUFU 40 %, issue slots 61 % — because only TWO softmax
-// warps live on each SM sub-partition and each of them serialises  mbarrier wait -> tcgen05.ld -> exp pass ->
-// tcgen05.st -> arrive  (~470 of ~1560 cycles per 64-key block are latency, not work).  v8 hides that latency with
-// occupancy instead of buffering:
-//   * 4 CTAs per SM (192 threads, 128 TMEM columns, ~50 KB smem each) -> FOUR softmax warps per sub-partition, each
-//     belonging to a different CTA / query tile, so some warp is always in its exponential pass;
-//   * per CTA the pipeline is strictly serial and needs ONE S buffer:  QK^T(j) -> softmax(j) -> [P.V(j); QK^T(j+1)];
-//     P_j (fp16) is stored over the first 32 columns of S_j and QK^T(j+1) is issued right behind P.V(j) by the same
-//     thread: tcgen05.mma instructions of one thread execute in issue order, so the overwrite of S/P cannot pass the
-//     read of P (define ESMB200_ATTN8_SAFE_WAR to add an explicit commit/wait between them);
-//   * the commit that signals S_{j+1} also covers P.V(j): when a softmax thread holds S_{j+1}, O already contains block
-//     j, so the rare reference-max raise rescales O without a further barrier, and no o_free hand-off is needed either
-//     (the first P.V of the next tile is gated by p_full, which every thread arrives on after it has read O);
-//   * fewer instructions per key: the block maximum is no longer tracked.  P = exp(s - m_ref) against a lazily raised
-//     reference; a block whose ROW SUM exceeds 2^12 (or is not finite) is the signal that m_ref must be raised — the
-//     row sum is needed anyway, the 64 FMNMX per row and block are gone (they were ~1/6 of the issue slots).
-// Exactness: softmax is invariant to the reference, P is rounded to fp16 relative to it (values <= 2^12 keep the full
-// 11-bit significand), row sums and O are fp32.
-//
-// TMEM (128 columns per CTA, 4 CTAs/SM = all 512): S/P [0,64) | O [64,128).
-//
-// DS = 2 (64 < head_dim <= 128, ESM-2 15B): a head is TWO 64-wide slots (elementwise.cuh head_slot).  QK^T accumulates
-// both slots into the same S (8 MMAs), P.V runs once per slot into two 64-column halves of O: 256 TMEM columns, twice
-// the shared memory -> 2 CTAs per SM.  Two CTAs do not hide the serial per-CTA chain (first version: 400 TF/s), and
-// 256 columns leave room for a second S buffer: S0 [0,64) | S1 [64,128) | O [128,256), so P_j and S_{j+1} do not share
-// columns.  Issuing QK^T(j+1) BEFORE the wait for P_j (ESMB200_ATTN8_DS2_EARLY_QK) would let the tensor core fill S_{j+1}
-// under the softmax of block j, but with two 32 KB K/V stages per CTA the K/V of block j+1 is then still in flight
-// (clock64 trace: 1640 cycles of the 2730-cycle block spent on kv_full) — the default keeps the d = 64 order
-// [P.V(j); QK^T(j+1)].  Either way the rare reference-max raise waits on pv_done (one commit per P.V) before it rescales O.
-// (A 3-CTA/SM build — 96 registers, both 32-column S loads of a block in flight behind one wait — measured slower:
-// 2.32-2.47 ms vs 2.04-2.06 ms at B = 256, profiles/r02_attention_sweep.txt: occupancy beats per-warp load depth.)
+// DS = 2 (64 < head_dim <= 128, ESM-2 15B): a head is TWO 64-wide slots (elementwise.cuh head_slot); S sums both slots,
+// O has a half per slot.  SPLIT ("fp32x3" precision): q, k, v and P are fp16 hi | lo pairs and every product runs
+// hi*hi + lo*hi + hi*lo into the same fp32 accumulator.
 #pragma once
 
 #include "attention_common.cuh"
@@ -47,496 +23,222 @@ constexpr int HEAD_DIM = 64;
 constexpr int KV_STAGES = 2;
 constexpr int Q_BYTES = 128 * 64 * 2;  // 16 KB
 constexpr int KV_BYTES = 64 * 64 * 2;  // 8 KB per K tile and per V tile
-constexpr int NUM_THREADS = 192;       // warp 0 TMA, warp 1 MMA issuer + TMEM owner, warps 2-5 softmax (thread = query row)
-constexpr int CTAS_PER_SM = 4;
-constexpr int TMEM_COLS = 128;
-constexpr int SMEM_BYTES = Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 128;
-// SPLIT ("fp32x3" precision): q, k, v and P are fp16 hi | lo pairs, every product runs hi*hi + lo*hi + hi*lo into the
-// same fp32 accumulator.  Twice the shared memory per tile -> 2 CTAs per SM.
-constexpr int SMEM_BYTES_SPLIT = 2 * Q_BYTES + KV_STAGES * 4 * KV_BYTES + 1024 + 128;
-constexpr int CTAS_PER_SM_SPLIT = 2;
-constexpr int TMEM_COLS_WIDE = 256;    // DS = 2: S0/P0 [0,64) | S1/P1 [64,128) | O [128,256)
-constexpr float SUM_LIMIT = 4096.0f;   // raise the reference when a block's row sum exceeds this
+constexpr int NUM_THREADS = 256;
+constexpr int smem_bytes(int np) { return np * Q_BYTES + KV_STAGES * 2 * np * KV_BYTES + 1024 + 64; }
 }  // namespace attn8_cfg
 
-// exp2 of the 32 scores in sv (already in registers) against the reference mneg = -m_ref * log2(e); returns the packed
-// fp16 probabilities in pk[16] and adds the fp32 row sum into sum[4].  POLY: every POLY-th pair takes the FMA pipe.
-template <int POLY>
-__device__ __forceinline__ void attn8_exp_half(const uint32_t (&sv)[32], uint32_t wd, float mneg, float (&sum)[4],
-                                               uint32_t (&pk)[16]) {
-  constexpr float LOG2E = attn_cfg::LOG2E;
-  if (wd == 0xFFFFFFFFu) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float s0 = __uint_as_float(sv[2 * i]), s1 = __uint_as_float(sv[2 * i + 1]);
-      float x0, x1, p0, p1;
-      fma2(x0, x1, s0, s1, LOG2E, LOG2E, mneg, mneg);
-      if (POLY > 0 && (i % (POLY > 0 ? POLY : 1)) == 0) {
-        exp2_fma_pair(x0, x1, p0, p1);
-      } else {
-        p0 = ex2_approx(x0);
-        p1 = ex2_approx(x1);
-      }
-      add2(sum[(i & 1) * 2], sum[(i & 1) * 2 + 1], sum[(i & 1) * 2], sum[(i & 1) * 2 + 1], p0, p1);
-      pk[i] = pack_half2(p0, p1);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const bool k0 = (wd >> (2 * i)) & 1u, k1 = (wd >> (2 * i + 1)) & 1u;
-      const float s0 = k0 ? __uint_as_float(sv[2 * i]) : -INFINITY;
-      const float s1 = k1 ? __uint_as_float(sv[2 * i + 1]) : -INFINITY;
-      const float p0 = ex2_approx(fmaf(s0, LOG2E, mneg));  // ex2(-inf) = 0 for masked keys
-      const float p1 = ex2_approx(fmaf(s1, LOG2E, mneg));
-      sum[i & 3] += p0 + p1;
-      pk[i] = pack_half2(p0, p1);
-    }
-  }
-}
-
-template <int POLY, bool SPLIT = false, int DS = 1>
-__global__ void __launch_bounds__(attn8_cfg::NUM_THREADS,
-                                  (SPLIT || DS == 2) ? attn8_cfg::CTAS_PER_SM_SPLIT : attn8_cfg::CTAS_PER_SM)
-attention_fwd_kernel_v8(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
-                        const AttnParams p) {
+template <bool SPLIT, int DS>
+__global__ void __launch_bounds__(attn8_cfg::NUM_THREADS, (SPLIT || DS == 2) ? 1 : 2)
+attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
+                     const AttnParams p) {
   using namespace attn8_cfg;
   constexpr float LOG2E = attn_cfg::LOG2E;
   static_assert(!(SPLIT && DS == 2), "fp32x3 operands and two-slot heads are not combined");
   constexpr int NP = (SPLIT || DS == 2) ? 2 : 1;  // operand tiles per Q / K / V: hi (+ lo), or slot 0 (+ slot 1)
   constexpr int HEAD_COLS = HEAD_DIM * DS;        // columns of one head in qkv / ctx
-  constexpr int TCOLS = DS == 2 ? TMEM_COLS_WIDE : TMEM_COLS;
-  constexpr int SBUF = DS == 2 ? 2 : 1;           // S buffers (block g uses buffer g % SBUF, g = running block count)
-  constexpr int QB = NP * Q_BYTES;             // Q tile(s) of one work item
-  constexpr int KB = NP * KV_BYTES;            // K tile(s) / V tile(s) of one stage
+  constexpr int KB = NP * KV_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_q = smem;                                   // [hi | lo]
-  uint8_t* smem_k = smem + QB;                              // KV_STAGES x [hi | lo]
-  uint8_t* smem_v = smem + QB + KV_STAGES * KB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + QB + KV_STAGES * 2 * KB);
-  uint64_t* q_full = bars;         // [1] TMA -> MMA
-  uint64_t* q_empty = bars + 1;    // [1] MMA -> TMA (every QK^T of the tile has completed)
-  uint64_t* kv_full = bars + 2;    // [2] TMA -> MMA
-  uint64_t* kv_empty = bars + 4;   // [2] MMA -> TMA: the commit behind P.V(j) releases K_j and V_j together (every tcgen05
-                                   // instruction of the issuing thread costs ~94 cycles of the per-block chain: one commit less)
-  uint64_t* s_full = bars + 6;     // [SBUF] MMA -> softmax: S_j written (DS 1: and P.V(j-1) accumulated)
-  uint64_t* p_full = bars + 8;     // [SBUF] softmax -> MMA: P_j stored (128 arrivals).  One per S buffer: with two buffers a
-                                   // fast warp is a block ahead of a slow one, and arrivals on ONE barrier are anonymous
-  uint64_t* o_full = bars + 10;    // [1] MMA -> softmax: last P.V of the tile accumulated
-  uint64_t* pv_done = bars + 11;   // [1] DS 2: one completion per P.V (reference-max raise); ESMB200_ATTN8_SAFE_WAR
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  uint8_t* smem_q = smem;                                 // [NP]
+  uint8_t* smem_k = smem + NP * Q_BYTES;                  // [KV_STAGES][NP]
+  uint8_t* smem_v = smem + NP * Q_BYTES + KV_STAGES * KB;  // [KV_STAGES][NP]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NP * Q_BYTES + 2 * KV_STAGES * KB);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;  // [KV_STAGES]
 
-  // Roles: 0 = TMA producer, 1 = MMA issuer + TMEM owner, 2-5 = softmax (the four TMEM lane quarters need warps 2-5).
-  // Warps 0 and 1 sit on scheduler sub-partitions 0 and 1 in EVERY CTA; tcgen05 instructions of one sub-partition are
-  // dispatched one after the other (~80 cycles each, measured), so with the issuer always on warp 1 the four CTAs of an
-  // SM serialised their 11 instructions per block on one port.  CTAs of the second / fourth residency slot swap the two
-  // control warps (ESMB200_ATTN8_NO_ROLE_SWAP disables it for A/B).
-#ifdef ESMB200_ATTN8_NO_ROLE_SWAP
-  const uint32_t swap = 0;
-#else
-  const uint32_t swap = p.num_sms > 0 ? ((blockIdx.x / (uint32_t)p.num_sms) & 1u) : 0u;
-#endif
-  const uint32_t warp_phys = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0);  // warp-uniform for the compiler
-  const uint32_t warp = warp_phys < 2 ? (warp_phys ^ swap) : warp_phys;
-  const uint32_t lane = threadIdx.x % 32;
   const int nqt = (p.T + BLOCK_Q - 1) / BLOCK_Q;
-  const int total = p.B * p.H * nqt;
+  const int w = blockIdx.x;
+  const int qt = w % nqt, h = (w / nqt) % p.H, b = w / (nqt * p.H);
+  const int row_base = (b / p.cols) * p.T;
+  const int x0 = (b % p.cols) * 3 * p.E + h * HEAD_COLS;
+  const int part_off = SPLIT ? p.lo_off : HEAD_DIM;  // column distance of the second operand tile
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_kv);
     mbar_init(q_full, 1);
-    mbar_init(q_empty, 1);
-    for (int i = 0; i < KV_STAGES; ++i) {
-      mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    mbar_init(&s_full[0], 1);
-    mbar_init(&s_full[1], 1);
-    mbar_init(&p_full[0], 128);
-    mbar_init(&p_full[1], 128);
-    mbar_init(o_full, 1);
-    mbar_init(pv_done, 1);
+    for (int i = 0; i < KV_STAGES; ++i) mbar_init(&kv_full[i], 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TCOLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();  // everything below reads the previous kernel's output (qkv, key bits) or writes ctx
-  const uint32_t tmem_s = *tmem_slot;  // P_j occupies the first 32 columns of S_j
-  const uint32_t tmem_o = tmem_s + 64 * SBUF;
+  const int nblk = (p.kvlen[b] + BLOCK_KV - 1) / BLOCK_KV;
 
-  auto n_blocks = [&](int w) -> int {
-    const int b = w / (nqt * p.H);
-    return (p.kvlen[b] + BLOCK_KV - 1) / BLOCK_KV;
+  auto load_kv = [&](int j) {
+    const int s = j % KV_STAGES;
+    mbar_arrive_expect_tx(&kv_full[s], 2 * KB);
+#pragma unroll
+    for (int part = 0; part < NP; ++part) {
+      tma_load_2d(smem_k + s * KB + part * KV_BYTES, &tmap_kv, &kv_full[s], x0 + p.E + part * part_off,
+                  row_base + j * BLOCK_KV);
+      tma_load_2d(smem_v + s * KB + part * KV_BYTES, &tmap_kv, &kv_full[s], x0 + 2 * p.E + part * part_off,
+                  row_base + j * BLOCK_KV);
+    }
   };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      uint32_t g = 0, tq = 0;
-      for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int nblk = n_blocks(w);
-        if (nblk == 0) continue;
-        const int qt = w % nqt, h = (w / nqt) % p.H, b = w / (nqt * p.H);
-        const int row_base = (b / p.cols) * p.T;
-        const int x0 = (b % p.cols) * 3 * p.E + h * HEAD_COLS;
-        const int part_off = SPLIT ? p.lo_off : HEAD_DIM;  // column distance of the second operand tile
-        mbar_wait_relaxed(q_empty, (tq & 1) ^ 1);
-        mbar_arrive_expect_tx(q_full, QB);
+  if (threadIdx.x == 0 && nblk > 0) {
+    mbar_arrive_expect_tx(q_full, NP * Q_BYTES);
 #pragma unroll
-        for (int part = 0; part < NP; ++part)
-          tma_load_2d(smem_q + part * Q_BYTES, &tmap_q, q_full, x0 + part * part_off, row_base + qt * BLOCK_Q);
-        for (int i = 0; i < nblk; ++i, ++g) {
-          const uint32_t s = g % KV_STAGES;
-          mbar_wait_relaxed(&kv_empty[s], ((g / KV_STAGES) & 1) ^ 1);
-          mbar_arrive_expect_tx(&kv_full[s], 2 * KB);
-#pragma unroll
-          for (int part = 0; part < NP; ++part) {
-            tma_load_2d(smem_k + s * KB + part * KV_BYTES, &tmap_kv, &kv_full[s], x0 + p.E + part * part_off,
-                        row_base + i * BLOCK_KV);
-            tma_load_2d(smem_v + s * KB + part * KV_BYTES, &tmap_kv, &kv_full[s], x0 + 2 * p.E + part * part_off,
-                        row_base + i * BLOCK_KV);
-          }
-        }
-        ++tq;
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: QK^T(0), then [P.V(j); QK^T(j+1)] per block =====================
-    // The WHOLE warp runs this loop and only the tcgen05 instructions sit under elect_one(): with every operand derived
-    // from warp-uniform values (shuffles of lane 0, kernel parameters, loop counters) ptxas keeps descriptors and TMEM
-    // addresses in uniform registers and emits the eight UTCHMMA of a block back to back.  The round-1 form — `if
-    // (lane == 0)` around the loop — made every operand "divergent": each tcgen05.mma was wrapped in an ELECT / 2x
-    // R2UR.BROADCAST / BRA.U.ANY waterfall, ~94 cycles per instruction on the per-block critical chain (clock64 trace,
-    // scripts/attn_trace8.py).
-    {
-      constexpr uint32_t idesc_qk = umma_idesc_f16(128, 64, false);
-      constexpr uint32_t idesc_pv = umma_idesc_f16(128, 64, true);
-      const uint32_t u_smem = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-      const uint32_t u_q = u_smem, u_k = u_smem + QB, u_v = u_smem + QB + KV_STAGES * KB;
-      const uint32_t u_bars = u_smem + QB + KV_STAGES * 2 * KB;  // byte address of bars[0]
-      const uint32_t u_tmem_s = __shfl_sync(0xffffffffu, tmem_s, 0);
-      const uint32_t u_tmem_o = u_tmem_s + 64 * SBUF;
-      auto bar_addr = [&](const uint64_t* b) -> uint32_t { return u_bars + (uint32_t)(b - bars) * 8u; };
-      const uint64_t qdesc = umma_smem_desc_sw128(u_q, 1024, 0);
-      const uint64_t qdesc_lo = umma_smem_desc_sw128(u_q + Q_BYTES, 1024, 0);  // SPLIT: lo; DS 2: slot 1
-      uint32_t g = 0, tq = 0, np = 0;
-      auto issue_qk = [&](uint32_t gg, bool last) {
-        const uint32_t s = gg % KV_STAGES;
-        mbar_wait(&kv_full[s], (gg / KV_STAGES) & 1);
-        tc_fence_after();
-        ATRACE(3, gg);
-        const uint64_t kdesc = umma_smem_desc_sw128(u_k + s * KB, 1024, 0);
-        const uint32_t sb = gg % SBUF;
-        const uint32_t tmem_sb = u_tmem_s + sb * 64;
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_sb, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-          if constexpr (SPLIT) {  // + q_lo k_hi + q_hi k_lo
-            const uint64_t kdesc_lo = umma_smem_desc_sw128(u_k + s * KB + KV_BYTES, 1024, 0);
-#pragma unroll
-            for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(u_tmem_s, qdesc_lo + 2 * k, kdesc + 2 * k, idesc_qk, 1u);
-#pragma unroll
-            for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(u_tmem_s, qdesc + 2 * k, kdesc_lo + 2 * k, idesc_qk, 1u);
-          }
-          if constexpr (DS == 2) {  // + q[slot 1] . k[slot 1]
-            const uint64_t kdesc1 = umma_smem_desc_sw128(u_k + s * KB + KV_BYTES, 1024, 0);
-#pragma unroll
-            for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_sb, qdesc_lo + 2 * k, kdesc1 + 2 * k, idesc_qk, 1u);
-          }
-          tc_commit_addr(bar_addr(&s_full[sb]));
-          if (last) tc_commit_addr(bar_addr(q_empty));  // every QK^T of this tile issued: Q may be reloaded when they finish
-        }
-        __syncwarp();
-        ATRACE(4, gg);
-      };
-      for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int nblk = __shfl_sync(0xffffffffu, n_blocks(w), 0);
-        if (nblk == 0) continue;
-        mbar_wait(q_full, tq & 1);
-        issue_qk(g, nblk == 1);
-        for (int j = 0; j < nblk; ++j, ++g, ++np) {
-          const uint32_t s = g % KV_STAGES;
-#ifdef ESMB200_ATTN8_DS2_EARLY_QK
-          if constexpr (DS == 2) {  // S_{j+1} is produced while the softmax warps work on S_j
-            if (j + 1 < nblk) issue_qk(g + 1, j + 2 == nblk);
-          }
-#endif
-          ATRACE(0, g);
-#ifndef ESMB200_ATTN8_DS2_EARLY_QK
-          // K/V of the next block: wait now, while the softmax warps are still busy with block j
-          if (j + 1 < nblk) mbar_wait(&kv_full[(g + 1) % KV_STAGES], ((g + 1) / KV_STAGES) & 1);
-#endif
-          // P_j stored (first block of a tile: and the previous O read out).  (A spinning mbarrier.test_wait here was measured:
-          // same stand-alone time, ~1 % slower in-step — the spinning warp takes issue slots from the softmax warps.)
-          mbar_wait(&p_full[g % SBUF], (g / SBUF) & 1);
-          tc_fence_after();
-          ATRACE(1, g);
-          const uint32_t tmem_p = u_tmem_s + (g % SBUF) * 64;
-          const uint64_t vdesc = umma_smem_desc_sw128(u_v + s * KB, 1024, 8192);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BLOCK_KV / 16; ++k)
-              umma_ts(u_tmem_o, tmem_p + 8 * k, vdesc + 128 * k, idesc_pv, (j | k) != 0 ? 1u : 0u);
-            if constexpr (SPLIT) {  // + p_lo v_hi + p_hi v_lo (P_lo lives in columns [32,64) of the S buffer)
-              const uint64_t vdesc_lo = umma_smem_desc_sw128(u_v + s * KB + KV_BYTES, 1024, 8192);
-#pragma unroll
-              for (int k = 0; k < BLOCK_KV / 16; ++k) umma_ts(u_tmem_o, u_tmem_s + 32 + 8 * k, vdesc + 128 * k, idesc_pv, 1u);
-#pragma unroll
-              for (int k = 0; k < BLOCK_KV / 16; ++k) umma_ts(u_tmem_o, u_tmem_s + 8 * k, vdesc_lo + 128 * k, idesc_pv, 1u);
-            }
-            if constexpr (DS == 2) {  // O[:, 64:128] += P . v[slot 1]
-              const uint64_t vdesc1 = umma_smem_desc_sw128(u_v + s * KB + KV_BYTES, 1024, 8192);
-#pragma unroll
-              for (int k = 0; k < BLOCK_KV / 16; ++k)
-                umma_ts(u_tmem_o + 64, tmem_p + 8 * k, vdesc1 + 128 * k, idesc_pv, (j | k) != 0 ? 1u : 0u);
-            }
-            tc_commit_addr(bar_addr(&kv_empty[s]));
-            if constexpr (DS == 2) tc_commit_addr(bar_addr(pv_done));
-#ifdef ESMB200_ATTN8_SAFE_WAR
-            if constexpr (DS == 1) tc_commit_addr(bar_addr(pv_done));
-#endif
-            if constexpr (DS == 2) {
-              if (j + 1 == nblk) tc_commit_addr(bar_addr(o_full));
-            }
-          }
-          __syncwarp();
-          ATRACE(2, g);
-#ifdef ESMB200_ATTN8_SAFE_WAR
-          if constexpr (DS == 1) {
-            mbar_wait(pv_done, np & 1);
-            tc_fence_after();
-          }
-#endif
-#ifndef ESMB200_ATTN8_DS2_EARLY_QK
-          if constexpr (DS == 2) {
-            if (j + 1 < nblk) issue_qk(g + 1, j + 2 == nblk);
-          }
-#endif
-          if constexpr (DS == 1) {
-            if (j + 1 < nblk) {
-              issue_qk(g + 1, j + 2 == nblk);
-            } else {
-              if (elect_one()) tc_commit_addr(bar_addr(o_full));
-              __syncwarp();
-            }
-          }
-        }
-        ++tq;
-      }
-    }
-  } else {
-    // ===================== softmax / output warps (2-5): one thread per query row =====================
-    const uint32_t quarter = warp % 4;
-    const uint32_t row_local = quarter * 32 + lane;
-    const uint32_t lane_addr = (quarter * 32u) << 16;
-    const uint32_t ts0 = tmem_s + lane_addr;
-    uint32_t ns = 0, nt = 0;  // S blocks / tiles consumed so far (barrier phases)
-    for (int w = blockIdx.x; w < total; w += gridDim.x) {
-      const int qt = w % nqt, h = (w / nqt) % p.H, b = w / (nqt * p.H);
-      const int nblk = n_blocks(w);
-      const int row_base = (b / p.cols) * p.T;
-      const int t = qt * BLOCK_Q + row_local;
-      float m_ref = 0.f, l_run = 0.f;
-      bool seeded = false;  // m_ref holds the exact maximum of the first block that has an attendable key
-      const uint32_t* kb_ptr = p.keybits + (size_t)b * p.words;
-
-      for (int j = 0; j < nblk; ++j, ++ns) {
-        const uint2 kw2 = __ldg(reinterpret_cast<const uint2*>(kb_ptr + j * 2));
-        const uint32_t kw[2] = {kw2.x, kw2.y};
-        const uint32_t sb = ns % SBUF;
-        const uint32_t ts = ts0 + sb * 64;
-        if (threadIdx.x == 64) ATRACE(5, ns);
-        mbar_wait(&s_full[sb], (ns / SBUF) & 1);
-        tc_fence_after();
-        if (threadIdx.x == 64) ATRACE(6, ns);
-        if (!seeded) {  // uniform over the CTA: the key mask is per sequence
-          float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t sv[32];
-            tmem_ld_32x32b_x32(ts + c * 32, sv);
-            tmem_wait_ld_dep(sv);
-            const uint32_t wd = kw[c];
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              mx[i & 3] = fmaxf(mx[i & 3], (wd == 0xFFFFFFFFu || ((wd >> i) & 1u)) ? __uint_as_float(sv[i]) : -INFINITY);
-          }
-          const float m0 = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-          if ((kw[0] | kw[1]) != 0u) {
-            m_ref = m0;
-            seeded = true;
-          }
-        }
-
-        float rsum = 0.f;
-        uint32_t pk[2][16];
-        [[maybe_unused]] uint32_t pl[2][16];  // SPLIT: the lo halves of P
-        for (int trip = 0;; ++trip) {
-          const float mneg = -m_ref * LOG2E;
-          float sum[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t sv[32];
-            tmem_ld_32x32b_x32(ts + c * 32, sv);
-            tmem_wait_ld_dep(sv);
-            if constexpr (SPLIT) {
-              const uint32_t wd = kw[c];
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const bool k0 = (wd >> (2 * i)) & 1u, k1 = (wd >> (2 * i + 1)) & 1u;
-                const float p0 = k0 ? ex2_approx(fmaf(__uint_as_float(sv[2 * i]), LOG2E, mneg)) : 0.f;
-                const float p1 = k1 ? ex2_approx(fmaf(__uint_as_float(sv[2 * i + 1]), LOG2E, mneg)) : 0.f;
-                sum[i & 3] += p0 + p1;
-                const __half2 h2 = __floats2half2_rn(p0, p1);
-                const float2 f = __half22float2(h2);
-                pk[c][i] = *reinterpret_cast<const uint32_t*>(&h2);
-                pl[c][i] = pack_half2(p0 - f.x, p1 - f.y);
-              }
-            } else {
-              attn8_exp_half<POLY>(sv, kw[c], mneg, sum, pk[c]);
-            }
-          }
-          rsum = (sum[0] + sum[1]) + (sum[2] + sum[3]);
-          if (trip == 1) break;
-          const bool raise = !(rsum <= SUM_LIMIT);  // also true for inf / NaN (exp overflow)
-          if (!__any_sync(0xffffffffu, raise)) break;
-          // rare: some score of this block lies far above the reference.  Find the block maximum, raise the reference
-          // of this warp's rows, rescale O (P.V(j-1) has completed: the commit behind QK^T(j) covers it) and the row
-          // sum, and redo the block.  S_j is intact: P_j has not been stored over it yet.
-          float bmax = -INFINITY;
-#pragma unroll 1
-          for (int c = 0; c < 2; ++c) {
-            uint32_t sv[32];
-            tmem_ld_32x32b_x32(ts + c * 32, sv);
-            tmem_wait_ld_dep(sv);
-            const uint32_t wd = kw[c];
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if ((wd >> i) & 1u) bmax = fmaxf(bmax, __uint_as_float(sv[i]));
-          }
-          const float m_new = fmaxf(m_ref, bmax);
-          const float alpha = ex2_approx((m_ref - m_new) * LOG2E);
-          if (j > 0) {
-            if constexpr (DS == 2) {  // P.V(j-1) = completion ns-1 of pv_done; P.V(j-2) finished before QK^T(j) did
-              mbar_wait(pv_done, (ns - 1) & 1);
-              tc_fence_after();
-            }
-#pragma unroll 1
-            for (int q8 = 0; q8 < 4 * DS; ++q8) {
-              uint32_t ov[16];
-              tmem_ld_32x32b_x16(tmem_o + lane_addr + q8 * 16, ov);
-              tmem_wait_ld();
-#pragma unroll
-              for (int i = 0; i < 16; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-              tmem_st_32x32b_x16(tmem_o + lane_addr + q8 * 16, ov);
-            }
-          }
-          l_run *= alpha;
-          m_ref = m_new;
-        }
-        // P_j over the first 32 columns of S_j (this thread's own row, already consumed)
-        if (threadIdx.x == 64) ATRACE(8, ns);
-        tmem_st_32x32b_x16(ts, pk[0]);
-        tmem_st_32x32b_x16(ts + 16, pk[1]);
-        if constexpr (SPLIT) {
-          tmem_st_32x32b_x16(ts + 32, pl[0]);
-          tmem_st_32x32b_x16(ts + 48, pl[1]);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&p_full[sb]);
-        if (threadIdx.x == 64) ATRACE(9, ns);
-        l_run += rsum;
-      }
-
-      // ---- tile epilogue: O / l -> ctx (one 64-column slot at a time)
-      float inv = 0.f;
-      if (nblk > 0) {
-        mbar_wait(o_full, nt & 1);
-        ++nt;
-        tc_fence_after();
-        inv = l_run > 0.f ? 1.0f / l_run : 0.f;
-      }
-      if (t < p.T && p.row_max != nullptr) {
-        const size_t si = ((size_t)b * p.H + h) * p.T + t;
-        p.row_max[si] = m_ref;
-        p.row_sum[si] = l_run;
-      }
-      const size_t pitch = SPLIT ? 2 * (size_t)p.E : (size_t)p.E;  // SPLIT: ctx [M, 2E] = hi | lo
-      uint4* dst0 = reinterpret_cast<uint4*>(p.ctx + ((size_t)(row_base + t) * p.cols + b % p.cols) * pitch + h * HEAD_COLS);
-#pragma unroll
-      for (int slot = 0; slot < DS; ++slot) {
-        uint32_t outv[32];
-        [[maybe_unused]] uint32_t outl[32];  // SPLIT: lo halves of the context
-        if (nblk > 0) {
-#pragma unroll
-          for (int hlf = 0; hlf < 2; ++hlf) {
-            uint32_t ov[32];
-            tmem_ld_32x32b_x32(tmem_o + lane_addr + slot * 64 + hlf * 32, ov);
-            tmem_wait_ld_dep(ov);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float y0 = __uint_as_float(ov[2 * i]) * inv, y1 = __uint_as_float(ov[2 * i + 1]) * inv;
-              const __half2 h2 = __floats2half2_rn(y0, y1);
-              outv[hlf * 16 + i] = *reinterpret_cast<const uint32_t*>(&h2);
-              if constexpr (SPLIT) {
-                const float2 f = __half22float2(h2);
-                outl[hlf * 16 + i] = pack_half2(y0 - f.x, y1 - f.y);
-              }
-            }
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            outv[i] = 0u;
-            if constexpr (SPLIT) outl[i] = 0u;
-          }
-        }
-        if (t < p.T) {
-          uint4* dst = dst0 + slot * 8;
-#pragma unroll
-          for (int v = 0; v < 8; ++v) dst[v] = make_uint4(outv[4 * v], outv[4 * v + 1], outv[4 * v + 2], outv[4 * v + 3]);
-          if constexpr (SPLIT) {
-            uint4* dl = dst + p.E / 8;
-#pragma unroll
-            for (int v = 0; v < 8; ++v) dl[v] = make_uint4(outl[4 * v], outl[4 * v + 1], outl[4 * v + 2], outl[4 * v + 3]);
-          }
-        }
-      }
-      if (nblk > 0) tc_fence_before();  // O has been read: the arrival on p_full of the next tile's first block orders it
-    }
+    for (int part = 0; part < NP; ++part)
+      tma_load_2d(smem_q + part * Q_BYTES, &tmap_q, q_full, x0 + part * part_off, row_base + qt * BLOCK_Q);
+    for (int j = 0; j < KV_STAGES && j < nblk; ++j) load_kv(j);
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_s, TCOLS);
+  const uint32_t q_base = smem_u32(smem_q), k_base = smem_u32(smem_k), v_base = smem_u32(smem_v);
+  const uint32_t qrow = warp * 16;
+  const uint32_t* kb_ptr = p.keybits + (size_t)b * p.words;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[DS][8][4];
+#pragma unroll
+  for (int sl = 0; sl < DS; ++sl)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) o[sl][i][0] = o[sl][i][1] = o[sl][i][2] = o[sl][i][3] = 0.f;
+
+  if (nblk > 0) mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int s = j % KV_STAGES;
+    const uint2 kw2 = __ldg(reinterpret_cast<const uint2*>(kb_ptr + j * 2));
+    mbar_wait(&kv_full[s], (j / KV_STAGES) & 1);
+    const uint32_t kst = k_base + s * KB, vst = v_base + s * KB;
+    float sc[8][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) sc[i][0] = sc[i][1] = sc[i][2] = sc[i][3] = 0.f;
+    qk_tile<8>(sc, q_base, qrow, kst, 0);
+    if constexpr (SPLIT) {  // + q_lo k_hi + q_hi k_lo
+      qk_tile<8>(sc, q_base + Q_BYTES, qrow, kst, 0);
+      qk_tile<8>(sc, q_base, qrow, kst + KV_BYTES, 0);
+    }
+    if constexpr (DS == 2) qk_tile<8>(sc, q_base + Q_BYTES, qrow, kst + KV_BYTES, 0);  // + q[slot 1] . k[slot 1]
+
+    // key-padding mask, running maximum, rescale
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      const uint32_t wd = nb < 4 ? kw2.x : kw2.y;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const uint32_t key = (nb % 4) * 8 + 2 * c + e;
+        if (!((wd >> key) & 1u)) sc[nb][e] = sc[nb][2 + e] = -INFINITY;
+        mx[0] = fmaxf(mx[0], sc[nb][e]);
+        mx[1] = fmaxf(mx[1], sc[nb][2 + e]);
+      }
+    }
+    float ref[2], alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float mn = fmaxf(m[r], quad_max(mx[r]));
+      alpha[r] = (mn == -INFINITY) ? 1.f : ex2_approx((m[r] - mn) * LOG2E);  // ex2(-inf) = 0 before the first key
+      m[r] = mn;
+      ref[r] = (mn == -INFINITY) ? 0.f : -mn * LOG2E;
+      l[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int sl = 0; sl < DS; ++sl)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        o[sl][i][0] *= alpha[0]; o[sl][i][1] *= alpha[0];
+        o[sl][i][2] *= alpha[1]; o[sl][i][3] *= alpha[1];
+      }
+    uint32_t ph[8][2];
+    [[maybe_unused]] uint32_t pl[8][2];  // SPLIT: lo halves of P
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float p0 = ex2_approx(fmaf(sc[nb][2 * r], LOG2E, ref[r]));
+        const float p1 = ex2_approx(fmaf(sc[nb][2 * r + 1], LOG2E, ref[r]));
+        l[r] += p0 + p1;
+        const __half2 h2 = __floats2half2_rn(p0, p1);
+        ph[nb][r] = *reinterpret_cast<const uint32_t*>(&h2);
+        if constexpr (SPLIT) {
+          const float2 f = __half22float2(h2);
+          pl[nb][r] = pack_half2(p0 - f.x, p1 - f.y);
+        }
+      }
+    }
+    // O += P V: A fragment of keys [16 kk, 16 kk + 16) = S blocks 2 kk, 2 kk + 1
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint32_t a[4] = {ph[2 * kk][0], ph[2 * kk][1], ph[2 * kk + 1][0], ph[2 * kk + 1][1]};
+      [[maybe_unused]] uint32_t al[4];
+      if constexpr (SPLIT) {
+        al[0] = pl[2 * kk][0]; al[1] = pl[2 * kk][1]; al[2] = pl[2 * kk + 1][0]; al[3] = pl[2 * kk + 1][1];
+      }
+#pragma unroll
+      for (int n2 = 0; n2 < 4; ++n2) {
+        uint32_t bv[4];
+        ldsm_bt(vst, kk, 16 * n2, bv);
+        mma16816(o[0][2 * n2], a, bv[0], bv[1]);
+        mma16816(o[0][2 * n2 + 1], a, bv[2], bv[3]);
+        if constexpr (SPLIT) {  // + p_lo v_hi + p_hi v_lo
+          mma16816(o[0][2 * n2], al, bv[0], bv[1]);
+          mma16816(o[0][2 * n2 + 1], al, bv[2], bv[3]);
+          uint32_t bl[4];
+          ldsm_bt(vst + KV_BYTES, kk, 16 * n2, bl);
+          mma16816(o[0][2 * n2], a, bl[0], bl[1]);
+          mma16816(o[0][2 * n2 + 1], a, bl[2], bl[3]);
+        }
+        if constexpr (DS == 2) {  // O[:, 64:128] += P . v[slot 1]
+          uint32_t b1[4];
+          ldsm_bt(vst + KV_BYTES, kk, 16 * n2, b1);
+          mma16816(o[DS - 1][2 * n2], a, b1[0], b1[1]);
+          mma16816(o[DS - 1][2 * n2 + 1], a, b1[2], b1[3]);
+        }
+      }
+    }
+    __syncthreads();  // every warp is done with stage s
+    if (threadIdx.x == 0 && j + KV_STAGES < nblk) load_kv(j + KV_STAGES);
+  }
+
+  // ---- O / l -> ctx
+  const size_t pitch = SPLIT ? 2 * (size_t)p.E : (size_t)p.E;  // SPLIT: ctx [M, 2E] = hi | lo
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float lr = quad_sum(l[r]);
+    const int t = qt * BLOCK_Q + (int)(qrow + g + 8 * r);
+    if (t >= p.T) continue;
+    const float inv = lr > 0.f ? 1.0f / lr : 0.f;
+    if (p.row_max != nullptr && c == 0) {
+      const size_t si = ((size_t)b * p.H + h) * p.T + t;
+      p.row_max[si] = m[r] == -INFINITY ? 0.f : m[r];
+      p.row_sum[si] = lr;
+    }
+    __half* dst = p.ctx + ((size_t)(row_base + t) * p.cols + b % p.cols) * pitch + h * HEAD_COLS;
+#pragma unroll
+    for (int sl = 0; sl < DS; ++sl)
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb) {
+        const float y0 = o[sl][nb][2 * r] * inv, y1 = o[sl][nb][2 * r + 1] * inv;
+        const __half2 h2 = __floats2half2_rn(y0, y1);
+        const int col = sl * 64 + nb * 8 + 2 * (int)c;
+        *reinterpret_cast<__half2*>(dst + col) = h2;
+        if constexpr (SPLIT) {
+          const float2 f = __half22float2(h2);
+          *reinterpret_cast<__half2*>(dst + p.E + col) = __floats2half2_rn(y0 - f.x, y1 - f.y);
+        }
+      }
   }
 }
 
-template <int POLY, bool SPLIT = false, int DS = 1>
-inline cudaError_t launch_attention_v8_poly(const CUtensorMap& tmap_q, const CUtensorMap& tmap_kv, const AttnParams& p,
-                                            int num_sms, cudaStream_t stream) {
+template <bool SPLIT, int DS>
+inline cudaError_t launch_attention_ds(const CUtensorMap& tmap_q, const CUtensorMap& tmap_kv, const AttnParams& p,
+                                       cudaStream_t stream) {
   using namespace attn8_cfg;
-  constexpr bool two = SPLIT || DS == 2;
-  constexpr int smem = two ? SMEM_BYTES_SPLIT : SMEM_BYTES;
-  auto kern = attention_fwd_kernel_v8<POLY, SPLIT, DS>;
+  constexpr int smem = smem_bytes((SPLIT || DS == 2) ? 2 : 1);
+  auto kern = attention_fwd_kernel<SPLIT, DS>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   const long long total = (long long)p.B * p.H * ((p.T + BLOCK_Q - 1) / BLOCK_Q);
-  const long long cap = (long long)(two ? CTAS_PER_SM_SPLIT : CTAS_PER_SM) * num_sms;
-  const int grid = (int)(total < cap ? total : cap);
-  AttnParams pp = p;
-  pp.num_sms = num_sms;
-  return launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), smem, stream, tmap_q, tmap_kv, pp);
+  if (total > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+  return launch_pdl(kern, dim3((unsigned)total), dim3(NUM_THREADS), smem, stream, tmap_q, tmap_kv, p);
+}
+
+inline cudaError_t launch_attention_fwd(const CUtensorMap& tmap_q, const CUtensorMap& tmap_kv, const AttnParams& p,
+                                        cudaStream_t stream) {
+  if (p.lo_off > 0) return launch_attention_ds<true, 1>(tmap_q, tmap_kv, p, stream);
+  if (p.slots == 2) return launch_attention_ds<false, 2>(tmap_q, tmap_kv, p, stream);
+  return launch_attention_ds<false, 1>(tmap_q, tmap_kv, p, stream);
 }
 
 }  // namespace esmb200

@@ -1,9 +1,9 @@
-// esm_b200 — definitions shared by the attention kernels (sm_100a, head_dim 64): parameter blocks, tile constants,
-// the FMA-pipe exponential, developer tracing.
+// esm_b200 — definitions shared by the attention kernels (sm_90a, head_dim 64 per column slot): parameter block and
+// the warp-level Q.K^T tile product.
 //
-// The kernels replace /root/reference/esm/multihead_attention.py:357-394 (bmm(q,k^T) -> key-padding -inf mask ->
-// fp32 softmax -> bmm(P,v) -> (T,B,E) merge) without ever writing S or P to HBM.  Inputs come from the QKV GEMM
-// epilogue: qkv fp16 [B*T, 3E], q already scaled by d^-1/2 and rotated, k rotated.
+// The kernels replace esm/multihead_attention.py:357-394 (bmm(q,k^T) -> key-padding -inf mask -> fp32 softmax ->
+// bmm(P,v) -> (T,B,E) merge) without ever writing S or P to HBM.  Inputs come from the QKV GEMM epilogue: qkv fp16
+// [B*T, 3E], q already scaled by d^-1/2 and rotated, k rotated.
 #pragma once
 
 #include "common.cuh"
@@ -17,10 +17,8 @@ struct AttnParams {
   int words;                // words per sequence, multiple of 4
   __half* ctx;              // [B*T, E] attention output, heads merged (column h*64 + j)
   float* row_max;           // optional [B,H,T]: final softmax row max (of the scaled scores) ...
-  float* row_sum;           // optional [B,H,T]: ... and row sum of exp(s - max), for attention_probs_kernel
+  float* row_sum;           // optional [B,H,T]: ... and row sum of exp(s - max), for the probability kernels
   int lo_off = 0;           // fp32x3 precision: column offset (elements) of the lo halves in qkv [M, 6E] (= 3E)
-  int num_sms = 0;          // SMs of the device (set by the launcher): CTA b is assumed to sit on SM b % num_sms, used only to
-                            // spread the MMA-issuing warps of co-resident CTAs over two scheduler sub-partitions
   int slots = 1;            // 64-wide column slots per head: 1 (head_dim <= 64) or 2 (head_dim <= 128); E = H * 64 * slots
   int cols = 1;             // sequence s = (s / cols, s % cols) of a [B/cols, T, cols, 3E] tensor
                             // (MSA column attention: the T tokens of a sequence are `cols` rows apart)
@@ -30,64 +28,40 @@ namespace attn_cfg {
 constexpr int HEAD_DIM = 64;
 constexpr int TILE_BYTES = 128 * 64 * 2;  // 16 KB: 128 rows x 128 bytes
 constexpr float LOG2E = 1.4426950408889634f;
-// lazy softmax reference: the running reference max of a row is raised only when exp(s - m_ref) could exceed 2^8
-constexpr float RESCALE_TAU = 8.0f / 1.4426950408889634f;
 }  // namespace attn_cfg
 
-#ifdef ESMB200_TRACE
-// developer instrumentation (scripts/attn_trace.py): timestamps of CTA 0's softmax warp 2 / MMA thread
-__device__ long long g_attn_trace[8192];  // 10 slots x 400 blocks
-#define ATRACE(slot, idx) do { if (blockIdx.x == 0 && (idx) < 400) g_attn_trace[(slot) * 400 + (idx)] = clock64(); } while (0)
-#else
-#define ATRACE(slot, idx) do { } while (0)
-#endif
-
-namespace attn4_cfg {
-constexpr int BLOCK_Q = 128;
-constexpr int BLOCK_KV = 64;
-constexpr int HEAD_DIM = 64;
-constexpr int KV_STAGES = 4;
-constexpr int Q_BYTES = 128 * 64 * 2;   // 16 KB, double buffered
-constexpr int KV_BYTES = 64 * 64 * 2;   // 8 KB per K tile and per V tile
-constexpr int NUM_THREADS = 192;
-constexpr int TMEM_COLS = 256;
-constexpr int SMEM_BYTES = 2 * Q_BYTES + KV_STAGES * 2 * KV_BYTES + 1024 + 256;
-}  // namespace attn4_cfg
-
-// 2^x on the FMA pipe (Cody-Waite range reduction + cubic minimax polynomial on [-0.5, 0.5], max relative error 7.5e-5,
-// well below the fp16 rounding of P): used for one pair of keys in ESMB200_ATTN_POLY to take load off the MUFU pipe,
-// which bounds this kernel (16 ex2/clk/SM).  x <= ~12 here; very negative x is clamped to 2^-126 (rounds to 0 in fp16).
-__device__ __forceinline__ float exp2_fma(float x) {
-  x = fmaxf(x, -126.0f);
-  const float r = x + 12582912.0f;          // 1.5 * 2^23: the low mantissa bits of r hold round(x)
-  const float f = x - (r - 12582912.0f);    // in [-0.5, 0.5]
-  float p = fmaf(f, 0.0551716685f, 0.2426111251f);
-  p = fmaf(p, f, 0.6932609677f);
-  p = fmaf(p, f, 0.9999280572f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(r) << 23));
+// s[NB][4] += Q[16 rows from q_row0] . K[NB*8 keys from k_row0]^T over 64 head columns: Q and K are SW128 tiles with
+// 128-byte rows (TMA boxes of 64 fp16 columns).  Fragment layout of s: see mma16816 (row g / g + 8, key 8 nb + 2c..).
+template <int NB>
+__device__ __forceinline__ void qk_tile(float (&s)[NB][4], uint32_t q_base, uint32_t q_row0, uint32_t k_base,
+                                        uint32_t k_row0) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    uint32_t a[4];
+    ldsm_a(q_base, q_row0, kk, a);
+#pragma unroll
+    for (int n2 = 0; n2 < NB / 2; ++n2) {
+      uint32_t b[4];
+      ldsm_b(k_base, k_row0 + 16 * n2, kk, b);
+      mma16816(s[2 * n2], a, b[0], b[1]);
+      mma16816(s[2 * n2 + 1], a, b[2], b[3]);
+    }
+  }
 }
 
-// Every ESMB200_ATTN_POLY-th pair of keys takes the FMA-pipe exponential (0 = none).  Measured at B=64 (ms per launch),
-// scalar arithmetic: 0: 0.615, 4 (25 %): 0.594, 3 (37.5 %): 0.651, 2 (50 %): 0.658; with the packed FFMA2/FADD2 forms used
-// now: 0: 0.621, 4: 0.577, 3: 0.593, 2: 0.618 — beyond a quarter the extra ALU/FMA instructions cost more than the MUFU
-// cycles they save (the SM's issue slots are ~60 % busy in this kernel, profiles/r01_ncu_attention_v7_and_tied.txt).
-// the same for two values at once with packed FFMA2 / FADD2 arithmetic
-__device__ __forceinline__ void exp2_fma_pair(float x0, float x1, float& p0, float& p1) {
-  x0 = fmaxf(x0, -126.0f);
-  x1 = fmaxf(x1, -126.0f);
-  float r0, r1, n0, n1, f0, f1;
-  add2(r0, r1, x0, x1, 12582912.0f, 12582912.0f);
-  add2(n0, n1, r0, r1, -12582912.0f, -12582912.0f);
-  fma2(f0, f1, n0, n1, -1.0f, -1.0f, x0, x1);
-  fma2(p0, p1, f0, f1, 0.0551716685f, 0.0551716685f, 0.2426111251f, 0.2426111251f);
-  fma2(p0, p1, p0, p1, f0, f1, 0.6932609677f, 0.6932609677f);
-  fma2(p0, p1, p0, p1, f0, f1, 0.9999280572f, 0.9999280572f);
-  p0 = __int_as_float(__float_as_int(p0) + (__float_as_int(r0) << 23));
-  p1 = __int_as_float(__float_as_int(p1) + (__float_as_int(r1) << 23));
+// normalised probability of score s: exp(s - m) * inv for an attendable key (bit key % 32 of its key word), else 0
+__device__ __forceinline__ float masked_prob(float s, uint32_t kw, int key, float mneg, float inv) {
+  constexpr float LOG2E = attn_cfg::LOG2E;
+  return ((kw >> (key & 31)) & 1u) ? ex2_approx(fmaf(s, LOG2E, mneg)) * inv : 0.f;
 }
 
-#ifndef ESMB200_ATTN_POLY
-#define ESMB200_ATTN_POLY 4
-#endif
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 }  // namespace esmb200

@@ -1,24 +1,18 @@
-// esm_b200 — need_head_weights + return_contacts in ONE pass (sm_100a, head_dim <= 64, or <= 128 with DS = 2): the attention probabilities of a
-// layer are written to the stacked [B,L,H,T,T] result AND folded into the contact head's accumulators while they are
-// still in registers, so the 4*B*L*H*T^2-byte stack (24 GB at BASELINE.json configs[3]) is written once and never read
-// back.  r01 / attention_probs.cuh + contact_accumulate_kernel wrote it and re-read it (17 % + 14 % of configs[3]).
+// esm_b200 — need_head_weights + return_contacts in ONE pass (sm_90a, head_dim <= 64, or <= 128 with DS = 2): the
+// attention probabilities of a layer are written to the stacked [B,L,H,T,T] result AND folded into the contact head's
+// accumulators while they are still in registers, so the 4*B*L*H*T^2-byte stack is written once and never read back.
 //
-// Replaces /root/reference/esm/multihead_attention.py:397-400 (per-head probabilities) and the per-layer share of
-// ContactPredictionHead.forward, /root/reference/esm/modules.py:338-357 (eos masking, bos/eos crop, symmetrize :27-29,
-// apc :32-41), in the restated form of elementwise.cuh: with A_h the masked, cropped map of head h,
+// Replaces esm/multihead_attention.py:397-400 (per-head probabilities) and the per-layer share of
+// ContactPredictionHead.forward, esm/modules.py:338-357 (eos masking, bos/eos crop, symmetrize :27-29, apc :32-41), in
+// the restated form of elementwise.cuh: with A_h the masked, cropped map of head h,
 //     acc[b,i,j]        += sum_h w_h A_h[i,j]                  (one owner CTA per tile: plain read-modify-write)
 //     row_part[b,h,4kt+c,i] = sum_{j in 32-key quarter c of key tile kt} A_h[i,j]   (partials, summed by the caller)
 //     col_part[b,h,4qt+r,j] = sum_{i in 32-row quarter r of query tile qt} A_h[i,j]   (partials, summed by the caller)
 // No atomics: every output element has one writer and every sum a fixed order -> bit-reproducible contacts.
 //
-// One CTA = (128-key tile, 128-query tile, sequence) and LOOPS OVER THE HEADS: warp 8 lane 0 streams (Q_h, K_h) tiles
-// through a 2-stage TMA ring and issues S_h = Q_h K_h^T (4 x UMMA 128x128x16) into a double-buffered TMEM accumulator;
-// warps 0-15 (thread = query row x 32-key quarter: warps w, w+4, w+8, w+12 share the TMEM lanes of rows 32(w%4)..) turn
-// S_h into p = exp(s - m) / l with the statistics saved by the forward kernel, write the tile through a padded
-// shared-memory transpose (every global store is a 128-byte row segment) and accumulate.  A warp's loop is a latency
-// chain (TMEM load -> 32 exponentials -> transpose -> 32 row stores): the first version (4 compute warps, 2 CTAs/SM,
-// 128 accumulators per thread) ran at 22 K cycles per head with every unit idle (profiles/r02_ncu_contact_fused.txt);
-// sixteen compute warps with 32 accumulators each keep four warps per scheduler busy.
+// One CTA = (128-key tile, 128-query tile, sequence) and LOOPS OVER THE HEADS: thread 0 streams the (Q_h, K_h) tiles
+// through a 2-stage TMA ring; eight warps (16 query rows x 128 keys each) compute S_h = Q_h K_h^T with mma.sync, turn
+// it into p = exp(s - m) / l with the statistics saved by the forward kernel and accumulate in registers.
 #pragma once
 
 #include "attention_common.cuh"
@@ -47,13 +41,11 @@ struct ContactFuseParams {
 
 namespace cfuse_cfg {
 constexpr int BLOCK = 128;            // query rows and keys per tile
-constexpr int NUM_THREADS = 544;      // warps 0-15: thread = (query row, 32-key quarter); warp 16: TMA + MMA issuer
+constexpr int NUM_THREADS = 256;      // eight warps of 16 query rows x 128 keys
 constexpr int STAGES = 2;
 constexpr int TILE_BYTES = attn_cfg::TILE_BYTES;
-constexpr int TMEM_COLS = 256;        // S double buffer
 constexpr int smem_bytes(int ds) {  // ds operand tiles per Q and per K stage
-  return STAGES * 2 * ds * TILE_BYTES + 1024 /*align*/ + 128 /*barriers*/ + 16 * 32 * 33 * 4 /*transpose*/ +
-         128 * 4 /*row keep flags*/;
+  return STAGES * 2 * ds * TILE_BYTES + 1024 /*align*/ + 64 /*barriers*/ + 2 * 8 * BLOCK * 4 /*column sums*/;
 }
 }  // namespace cfuse_cfg
 
@@ -61,183 +53,154 @@ template <int DS>
 __global__ void __launch_bounds__(cfuse_cfg::NUM_THREADS, 1)
 attention_probs_contact_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const ContactFuseParams p) {
   using namespace cfuse_cfg;
-  constexpr float LOG2E = attn_cfg::LOG2E;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int STAGE_BYTES = DS * TILE_BYTES;        // Q (or K) tiles of one head: one per 64-wide slot
   uint8_t* smem_q = smem;                             // [STAGES][DS]
   uint8_t* smem_k = smem + STAGES * STAGE_BYTES;      // [STAGES][DS]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * 2 * STAGE_BYTES);
-  uint64_t* full = bars;         // [2] TMA -> MMA
-  uint64_t* empty = bars + 2;    // [2] MMA done with the stage -> TMA
-  uint64_t* s_full = bars + 4;   // [2] MMA -> softmax
-  uint64_t* s_free = bars + 6;   // [2] softmax -> MMA (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  float* tiles = reinterpret_cast<float*>(smem + STAGES * 2 * STAGE_BYTES + 128);  // [16][32*33]
-  float* rowkeep = tiles + 16 * 32 * 33;                                          // [128]
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * 2 * STAGE_BYTES);  // [STAGES] TMA -> warps
+  float* colsum = reinterpret_cast<float*>(smem + STAGES * 2 * STAGE_BYTES + 64);  // [2 (head parity)][8 warps][128]
 
-  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
   const int kt = blockIdx.x, qt = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * BLOCK, k0 = kt * BLOCK;
   const int row_base = b * p.T;
   const int nkt = gridDim.x, nqt = gridDim.y;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 512);
-    }
+    for (int i = 0; i < STAGES; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
   }
-  if (warp == 16) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_s = *tmem_slot;
   const bool live = k0 < p.kvlen[b];  // otherwise every key of this tile is masked: all probabilities are exactly 0
-
-  if (warp == 16) {
-    // ===================== TMA producer + MMA issuer =====================
-    if (lane == 0 && live) {
-      constexpr uint32_t idesc = umma_idesc_f16(128, 128, false);
-      auto load = [&](int h) {
-        const int s = h & 1;
-        mbar_arrive_expect_tx(&full[s], 2 * STAGE_BYTES);
+  auto load = [&](int h) {
+    const int s = h % STAGES;
+    mbar_arrive_expect_tx(&full[s], 2 * STAGE_BYTES);
 #pragma unroll
-        for (int sl = 0; sl < DS; ++sl) {
-          tma_load_2d(smem_q + s * STAGE_BYTES + sl * TILE_BYTES, &tmap_qkv, &full[s], (h * DS + sl) * 64, row_base + q0);
-          tma_load_2d(smem_k + s * STAGE_BYTES + sl * TILE_BYTES, &tmap_qkv, &full[s], p.E + (h * DS + sl) * 64,
-                      row_base + k0);
-        }
-      };
-      load(0);
-      if (p.H > 1) load(1);
-      for (int h = 0; h < p.H; ++h) {
-        const int s = h & 1;
-        const uint32_t ph = (h >> 1) & 1;
-        mbar_wait(&full[s], ph);
-        if (h >= 2) mbar_wait(&s_free[s], ((h - 2) >> 1) & 1);  // the softmax threads have read S of head h-2
-        tc_fence_after();
-#pragma unroll
-        for (int sl = 0; sl < DS; ++sl) {
-          const uint64_t qdesc = umma_smem_desc_sw128(smem_u32(smem_q + s * STAGE_BYTES + sl * TILE_BYTES), 1024, 0);
-          const uint64_t kdesc = umma_smem_desc_sw128(smem_u32(smem_k + s * STAGE_BYTES + sl * TILE_BYTES), 1024, 0);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_ss(tmem_s + s * 128, qdesc + 2 * k, kdesc + 2 * k, idesc, (sl | k) != 0);
-        }
-        tc_commit(&s_full[s]);
-        tc_commit(&empty[s]);
-        if (h + 2 < p.H) {
-          mbar_wait(&empty[s], ph);  // the MMAs of head h have read the stage
-          load(h + 2);
-        }
-      }
+    for (int sl = 0; sl < DS; ++sl) {
+      tma_load_2d(smem_q + s * STAGE_BYTES + sl * TILE_BYTES, &tmap_qkv, &full[s], (h * DS + sl) * 64, row_base + q0);
+      tma_load_2d(smem_k + s * STAGE_BYTES + sl * TILE_BYTES, &tmap_qkv, &full[s], p.E + (h * DS + sl) * 64,
+                  row_base + k0);
     }
-  } else {
-    // ===================== probabilities + contact accumulation: thread = (query row, 32-key quarter) =====================
-    const uint32_t rq = warp & 3;                 // row quarter: TMEM lanes 32*rq ..
-    const uint32_t cq = warp >> 2;                // key quarter: columns [32*cq, 32*cq + 32) of the tile
-    const uint32_t lane_addr = (rq * 32u) << 16;
-    const int trow = (int)(rq * 32 + lane);       // row of the tile
-    const int t = q0 + trow;                      // this thread's query position
-    const bool row_ok = t < p.T;
-    const int ncols = min(BLOCK, p.T - k0);
-    const int hi = p.lo + p.S;
-    const uint8_t* kp = p.keep ? p.keep + (size_t)b * p.T : nullptr;
-    // contact masks: position kept (not <eos>) and inside the bos/eos crop
-    const bool ri = row_ok && t >= p.lo && t < hi && (!kp || kp[t]);
-    if (cq == 0) rowkeep[trow] = ri ? 1.f : 0.f;
-    const int jlane = k0 + (int)cq * 32 + (int)lane;
-    const uint32_t cm = __ballot_sync(0xffffffffu, jlane < p.T && jlane >= p.lo && jlane < hi && (!kp || kp[jlane]));
-    const uint32_t wd = live ? __ldg(p.keybits + (size_t)b * p.words + kt * 4 + cq) : 0u;
-    const bool qpad = p.zero_pad_rows && row_ok && !((p.keybits[(size_t)b * p.words + (t >> 5)] >> (t & 31)) & 1u);
-    named_bar_sync(1, 512);  // rowkeep visible
-    float* tile = tiles + warp * (32 * 33);
-    const int t_warp0 = q0 + (int)rq * 32;
-    const int nrows = min(32, p.T - t_warp0);
-    const bool cols_ok = (int)cq * 32 < ncols;    // uniform over the warp
-    float acc[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  };
+  if (live && threadIdx.x == 0)
+    for (int h = 0; h < STAGES && h < p.H; ++h) load(h);
 
-    for (int h = 0; h < p.H; ++h) {
-      const int s = h & 1;
-      const float wh = __ldg(p.w + h);
-      float rs = 0.f, cs = 0.f;
-      if (live) {
-        const size_t si = ((size_t)b * p.H + h) * p.T + (row_ok ? t : 0);
-        const float mneg = -p.row_max[si] * LOG2E;
+  const int hi = p.lo + p.S;
+  const uint8_t* kp = p.keep ? p.keep + (size_t)b * p.T : nullptr;
+  const int ncols = min(BLOCK, p.T - k0);
+  // rows of this thread: t[r] = q0 + 16 warp + g + 8 r; contact masks: position kept (not <eos>) and inside the crop
+  int t[2];
+  bool row_ok[2], ri[2], qpad[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    t[r] = q0 + (int)(warp * 16 + g + 8 * r);
+    row_ok[r] = t[r] < p.T;
+    ri[r] = row_ok[r] && t[r] >= p.lo && t[r] < hi && (!kp || kp[t[r]]);
+    qpad[r] = p.zero_pad_rows && row_ok[r] && !((p.keybits[(size_t)b * p.words + (t[r] >> 5)] >> (t[r] & 31)) & 1u);
+  }
+  // columns of this thread: key k0 + 8 nb + 2 c + e
+  uint32_t cmask = 0u;  // bit 2 nb + e: column kept and inside the crop
+#pragma unroll
+  for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int j = k0 + nb * 8 + 2 * (int)c + e;
+      if (j < p.T && j >= p.lo && j < hi && (!kp || kp[j])) cmask |= 1u << (2 * nb + e);
+    }
+  uint32_t kw[4] = {0u, 0u, 0u, 0u};
+  if (live) {
+    const uint4 kw4 = __ldg(reinterpret_cast<const uint4*>(p.keybits + (size_t)b * p.words + kt * 4));
+    kw[0] = kw4.x; kw[1] = kw4.y; kw[2] = kw4.z; kw[3] = kw4.w;
+  }
+  float acc[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
+
+  for (int h = 0; h < p.H; ++h) {
+    const int s = h % STAGES;
+    const float wh = __ldg(p.w + h);
+    float sc[16][4];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) sc[i][0] = sc[i][1] = sc[i][2] = sc[i][3] = 0.f;
+    if (live) {
+      mbar_wait(&full[s], (h / STAGES) & 1);
+#pragma unroll
+      for (int sl = 0; sl < DS; ++sl)
+        qk_tile<16>(sc, smem_u32(smem_q + s * STAGE_BYTES + sl * TILE_BYTES), warp * 16,
+                    smem_u32(smem_k + s * STAGE_BYTES + sl * TILE_BYTES), 0);
+    }
+    float rs[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};  // row partials per 32-key quarter
+    float cs[16][2];                                               // column sums of this warp's 16 rows
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float mneg = 0.f, inv = 0.f;
+      if (live && row_ok[r]) {
+        const size_t si = ((size_t)b * p.H + h) * p.T + t[r];
+        mneg = -p.row_max[si] * attn_cfg::LOG2E;
         const float l = p.row_sum[si];
-        const float inv = (l > 0.f && !qpad) ? 1.0f / l : 0.f;  // esm2.py:135-139: rows of padded query tokens are zero
-        mbar_wait(&s_full[s], (h >> 1) & 1);
-        tc_fence_after();
-        uint32_t sv[32];
-        tmem_ld_32x32b_x32(tmem_s + lane_addr + s * 128 + cq * 32, sv);
-        tmem_wait_ld_dep(sv);
-        tc_fence_before();
-        mbar_arrive(&s_free[s]);  // S_h is in registers: the MMA of head h+2 may overwrite this buffer
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float pr = ((wd >> i) & 1u) ? ex2_approx(fmaf(__uint_as_float(sv[i]), LOG2E, mneg)) * inv : 0.f;
-          tile[lane * 33 + i] = pr;
-          const float x = (ri && ((cm >> i) & 1u)) ? pr : 0.f;
-          acc[i] = fmaf(wh, x, acc[i]);
-          rs += x;
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) tile[lane * 33 + i] = 0.f;
+        inv = (l > 0.f && !qpad[r]) ? 1.0f / l : 0.f;  // esm2.py:135-139: rows of padded query tokens are zero
       }
-      __syncwarp();
-      if (cols_ok && (int)cq * 32 + (int)lane < ncols) {
-        float* dst = p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + (size_t)t_warp0 * p.T + k0 + cq * 32 + lane;
-        if (nrows == 32) {
+      float* dst = p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + (size_t)t[r] * p.T + k0;
 #pragma unroll
-          for (int r = 0; r < 32; ++r) {  // 32 independent shared loads, then 32 row-segment stores
-            const float v = tile[r * 33 + lane];
-            dst[(size_t)r * p.T] = v;
-            cs = fmaf(v, rowkeep[rq * 32 + r], cs);
-          }
-        } else {
-          for (int r = 0; r < nrows; ++r) {
-            const float v = tile[r * 33 + lane];
-            dst[(size_t)r * p.T] = v;
-            cs = fmaf(v, rowkeep[rq * 32 + r], cs);
-          }
+      for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = nb * 8 + 2 * (int)c + e;
+          const float pr = live ? masked_prob(sc[nb][2 * r + e], kw[nb / 4], key, mneg, inv) : 0.f;
+          if (row_ok[r] && key < ncols) dst[key] = pr;
+          const float x = (ri[r] && ((cmask >> (2 * nb + e)) & 1u)) ? pr : 0.f;
+          acc[nb][2 * r + e] = fmaf(wh, x, acc[nb][2 * r + e]);
+          rs[r][nb / 4] += x;
+          if (r == 0) cs[nb][e] = x;
+          else cs[nb][e] += x;
         }
-      }
-      __syncwarp();
-      // row partial of this 32-key quarter (4 * nkt partials per row); column partials of this query tile
-      if (row_ok && t >= p.lo && t < hi)
-        p.row_part[(((size_t)b * p.H + h) * (4 * nkt) + 4 * kt + cq) * p.S + (t - p.lo)] = rs;  // 0 for <eos>
-      // column partial of this warp's 32 rows x 32 columns (4 * nqt partials per column): no cross-warp reduction, so the
-      // sixteen warps never meet at a barrier inside the head loop and overlap each other's TMEM / MUFU / store phases
-      if (jlane >= p.lo && jlane < hi && jlane < p.T)
-        p.col_part[(((size_t)b * p.H + h) * (4 * nqt) + 4 * qt + rq) * p.S + (jlane - p.lo)] = ((cm >> lane) & 1u) ? cs : 0.f;
     }
-    // acc tile: this CTA is the only writer of acc[b, rows of qt, columns of kt]; layers are separate launches
-    if (ri) {
-      float* dst = p.acc + ((size_t)b * p.S + (t - p.lo)) * p.S;
+    // row partial of each 32-key quarter (4 * nkt partials per row)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {  // fully unrolled: acc[] must stay in registers
-        const int j = k0 + (int)cq * 32 + i;
-        if (j >= p.lo && j < hi && j < p.T) dst[j - p.lo] += acc[i];
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float v = quad_sum(rs[r][q]);
+        if (c == 0 && row_ok[r] && t[r] >= p.lo && t[r] < hi)
+          p.row_part[(((size_t)b * p.H + h) * (4 * nkt) + 4 * kt + q) * p.S + (t[r] - p.lo)] = v;  // 0 for <eos>
       }
+    // column sums over the warp's 16 rows (lanes of equal c), then over the two warps of a 32-row quarter
+    float* cw = colsum + ((h & 1) * 8 + warp) * BLOCK;
+#pragma unroll
+    for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float v = cs[nb][e];
+        v += __shfl_xor_sync(0xffffffffu, v, 4);
+        v += __shfl_xor_sync(0xffffffffu, v, 8);
+        v += __shfl_xor_sync(0xffffffffu, v, 16);
+        if (g == 0) cw[nb * 8 + 2 * c + e] = v;
+      }
+    __syncthreads();  // every warp is done with stage s and has written its column sums
+    if (live && threadIdx.x == 0 && h + STAGES < p.H) load(h + STAGES);
+    const float* cr = colsum + (h & 1) * 8 * BLOCK;
+    for (int i = threadIdx.x; i < 4 * BLOCK; i += NUM_THREADS) {
+      const int rq = i / BLOCK, col = i % BLOCK, j = k0 + col;
+      if (j >= p.lo && j < hi && j < p.T)  // (4 * nqt partials per column; 0 for <eos> columns)
+        p.col_part[(((size_t)b * p.H + h) * (4 * nqt) + 4 * qt + rq) * p.S + (j - p.lo)] =
+            cr[(2 * rq) * BLOCK + col] + cr[(2 * rq + 1) * BLOCK + col];
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 16) {
-    tc_fence_after();
-    tmem_dealloc(tmem_s, TMEM_COLS);
+  // acc tile: this CTA is the only writer of acc[b, rows of qt, columns of kt]; layers are separate launches
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (!ri[r]) continue;
+    float* dst = p.acc + ((size_t)b * p.S + (t[r] - p.lo)) * p.S;
+#pragma unroll
+    for (int nb = 0; nb < 16; ++nb)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = k0 + nb * 8 + 2 * (int)c + e;
+        if (j >= p.lo && j < hi && j < p.T) dst[j - p.lo] += acc[nb][2 * r + e];
+      }
   }
 }
 

@@ -1,4 +1,4 @@
-// esm_b200 — need_head_weights=True: the normalised attention probabilities (sm_100a, head_dim 64).
+// esm_b200 — need_head_weights=True: the normalised attention probabilities (sm_90a).
 #pragma once
 
 #include "attention_common.cuh"
@@ -7,8 +7,8 @@ namespace esmb200 {
 
 // ---------------------------------------------------------------------------------------------------------------
 // need_head_weights=True: materialise the normalised probabilities (multihead_attention.py:379,397-400).
-// One CTA per (key block, query block, sequence*head): S = Q K^T again on the tensor core, then
-// p = exp(s - rowmax) / rowsum with the row statistics saved by attention_fwd_kernel, fp32 [B,H,T,T].
+// One CTA per (key block, query block, sequence*head): S = Q K^T again on the tensor cores (eight warps of 16 query
+// rows x 128 keys), then p = exp(s - rowmax) / rowsum with the row statistics saved by the forward kernel, fp32 [B,H,T,T].
 // ---------------------------------------------------------------------------------------------------------------
 struct ProbsParams {
   int B, T, H, E;
@@ -25,31 +25,25 @@ struct ProbsParams {
 };
 
 namespace probs_cfg {
-constexpr int NUM_THREADS = 128;
-constexpr int TMEM_COLS = 128;
+constexpr int NUM_THREADS = 256;
 constexpr int BLOCK_Q = 128, BLOCK_KV = 128;
-constexpr int SMEM_BYTES_SPLIT = 4 * attn_cfg::TILE_BYTES + 1024 + 64 + 4 * 32 * 33 * 4;  // fp32x3: Q, K as hi | lo
-constexpr int SMEM_BYTES = 2 * attn_cfg::TILE_BYTES + 1024 + 64 + 4 * 32 * 33 * 4;  // + per-warp transpose tiles
+constexpr int smem_bytes(int np) { return 2 * np * attn_cfg::TILE_BYTES + 1024 + 64; }
 }  // namespace probs_cfg
 
 // MODE 0: fp16 operands, head_dim <= 64 | 1 (SPLIT): fp32x3 hi|lo operands | 2: two 64-wide slots per head
 template <int MODE>
-__global__ void __launch_bounds__(probs_cfg::NUM_THREADS, MODE ? 2 : 4)
+__global__ void __launch_bounds__(probs_cfg::NUM_THREADS, MODE ? 1 : 2)
 attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const ProbsParams p) {
   using namespace attn_cfg;
   using namespace probs_cfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr bool SPLIT = MODE == 1;
   constexpr int NP = MODE ? 2 : 1;
-  uint8_t* smem_q = smem;                    // [hi | lo]
-  uint8_t* smem_k = smem + NP * TILE_BYTES;  // [hi | lo]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * NP * TILE_BYTES);
-  uint64_t* ld_full = bars;
-  uint64_t* mma_done = bars + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
+  uint8_t* smem_q = smem;                    // [hi | lo] or [slot 0 | slot 1]
+  uint8_t* smem_k = smem + NP * TILE_BYTES;  // [hi | lo] or [slot 0 | slot 1]
+  uint64_t* ld_full = reinterpret_cast<uint64_t*>(smem + 2 * NP * TILE_BYTES);
 
-  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
   const int kb = blockIdx.x, qb = blockIdx.y;
   const int b = blockIdx.z / p.H, h = blockIdx.z % p.H;
   const int q0 = qb * BLOCK_Q, k0 = kb * BLOCK_KV;
@@ -57,113 +51,71 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const Probs
 
   if (threadIdx.x == 0) {
     mbar_init(ld_full, 1);
-    mbar_init(mma_done, 1);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, probs_cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_s = *tmem_slot;
   const bool live = k0 < p.kvlen[b];  // otherwise every key of this block is masked: probabilities are exactly 0
 
-  if (live && threadIdx.x == 0) {
-    mbar_arrive_expect_tx(ld_full, 2 * NP * TILE_BYTES);
-    const int hc = h * HEAD_DIM * (MODE == 2 ? 2 : 1), po = MODE == 2 ? HEAD_DIM : p.lo_off;
+  float s[16][4];
 #pragma unroll
-    for (int part = 0; part < NP; ++part) {
-      tma_load_2d(smem_q + part * TILE_BYTES, &tmap_qkv, ld_full, hc + part * po, row_base + q0);
-      tma_load_2d(smem_k + part * TILE_BYTES, &tmap_qkv, ld_full, p.E + hc + part * po, row_base + k0);
+  for (int i = 0; i < 16; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+  if (live) {
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(ld_full, 2 * NP * TILE_BYTES);
+      const int hc = h * HEAD_DIM * (MODE == 2 ? 2 : 1), po = MODE == 2 ? HEAD_DIM : p.lo_off;
+#pragma unroll
+      for (int part = 0; part < NP; ++part) {
+        tma_load_2d(smem_q + part * TILE_BYTES, &tmap_qkv, ld_full, hc + part * po, row_base + q0);
+        tma_load_2d(smem_k + part * TILE_BYTES, &tmap_qkv, ld_full, p.E + hc + part * po, row_base + k0);
+      }
     }
     mbar_wait(ld_full, 0);
-    tc_fence_after();
-    constexpr uint32_t idesc_qk = umma_idesc_f16(128, 128, false);
-    const uint64_t qdesc = umma_smem_desc_sw128(smem_u32(smem_q), 1024, 0);
-    const uint64_t kdesc = umma_smem_desc_sw128(smem_u32(smem_k), 1024, 0);
-#pragma unroll
-    for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_s, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-    if constexpr (SPLIT) {
-      const uint64_t qlo = umma_smem_desc_sw128(smem_u32(smem_q + TILE_BYTES), 1024, 0);
-      const uint64_t klo = umma_smem_desc_sw128(smem_u32(smem_k + TILE_BYTES), 1024, 0);
-#pragma unroll
-      for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_s, qlo + 2 * k, kdesc + 2 * k, idesc_qk, 1u);
-#pragma unroll
-      for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_s, qdesc + 2 * k, klo + 2 * k, idesc_qk, 1u);
+    const uint32_t qs = smem_u32(smem_q), ks = smem_u32(smem_k);
+    qk_tile<16>(s, qs, warp * 16, ks, 0);
+    if constexpr (MODE == 1) {  // + q_lo k_hi + q_hi k_lo
+      qk_tile<16>(s, qs + TILE_BYTES, warp * 16, ks, 0);
+      qk_tile<16>(s, qs, warp * 16, ks + TILE_BYTES, 0);
     }
-    if constexpr (MODE == 2) {  // + q[slot 1] . k[slot 1]
-      const uint64_t q1 = umma_smem_desc_sw128(smem_u32(smem_q + TILE_BYTES), 1024, 0);
-      const uint64_t k1 = umma_smem_desc_sw128(smem_u32(smem_k + TILE_BYTES), 1024, 0);
-#pragma unroll
-      for (int k = 0; k < HEAD_DIM / 16; ++k) umma_ss(tmem_s, q1 + 2 * k, k1 + 2 * k, idesc_qk, 1u);
-    }
-    tc_commit(mma_done);
+    if constexpr (MODE == 2) qk_tile<16>(s, qs + TILE_BYTES, warp * 16, ks + TILE_BYTES, 0);  // + q[slot 1] . k[slot 1]
   }
-  __syncwarp();
 
-  // Each thread owns one query row in TMEM; the 32x32 fp32 piece of a warp is transposed through padded shared
-  // memory so that every global store instruction writes one 128-byte row segment (lane = key column).
-  const uint32_t quarter = warp % 4;
-  const int t_warp0 = q0 + quarter * 32;       // first query row of this warp
-  const int t = t_warp0 + lane;
-  const bool row_ok = t < p.T;
   const int ncols = min(BLOCK_KV, p.T - k0);
-  float* tile = reinterpret_cast<float*>(smem + 2 * NP * TILE_BYTES + 64) + warp * (32 * 33);
-  float* base = p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + k0;
-  float mneg = 0.f, inv = 0.f;
   uint32_t kw[4] = {0u, 0u, 0u, 0u};
   if (live) {
-    const size_t si = ((size_t)b * p.H + h) * p.T + (row_ok ? t : 0);
-    mneg = -p.row_max[si] * LOG2E;
-    const float l = p.row_sum[si];
-    inv = l > 0.f ? 1.0f / l : 0.f;
-    // esm2.py:135-139: rows of padded QUERY tokens are zero in the stacked result (padded key columns already are)
-    if (p.zero_pad_rows && row_ok && !((p.keybits[(size_t)b * p.words + (t >> 5)] >> (t & 31)) & 1u)) inv = 0.f;
     const uint4 kw4 = __ldg(reinterpret_cast<const uint4*>(p.keybits + (size_t)b * p.words + kb * 4));
     kw[0] = kw4.x; kw[1] = kw4.y; kw[2] = kw4.z; kw[3] = kw4.w;
-    mbar_wait(mma_done, 0);
-    tc_fence_after();
   }
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    if (c * 32 >= ncols) break;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int t = q0 + (int)(warp * 16 + g + 8 * r);
+    if (t >= p.T) continue;
+    float mneg = 0.f, inv = 0.f;
     if (live) {
-      uint32_t sv[32];
-      tmem_ld_32x32b_x32(tmem_s + ((quarter * 32u) << 16) + c * 32, sv);
-      tmem_wait_ld_dep(sv);
-      const uint32_t w = kw[c];
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        tile[lane * 33 + i] = ((w >> i) & 1u) ? ex2_approx(fmaf(__uint_as_float(sv[i]), LOG2E, mneg)) * inv : 0.f;
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) tile[lane * 33 + i] = 0.f;
+      const size_t si = ((size_t)b * p.H + h) * p.T + t;
+      mneg = -p.row_max[si] * LOG2E;
+      const float l = p.row_sum[si];
+      inv = l > 0.f ? 1.0f / l : 0.f;
+      // esm2.py:135-139: rows of padded QUERY tokens are zero in the stacked result (padded key columns already are)
+      if (p.zero_pad_rows && !((p.keybits[(size_t)b * p.words + (t >> 5)] >> (t & 31)) & 1u)) inv = 0.f;
     }
-    __syncwarp();
-    const int col = c * 32 + lane;
-    if (col < ncols) {
-      const int nrows = min(32, p.T - t_warp0);
-      for (int r = 0; r < nrows; ++r) base[(size_t)(t_warp0 + r) * p.T + col] = tile[r * 33 + lane];
+    float* dst = p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + (size_t)t * p.T + k0;
+#pragma unroll
+    for (int nb = 0; nb < 16; ++nb) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int key = nb * 8 + 2 * (int)c + e;
+        if (key < ncols) dst[key] = masked_prob(s[nb][2 * r + e], kw[nb / 4], key, mneg, inv);
+      }
     }
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_s, probs_cfg::TMEM_COLS);
   }
 }
 
 template <int MODE>
 inline cudaError_t launch_attention_probs_mode(const CUtensorMap& tmap_qkv, const ProbsParams& p, cudaStream_t stream) {
   using namespace probs_cfg;
-  constexpr int smem = MODE ? SMEM_BYTES_SPLIT : SMEM_BYTES;
+  constexpr int smem = smem_bytes(MODE ? 2 : 1);
   dim3 grid((p.T + BLOCK_KV - 1) / BLOCK_KV, (p.T + BLOCK_Q - 1) / BLOCK_Q, p.B * p.H);
   cudaError_t e = cudaFuncSetAttribute(attention_probs_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;

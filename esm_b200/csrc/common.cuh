@@ -1,8 +1,8 @@
-// esm_b200 — shared device-side primitives for the sm_100a kernels.
+// esm_b200 — shared device-side primitives for the sm_90a (Hopper) kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell programming model used by every kernel in this
-// directory: mbarrier (transaction barriers), TMA bulk-tensor loads, tcgen05 MMA / TMEM
-// allocation / TMEM load-store / commit, plus UMMA shared-memory and instruction descriptors.
+// Thin inline-PTX wrappers for the Hopper programming model used by every kernel in this directory: mbarrier
+// (transaction barriers), TMA bulk-tensor loads / stores / reduce-adds, wgmma (warpgroup MMA from shared-memory
+// descriptors), warp-level mma.sync + ldmatrix on 128B-swizzled TMA tiles.
 // No CUTLASS/CuTe dependency: everything is spelled out so `cuobjdump -sass` maps 1:1 to source.
 #pragma once
 
@@ -53,7 +53,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 
-// make barrier inits visible to the async proxy (TMA / tcgen05.commit)
+// make barrier inits visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
@@ -178,222 +178,119 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, MMA, TMEM <-> registers
+// warp-level tensor-core MMA (mma.sync m16n8k16, fp16 in / fp32 accumulate) and ldmatrix
+// Fragment layouts (PTX ISA "Matrix fragments for mma.m16n8k16"), g = lane / 4, c = lane % 4:
+//   A (16x16): a0 = (g, 2c..2c+1)  a1 = (g+8, 2c..)  a2 = (g, 8+2c..)  a3 = (g+8, 8+2c..)
+//   B (16x8):  b0 = (k 2c..2c+1, n g)  b1 = (k 8+2c.., n g)
+//   C (16x8):  c0,c1 = (g, 2c..2c+1)  c2,c3 = (g+8, 2c..2c+1)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {  // whole warp
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// the same with the barrier's shared-memory byte address (lets the caller keep it in a uniform register)
-__device__ __forceinline__ void tc_commit_addr(uint32_t bar_smem_addr) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_smem_addr) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 covers fp16 and bf16 operands with fp32 accumulation
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
 }
 
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// byte address of 16-byte chunk `chunk` (0..7) of row `row` in a tile of 128-byte rows written by a TMA box with
+// CU_TENSOR_MAP_SWIZZLE_128B (tile base 1024-byte aligned): the chunk index is XORed with row % 8
+__device__ __forceinline__ uint32_t sw128(uint32_t base, uint32_t row, uint32_t chunk) {
+  return base + row * 128u + ((chunk ^ (row & 7u)) << 4);
+}
 
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
+// A fragment of the 16 x 16 block (rows r0.., K columns 16*kk..) of a K-major SW128 tile
+__device__ __forceinline__ void ldsm_a(uint32_t base, uint32_t r0, uint32_t kk, uint32_t (&a)[4]) {
+  const uint32_t l = lane_id();
+  ldsm_x4(sw128(base, r0 + (l & 15u), 2u * kk + (l >> 4)), a);
+}
+// B fragments of two n8 blocks (rows n0..n0+15 of a K-major SW128 tile, K columns 16*kk..): b[0..1] block n0, b[2..3] n0+8
+__device__ __forceinline__ void ldsm_b(uint32_t base, uint32_t n0, uint32_t kk, uint32_t (&b)[4]) {
+  const uint32_t l = lane_id();
+  ldsm_x4(sw128(base, n0 + (l & 7u) + ((l >> 4) << 3), 2u * kk + ((l >> 3) & 1u)), b);
+}
+// B fragments of two n8 blocks from an MN-major SW128 tile (rows = K index, 64 N-elements per row; V in P.V):
+// K rows 16*kk.., N columns n0..n0+15: b[0..1] block n0, b[2..3] block n0+8
+__device__ __forceinline__ void ldsm_bt(uint32_t base, uint32_t kk, uint32_t n0, uint32_t (&b)[4]) {
+  const uint32_t l = lane_id();
+  ldsm_x4_t(sw128(base, 16u * kk + (l & 15u), n0 / 8u + (l >> 4)), b);
+}
+
+// ---------------------------------------------------------------------------------------------
+// wgmma (warpgroup MMA, sm_90a): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory
+// ---------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major 128B-swizzled tile with 128-byte rows (64 fp16), as written by a TMA box
+// {64, rows} with CU_TENSOR_MAP_SWIZZLE_128B:  bits [0,14) address >> 4, [16,30) LBO >> 4 (unused for swizzled K-major),
+// [32,46) SBO >> 4 = 1024 B between 8-row groups, [62,64) layout 1 = SWIZZLE_128B.  A 16-element K step is +32 bytes.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void reg_fence_f(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+// m64n256k16, fp16 x fp16 -> fp32; d[128] per thread: d[4*i + 0..1] = (row w*16 + g, col 8i + 2c..), d[4*i + 2..3] = row + 8
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
 
-
-// wait for this thread's outstanding tcgen05.ld and make the compiler treat r[] as produced HERE (needed when a
-// tcgen05.ld was issued early as a prefetch: uses of r[] must not be scheduled above the wait)
-__device__ __forceinline__ void tmem_wait_ld_dep(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]),
-                 "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]),
-                 "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-
-// Compiler-only fence: makes r[] look (re)defined here without emitting an instruction. Used after ONE
-// tcgen05.wait::ld that retires several in-flight tcgen05.ld: the wait carries the dependency for its own operand
-// array, this pins the other arrays behind it.
-__device__ __forceinline__ void reg_fence16(uint32_t (&r)[16]) {
-  asm volatile("" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                    "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]));
-}
-__device__ __forceinline__ void reg_fence(uint32_t (&r)[32]) {
-  asm volatile(""
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]),
-                 "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]),
-                 "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-        "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]),
-        "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// thread-block cluster / CTA-pair (cta_group::2) primitives
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the same-offset mbarrier of CTA `cta` of this cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n"
-      :
-      : "r"(smem_u32(bar)), "r"(cta)
-      : "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> even CTA of the pair
-
-// TMA load issued by either CTA of a pair; completion bytes are credited to the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0,
-                                                 int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0),
-        "r"(c1)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// commit of cta_group::2 MMAs, arriving on the same-offset mbarrier in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair_addr(uint32_t bar_smem_addr, uint16_t cta_mask) {  // uniform-register form
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          bar_smem_addr),
-      "h"(cta_mask)
-      : "memory");
-}
-// 256 x N x 16 MMA across the CTA pair: each CTA supplies 128 rows of A and N/2 rows of B from its own smem
-__device__ __forceinline__ void umma_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+// register budget hand-off between warpgroups (producer gives registers to the MMA warpgroups)
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---------------------------------------------------------------------------------------------
 // TMA stores (shared -> global), bulk async-groups
@@ -420,49 +317,16 @@ __device__ __forceinline__ void tma_store_wait_read() {
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix/instruction descriptors")
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a 128B-swizzled tile whose rows are 128 bytes wide
-// (64 x 16-bit elements), as written by a TMA box {64, rows} with CU_TENSOR_MAP_SWIZZLE_128B.
-//   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) descriptor version (1 on sm_100)
-//   bits [61,64) layout: 2 = SWIZZLE_128B
-// K-major use (rows = M/N index, 64 K-elements per row): SBO = 1024 (8 rows x 128 B), LBO unused.
-// MN-major use (rows = K index, 64 MN-elements per row): SBO = 1024 between 8-row K groups,
-//   LBO = byte stride between 64-wide MN atoms (unused when the tile is 64 wide).
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor, kind::f16, fp16 A/B, fp32 accumulate.
-//   bits [4,6) D format (1 = f32)   [7,10) A format (0 = f16)   [10,13) B format (0 = f16)
-//   bit 15 A major (0 = K)          bit 16 B major (0 = K, 1 = MN)
-//   bits [17,23) N >> 3             bits [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n, bool b_mn_major) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | ((b_mn_major ? 1u : 0u) << 16) | ((n >> 3) << 17) |
-         ((m >> 4) << 24);
-}
-
-// ---------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): a kernel launched with the programmatic-stream-serialization attribute may
 // start while its predecessor on the stream is still draining; everything it does before pdl_wait() (barrier init,
-// TMEM allocation, tensor-map prefetch) overlaps the predecessor's tail.  pdl_wait() returns when the predecessor has
+// tensor-map prefetch) overlaps the predecessor's tail.  pdl_wait() returns when the predecessor has
 // completed and its memory is visible; both instructions are no-ops in a normal launch.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // process-wide switch: -1 = not read yet (environment ESMB200_PDL, default OFF); esmb200_set_option("pdl", v) overrides.
-// Measured on B200 (scripts/pdl_ab.py, profiles/r02_pdl_ab.json): alternating on/off inside one process, the 33-layer
-// forward takes 54.07 / 53.93 ms (B=32) and 423.4 / 421.1 ms (B=256) with / without the attribute — the kernels are
-// persistent, so every CTA of a kernel ends within microseconds of the others and there is no tail to overlap the next
-// prologue with, while early-resident dependents spin in griddepcontrol.wait.  Kept as an option, off by default.
+// Kept as an option, off by default.
 inline int& pdl_flag() {
   static int flag = -1;
   return flag;
@@ -501,34 +365,21 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// 2^x, MUFU.EX2 (max rel. error 2^-22; ex2(-inf) = +0)
-// packed fp32 pair arithmetic (FFMA2 / FADD2 on sm_100): one instruction for two lanes of data
+// fp32 pair helpers (two independent scalar operations; kept as pairs so the callers read like the math)
 __device__ __forceinline__ void fma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-  asm("{ .reg .b64 ra, rb, rc, rd;\n\t"
-      "mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5}; mov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\t"
-      "mov.b64 {%0, %1}, rd; }"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+  d0 = fmaf(a0, b0, c0);
+  d1 = fmaf(a1, b1, c1);
 }
 __device__ __forceinline__ void add2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{ .reg .b64 ra, rb, rd;\n\t"
-      "mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5};\n\t"
-      "add.rn.f32x2 rd, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rd; }"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = a0 + b0;
+  d1 = a1 + b1;
 }
-
 __device__ __forceinline__ void mul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{ .reg .b64 ra, rb, rd;\n\t"
-      "mov.b64 ra, {%2, %3}; mov.b64 rb, {%4, %5};\n\t"
-      "mul.rn.f32x2 rd, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rd; }"
-      : "=f"(d0), "=f"(d1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = a0 * b0;
+  d1 = a1 * b1;
 }
 
+// 2^x, MUFU.EX2 (max rel. error 2^-22; ex2(-inf) = +0)
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -1,4 +1,4 @@
-// esm_b200 — HBM-bound row kernels around the tensor-core GEMMs (sm_100a).
+// esm_b200 — HBM-bound row kernels around the tensor-core GEMMs (sm_90a).
 //
 //   layernorm_rows    esm/modules.py:68-81,124,137 and esm/model/esm2.py:123 (torch.nn.LayerNorm, eps 1e-5, affine),
 //                     one warp per row, the row held in registers (single HBM read), fp16 or fp32 output

@@ -1,14 +1,13 @@
-// esm_b200 — GEMM v2: CTA-pair (cta_group::2) tcgen05 GEMM with TMA-store / TMA-reduce epilogues (sm_100a).
+// esm_b200 — GEMM: persistent warp-specialised wgmma GEMM with fused epilogues (sm_90a).
 //
-// Same math and epilogues as gemm.cuh (see there for the reference lines each epilogue replaces); what changes is how
-// the SM pair is driven:
-//   * a cluster of 2 CTAs owns a 256x256 output tile; each CTA TMA-loads 128 rows of A and 128 rows (half of N) of B
-//     per 64-wide K slab, and ONE thread of the leader CTA issues tcgen05.mma.cta_group::2 (UMMA 256x256x16), so every
-//     byte of B staged in shared memory feeds both tensor cores (half the smem fill traffic per FLOP of v1);
-//   * 5-stage TMA ring (32 KB/stage/CTA), 2x256-column TMEM accumulator double buffer per CTA;
-//   * epilogue: TMEM -> registers (bias / q-scale+RoPE / erf-GELU) -> 128B-swizzled smem tile -> one TMA bulk store
-//     per 128x64 fp16 (or 128x32 fp32) block; the residual add is a TMA *reduce-add* into the fp32 stream, so x is
-//     never read back into the SM.
+//   out[M, N] = epilogue(A[M, K] . B[N, K]^T), A and B fp16 K-major, fp32 accumulation.
+//   * one CTA per SM walks 128 x 256 output tiles (tile = m_blk * tiles_n + n_blk, strided over the grid);
+//   * warpgroup 0: one thread streams 64-wide K slabs of A (128 rows) and B (256 rows) through a 4-stage TMA ring
+//     (48 KB per stage, 128B swizzle) and keeps running ahead into the next tile while the MMA warpgroups finish;
+//   * warpgroups 1 and 2: rows [0,64) and [64,128) of the tile, wgmma m64n256k16 straight from the swizzled stages,
+//     one slab in flight behind the one being issued; the accumulators (128 fp32 registers per thread) are turned into
+//     the output by the epilogue in registers: bias / q-scale + RoPE / erf-GELU, fp16 or fp32 stores, or the
+//     residual update x += y (each element has exactly one writer: no atomics, bit-reproducible).
 #pragma once
 
 #include "gemm_common.cuh"
@@ -16,561 +15,209 @@
 namespace esmb200 {
 
 namespace gemm2_cfg {
-constexpr int BLOCK_M = 128;   // rows per CTA
-constexpr int PAIR_M = 256;    // rows per cluster tile
+constexpr int BLOCK_M = 128;
 constexpr int BLOCK_N = 256;
-constexpr int HALF_N = 128;    // B rows loaded by each CTA
+constexpr int HALF_N = 128;   // B rows per TMA box (two boxes per stage)
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int STAGES = 5;
+constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int B_STAGE_BYTES = HALF_N * BLOCK_K * 2;   // 16 KB
+constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int ACC_STAGES = 2;
-constexpr int TMEM_COLS = 512;
 constexpr int BOX_M = 128;        // rows of an A-operand TMA box
-constexpr int NUM_THREADS = 384;  // warps 0-3: TMA / MMA / TMEM alloc / spare, warps 4-11: epilogue (168 regs/thread:
-                                  // 3 warps per SMSP share its 16 K registers; setmaxnreg 40/232 was tried — ptxas 12.9
-                                  // then spills the control warps or fails to allocate the epilogue branch)
-constexpr int FIRST_EPI_WARP = 4;
-constexpr int STG_BYTES = 128 * 128;  // 128 rows x 128 B staging tile
-constexpr int NUM_STG = 4;            // 2 per 128-column half
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + NUM_STG * STG_BYTES + 1024 + 256;
+constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 }  // namespace gemm2_cfg
 
-// thread `row` writes its 8 x 16-byte chunks of a 128-byte row into a SWIZZLE_128B staging tile
-__device__ __forceinline__ void stage_row_sw128(uint8_t* stg, uint32_t row, const uint32_t (&v)[32]) {
-  const uint32_t base = smem_u32(stg) + row * 128;
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const uint32_t addr = base + (((uint32_t)c ^ (row & 7u)) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[4 * c]), "r"(v[4 * c + 1]),
-                 "r"(v[4 * c + 2]), "r"(v[4 * c + 3])
-                 : "memory");
-  }
-}
-
-// (a variant writing fp16 rows straight from registers to global memory, without smem staging, measured slower:
-// profiles/r01_epilogue_experiments.txt)
 // SPLIT ("fp32x3" precision): both operands are stored as fp16 hi | lo halves along K (A [M,2K], B [N,2K]); the K loop
 // runs hi*hi + lo*hi + hi*lo (three passes over the same fp32 accumulator: 22 significand bits per operand, the
 // dropped lo*lo term is 2^-22 relative), and fp16 outputs are written as hi | lo pairs as well (lo part p.lo_col_off
-// columns to the right).  Requires K % 64 == 0.
+// columns to the right, row pitch 2 * ldo).  Requires K % 64 == 0.
 template <int EPI, bool SPLIT = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(gemm2_cfg::NUM_THREADS, 1)
+__global__ void __launch_bounds__(gemm2_cfg::NUM_THREADS, 1)
 gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+                 const GemmParams p) {
   using namespace gemm2_cfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint8_t* smem_stg = smem + STAGES * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + NUM_STG * STG_BYTES);
-  uint64_t* full_bar = bars;                              // [STAGES]     used in the leader CTA only
-  uint64_t* empty_bar = bars + STAGES;                    // [STAGES]     one per CTA
-  uint64_t* tfull_bar = bars + 2 * STAGES;                // [ACC_STAGES] one per CTA
-  uint64_t* tempty_bar = bars + 2 * STAGES + ACC_STAGES;  // [ACC_STAGES] used in the leader CTA only
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * ACC_STAGES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* full_bar = bars;            // [STAGES] TMA -> MMA
+  uint64_t* empty_bar = bars + STAGES;  // [STAGES] MMA warpgroups -> TMA (one arrival each)
 
-  const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0);  // warp-uniform for the compiler
-  const uint32_t lane = threadIdx.x % 32;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  const int tiles_m = (p.M + PAIR_M - 1) / PAIR_M;
+  const uint32_t wg = __shfl_sync(0xffffffffu, threadIdx.x / 128, 0);
+  const int tiles_m = (p.M + BLOCK_M - 1) / BLOCK_M;
   const int tiles_n = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = tiles_m * tiles_n;
   const int num_kb1 = (p.K + BLOCK_K - 1) / BLOCK_K;  // a partial last K slab is zero-filled by TMA on both operands
   const int num_kb = SPLIT ? 3 * num_kb1 : num_kb1;   // SPLIT: slab kb/3, operand halves by kb%3
-  // Tile walk of this cluster (tile = m_blk * tiles_n + n_blk).  Default: strided — at any moment the clusters cover a few
-  // adjacent 256-row slabs of A and all of B, which keeps a long-K A slab (fc2: 2.6 MB) L2-resident while it is reused.
-  // p.chunked: one contiguous run per cluster, so consecutive tiles share their rows (the RoPE epilogue then reloads
-  // its cos/sin registers once per slab); only for short K, where 74 concurrent A slabs fit the L2.
-  int tile_first, tile_step, tile_count;
-  if (p.chunked) {
-    const int per = num_tiles / num_clusters, rem = num_tiles % num_clusters;
-    tile_first = cluster_id * per + (cluster_id < rem ? cluster_id : rem);
-    tile_count = per + (cluster_id < rem ? 1 : 0);
-    tile_step = 1;
-  } else {
-    tile_first = cluster_id;
-    tile_step = num_clusters;
-    tile_count = cluster_id < num_tiles ? (num_tiles - cluster_id + num_clusters - 1) / num_clusters : 0;
-  }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_out);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 2);   // one arrival per CTA of the pair (+ the transaction bytes of both)
-      mbar_init(&empty_bar[i], 1);  // multicast tcgen05.commit from the leader
-    }
-    for (int i = 0; i < ACC_STAGES; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 16);  // 8 epilogue warps x 2 CTAs
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc_pair(tmem_slot, TMEM_COLS);
-    tmem_relinquish_pair();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
+  __syncthreads();
   pdl_launch_dependents();
-  pdl_wait();  // A (and x for the reduce-add) come from the previous kernel on the stream
-  const uint32_t tmem_base = *tmem_slot;
+  pdl_wait();  // A (and x for the residual update) come from the previous kernel on the stream
 
-  if (warp == 0) {
-    // ===================== TMA producer (one lane per CTA) =====================
-    if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = tile_first, it = 0; it < tile_count; tile += tile_step, ++it) {
-        const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
-        const int a_row = m_blk * PAIR_M + rank * BLOCK_M;
-        const int b_row = n_blk * BLOCK_N + rank * HALF_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait_relaxed(&empty_bar[stage], phase ^ 1);
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / tiles_n) * BLOCK_M, n0 = (tile % tiles_n) * BLOCK_N;
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const uint32_t s = it % STAGES;
+          while (!mbar_try_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1)) __nanosleep(64);
           int a_col = kb * BLOCK_K, b_col = kb * BLOCK_K;
           if constexpr (SPLIT) {
             const int part = kb % 3;  // 0: hi*hi, 1: lo*hi, 2: hi*lo
             a_col = (kb / 3) * BLOCK_K + (part == 1 ? p.K : 0);
             b_col = (kb / 3) * BLOCK_K + (part == 2 ? p.K : 0);
           }
-          tma_load_2d_pair(smem_a + stage * A_STAGE_BYTES, &tmap_a, &full_bar[stage], a_col, a_row);
-          tma_load_2d_pair(smem_b + stage * B_STAGE_BYTES, &tmap_b, &full_bar[stage], b_col, b_row);
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * STAGE_BYTES);
-          else mbar_arrive_remote(&full_bar[stage], 0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
+          tma_load_2d(smem_a + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], a_col, m0);
+          tma_load_2d(smem_b + s * B_STAGE_BYTES, &tmap_b, &full_bar[s], b_col, n0);
+          tma_load_2d(smem_b + s * B_STAGE_BYTES + HALF_N * 128, &tmap_b, &full_bar[s], b_col, n0 + HALF_N);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA): the whole warp runs the loop, one elected lane issues =====================
-    // Convergent control flow + operands derived from warp-uniform values keep descriptors, TMEM addresses and barrier
-    // addresses in uniform registers, so the four UTCHMMA of a K slab and the commit are issued back to back.  With
-    // `if (lane == 0)` around the loop ptxas wrapped every tcgen05 instruction in an ELECT / R2UR.BROADCAST / BRA.U.ANY
-    // waterfall (~94 cycles each, measured in the attention kernel): 5 x 94 per slab against 512 cycles of tensor work.
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_f16(PAIR_M, BLOCK_N, false);
-      const uint32_t u_smem = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-      const uint32_t u_a = u_smem, u_b = u_smem + STAGES * A_STAGE_BYTES;
-      const uint32_t u_bars = u_smem + STAGES * STAGE_BYTES + NUM_STG * STG_BYTES;
-      const uint32_t u_empty = u_bars + STAGES * 8, u_tfull = u_bars + 2 * STAGES * 8;
-      const uint32_t u_tmem = __shfl_sync(0xffffffffu, tmem_base, 0);
-      uint32_t stage = 0, phase = 0;
-      int iter = 0;
-      for (int tile = tile_first; iter < tile_count; tile += tile_step, ++iter) {
-        const uint32_t as = iter & 1, aph = (iter >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = u_tmem + as * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = umma_smem_desc_sw128(u_a + stage * A_STAGE_BYTES, 1024, 0);
-          const uint64_t bdesc = umma_smem_desc_sw128(u_b + stage * B_STAGE_BYTES, 1024, 0);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_ss_pair(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            tc_commit_pair_addr(u_empty + stage * 8, 0b11);
-            if (kb == num_kb - 1) tc_commit_pair_addr(u_tfull + as * 8, 0b11);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= FIRST_EPI_WARP) {
-    // ===================== epilogue: TMEM -> regs -> swizzled smem -> TMA store / reduce =====================
-    const uint32_t ew = warp - FIRST_EPI_WARP;
-    const uint32_t quarter = warp % 4;
-    const uint32_t chalf = ew / 4;
-    const uint32_t row_local = quarter * 32 + lane;
-    const bool issuer = (ew % 4 == 0) && lane == 0;
-    const uint32_t bar_id = 1 + chalf;
-    uint32_t store_iter = 0;
-    int iter = 0;
-    [[maybe_unused]] float rc[32], rs[32];  // EPI_QKV_ROPE: cos / sin of this thread's row
-    [[maybe_unused]] int rope_blk = -1;
-    [[maybe_unused]] int rope_row = 0;      // row of the current tile (set per tile)
-    // table columns [slot*32, slot*32 + 32) of this thread's token position -> rc / rs
-    [[maybe_unused]] auto load_rope = [&](int slot) {
-      const int t = (rope_row < p.M) ? (rope_row % p.T) : 0;
-      const int ld = p.rope_ld == 64 ? 64 : 32;
-      const float4* cs4 = reinterpret_cast<const float4*>(p.rope_cos + (size_t)t * ld + slot * 32);
-      const float4* sn4 = reinterpret_cast<const float4*>(p.rope_sin + (size_t)t * ld + slot * 32);
-#pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        const float4 c = __ldg(cs4 + j4), sn = __ldg(sn4 + j4);
-        rc[4 * j4 + 0] = c.x; rc[4 * j4 + 1] = c.y; rc[4 * j4 + 2] = c.z; rc[4 * j4 + 3] = c.w;
-        rs[4 * j4 + 0] = sn.x; rs[4 * j4 + 1] = sn.y; rs[4 * j4 + 2] = sn.z; rs[4 * j4 + 3] = sn.w;
-      }
-    };
-    for (int tile = tile_first; iter < tile_count; tile += tile_step, ++iter) {
-      const int m_blk = tile / tiles_n, n_blk = tile % tiles_n;
-      const uint32_t as = iter & 1, aph = (iter >> 1) & 1;
-      const int row0 = m_blk * PAIR_M + rank * BLOCK_M;
-      const int row = row0 + row_local;
-      rope_row = row;
-      if constexpr (EPI == EPI_QKV_ROPE) {  // before the wait: the loads fly while the tile is still being multiplied
-      // cos/sin of this thread's token position, 64 registers, reloaded only when the 256-row slab changes (tiles are
-      // walked n-fastest, so once per tiles_n tiles) — r01 re-read them from L2 for every 64-column head group
-      // (256 B per thread and group, long-scoreboard stalls in the shortest-K GEMM of the layer).
-      if (p.rope_cos != nullptr && m_blk != rope_blk && p.rope_ld != 64) {
-        rope_blk = m_blk;
-        load_rope(0);
-      }
-      }
-      mbar_wait(&tfull_bar[as], aph);
-      tc_fence_after();
-      const uint32_t taddr0 = tmem_base + ((quarter * 32u) << 16) + as * BLOCK_N + chalf * 128;
-      const int col0 = n_blk * BLOCK_N + chalf * 128;
-
-      if constexpr (SPLIT && (EPI == EPI_BIAS_GELU || EPI == EPI_QKV_ROPE)) {
-        // fp32x3 precision: the fp32 result y of every element is written as fp16 hi = rn(y) and lo = rn(y - hi)
-        const bool rope = EPI == EPI_QKV_ROPE && p.rope_cos != nullptr;
-#pragma unroll 1
-        for (int g = 0; g < 2; ++g) {
-          const int col = col0 + g * 64;
-          if (col >= p.N) break;  // uniform over the 4 warps of this column half
-          uint32_t lo[32], hi[32];
-          tmem_ld_32x32b_x32(taddr0 + g * 64, lo);
-          tmem_ld_32x32b_x32(taddr0 + g * 64 + 32, hi);
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + col);
-          const int sect = (EPI == EPI_QKV_ROPE) ? col / p.E : 2;
-          const float sc = (EPI == EPI_QKV_ROPE && sect == 0) ? p.q_scale : 1.0f;
-          tmem_wait_ld_dep(lo);
-          reg_fence(hi);
-#pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) {
-            const float4 bl = __ldg(b4 + j4), bh = __ldg(b4 + 8 + j4);
-            const float bls[4] = {bl.x, bl.y, bl.z, bl.w}, bhs[4] = {bh.x, bh.y, bh.z, bh.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int j = 4 * j4 + e;
-              float a = __uint_as_float(lo[j]) + bls[e], b = __uint_as_float(hi[j]) + bhs[e];
-              if constexpr (EPI == EPI_BIAS_GELU) {
-                a = gelu_erf(a);
-                b = gelu_erf(b);
-              } else {
-                a *= sc;
-                b *= sc;
-                if (sect < 2 && rope) {
-                  const float ra = a * rc[j] - b * rs[j], rb = b * rc[j] + a * rs[j];
-                  a = ra;
-                  b = rb;
-                }
-              }
-              lo[j] = __float_as_uint(a);
-              hi[j] = __float_as_uint(b);
-            }
-          }
-#pragma unroll 1
-          for (int part = 0; part < 2; ++part) {
-            uint8_t* stg = smem_stg + (chalf * 2 + (store_iter & 1)) * STG_BYTES;
-            if (issuer) tma_store_wait_read<1>();
-            named_bar_sync(bar_id, 128);
-            const uint32_t srow = smem_u32(stg) + row_local * 128;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              const uint32_t (&src)[32] = c < 4 ? lo : hi;
-              const int o = (c & 3) * 8;
-              uint32_t w4[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float y0 = __uint_as_float(src[o + 2 * q]), y1 = __uint_as_float(src[o + 2 * q + 1]);
-                const __half2 h2 = __floats2half2_rn(y0, y1);
-                if (part == 0) {
-                  w4[q] = *reinterpret_cast<const uint32_t*>(&h2);
-                } else {
-                  const float2 f = __half22float2(h2);
-                  w4[q] = pack_half2(y0 - f.x, y1 - f.y);
-                }
-              }
-              const uint32_t addr = srow + (((uint32_t)c ^ (row_local & 7u)) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(w4[0]), "r"(w4[1]), "r"(w4[2]),
-                           "r"(w4[3])
-                           : "memory");
-            }
-            fence_proxy_async_smem();
-            named_bar_sync(bar_id, 128);
-            if (issuer && row0 < p.M) {
-              tma_store_2d(&tmap_out, stg, col + part * p.lo_col_off, row0);
-              tma_store_commit();
-            }
-            ++store_iter;
-          }
-        }
-      } else if constexpr (EPI == EPI_BIAS_GELU || EPI == EPI_GELU_MATHONLY || EPI == EPI_F16_STOREONLY ||
-                    EPI == EPI_FMA_MATHONLY) {
-        // All four 32-column TMEM loads of this warp's 128 columns are issued back to back and retired by ONE
-        // tcgen05.wait::ld: measured on B200 (profiles/r01_epilogue_experiments.txt) every extra ld->wait round trip
-        // in the epilogue slows the concurrently running MMA mainloop (4 waits per tile: -15 %, 1 wait: -0 %).
-        // Each 32-column piece is then biased, GELU'd, packed to fp16 and written to the staging tile right away so
-        // that only the 128 accumulator registers stay live.
-        uint32_t acc[4][32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (col0 + c * 32 < p.N) tmem_ld_32x32b_x32(taddr0 + c * 32, acc[c]);
-        tmem_wait_ld_dep(acc[0]);
-        reg_fence(acc[1]);
-        reg_fence(acc[2]);
-        reg_fence(acc[3]);
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          const int col = col0 + g * 64;
-          if (col >= p.N) break;  // uniform over the 4 warps of this column half
-          uint8_t* stg = smem_stg + (chalf * 2 + (store_iter & 1)) * STG_BYTES;
-          if constexpr (EPI != EPI_GELU_MATHONLY && EPI != EPI_FMA_MATHONLY) {
-            if (issuer) tma_store_wait_read<1>();  // the store that used this buffer two iterations ago has read it
-            named_bar_sync(bar_id, 128);
-          }
-          const uint32_t srow = smem_u32(stg) + row_local * 128;
-          uint32_t sink = 0;
-#pragma unroll
-          for (int hf = 0; hf < 2; ++hf) {
-            const uint32_t (&a)[32] = acc[2 * g + hf];
-            const float4* b4 = reinterpret_cast<const float4*>(p.bias + col + hf * 32);
-#pragma unroll
-            for (int v = 0; v < 4; ++v) {  // 8 columns -> one 16-byte chunk of the 128-byte staging row
-              const float4 b0 = __ldg(b4 + 2 * v), b1 = __ldg(b4 + 2 * v + 1);
-              auto act = [](float x) {
-                if constexpr (EPI == EPI_F16_STOREONLY) return x;
-                else if constexpr (EPI == EPI_FMA_MATHONLY) {
-                  float y = x;
-#pragma unroll
-                  for (int q = 0; q < 15; ++q) y = fmaf(y, x, 0.125f);
-                  return y;
-                } else return gelu_erf(x);
-              };
-              uint32_t o0, o1, o2, o3;
-              if constexpr (EPI == EPI_BIAS_GELU) {  // product path: packed f32x2 GELU
-                float y[8], xb[8];
-                add2(xb[0], xb[1], __uint_as_float(a[8 * v + 0]), __uint_as_float(a[8 * v + 1]), b0.x, b0.y);
-                add2(xb[2], xb[3], __uint_as_float(a[8 * v + 2]), __uint_as_float(a[8 * v + 3]), b0.z, b0.w);
-                add2(xb[4], xb[5], __uint_as_float(a[8 * v + 4]), __uint_as_float(a[8 * v + 5]), b1.x, b1.y);
-                add2(xb[6], xb[7], __uint_as_float(a[8 * v + 6]), __uint_as_float(a[8 * v + 7]), b1.z, b1.w);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) gelu_erf2(xb[2 * q], xb[2 * q + 1], y[2 * q], y[2 * q + 1]);
-                o0 = pack_half2(y[0], y[1]);
-                o1 = pack_half2(y[2], y[3]);
-                o2 = pack_half2(y[4], y[5]);
-                o3 = pack_half2(y[6], y[7]);
-              } else {
-                o0 = pack_half2(act(__uint_as_float(a[8 * v + 0]) + b0.x), act(__uint_as_float(a[8 * v + 1]) + b0.y));
-                o1 = pack_half2(act(__uint_as_float(a[8 * v + 2]) + b0.z), act(__uint_as_float(a[8 * v + 3]) + b0.w));
-                o2 = pack_half2(act(__uint_as_float(a[8 * v + 4]) + b1.x), act(__uint_as_float(a[8 * v + 5]) + b1.y));
-                o3 = pack_half2(act(__uint_as_float(a[8 * v + 6]) + b1.z), act(__uint_as_float(a[8 * v + 7]) + b1.w));
-              }
-              if constexpr (EPI == EPI_GELU_MATHONLY || EPI == EPI_FMA_MATHONLY) {
-                sink ^= o0 ^ o1 ^ o2 ^ o3;
-              } else {
-                const uint32_t chunk = (uint32_t)(hf * 4 + v);
-                const uint32_t addr = srow + ((chunk ^ (row_local & 7u)) << 4);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(o0), "r"(o1), "r"(o2), "r"(o3)
-                             : "memory");
-              }
-            }
-          }
-          if constexpr (EPI == EPI_GELU_MATHONLY || EPI == EPI_FMA_MATHONLY) {
-            if (sink == 0x7fffffffu && row == -1) reinterpret_cast<uint32_t*>(p.out)[0] = sink;
-          } else {
-            fence_proxy_async_smem();
-            named_bar_sync(bar_id, 128);
-            if (issuer && row0 < p.M) {  // rows past M are clipped by the tensor map; a fully outside box is skipped
-              tma_store_2d(&tmap_out, stg, col, row0);
-              tma_store_commit();
-            }
-            ++store_iter;
-          }
-        }
-      } else if constexpr (EPI == EPI_QKV_ROPE) {
-        const bool rope = p.rope_cos != nullptr;
-#pragma unroll 1
-        for (int g = 0; g < 2; ++g) {
-          const int col = col0 + g * 64;
-          if (col >= p.N) break;  // uniform over the 4 warps of this column half
-          uint32_t lo[32], hi[32];
-          tmem_ld_32x32b_x32(taddr0 + g * 64, lo);
-          tmem_ld_32x32b_x32(taddr0 + g * 64 + 32, hi);
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + col);
-          const int sect = col / p.E;  // 0 q, 1 k, 2 v
-          const float sc = (sect == 0) ? p.q_scale : 1.0f;
-          // head_dim > 64: two 64-wide slots per head with different frequencies — reload per group (15B only)
-          if (rope && sect < 2 && p.rope_ld == 64) load_rope((col >> 6) & 1);
-          tmem_wait_ld_dep(lo);  // one wait retires both loads
-          reg_fence(hi);
-          if (sect < 2 && rope) {
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) {
-              const float4 bl = __ldg(b4 + j4), bh = __ldg(b4 + 8 + j4);
-              const float bls[4] = {bl.x, bl.y, bl.z, bl.w}, bhs[4] = {bh.x, bh.y, bh.z, bh.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int j = 4 * j4 + e;
-                const float a = (__uint_as_float(lo[j]) + bls[e]) * sc, b = (__uint_as_float(hi[j]) + bhs[e]) * sc;
-                lo[j] = __float_as_uint(a * rc[j] - b * rs[j]);  // rotary_embedding.py:16-20, rotate_half = cat(-x2, x1)
-                hi[j] = __float_as_uint(b * rc[j] + a * rs[j]);
-              }
-            }
-          } else {  // v, or q/k without rotary embedding (MSA axial attention): bias (+ q scale) only
-#pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) {
-              const float4 bl = __ldg(b4 + j4), bh = __ldg(b4 + 8 + j4);
-              const float bls[4] = {bl.x, bl.y, bl.z, bl.w}, bhs[4] = {bh.x, bh.y, bh.z, bh.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int j = 4 * j4 + e;
-                lo[j] = __float_as_uint((__uint_as_float(lo[j]) + bls[e]) * sc);
-                hi[j] = __float_as_uint((__uint_as_float(hi[j]) + bhs[e]) * sc);
-              }
-            }
-          }
-          uint8_t* stg = smem_stg + (chalf * 2 + (store_iter & 1)) * STG_BYTES;
-          if (issuer) tma_store_wait_read<1>();
-          named_bar_sync(bar_id, 128);
-          const uint32_t srow = smem_u32(stg) + row_local * 128;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {  // 8 columns -> one 16-byte chunk of the 128-byte staging row
-            const uint32_t (&src)[32] = c < 4 ? lo : hi;
-            const int o = (c & 3) * 8;
-            const uint32_t addr = srow + (((uint32_t)c ^ (row_local & 7u)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr),
-                         "r"(pack_half2(__uint_as_float(src[o + 0]), __uint_as_float(src[o + 1]))),
-                         "r"(pack_half2(__uint_as_float(src[o + 2]), __uint_as_float(src[o + 3]))),
-                         "r"(pack_half2(__uint_as_float(src[o + 4]), __uint_as_float(src[o + 5]))),
-                         "r"(pack_half2(__uint_as_float(src[o + 6]), __uint_as_float(src[o + 7])))
-                         : "memory");
-          }
-          fence_proxy_async_smem();
-          named_bar_sync(bar_id, 128);
-          if (issuer && row0 < p.M) {
-            tma_store_2d(&tmap_out, stg, col, row0);
-            tma_store_commit();
-          }
-          ++store_iter;
-        }
-#ifdef ESMB200_EXPERIMENTS
-      } else if constexpr (EPI == EPI_LD_X16) {  // profiling only: 8 loads of 16 columns
-        uint32_t sink = 0;
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          uint32_t acc[16];
-          tmem_ld_32x32b_x16(taddr0 + c * 16, acc);
-          tmem_wait_ld();
-          sink ^= acc[c];
-        }
-        if (sink == 0x7fffffffu && row == -1) reinterpret_cast<uint32_t*>(p.out)[0] = sink;
-      } else if constexpr (EPI == EPI_LD_4WARPS) {  // profiling only: half of the warps read the whole tile
-        uint32_t sink = 0;
-        if (chalf == 0) {
-#pragma unroll 1
-          for (int c = 0; c < 8; ++c) {
-            uint32_t acc[32];
-            tmem_ld_32x32b_x32(tmem_base + ((quarter * 32u) << 16) + as * BLOCK_N + c * 32, acc);
-            tmem_wait_ld_dep(acc);
-            sink ^= acc[c];
-          }
-        }
-        if (sink == 0x7fffffffu && row == -1) reinterpret_cast<uint32_t*>(p.out)[0] = sink;
-      } else if constexpr (EPI == EPI_LD_BATCH) {  // profiling only: 4 loads in flight, one wait
-        uint32_t a0[32], a1[32], a2[32], a3[32];
-        tmem_ld_32x32b_x32(taddr0, a0);
-        tmem_ld_32x32b_x32(taddr0 + 32, a1);
-        tmem_ld_32x32b_x32(taddr0 + 64, a2);
-        tmem_ld_32x32b_x32(taddr0 + 96, a3);
-        tmem_wait_ld();
-        const uint32_t sink = a0[1] ^ a1[2] ^ a2[3] ^ a3[4];
-        if (sink == 0x7fffffffu && row == -1) reinterpret_cast<uint32_t*>(p.out)[0] = sink;
-      } else if constexpr (EPI == EPI_LDONLY) {  // profiling only
-        uint32_t sink = 0;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t acc[32];
-          tmem_ld_32x32b_x32(taddr0 + c * 32, acc);
-          tmem_wait_ld_dep(acc);
-          sink ^= acc[c];
-        }
-        if (sink == 0x7fffffffu && row == -1) reinterpret_cast<uint32_t*>(p.out)[0] = sink;
-#endif
-      } else if constexpr (EPI < EPI_NONE) {
-        // one tcgen05.wait::ld per tile and warp (see the fp16 path)
-        uint32_t acc4[4][32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (col0 + c * 32 < p.N) tmem_ld_32x32b_x32(taddr0 + c * 32, acc4[c]);
-        tmem_wait_ld_dep(acc4[0]);
-        reg_fence(acc4[1]);
-        reg_fence(acc4[2]);
-        reg_fence(acc4[3]);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int col = col0 + c * 32;
-          if (col >= p.N) break;
-          uint32_t (&acc)[32] = acc4[c];
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + col);
-#pragma unroll
-          for (int v = 0; v < 8; ++v) {
-            const float4 b = __ldg(b4 + v);
-            float o0 = __uint_as_float(acc[4 * v + 0]) + b.x, o1 = __uint_as_float(acc[4 * v + 1]) + b.y;
-            float o2 = __uint_as_float(acc[4 * v + 2]) + b.z, o3 = __uint_as_float(acc[4 * v + 3]) + b.w;
-            if constexpr (EPI == EPI_BIAS_GELU_F32) {
-              o0 = gelu_erf(o0); o1 = gelu_erf(o1); o2 = gelu_erf(o2); o3 = gelu_erf(o3);
-            }
-            acc[4 * v + 0] = __float_as_uint(o0); acc[4 * v + 1] = __float_as_uint(o1);
-            acc[4 * v + 2] = __float_as_uint(o2); acc[4 * v + 3] = __float_as_uint(o3);
-          }
-          uint8_t* stg = smem_stg + (chalf * 2 + (store_iter & 1)) * STG_BYTES;
-          if (issuer) tma_store_wait_read<1>();
-          named_bar_sync(bar_id, 128);
-          stage_row_sw128(stg, row_local, acc);
-          fence_proxy_async_smem();
-          named_bar_sync(bar_id, 128);
-          if (issuer && row0 < p.M) {
-            if constexpr (EPI == EPI_BIAS_RESIDUAL) tma_reduce_add_2d(&tmap_out, stg, col, row0);
-            else tma_store_2d(&tmap_out, stg, col, row0);
-            tma_store_commit();
-          }
-          ++store_iter;
-        }
-      }
-      // every TMEM read of this warp has completed -> one arrival per warp on the leader's barrier
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty_bar[as], 0);
-    }
-    if (issuer) tma_store_wait_all();
+    return;
   }
 
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, TMEM_COLS);
+  // ===================== MMA + epilogue warpgroups =====================
+  setmaxnreg_inc<232>();
+  const uint32_t mw = wg - 1;                    // rows [64 mw, 64 mw + 64) of the tile
+  const uint32_t warp = (threadIdx.x / 32) % 4;  // rows [16 warp, +16) of the warpgroup's 64
+  const uint32_t lane = threadIdx.x % 32;
+  const uint32_t g = lane / 4, c = lane % 4;
+  const bool signal = (threadIdx.x % 128) == 0;
+  const uint32_t a_base = smem_u32(smem_a) + mw * 64 * 128;
+  const uint32_t b_base = smem_u32(smem_b);
+  const size_t pitch = (SPLIT && (EPI == EPI_QKV_ROPE || EPI == EPI_BIAS_GELU)) ? 2 * (size_t)p.ldo : (size_t)p.ldo;
+  uint32_t it = 0;
+  float acc[128];
+
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m0 = (tile / tiles_n) * BLOCK_M, n0 = (tile % tiles_n) * BLOCK_N;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const uint32_t s = it % STAGES;
+      // plain try_wait loops in this kernel: the watchdog's printf is a function call, and any call in a wgmma kernel
+      // makes ptxas serialise every wgmma (C7510)
+      while (!mbar_try_wait(&full_bar[s], (it / STAGES) & 1)) {
+      }
+      wgmma_fence();
+      const uint64_t da = wgmma_desc_sw128(a_base + s * A_STAGE_BYTES);
+      const uint64_t db = wgmma_desc_sw128(b_base + s * B_STAGE_BYTES);
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) wgmma_m64n256k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous slab's MMAs have read their stage
+      if (kb > 0 && signal) mbar_arrive(&empty_bar[(it + STAGES - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    reg_fence_f(acc);
+    if (signal) mbar_arrive(&empty_bar[(it + STAGES - 1) % STAGES]);
+
+    // ---- epilogue: thread holds rows r0 and r0 + 8, columns n0 + 8 i + 2 c + {0, 1} for i < 32
+    const int r0 = m0 + (int)(mw * 64 + warp * 16 + g);
+    const int rows[2] = {r0, r0 + 8};
+    if constexpr (EPI == EPI_QKV_ROPE) {
+      const bool rope = p.rope_cos != nullptr;
+      const int ld = p.rope_ld == 64 ? 64 : 32;
+#pragma unroll
+      for (int gi = 0; gi < 4; ++gi) {  // 64-column groups: column j pairs with j + 32 (same thread)
+        const int col0 = n0 + gi * 64;
+        if (col0 >= p.N) break;
+        const int sect = col0 / p.E;  // 0 q, 1 k, 2 v
+        const float sc = (sect == 0) ? p.q_scale : 1.0f;
+        const int slot = p.rope_ld == 64 ? ((col0 >> 6) & 1) : 0;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = rows[hr];
+          if (row >= p.M) continue;
+          const int t = row % p.T;
+          __half* o = reinterpret_cast<__half*>(p.out) + (size_t)row * pitch;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int j = 8 * q + 2 * (int)c;  // column pair (j, j + 1) and (j + 32, j + 33) of the group
+            const float2 bl = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + j));
+            const float2 bh = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + j));
+            float a0 = (acc[4 * (8 * gi + q) + 2 * hr] + bl.x) * sc, a1 = (acc[4 * (8 * gi + q) + 2 * hr + 1] + bl.y) * sc;
+            float b0 = (acc[4 * (8 * gi + q + 4) + 2 * hr] + bh.x) * sc;
+            float b1 = (acc[4 * (8 * gi + q + 4) + 2 * hr + 1] + bh.y) * sc;
+            if (sect < 2 && rope) {  // rotary_embedding.py:16-20, rotate_half = cat(-x2, x1)
+              const float2 cs = __ldg(reinterpret_cast<const float2*>(p.rope_cos + (size_t)t * ld + slot * 32 + j));
+              const float2 sn = __ldg(reinterpret_cast<const float2*>(p.rope_sin + (size_t)t * ld + slot * 32 + j));
+              const float ra0 = a0 * cs.x - b0 * sn.x, rb0 = b0 * cs.x + a0 * sn.x;
+              const float ra1 = a1 * cs.y - b1 * sn.y, rb1 = b1 * cs.y + a1 * sn.y;
+              a0 = ra0; b0 = rb0; a1 = ra1; b1 = rb1;
+            }
+            const __half2 ha = __floats2half2_rn(a0, a1), hb = __floats2half2_rn(b0, b1);
+            *reinterpret_cast<__half2*>(o + col0 + j) = ha;
+            *reinterpret_cast<__half2*>(o + col0 + 32 + j) = hb;
+            if constexpr (SPLIT) {
+              const float2 fa = __half22float2(ha), fb = __half22float2(hb);
+              *reinterpret_cast<__half2*>(o + p.lo_col_off + col0 + j) = __floats2half2_rn(a0 - fa.x, a1 - fa.y);
+              *reinterpret_cast<__half2*>(o + p.lo_col_off + col0 + 32 + j) = __floats2half2_rn(b0 - fb.x, b1 - fb.y);
+            }
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = n0 + 8 * i + 2 * (int)c;
+        if (col >= p.N) break;  // N % 32 == 0 (fp32) / % 64 == 0 (fp16): whole 8-column blocks are in or out
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row = rows[hr];
+          if (row >= p.M) continue;
+          float y0 = acc[4 * i + 2 * hr] + bb.x, y1 = acc[4 * i + 2 * hr + 1] + bb.y;
+          if constexpr (EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_GELU_F32) {
+            y0 = gelu_erf(y0);
+            y1 = gelu_erf(y1);
+          }
+          if constexpr (EPI == EPI_BIAS_GELU) {
+            __half* o = reinterpret_cast<__half*>(p.out) + (size_t)row * pitch + col;
+            const __half2 h = __floats2half2_rn(y0, y1);
+            *reinterpret_cast<__half2*>(o) = h;
+            if constexpr (SPLIT) {
+              const float2 f = __half22float2(h);
+              *reinterpret_cast<__half2*>(o + p.lo_col_off) = __floats2half2_rn(y0 - f.x, y1 - f.y);
+            }
+          } else {
+            float2* o = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * pitch + col);
+            if constexpr (EPI == EPI_BIAS_RESIDUAL) {
+              const float2 x = *o;
+              *o = make_float2(x.x + y0, x.y + y1);
+            } else {
+              *o = make_float2(y0, y1);
+            }
+          }
+        }
+      }
+    }
   }
 }
 
 template <int EPI, bool SPLIT = false>
-inline cudaError_t launch_gemm2_epi(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                                    const GemmParams& p, int num_sms, cudaStream_t stream) {
+inline cudaError_t launch_gemm2_epi(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int num_sms,
+                                    cudaStream_t stream) {
   using namespace gemm2_cfg;
   cudaError_t e =
       cudaFuncSetAttribute(gemm2_f16_kernel<EPI, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   if (e != cudaSuccess) return e;
-  const int tiles = ((p.M + PAIR_M - 1) / PAIR_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
-  const int max_clusters = num_sms / 2;
-  const int clusters = tiles < max_clusters ? tiles : max_clusters;
-  return launch_pdl(gemm2_f16_kernel<EPI, SPLIT>, dim3(2 * clusters), dim3(NUM_THREADS), SMEM_BYTES, stream, ta, tb, tout,
-                    p);
+  const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
+  const int grid = tiles < num_sms ? tiles : num_sms;
+  return launch_pdl(gemm2_f16_kernel<EPI, SPLIT>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, ta, tb, p);
 }
 
 }  // namespace esmb200

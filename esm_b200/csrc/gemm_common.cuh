@@ -1,6 +1,6 @@
-// esm_b200 — definitions shared by the tcgen05 GEMM kernels (sm_100a): epilogue ids, parameter block, erf-GELU.
+// esm_b200 — definitions shared by the GEMM kernels (sm_90a): epilogue ids, parameter block, erf-GELU.
 //
-// Epilogues (reference lines they replace, /root/reference/esm/...):
+// Epilogues (reference lines they replace, esm/...):
 //   QKV_ROPE      multihead_attention.py:258-261 (q/k/v Linear + bias, q *= d^-1/2) + :354-355 /
 //                 rotary_embedding.py:11-20 (rotate-half RoPE on q,k) -> fp16 [M,3E]
 //   BIAS_RESIDUAL multihead_attention.py:395 + modules.py:134, and modules.py:139-140
@@ -13,12 +13,7 @@
 
 namespace esmb200 {
 
-enum : int { EPI_QKV_ROPE = 0, EPI_BIAS_RESIDUAL = 1, EPI_BIAS_GELU = 2, EPI_BIAS_F32 = 3, EPI_BIAS_GELU_F32 = 4,
-              EPI_NONE = 5 /* profiling only: accumulators are discarded */,
-              EPI_LDONLY = 6 /* profiling only: accumulators are read from TMEM and discarded */,
-              EPI_LD_X16 = 7, EPI_LD_4WARPS = 8, EPI_LD_BATCH = 9 /* profiling only: TMEM read pattern variants */,
-              EPI_GELU_MATHONLY = 10, EPI_F16_STOREONLY = 11 /* profiling only: halves of the fc1 epilogue */,
-              EPI_FMA_MATHONLY = 12 /* profiling only: 15 dependent FMAs per element instead of GELU, no MUFU */ };
+enum : int { EPI_QKV_ROPE = 0, EPI_BIAS_RESIDUAL = 1, EPI_BIAS_GELU = 2, EPI_BIAS_F32 = 3, EPI_BIAS_GELU_F32 = 4 };
 
 struct GemmParams {
   int M, N, K;
@@ -33,7 +28,6 @@ struct GemmParams {
   int T;                  // tokens per sequence: position of row r is r % T
   int E;                  // embed dim: columns [0,E) = q, [E,2E) = k, [2E,3E) = v
   float q_scale;          // head_dim^-0.5
-  int chunked;            // tile walk: 1 = one contiguous run of tiles per cluster (see gemm2.cuh)
   int lo_col_off;         // SPLIT kernels with fp16 output: the lo half of column c is written at column c + lo_col_off
 };
 
@@ -54,28 +48,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   const float e = ex2_approx(z * (z * -1.4426950408889634f));
   const float q = poly * e;
   return x * (x >= 0.f ? 1.0f - q : q);
-}
-
-// The same for two values at once with packed f32x2 arithmetic (FFMA2 / FMUL2): ~20 issue slots per pair instead of 30.
-// The fc1 epilogue is instruction-energy bound under the 1 kW cap (profiles/r01_epilogue_experiments.txt).
-__device__ __forceinline__ void gelu_erf2(float x0, float x1, float& y0, float& y1) {
-  constexpr float PC = 0.3275911f * 0.70710678118654752440f;
-  float d0, d1, p0, p1, s0, s1, q0, q1, r0, r1, t0, t1;
-  fma2(d0, d1, fabsf(x0), fabsf(x1), PC, PC, 1.0f, 1.0f);
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(d0));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(d1));
-  fma2(p0, p1, t0, t1, 0.5f * 1.061405429f, 0.5f * 1.061405429f, 0.5f * -1.453152027f, 0.5f * -1.453152027f);
-  fma2(p0, p1, p0, p1, t0, t1, 0.5f * 1.421413741f, 0.5f * 1.421413741f);
-  fma2(p0, p1, p0, p1, t0, t1, 0.5f * -0.284496736f, 0.5f * -0.284496736f);
-  fma2(p0, p1, p0, p1, t0, t1, 0.5f * 0.254829592f, 0.5f * 0.254829592f);
-  mul2(p0, p1, p0, p1, t0, t1);
-  mul2(s0, s1, x0, x1, -0.5f * 1.4426950408889634f, -0.5f * 1.4426950408889634f);
-  mul2(s0, s1, s0, s1, x0, x1);  // -x^2/2 * log2(e)
-  mul2(q0, q1, p0, p1, ex2_approx(s0), ex2_approx(s1));
-  mul2(q0, q1, q0, q1, x0, x1);                   // x * q
-  fma2(r0, r1, q0, q1, -1.0f, -1.0f, x0, x1);     // x - x * q
-  y0 = x0 >= 0.f ? r0 : q0;
-  y1 = x1 >= 0.f ? r1 : q1;
 }
 
 }  // namespace esmb200

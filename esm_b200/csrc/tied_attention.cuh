@@ -1,6 +1,6 @@
-// esm_b200 — MSA tied row attention (sm_100a, head_dim 64).
+// esm_b200 — MSA tied row attention (sm_90a, head_dim 64).
 //
-// Replaces /root/reference/esm/axial_attention.py:71-111 (RowSelfAttention.compute_attention_weights /
+// Replaces esm/axial_attention.py:71-111 (RowSelfAttention.compute_attention_weights /
 // compute_attention_update): the attention logits are SUMMED over the R alignment rows,
 //     S[h,b,i,j] = sum_r sum_e q[b,r,i,h,e] * k[b,r,j,h,e]                      (einsum "rinhd,rjnhd->hnij", :87)
 //     P = softmax_j(S)  (padded key columns filled with -10000, :94-97)          (:105)
@@ -9,16 +9,16 @@
 // for the logits the K loop simply walks over the rows r (row offset r*C, 64 K-elements per step), for the update the
 // V tile of row r is the MN-major B operand, exactly like V in the flash-attention kernels.  No regrouping copies.
 //
-//   tied_scores_kernel : one CTA per (b, h, 128 query columns, 256 key columns); K = R*64; fp32 logits -> S [H,B,C,C]
+//   tied_scores_kernel : one CTA per (b, h, 128 query columns, 128 key columns); K = R*64; fp32 logits -> S [H,B,C,C]
 //   tied_softmax_kernel: one warp per logits row; fp32 softmax; writes fp16 P [H*B*C, Cp] (Cp = C rounded up to 64,
 //                        zero filled) and, on request, the fp32 probabilities in place of the logits
 //   tied_pv_kernel     : one CTA per (b, h, 128 query columns, 4 alignment rows): D[128, 4 x 64] += P_tile V_r tile
 //                        over the key columns; fp16 context -> ctx [B*R*C, E]
-// Roles inside the MMA kernels (192 threads): warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, warp 2 allocates
-// TMEM, warps 2-5 = epilogue (one TMEM lane = one output row per thread).
+// Inside the MMA kernels (256 threads) thread 0 streams the operand tiles through a TMA ring (mbarrier completion) and
+// all eight warps multiply with mma.sync from ldmatrix reads of the 128B-swizzled tiles.
 #pragma once
 
-#include "common.cuh"
+#include "attention_common.cuh"
 
 namespace esmb200 {
 
@@ -35,18 +35,17 @@ struct TiedParams {
 };
 
 namespace tied_cfg {
-constexpr int NUM_THREADS = 192;
-// scores
-constexpr int S_BM = 128, S_BN = 256, S_STAGES = 4;
+constexpr int NUM_THREADS = 256;
+// scores: 8 warps as 4 (rows) x 2 (columns), warp tile 32 x 64
+constexpr int S_BM = 128, S_BN = 128, S_STAGES = 4;
 constexpr int S_A_BYTES = S_BM * 128, S_B_BYTES = S_BN * 128;
-constexpr int S_STAGE_BYTES = S_A_BYTES + S_B_BYTES;                 // 48 KB
+constexpr int S_STAGE_BYTES = S_A_BYTES + S_B_BYTES;                 // 32 KB
 constexpr int S_SMEM_BYTES = S_STAGES * S_STAGE_BYTES + 1024 + 256;
-// update
-constexpr int V_BM = 128, V_ROWS = 4, V_STAGES = 2;  // 2 stages = 96 KB: two CTAs per SM, one's epilogue under the other's MMAs
+// update: warp w owns query rows [16 w, 16 w + 16) of every alignment row of the CTA
+constexpr int V_BM = 128, V_ROWS = 4, V_STAGES = 2;
 constexpr int V_P_BYTES = V_BM * 128, V_V_BYTES = 64 * 128;          // 16 KB + 4 x 8 KB
 constexpr int V_STAGE_BYTES = V_P_BYTES + V_ROWS * V_V_BYTES;        // 48 KB
 constexpr int V_SMEM_BYTES = V_STAGES * V_STAGE_BYTES + 1024 + 256;
-constexpr int TMEM_COLS = 256;
 }  // namespace tied_cfg
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -58,109 +57,61 @@ tied_scores_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
   using namespace tied_cfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S_STAGES * S_STAGE_BYTES);
-  uint64_t* full = bars;                 // [S_STAGES]
-  uint64_t* empty = bars + S_STAGES;     // [S_STAGES]
-  uint64_t* done = bars + 2 * S_STAGES;  // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S_STAGES + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S_STAGES * S_STAGE_BYTES);  // [S_STAGES]
 
-  const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;  // warp: uniform for ptxas
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
+  const uint32_t wm = warp % 4, wn = warp / 4;
   const int m0 = blockIdx.x * S_BM, n0 = blockIdx.y * S_BN;
   const int b = blockIdx.z / p.H, h = blockIdx.z % p.H;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < S_STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    mbar_init(done, 1);
+    for (int i = 0; i < S_STAGES; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_d = *tmem_slot;
+  auto load = [&](int r) {
+    const int s = r % S_STAGES;
+    const int row = (b * p.R + r) * p.C;
+    mbar_arrive_expect_tx(&full[s], S_STAGE_BYTES);
+    tma_load_2d(smem + s * S_STAGE_BYTES, &tmap_q, &full[s], h * 64, row + m0);
+    tma_load_2d(smem + s * S_STAGE_BYTES + S_A_BYTES, &tmap_k, &full[s], p.E + h * 64, row + n0);
+  };
+  if (threadIdx.x == 0)
+    for (int r = 0; r < S_STAGES && r < p.R; ++r) load(r);
 
-  // Both control warps run their loops warp-convergent with operands derived from warp-uniform values; only the TMA /
-  // tcgen05 instructions sit under elect_one() (no per-instruction ELECT / R2UR / BRA.U.ANY waterfall: the R-deep loop of
-  // this kernel was issue-bound, 5 x ~94 cycles per alignment row against 256 cycles of tensor work).
-  const uint32_t u_smem = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-  const uint32_t u_bars = u_smem + S_STAGES * S_STAGE_BYTES;
-  if (warp == 0) {
-    for (int r = 0; r < p.R; ++r) {
-      const uint32_t s = r % S_STAGES;
-      mbar_wait_relaxed(&empty[s], ((r / S_STAGES) & 1) ^ 1);
-      const int row = (b * p.R + r) * p.C;
-      const uint32_t st = u_smem + s * S_STAGE_BYTES, fb = u_bars + s * 8;
-      if (elect_one()) {
-        mbar_arrive_expect_tx_addr(fb, S_STAGE_BYTES);
-        tma_load_2d_addr(st, &tmap_q, fb, h * 64, row + m0);
-        tma_load_2d_addr(st + S_A_BYTES, &tmap_k, fb, p.E + h * 64, row + n0);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_f16(S_BM, S_BN, false);
-    const uint32_t u_tmem = __shfl_sync(0xffffffffu, tmem_d, 0);
-    for (int r = 0; r < p.R; ++r) {
-      const uint32_t s = r % S_STAGES;
-      mbar_wait(&full[s], (r / S_STAGES) & 1);
-      tc_fence_after();
-      const uint64_t adesc = umma_smem_desc_sw128(u_smem + s * S_STAGE_BYTES, 1024, 0);
-      const uint64_t bdesc = umma_smem_desc_sw128(u_smem + s * S_STAGE_BYTES + S_A_BYTES, 1024, 0);
-      if (elect_one()) {
+  float acc[2][8][4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_ss(u_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (r | k) != 0 ? 1u : 0u);
-        tc_commit_addr(u_bars + (S_STAGES + s) * 8);
-        if (r + 1 == p.R) tc_commit_addr(u_bars + 2 * S_STAGES * 8);
-      }
-      __syncwarp();
-    }
-  } else {
-    const uint32_t quarter = warp % 4;
-    const int ci = m0 + quarter * 32 + lane;
-    mbar_wait(done, 0);
-    tc_fence_after();
-    float* dst = p.S + ((size_t)(h * p.B + b) * p.C + ci) * p.C;
-    const bool vec_ok = (p.C % 4) == 0;
-#pragma unroll 1
-    for (int c = 0; c < S_BN / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32b_x32(tmem_d + ((quarter * 32u) << 16) + c * 32, v);
-      tmem_wait_ld_dep(v);
-      const int cj0 = n0 + c * 32;
-      if (ci < p.C && cj0 < p.C) {
-        if (vec_ok && cj0 + 32 <= p.C) {
-          float4* d4 = reinterpret_cast<float4*>(dst + cj0);
+  for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-          for (int i = 0; i < 8; ++i)
-            d4[i] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                                __uint_as_float(v[4 * i + 3]));
-        } else {
+    for (int i = 0; i < 8; ++i) acc[mi][i][0] = acc[mi][i][1] = acc[mi][i][2] = acc[mi][i][3] = 0.f;
+  for (int r = 0; r < p.R; ++r) {
+    const int s = r % S_STAGES;
+    mbar_wait(&full[s], (r / S_STAGES) & 1);
+    const uint32_t st = smem_u32(smem + s * S_STAGE_BYTES);
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (cj0 + i < p.C) dst[cj0 + i] = __uint_as_float(v[i]);
+    for (int mi = 0; mi < 2; ++mi) qk_tile<8>(acc[mi], st, wm * 32 + mi * 16, st + S_A_BYTES, wn * 64);
+    __syncthreads();  // every warp is done with stage s
+    if (threadIdx.x == 0 && r + S_STAGES < p.R) load(r + S_STAGES);
+  }
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int ci = m0 + (int)(wm * 32 + mi * 16 + g + 8 * hr);
+      if (ci >= p.C) continue;
+      float* dst = p.S + ((size_t)(h * p.B + b) * p.C + ci) * p.C;
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int cj = n0 + (int)(wn * 64 + nb * 8 + 2 * c) + e;
+          if (cj < p.C) dst[cj] = acc[mi][nb][2 * hr + e];
         }
-      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_d, TMEM_COLS);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -217,116 +168,81 @@ tied_softmax_kernel(const TiedParams p) {
 // ---------------------------------------------------------------------------------------------------------------
 // ctx_r = P V_r for 4 alignment rows r per CTA
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(tied_cfg::NUM_THREADS, 2)
+__global__ void __launch_bounds__(tied_cfg::NUM_THREADS, 1)
 tied_pv_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constant__ CUtensorMap tmap_v,
                const TiedParams p) {
   using namespace tied_cfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + V_STAGES * V_STAGE_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + V_STAGES;
-  uint64_t* done = bars + 2 * V_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * V_STAGES + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + V_STAGES * V_STAGE_BYTES);  // [V_STAGES]
 
-  const uint32_t warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;  // warp: uniform for ptxas
+  const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
   const int m0 = blockIdx.x * V_BM;
   const int r0 = blockIdx.y * V_ROWS;
   const int nr = min(V_ROWS, p.R - r0);
   const int b = blockIdx.z / p.H, h = blockIdx.z % p.H;
   const int nk = p.Cp / 64;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_p);
     tma_prefetch_desc(&tmap_v);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < V_STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    mbar_init(done, 1);
+    for (int i = 0; i < V_STAGES; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  const uint32_t tmem_d = *tmem_slot;
+  auto load = [&](int j) {
+    const int s = j % V_STAGES;
+    uint8_t* st = smem + s * V_STAGE_BYTES;
+    mbar_arrive_expect_tx(&full[s], V_P_BYTES + nr * V_V_BYTES);
+    tma_load_2d(st, &tmap_p, &full[s], j * 64, (h * p.B + b) * p.C + m0);
+    for (int i = 0; i < nr; ++i)
+      tma_load_2d(st + V_P_BYTES + i * V_V_BYTES, &tmap_v, &full[s], 2 * p.E + h * 64, (b * p.R + r0 + i) * p.C + j * 64);
+  };
+  if (threadIdx.x == 0)
+    for (int j = 0; j < V_STAGES && j < nk; ++j) load(j);
 
-  // warp-convergent control warps, see tied_scores_kernel (16 MMAs per 64-key slab were 16 waterfalls here)
-  const uint32_t u_smem = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-  const uint32_t u_bars = u_smem + (uint32_t)(reinterpret_cast<uint8_t*>(bars) - smem);
-  if (warp == 0) {
-    for (int j = 0; j < nk; ++j) {
-      const uint32_t s = j % V_STAGES;
-      mbar_wait_relaxed(&empty[s], ((j / V_STAGES) & 1) ^ 1);
-      const uint32_t st = u_smem + s * V_STAGE_BYTES, fb = u_bars + s * 8;
-      if (elect_one()) {
-        mbar_arrive_expect_tx_addr(fb, V_P_BYTES + nr * V_V_BYTES);
-        tma_load_2d_addr(st, &tmap_p, fb, j * 64, (h * p.B + b) * p.C + m0);
-        for (int i = 0; i < nr; ++i)
-          tma_load_2d_addr(st + V_P_BYTES + i * V_V_BYTES, &tmap_v, fb, 2 * p.E + h * 64,
-                           (b * p.R + r0 + i) * p.C + j * 64);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_f16(V_BM, 64, true);
-    const uint32_t u_tmem = __shfl_sync(0xffffffffu, tmem_d, 0);
-    for (int j = 0; j < nk; ++j) {
-      const uint32_t s = j % V_STAGES;
-      mbar_wait(&full[s], (j / V_STAGES) & 1);
-      tc_fence_after();
-      const uint32_t base = u_smem + s * V_STAGE_BYTES;
-      const uint64_t pdesc = umma_smem_desc_sw128(base, 1024, 0);
-      if (elect_one()) {
-        for (int i = 0; i < nr; ++i) {
-          const uint64_t vdesc = umma_smem_desc_sw128(base + V_P_BYTES + i * V_V_BYTES, 1024, 8192);
+  float acc[V_ROWS][8][4];
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_ss(u_tmem + 64 * i, pdesc + 2 * k, vdesc + 128 * k, idesc, (j | k) != 0 ? 1u : 0u);
+  for (int i = 0; i < V_ROWS; ++i)
+#pragma unroll
+    for (int n = 0; n < 8; ++n) acc[i][n][0] = acc[i][n][1] = acc[i][n][2] = acc[i][n][3] = 0.f;
+  for (int j = 0; j < nk; ++j) {
+    const int s = j % V_STAGES;
+    mbar_wait(&full[s], (j / V_STAGES) & 1);
+    const uint32_t st = smem_u32(smem + s * V_STAGE_BYTES);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      ldsm_a(st, warp * 16, kk, a);
+#pragma unroll
+      for (int i = 0; i < V_ROWS; ++i) {
+        if (i >= nr) break;
+#pragma unroll
+        for (int n2 = 0; n2 < 4; ++n2) {
+          uint32_t bv[4];
+          ldsm_bt(st + V_P_BYTES + i * V_V_BYTES, kk, 16 * n2, bv);
+          mma16816(acc[i][2 * n2], a, bv[0], bv[1]);
+          mma16816(acc[i][2 * n2 + 1], a, bv[2], bv[3]);
         }
-        tc_commit_addr(u_bars + (V_STAGES + s) * 8);
-        if (j + 1 == nk) tc_commit_addr(u_bars + 2 * V_STAGES * 8);
-      }
-      __syncwarp();
-    }
-  } else {
-    const uint32_t quarter = warp % 4;
-    const int ci = m0 + quarter * 32 + lane;
-    mbar_wait(done, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int i = 0; i < nr; ++i) {
-      uint32_t out[32];
-#pragma unroll
-      for (int hlf = 0; hlf < 2; ++hlf) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_d + ((quarter * 32u) << 16) + 64 * i + 32 * hlf, v);
-        tmem_wait_ld_dep(v);
-#pragma unroll
-        for (int e = 0; e < 16; ++e)
-          out[hlf * 16 + e] = pack_half2(__uint_as_float(v[2 * e]), __uint_as_float(v[2 * e + 1]));
-      }
-      if (ci < p.C) {
-        uint4* dst = reinterpret_cast<uint4*>(p.ctx + ((size_t)(b * p.R + r0 + i) * p.C + ci) * p.E + h * 64);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dst[e] = make_uint4(out[4 * e], out[4 * e + 1], out[4 * e + 2], out[4 * e + 3]);
       }
     }
+    __syncthreads();  // every warp is done with stage s
+    if (threadIdx.x == 0 && j + V_STAGES < nk) load(j + V_STAGES);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_d, TMEM_COLS);
+#pragma unroll
+  for (int i = 0; i < V_ROWS; ++i) {
+    if (i >= nr) break;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int ci = m0 + (int)(warp * 16 + g + 8 * hr);
+      if (ci >= p.C) continue;
+      __half* dst = p.ctx + ((size_t)(b * p.R + r0 + i) * p.C + ci) * p.E + h * 64;
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+        *reinterpret_cast<__half2*>(dst + n * 8 + 2 * c) = __floats2half2_rn(acc[i][n][2 * hr], acc[i][n][2 * hr + 1]);
+    }
   }
 }
 

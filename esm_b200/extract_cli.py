@@ -10,7 +10,7 @@ torch.save in line, so the GPU idles during the copies and the pickling):
     device: only what was asked for crosses PCIe;
   * device->host copies go to pinned staging buffers on a side stream and are overlapped with the next batch's forward
     (two staging slots); slicing + `torch.save` run in writer threads;
-  * the default token budget is larger (the reference's 4096 tokens leave a B200 idle);
+  * the default token budget is larger (the reference's 4096 tokens leave an H100 idle);
   * under torchrun the token-budget batches are dealt round-robin to the ranks, each rank writes its own files, and no
     collective is needed because the outputs are files.
 """

@@ -8,7 +8,7 @@ transformer block at run time:
     import esm, esm_b200.integration
     esm_b200.integration.patch_reference()            # esm.modules.TransformerLayer.forward -> C ABI on CUDA tensors
     model, alphabet = esm.pretrained.esm2_t33_650M_UR50D()
-    out = model.cuda()(tokens.cuda(), repr_layers=[33])   # the reference's own esm2.py:77-144 loop, B200 kernels inside
+    out = model.cuda()(tokens.cuda(), repr_layers=[33])   # the reference's own esm2.py:77-144 loop, H100 kernels inside
 
 Only rotary (ESM-2) layers on CUDA tensors are dispatched — exactly the seam SURVEY §8b names
 (`esm/modules.py:120-142` called from `esm/model/esm2.py:111-116`); ESM-1 layers (learned positions, bias_kv) and CPU

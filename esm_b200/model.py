@@ -118,7 +118,7 @@ class LayerBinding:
         self.release()
         for p in ps:
             if not p.is_cuda:
-                raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only: move the model with .cuda(); "
+                raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
                                         "there is no CPU fallback")
         lib = _lib.load()
         keep = [_f32(p) for p in ps]
@@ -222,7 +222,7 @@ def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Te
     """esmb200_stack_forward on x fp32 (B,T,E) in place. repr_out: {layer index (0-based): (B,T,E) tensor to fill}.
     Returns {layer index: (B,H,T,T) fp32} for the indices in attn_layers."""
     if not x.is_cuda:
-        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
     assert x.dtype == torch.float32 and x.is_contiguous()
     lib = _lib.load()
     B, T, E = x.shape
@@ -275,8 +275,8 @@ class RobertaLMHead(nn.Module):
     `forward(features)` is the plain PyTorch evaluation (used on already layer-normed features, e.g. by callers that
     hold a representation).  `forward_native(x_pre_ln, ln_w, ln_b, eps)` is what ESM2.forward uses on the GPU: it
     starts from the residual stream BEFORE emb_layer_norm_after and runs the whole tail through libesmb200.so
-    (LayerNorm->fp16 | tcgen05 GEMM + bias + erf-GELU | LayerNorm->fp16 | tcgen05 GEMM onto the 33 tokens, padded to 64
-    output columns), replacing ~25 ms of fp32 cuBLAS + elementwise passes per 256x1024-token batch by ~2 ms."""
+    (LayerNorm->fp16 | wgmma GEMM + bias + erf-GELU | LayerNorm->fp16 | wgmma GEMM onto the 33 tokens, padded to 64
+    output columns) instead of fp32 cuBLAS + elementwise passes."""
 
     def __init__(self, embed_dim, output_dim, weight):
         super().__init__()
@@ -549,7 +549,7 @@ class ESM2(nn.Module):
             need_head_weights = True
         assert tokens.ndim == 2
         if not tokens.is_cuda:
-            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only: pass tokens.cuda(); no CPU fallback")
+            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
         lib = _lib.load()
         if tokens.dtype != torch.int64:
             if tokens.dtype.is_floating_point or tokens.dtype == torch.bool:

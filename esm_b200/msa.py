@@ -1,12 +1,12 @@
-"""MSA-Transformer axial block on the sm_100a kernels — host-side mirror of
+"""MSA-Transformer axial block on the sm_90a kernels — host-side mirror of
 /root/reference/esm/modules.py:145-221 (AxialTransformerLayer, NormalizedResidualBlock :360-392,
 FeedForwardNetwork :395-418) and /root/reference/esm/axial_attention.py (RowSelfAttention :11-130,
 ColumnSelfAttention :133-239), with the reference's parameter names so its state dicts load.
 
 CUDA path for BASELINE.json configs[4] (SURVEY §8f #3).  All the arithmetic of the block runs in libesmb200.so:
   * LayerNorm -> fp16, q/k/v projection (+ bias, q scale; no rotary embedding), out-projection + residual,
-    fc1 + erf-GELU, fc2 + residual: the same tcgen05 GEMM / LayerNorm kernels as the ESM-2 path;
-  * tied row attention (logits summed over the R rows, axial_attention.py:87): esmb200_tied_row_attention — a tcgen05
+    fc1 + erf-GELU, fc2 + residual: the same wgmma GEMM / LayerNorm kernels as the ESM-2 path;
+  * tied row attention (logits summed over the R rows, axial_attention.py:87): esmb200_tied_row_attention — a tensor-core
     contraction over K = R*64 that walks the alignment rows with TMA boxes taken straight from the projection output,
     a row softmax (with the reference's -10000 fill on padded key columns), and the P.V update with V tiles as the
     MN-major operand (csrc/tied_attention.cuh);
@@ -107,7 +107,7 @@ class AxialTransformerLayer(nn.Module):
         self.release()
         for p in ps:
             if not p.is_cuda:
-                raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only: move the model with .cuda(); "
+                raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
                                         "there is no CPU fallback")
             if p.dtype != torch.float32 or not p.is_contiguous():
                 raise _lib.Esmb200Error("esm_b200 expects contiguous fp32 master parameters")
@@ -178,7 +178,7 @@ class AxialTransformerLayer(nn.Module):
         if self_attn_mask is not None:
             raise NotImplementedError
         if not x.is_cuda:
-            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         R, C, B, E = x.shape
         xb = x.permute(2, 0, 1, 3).contiguous().float()  # [B,R,C,E], updated in place by the residual epilogues
         row_probs, col_probs = self.forward_batch_major(xb, self_attn_padding_mask, need_head_weights)
@@ -265,7 +265,7 @@ def run_axial_stack(layers: Sequence[AxialTransformerLayer], xb: torch.Tensor,
     """esmb200_axial_stack_forward on xb [B,R,C,E] fp32 in place (msa_transformer.py:190-201's loop).
     Returns {layer index: row attention [H,B,C,C] fp32} for the indices in row_attn_layers."""
     if not xb.is_cuda:
-        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
     assert xb.dtype == torch.float32 and xb.is_contiguous()
     lib = _lib.load()
     B, R, C, E = xb.shape
@@ -366,7 +366,7 @@ class MSATransformer(nn.Module):
     def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
         assert tokens.ndim == 3
         if not tokens.is_cuda:
-            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_100a) only: pass tokens.cuda(); no CPU fallback")
+            raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
         if return_contacts and not self.contacts_without_col_attentions:
             need_head_weights = True  # msa_transformer.py:149-150
         lib = _lib.load()

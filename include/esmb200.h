@@ -1,4 +1,4 @@
-/* esmb200.h — C ABI of the B200-native ESM-2 transformer-layer forward path (libesmb200.so).
+/* esmb200.h — C ABI of the H100-native ESM-2 transformer-layer forward path (libesmb200.so).
  *
  * The reference (facebookresearch/esm, fair-esm 2.0.1) is pure Python and has no FFI for this path; the seam this
  * library sits behind is the Python method
@@ -256,10 +256,7 @@ int esmb200_gemm_split(int32_t epilogue, const void* a, const void* w, const flo
 int esmb200_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                             int32_t H, void* scratch, void* stream);
 
-/* ---- process-wide kernel selection knobs (A/B measurements; the defaults are the product configuration) ----
- * "attn"      8 (attention8.cuh, 4 CTAs/SM) | 7 (attention7.cuh, the round-1 kernel: only in a library built with
- *             -DESMB200_EXPERIMENTS, A/B measurements)                                          env ESMB200_ATTN
- * "attn_poly" 0 | 2 | 3 | 4 (default): every n-th pair of softmax exponentials on the FMA pipe   env ESMB200_ATTN_POLY
+/* ---- process-wide launch knobs (A/B measurements; the defaults are the product configuration) ----
  * "pdl"       0 (default) | 1: programmatic dependent launch between the layer's kernels        env ESMB200_PDL
  * Returns ESMB200_EINVAL for an unknown name or value. Not thread-safe against concurrent launches. */
 int esmb200_set_option(const char* name, int32_t value);

@@ -1,4 +1,4 @@
-"""BASELINE.json configs[3]: esm2_t36_3B_UR50D contact-prediction forward (need_head_weights=True), L=512, 1xB200.
+"""BASELINE.json configs[3]: esm2_t36_3B_UR50D contact-prediction forward (need_head_weights=True), L=512, 1xH100.
 Seeded random-init weights, B=16 (SURVEY §8d proposes 16; BASELINE.json leaves the batch open). Prints seq/s with and
 without the attention/contact outputs. Developer/profile tool."""
 import json

@@ -1,5 +1,5 @@
 """BASELINE.json configs[4]: esm_msa1b_t12_100M axial (row + column) attention forward on a synthetic 128 x 512 MSA,
-1xB200: 12 AxialTransformerLayers (E=768, H=12, F=3072), seeded random weights. Prints ms per MSA. Developer tool."""
+1xH100: 12 AxialTransformerLayers (E=768, H=12, F=3072), seeded random weights. Prints ms per MSA. Developer tool."""
 import json
 import os
 import sys

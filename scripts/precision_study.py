@@ -1,9 +1,8 @@
 """CPU study (no GPU): which fp16 roundings drive the error of the ESM-2 forward in the sharp-softmax regime.
 
 Emulates the CUDA path's operand roundings inside the fp32 oracle (6 layers, 650M width, q/k weights x3) and switches
-them off selectively.  Output committed as profiles/r02_precision_study.txt; conclusion in DESIGN.md section 4:
-splitting only q.k^T does not help (1.6e-2 -> 1.4e-2), an exact logit path leaves 6e-3, only full hi+lo operands
-("fp32x3") restore fp32-grade parity.   python scripts/precision_study.py [qk_gain]
+them off selectively: shows which roundings drive the error, and that full hi+lo operands ("fp32x3") restore
+fp32-grade parity.   python scripts/precision_study.py [qk_gain]
 """
 import os
 import sys

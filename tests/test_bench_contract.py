@@ -1,4 +1,4 @@
-"""CPU: the reference arm of bench.py (`--impl reference`: the unmodified reference from baseline/_ref, else the oracle port, timed on the host cores) prints exactly one
+"""CPU: the reference arm of bench.py (`--impl reference`: the unmodified reference from oracle/_ref, else the oracle port, timed on the host cores) prints exactly one
 JSON line with the keys the driver's contract names."""
 import json
 import os
@@ -20,7 +20,7 @@ def test_reference_arm_prints_one_contract_line():
               "config", "cpu_baseline", "e2e"):
         assert k in d, k
     assert d["value"] > 0 and d["steps"] == 1
-    has_ref = os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "esm"))
+    has_ref = os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "esm"))
     assert d["cpu_baseline"]["kind"] == ("reference" if has_ref else "port")
     assert d["cpu_baseline"]["cores"] >= 1 and d["cpu_baseline"]["sample"]
     assert d["e2e"]["value"] == d["value"] and d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0

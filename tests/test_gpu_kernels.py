@@ -1,4 +1,4 @@
-"""GPU (-m gpu): each sm_100a kernel, called through the C ABI, against a plain PyTorch fp32 evaluation of the same
+"""GPU (-m gpu): each sm_90a kernel, called through the C ABI, against a plain PyTorch fp32 evaluation of the same
 op on the same device.  Inputs to the tensor-core kernels are rounded to fp16 first, so the comparison isolates the
 kernel (fp32 accumulation order) from the operand-precision choice; tolerances are stated per test."""
 import ctypes

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the MSA axial block (esm_b200.msa.AxialTransformerLayer -> C ABI -> sm_100a kernels) against the
+"""GPU (-m gpu): the MSA axial block (esm_b200.msa.AxialTransformerLayer -> C ABI -> sm_90a kernels) against the
 committed outputs of the reference's AxialTransformerLayer and against the CPU oracle. Same tolerance as the ESM-2
 path (fp16 operands): rel-Frobenius <= 3e-3 on the layer output, probabilities max-abs <= 1e-2."""
 import os

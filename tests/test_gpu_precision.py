@@ -1,7 +1,7 @@
 """GPU (-m gpu): the "fp32x3" precision mode (every MMA operand an fp16 hi + lo pair, three products per MMA) and the
 sharp-softmax regime VERDICT r1 asked to gate.
 
-Why a second precision exists (scripts/precision_study.py, profiles/r02_precision_study.txt): with q/k weights scaled
+Why a second precision exists (scripts/precision_study.py): with q/k weights scaled
 x3 the random-weight network is ill-conditioned — a 5e-4 perturbation of the residual stream grows ~10x over six layers
 because near-one-hot softmaxes flip.  Emulating the roundings on the CPU shows that splitting ONLY q.k^T (the r1
 verdict's proposal) moves the 6-layer error from 1.6e-2 to 1.4e-2; an exact logit path still leaves 6e-3 from the fp16
@@ -55,8 +55,8 @@ def test_gemm_split_is_fp32_grade(M, N, K):
     r = rel_fro(out, ref)
     fp32 = rel_fro(a @ w.t() + bias, ref)  # cuBLAS fp32 (TF32 off) on the same inputs
     print(f"PARITY gemm_split {M}x{N}x{K} rel_fro={r:.3e} (fp32 cuBLAS {fp32:.3e})")
-    # tcgen05 accumulates in fp32 with truncation: the error grows like (3K/16 accumulation steps) x 2^-25 — measured
-    # 4.7e-6 (K=1280), 1.8e-5 (K=5120) — two orders below the fp16 mode's 3e-4, one above an IEEE fp32 dot product
+    # the tensor cores accumulate in fp32 with truncation: the error grows like (3K/16 accumulation steps) x 2^-25, two
+    # orders below the fp16 mode's 3e-4 and one above an IEEE fp32 dot product
     assert r <= 4e-5
     # fp16-output epilogue: hi | lo pair reproduces the fp32 GELU result
     if N % 64 == 0:

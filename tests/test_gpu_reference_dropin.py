@@ -1,8 +1,7 @@
 """GPU (-m gpu): the UNMODIFIED reference running on top of libesmb200.so (INTEGRATION.md Option B, VERDICT r1 missing #3).
 
-The reference package is imported from `baseline/_ref` (the offline `pip install --target baseline/_ref /root/reference`
-recorded in DESIGN.md; git-ignored, travels with the snapshot) — never from /root/reference, which does not exist on the
-GPU box.  `esm_b200.integration.patch_reference()` substitutes `esm.modules.TransformerLayer.forward`, the seam SURVEY
+The reference package is imported from `oracle/_ref`, which build() makes by the recipe in oracle/reference.py
+(git-ignored; it travels with the tree to the GPU machine).  `esm_b200.integration.patch_reference()` substitutes `esm.modules.TransformerLayer.forward`, the seam SURVEY
 §8b names (`esm/modules.py:120-142` called from `esm/model/esm2.py:111-116`), exactly like the reference's own apex
 FusedLayerNorm substitution (`esm/modules.py:68-81`); everything else — `ESM2.forward`'s loop, embedding prologue, LM
 head, contact head — is the reference's own code executing on the GPU.
@@ -16,7 +15,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def rel_fro(a, b):
@@ -26,7 +25,7 @@ def rel_fro(a, b):
 @pytest.fixture(scope="module")
 def esm_ref():
     if not os.path.isdir(os.path.join(REF, "esm")):
-        pytest.skip("baseline/_ref (offline install of the reference) is not present")
+        pytest.fail("oracle/_ref/esm is missing: build() copies the reference there (oracle/reference.py)")
     sys.path.insert(0, REF)
     try:
         import esm  # the reference
