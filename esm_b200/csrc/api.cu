@@ -129,6 +129,12 @@ int make_tmap_f16(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t col
   return make_tmap_2d(map, ptr, 2, rows, cols, ld_elems, box_rows);
 }
 
+// output of gemm2_f16_kernel: dense row-major [rows, cols] fp16 (esize 2) or fp32 (esize 4), written in boxes of one
+// MMA warpgroup's 64 rows
+int make_gemm_out_map(CUtensorMap* map, const void* out, int esize, uint64_t rows, uint64_t cols) {
+  return make_tmap_2d(map, out, esize, rows, cols, cols, gemm2_cfg::OUT_BOX_ROWS);
+}
+
 // 64-wide column slots per head on the attention side: 1 for head_dim <= 64, 2 up to 128 (elementwise.cuh head_slot)
 inline int head_slots(int E, int H) { return (H > 0 && E / H > 64) ? 2 : 1; }
 
@@ -160,29 +166,29 @@ int check_device() {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st,
-                int tag = T_GEMM_OTHER, bool split = false) {
+int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmParams& p,
+                cudaStream_t st, int tag = T_GEMM_OTHER, bool split = false) {
   ProfScope ps(tag, st);
   cudaError_t e;
   if (split) {  // fp32x3 precision: operands stored as fp16 hi | lo along K (gemm2.cuh)
     if (p.K % 64 != 0) return fail(ESMB200_EINVAL, "fp32x3 precision needs K % 64 == 0");
     switch (epi) {
-      case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE, true>(ta, tb, p, num_sms(), st); break;
-      case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL, true>(ta, tb, p, num_sms(), st); break;
-      case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU, true>(ta, tb, p, num_sms(), st); break;
-      case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32, true>(ta, tb, p, num_sms(), st); break;
-      case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32, true>(ta, tb, p, num_sms(), st); break;
+      case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE, true>(ta, tb, to, p, num_sms(), st); break;
+      case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL, true>(ta, tb, to, p, num_sms(), st); break;
+      case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU, true>(ta, tb, to, p, num_sms(), st); break;
+      case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32, true>(ta, tb, to, p, num_sms(), st); break;
+      case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32, true>(ta, tb, to, p, num_sms(), st); break;
       default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
     }
     if (e != cudaSuccess) return fail_cuda(e, "gemm launch (fp32x3)");
     return ESMB200_OK;
   }
   switch (epi) {
-    case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE>(ta, tb, p, num_sms(), st); break;
-    case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL>(ta, tb, p, num_sms(), st); break;
-    case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU>(ta, tb, p, num_sms(), st); break;
-    case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32>(ta, tb, p, num_sms(), st); break;
-    case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32>(ta, tb, p, num_sms(), st); break;
+    case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32>(ta, tb, to, p, num_sms(), st); break;
     default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
   }
   if (e != cudaSuccess) return fail_cuda(e, "gemm launch");
@@ -498,6 +504,7 @@ int carve_workspace(Workspace* ws, void* workspace, size_t bytes, int E, int H, 
 
 struct ActMaps {
   CUtensorMap xn, ctx, h;       // A operands (fp16, box {64,128})
+  CUtensorMap qkv_o, h_o, x_o;  // GEMM outputs: qkv and h (fp16), the fp32 residual stream x
 };
 
 int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* rope_cos, const float* rope_sin,
@@ -517,11 +524,11 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   // q,k,v projections + bias + q scale + RoPE (multihead_attention.py:258-261,354-355)
   GemmParams g;
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = 3 * Ea; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * Ea;
+  g.M = M; g.N = 3 * Ea; g.K = E; g.bias = L->b_qkv;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = Ea; g.q_scale = L->q_scale;
   g.lo_col_off = 3 * Ea;
   g.rope_ld = 32 * L->slots;
-  int rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV, split);
+  int rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV, split);
   if (rc) return rc;
   // attention (multihead_attention.py:357-394)
   rc = run_attention(ws.qkv, ws.ctx, attn_probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split, contact,
@@ -529,8 +536,8 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   if (rc) return rc;
   // out_proj + residual (multihead_attention.py:395, modules.py:134)
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = E; g.K = Ea; g.bias = L->out_b; g.out = x; g.ldo = E;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT, split);
+  g.M = M; g.N = E; g.K = Ea; g.bias = L->out_b;
+  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT, split);
   if (rc) return rc;
   // LN2 -> fp16 (modules.py:137)
   {
@@ -541,21 +548,24 @@ int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* ro
   if (e != cudaSuccess) return fail_cuda(e, "layernorm2");
   // fc1 + GELU (modules.py:138)
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.out = ws.h; g.ldo = F; g.lo_col_off = F;
-  rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, g, st, T_FC1, split);
+  g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.lo_col_off = F;
+  rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1, split);
   if (rc) return rc;
   // fc2 + residual (modules.py:139-140)
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b; g.out = x; g.ldo = E;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, g, st, T_FC2, split);
+  g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b;
+  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, g, st, T_FC2, split);
   return rc;
 }
 
-int make_act_maps(ActMaps* am, const Workspace& ws, int E, int H, int F, int M, int split = 0) {
+int make_act_maps(ActMaps* am, const Workspace& ws, float* x, int E, int H, int F, int M, int split = 0) {
   const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;  // fp32x3: activations are [rows, 2 * width]
   int rc = make_tmap_f16(&am->xn, ws.xn, M, pf * E, pf * E, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&am->ctx, ws.ctx, M, pf * Ea, pf * Ea, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&am->h, ws.h, M, pf * F, pf * F, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_gemm_out_map(&am->qkv_o, ws.qkv, 2, M, pf * 3 * Ea);
+  if (!rc) rc = make_gemm_out_map(&am->h_o, ws.h, 2, M, pf * F);
+  if (!rc) rc = make_gemm_out_map(&am->x_o, x, 4, M, E);
   return rc;
 }
 }  // namespace
@@ -590,7 +600,7 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
   rc = carve_workspace(&ws, workspace, workspace_bytes, E, H, F, B, T, split);
   if (rc) return rc;
   ActMaps am;
-  rc = make_act_maps(&am, ws, E, H, F, B * T, split);
+  rc = make_act_maps(&am, ws, x, E, H, F, B * T, split);
   if (rc) return rc;
   rc = run_key_bits(pad_mask, ws.as, B, T, st);
   if (rc) return rc;
@@ -666,15 +676,16 @@ int esmb200_gemm_f16(int32_t epilogue, const void* a, const void* w, const float
   if (rc) return rc;
   if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
     return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, to;
   rc = make_tmap_f16(&ta, a, M, K, K, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, N, K, K, gemm2_cfg::HALF_N);
+  if (!rc) rc = make_gemm_out_map(&to, out, f16_out ? 2 : 4, M, N);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = N; g.K = K; g.bias = bias; g.out = out; g.ldo = N;
+  g.M = M; g.N = N; g.K = K; g.bias = bias;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, g, static_cast<cudaStream_t>(stream));
+  return launch_gemm(epilogue, ta, tb, to, g, static_cast<cudaStream_t>(stream));
 }
 
 // ---- fp32x3 precision building blocks (hi | lo fp16 operands): used by the LM head and the kernel-level parity tests
@@ -711,15 +722,16 @@ int esmb200_gemm_split(int32_t epilogue, const void* a, const void* w, const flo
   if (rc) return rc;
   if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
     return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, to;
   rc = make_tmap_f16(&ta, a, M, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, N, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::HALF_N);
+  if (!rc) rc = f16_out ? make_gemm_out_map(&to, out, 2, M, 2 * (uint64_t)N) : make_gemm_out_map(&to, out, 4, M, N);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = N; g.K = K; g.bias = bias; g.out = out; g.ldo = N; g.lo_col_off = N;
+  g.M = M; g.N = N; g.K = K; g.bias = bias; g.lo_col_off = N;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, true);
+  return launch_gemm(epilogue, ta, tb, to, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, true);
 }
 
 int esmb200_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
@@ -743,15 +755,16 @@ int esmb200_gemm_qkv_f16(const void* a, const void* w, const float* bias, void* 
     return fail(ESMB200_EINVAL, "rope tables must be given together with T, or not at all");
   int rc = check_device();
   if (rc) return rc;
-  CUtensorMap ta, tb;
+  CUtensorMap ta, tb, to;
   rc = make_tmap_f16(&ta, a, M, E, E, gemm2_cfg::BOX_M);
   if (!rc) rc = make_tmap_f16(&tb, w, 3 * (uint64_t)E, E, E, gemm2_cfg::HALF_N);
+  if (!rc) rc = make_gemm_out_map(&to, out, 2, M, 3 * (uint64_t)E);
   if (rc) return rc;
   GemmParams g;
   memset(&g, 0, sizeof g);
-  g.M = M; g.N = 3 * E; g.K = E; g.bias = bias; g.out = out; g.ldo = 3 * E;
+  g.M = M; g.N = 3 * E; g.K = E; g.bias = bias;
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T > 0 ? T : 1; g.E = E; g.q_scale = q_scale;
-  return launch_gemm(EPI_QKV_ROPE, ta, tb, g, static_cast<cudaStream_t>(stream));
+  return launch_gemm(EPI_QKV_ROPE, ta, tb, to, g, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
@@ -908,7 +921,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   uint8_t* tied_scratch = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024)) + base_bytes;
   const size_t tied_bytes = esmb200_tied_row_attention_scratch_bytes(B, C, H);
   ActMaps am;
-  rc = make_act_maps(&am, ws, E, H, F, M);
+  rc = make_act_maps(&am, ws, x, E, H, F, M);
   if (rc) return rc;
   rc = run_key_bits(col_pad_mask, ws.as, B * C, R, st);  // column attention: B*C sequences of R keys
   if (rc) return rc;
@@ -928,9 +941,9 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     }
     if (e != cudaSuccess) return fail_cuda(e, "row layernorm");
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * E;
+    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv;
     g.T = 1; g.E = E; g.q_scale = row_scale;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV);
+    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV);
     if (rc) return rc;
     if (pad_mask) {
       ProfScope ps(T_KEYBITS, st);
@@ -941,8 +954,8 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
                        tied_scratch, tied_bytes, stream);
     if (rc) return rc;
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = E; g.bias = L->out_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT);
+    g.M = M; g.N = E; g.K = E; g.bias = L->out_b;
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT);
     if (rc) return rc;
     // ---------------- column attention (modules.py:208-212; axial_attention.py:182-239) ----------------
     L = col_layers[i];
@@ -952,9 +965,9 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     }
     if (e != cudaSuccess) return fail_cuda(e, "column layernorm");
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv; g.out = ws.qkv; g.ldo = 3 * E;
+    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv;
     g.T = 1; g.E = E; g.q_scale = 0.125f;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, g, st, T_QKV);
+    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV);
     if (rc) return rc;
     {
       AttnParams ap;
@@ -966,8 +979,8 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     }
     if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = E; g.bias = L->out_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, g, st, T_OUT);
+    g.M = M; g.N = E; g.K = E; g.bias = L->out_b;
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT);
     if (rc) return rc;
     // ---------------- feed-forward (modules.py:213-214, 413-418) ----------------
     {
@@ -976,12 +989,12 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     }
     if (e != cudaSuccess) return fail_cuda(e, "ffn layernorm");
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.out = ws.h; g.ldo = F;
-    rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, g, st, T_FC1);
+    g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b;
+    rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1);
     if (rc) return rc;
     memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b; g.out = x; g.ldo = E;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, g, st, T_FC2);
+    g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b;
+    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, g, st, T_FC2);
     if (rc) return rc;
   }
   return ESMB200_OK;

@@ -203,6 +203,17 @@ __device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
                : "r"(addr));
 }
 
+// stmatrix: the inverse of ldsm_x4 — thread l supplies the address of row l % 8 of matrix l / 8, and r[j] holds
+// (row lane / 4, columns 2 (lane % 4) ..+1) of matrix j, which is the mma / wgmma accumulator fragment layout
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+
 // byte address of 16-byte chunk `chunk` (0..7) of row `row` in a tile of 128-byte rows written by a TMA box with
 // CU_TENSOR_MAP_SWIZZLE_128B (tile base 1024-byte aligned): the chunk index is XORed with row % 8
 __device__ __forceinline__ uint32_t sw128(uint32_t base, uint32_t row, uint32_t chunk) {

@@ -6,8 +6,11 @@
 //     (48 KB per stage, 128B swizzle) and keeps running ahead into the next tile while the MMA warpgroups finish;
 //   * warpgroups 1 and 2: rows [0,64) and [64,128) of the tile, wgmma m64n256k16 straight from the swizzled stages,
 //     one slab in flight behind the one being issued; the accumulators (128 fp32 registers per thread) are turned into
-//     the output by the epilogue in registers: bias / q-scale + RoPE / erf-GELU, fp16 or fp32 stores, or the
-//     residual update x += y (each element has exactly one writer: no atomics, bit-reproducible).
+//     the output by the epilogue: bias / q-scale + RoPE / erf-GELU in registers, then box by box (64 rows x 128 bytes)
+//     into a 128B-swizzled staging buffer in shared memory (stmatrix for fp16, st.shared for fp32), which one thread
+//     hands to a TMA store, or for the residual update x += y to a TMA reduce-add performed by the L2 (each element
+//     has exactly one writer and one add: bit-reproducible).  Two staging buffers per warpgroup, so the stores drain
+//     while the warpgroup fills the next box and runs the next tile's MMAs.
 #pragma once
 
 #include "gemm_common.cuh"
@@ -24,24 +27,39 @@ constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int BOX_M = 128;        // rows of an A-operand TMA box
+constexpr int OUT_BOX_ROWS = 64;  // rows of an output TMA box: one MMA warpgroup's half of the tile
+constexpr int OUT_BOX_BYTES = OUT_BOX_ROWS * 128;  // 64 fp16 or 32 fp32 columns per row
+constexpr int OUT_BUFS = 2;       // staging buffers per MMA warpgroup
 constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * OUT_BUFS * OUT_BOX_BYTES + 1024 + 256;  // 230656 B
 }  // namespace gemm2_cfg
+
+// An fp16 64 x 64 output box of one MMA warpgroup into a 128B-swizzled staging buffer (the layout the output TMA map
+// reads): h[2 b + hr] holds the warp's rows g + 8 hr, columns 8 b + 2 c ..+1 (the accumulator fragment layout, which is
+// stmatrix's).  Each x4 writes blocks 2s, 2s + 1 for both row halves; 8 rows x 16 bytes per matrix, conflict-free.
+__device__ __forceinline__ void stage_box_f16(uint32_t buf, uint32_t warp, uint32_t lane, const uint32_t (&h)[16]) {
+  const uint32_t m = lane / 8;  // matrix this lane addresses: block 2s + m / 2, row half m % 2
+#pragma unroll
+  for (int s = 0; s < 4; ++s)
+    stsm_x4(sw128(buf, warp * 16 + (m % 2) * 8 + lane % 8, 2 * s + m / 2), h[4 * s], h[4 * s + 1], h[4 * s + 2],
+            h[4 * s + 3]);
+}
 
 // SPLIT ("fp32x3" precision): both operands are stored as fp16 hi | lo halves along K (A [M,2K], B [N,2K]); the K loop
 // runs hi*hi + lo*hi + hi*lo (three passes over the same fp32 accumulator: 22 significand bits per operand, the
 // dropped lo*lo term is 2^-22 relative), and fp16 outputs are written as hi | lo pairs as well (lo part p.lo_col_off
-// columns to the right, row pitch 2 * ldo).  Requires K % 64 == 0.
+// columns to the right in an [M, 2N] output map).  Requires K % 64 == 0.
 template <int EPI, bool SPLIT = false>
 __global__ void __launch_bounds__(gemm2_cfg::NUM_THREADS, 1)
 gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmParams p) {
+                 const __grid_constant__ CUtensorMap tmap_o, const GemmParams p) {
   using namespace gemm2_cfg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint8_t* smem_out = smem + STAGES * STAGE_BYTES;  // [2 warpgroups][OUT_BUFS] output boxes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_out + 2 * OUT_BUFS * OUT_BOX_BYTES);
   uint64_t* full_bar = bars;            // [STAGES] TMA -> MMA
   uint64_t* empty_bar = bars + STAGES;  // [STAGES] MMA warpgroups -> TMA (one arrival each)
 
@@ -55,6 +73,7 @@ gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_o);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);
@@ -100,9 +119,29 @@ gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const bool signal = (threadIdx.x % 128) == 0;
   const uint32_t a_base = smem_u32(smem_a) + mw * 64 * 128;
   const uint32_t b_base = smem_u32(smem_b);
-  const size_t pitch = (SPLIT && (EPI == EPI_QKV_ROPE || EPI == EPI_BIAS_GELU)) ? 2 * (size_t)p.ldo : (size_t)p.ldo;
+  uint8_t* const out_bufs = smem_out + mw * OUT_BUFS * OUT_BOX_BYTES;
+  uint32_t ob = 0;  // staging buffer the warpgroup fills next
   uint32_t it = 0;
   float acc[128];
+
+  // Hand the filled staging buffer to the TMA engine as the output box at (column c0, row c1).  Every thread fences
+  // its shared-memory writes for the async proxy; before the warpgroup barrier the issuing thread waits until the
+  // previous box's store has finished reading the other buffer, so after the barrier that buffer is free to fill while
+  // this box drains (one barrier per box).  Only the issuing thread commits bulk groups, so only it may wait on them.
+  auto store_box = [&](int c0, int c1) {
+    fence_proxy_async_smem();
+    if (signal) tma_store_wait_read<0>();
+    named_bar_sync(1 + mw, 128);
+    if (signal) {
+      if constexpr (EPI == EPI_BIAS_RESIDUAL) {
+        tma_reduce_add_2d(&tmap_o, out_bufs + ob * OUT_BOX_BYTES, c0, c1);
+      } else {
+        tma_store_2d(&tmap_o, out_bufs + ob * OUT_BOX_BYTES, c0, c1);
+      }
+      tma_store_commit();
+    }
+    ob ^= 1;
+  };
 
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m0 = (tile / tiles_n) * BLOCK_M, n0 = (tile % tiles_n) * BLOCK_N;
@@ -125,99 +164,132 @@ gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     reg_fence_f(acc);
     if (signal) mbar_arrive(&empty_bar[(it + STAGES - 1) % STAGES]);
 
-    // ---- epilogue: thread holds rows r0 and r0 + 8, columns n0 + 8 i + 2 c + {0, 1} for i < 32
+    // ---- epilogue: thread holds rows r0 and r0 + 8, columns n0 + 8 i + 2 c + {0, 1} for i < 32.  Boxes whose first
+    // column is >= N are skipped (N % 64 == 0 for fp16 outputs, so fp16 boxes are whole); TMA clips rows >= M and the
+    // columns >= N of a partial fp32 box.
     const int r0 = m0 + (int)(mw * 64 + warp * 16 + g);
-    const int rows[2] = {r0, r0 + 8};
-    if constexpr (EPI == EPI_QKV_ROPE) {
-      const bool rope = p.rope_cos != nullptr;
-      const int ld = p.rope_ld == 64 ? 64 : 32;
+    const int box_row = m0 + (int)mw * 64;
+    if constexpr (EPI == EPI_QKV_ROPE || EPI == EPI_BIAS_GELU) {
 #pragma unroll
-      for (int gi = 0; gi < 4; ++gi) {  // 64-column groups: column j pairs with j + 32 (same thread)
+      for (int gi = 0; gi < 4; ++gi) {  // 64-column boxes
         const int col0 = n0 + gi * 64;
         if (col0 >= p.N) break;
-        const int sect = col0 / p.E;  // 0 q, 1 k, 2 v
-        const float sc = (sect == 0) ? p.q_scale : 1.0f;
-        const int slot = p.rope_ld == 64 ? ((col0 >> 6) & 1) : 0;
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const int row = rows[hr];
-          if (row >= p.M) continue;
-          const int t = row % p.T;
-          __half* o = reinterpret_cast<__half*>(p.out) + (size_t)row * pitch;
+        uint32_t hi[16], lo[16];  // [2 b + hr]: 8-column block b of the box, rows r0 + 8 hr
+        if constexpr (EPI == EPI_QKV_ROPE) {  // column j pairs with j + 32 (same thread)
+          const int sect = col0 / p.E;  // 0 q, 1 k, 2 v
+          const float sc = (sect == 0) ? p.q_scale : 1.0f;
+          // Every bias / table load of the box is issued before the first is used: one memory latency per box rather
+          // than one per column pair (the rotation's branch would otherwise split them into dependent steps).
+          float2 bl[4], bh[4], cs[2][4], sn[2][4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const int j = 8 * q + 2 * (int)c;  // column pair (j, j + 1) and (j + 32, j + 33) of the group
-            const float2 bl = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + j));
-            const float2 bh = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + j));
-            float a0 = (acc[4 * (8 * gi + q) + 2 * hr] + bl.x) * sc, a1 = (acc[4 * (8 * gi + q) + 2 * hr + 1] + bl.y) * sc;
-            float b0 = (acc[4 * (8 * gi + q + 4) + 2 * hr] + bh.x) * sc;
-            float b1 = (acc[4 * (8 * gi + q + 4) + 2 * hr + 1] + bh.y) * sc;
-            if (sect < 2 && rope) {  // rotary_embedding.py:16-20, rotate_half = cat(-x2, x1)
-              const float2 cs = __ldg(reinterpret_cast<const float2*>(p.rope_cos + (size_t)t * ld + slot * 32 + j));
-              const float2 sn = __ldg(reinterpret_cast<const float2*>(p.rope_sin + (size_t)t * ld + slot * 32 + j));
-              const float ra0 = a0 * cs.x - b0 * sn.x, rb0 = b0 * cs.x + a0 * sn.x;
-              const float ra1 = a1 * cs.y - b1 * sn.y, rb1 = b1 * cs.y + a1 * sn.y;
-              a0 = ra0; b0 = rb0; a1 = ra1; b1 = rb1;
-            }
-            const __half2 ha = __floats2half2_rn(a0, a1), hb = __floats2half2_rn(b0, b1);
-            *reinterpret_cast<__half2*>(o + col0 + j) = ha;
-            *reinterpret_cast<__half2*>(o + col0 + 32 + j) = hb;
-            if constexpr (SPLIT) {
-              const float2 fa = __half22float2(ha), fb = __half22float2(hb);
-              *reinterpret_cast<__half2*>(o + p.lo_col_off + col0 + j) = __floats2half2_rn(a0 - fa.x, a1 - fa.y);
-              *reinterpret_cast<__half2*>(o + p.lo_col_off + col0 + 32 + j) = __floats2half2_rn(b0 - fb.x, b1 - fb.y);
+            bl[q] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * q + 2 * (int)c));
+            bh[q] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + 8 * q + 2 * (int)c));
+          }
+          const bool rotate = sect < 2 && p.rope_cos != nullptr;  // uniform over the box
+          if (rotate) {
+            const int ld = p.rope_ld == 64 ? 64 : 32;
+            const int slot = p.rope_ld == 64 ? ((col0 >> 6) & 1) : 0;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const int t = (r0 + 8 * hr) % p.T;  // rows >= M read a valid table row too; TMA drops them
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const size_t at = (size_t)t * ld + slot * 32 + 8 * q + 2 * (int)c;
+                cs[hr][q] = __ldg(reinterpret_cast<const float2*>(p.rope_cos + at));
+                sn[hr][q] = __ldg(reinterpret_cast<const float2*>(p.rope_sin + at));
+              }
             }
           }
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {  // column pair (j, j + 1) and (j + 32, j + 33) of the box, j = 8 q + 2 c
+              float a0 = (acc[4 * (8 * gi + q) + 2 * hr] + bl[q].x) * sc;
+              float a1 = (acc[4 * (8 * gi + q) + 2 * hr + 1] + bl[q].y) * sc;
+              float b0 = (acc[4 * (8 * gi + q + 4) + 2 * hr] + bh[q].x) * sc;
+              float b1 = (acc[4 * (8 * gi + q + 4) + 2 * hr + 1] + bh[q].y) * sc;
+              if (rotate) {  // rotary_embedding.py:16-20, rotate_half = cat(-x2, x1)
+                const float2 co = cs[hr][q], si = sn[hr][q];
+                const float ra0 = a0 * co.x - b0 * si.x, rb0 = b0 * co.x + a0 * si.x;
+                const float ra1 = a1 * co.y - b1 * si.y, rb1 = b1 * co.y + a1 * si.y;
+                a0 = ra0; b0 = rb0; a1 = ra1; b1 = rb1;
+              }
+              hi[2 * q + hr] = pack_half2(a0, a1);
+              hi[2 * (q + 4) + hr] = pack_half2(b0, b1);
+              if constexpr (SPLIT) {
+                const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * q + hr]));
+                const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * (q + 4) + hr]));
+                lo[2 * q + hr] = pack_half2(a0 - fa.x, a1 - fa.y);
+                lo[2 * (q + 4) + hr] = pack_half2(b0 - fb.x, b1 - fb.y);
+              }
+            }
+          }
+        } else {
+#pragma unroll
+          for (int b = 0; b < 8; ++b) {
+            const int i = 8 * gi + b;
+            const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * b + 2 * (int)c));
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const float y0 = gelu_erf(acc[4 * i + 2 * hr] + bb.x), y1 = gelu_erf(acc[4 * i + 2 * hr + 1] + bb.y);
+              hi[2 * b + hr] = pack_half2(y0, y1);
+              if constexpr (SPLIT) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * b + hr]));
+                lo[2 * b + hr] = pack_half2(y0 - f.x, y1 - f.y);
+              }
+            }
+          }
+        }
+        stage_box_f16(smem_u32(out_bufs + ob * OUT_BOX_BYTES), warp, lane, hi);
+        store_box(col0, box_row);
+        if constexpr (SPLIT) {  // the lo halves: p.lo_col_off columns to the right in the [M, 2N] output map
+          stage_box_f16(smem_u32(out_bufs + ob * OUT_BOX_BYTES), warp, lane, lo);
+          store_box(p.lo_col_off + col0, box_row);
         }
       }
-    } else {
+    } else {  // fp32 output: 32-column boxes
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int col = n0 + 8 * i + 2 * (int)c;
-        if (col >= p.N) break;  // N % 32 == 0 (fp32) / % 64 == 0 (fp16): whole 8-column blocks are in or out
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+      for (int gi = 0; gi < 8; ++gi) {
+        const int col0 = n0 + gi * 32;
+        if (col0 >= p.N) break;
+        const uint32_t buf = smem_u32(out_bufs + ob * OUT_BOX_BYTES);
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const int row = rows[hr];
-          if (row >= p.M) continue;
-          float y0 = acc[4 * i + 2 * hr] + bb.x, y1 = acc[4 * i + 2 * hr + 1] + bb.y;
-          if constexpr (EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_GELU_F32) {
-            y0 = gelu_erf(y0);
-            y1 = gelu_erf(y1);
-          }
-          if constexpr (EPI == EPI_BIAS_GELU) {
-            __half* o = reinterpret_cast<__half*>(p.out) + (size_t)row * pitch + col;
-            const __half2 h = __floats2half2_rn(y0, y1);
-            *reinterpret_cast<__half2*>(o) = h;
-            if constexpr (SPLIT) {
-              const float2 f = __half22float2(h);
-              *reinterpret_cast<__half2*>(o + p.lo_col_off) = __floats2half2_rn(y0 - f.x, y1 - f.y);
+        for (int b = 0; b < 4; ++b) {
+          const int i = 4 * gi + b;
+          // N % 16 == 0: an 8-column block is wholly in or out; the bias of an out-of-range block is never stored
+          const float2 bb = col0 + 8 * b < p.N
+                                ? __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * b + 2 * (int)c))
+                                : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            float y0 = acc[4 * i + 2 * hr] + bb.x, y1 = acc[4 * i + 2 * hr + 1] + bb.y;
+            if constexpr (EPI == EPI_BIAS_GELU_F32) {
+              y0 = gelu_erf(y0);
+              y1 = gelu_erf(y1);
             }
-          } else {
-            float2* o = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * pitch + col);
-            if constexpr (EPI == EPI_BIAS_RESIDUAL) {
-              const float2 x = *o;
-              *o = make_float2(x.x + y0, x.y + y1);
-            } else {
-              *o = make_float2(y0, y1);
-            }
+            // bytes 32 b + 8 c of row 16 warp + 8 hr + g: 16-byte chunk 2 b + c / 2; 8 rows x 32 bytes per warp
+            // store spread over all 32 banks twice (the minimum two wavefronts)
+            st_shared_f32x2(sw128(buf, warp * 16 + 8 * hr + g, 2 * b + c / 2) + (c % 2) * 8, y0, y1);
           }
         }
+        store_box(col0, box_row);  // EPI_BIAS_RESIDUAL: x += y in the L2
       }
     }
   }
+  if (signal) tma_store_wait_all();  // the staging buffers must outlive the stores reading them
 }
 
 template <int EPI, bool SPLIT = false>
-inline cudaError_t launch_gemm2_epi(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int num_sms,
-                                    cudaStream_t stream) {
+inline cudaError_t launch_gemm2_epi(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
+                                    const GemmParams& p, int num_sms, cudaStream_t stream) {
   using namespace gemm2_cfg;
   cudaError_t e =
       cudaFuncSetAttribute(gemm2_f16_kernel<EPI, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   if (e != cudaSuccess) return e;
   const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
   const int grid = tiles < num_sms ? tiles : num_sms;
-  return launch_pdl(gemm2_f16_kernel<EPI, SPLIT>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, ta, tb, p);
+  return launch_pdl(gemm2_f16_kernel<EPI, SPLIT>, dim3(grid), dim3(NUM_THREADS), SMEM_BYTES, stream, ta, tb, to, p);
 }
 
 }  // namespace esmb200

@@ -17,9 +17,7 @@ enum : int { EPI_QKV_ROPE = 0, EPI_BIAS_RESIDUAL = 1, EPI_BIAS_GELU = 2, EPI_BIA
 
 struct GemmParams {
   int M, N, K;
-  const float* bias;      // [N] fp32
-  void* out;              // fp16 or fp32, row-major [M, ldo]
-  int ldo;
+  const float* bias;      // [N] fp32 (the output, fp16 or fp32 row-major [M, N], is the kernel's output tensor map)
   // EPI_QKV_ROPE only
   const float* rope_cos;  // [T, rope_ld] fp32 (angle t * inv_freq[j], j < d/2; further columns are padding)
   const float* rope_sin;
