@@ -166,33 +166,37 @@ int check_device() {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+template <bool SPLIT>
+cudaError_t launch_gemm_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
+                            const GemmParams& p, cudaStream_t st) {
+  switch (epi) {
+    case EPI_QKV_ROPE: return launch_gemm2_epi<EPI_QKV_ROPE, SPLIT>(ta, tb, to, p, num_sms(), st);
+    case EPI_BIAS_RESIDUAL: return launch_gemm2_epi<EPI_BIAS_RESIDUAL, SPLIT>(ta, tb, to, p, num_sms(), st);
+    case EPI_BIAS_GELU: return launch_gemm2_epi<EPI_BIAS_GELU, SPLIT>(ta, tb, to, p, num_sms(), st);
+    case EPI_BIAS_F32: return launch_gemm2_epi<EPI_BIAS_F32, SPLIT>(ta, tb, to, p, num_sms(), st);
+    case EPI_BIAS_GELU_F32: return launch_gemm2_epi<EPI_BIAS_GELU_F32, SPLIT>(ta, tb, to, p, num_sms(), st);
+    default: return cudaErrorInvalidValue;  // launch_gemm rejects unknown epilogues first
+  }
+}
+
 int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmParams& p,
                 cudaStream_t st, int tag = T_GEMM_OTHER, bool split = false) {
   ProfScope ps(tag, st);
-  cudaError_t e;
-  if (split) {  // fp32x3 precision: operands stored as fp16 hi | lo along K (gemm2.cuh)
-    if (p.K % 64 != 0) return fail(ESMB200_EINVAL, "fp32x3 precision needs K % 64 == 0");
-    switch (epi) {
-      case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE, true>(ta, tb, to, p, num_sms(), st); break;
-      case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL, true>(ta, tb, to, p, num_sms(), st); break;
-      case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU, true>(ta, tb, to, p, num_sms(), st); break;
-      case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32, true>(ta, tb, to, p, num_sms(), st); break;
-      case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32, true>(ta, tb, to, p, num_sms(), st); break;
-      default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "gemm launch (fp32x3)");
-    return ESMB200_OK;
-  }
-  switch (epi) {
-    case EPI_QKV_ROPE: e = launch_gemm2_epi<EPI_QKV_ROPE>(ta, tb, to, p, num_sms(), st); break;
-    case EPI_BIAS_RESIDUAL: e = launch_gemm2_epi<EPI_BIAS_RESIDUAL>(ta, tb, to, p, num_sms(), st); break;
-    case EPI_BIAS_GELU: e = launch_gemm2_epi<EPI_BIAS_GELU>(ta, tb, to, p, num_sms(), st); break;
-    case EPI_BIAS_F32: e = launch_gemm2_epi<EPI_BIAS_F32>(ta, tb, to, p, num_sms(), st); break;
-    case EPI_BIAS_GELU_F32: e = launch_gemm2_epi<EPI_BIAS_GELU_F32>(ta, tb, to, p, num_sms(), st); break;
-    default: return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
-  }
-  if (e != cudaSuccess) return fail_cuda(e, "gemm launch");
+  // fp32x3 precision: operands stored as fp16 hi | lo along K (gemm2.cuh)
+  if (split && p.K % 64 != 0) return fail(ESMB200_EINVAL, "fp32x3 precision needs K % 64 == 0");
+  if (epi < EPI_QKV_ROPE || epi > EPI_BIAS_GELU_F32) return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
+  const cudaError_t e =
+      split ? launch_gemm_epi<true>(epi, ta, tb, to, p, st) : launch_gemm_epi<false>(epi, ta, tb, to, p, st);
+  if (e != cudaSuccess) return fail_cuda(e, split ? "gemm launch (fp32x3)" : "gemm launch");
   return ESMB200_OK;
+}
+
+// every GemmParams field an epilogue does not read stays zero
+GemmParams gemm_params(int M, int N, int K, const float* bias) {
+  GemmParams g;
+  memset(&g, 0, sizeof g);
+  g.M = M; g.N = N; g.K = K; g.bias = bias;
+  return g;
 }
 
 // scratch layout of the attention kernels
@@ -202,24 +206,20 @@ struct AttnScratch {
   float* row_max;
   float* row_sum;
   int words;
+  size_t bytes;  // size of the whole layout
 };
 
-size_t attn_scratch_bytes(int B, int T, int H) {
-  const int words = (int)align_up((size_t)(T + 31) / 32, 4);
-  return align_up((size_t)B * words * 4, 256) + align_up((size_t)B * 4, 256) + 2 * align_up((size_t)B * H * T * 4, 256);
-}
-
-AttnScratch carve_attn_scratch(void* scratch, int B, int T, int H) {
+// the one definition of the layout: base 0 measures it (esmb200_attention_scratch_bytes), a device address carves it
+AttnScratch attn_scratch_layout(uintptr_t base, int B, int T, int H) {
   AttnScratch s;
   s.words = (int)align_up((size_t)(T + 31) / 32, 4);
-  uint8_t* p = static_cast<uint8_t*>(scratch);
-  s.keybits = reinterpret_cast<uint32_t*>(p);
-  p += align_up((size_t)B * s.words * 4, 256);
-  s.kvlen = reinterpret_cast<int*>(p);
-  p += align_up((size_t)B * 4, 256);
-  s.row_max = reinterpret_cast<float*>(p);
-  p += align_up((size_t)B * H * T * 4, 256);
-  s.row_sum = reinterpret_cast<float*>(p);
+  const size_t keybits = align_up((size_t)B * s.words * 4, 256), kvlen = align_up((size_t)B * 4, 256);
+  const size_t stats = align_up((size_t)B * H * T * 4, 256);
+  s.keybits = reinterpret_cast<uint32_t*>(base);
+  s.kvlen = reinterpret_cast<int*>(base + keybits);
+  s.row_max = reinterpret_cast<float*>(base + keybits + kvlen);
+  s.row_sum = reinterpret_cast<float*>(base + keybits + kvlen + stats);
+  s.bytes = keybits + kvlen + 2 * stats;
   return s;
 }
 
@@ -304,6 +304,58 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
   return ESMB200_OK;
 }
 
+// MSA column attention (axial_attention.py:182-239) straight from the row-major qkv [B*R*C, 3E]: one "sequence" of R
+// tokens per alignment column, read with strided TMA boxes (qkv viewed as [B*R, C*3E], AttnParams::cols), no
+// regrouping copy.  s holds the key bits of the B*C column sequences.
+int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B, int R, int C, int H,
+                         cudaStream_t st) {
+  const int E = H * 64;
+  CUtensorMap tq, tkv;
+  const uint64_t wide = (uint64_t)C * 3 * E;  // token r of column c at row r, x = c*3E
+  int rc;
+  if ((rc = make_tmap_f16(&tq, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_Q))) return rc;
+  if ((rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_KV))) return rc;
+  AttnParams ap;
+  ap.B = B * C; ap.T = R; ap.H = H; ap.E = E;
+  ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
+  ap.ctx = static_cast<__half*>(ctx);
+  ap.row_max = nullptr; ap.row_sum = nullptr;
+  ap.cols = C;
+  cudaError_t e;
+  {
+    ProfScope ps(T_ATTN, st);
+    e = launch_attention_fwd(tq, tkv, ap, st);
+  }
+  if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
+  return ESMB200_OK;
+}
+
+// LayerNorm -> fp16 GEMM operand [M, E], or with split the fp32x3 hi | lo halves [M, 2E]
+int layernorm_f16(const float* x, const float* w, const float* b, void* out, int M, int E, float eps, bool split,
+                  int tag, cudaStream_t st) {
+  cudaError_t e;
+  {
+    ProfScope ps(tag, st);
+    e = split ? launch_layernorm<2>(x, w, b, out, M, E, eps, st) : launch_layernorm<1>(x, w, b, out, M, E, eps, st);
+  }
+  if (e != cudaSuccess) return fail_cuda(e, split ? "layernorm_split" : "layernorm_f16");
+  return ESMB200_OK;
+}
+
+// fp32 [rows, K] -> fp16 [rows, K], or with split the fp32x3 hi | lo halves [rows, 2K]
+int convert_f16(const float* src, void* dst, size_t rows, int K, bool split, cudaStream_t st) {
+  const size_t n = rows * (size_t)K;
+  size_t blocks = (n + 255) / 256;
+  if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
+  ProfScope ps(T_CONVERT, st);
+  if (split)
+    convert_f32_split_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), rows, K);
+  else
+    convert_f32_f16_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), n);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -328,6 +380,146 @@ struct esmb200_layer {
   CUtensorMap tm_qkv, tm_out, tm_fc1, tm_fc2;  // B operands, box {64, 128 rows}
 };
 
+namespace {
+struct Workspace {
+  __half* xn;
+  __half* qkv;
+  __half* ctx;
+  __half* h;     // aliases qkv + ctx
+  AttnScratch as;
+  size_t bytes;  // size of the whole layout, including 1024 bytes to align the caller's pointer
+};
+
+// the one definition of the layer workspace: nullptr measures it (esmb200_workspace_bytes), a device pointer carves it
+Workspace workspace_layout(void* workspace, int E, int H, int F, int B, int T, int split) {
+  const size_t M = (size_t)B * T, Ea = (size_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;
+  const uintptr_t base = workspace ? align_up(reinterpret_cast<uintptr_t>(workspace), 1024) : 0;
+  const size_t xn = align_up(M * E * 2 * pf, 1024);  // fp16 [M,E] (hi | lo)
+  const size_t qkv = align_up(M * 3 * Ea * 2 * pf, 1024), ctx = align_up(M * Ea * 2 * pf, 1024);
+  const size_t h = align_up(M * F * 2 * pf, 1024);
+  const size_t scratch = xn + (qkv + ctx > h ? qkv + ctx : h);
+  Workspace ws;
+  ws.xn = reinterpret_cast<__half*>(base);
+  ws.qkv = ws.h = reinterpret_cast<__half*>(base + xn);
+  ws.ctx = reinterpret_cast<__half*>(base + xn + qkv);
+  ws.as = attn_scratch_layout(base + scratch, B, T, H);
+  ws.bytes = scratch + ws.as.bytes + 1024;
+  return ws;
+}
+
+struct ActMaps {
+  CUtensorMap xn, ctx, h;       // A operands (fp16, box {64,128})
+  CUtensorMap qkv_o, h_o, x_o;  // GEMM outputs: qkv and h (fp16), the fp32 residual stream x
+};
+
+// x += out_proj(attend()) after LN1 -> fp16 and the q,k,v projection (+ bias, q scale, RoPE when rope_cos is given):
+// the self-attention half of an ESM-2 layer (multihead_attention.py:258-261,354-355,395; modules.py:124-134) and each
+// axial attention sub-layer of the MSA stack.  `attend` reads ws.qkv and writes ws.ctx.
+template <class Attend>
+int attention_block(const esmb200_layer* L, float* x, int M, int T, const float* rope_cos, const float* rope_sin,
+                    float q_scale, const Workspace& ws, const ActMaps& am, cudaStream_t st, Attend attend) {
+  const bool split = L->split != 0;
+  int rc = layernorm_f16(x, L->ln1_w, L->ln1_b, ws.xn, M, L->E, L->eps, split, T_LN1, st);
+  if (rc) return rc;
+  GemmParams g = gemm_params(M, 3 * L->Ea, L->E, L->b_qkv);
+  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.rope_ld = 32 * L->slots; g.T = T; g.E = L->Ea; g.q_scale = q_scale;
+  g.lo_col_off = 3 * L->Ea;
+  if ((rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV, split))) return rc;
+  if ((rc = attend())) return rc;
+  return launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, gemm_params(M, L->E, L->Ea, L->out_b), st, T_OUT,
+                     split);
+}
+
+// x += fc2(GELU(fc1(LN2(x)))) (modules.py:137-140, 413-418)
+int ffn_block(const esmb200_layer* L, float* x, int M, const Workspace& ws, const ActMaps& am, cudaStream_t st) {
+  const bool split = L->split != 0;
+  int rc = layernorm_f16(x, L->ln2_w, L->ln2_b, ws.xn, M, L->E, L->eps, split, T_LN2, st);
+  if (rc) return rc;
+  GemmParams g = gemm_params(M, L->F, L->E, L->fc1_b);
+  g.lo_col_off = L->F;
+  if ((rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1, split))) return rc;
+  return launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, gemm_params(M, L->E, L->F, L->fc2_b), st, T_FC2,
+                     split);
+}
+
+int make_act_maps(ActMaps* am, const Workspace& ws, float* x, int E, int H, int F, int M, int split = 0) {
+  const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;  // fp32x3: activations are [rows, 2 * width]
+  int rc = make_tmap_f16(&am->xn, ws.xn, M, pf * E, pf * E, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_tmap_f16(&am->ctx, ws.ctx, M, pf * Ea, pf * Ea, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_tmap_f16(&am->h, ws.h, M, pf * F, pf * F, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_gemm_out_map(&am->qkv_o, ws.qkv, 2, M, pf * 3 * Ea);
+  if (!rc) rc = make_gemm_out_map(&am->h_o, ws.h, 2, M, pf * F);
+  if (!rc) rc = make_gemm_out_map(&am->x_o, x, 4, M, E);
+  return rc;
+}
+
+// The standalone GEMMs: out = epilogue(a . w^T + bias) with a [M, K] and w [N, K] fp16, or with split their fp32x3
+// hi | lo halves [M, 2K] and [N, 2K] and an fp16 output as hi | lo [M, 2N].  The arguments are validated by the caller.
+int run_gemm(int epi, const void* a, const void* w, const float* bias, void* out, int M, int N, int K,
+             const float* rope_cos, const float* rope_sin, int T, int E, float q_scale, bool split, void* stream) {
+  const bool f16_out = (epi == EPI_QKV_ROPE || epi == EPI_BIAS_GELU);
+  const uint64_t pf = split ? 2 : 1;
+  CUtensorMap ta, tb, to;
+  int rc = make_tmap_f16(&ta, a, M, pf * K, pf * K, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_tmap_f16(&tb, w, N, pf * K, pf * K, gemm2_cfg::HALF_N);
+  if (!rc) rc = f16_out ? make_gemm_out_map(&to, out, 2, M, pf * N) : make_gemm_out_map(&to, out, 4, M, N);
+  if (rc) return rc;
+  GemmParams g = gemm_params(M, N, K, bias);
+  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = q_scale;
+  g.lo_col_off = N;
+  return launch_gemm(epi, ta, tb, to, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, split);
+}
+
+// esmb200_gemm_f16 and esmb200_gemm_split
+int gemm_epilogue_entry(int epi, const void* a, const void* w, const float* bias, void* out, int M, int N, int K,
+                        const float* rope_cos, const float* rope_sin, int T, int E, bool split, void* stream) {
+  if (!a || !w || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
+  const bool f16_out = (epi == EPI_QKV_ROPE || epi == EPI_BIAS_GELU);
+  if (M <= 0 || N <= 0 || K <= 0 || K % (split ? 64 : 8) != 0 || N % (f16_out ? 64 : 32) != 0)
+    return fail(ESMB200_EINVAL, std::string(split ? "split gemm needs K % 64 == 0" : "gemm needs K % 8 == 0") +
+                                    " and N % 64 == 0 (fp16 output) / N % 32 == 0 (fp32 output)");
+  if (split && (epi < 0 || epi > EPI_BIAS_GELU_F32)) return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
+  int rc = check_device();
+  if (rc) return rc;
+  if (epi == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
+    return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
+  return run_gemm(epi, a, w, bias, out, M, N, K, rope_cos, rope_sin, T, E, 0.125f, split, stream);
+}
+
+// esmb200_attention (head_dim <= 64), esmb200_attention128 (slots = 2) and esmb200_attention_split (fp32x3)
+int attention_entry(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int B, int T, int H,
+                    void* scratch, void* stream, bool split, int slots) {
+  if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
+  if (B <= 0 || T <= 0 || H <= 0 || H > 64) return fail(ESMB200_EINVAL, "bad shape");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const AttnScratch s = attn_scratch_layout(reinterpret_cast<uintptr_t>(scratch), B, T, H);
+  rc = run_key_bits(pad_mask, s, B, T, st);
+  if (rc) return rc;
+  return run_attention(qkv, ctx, attn_probs, 0, 0, s, B, T, H, st, split, nullptr, slots);
+}
+
+// MSA stack workspace: the layer workspace of the B*C column sequences of R tokens, then the tied row-attention scratch
+struct AxialWorkspace {
+  Workspace ws;
+  uint8_t* tied;
+  size_t tied_bytes;
+  size_t bytes;
+};
+
+// the one definition of the MSA stack workspace: nullptr measures it (esmb200_axial_workspace_bytes), a device pointer
+// carves it
+AxialWorkspace axial_workspace_layout(void* workspace, int E, int F, int B, int R, int C) {
+  AxialWorkspace a;
+  a.ws = workspace_layout(workspace, E, E / 64, F, B * C, R, 0);
+  a.tied = reinterpret_cast<uint8_t*>(a.ws.xn) + a.ws.bytes;
+  a.tied_bytes = esmb200_tied_row_attention_scratch_bytes(B, C, E / 64);
+  a.bytes = a.ws.bytes + a.tied_bytes + 1024;
+  return a;
+}
+}  // namespace
+
 extern "C" {
 
 int esmb200_abi_version(void) { return ESMB200_ABI_VERSION; }
@@ -336,13 +528,7 @@ const char* esmb200_last_error(void) { return g_last_error.c_str(); }
 
 int esmb200_convert_f16(const float* src, void* dst, size_t n, void* stream) {
   if (n == 0) return ESMB200_OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  size_t blocks = (n + 255) / 256;
-  if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
-  ProfScope ps(T_CONVERT, st);
-  convert_f32_f16_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), n);
-  CK(cudaGetLastError());
-  return ESMB200_OK;
+  return convert_f16(src, dst, n, 1, false, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_layer_destroy(esmb200_layer* L) {
@@ -368,28 +554,21 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   if (E % 16 != 0) return fail(ESMB200_EINVAL, "embed_dim must be a multiple of 16");
   const bool has_ffn = w->fc1_weight != nullptr;  // NULL fc1_weight: attention-only layer (MSA row-attention sub-layer)
   if (has_ffn && (F <= 0 || F % 64 != 0)) return fail(ESMB200_EINVAL, "ffn_dim must be a positive multiple of 64");
+  if (w->precision != 0 && w->precision != 1)
+    return fail(ESMB200_EINVAL, "precision must be 0 (fp16 operands) or 1 (fp32x3: fp16 hi|lo operands)");
+  const int split = w->precision;
+  const int slots = head_slots(E, H);
+  if (split && slots == 2) return fail(ESMB200_EINVAL, "fp32x3 precision is not available for head_dim > 64");
+  if (split && E % 64 != 0)
+    return fail(ESMB200_EINVAL, "fp32x3 precision needs embed_dim % 64 == 0 (all ESM-2 models except 35M)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   esmb200_layer* L = new esmb200_layer();
   memset(static_cast<void*>(L), 0, sizeof(*L));
-  const int slots = head_slots(E, H);
   const int Ea = 64 * slots * H;
   L->E = E; L->H = H; L->F = has_ffn ? F : 0; L->d = d; L->slots = slots; L->Ea = Ea; L->eps = w->ln_eps;
   L->q_scale = 1.0f / sqrtf((float)d);
   L->ln1_w = w->ln1_weight; L->ln1_b = w->ln1_bias; L->ln2_w = w->ln2_weight; L->ln2_b = w->ln2_bias;
   L->out_b = w->out_bias; L->fc1_b = w->fc1_bias; L->fc2_b = w->fc2_bias;
-  if (w->precision != 0 && w->precision != 1) {
-    delete L;
-    return fail(ESMB200_EINVAL, "precision must be 0 (fp16 operands) or 1 (fp32x3: fp16 hi|lo operands)");
-  }
-  const int split = w->precision;
-  if (split && slots == 2) {
-    delete L;
-    return fail(ESMB200_EINVAL, "fp32x3 precision is not available for head_dim > 64");
-  }
-  if (split && (E % 64 != 0 || (has_ffn && F % 64 != 0))) {
-    delete L;
-    return fail(ESMB200_EINVAL, "fp32x3 precision needs embed_dim % 64 == 0 (all ESM-2 models except 35M)");
-  }
   L->split = split;
   const size_t pf = split ? 2 : 1;  // fp32x3: every K extent doubles (hi | lo)
   const size_t EaE = (size_t)Ea * E, EF = (size_t)E * F;
@@ -407,48 +586,27 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   }
   ALLOC(L->b_qkv, (size_t)3 * Ea * 4);
 #undef ALLOC
-  auto convert = [&](const float* src, __half* dst, size_t rows, int K) -> int {  // [rows,K] fp32 -> fp16 (hi | lo)
-    if (!split) return esmb200_convert_f16(src, dst, rows * (size_t)K, stream);
-    size_t blocks = (rows * (size_t)K + 255) / 256;
-    if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
+  // every head goes into its zero-padded 64-wide slot(s) (elementwise.cuh head_slot; for head_dim 64 the identity)
+  e = cudaMemsetAsync(L->w_qkv, 0, 3 * EaE * 2 * pf, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(L->w_out, 0, EaE * 2 * pf, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(L->b_qkv, 0, (size_t)3 * Ea * 4, st);
+  if (e != cudaSuccess) rc = fail_cuda(e, "memset(packed weights)");
+  const float* ws3[3] = {w->q_weight, w->k_weight, w->v_weight};
+  const float* bs3[3] = {w->q_bias, w->k_bias, w->v_bias};
+  const unsigned blocks = (unsigned)(((size_t)E * E + 255) / 256);
+  for (int s3 = 0; s3 < 3 && !rc; ++s3) {
     ProfScope ps(T_CONVERT, st);
-    convert_f32_split_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, dst, rows, K);
-    cudaError_t ce = cudaGetLastError();
-    return ce == cudaSuccess ? ESMB200_OK : fail_cuda(ce, "convert_f32_split");
-  };
-  if (d == 64 && !split) {  // slots are full: plain conversion
-    rc = esmb200_convert_f16(w->q_weight, L->w_qkv, EaE, stream);
-    if (!rc) rc = esmb200_convert_f16(w->k_weight, L->w_qkv + EaE, EaE, stream);
-    if (!rc) rc = esmb200_convert_f16(w->v_weight, L->w_qkv + 2 * EaE, EaE, stream);
-    if (!rc) rc = esmb200_convert_f16(w->out_weight, L->w_out, EaE, stream);
-    if (!rc) {
-      e = cudaMemcpyAsync(L->b_qkv, w->q_bias, (size_t)E * 4, cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(L->b_qkv + E, w->k_bias, (size_t)E * 4, cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(L->b_qkv + 2 * E, w->v_bias, (size_t)E * 4, cudaMemcpyDeviceToDevice, st);
-      if (e != cudaSuccess) rc = fail_cuda(e, "bias pack");
-    }
-  } else {  // head_dim < 64 (scatter every head into its zero-padded 64-wide slot) and / or hi | lo operands
-    e = cudaMemsetAsync(L->w_qkv, 0, 3 * EaE * 2 * pf, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(L->w_out, 0, EaE * 2 * pf, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(L->b_qkv, 0, (size_t)3 * Ea * 4, st);
-    if (e != cudaSuccess) rc = fail_cuda(e, "memset(packed weights)");
-    const float* ws3[3] = {w->q_weight, w->k_weight, w->v_weight};
-    const float* bs3[3] = {w->q_bias, w->k_bias, w->v_bias};
-    const unsigned blocks = (unsigned)(((size_t)E * E + 255) / 256);
-    for (int s3 = 0; s3 < 3 && !rc; ++s3) {
-      ProfScope ps(T_CONVERT, st);
-      pack_head_rows_kernel<<<blocks, 256, 0, st>>>(ws3[s3], bs3[s3], L->w_qkv + (size_t)s3 * EaE * pf, L->b_qkv + s3 * Ea,
-                                                    E, d, split);
-      if ((e = cudaGetLastError()) != cudaSuccess) rc = fail_cuda(e, "pack_head_rows");
-    }
-    if (!rc) {
-      ProfScope ps(T_CONVERT, st);
-      pack_head_cols_kernel<<<blocks, 256, 0, st>>>(w->out_weight, L->w_out, E, Ea, d, split);
-      if ((e = cudaGetLastError()) != cudaSuccess) rc = fail_cuda(e, "pack_head_cols");
-    }
+    pack_head_rows_kernel<<<blocks, 256, 0, st>>>(ws3[s3], bs3[s3], L->w_qkv + (size_t)s3 * EaE * pf, L->b_qkv + s3 * Ea,
+                                                  E, d, split);
+    if ((e = cudaGetLastError()) != cudaSuccess) rc = fail_cuda(e, "pack_head_rows");
   }
-  if (!rc && has_ffn) rc = convert(w->fc1_weight, L->w_fc1, F, E);
-  if (!rc && has_ffn) rc = convert(w->fc2_weight, L->w_fc2, E, F);
+  if (!rc) {
+    ProfScope ps(T_CONVERT, st);
+    pack_head_cols_kernel<<<blocks, 256, 0, st>>>(w->out_weight, L->w_out, E, Ea, d, split);
+    if ((e = cudaGetLastError()) != cudaSuccess) rc = fail_cuda(e, "pack_head_cols");
+  }
+  if (!rc && has_ffn) rc = convert_f16(w->fc1_weight, L->w_fc1, F, E, split, st);
+  if (!rc && has_ffn) rc = convert_f16(w->fc2_weight, L->w_fc2, E, F, split, st);
   const uint32_t wbox = gemm2_cfg::HALF_N;
   if (!rc) rc = make_tmap_f16(&L->tm_qkv, L->w_qkv, 3 * (uint64_t)Ea, pf * E, pf * E, wbox);
   if (!rc) rc = make_tmap_f16(&L->tm_out, L->w_out, E, pf * Ea, pf * Ea, wbox);
@@ -465,110 +623,12 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
 size_t esmb200_attention_scratch_bytes(int32_t B, int32_t T) {
   // H is bounded by E/64; the stats arrays are sized by the caller-visible worst case through workspace_bytes,
   // this standalone entry sizes them for H <= 64.
-  return attn_scratch_bytes(B, T, 64);
+  return attn_scratch_layout(0, B, T, 64).bytes;
 }
 
 size_t esmb200_workspace_bytes(int32_t E, int32_t H, int32_t F, int32_t B, int32_t T, int32_t precision) {
-  const size_t M = (size_t)B * T, Ea = (size_t)64 * head_slots(E, H) * H, pf = precision ? 2 : 1;
-  const size_t a = align_up(M * E * 2 * pf, 1024);                  // xn fp16 [M,E] (hi | lo)
-  const size_t big_qkv_ctx = align_up(M * 3 * Ea * 2 * pf, 1024) + align_up(M * Ea * 2 * pf, 1024);
-  const size_t big_h = align_up(M * F * 2 * pf, 1024);
-  const size_t big = big_qkv_ctx > big_h ? big_qkv_ctx : big_h;    // h aliases qkv+ctx
-  return a + big + attn_scratch_bytes(B, T, H) + 1024;
+  return workspace_layout(nullptr, E, H, F, B, T, precision).bytes;
 }
-
-namespace {
-struct Workspace {
-  __half* xn;
-  __half* qkv;
-  __half* ctx;
-  __half* h;
-  AttnScratch as;
-};
-
-int carve_workspace(Workspace* ws, void* workspace, size_t bytes, int E, int H, int F, int B, int T, int split) {
-  if (bytes < esmb200_workspace_bytes(E, H, F, B, T, split)) return fail(ESMB200_EWORKSPACE, "workspace too small");
-  const size_t M = (size_t)B * T, Ea = (size_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;
-  uint8_t* p = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024));
-  ws->xn = reinterpret_cast<__half*>(p);
-  p += align_up(M * E * 2 * pf, 1024);
-  ws->qkv = reinterpret_cast<__half*>(p);
-  ws->h = reinterpret_cast<__half*>(p);
-  ws->ctx = reinterpret_cast<__half*>(p + align_up(M * 3 * Ea * 2 * pf, 1024));
-  const size_t big_qkv_ctx = align_up(M * 3 * Ea * 2 * pf, 1024) + align_up(M * Ea * 2 * pf, 1024);
-  const size_t big_h = align_up(M * F * 2 * pf, 1024);
-  p += big_qkv_ctx > big_h ? big_qkv_ctx : big_h;
-  ws->as = carve_attn_scratch(p, B, T, H);
-  return ESMB200_OK;
-}
-
-struct ActMaps {
-  CUtensorMap xn, ctx, h;       // A operands (fp16, box {64,128})
-  CUtensorMap qkv_o, h_o, x_o;  // GEMM outputs: qkv and h (fp16), the fp32 residual stream x
-};
-
-int layer_forward_impl(esmb200_layer* L, float* x, int B, int T, const float* rope_cos, const float* rope_sin,
-                       float* attn_probs, long long attn_batch_stride, int attn_flags, const Workspace& ws,
-                       const ActMaps& am, cudaStream_t st, const ContactLayer* contact = nullptr) {
-  const int E = L->E, F = L->F, H = L->H, Ea = L->Ea;
-  const int M = B * T;
-  const bool split = L->split != 0;
-  cudaError_t e = cudaSuccess;
-  // LN1 -> fp16 (modules.py:124)
-  {
-    ProfScope ps(T_LN1, st);
-    e = split ? launch_layernorm<2>(x, L->ln1_w, L->ln1_b, ws.xn, M, E, L->eps, st)
-              : launch_layernorm<1>(x, L->ln1_w, L->ln1_b, ws.xn, M, E, L->eps, st);
-  }
-  if (e != cudaSuccess) return fail_cuda(e, "layernorm1");
-  // q,k,v projections + bias + q scale + RoPE (multihead_attention.py:258-261,354-355)
-  GemmParams g;
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = 3 * Ea; g.K = E; g.bias = L->b_qkv;
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = Ea; g.q_scale = L->q_scale;
-  g.lo_col_off = 3 * Ea;
-  g.rope_ld = 32 * L->slots;
-  int rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV, split);
-  if (rc) return rc;
-  // attention (multihead_attention.py:357-394)
-  rc = run_attention(ws.qkv, ws.ctx, attn_probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split, contact,
-                     L->slots);
-  if (rc) return rc;
-  // out_proj + residual (multihead_attention.py:395, modules.py:134)
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = E; g.K = Ea; g.bias = L->out_b;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT, split);
-  if (rc) return rc;
-  // LN2 -> fp16 (modules.py:137)
-  {
-    ProfScope ps(T_LN2, st);
-    e = split ? launch_layernorm<2>(x, L->ln2_w, L->ln2_b, ws.xn, M, E, L->eps, st)
-              : launch_layernorm<1>(x, L->ln2_w, L->ln2_b, ws.xn, M, E, L->eps, st);
-  }
-  if (e != cudaSuccess) return fail_cuda(e, "layernorm2");
-  // fc1 + GELU (modules.py:138)
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b; g.lo_col_off = F;
-  rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1, split);
-  if (rc) return rc;
-  // fc2 + residual (modules.py:139-140)
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b;
-  rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, g, st, T_FC2, split);
-  return rc;
-}
-
-int make_act_maps(ActMaps* am, const Workspace& ws, float* x, int E, int H, int F, int M, int split = 0) {
-  const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;  // fp32x3: activations are [rows, 2 * width]
-  int rc = make_tmap_f16(&am->xn, ws.xn, M, pf * E, pf * E, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&am->ctx, ws.ctx, M, pf * Ea, pf * Ea, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&am->h, ws.h, M, pf * F, pf * F, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_gemm_out_map(&am->qkv_o, ws.qkv, 2, M, pf * 3 * Ea);
-  if (!rc) rc = make_gemm_out_map(&am->h_o, ws.h, 2, M, pf * F);
-  if (!rc) rc = make_gemm_out_map(&am->x_o, x, 4, M, E);
-  return rc;
-}
-}  // namespace
 
 int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
                           int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
@@ -596,9 +656,8 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
     if (layers[i]->E != E || layers[i]->F != F || layers[i]->H != H || layers[i]->split != layers[0]->split)
       return fail(ESMB200_EINVAL, "layers of one stack must share E, H, F and precision");
   const int split = layers[0]->split;
-  Workspace ws;
-  rc = carve_workspace(&ws, workspace, workspace_bytes, E, H, F, B, T, split);
-  if (rc) return rc;
+  const Workspace ws = workspace_layout(workspace, E, H, F, B, T, split);
+  if (workspace_bytes < ws.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   ActMaps am;
   rc = make_act_maps(&am, ws, x, E, H, F, B * T, split);
   if (rc) return rc;
@@ -606,6 +665,7 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
   if (rc) return rc;
   const int nt128 = (T + 127) / 128;
   for (int i = 0; i < n_layers; ++i) {
+    esmb200_layer* L = layers[i];
     ContactLayer cl;
     if (contact) {
       const int S = contact->hi - contact->lo;
@@ -614,8 +674,12 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
       cl.row_part = contact->row_part + (size_t)i * 4 * part; cl.col_part = contact->col_part + (size_t)i * 4 * part;
       cl.lo = contact->lo; cl.S = S;
     }
-    rc = layer_forward_impl(layers[i], x, B, T, rope_cos, rope_sin, attn_out ? attn_out[i] : nullptr, attn_batch_stride,
-                            attn_flags, ws, am, st, contact ? &cl : nullptr);
+    float* probs = attn_out ? attn_out[i] : nullptr;
+    rc = attention_block(L, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
+      return run_attention(ws.qkv, ws.ctx, probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split != 0,
+                           contact ? &cl : nullptr, L->slots);  // multihead_attention.py:357-394
+    });
+    if (!rc) rc = ffn_block(L, x, B * T, ws, am, st);
     if (rc) return rc;
     if (repr_out && repr_out[i])
       CK(cudaMemcpyAsync(repr_out[i], x, (size_t)B * T * E * 4, cudaMemcpyDeviceToDevice, st));
@@ -659,92 +723,37 @@ int esmb200_layernorm(const float* x, const float* weight, const float* bias, fl
 int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias, void* out, int32_t M, int32_t E,
                           float eps, void* stream) {
   if (!x || !weight || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
-  ProfScope ps(T_LN1, static_cast<cudaStream_t>(stream));
-  cudaError_t e = launch_layernorm<1>(x, weight, bias, out, M, E, eps, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail_cuda(e, "layernorm_f16");
-  return ESMB200_OK;
+  return layernorm_f16(x, weight, bias, out, M, E, eps, false, T_LN1, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_gemm_f16(int32_t epilogue, const void* a, const void* w, const float* bias, void* out, int32_t M,
                      int32_t N, int32_t K, const float* rope_cos, const float* rope_sin, int32_t T, int32_t E,
                      void* stream) {
-  if (!a || !w || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
-  const bool f16_out = (epilogue == EPI_QKV_ROPE || epilogue == EPI_BIAS_GELU);
-  if (M <= 0 || N <= 0 || K <= 0 || K % 8 != 0 || N % (f16_out ? 64 : 32) != 0)
-    return fail(ESMB200_EINVAL, "gemm needs K % 8 == 0 and N % 64 == 0 (fp16 output) / N % 32 == 0 (fp32 output)");
-  int rc = check_device();
-  if (rc) return rc;
-  if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
-    return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb, to;
-  rc = make_tmap_f16(&ta, a, M, K, K, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&tb, w, N, K, K, gemm2_cfg::HALF_N);
-  if (!rc) rc = make_gemm_out_map(&to, out, f16_out ? 2 : 4, M, N);
-  if (rc) return rc;
-  GemmParams g;
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = N; g.K = K; g.bias = bias;
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, to, g, static_cast<cudaStream_t>(stream));
+  return gemm_epilogue_entry(epilogue, a, w, bias, out, M, N, K, rope_cos, rope_sin, T, E, false, stream);
 }
 
 // ---- fp32x3 precision building blocks (hi | lo fp16 operands): used by the LM head and the kernel-level parity tests
 int esmb200_layernorm_split(const float* x, const float* weight, const float* bias, void* out, int32_t M, int32_t E,
                             float eps, void* stream) {
   if (!x || !weight || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
-  ProfScope ps(T_LN1, static_cast<cudaStream_t>(stream));
-  cudaError_t e = launch_layernorm<2>(x, weight, bias, out, M, E, eps, static_cast<cudaStream_t>(stream));
-  if (e != cudaSuccess) return fail_cuda(e, "layernorm_split");
-  return ESMB200_OK;
+  return layernorm_f16(x, weight, bias, out, M, E, eps, true, T_LN1, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_convert_split(const float* src, void* dst, int64_t rows, int32_t K, void* stream) {
   if (!src || !dst) return fail(ESMB200_EINVAL, "null argument");
   if (rows <= 0 || K <= 0) return ESMB200_OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  size_t blocks = ((size_t)rows * K + 255) / 256;
-  if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
-  ProfScope ps(T_CONVERT, st);
-  convert_f32_split_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, static_cast<__half*>(dst), (size_t)rows, K);
-  CK(cudaGetLastError());
-  return ESMB200_OK;
+  return convert_f16(src, dst, (size_t)rows, K, true, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_gemm_split(int32_t epilogue, const void* a, const void* w, const float* bias, void* out, int32_t M,
                        int32_t N, int32_t K, const float* rope_cos, const float* rope_sin, int32_t T, int32_t E,
                        void* stream) {
-  if (!a || !w || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
-  const bool f16_out = (epilogue == EPI_QKV_ROPE || epilogue == EPI_BIAS_GELU);
-  if (M <= 0 || N <= 0 || K <= 0 || K % 64 != 0 || N % (f16_out ? 64 : 32) != 0)
-    return fail(ESMB200_EINVAL, "split gemm needs K % 64 == 0 and N % 64 == 0 (fp16 output) / N % 32 == 0 (fp32 output)");
-  if (epilogue < 0 || epilogue > EPI_BIAS_GELU_F32) return fail(ESMB200_EINVAL, "unknown GEMM epilogue");
-  int rc = check_device();
-  if (rc) return rc;
-  if (epilogue == EPI_QKV_ROPE && (!rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
-    return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E");
-  CUtensorMap ta, tb, to;
-  rc = make_tmap_f16(&ta, a, M, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&tb, w, N, 2 * (uint64_t)K, 2 * (uint64_t)K, gemm2_cfg::HALF_N);
-  if (!rc) rc = f16_out ? make_gemm_out_map(&to, out, 2, M, 2 * (uint64_t)N) : make_gemm_out_map(&to, out, 4, M, N);
-  if (rc) return rc;
-  GemmParams g;
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = N; g.K = K; g.bias = bias; g.lo_col_off = N;
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
-  return launch_gemm(epilogue, ta, tb, to, g, static_cast<cudaStream_t>(stream), T_GEMM_OTHER, true);
+  return gemm_epilogue_entry(epilogue, a, w, bias, out, M, N, K, rope_cos, rope_sin, T, E, true, stream);
 }
 
 int esmb200_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                             int32_t H, void* scratch, void* stream) {
-  if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
-  if (B <= 0 || T <= 0 || H <= 0 || H > 64) return fail(ESMB200_EINVAL, "bad shape");
-  int rc = check_device();
-  if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  AttnScratch s = carve_attn_scratch(scratch, B, T, H);
-  rc = run_key_bits(pad_mask, s, B, T, st);
-  if (rc) return rc;
-  return run_attention(qkv, ctx, attn_probs, 0, 0, s, B, T, H, st, true);
+  return attention_entry(qkv, pad_mask, ctx, attn_probs, B, T, H, scratch, stream, true, 1);
 }
 
 int esmb200_gemm_qkv_f16(const void* a, const void* w, const float* bias, void* out, int32_t M, int32_t E, float q_scale,
@@ -755,42 +764,18 @@ int esmb200_gemm_qkv_f16(const void* a, const void* w, const float* bias, void* 
     return fail(ESMB200_EINVAL, "rope tables must be given together with T, or not at all");
   int rc = check_device();
   if (rc) return rc;
-  CUtensorMap ta, tb, to;
-  rc = make_tmap_f16(&ta, a, M, E, E, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&tb, w, 3 * (uint64_t)E, E, E, gemm2_cfg::HALF_N);
-  if (!rc) rc = make_gemm_out_map(&to, out, 2, M, 3 * (uint64_t)E);
-  if (rc) return rc;
-  GemmParams g;
-  memset(&g, 0, sizeof g);
-  g.M = M; g.N = 3 * E; g.K = E; g.bias = bias;
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T > 0 ? T : 1; g.E = E; g.q_scale = q_scale;
-  return launch_gemm(EPI_QKV_ROPE, ta, tb, to, g, static_cast<cudaStream_t>(stream));
+  return run_gemm(EPI_QKV_ROPE, a, w, bias, out, M, 3 * E, E, rope_cos, rope_sin, T > 0 ? T : 1, E, q_scale, false,
+                  stream);
 }
 
 int esmb200_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                       int32_t H, void* scratch, void* stream) {
-  if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
-  if (B <= 0 || T <= 0 || H <= 0 || H > 64) return fail(ESMB200_EINVAL, "bad shape");
-  int rc = check_device();
-  if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  AttnScratch s = carve_attn_scratch(scratch, B, T, H);
-  rc = run_key_bits(pad_mask, s, B, T, st);
-  if (rc) return rc;
-  return run_attention(qkv, ctx, attn_probs, 0, 0, s, B, T, H, st);
+  return attention_entry(qkv, pad_mask, ctx, attn_probs, B, T, H, scratch, stream, false, 1);
 }
 
 int esmb200_attention128(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                          int32_t H, void* scratch, void* stream) {
-  if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
-  if (B <= 0 || T <= 0 || H <= 0 || H > 64) return fail(ESMB200_EINVAL, "bad shape");
-  int rc = check_device();
-  if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  AttnScratch s = carve_attn_scratch(scratch, B, T, H);
-  rc = run_key_bits(pad_mask, s, B, T, st);
-  if (rc) return rc;
-  return run_attention(qkv, ctx, attn_probs, 0, 0, s, B, T, H, st, false, nullptr, 2);
+  return attention_entry(qkv, pad_mask, ctx, attn_probs, B, T, H, scratch, stream, false, 2);
 }
 
 // ---- MSA axial attention (esm/axial_attention.py) -----------------------------------------------------------------
@@ -859,33 +844,14 @@ int esmb200_column_attention(const void* qkv, const uint8_t* pad_mask, void* ctx
   int rc = check_device();
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int E = H * 64;
-  const int S = B * C;  // one "sequence" of R tokens per alignment column
-  AttnScratch s = carve_attn_scratch(scratch, S, R, H);
-  rc = run_key_bits(pad_mask, s, S, R, st);
+  const AttnScratch s = attn_scratch_layout(reinterpret_cast<uintptr_t>(scratch), B * C, R, H);
+  rc = run_key_bits(pad_mask, s, B * C, R, st);
   if (rc) return rc;
-  CUtensorMap tq, tkv;
-  const uint64_t wide = (uint64_t)C * 3 * E;  // qkv viewed as [B*R, C*3E]: token r of column c at row r, x = c*3E
-  if ((rc = make_tmap_f16(&tq, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_Q))) return rc;
-  if ((rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_KV))) return rc;
-  AttnParams ap;
-  ap.B = S; ap.T = R; ap.H = H; ap.E = E;
-  ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
-  ap.ctx = static_cast<__half*>(ctx);
-  ap.row_max = nullptr; ap.row_sum = nullptr;
-  ap.cols = C;
-  cudaError_t e;
-  {
-    ProfScope ps(T_ATTN, st);
-    e = launch_attention_fwd(tq, tkv, ap, st);
-  }
-  if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
-  return ESMB200_OK;
+  return run_column_attention(qkv, ctx, s, B, R, C, H, st);
 }
 
-
 size_t esmb200_axial_workspace_bytes(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C) {
-  return esmb200_workspace_bytes(E, E / 64, F, B * C, R, 0) + esmb200_tied_row_attention_scratch_bytes(B, C, E / 64) + 1024;
+  return axial_workspace_layout(nullptr, E, F, B, R, C).bytes;
 }
 
 // (A CUDA-graph replay of this launch sequence was measured: 20.70 vs 20.77 ms per 128 x 512 MSA — the ~2 ms between the
@@ -905,102 +871,44 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   const int E = col_layers[0]->E, F = col_layers[0]->F, H = col_layers[0]->H;
   if (F <= 0) return fail(ESMB200_EINVAL, "col_layers carry the feed-forward weights");
   for (int i = 0; i < n_layers; ++i)
-    if (row_layers[i]->E != E || col_layers[i]->E != E || col_layers[i]->F != F)
-      return fail(ESMB200_EINVAL, "layers of one stack must share E and F");
-  if (workspace_bytes < esmb200_axial_workspace_bytes(E, F, B, R, C))
-    return fail(ESMB200_EWORKSPACE, "workspace too small");
-  const int M = B * R * C;
-  Workspace ws;
+    if (row_layers[i]->E != E || col_layers[i]->E != E || col_layers[i]->F != F || row_layers[i]->H != H ||
+        col_layers[i]->H != H)
+      return fail(ESMB200_EINVAL, "layers of one stack must share E, H and F");
+  const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C);
+  if (workspace_bytes < aw.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   if (E != 64 * H) return fail(ESMB200_EINVAL, "the MSA axial path needs head_dim 64");
   for (int i = 0; i < n_layers; ++i)
     if (row_layers[i]->split || col_layers[i]->split)
       return fail(ESMB200_EINVAL, "the MSA axial path runs with fp16 operands only (precision 0)");
-  const size_t base_bytes = esmb200_workspace_bytes(E, H, F, B * C, R, 0);
-  rc = carve_workspace(&ws, workspace, base_bytes, E, H, F, B * C, R, 0);
-  if (rc) return rc;
-  uint8_t* tied_scratch = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace), 1024)) + base_bytes;
-  const size_t tied_bytes = esmb200_tied_row_attention_scratch_bytes(B, C, H);
+  const int M = B * R * C;
+  const Workspace& ws = aw.ws;
   ActMaps am;
   rc = make_act_maps(&am, ws, x, E, H, F, M);
   if (rc) return rc;
   rc = run_key_bits(col_pad_mask, ws.as, B * C, R, st);  // column attention: B*C sequences of R keys
   if (rc) return rc;
-  CUtensorMap tcq, tckv;
-  const uint64_t wide = (uint64_t)C * 3 * E;
-  if ((rc = make_tmap_f16(&tcq, ws.qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_Q))) return rc;
-  if ((rc = make_tmap_f16(&tckv, ws.qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_KV))) return rc;
   const float row_scale = 0.125f / sqrtf((float)R);  // axial_attention.py:36-38
-  cudaError_t e;
-  GemmParams g;
   for (int i = 0; i < n_layers; ++i) {
-    // ---------------- tied row attention (modules.py:202-207; axial_attention.py:71-130) ----------------
-    esmb200_layer* L = row_layers[i];
-    {
-      ProfScope ps(T_LN1, st);
-      e = launch_layernorm<1>(x, L->ln1_w, L->ln1_b, ws.xn, M, E, L->eps, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "row layernorm");
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv;
-    g.T = 1; g.E = E; g.q_scale = row_scale;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV);
-    if (rc) return rc;
-    if (pad_mask) {
-      ProfScope ps(T_KEYBITS, st);
-      zero_q_at_pads_kernel<<<(M + 7) / 8, 256, 0, st>>>(ws.qkv, pad_mask, M, E);
-      CK(cudaGetLastError());
-    }
-    rc = tied_row_impl(ws.qkv, pad_mask, (long long)R * C, ws.ctx, row_attn_out ? row_attn_out[i] : nullptr, B, R, C, H,
-                       tied_scratch, tied_bytes, stream);
-    if (rc) return rc;
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = E; g.bias = L->out_b;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT);
-    if (rc) return rc;
-    // ---------------- column attention (modules.py:208-212; axial_attention.py:182-239) ----------------
-    L = col_layers[i];
-    {
-      ProfScope ps(T_LN1, st);
-      e = launch_layernorm<1>(x, L->ln1_w, L->ln1_b, ws.xn, M, E, L->eps, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "column layernorm");
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = 3 * E; g.K = E; g.bias = L->b_qkv;
-    g.T = 1; g.E = E; g.q_scale = 0.125f;
-    rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV);
-    if (rc) return rc;
-    {
-      AttnParams ap;
-      ap.B = B * C; ap.T = R; ap.H = H; ap.E = E;
-      ap.keybits = ws.as.keybits; ap.kvlen = ws.as.kvlen; ap.words = ws.as.words;
-      ap.ctx = ws.ctx; ap.row_max = nullptr; ap.row_sum = nullptr; ap.cols = C;
-      ProfScope ps(T_ATTN, st);
-      e = launch_attention_fwd(tcq, tckv, ap, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = E; g.bias = L->out_b;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, g, st, T_OUT);
-    if (rc) return rc;
-    // ---------------- feed-forward (modules.py:213-214, 413-418) ----------------
-    {
-      ProfScope ps(T_LN2, st);
-      e = launch_layernorm<1>(x, L->ln2_w, L->ln2_b, ws.xn, M, E, L->eps, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "ffn layernorm");
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = F; g.K = E; g.bias = L->fc1_b;
-    rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1);
-    if (rc) return rc;
-    memset(&g, 0, sizeof g);
-    g.M = M; g.N = E; g.K = F; g.bias = L->fc2_b;
-    rc = launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, g, st, T_FC2);
+    // tied row attention (modules.py:202-207; axial_attention.py:71-130)
+    rc = attention_block(row_layers[i], x, M, 1, nullptr, nullptr, row_scale, ws, am, st, [&]() -> int {
+      if (pad_mask) {
+        ProfScope ps(T_KEYBITS, st);
+        zero_q_at_pads_kernel<<<(M + 7) / 8, 256, 0, st>>>(ws.qkv, pad_mask, M, E);
+        CK(cudaGetLastError());
+      }
+      return tied_row_impl(ws.qkv, pad_mask, (long long)R * C, ws.ctx, row_attn_out ? row_attn_out[i] : nullptr, B, R,
+                           C, H, aw.tied, aw.tied_bytes, stream);
+    });
+    // column attention (modules.py:208-212; axial_attention.py:182-239)
+    if (!rc)
+      rc = attention_block(col_layers[i], x, M, 1, nullptr, nullptr, col_layers[i]->q_scale, ws, am, st,
+                           [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st); });
+    // feed-forward (modules.py:213-214)
+    if (!rc) rc = ffn_block(col_layers[i], x, M, ws, am, st);
     if (rc) return rc;
   }
   return ESMB200_OK;
 }
-
-
 
 int esmb200_msa_embed(const int64_t* tokens, const float* embed_table, const float* pos_table, const float* msa_pos,
                       int32_t msa_pos_dim, const float* ln_weight, const float* ln_bias, float eps, float* x,

@@ -338,29 +338,20 @@ class RobertaLMHead(nn.Module):
         M = B * T
         dev = x_pre.device
         w_dense, w_out, b_out, V, npad, b_dense, ln2_w, ln2_b = self._pack()
-        if precision:
-            wd, wo = self._pack_split()
-            a16 = torch.empty((M, 2 * E), dtype=torch.float16, device=dev)
-            _lib.check(lib.esmb200_layernorm_split(_ptr(x_pre), _ptr(ln_w), _ptr(ln_b), _ptr(a16), M, E, eps, _stream()))
-            h = torch.empty((M, E), dtype=torch.float32, device=dev)
-            _lib.check(lib.esmb200_gemm_split(_lib.EPI_BIAS_GELU_F32, _ptr(a16), _ptr(wd), _ptr(b_dense), _ptr(h), M, E, E,
-                                              None, None, 0, 0, _stream()))
-            _lib.check(lib.esmb200_layernorm_split(_ptr(h), _ptr(ln2_w), _ptr(ln2_b), _ptr(a16), M, E,
-                                                   self.layer_norm.eps, _stream()))
-            logits = torch.empty((M, npad), dtype=torch.float32, device=dev)
-            _lib.check(lib.esmb200_gemm_split(_lib.EPI_BIAS_F32, _ptr(a16), _ptr(wo), _ptr(b_out), _ptr(logits), M, npad, E,
-                                              None, None, 0, 0, _stream()))
-            return logits.view(B, T, npad)[:, :, :V].contiguous()
-        a16 = torch.empty((M, E), dtype=torch.float16, device=dev)
-        _lib.check(lib.esmb200_layernorm_f16(_ptr(x_pre), _ptr(ln_w), _ptr(ln_b), _ptr(a16), M, E, eps, _stream()))
+        if precision:  # fp32x3: the GEMM operands are fp16 hi | lo halves along K
+            w_dense, w_out = self._pack_split()
+            layernorm, gemm, width = lib.esmb200_layernorm_split, lib.esmb200_gemm_split, 2 * E
+        else:
+            layernorm, gemm, width = lib.esmb200_layernorm_f16, lib.esmb200_gemm_f16, E
+        a16 = torch.empty((M, width), dtype=torch.float16, device=dev)
+        _lib.check(layernorm(_ptr(x_pre), _ptr(ln_w), _ptr(ln_b), _ptr(a16), M, E, eps, _stream()))
         h = torch.empty((M, E), dtype=torch.float32, device=dev)
-        _lib.check(lib.esmb200_gemm_f16(_lib.EPI_BIAS_GELU_F32, _ptr(a16), _ptr(w_dense), _ptr(b_dense),
-                                        _ptr(h), M, E, E, None, None, 0, 0, _stream()))
-        _lib.check(lib.esmb200_layernorm_f16(_ptr(h), _ptr(ln2_w), _ptr(ln2_b),
-                                             _ptr(a16), M, E, self.layer_norm.eps, _stream()))
+        _lib.check(gemm(_lib.EPI_BIAS_GELU_F32, _ptr(a16), _ptr(w_dense), _ptr(b_dense), _ptr(h), M, E, E,
+                        None, None, 0, 0, _stream()))
+        _lib.check(layernorm(_ptr(h), _ptr(ln2_w), _ptr(ln2_b), _ptr(a16), M, E, self.layer_norm.eps, _stream()))
         logits = torch.empty((M, npad), dtype=torch.float32, device=dev)
-        _lib.check(lib.esmb200_gemm_f16(_lib.EPI_BIAS_F32, _ptr(a16), _ptr(w_out), _ptr(b_out), _ptr(logits), M, npad, E,
-                                        None, None, 0, 0, _stream()))
+        _lib.check(gemm(_lib.EPI_BIAS_F32, _ptr(a16), _ptr(w_out), _ptr(b_out), _ptr(logits), M, npad, E,
+                        None, None, 0, 0, _stream()))
         return logits.view(B, T, npad)[:, :, :V].contiguous()  # [B,T,V] packed like the reference's (esm2.py:129)
 
 

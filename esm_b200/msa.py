@@ -11,7 +11,7 @@ CUDA path for BASELINE.json configs[4] (SURVEY §8f #3).  All the arithmetic of 
     a row softmax (with the reference's -10000 fill on padded key columns), and the P.V update with V tiles as the
     MN-major operand (csrc/tied_attention.cuh);
   * column attention: esmb200_column_attention — the flash-attention kernel with strided TMA boxes, one "sequence" of
-    R rows per alignment column, no regrouping copy (csrc/attention4.cuh, AttnParams::cols).
+    R rows per alignment column, no regrouping copy (csrc/attention8.cuh, AttnParams::cols).
 PyTorch is used for the buffers, for zeroing q at padded positions (axial_attention.py:82-85, one masked_fill_) and, only
 when the column attention MAPS are requested, for regrouping qkv column-major.
 
@@ -221,7 +221,7 @@ class AxialTransformerLayer(nn.Module):
                                                 (d ** -0.5) / math.sqrt(R), None, None, 0, _stream()))
             if padding_mask is not None:  # q zeroed at padded positions (:82-85)
                 qkv.view(B, R, C, 3, E)[:, :, :, 0].masked_fill_(pm[..., None], 0)
-            row_probs = torch.empty((H, B, C, C), dtype=torch.float32, device=dev) if need_probs else None
+            row_probs = torch.empty((H, B, C, C), dtype=torch.float32, device=dev)
             nbytes = lib.esmb200_tied_row_attention_scratch_bytes(B, C, H)
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             _lib.check(lib.esmb200_tied_row_attention(_ptr(qkv), _ptr(key_pad), _ptr(ctx), _ptr(row_probs), B, R, C, H,
@@ -235,17 +235,13 @@ class AxialTransformerLayer(nn.Module):
             _lib.check(lib.esmb200_gemm_qkv_f16(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, d ** -0.5, None, None, 0,
                                                 _stream()))
             scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B * C, R), dtype=torch.uint8, device=dev)
-            col_probs = None
-            if not need_probs:  # q/k/v tiles are fetched straight from the row-major qkv (strided TMA boxes)
-                _lib.check(lib.esmb200_column_attention(_ptr(qkv), _ptr(col_pad), _ptr(ctx), B, R, C, H, _ptr(scratch),
-                                                        _stream()))
-            else:               # probabilities requested: regroup column-major and use the probs-writing path
-                qkv_t = qkv.view(B, R, C, 3 * E).permute(0, 2, 1, 3).contiguous()                  # [B*C, R, 3E]
-                ctx_t = torch.empty((B * C * R, E), dtype=torch.float16, device=dev)
-                col_probs = torch.empty((B * C, H, R, R), dtype=torch.float32, device=dev)
-                _lib.check(lib.esmb200_attention(_ptr(qkv_t), _ptr(col_pad), _ptr(ctx_t), _ptr(col_probs), B * C, R, H,
-                                                 _ptr(scratch), _stream()))
-                ctx.view(B, R, C, E).copy_(ctx_t.view(B, C, R, E).permute(0, 2, 1, 3))
+            # the maps are wanted: regroup qkv column-major and use the probability-writing path
+            qkv_t = qkv.view(B, R, C, 3 * E).permute(0, 2, 1, 3).contiguous()                      # [B*C, R, 3E]
+            ctx_t = torch.empty((B * C * R, E), dtype=torch.float16, device=dev)
+            col_probs = torch.empty((B * C, H, R, R), dtype=torch.float32, device=dev)
+            _lib.check(lib.esmb200_attention(_ptr(qkv_t), _ptr(col_pad), _ptr(ctx_t), _ptr(col_probs), B * C, R, H,
+                                             _ptr(scratch), _stream()))
+            ctx.view(B, R, C, E).copy_(ctx_t.view(B, C, R, E).permute(0, 2, 1, 3))
             _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["col_out"], blk.layer.out_proj.bias, x2)
 
             # ================= feed-forward (modules.py:413-418) =================
@@ -254,9 +250,8 @@ class AxialTransformerLayer(nn.Module):
             hbuf = torch.empty((M, Fd), dtype=torch.float16, device=dev)
             _gemm(_lib.EPI_BIAS_GELU, xn, pk["fc1"], blk.layer.fc1.bias, hbuf)
             _gemm(_lib.EPI_BIAS_RESIDUAL, hbuf, pk["fc2"], blk.layer.fc2.bias, x2)
-        if need_probs:
-            # reference shapes: column_attn [H, C, B, R, R] (axial_attention.py:206), row_attn [H, B, C, C] (:87)
-            col_probs = col_probs.view(B, C, H, R, R).permute(2, 1, 0, 3, 4).contiguous()
+        # reference shapes: column_attn [H, C, B, R, R] (axial_attention.py:206), row_attn [H, B, C, C] (:87)
+        col_probs = col_probs.view(B, C, H, R, R).permute(2, 1, 0, 3, 4).contiguous()
         return row_probs, col_probs
 
 

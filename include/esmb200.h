@@ -17,7 +17,8 @@
  *     scripts/fold.py:165-178's handler keeps working
  *   - activations: residual stream x is fp32 [B, T, E] row-major (batch-major, i.e. the reference's (T,B,E)
  *     transposed); MMA operands are fp16 with fp32 accumulation; LayerNorm / softmax / residual adds are fp32
- *   - head_dim <= 64 (every esm.pretrained.esm2_* model except the 15B one, whose heads are 128 wide); no CPU fallback
+ *   - even head_dim <= 128 (every esm.pretrained.esm2_* model; heads narrower than 64 run in zero-padded 64-wide
+ *     slots, 128-wide heads in two); no CPU fallback
  */
 #ifndef ESMB200_H_
 #define ESMB200_H_
@@ -141,7 +142,8 @@ int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
- * 2 gelu -> fp16, 3 fp32, 4 gelu -> fp32. rope_* / T / E only for epilogue 0. K % 64 == 0, N % 64 == 0. */
+ * 2 gelu -> fp16, 3 fp32, 4 gelu -> fp32. rope_* / T / E only for epilogue 0. K % 8 == 0; N % 64 == 0 for an fp16
+ * output (epilogues 0, 2), N % 32 == 0 for an fp32 one. */
 int esmb200_gemm_f16(int32_t epilogue, const void* a_f16, const void* w_f16, const float* bias, void* out, int32_t M,
                      int32_t N, int32_t K, const float* rope_cos, const float* rope_sin, int32_t T, int32_t E,
                      void* stream);

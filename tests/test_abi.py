@@ -39,6 +39,27 @@ def test_workspace_size_is_pure_host_arithmetic():
     assert lib.esmb200_workspace_bytes(1280, 20, 5120, 256, 1024, 1) >= 2 * 256 * 1024 * (1280 * 2 + 5120 * 2)  # fp32x3
 
 
+@pytest.mark.parametrize("fn,args,nbytes", [
+    ("esmb200_workspace_bytes", (1280, 20, 5120, 256, 1024, 0), 3397421056),
+    ("esmb200_workspace_bytes", (1280, 20, 5120, 256, 1024, 1), 6752864256),
+    ("esmb200_workspace_bytes", (320, 20, 1280, 3, 1003, 0), 33222912),       # head_dim 16, odd T
+    ("esmb200_workspace_bytes", (5120, 40, 20480, 16, 1024, 0), 844107008),   # head_dim 128: two slots per head
+    ("esmb200_workspace_bytes", (2560, 40, 10240, 16, 512, 0), 212338944),
+    ("esmb200_workspace_bytes", (640, 20, 2560, 5, 77, 1), 8934400),
+    ("esmb200_axial_workspace_bytes", (768, 3072, 1, 128, 512), 528496640),
+    ("esmb200_axial_workspace_bytes", (128, 512, 2, 5, 130), 2165760),
+    ("esmb200_axial_workspace_bytes", (256, 1024, 3, 7, 61), 3603712),
+    ("esmb200_attention_scratch_bytes", (2, 1024), 1049088),
+    ("esmb200_attention_scratch_bytes", (33, 77), 1302016),
+    ("esmb200_tied_row_attention_scratch_bytes", (1, 512, 12), 18876416),
+    ("esmb200_tied_row_attention_scratch_bytes", (2, 130, 4), 943104),
+])
+def test_workspace_layout_is_pinned(fn, args, nbytes):
+    """Exact sizes of every workspace / scratch layout: callers allocate from these, so a layout change shows here."""
+    from esm_b200 import _lib
+    assert getattr(_lib.load(), fn)(*args) == nbytes
+
+
 def test_product_package_never_imports_the_oracle():
     bad = []
     for dirpath, _, files in os.walk(os.path.join(ROOT, "esm_b200")):
