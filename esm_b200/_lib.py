@@ -24,6 +24,7 @@ EXPORTS = (
     "esmb200_layer_forward",
     "esmb200_stack_forward",
     "esmb200_embed_tokens",
+    "esmb200_esm1b_embed",
     "esmb200_layernorm",
     "esmb200_mean_pool",
     "esmb200_gemm_f16",
@@ -119,6 +120,9 @@ def _declare(lib):
     lib.esmb200_embed_tokens.restype = c_int32
     lib.esmb200_embed_tokens.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                          c_int32, c_void_p]
+    lib.esmb200_esm1b_embed.restype = c_int32
+    lib.esmb200_esm1b_embed.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int32, c_int32,
+                                        c_int32, c_void_p, c_int32, c_int32, c_int32, c_void_p]
     lib.esmb200_layernorm.restype = c_int32
     lib.esmb200_layernorm.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_mean_pool.restype = c_int32

@@ -635,8 +635,9 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
                           float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
                           int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
                           size_t workspace_bytes, void* stream) {
-  if (!layers || n_layers <= 0 || !x || !rope_cos || !rope_sin || !workspace)
-    return fail(ESMB200_EINVAL, "null argument");
+  if (!layers || n_layers <= 0 || !x || !workspace) return fail(ESMB200_EINVAL, "null argument");
+  if ((rope_cos == nullptr) != (rope_sin == nullptr))  // both NULL: no rotary embedding (ESM-1b / ESM-1v)
+    return fail(ESMB200_EINVAL, "rope_cos and rope_sin must both be given or both be NULL");
   if (contact) {
     if (!attn_out) return fail(ESMB200_EINVAL, "a contact job needs attn_out for every layer");
     for (int i = 0; i < n_layers; ++i)
@@ -707,6 +708,35 @@ int esmb200_embed_tokens(const int64_t* tokens, const float* table, float* x, in
   if (chunks < 1) chunks = 1;
   embed_tokens_kernel<<<dim3(chunks, B), 256, 0, static_cast<cudaStream_t>(stream)>>>(tokens, table, x, T, E, padding_idx,
                                                                                      mask_idx, token_dropout);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
+int esmb200_esm1b_embed(const int64_t* tokens, const float* embed_table, const float* pos_table, const float* ln_weight,
+                        const float* ln_bias, float eps, int32_t token_dropout, int32_t padding_idx, int32_t mask_idx,
+                        float* x, int32_t B, int32_t T, int32_t E, void* stream) {
+  if (!tokens || !embed_table || !pos_table || !x) return fail(ESMB200_EINVAL, "null argument");
+  if ((ln_weight == nullptr) != (ln_bias == nullptr))
+    return fail(ESMB200_EINVAL, "ln_weight and ln_bias must both be given or both be NULL");
+  if (B <= 0 || B > 65535 || T <= 0 || T > 12288 || E <= 0 || E % 4 != 0 || E > 20 * 128)
+    return fail(ESMB200_EINVAL, "bad shape");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope ps(T_EMBED, st);
+  int chunks = (8 * num_sms() + B - 1) / B;  // >= 8 blocks per SM over the batch, at least 8 rows (one per warp) per block
+  if (chunks > (T + 7) / 8) chunks = (T + 7) / 8;
+  if (chunks < 1) chunks = 1;
+  const int rows = (T + chunks - 1) / chunks;
+  const dim3 grid(chunks, B);
+  const size_t smem = (size_t)rows * sizeof(int);
+  if (E <= 4 * 128)
+    esm1b_embed_kernel<4><<<grid, 256, smem, st>>>(tokens, embed_table, pos_table, ln_weight, ln_bias, eps, token_dropout,
+                                                    padding_idx, mask_idx, x, T, E);
+  else if (E <= 10 * 128)
+    esm1b_embed_kernel<10><<<grid, 256, smem, st>>>(tokens, embed_table, pos_table, ln_weight, ln_bias, eps, token_dropout,
+                                                     padding_idx, mask_idx, x, T, E);
+  else
+    esm1b_embed_kernel<20><<<grid, 256, smem, st>>>(tokens, embed_table, pos_table, ln_weight, ln_bias, eps, token_dropout,
+                                                     padding_idx, mask_idx, x, T, E);
   CK(cudaGetLastError());
   return ESMB200_OK;
 }

@@ -4,6 +4,7 @@
 //                     one warp per row, the row held in registers (single HBM read), fp16 or fp32 output
 //   embed_tokens      esm/model/esm2.py:84-95 (embedding gather, <mask> zeroing, token-dropout rescale
 //                     0.88/(1-mask_ratio), pad zeroing)
+//   esm1b_embed       esm/model/esm1.py:121-139 (the same, plus learned positions and emb_layer_norm_before)
 //   key_bits          esm/model/esm2.py:82 + multihead_attention.py:368-374 (key padding mask) packed to 1 bit/key
 //   mean_pool         scripts/extract.py:116-119 per-sequence mean representation
 //   convert_f32_f16   weight packing (fp32 nn.Linear weights -> fp16 MMA operands)
@@ -354,6 +355,117 @@ msa_embed_kernel(const int64_t* __restrict__ tokens, const float* __restrict__ e
         o.w = ((v[i].w - mean) * rstd * g.w + b.w) * keep;
         out[idx] = o;
       }
+    }
+  }
+}
+
+// ESM-1b / ESM-1v embedding prologue (/root/reference/esm/model/esm1.py:121-139) in one pass over the rows:
+//   x = embed_tokens[tok]; token_dropout: <mask> rows zeroed, x = (x * 0.88) / (1 - n_mask / n_nonpad);
+//   x += embed_positions[pos] with pos = cumsum(tok != pad) * (tok != pad) + padding_idx (modules.py:247-248);
+//   x = LayerNorm(x) when emb_layer_norm_before is present (gamma != NULL); x *= (1 - is_pad).
+// grid (row chunks, B), 8 warps: warp 0 walks the sequence up to the end of the block's chunk with 32-token ballots and
+// leaves the chunk's positions in shared memory (any pad pattern, not only trailing pads); with token_dropout every
+// thread also counts <mask> / <pad> over the whole sequence.  Then one warp per row, the row held in registers.
+template <int MAXV>
+__global__ void __launch_bounds__(256)
+esm1b_embed_kernel(const int64_t* __restrict__ tokens, const float* __restrict__ embed_table,
+                   const float* __restrict__ pos_table, const float* __restrict__ gamma,
+                   const float* __restrict__ beta, float eps, int token_dropout, int padding_idx, int mask_idx,
+                   float* __restrict__ x, int T, int E) {
+  extern __shared__ int s_pos[];  // [rows of this chunk]
+  __shared__ int s_cnt[2];
+  const int b = blockIdx.y;
+  const int64_t* tok = tokens + (size_t)b * T;
+  const int rows = (T + gridDim.x - 1) / gridDim.x;
+  const int t0 = blockIdx.x * rows, t1 = min(T, t0 + rows);
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
+  __syncthreads();
+  if (warp == 0) {
+    int base = 0;
+    for (int c0 = 0; c0 < t1; c0 += 32) {
+      const int c = c0 + lane;
+      const bool nonpad = c < T && tok[c] != padding_idx;
+      const uint32_t bits = __ballot_sync(0xffffffffu, nonpad);
+      if (c >= t0 && c < t1)
+        s_pos[c - t0] = nonpad ? base + __popc(bits & (0xffffffffu >> (31 - lane))) + padding_idx : padding_idx;
+      base += __popc(bits);
+    }
+  }
+  if (token_dropout) {
+    int n_mask = 0, n_pad = 0;
+    for (int t = threadIdx.x; t < T; t += blockDim.x) {
+      const int64_t v = tok[t];
+      n_mask += (v == mask_idx);
+      n_pad += (v == padding_idx);
+    }
+    n_mask = __reduce_add_sync(0xffffffffu, n_mask);
+    n_pad = __reduce_add_sync(0xffffffffu, n_pad);
+    if (lane == 0) {
+      atomicAdd(&s_cnt[0], n_mask);
+      atomicAdd(&s_cnt[1], n_pad);
+    }
+  }
+  __syncthreads();
+  // esm1.py:128-131 (python evaluates 1 - 0.15*0.8 in double, the tensor ops run in fp32: multiply first, then divide)
+  const float keep_scale = (float)(1.0 - 0.15 * 0.8);
+  const float denom = 1.0f - (float)s_cnt[0] / (float)(T - s_cnt[1]);
+  const int nvec = E / 4;
+  for (int t = t0 + warp; t < t1; t += blockDim.x / 32) {
+    const int64_t v = tok[t];
+    const bool zero_emb = token_dropout && v == mask_idx;
+    const float4* e4 = reinterpret_cast<const float4*>(embed_table + (size_t)v * E);
+    const float4* p4 = reinterpret_cast<const float4*>(pos_table + (size_t)s_pos[t - t0] * E);
+    float4 r[MAXV];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int idx = lane + i * 32;
+      if (idx < nvec) {
+        float4 e = zero_emb ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldg(e4 + idx);
+        if (token_dropout) {
+          e.x = (e.x * keep_scale) / denom;
+          e.y = (e.y * keep_scale) / denom;
+          e.z = (e.z * keep_scale) / denom;
+          e.w = (e.w * keep_scale) / denom;
+        }
+        const float4 p = __ldg(p4 + idx);
+        r[i] = make_float4(e.x + p.x, e.y + p.y, e.z + p.z, e.w + p.w);
+        s += (r[i].x + r[i].y) + (r[i].z + r[i].w);
+      }
+    }
+    const float keep = v == padding_idx ? 0.f : 1.f;
+    float4* out = reinterpret_cast<float4*>(x + ((size_t)b * T + t) * E);
+    if (gamma) {  // emb_layer_norm_before (esm1.py:136-137)
+      const float mean = warp_sum(s) / (float)E;
+      float q = 0.f;
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nvec) {
+          const float a = r[i].x - mean, bb = r[i].y - mean, cc = r[i].z - mean, d = r[i].w - mean;
+          q += (a * a + bb * bb) + (cc * cc + d * d);
+        }
+      }
+      const float rstd = rsqrtf(warp_sum(q) / (float)E + eps);
+      const float4* g4 = reinterpret_cast<const float4*>(gamma);
+      const float4* b4 = reinterpret_cast<const float4*>(beta);
+#pragma unroll
+      for (int i = 0; i < MAXV; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nvec) {
+          const float4 g = __ldg(g4 + idx), bt = __ldg(b4 + idx);
+          r[i].x = (r[i].x - mean) * rstd * g.x + bt.x;
+          r[i].y = (r[i].y - mean) * rstd * g.y + bt.y;
+          r[i].z = (r[i].z - mean) * rstd * g.z + bt.z;
+          r[i].w = (r[i].w - mean) * rstd * g.w + bt.w;
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int idx = lane + i * 32;
+      if (idx < nvec) out[idx] = make_float4(r[i].x * keep, r[i].y * keep, r[i].z * keep, r[i].w * keep);
     }
   }
 }

@@ -34,7 +34,9 @@ INCLUDE_CHOICES = ("mean", "per_tok", "bos", "contacts")
 
 def create_parser():
     p = argparse.ArgumentParser(description="Extract per-token representations and model outputs for sequences in a FASTA file")
-    p.add_argument("model_location", type=str, help="ESM-2 model name (esm2_t33_650M_UR50D, ...) or a local .pt file")
+    p.add_argument("model_location", type=str,
+                   help="ESM-2, ESM-1b or ESM-1v model name (esm2_t33_650M_UR50D, esm1b_t33_650M_UR50S, "
+                        "esm1v_t33_650M_UR90S_1, ...) or a local .pt file")
     p.add_argument("fasta_file", type=pathlib.Path)
     p.add_argument("output_dir", type=pathlib.Path)
     p.add_argument("--toks_per_batch", type=int, default=65536, help="maximum batch size in tokens")

@@ -10,11 +10,13 @@ transformer block at run time:
     model, alphabet = esm.pretrained.esm2_t33_650M_UR50D()
     out = model.cuda()(tokens.cuda(), repr_layers=[33])   # the reference's own esm2.py:77-144 loop, H100 kernels inside
 
-Only rotary (ESM-2) layers on CUDA tensors are dispatched — exactly the seam SURVEY §8b names
-(`esm/modules.py:120-142` called from `esm/model/esm2.py:111-116`); ESM-1 layers (learned positions, bias_kv) and CPU
-tensors keep the reference's PyTorch path, like the FusedLayerNorm fallback.  This is the drop-in proof, not the fast
-path: the reference's loop still transposes to (T,B,E) and round-trips through Python between layers, and its
-embedding prologue / LM head / contact head stay PyTorch; `esm_b200.ESM2` runs the whole loop in one C call.
+Layers on CUDA tensors without bias_k are dispatched — exactly the seam SURVEY §8b names (`esm/modules.py:120-142`
+called from `esm/model/esm2.py:111-116` and `esm/model/esm1.py:155-158`): the rotary ESM-2 layers, and the ESM-1b /
+ESM-1v layers of `ProteinBertModel` (learned positions, added by the reference's own prologue; the layer runs without
+rotary tables).  ESM-1 layers (bias_kv attention) and CPU tensors keep the reference's PyTorch path, like the
+FusedLayerNorm fallback.  This is the drop-in proof, not the fast path: the reference's loop still transposes to
+(T,B,E) and round-trips through Python between layers, and its embedding prologue / LM head / contact head stay
+PyTorch; `esm_b200.ESM2` and `esm_b200.ProteinBertModel` run the whole loop in one C call.
 """
 from __future__ import annotations
 
@@ -24,9 +26,12 @@ _ORIGINAL = {}
 
 
 def _dispatchable(layer, x) -> bool:
-    return bool(x.is_cuda and getattr(layer, "use_rotary_embeddings", False)
-                and getattr(layer.self_attn, "bias_k", None) is None
-                and getattr(layer.self_attn, "rot_emb", None) is not None)
+    """CUDA input and no bias_k (ESM-1's extra learned key/value): a rotary ESM-2 layer, or an ESM-1b / ESM-1v layer
+    that has neither rotary embedding nor bias_kv."""
+    if not x.is_cuda or getattr(layer.self_attn, "bias_k", None) is not None:
+        return False
+    rotary = getattr(layer, "use_rotary_embeddings", False)
+    return (getattr(layer.self_attn, "rot_emb", None) is not None) == bool(rotary)
 
 
 def patch_reference(esm_modules=None) -> None:

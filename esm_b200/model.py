@@ -3,6 +3,8 @@
 Mirrors (same names, argument meaning, state-dict keys and result dict):
     esm.modules.TransformerLayer.forward       /root/reference/esm/modules.py:120-142
     esm.model.esm2.ESM2.__init__ / forward     /root/reference/esm/model/esm2.py:15-144
+(ProteinLanguageModel holds ESM2's forward; esm_b200.esm1.ProteinBertModel, ESM-1b / ESM-1v, reuses it with learned
+positions and layers built with use_rotary_embeddings=False.)
 PyTorch owns parameters, activations and the workspace (torch tensors) and provides the CUDA stream; every layer's
 compute goes through the C ABI in include/esmb200.h.  There is no CPU or eager fallback: on a non-CUDA tensor, or
 when libesmb200.so is missing, the forward raises.
@@ -48,7 +50,7 @@ class RotaryEmbedding(nn.Module):
 class MultiheadAttention(nn.Module):
     """Parameter container with the reference's names (multihead_attention.py:109-113,130-132)."""
 
-    def __init__(self, embed_dim: int, num_heads: int):
+    def __init__(self, embed_dim: int, num_heads: int, use_rotary_embeddings: bool = True):
         super().__init__()
         self.embed_dim = embed_dim
         self.num_heads = num_heads
@@ -57,7 +59,8 @@ class MultiheadAttention(nn.Module):
         self.v_proj = nn.Linear(embed_dim, embed_dim)
         self.q_proj = nn.Linear(embed_dim, embed_dim)
         self.out_proj = nn.Linear(embed_dim, embed_dim)
-        self.rot_emb = RotaryEmbedding(self.head_dim)
+        # ESM-1b / ESM-1v layers have no rotary embedding (multihead_attention.py:126-128): no inv_freq key
+        self.rot_emb = RotaryEmbedding(self.head_dim) if use_rotary_embeddings else None
 
 
 def rope_tables(inv_freq: torch.Tensor, seq_len: int):
@@ -149,14 +152,16 @@ class LayerBinding:
 
 
 class TransformerLayer(nn.Module):
-    """Pre-LN transformer block of ESM-2 (modules.py:84-142) executed by libesmb200.so."""
+    """Pre-LN transformer block of ESM-2 (modules.py:84-142) executed by libesmb200.so.  With
+    `use_rotary_embeddings=False` it is the ESM-1b / ESM-1v block (esm1.py:73-79: no bias_kv, ESM1bLayerNorm)."""
 
-    def __init__(self, embed_dim: int, ffn_embed_dim: int, attention_heads: int):
+    def __init__(self, embed_dim: int, ffn_embed_dim: int, attention_heads: int, use_rotary_embeddings: bool = True):
         super().__init__()
         self.embed_dim = embed_dim
         self.ffn_embed_dim = ffn_embed_dim
         self.attention_heads = attention_heads
-        self.self_attn = MultiheadAttention(embed_dim, attention_heads)
+        self.use_rotary_embeddings = use_rotary_embeddings
+        self.self_attn = MultiheadAttention(embed_dim, attention_heads, use_rotary_embeddings)
         self.self_attn_layer_norm = nn.LayerNorm(embed_dim)
         self.fc1 = nn.Linear(embed_dim, ffn_embed_dim)
         self.fc2 = nn.Linear(ffn_embed_dim, embed_dim)
@@ -193,7 +198,8 @@ def layer_forward(binding: LayerBinding, x, self_attn_mask=None, self_attn_paddi
     # tensor it also returns as representations[0] (esm2.py:99-106): contiguous()/float() would hand that storage back.
     xb = torch.empty((B, T, E), dtype=torch.float32, device=x.device)
     xb.copy_(x.transpose(0, 1))
-    cos, sin = rope_tables(binding.module.self_attn.rot_emb.inv_freq, T)
+    rot = getattr(binding.module.self_attn, "rot_emb", None)
+    cos, sin = rope_tables(rot.inv_freq, T) if rot is not None else (None, None)  # ESM-1b layers: no rotation
     attn = run_stack([binding], xb, self_attn_padding_mask, cos, sin, None, [0] if need_head_weights else [])
     out = xb.transpose(0, 1).to(x.dtype)
     if need_head_weights:
@@ -217,9 +223,11 @@ def _workspace(nbytes: int, device: torch.device) -> torch.Tensor:
 
 
 def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Tensor],
-              rope_cos: torch.Tensor, rope_sin: torch.Tensor, repr_out: Optional[Dict[int, torch.Tensor]],
-              attn_layers: Sequence[int], zero_pad_rows: bool = False, contact_job=None):
+              rope_cos: Optional[torch.Tensor], rope_sin: Optional[torch.Tensor],
+              repr_out: Optional[Dict[int, torch.Tensor]], attn_layers: Sequence[int], zero_pad_rows: bool = False,
+              contact_job=None):
     """esmb200_stack_forward on x fp32 (B,T,E) in place. repr_out: {layer index (0-based): (B,T,E) tensor to fill}.
+    rope_cos = rope_sin = None: layers without rotary embedding (ESM-1b / ESM-1v).
     Returns {layer index: (B,H,T,T) fp32} for the indices in attn_layers."""
     if not x.is_cuda:
         raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
@@ -466,13 +474,13 @@ class ContactPredictionHead(nn.Module):
         return self.activation(logits)
 
 
-class ESM2(nn.Module):
-    """Drop-in for esm.model.esm2.ESM2 (esm2.py:14-147): same constructor, same state-dict keys (so
-    `load_state_dict(reference_model.state_dict())` and the esm2_t*.pt checkpoints load), same forward contract."""
+class ProteinLanguageModel(nn.Module):
+    """The forward path ESM2 and ProteinBertModel (ESM-1b / ESM-1v, esm_b200.esm1) share: embedding prologue (`_embed`)
+    -> one esmb200_stack_forward (rotary tables from `_rope_tables`, or none) with the contact job fused -> LM head from
+    the pre-LN stream -> final LayerNorm.  The two models differ only in those two hooks and their constructors."""
 
-    def __init__(self, num_layers: int = 33, embed_dim: int = 1280, attention_heads: int = 20,
-                 alphabet: Union[Alphabet, str] = "ESM-1b", token_dropout: bool = True):
-        super().__init__()
+    def _init_encoder(self, num_layers: int, embed_dim: int, attention_heads: int, ffn_embed_dim: int,
+                      alphabet: Union[Alphabet, str], token_dropout: bool, use_rotary_embeddings: bool):
         self.num_layers = num_layers
         self.embed_dim = embed_dim
         self.attention_heads = attention_heads
@@ -490,18 +498,20 @@ class ESM2(nn.Module):
         self.embed_scale = 1
         self.embed_tokens = nn.Embedding(self.alphabet_size, embed_dim, padding_idx=self.padding_idx)
         self.layers = nn.ModuleList(
-            [TransformerLayer(embed_dim, 4 * embed_dim, attention_heads) for _ in range(num_layers)])
+            [TransformerLayer(embed_dim, ffn_embed_dim, attention_heads, use_rotary_embeddings)
+             for _ in range(num_layers)])
         self.contact_head = ContactPredictionHead(num_layers * attention_heads, self.prepend_bos, self.append_eos,
                                                   eos_idx=self.eos_idx)
+
+    def _init_head(self, embed_dim: int):
         self.emb_layer_norm_after = nn.LayerNorm(embed_dim)
         self.lm_head = RobertaLMHead(embed_dim, self.alphabet_size, self.embed_tokens.weight)
-        self._rope_cache = None
         self._mirrors: Dict[str, tuple] = {}
         self.precision = "fp16"
 
     PRECISIONS = {"fp16": 0, "fp32x3": 1}
 
-    def set_precision(self, name: str) -> "ESM2":
+    def set_precision(self, name: str) -> "ProteinLanguageModel":
         """"fp16" (default): fp16 MMA operands, fp32 accumulation — the fast path bench.py measures.
         "fp32x3": every MMA operand (LayerNorm output, weights, q, k, v, softmax probabilities, context, FFN hidden) is
         an fp16 hi + lo pair and every product runs hi*hi + lo*hi + hi*lo into the fp32 accumulator: 22 significand bits
@@ -517,11 +527,12 @@ class ESM2(nn.Module):
         return self
 
     def _rope_tables(self, T: int):
-        inv = self.layers[0].self_attn.rot_emb.inv_freq
-        key = (T, inv.device, inv.data_ptr())
-        if self._rope_cache is None or self._rope_cache[0] != key:
-            self._rope_cache = (key,) + rope_tables(inv, T)
-        return self._rope_cache[1], self._rope_cache[2]
+        """(cos, sin) tables for esmb200_stack_forward, or (None, None) for layers without rotary embedding."""
+        raise NotImplementedError
+
+    def _embed(self, tokens: torch.Tensor, x: torch.Tensor) -> None:
+        """Embedding prologue: fill the fp32 residual stream x [B,T,E] from tokens [B,T] (int64, contiguous)."""
+        raise NotImplementedError
 
     def _mirror(self, name: str, p: torch.Tensor) -> torch.Tensor:
         """fp32 mirror of a non-fp32 parameter (model.half()), cached until the parameter changes."""
@@ -558,11 +569,8 @@ class ESM2(nn.Module):
         cast = (lambda t: t) if dtype == torch.float32 else (lambda t: t.to(dtype))
 
         with torch.cuda.device(tokens.device):
-            # esm2.py:84-95 embedding prologue
             x = torch.empty((B, T, E), dtype=torch.float32, device=tokens.device)
-            table = self._mirror("embed_tokens", self.embed_tokens.weight)
-            _lib.check(lib.esmb200_embed_tokens(_ptr(tokens), _ptr(table), _ptr(x), B, T, E,
-                                                self.padding_idx, self.mask_idx, int(self.token_dropout), _stream()))
+            self._embed(tokens, x)
             if 0 in repr_layers:
                 hidden[0] = cast(x.clone())
             # esm2.py:108-109 drops the mask when the batch has no padding; that test is a device->host sync, which
@@ -602,3 +610,29 @@ class ESM2(nn.Module):
 
     def predict_contacts(self, tokens):
         return self(tokens, return_contacts=True)["contacts"]
+
+
+class ESM2(ProteinLanguageModel):
+    """Drop-in for esm.model.esm2.ESM2 (esm2.py:14-147): same constructor, same state-dict keys (so
+    `load_state_dict(reference_model.state_dict())` and the esm2_t*.pt checkpoints load), same forward contract."""
+
+    def __init__(self, num_layers: int = 33, embed_dim: int = 1280, attention_heads: int = 20,
+                 alphabet: Union[Alphabet, str] = "ESM-1b", token_dropout: bool = True):
+        super().__init__()
+        self._init_encoder(num_layers, embed_dim, attention_heads, 4 * embed_dim, alphabet, token_dropout, True)
+        self._init_head(embed_dim)
+        self._rope_cache = None
+
+    def _rope_tables(self, T: int):
+        inv = self.layers[0].self_attn.rot_emb.inv_freq
+        key = (T, inv.device, inv.data_ptr())
+        if self._rope_cache is None or self._rope_cache[0] != key:
+            self._rope_cache = (key,) + rope_tables(inv, T)
+        return self._rope_cache[1], self._rope_cache[2]
+
+    def _embed(self, tokens: torch.Tensor, x: torch.Tensor) -> None:
+        """esm2.py:84-95"""
+        B, T, E = x.shape
+        table = self._mirror("embed_tokens", self.embed_tokens.weight)
+        _lib.check(_lib.load().esmb200_embed_tokens(_ptr(tokens), _ptr(table), _ptr(x), B, T, E, self.padding_idx,
+                                                    self.mask_idx, int(self.token_dropout), _stream()))

@@ -290,7 +290,7 @@ def run_axial_stack(layers: Sequence[AxialTransformerLayer], xb: torch.Tensor,
 
 class LearnedPositionalEmbedding(nn.Embedding):
     """Parameter container with the reference's shape (modules.py:224-239: max_positions + padding_idx + 1 rows);
-    the lookup itself is part of esmb200_msa_embed."""
+    the lookup itself is part of esmb200_msa_embed (MSA Transformer) or esmb200_esm1b_embed (ESM-1b / ESM-1v)."""
 
     def __init__(self, num_embeddings: int, embedding_dim: int, padding_idx: int):
         super().__init__(num_embeddings + padding_idx + 1, embedding_dim, padding_idx)

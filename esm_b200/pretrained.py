@@ -76,9 +76,12 @@ def _random_init_or_raise(model_name: str, path: str, allow_random_init: bool) -
                   f"(model.random_init = True); its outputs are meaningless as embeddings.")
 
 
-def load_model_and_alphabet_local(model_location: str) -> Tuple[ESM2, Alphabet]:
-    """pretrained.py:67-77 / 164-183 for ESM-2 ("esm2*" file names): reads {"cfg": {"model": ...}, "model": sd}."""
+def load_model_and_alphabet_local(model_location: str):
+    """pretrained.py:67-77 / 164-183 for ESM-2: reads {"cfg": {"model": ...}, "model": sd}.  A v1 checkpoint
+    ({"args": Namespace, "model": sd}: ESM-1b / ESM-1v) is read by the v1 `roberta_large` loader (pretrained.py:85-101)."""
     data = torch.load(str(model_location), map_location="cpu", weights_only=False)
+    if "cfg" not in data and "args" in data:
+        return _load_esm1b(model_location, data)
     cfg = data["cfg"]["model"]
     get = (lambda k: cfg[k]) if isinstance(cfg, dict) else (lambda k: getattr(cfg, k))
     model = ESM2(num_layers=get("encoder_layers"), embed_dim=get("encoder_embed_dim"),
@@ -99,8 +102,13 @@ def load_model_and_alphabet(model_name: str, seed: int = 0, allow_random_init: b
     on the CPU); checkpoints are loaded on the CPU like the reference does."""
     if model_name.endswith(".pt"):
         return load_model_and_alphabet_local(model_name)
+    if model_name in ESM1B_ARCH:
+        return load_esm1b_model_and_alphabet(model_name, seed, allow_random_init, device)
+    if model_name.startswith("esm1_"):
+        raise ValueError(f"{model_name!r} is an ESM-1 model: ESM-1 (bias_kv attention) is not supported by esm_b200")
     if model_name not in ESM2_ARCH:
-        raise ValueError(f"esm_b200 covers the ESM-2 family only; unknown model {model_name!r}")
+        raise ValueError(f"unknown model {model_name!r}: this loader covers ESM-2 and ESM-1b / ESM-1v (the MSA "
+                         "Transformer loads through load_msa_model_and_alphabet)")
     path = _hub_path(model_name)
     if os.path.exists(path):
         return load_model_and_alphabet_local(path)
@@ -140,6 +148,118 @@ def esm2_t30_150M_UR50D(allow_random_init: bool = False):
 
 def esm2_t48_15B_UR50D(allow_random_init: bool = False):
     return load_model_and_alphabet("esm2_t48_15B_UR50D", allow_random_init=allow_random_init)
+
+
+# ---- ESM-1b / ESM-1v: ProteinBertModel, arch "roberta_large" (pretrained.py:85-101, 267-341) ----------------------
+_ESM1B_ARGS = dict(arch="roberta_large", layers=33, embed_dim=1280, ffn_embed_dim=5120, attention_heads=20,
+                   max_positions=1024, emb_layer_norm_before=True, token_dropout=True)
+ESM1B_ARCH = {  # name -> constructor arguments (the checkpoints' args after the prefix upgrade)
+    "esm1b_t33_650M_UR50S": _ESM1B_ARGS,
+    "esm1v_t33_650M_UR90S_1": _ESM1B_ARGS,
+    "esm1v_t33_650M_UR90S_2": _ESM1B_ARGS,
+    "esm1v_t33_650M_UR90S_3": _ESM1B_ARGS,
+    "esm1v_t33_650M_UR90S_4": _ESM1B_ARGS,
+    "esm1v_t33_650M_UR90S_5": _ESM1B_ARGS,
+}
+
+
+def _upgrade_esm1b_checkpoint(data, alphabet: Alphabet):
+    """pretrained.py:90-100: strip "encoder_" from argument names and the "sentence_encoder." / "encoder." prefixes
+    from parameter names, zero the <mask> row of embed_tokens (token dropout), and infer emb_layer_norm_before from
+    the keys."""
+    strip_arg = lambda k: "".join(k.split("encoder_")[1:] if "encoder" in k else k)
+    strip1 = lambda k: "".join(k.split("encoder.")[1:] if "encoder" in k else k)
+    strip2 = lambda k: "".join(k.split("sentence_encoder.")[1:] if "sentence_encoder" in k else k)
+    args = {strip_arg(k): v for k, v in vars(data["args"]).items()}
+    state = {strip1(strip2(k)): v for k, v in data["model"].items()}
+    state["embed_tokens.weight"][alphabet.mask_idx].zero_()
+    args["emb_layer_norm_before"] = any(k.startswith("emb_layer_norm_before") for k in state)
+    return args, state
+
+
+def _load_esm1b(model_location: str, data):
+    from .esm1 import ProteinBertModel
+    arch = getattr(data["args"], "arch", None)
+    if arch == "protein_bert_base":
+        raise ValueError(f"{model_location}: an ESM-1 checkpoint; ESM-1 (bias_kv attention) is not supported by esm_b200")
+    if arch != "roberta_large":
+        raise ValueError(f"{model_location}: unsupported v1 checkpoint architecture {arch!r}")
+    reg = str(model_location)[:-3] + "-contact-regression.pt"
+    if os.path.exists(reg):  # ESM-1b ships one; ESM-1v has none (pretrained.py:18-21), which warns below
+        data["model"].update(torch.load(reg, map_location="cpu", weights_only=False)["model"])
+    alphabet = Alphabet.from_architecture("roberta_large")
+    args, state = _upgrade_esm1b_checkpoint(data, alphabet)
+    model = ProteinBertModel(Namespace(**args), alphabet)
+    _load_checked(model, state, "ProteinBertModel")
+    model.random_init = False
+    return model.eval(), alphabet
+
+
+def load_esm1b_model_and_alphabet(model_name: str, seed: int = 0, allow_random_init: bool = False, device=None):
+    """ESM-1b / ESM-1v by name (hub cache) or from a local v1 .pt file."""
+    from .esm1 import ProteinBertModel
+    if model_name.endswith(".pt"):
+        return load_model_and_alphabet_local(model_name)
+    if model_name not in ESM1B_ARCH:
+        raise ValueError(f"unknown ESM-1b / ESM-1v model {model_name!r}")
+    path = _hub_path(model_name)
+    if os.path.exists(path):
+        return load_model_and_alphabet_local(path)
+    _random_init_or_raise(model_name, path, allow_random_init)
+    gen_state = torch.random.get_rng_state()
+    torch.manual_seed(seed)
+    alphabet = Alphabet.from_architecture("roberta_large")
+    if device is not None:
+        with torch.device(device):
+            model = ProteinBertModel(Namespace(**ESM1B_ARCH[model_name]), alphabet)
+    else:
+        model = ProteinBertModel(Namespace(**ESM1B_ARCH[model_name]), alphabet)
+    torch.random.set_rng_state(gen_state)
+    model.random_init = True
+    return model.eval(), alphabet
+
+
+def esm1b_t33_650M_UR50S(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1b_t33_650M_UR50S", allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S(allow_random_init: bool = False):
+    """Alias of esm1v_t33_650M_UR90S_1, like the reference (pretrained.py:285-291)."""
+    return esm1v_t33_650M_UR90S_1(allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S_1(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1v_t33_650M_UR90S_1", allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S_2(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1v_t33_650M_UR90S_2", allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S_3(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1v_t33_650M_UR90S_3", allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S_4(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1v_t33_650M_UR90S_4", allow_random_init=allow_random_init)
+
+
+def esm1v_t33_650M_UR90S_5(allow_random_init: bool = False):
+    return load_esm1b_model_and_alphabet("esm1v_t33_650M_UR90S_5", allow_random_init=allow_random_init)
+
+
+def _esm1_unsupported(name: str):
+    def factory(*args, **kwargs):
+        raise ValueError(f"{name!r} is an ESM-1 model: ESM-1 (bias_kv attention) is not supported by esm_b200")
+    factory.__name__ = name
+    return factory
+
+
+esm1_t34_670M_UR50S = _esm1_unsupported("esm1_t34_670M_UR50S")
+esm1_t34_670M_UR50D = _esm1_unsupported("esm1_t34_670M_UR50D")
+esm1_t34_670M_UR100 = _esm1_unsupported("esm1_t34_670M_UR100")
+esm1_t12_85M_UR50S = _esm1_unsupported("esm1_t12_85M_UR50S")
+esm1_t6_43M_UR50S = _esm1_unsupported("esm1_t6_43M_UR50S")
 
 
 # ---- MSA Transformer (pretrained.py:104-125, 293-300) -----------------------------------------------------------

@@ -19,6 +19,8 @@
  *     transposed); MMA operands are fp16 with fp32 accumulation; LayerNorm / softmax / residual adds are fp32
  *   - even head_dim <= 128 (every esm.pretrained.esm2_* model; heads narrower than 64 run in zero-padded 64-wide
  *     slots, 128-wide heads in two); no CPU fallback
+ *   - ESM-1b / ESM-1v (esm/model/esm1.py, arch roberta_large) run the same layers without rotary tables, after
+ *     esmb200_esm1b_embed
  */
 #ifndef ESMB200_H_
 #define ESMB200_H_
@@ -90,7 +92,10 @@ size_t esmb200_workspace_bytes(int32_t embed_dim, int32_t num_heads, int32_t ffn
  *   x          fp32 [B,T,E], updated in place
  *   pad_mask   uint8/bool [B,T], nonzero = padding key (self_attn_padding_mask, esm2.py:82), or NULL
  *   rope_cos/sin fp32 [T,32] (head_dim <= 64) or [T,64] (head_dim <= 128): cos/sin(t * inv_freq[j]) for j < head_dim/2
- *              (rotary_embedding.py:47-61), built by the caller; columns >= head_dim/2 are ignored
+ *              (rotary_embedding.py:47-61), built by the caller; columns >= head_dim/2 are ignored.
+ *              Both NULL: no rotary embedding, q and k stay unrotated (ESM-1b / ESM-1v layers, whose positions are
+ *              added by esmb200_esm1b_embed; multihead_attention.py:354 with rot_emb = None). Exactly one NULL is
+ *              ESMB200_EINVAL. The same holds for esmb200_stack_forward.
  *   attn_probs fp32 [B,H,T,T] or NULL: softmax probabilities per head (need_head_weights=True,
  *              multihead_attention.py:397-400, batch-major i.e. already transposed as esm2.py:121 does) */
 int esmb200_layer_forward(esmb200_layer* layer, float* x, const uint8_t* pad_mask, int32_t B, int32_t T,
@@ -110,7 +115,8 @@ typedef struct esmb200_contact_job {
   int32_t lo, hi;       /* cropped positions [lo,hi): 1 .. T-1 for <cls> ... <eos> */
 } esmb200_contact_job;
 
-/* The layer loop of ESM2.forward (esm2.py:111-121): runs n_layers layers in place on x.
+/* The layer loop of ESM2.forward (esm2.py:111-121), and of ProteinBertModel.forward for ESM-1b / ESM-1v (esm1.py:155-163)
+ * with rope_cos == rope_sin == NULL: runs n_layers layers in place on x.
  *   repr_out[i]  NULL or fp32 [B,T,E]: copy of x after layer i (hidden_representations[i+1], esm2.py:117-118)
  *   attn_out[i]  NULL or fp32 [B,H,T,T]: attention probabilities of layer i (esm2.py:119-121); batch b starts at
  *                attn_out[i] + b * attn_batch_stride elements (0 = contiguous H*T*T), so the caller can point layer i
@@ -128,6 +134,18 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
  * 0.88/(1 - n_mask/n_nonpad) when token_dropout, zero pad rows. tokens int64 [B,T] -> x fp32 [B,T,E]. */
 int esmb200_embed_tokens(const int64_t* tokens, const float* table, float* x, int32_t B, int32_t T, int32_t E,
                          int32_t padding_idx, int32_t mask_idx, int32_t token_dropout, void* stream);
+
+/* Embedding prologue of ProteinBertModel.forward for ESM-1b / ESM-1v (esm/model/esm1.py:121-139), one launch:
+ *   x = embed_table[tok]; token_dropout != 0: <mask> rows zeroed, x = (x * 0.88) / (1 - n_mask/n_nonpad);
+ *   x += pos_table[cumsum(tok != pad) * (tok != pad) + padding_idx] (LearnedPositionalEmbedding, modules.py:240-257;
+ *   a pad anywhere in the sequence is handled); ln_weight/ln_bias given: LayerNorm with eps (emb_layer_norm_before);
+ *   pad rows zeroed.
+ * tokens int64 [B,T]; embed_table [V,E]; pos_table [max_positions + padding_idx + 1, E] with T <= max_positions (the
+ * caller checks, as the reference raises ValueError); ln_weight, ln_bias [E] both or neither. x fp32 [B,T,E].
+ * E % 4 == 0, E <= 2560, T <= 12288. */
+int esmb200_esm1b_embed(const int64_t* tokens, const float* embed_table, const float* pos_table, const float* ln_weight,
+                        const float* ln_bias, float eps, int32_t token_dropout, int32_t padding_idx, int32_t mask_idx,
+                        float* x, int32_t B, int32_t T, int32_t E, void* stream);
 
 /* torch.nn.LayerNorm over the last dim (ESM1bLayerNorm, modules.py:68-81; emb_layer_norm_after, esm2.py:123):
  * fp32 [M,E] -> fp32 [M,E]. out may alias x. */
