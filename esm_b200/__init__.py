@@ -6,6 +6,7 @@
 
     msa_model, msa_alphabet = pretrained.esm_msa1b_t12_100M_UR50S()   # MSA Transformer: tokens [B, R, C]
     esm1v_model, _ = pretrained.esm1v_t33_650M_UR90S_1()              # ESM-1b / ESM-1v: ProteinBertModel
+    lp = variants.masked_marginals(esm1v_model.cuda(), tokens)          # variant scoring (predict.py), batched
 
 Compute goes through the C ABI of libesmb200.so (include/esmb200.h); see DESIGN.md / INTEGRATION.md.
 """
@@ -13,6 +14,6 @@ from .alphabet import Alphabet, BatchConverter  # noqa: F401
 from .model import ESM2, TransformerLayer  # noqa: F401
 from .esm1 import ProteinBertModel  # noqa: F401
 from .msa import AxialTransformerLayer, MSATransformer  # noqa: F401
-from . import pretrained  # noqa: F401
+from . import pretrained, variants  # noqa: F401
 
 __version__ = "0.1.0"

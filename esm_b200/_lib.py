@@ -27,6 +27,7 @@ EXPORTS = (
     "esmb200_esm1b_embed",
     "esmb200_layernorm",
     "esmb200_mean_pool",
+    "esmb200_log_softmax_rows",
     "esmb200_gemm_f16",
     "esmb200_gemm_qkv_f16",
     "esmb200_attention_scratch_bytes",
@@ -127,6 +128,8 @@ def _declare(lib):
     lib.esmb200_layernorm.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_mean_pool.restype = c_int32
     lib.esmb200_mean_pool.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]
+    lib.esmb200_log_softmax_rows.restype = c_int32
+    lib.esmb200_log_softmax_rows.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -52,7 +52,8 @@ int fail_cuda(cudaError_t e, const char* what) {
 
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
-                     T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_COUNT };
+                     T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
+                     T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1008,6 +1009,18 @@ int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_
   if (E % 4 != 0) return fail(ESMB200_EINVAL, "mean_pool needs E % 4 == 0");
   dim3 grid((E + 127) / 128, B);
   mean_pool_kernel<<<grid, 256, 0, st>>>(x, lengths, out, T, E);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
+int esmb200_log_softmax_rows(const float* logits, int64_t ld, int32_t n, int32_t V, const int64_t* target, float* out,
+                             void* stream) {
+  if (!logits || !out) return fail(ESMB200_EINVAL, "null argument");
+  if (n < 0 || V <= 0 || V > 64 || ld < V) return fail(ESMB200_EINVAL, "log_softmax_rows needs 0 < V <= 64 and ld >= V");
+  if (n == 0) return ESMB200_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope ps(T_LOG_SOFTMAX, st);
+  log_softmax_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(logits, ld, n, V, target, out);
   CK(cudaGetLastError());
   return ESMB200_OK;
 }

@@ -7,6 +7,8 @@
 //   esm1b_embed       esm/model/esm1.py:121-139 (the same, plus learned positions and emb_layer_norm_before)
 //   key_bits          esm/model/esm2.py:82 + multihead_attention.py:368-374 (key padding mask) packed to 1 bit/key
 //   mean_pool         scripts/extract.py:116-119 per-sequence mean representation
+//   log_softmax_rows  examples/variant-prediction/predict.py:142,175,194,211 (torch.log_softmax over the vocabulary)
+//                     and the target gather of :114,143
 //   convert_f32_f16   weight packing (fp32 nn.Linear weights -> fp16 MMA operands)
 #pragma once
 
@@ -208,6 +210,37 @@ mean_pool_kernel(const float* __restrict__ x, const int* __restrict__ lengths, f
     }
     const float inv = 1.0f / (float)n;  // n == 0: inf * 0 = NaN like the reference's mean over an empty slice
     *reinterpret_cast<float4*>(out + (size_t)b * E + col) = make_float4(s.x * inv, s.y * inv, s.z * inv, s.w * inv);
+  }
+}
+
+// log_softmax over the first V <= 64 columns of each row: one warp per row, lane l holds columns l and l + 32. The
+// arithmetic follows PyTorch's warp-per-row softmax for rows of at most 64 elements: row max, per-lane sum of
+// expf(x - max) in column order, xor-butterfly sums, then (x - max) - logf(sum). expf / logf are the accurate library
+// functions, not ex2.approx. target == nullptr: out [n, V]; otherwise out[i] = the value of column target[i] (in [0, V),
+// checked by the caller).
+__global__ void __launch_bounds__(256)
+log_softmax_rows_kernel(const float* __restrict__ logits, int64_t ld, int n, int V, const int64_t* __restrict__ target,
+                        float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (row >= n) return;
+  const float* x = logits + (size_t)row * ld;
+  const float v0 = lane < V ? x[lane] : -INFINITY;
+  const float v1 = lane + 32 < V ? x[lane + 32] : -INFINITY;
+  float m = fmaxf(v0, v1);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  float s = expf(v0 - m);
+  s += expf(v1 - m);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float lse = logf(s);
+  if (target) {
+    if (lane == 0) out[row] = (x[target[row]] - m) - lse;
+  } else {
+    float* y = out + (size_t)row * V;
+    if (lane < V) y[lane] = (v0 - m) - lse;
+    if (lane + 32 < V) y[lane + 32] = (v1 - m) - lse;
   }
 }
 

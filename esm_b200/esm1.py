@@ -62,9 +62,9 @@ class ProteinBertModel(ProteinLanguageModel):
             _ptr(tokens), _ptr(table), _ptr(pos), _ptr(ln_w), _ptr(ln_b), ln.eps if ln is not None else 1e-5,
             int(self.token_dropout), self.padding_idx, self.mask_idx, _ptr(x), B, T, E, _stream()))
 
-    def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
+    def _stack(self, tokens, *args, **kwargs):
+        """forward's stack step (also the variant scorers'), behind the reference's length check."""
         max_positions = self.embed_positions.max_positions
         if tokens.size(1) > max_positions:  # modules.py:242-246
             raise ValueError(f"Sequence length {tokens.size(1)} above maximum  sequence length of {max_positions}")
-        return super().forward(tokens, repr_layers=repr_layers, need_head_weights=need_head_weights,
-                               return_contacts=return_contacts)
+        return super()._stack(tokens, *args, **kwargs)

@@ -545,14 +545,16 @@ class ProteinLanguageModel(nn.Module):
             self._mirrors[name] = hit
         return hit[1]
 
-    @torch.no_grad()
-    def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
-        if return_contacts:
-            need_head_weights = True
+    def _stack(self, tokens, repr_layers=frozenset(), need_head_weights=False, return_contacts=False,
+               cast=lambda t: t):
+        """The stack step of `forward` (esm2.py:82-121): embedding prologue and one esmb200_stack_forward.
+        Returns (tokens int64 contiguous, x, hidden, attn_t, cjob): x is the fp32 residual stream [B,T,E] BEFORE
+        emb_layer_norm_after, hidden {i: cast(representation)} for the requested layers below num_layers, attn_t
+        run_stack's attention maps, cjob the fused contact job or None.  Runs under torch.cuda.device(tokens.device)."""
         assert tokens.ndim == 2
         if not tokens.is_cuda:
             raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
-        lib = _lib.load()
+        _lib.load()
         if tokens.dtype != torch.int64:
             if tokens.dtype.is_floating_point or tokens.dtype == torch.bool:
                 raise TypeError(f"tokens must be an integer tensor, got {tokens.dtype}")
@@ -562,11 +564,8 @@ class ProteinLanguageModel(nn.Module):
         torch._assert_async(((tokens >= 0) & (tokens < self.alphabet_size)).all())
         B, T = tokens.shape
         E, N = self.embed_dim, self.num_layers
-        dtype = self.embed_tokens.weight.dtype  # fp32, or fp16/bf16 after model.half() (esmfold.py:59-62)
         padding_mask = tokens.eq(self.padding_idx)  # esm2.py:82
-        repr_layers = set(repr_layers)
         hidden: Dict[int, torch.Tensor] = {}
-        cast = (lambda t: t) if dtype == torch.float32 else (lambda t: t.to(dtype))
 
         with torch.cuda.device(tokens.device):
             x = torch.empty((B, T, E), dtype=torch.float32, device=tokens.device)
@@ -588,6 +587,28 @@ class ProteinLanguageModel(nn.Module):
                                contact_job=cjob["job"] if cjob else None)
             for i, t in repr_out.items():
                 hidden[i + 1] = cast(t)
+        return tokens, x, hidden, attn_t, cjob
+
+    def _lm_head_rows(self, x_rows: torch.Tensor) -> torch.Tensor:
+        """The LM head (esm2.py:123,129) on selected rows [n,E] of the pre-LN stream: fp32 logits [n,V], also after
+        model.half()."""
+        ln = self.emb_layer_norm_after
+        ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)
+        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln_w, ln_b, ln.eps, self.PRECISIONS[self.precision])[0]
+
+    @torch.no_grad()
+    def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
+        if return_contacts:
+            need_head_weights = True
+        dtype = self.embed_tokens.weight.dtype  # fp32, or fp16/bf16 after model.half() (esmfold.py:59-62)
+        repr_layers = set(repr_layers)
+        cast = (lambda t: t) if dtype == torch.float32 else (lambda t: t.to(dtype))
+        tokens, x, hidden, attn_t, cjob = self._stack(tokens, repr_layers, need_head_weights, return_contacts, cast)
+        lib = _lib.load()
+        B, T = tokens.shape
+        E, N = self.embed_dim, self.num_layers
+
+        with torch.cuda.device(tokens.device):
             # esm2.py:129 LM head, from the pre-LN stream (its first step is the same emb_layer_norm_after)
             ln = self.emb_layer_norm_after
             ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)

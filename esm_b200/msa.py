@@ -359,11 +359,46 @@ class MSATransformer(nn.Module):
 
     @torch.no_grad()
     def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
+        if return_contacts and not self.contacts_without_col_attentions:
+            need_head_weights = True  # msa_transformer.py:149-150
+        repr_layers = set(repr_layers)
+        tokens, x, hidden, row_attn, col_attn = self._stack(tokens, repr_layers, need_head_weights, return_contacts)
+        lib = _lib.load()
+        B, R, C = tokens.shape
+        E, N = self.args.embed_dim, self.args.layers
+        want_rows = need_head_weights or return_contacts
+        dev = tokens.device
+        with torch.cuda.device(dev):
+            ln = self.emb_layer_norm_after
+            logits = self.lm_head.forward_native(x.view(B, R * C, E), ln.weight, ln.bias, ln.eps).view(B, R, C, -1)
+            _lib.check(lib.esmb200_layernorm(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(x), B * R * C, E, ln.eps,
+                                             _stream()))
+        if N in repr_layers:
+            hidden[N] = x  # the last representation is post-LayerNorm (msa_transformer.py:204-209)
+        result = {"logits": logits, "representations": hidden}
+        if want_rows:
+            # H,B,C,C per layer -> B,L,H,C,C (msa_transformer.py:196-197,215)
+            row_attentions = torch.stack([row_attn[i].permute(1, 0, 2, 3) for i in range(N)], 1)
+            result["row_attentions"] = row_attentions
+            if need_head_weights:
+                result["col_attentions"] = torch.stack(col_attn, 1)  # B,L,H,C,R,R
+            if return_contacts:
+                result["contacts"] = self.contact_head(tokens, row_attentions)
+        return result
+
+    def _lm_head_rows(self, x_rows: torch.Tensor) -> torch.Tensor:
+        """The LM head (msa_transformer.py:204-210) on selected rows [n,E] of the pre-LN stream: fp32 logits [n,V]."""
+        ln = self.emb_layer_norm_after
+        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln.weight, ln.bias, ln.eps)[0]
+
+    def _stack(self, tokens, repr_layers=frozenset(), need_head_weights=False, return_contacts=False):
+        """The stack step of `forward` (msa_transformer.py:147-201): embedding prologue and the axial layers.
+        Returns (tokens contiguous, x, hidden, row_attn, col_attn): x is the fp32 residual stream [B,R,C,E] BEFORE
+        emb_layer_norm_after, hidden {i: representation} for the requested layers below num_layers, row_attn
+        {layer: [H,B,C,C]} and col_attn [B,H,C,R,R] per layer when the maps are asked for."""
         assert tokens.ndim == 3
         if not tokens.is_cuda:
             raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
-        if return_contacts and not self.contacts_without_col_attentions:
-            need_head_weights = True  # msa_transformer.py:149-150
         lib = _lib.load()
         tokens = tokens.contiguous()
         B, R, C = tokens.shape
@@ -411,22 +446,7 @@ class MSATransformer(nn.Module):
                     if stop < N:
                         hidden[stop] = x.clone()
                     start = stop
-            ln = self.emb_layer_norm_after
-            logits = self.lm_head.forward_native(x.view(B, R * C, E), ln.weight, ln.bias, ln.eps).view(B, R, C, -1)
-            _lib.check(lib.esmb200_layernorm(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(x), B * R * C, E, ln.eps,
-                                             _stream()))
-        if N in repr_layers:
-            hidden[N] = x  # the last representation is post-LayerNorm (msa_transformer.py:204-209)
-        result = {"logits": logits, "representations": hidden}
-        if want_rows:
-            # H,B,C,C per layer -> B,L,H,C,C (msa_transformer.py:196-197,215)
-            row_attentions = torch.stack([row_attn[i].permute(1, 0, 2, 3) for i in range(N)], 1)
-            result["row_attentions"] = row_attentions
-            if need_head_weights:
-                result["col_attentions"] = torch.stack(col_attn, 1)  # B,L,H,C,R,R
-            if return_contacts:
-                result["contacts"] = self.contact_head(tokens, row_attentions)
-        return result
+        return tokens, x, hidden, row_attn, col_attn
 
     def predict_contacts(self, tokens):
         """msa_transformer.py:222-223; only the contacts are returned, so the column attention maps are not built."""

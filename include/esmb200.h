@@ -21,6 +21,9 @@
  *     slots, 128-wide heads in two); no CPU fallback
  *   - ESM-1b / ESM-1v (esm/model/esm1.py, arch roberta_large) run the same layers without rotary tables, after
  *     esmb200_esm1b_embed
+ *   - variant-effect scoring (examples/variant-prediction/predict.py; esm_b200.variants) batches the masked copies
+ *     into one esmb200_stack_forward per chunk, runs the LM head on the masked rows only and finishes with
+ *     esmb200_log_softmax_rows
  */
 #ifndef ESMB200_H_
 #define ESMB200_H_
@@ -157,6 +160,14 @@ int esmb200_layernorm(const float* x, const float* weight, const float* bias, fl
 int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_t B, int32_t T, int32_t E,
                       void* stream);
 
+/* log_softmax over the first V columns of each row (examples/variant-prediction/predict.py:142,175,194,211:
+ * torch.log_softmax(logits, -1)), fp32, one warp per row: row max, sum of expf(x - max), logf (accurate, not
+ * ex2.approx: matches torch.log_softmax to ~1e-6). logits fp32 [n, ld], V <= ld, V <= 64.
+ * target NULL: out fp32 [n, V]. target int64 [n]: out fp32 [n] = the log-probability of column target[i]
+ * (predict.py:114,143). Targets must lie in [0, V); the caller checks them. n == 0 launches nothing. */
+int esmb200_log_softmax_rows(const float* logits, int64_t ld, int32_t n, int32_t V, const int64_t* target,
+                             float* out, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -253,7 +264,7 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *   synchronising on the recorded events, and resets the record list.
  *   tags: 0 LN1->f16, 1 QKV+RoPE GEMM, 2 attention, 3 out-proj GEMM, 4 LN2->f16, 5 fc1+GELU GEMM, 6 fc2 GEMM,
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
- *         14 tied row logits, 15 tied row softmax, 16 tied row update */
+ *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
