@@ -262,10 +262,10 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
   cudaError_t e;
   {
     CUtensorMap tkv;
-    rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * T, qcols, qcols, attn8_cfg::BLOCK_KV);
+    rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * T, qcols, qcols, attention_fwd_kv_box_rows(ap));
     if (rc) return rc;
     ProfScope ps(T_ATTN, st);
-    e = launch_attention_fwd(tq, tkv, ap, st);
+    e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "attention launch");
   if (probs && contact && !split) {
@@ -311,21 +311,21 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
 int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B, int R, int C, int H,
                          cudaStream_t st) {
   const int E = H * 64;
-  CUtensorMap tq, tkv;
-  const uint64_t wide = (uint64_t)C * 3 * E;  // token r of column c at row r, x = c*3E
-  int rc;
-  if ((rc = make_tmap_f16(&tq, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_Q))) return rc;
-  if ((rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * R, wide, wide, attn8_cfg::BLOCK_KV))) return rc;
   AttnParams ap;
   ap.B = B * C; ap.T = R; ap.H = H; ap.E = E;
   ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
   ap.ctx = static_cast<__half*>(ctx);
   ap.row_max = nullptr; ap.row_sum = nullptr;
   ap.cols = C;
+  CUtensorMap tq, tkv;
+  const uint64_t wide = (uint64_t)C * 3 * E;  // token r of column c at row r, x = c*3E
+  int rc;
+  if ((rc = make_tmap_f16(&tq, qkv, (uint64_t)B * R, wide, wide, 128))) return rc;
+  if ((rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * R, wide, wide, attention_fwd_kv_box_rows(ap)))) return rc;
   cudaError_t e;
   {
     ProfScope ps(T_ATTN, st);
-    e = launch_attention_fwd(tq, tkv, ap, st);
+    e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
   return ESMB200_OK;

@@ -1,4 +1,5 @@
-// esm_b200 — attention forward (sm_90a): flash attention with TMA-fed K/V stages and warp-level tensor-core MMAs.
+// esm_b200 — attention forward (sm_90a): flash attention with TMA-fed K/V stages and warp-level tensor-core MMAs, for
+// the inputs the warpgroup kernel (attention_wg.cuh) does not take: fp32x3 operands and 128-wide heads.
 //
 // Replaces esm/multihead_attention.py:357-394.  One CTA per (sequence, head, 128-query tile), eight warps of 16 query
 // rows each.  Thread 0 loads the Q tile once and streams 64-key K/V blocks through a two-stage TMA ring (mbarrier
@@ -13,6 +14,7 @@
 #pragma once
 
 #include "attention_common.cuh"
+#include "attention_wg.cuh"
 
 namespace esmb200 {
 
@@ -234,11 +236,21 @@ inline cudaError_t launch_attention_ds(const CUtensorMap& tmap_q, const CUtensor
   return launch_pdl(kern, dim3((unsigned)total), dim3(NUM_THREADS), smem, stream, tmap_q, tmap_kv, p);
 }
 
+// fp16 operands in one 64-wide slot run on the warpgroup-MMA kernel (attention_wg.cuh); fp32x3 operands and two-slot
+// heads on attention_fwd_kernel above
+inline bool attention_fwd_uses_wg(const AttnParams& p) { return p.lo_off == 0 && p.slots == 1; }
+
+// Rows of the K/V TMA box the launched kernel expects (tmap_kv of launch_attention_fwd); the Q box is 128 rows for
+// every kernel (and the probability kernels that share the Q map)
+inline int attention_fwd_kv_box_rows(const AttnParams& p) {
+  return attention_fwd_uses_wg(p) ? attn_wg_cfg::BLOCK_KV : attn8_cfg::BLOCK_KV;
+}
+
 inline cudaError_t launch_attention_fwd(const CUtensorMap& tmap_q, const CUtensorMap& tmap_kv, const AttnParams& p,
-                                        cudaStream_t stream) {
+                                        int num_sms, cudaStream_t stream) {
+  if (attention_fwd_uses_wg(p)) return launch_attention_wg(tmap_q, tmap_kv, p, num_sms, stream);
   if (p.lo_off > 0) return launch_attention_ds<true, 1>(tmap_q, tmap_kv, p, stream);
-  if (p.slots == 2) return launch_attention_ds<false, 2>(tmap_q, tmap_kv, p, stream);
-  return launch_attention_ds<false, 1>(tmap_q, tmap_kv, p, stream);
+  return launch_attention_ds<false, 2>(tmap_q, tmap_kv, p, stream);
 }
 
 }  // namespace esmb200
