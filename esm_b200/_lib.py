@@ -51,6 +51,11 @@ EXPORTS = (
     "esmb200_convert_split",
     "esmb200_gemm_split",
     "esmb200_attention_split",
+    "esmb200_axial_workspace_bytes_split",
+    "esmb200_gemm_qkv_split",
+    "esmb200_tied_row_attention_split_scratch_bytes",
+    "esmb200_tied_row_attention_split",
+    "esmb200_column_attention_split",
 )
 
 ABI_VERSION = 2
@@ -185,6 +190,18 @@ def _declare(lib):
     lib.esmb200_attention_split.restype = c_int32
     lib.esmb200_attention_split.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p,
                                             c_void_p]
+    lib.esmb200_axial_workspace_bytes_split.restype = c_size_t
+    lib.esmb200_axial_workspace_bytes_split.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32]
+    lib.esmb200_gemm_qkv_split.restype = c_int32
+    lib.esmb200_gemm_qkv_split.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
+    lib.esmb200_tied_row_attention_split_scratch_bytes.restype = c_size_t
+    lib.esmb200_tied_row_attention_split_scratch_bytes.argtypes = [c_int32, c_int32, c_int32]
+    lib.esmb200_tied_row_attention_split.restype = c_int32
+    lib.esmb200_tied_row_attention_split.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
+                                                     c_int32, c_void_p, c_size_t, c_void_p]
+    lib.esmb200_column_attention_split.restype = c_int32
+    lib.esmb200_column_attention_split.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                                   c_void_p, c_void_p]
     lib.esmb200_set_option.restype = c_int32
     lib.esmb200_set_option.argtypes = [c_char_p, c_int32]
     lib.esmb200_convert_f16.restype = c_int32

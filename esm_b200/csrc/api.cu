@@ -307,18 +307,20 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
 
 // MSA column attention (axial_attention.py:182-239) straight from the row-major qkv [B*R*C, 3E]: one "sequence" of R
 // tokens per alignment column, read with strided TMA boxes (qkv viewed as [B*R, C*3E], AttnParams::cols), no
-// regrouping copy.  s holds the key bits of the B*C column sequences.
+// regrouping copy.  s holds the key bits of the B*C column sequences.  split (fp32x3): qkv [B*R*C, 6E] (viewed as
+// [B*R, C*6E], lo halves 3E to the right), ctx [B*R*C, 2E].
 int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B, int R, int C, int H,
-                         cudaStream_t st) {
+                         cudaStream_t st, bool split = false) {
   const int E = H * 64;
   AttnParams ap;
   ap.B = B * C; ap.T = R; ap.H = H; ap.E = E;
+  ap.lo_off = split ? 3 * E : 0;
   ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
   ap.ctx = static_cast<__half*>(ctx);
   ap.row_max = nullptr; ap.row_sum = nullptr;
   ap.cols = C;
   CUtensorMap tq, tkv;
-  const uint64_t wide = (uint64_t)C * 3 * E;  // token r of column c at row r, x = c*3E
+  const uint64_t wide = (uint64_t)C * (split ? 6 : 3) * E;  // token r of column c at row r, x = c*3E (split: c*6E)
   int rc;
   if ((rc = make_tmap_f16(&tq, qkv, (uint64_t)B * R, wide, wide, 128))) return rc;
   if ((rc = make_tmap_f16(&tkv, qkv, (uint64_t)B * R, wide, wide, attention_fwd_kv_box_rows(ap)))) return rc;
@@ -509,13 +511,19 @@ struct AxialWorkspace {
   size_t bytes;
 };
 
-// the one definition of the MSA stack workspace: nullptr measures it (esmb200_axial_workspace_bytes), a device pointer
-// carves it
-AxialWorkspace axial_workspace_layout(void* workspace, int E, int F, int B, int R, int C) {
+// scratch of the tied row attention: fp32 logits [H,B,C,C], then P [H*B*C, Cp] fp16 (split: hi | lo, [H*B*C, 2*Cp])
+size_t tied_scratch_bytes(int B, int C, int H, int split) {
+  const size_t Cp = align_up((size_t)C, 64), pf = split ? 2 : 1;
+  return align_up((size_t)H * B * C * C * 4, 1024) + align_up((size_t)H * B * C * Cp * 2 * pf, 1024) + 2048;
+}
+
+// the one definition of the MSA stack workspace: nullptr measures it (esmb200_axial_workspace_bytes and its _split
+// variant), a device pointer carves it
+AxialWorkspace axial_workspace_layout(void* workspace, int E, int F, int B, int R, int C, int split) {
   AxialWorkspace a;
-  a.ws = workspace_layout(workspace, E, E / 64, F, B * C, R, 0);
+  a.ws = workspace_layout(workspace, E, E / 64, F, B * C, R, split);
   a.tied = reinterpret_cast<uint8_t*>(a.ws.xn) + a.ws.bytes;
-  a.tied_bytes = esmb200_tied_row_attention_scratch_bytes(B, C, E / 64);
+  a.tied_bytes = tied_scratch_bytes(B, C, E / 64, split);
   a.bytes = a.ws.bytes + a.tied_bytes + 1024;
   return a;
 }
@@ -763,7 +771,8 @@ int esmb200_gemm_f16(int32_t epilogue, const void* a, const void* w, const float
   return gemm_epilogue_entry(epilogue, a, w, bias, out, M, N, K, rope_cos, rope_sin, T, E, false, stream);
 }
 
-// ---- fp32x3 precision building blocks (hi | lo fp16 operands): used by the LM head and the kernel-level parity tests
+// ---- fp32x3 precision building blocks (hi | lo fp16 operands): used by the LM head, the MSA layer's attention-map path
+// and the kernel-level parity tests
 int esmb200_layernorm_split(const float* x, const float* weight, const float* bias, void* out, int32_t M, int32_t E,
                             float eps, void* stream) {
   if (!x || !weight || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
@@ -799,6 +808,15 @@ int esmb200_gemm_qkv_f16(const void* a, const void* w, const float* bias, void* 
                   stream);
 }
 
+int esmb200_gemm_qkv_split(const void* a, const void* w, const float* bias, void* out, int32_t M, int32_t E,
+                           float q_scale, void* stream) {
+  if (!a || !w || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
+  if (M <= 0 || E <= 0 || E % 64 != 0) return fail(ESMB200_EINVAL, "qkv gemm needs E % 64 == 0");
+  int rc = check_device();
+  if (rc) return rc;
+  return run_gemm(EPI_QKV_ROPE, a, w, bias, out, M, 3 * E, E, nullptr, nullptr, 1, E, q_scale, true, stream);
+}
+
 int esmb200_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                       int32_t H, void* scratch, void* stream) {
   return attention_entry(qkv, pad_mask, ctx, attn_probs, B, T, H, scratch, stream, false, 1);
@@ -811,18 +829,21 @@ int esmb200_attention128(const void* qkv, const uint8_t* pad_mask, void* ctx, fl
 
 // ---- MSA axial attention (esm/axial_attention.py) -----------------------------------------------------------------
 size_t esmb200_tied_row_attention_scratch_bytes(int32_t B, int32_t C, int32_t H) {
-  const size_t Cp = align_up((size_t)C, 64);
-  return align_up((size_t)H * B * C * C * 4, 1024) + align_up((size_t)H * B * C * Cp * 2, 1024) + 2048;
+  return tied_scratch_bytes(B, C, H, 0);
+}
+
+size_t esmb200_tied_row_attention_split_scratch_bytes(int32_t B, int32_t C, int32_t H) {
+  return tied_scratch_bytes(B, C, H, 1);
 }
 
 static int tied_row_impl(const void* qkv, const uint8_t* key_pad, long long key_pad_stride, void* ctx,
                          float* attn_probs, int32_t B, int32_t R, int32_t C, int32_t H, void* scratch,
-                         size_t scratch_bytes, void* stream) {
+                         size_t scratch_bytes, void* stream, bool split = false) {
   if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
   if (B <= 0 || R <= 0 || C <= 0 || H <= 0 || H > 64 || (long long)B * H > 65535)
     return fail(ESMB200_EINVAL, "bad shape");
   if (C > TIED_MAX_C) return fail(ESMB200_EINVAL, "tied row attention supports at most 1024 alignment columns");
-  if (scratch_bytes < esmb200_tied_row_attention_scratch_bytes(B, C, H))
+  if (scratch_bytes < tied_scratch_bytes(B, C, H, split))
     return fail(ESMB200_EWORKSPACE, "tied row attention scratch too small");
   int rc = check_device();
   if (rc) return rc;
@@ -833,31 +854,32 @@ static int tied_row_impl(const void* qkv, const uint8_t* key_pad, long long key_
   TiedParams tp;
   tp.B = B; tp.R = R; tp.C = C; tp.H = H; tp.E = E; tp.Cp = (int)Cp;
   tp.S = attn_probs ? attn_probs : reinterpret_cast<float*>(sp);
-  tp.P = reinterpret_cast<__half*>(sp + align_up((size_t)H * B * C * C * 4, 1024));
+  tp.P = reinterpret_cast<__half*>(sp + align_up((size_t)H * B * C * C * 4, 1024));  // [H*B*C, Cp] (split: 2*Cp)
   tp.ctx = static_cast<__half*>(ctx);
   tp.key_pad = key_pad;
   tp.key_pad_stride = key_pad_stride;
   tp.write_probs = attn_probs ? 1 : 0;
   const uint64_t rows = (uint64_t)B * R * C;
+  const uint64_t qcols = (uint64_t)(split ? 6 : 3) * E, pcols = (split ? 2 : 1) * Cp;  // split: hi | lo
   CUtensorMap tq, tk, tv, tpm;
-  if ((rc = make_tmap_f16(&tq, qkv, rows, (uint64_t)3 * E, (uint64_t)3 * E, tied_cfg::S_BM))) return rc;
-  if ((rc = make_tmap_f16(&tk, qkv, rows, (uint64_t)3 * E, (uint64_t)3 * E, tied_cfg::S_BN))) return rc;
-  if ((rc = make_tmap_f16(&tv, qkv, rows, (uint64_t)3 * E, (uint64_t)3 * E, 64))) return rc;
-  if ((rc = make_tmap_f16(&tpm, tp.P, (uint64_t)H * B * C, Cp, Cp, tied_cfg::V_BM))) return rc;
+  if ((rc = make_tmap_f16(&tq, qkv, rows, qcols, qcols, tied_cfg::S_BM))) return rc;
+  if ((rc = make_tmap_f16(&tk, qkv, rows, qcols, qcols, tied_cfg::S_BN))) return rc;
+  if ((rc = make_tmap_f16(&tv, qkv, rows, qcols, qcols, 64))) return rc;
+  if ((rc = make_tmap_f16(&tpm, tp.P, (uint64_t)H * B * C, pcols, pcols, tied_cfg::V_BM))) return rc;
   cudaError_t e;
   {
     ProfScope ps(T_TIED_SCORES, st);
-    e = launch_tied_scores(tq, tk, tp, st);
+    e = split ? launch_tied_scores<true>(tq, tk, tp, st) : launch_tied_scores<false>(tq, tk, tp, st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "tied scores launch");
   {
     ProfScope ps(T_TIED_SOFTMAX, st);
-    e = launch_tied_softmax(tp, st);
+    e = split ? launch_tied_softmax<true>(tp, st) : launch_tied_softmax<false>(tp, st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "tied softmax launch");
   {
     ProfScope ps(T_TIED_PV, st);
-    e = launch_tied_pv(tpm, tv, tp, st);
+    e = split ? launch_tied_pv<true>(tpm, tv, tp, st) : launch_tied_pv<false>(tpm, tv, tp, st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "tied update launch");
   return ESMB200_OK;
@@ -868,8 +890,14 @@ int esmb200_tied_row_attention(const void* qkv, const uint8_t* key_pad, void* ct
   return tied_row_impl(qkv, key_pad, C, ctx, attn_probs, B, R, C, H, scratch, scratch_bytes, stream);
 }
 
-int esmb200_column_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, int32_t B, int32_t R, int32_t C,
-                             int32_t H, void* scratch, void* stream) {
+int esmb200_tied_row_attention_split(const void* qkv, const uint8_t* key_pad, void* ctx, float* attn_probs, int32_t B,
+                                     int32_t R, int32_t C, int32_t H, void* scratch, size_t scratch_bytes,
+                                     void* stream) {
+  return tied_row_impl(qkv, key_pad, C, ctx, attn_probs, B, R, C, H, scratch, scratch_bytes, stream, true);
+}
+
+static int column_entry(const void* qkv, const uint8_t* pad_mask, void* ctx, int32_t B, int32_t R, int32_t C,
+                        int32_t H, void* scratch, void* stream, bool split) {
   if (!qkv || !ctx || !scratch) return fail(ESMB200_EINVAL, "null argument");
   if (B <= 0 || R <= 0 || C <= 0 || H <= 0 || H > 64) return fail(ESMB200_EINVAL, "bad shape");
   int rc = check_device();
@@ -878,11 +906,25 @@ int esmb200_column_attention(const void* qkv, const uint8_t* pad_mask, void* ctx
   const AttnScratch s = attn_scratch_layout(reinterpret_cast<uintptr_t>(scratch), B * C, R, H);
   rc = run_key_bits(pad_mask, s, B * C, R, st);
   if (rc) return rc;
-  return run_column_attention(qkv, ctx, s, B, R, C, H, st);
+  return run_column_attention(qkv, ctx, s, B, R, C, H, st, split);
+}
+
+int esmb200_column_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, int32_t B, int32_t R, int32_t C,
+                             int32_t H, void* scratch, void* stream) {
+  return column_entry(qkv, pad_mask, ctx, B, R, C, H, scratch, stream, false);
+}
+
+int esmb200_column_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, int32_t B, int32_t R, int32_t C,
+                                   int32_t H, void* scratch, void* stream) {
+  return column_entry(qkv, pad_mask, ctx, B, R, C, H, scratch, stream, true);
 }
 
 size_t esmb200_axial_workspace_bytes(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C) {
-  return axial_workspace_layout(nullptr, E, F, B, R, C).bytes;
+  return axial_workspace_layout(nullptr, E, F, B, R, C, 0).bytes;
+}
+
+size_t esmb200_axial_workspace_bytes_split(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C) {
+  return axial_workspace_layout(nullptr, E, F, B, R, C, 1).bytes;
 }
 
 // (A CUDA-graph replay of this launch sequence was measured: 20.70 vs 20.77 ms per 128 x 512 MSA — the ~2 ms between the
@@ -901,20 +943,21 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int E = col_layers[0]->E, F = col_layers[0]->F, H = col_layers[0]->H;
   if (F <= 0) return fail(ESMB200_EINVAL, "col_layers carry the feed-forward weights");
+  const int split = col_layers[0]->split;
   for (int i = 0; i < n_layers; ++i)
     if (row_layers[i]->E != E || col_layers[i]->E != E || col_layers[i]->F != F || row_layers[i]->H != H ||
         col_layers[i]->H != H)
       return fail(ESMB200_EINVAL, "layers of one stack must share E, H and F");
-  const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C);
+  for (int i = 0; i < n_layers; ++i)
+    if (row_layers[i]->split != split || col_layers[i]->split != split)
+      return fail(ESMB200_EINVAL, "the row and column layers of one stack must share one precision");
+  const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C, split);
   if (workspace_bytes < aw.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   if (E != 64 * H) return fail(ESMB200_EINVAL, "the MSA axial path needs head_dim 64");
-  for (int i = 0; i < n_layers; ++i)
-    if (row_layers[i]->split || col_layers[i]->split)
-      return fail(ESMB200_EINVAL, "the MSA axial path runs with fp16 operands only (precision 0)");
   const int M = B * R * C;
   const Workspace& ws = aw.ws;
   ActMaps am;
-  rc = make_act_maps(&am, ws, x, E, H, F, M);
+  rc = make_act_maps(&am, ws, x, E, H, F, M, split);
   if (rc) return rc;
   rc = run_key_bits(col_pad_mask, ws.as, B * C, R, st);  // column attention: B*C sequences of R keys
   if (rc) return rc;
@@ -924,16 +967,19 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     rc = attention_block(row_layers[i], x, M, 1, nullptr, nullptr, row_scale, ws, am, st, [&]() -> int {
       if (pad_mask) {
         ProfScope ps(T_KEYBITS, st);
-        zero_q_at_pads_kernel<<<(M + 7) / 8, 256, 0, st>>>(ws.qkv, pad_mask, M, E);
+        if (split)
+          zero_q_at_pads_kernel<true><<<(M + 7) / 8, 256, 0, st>>>(ws.qkv, pad_mask, M, E);
+        else
+          zero_q_at_pads_kernel<false><<<(M + 7) / 8, 256, 0, st>>>(ws.qkv, pad_mask, M, E);
         CK(cudaGetLastError());
       }
       return tied_row_impl(ws.qkv, pad_mask, (long long)R * C, ws.ctx, row_attn_out ? row_attn_out[i] : nullptr, B, R,
-                           C, H, aw.tied, aw.tied_bytes, stream);
+                           C, H, aw.tied, aw.tied_bytes, stream, split != 0);
     });
     // column attention (modules.py:208-212; axial_attention.py:182-239)
     if (!rc)
       rc = attention_block(col_layers[i], x, M, 1, nullptr, nullptr, col_layers[i]->q_scale, ws, am, st,
-                           [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st); });
+                           [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st, split != 0); });
     // feed-forward (modules.py:213-214)
     if (!rc) rc = ffn_block(col_layers[i], x, M, ws, am, st);
     if (rc) return rc;

@@ -52,7 +52,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_co
   const int w = blockIdx.x;
   const int qt = w % nqt, h = (w / nqt) % p.H, b = w / (nqt * p.H);
   const int row_base = (b / p.cols) * p.T;
-  const int x0 = (b % p.cols) * 3 * p.E + h * HEAD_COLS;
+  const int x0 = (b % p.cols) * (SPLIT ? 6 : 3) * p.E + h * HEAD_COLS;  // SPLIT: a token's qkv is 6E wide (hi | lo)
   const int part_off = SPLIT ? p.lo_off : HEAD_DIM;  // column distance of the second operand tile
   const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
 

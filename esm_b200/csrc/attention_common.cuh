@@ -20,7 +20,7 @@ struct AttnParams {
   float* row_sum;           // optional [B,H,T]: ... and row sum of exp(s - max), for the probability kernels
   int lo_off = 0;           // fp32x3 precision: column offset (elements) of the lo halves in qkv [M, 6E] (= 3E)
   int slots = 1;            // 64-wide column slots per head: 1 (head_dim <= 64) or 2 (head_dim <= 128); E = H * 64 * slots
-  int cols = 1;             // sequence s = (s / cols, s % cols) of a [B/cols, T, cols, 3E] tensor
+  int cols = 1;             // sequence s = (s / cols, s % cols) of a [B/cols, T, cols, 3E] tensor (fp32x3: 6E)
                             // (MSA column attention: the T tokens of a sequence are `cols` rows apart)
 };
 

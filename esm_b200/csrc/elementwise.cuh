@@ -300,14 +300,18 @@ __global__ void pack_head_cols_kernel(const float* __restrict__ w, __half* __res
 
 // MSA row attention: q is zeroed at padded positions before the logits are summed over the alignment rows
 // (/root/reference/esm/axial_attention.py:82-85).  qkv [M, 3E] fp16, pad [M] (1 = padding); one warp per row.
+// SPLIT (fp32x3): qkv [M, 6E] = [q k v]_hi | [q k v]_lo, and q_lo (columns [3E, 4E)) is zeroed as well.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256)
 zero_q_at_pads_kernel(__half* __restrict__ qkv, const uint8_t* __restrict__ pad, int M, int E) {
   pdl_launch_dependents();
   pdl_wait();
   const int row = blockIdx.x * 8 + threadIdx.x / 32;
   if (row >= M || !pad[row]) return;
-  uint4* q = reinterpret_cast<uint4*>(qkv + (size_t)row * 3 * E);  // E % 64 == 0: E*2 bytes is a multiple of 16
+  uint4* q = reinterpret_cast<uint4*>(qkv + (size_t)row * (SPLIT ? 6 : 3) * E);  // E % 64 == 0: 16-byte aligned
   for (int i = threadIdx.x % 32; i < E / 8; i += 32) q[i] = make_uint4(0u, 0u, 0u, 0u);
+  if constexpr (SPLIT)
+    for (int i = threadIdx.x % 32; i < E / 8; i += 32) q[3 * E / 8 + i] = make_uint4(0u, 0u, 0u, 0u);
 }
 
 // MSA Transformer embedding prologue (/root/reference/esm/model/msa_transformer.py:155-172): for every token of an

@@ -18,6 +18,9 @@ when the column attention MAPS are requested, for regrouping qkv column-major.
 Padding: the reference fills padded keys with -10000, this path gives them probability exactly 0 in the column
 attention — identical unless every key of a column is padded (there the reference averages v uniformly, this path
 returns 0); such positions are themselves padding.  head_dim 64, inference only.
+
+Precision: fp16 MMA operands by default; `MSATransformer.set_precision("fp32x3")` runs every GEMM and attention operand
+of the axial stack and the LM head as an fp16 hi | lo pair (the _split entry points; DESIGN.md section 4).
 """
 from __future__ import annotations
 
@@ -65,17 +68,32 @@ class _ResidualBlock(nn.Module):
         self.layer_norm = nn.LayerNorm(embed_dim)
 
 
-def _gemm(epi: int, a16: torch.Tensor, w16: torch.Tensor, bias: torch.Tensor, out: torch.Tensor) -> None:
+def _gemm(epi: int, a16: torch.Tensor, w16: torch.Tensor, bias: torch.Tensor, out: torch.Tensor,
+          split: bool = False) -> None:
+    """split (fp32x3): a16 [M,2K] and w16 [N,2K] are hi | lo halves along K (esmb200_gemm_split)."""
     M, K = a16.shape
     N = w16.shape[0]
-    _lib.check(_lib.load().esmb200_gemm_f16(epi, _ptr(a16), _ptr(w16), _ptr(bias), _ptr(out), M, N, K, None, None, 0, 0,
-                                            _stream()))
+    lib = _lib.load()
+    gemm = lib.esmb200_gemm_split if split else lib.esmb200_gemm_f16
+    _lib.check(gemm(epi, _ptr(a16), _ptr(w16), _ptr(bias), _ptr(out), M, N, K // 2 if split else K, None, None, 0, 0,
+                    _stream()))
 
 
-def _ln16(x: torch.Tensor, ln: nn.LayerNorm, out16: torch.Tensor) -> None:
+def _ln16(x: torch.Tensor, ln: nn.LayerNorm, out16: torch.Tensor, split: bool = False) -> None:
+    """LayerNorm -> fp16 [M,E], or with split the fp32x3 hi | lo halves [M,2E]."""
     M, E = x.shape
-    _lib.check(_lib.load().esmb200_layernorm_f16(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(out16), M, E, ln.eps,
-                                                 _stream()))
+    lib = _lib.load()
+    fn = lib.esmb200_layernorm_split if split else lib.esmb200_layernorm_f16
+    _lib.check(fn(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(out16), M, E, ln.eps, _stream()))
+
+
+def _split16(w: torch.Tensor) -> torch.Tensor:
+    """fp32 [N,K] -> fp16 [N,2K] hi | lo (esmb200_convert_split), the fp32x3 form of a GEMM weight."""
+    w = w.detach().float().contiguous()
+    N, K = w.shape
+    out = torch.empty((N, 2 * K), dtype=torch.float16, device=w.device)
+    _lib.check(_lib.load().esmb200_convert_split(_ptr(w), _ptr(out), N, K, _stream()))
+    return out
 
 
 class AxialTransformerLayer(nn.Module):
@@ -97,11 +115,12 @@ class AxialTransformerLayer(nn.Module):
         self._packed_key = None
         self._handles = None
         self._handles_key = None
+        self.precision = 0  # 0 = fp16 MMA operands, 1 = "fp32x3" (esmb200.h: esmb200_layer_weights.precision)
 
     # ---- C-ABI handles: (row attention-only layer, column attention + feed-forward layer) ----------------------
     def handles(self):
         ps = list(self.parameters())
-        key = tuple((p.data_ptr(), p._version) for p in ps)
+        key = (self.precision,) + tuple((p.data_ptr(), p._version) for p in ps)
         if self._handles is not None and key == self._handles_key:
             return self._handles
         self.release()
@@ -118,6 +137,7 @@ class AxialTransformerLayer(nn.Module):
             w = _lib.LayerWeights()
             w.embed_dim, w.num_heads, w.ffn_dim = self.embedding_dim, self.num_heads, self.ffn_embedding_dim
             w.ln_eps = attn_blk.layer_norm.eps
+            w.precision = self.precision
             w.ln1_weight, w.ln1_bias = attn_blk.layer_norm.weight.data_ptr(), attn_blk.layer_norm.bias.data_ptr()
             for n in ("q", "k", "v", "out"):
                 lin = getattr(a, n + "_proj")
@@ -151,21 +171,26 @@ class AxialTransformerLayer(nn.Module):
         except Exception:
             pass
 
-    # ---- fp16 operand copies (re-made when a parameter changes) ------------------------------------------------
+    # ---- GEMM operand copies: fp16, or fp32x3 hi | lo halves (re-made when a parameter or the precision changes) ----
     def _pack(self):
         ps = list(self.parameters())
-        key = tuple((p.data_ptr(), p._version) for p in ps)
+        key = (self.precision,) + tuple((p.data_ptr(), p._version) for p in ps)
         if self._packed is None or key != self._packed_key:
+            if self.precision:
+                op = _split16
+            else:
+                def op(w):
+                    return w.detach().half().contiguous()
+
             def qkv(a):
-                w = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0).detach().half().contiguous()
+                w = op(torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0))
                 b = torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias], 0).detach().float().contiguous()
                 return w, b
             row, col, ffn = self.row_self_attention.layer, self.column_self_attention.layer, self.feed_forward_layer.layer
             self._packed = {
                 "row_qkv": qkv(row), "col_qkv": qkv(col),
-                "row_out": row.out_proj.weight.detach().half().contiguous(),
-                "col_out": col.out_proj.weight.detach().half().contiguous(),
-                "fc1": ffn.fc1.weight.detach().half().contiguous(), "fc2": ffn.fc2.weight.detach().half().contiguous(),
+                "row_out": op(row.out_proj.weight), "col_out": op(col.out_proj.weight),
+                "fc1": op(ffn.fc1.weight), "fc2": op(ffn.fc2.weight),
             }
             self._packed_key = key
         return self._packed
@@ -187,13 +212,25 @@ class AxialTransformerLayer(nn.Module):
             return out, col_probs, row_probs
         return out
 
+    def _qkv(self, xn: torch.Tensor, w: torch.Tensor, b: torch.Tensor, qkv: torch.Tensor, M: int, E: int,
+             q_scale: float) -> None:
+        """The q/k/v projection without rotary embedding, q columns scaled by q_scale (axial_attention.py:79-81,
+        199-202): qkv [M,3E] fp16, or [M,6E] hi | lo with fp32x3."""
+        lib = _lib.load()
+        if self.precision:
+            _lib.check(lib.esmb200_gemm_qkv_split(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, q_scale, _stream()))
+        else:
+            _lib.check(lib.esmb200_gemm_qkv_f16(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, q_scale, None, None, 0,
+                                                _stream()))
+
     @torch.no_grad()
     def forward_batch_major(self, xb: torch.Tensor, padding_mask: Optional[torch.Tensor] = None,
                             need_probs: bool = False):
         """In-place layer on the batch-major residual stream xb [B,R,C,E] fp32 (what MSATransformer keeps between
         layers).  padding_mask [B,R,C] bool or None.  Returns (row_attn [H,B,C,C], column_attn [H,C,B,R,R]) or
         (None, None).  Without attention maps this is one esmb200_axial_stack_forward call; with them the sub-layers
-        are driven one C-ABI call at a time so that the column-attention maps can be produced too."""
+        are driven one C-ABI call at a time so that the column-attention maps can be produced too.  With precision 1
+        (fp32x3) every GEMM / attention operand below is an fp16 hi | lo pair, twice as wide."""
         if not need_probs:
             run_axial_stack([self], xb, padding_mask)
             return None, None
@@ -202,11 +239,13 @@ class AxialTransformerLayer(nn.Module):
         H, d, Fd = self.num_heads, 64, self.ffn_embedding_dim
         M = B * R * C
         dev = xb.device
+        split = bool(self.precision)
+        pf = 2 if split else 1
         pk = self._pack()
         x2 = xb.view(M, E)
-        xn = torch.empty((M, E), dtype=torch.float16, device=dev)
-        qkv = torch.empty((M, 3 * E), dtype=torch.float16, device=dev)
-        ctx = torch.empty((M, E), dtype=torch.float16, device=dev)
+        xn = torch.empty((M, pf * E), dtype=torch.float16, device=dev)
+        qkv = torch.empty((M, pf * 3 * E), dtype=torch.float16, device=dev)
+        ctx = torch.empty((M, pf * E), dtype=torch.float16, device=dev)
         key_pad = col_pad = None
         if padding_mask is not None:
             pm = padding_mask.to(device=dev, dtype=torch.bool)
@@ -215,41 +254,48 @@ class AxialTransformerLayer(nn.Module):
         with torch.cuda.device(dev):
             # ================= tied row attention (axial_attention.py:71-111) =================
             blk = self.row_self_attention
-            _ln16(x2, blk.layer_norm, xn)
+            _ln16(x2, blk.layer_norm, xn, split)
             w, b = pk["row_qkv"]
-            _lib.check(lib.esmb200_gemm_qkv_f16(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E,
-                                                (d ** -0.5) / math.sqrt(R), None, None, 0, _stream()))
-            if padding_mask is not None:  # q zeroed at padded positions (:82-85)
-                qkv.view(B, R, C, 3, E)[:, :, :, 0].masked_fill_(pm[..., None], 0)
+            self._qkv(xn, w, b, qkv, M, E, (d ** -0.5) / math.sqrt(R))
+            if padding_mask is not None:  # q (both halves with fp32x3) zeroed at padded positions (:82-85)
+                q5 = qkv.view(B, R, C, 3 * pf, E)
+                q5[:, :, :, 0].masked_fill_(pm[..., None], 0)
+                if split:
+                    q5[:, :, :, 3].masked_fill_(pm[..., None], 0)
             row_probs = torch.empty((H, B, C, C), dtype=torch.float32, device=dev)
-            nbytes = lib.esmb200_tied_row_attention_scratch_bytes(B, C, H)
+            if split:
+                nbytes = lib.esmb200_tied_row_attention_split_scratch_bytes(B, C, H)
+                tied = lib.esmb200_tied_row_attention_split
+            else:
+                nbytes = lib.esmb200_tied_row_attention_scratch_bytes(B, C, H)
+                tied = lib.esmb200_tied_row_attention
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _lib.check(lib.esmb200_tied_row_attention(_ptr(qkv), _ptr(key_pad), _ptr(ctx), _ptr(row_probs), B, R, C, H,
-                                                      _ptr(scratch), nbytes, _stream()))
-            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["row_out"], blk.layer.out_proj.bias, x2)            # :110 + residual
+            _lib.check(tied(_ptr(qkv), _ptr(key_pad), _ptr(ctx), _ptr(row_probs), B, R, C, H, _ptr(scratch), nbytes,
+                            _stream()))
+            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["row_out"], blk.layer.out_proj.bias, x2, split)     # :110 + residual
 
             # ================= column attention (axial_attention.py:182-222) =================
             blk = self.column_self_attention
-            _ln16(x2, blk.layer_norm, xn)
+            _ln16(x2, blk.layer_norm, xn, split)
             w, b = pk["col_qkv"]
-            _lib.check(lib.esmb200_gemm_qkv_f16(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, d ** -0.5, None, None, 0,
-                                                _stream()))
+            self._qkv(xn, w, b, qkv, M, E, d ** -0.5)
             scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B * C, R), dtype=torch.uint8, device=dev)
             # the maps are wanted: regroup qkv column-major and use the probability-writing path
-            qkv_t = qkv.view(B, R, C, 3 * E).permute(0, 2, 1, 3).contiguous()                      # [B*C, R, 3E]
-            ctx_t = torch.empty((B * C * R, E), dtype=torch.float16, device=dev)
+            qkv_t = qkv.view(B, R, C, pf * 3 * E).permute(0, 2, 1, 3).contiguous()             # [B*C, R, 3E] (6E)
+            ctx_t = torch.empty((B * C * R, pf * E), dtype=torch.float16, device=dev)
             col_probs = torch.empty((B * C, H, R, R), dtype=torch.float32, device=dev)
-            _lib.check(lib.esmb200_attention(_ptr(qkv_t), _ptr(col_pad), _ptr(ctx_t), _ptr(col_probs), B * C, R, H,
-                                             _ptr(scratch), _stream()))
-            ctx.view(B, R, C, E).copy_(ctx_t.view(B, C, R, E).permute(0, 2, 1, 3))
-            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["col_out"], blk.layer.out_proj.bias, x2)
+            attention = lib.esmb200_attention_split if split else lib.esmb200_attention
+            _lib.check(attention(_ptr(qkv_t), _ptr(col_pad), _ptr(ctx_t), _ptr(col_probs), B * C, R, H, _ptr(scratch),
+                                 _stream()))
+            ctx.view(B, R, C, pf * E).copy_(ctx_t.view(B, C, R, pf * E).permute(0, 2, 1, 3))
+            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["col_out"], blk.layer.out_proj.bias, x2, split)
 
             # ================= feed-forward (modules.py:413-418) =================
             blk = self.feed_forward_layer
-            _ln16(x2, blk.layer_norm, xn)
-            hbuf = torch.empty((M, Fd), dtype=torch.float16, device=dev)
-            _gemm(_lib.EPI_BIAS_GELU, xn, pk["fc1"], blk.layer.fc1.bias, hbuf)
-            _gemm(_lib.EPI_BIAS_RESIDUAL, hbuf, pk["fc2"], blk.layer.fc2.bias, x2)
+            _ln16(x2, blk.layer_norm, xn, split)
+            hbuf = torch.empty((M, pf * Fd), dtype=torch.float16, device=dev)
+            _gemm(_lib.EPI_BIAS_GELU, xn, pk["fc1"], blk.layer.fc1.bias, hbuf, split)
+            _gemm(_lib.EPI_BIAS_RESIDUAL, hbuf, pk["fc2"], blk.layer.fc2.bias, x2, split)
         # reference shapes: column_attn [H, C, B, R, R] (axial_attention.py:206), row_attn [H, B, C, C] (:87)
         col_probs = col_probs.view(B, C, H, R, R).permute(2, 1, 0, 3, 4).contiguous()
         return row_probs, col_probs
@@ -271,7 +317,10 @@ def run_axial_stack(layers: Sequence[AxialTransformerLayer], xb: torch.Tensor,
         hs = [l.handles() for l in layers]
         rows = (ctypes.c_void_p * n)(*[h[0] for h in hs])
         cols = (ctypes.c_void_p * n)(*[h[1] for h in hs])
-        nbytes = lib.esmb200_axial_workspace_bytes(E, Fd, B, R, C)
+        if layers[0].precision:  # every layer of one call shares the precision (EINVAL otherwise)
+            nbytes = lib.esmb200_axial_workspace_bytes_split(E, Fd, B, R, C)
+        else:
+            nbytes = lib.esmb200_axial_workspace_bytes(E, Fd, B, R, C)
         ws = _workspace(nbytes, dev)
         pm = cm = None
         if padding_mask is not None:
@@ -346,8 +395,24 @@ class MSATransformer(nn.Module):
         self.emb_layer_norm_before = nn.LayerNorm(E)
         self.emb_layer_norm_after = nn.LayerNorm(E)
         self.lm_head = RobertaLMHead(embed_dim=E, output_dim=self.alphabet_size, weight=self.embed_tokens.weight)
+        self.precision = "fp16"
 
     contacts_without_col_attentions = False  # True: return_contacts alone does not materialise col_attentions
+
+    PRECISIONS = {"fp16": 0, "fp32x3": 1}
+
+    def set_precision(self, name: str) -> "MSATransformer":
+        """"fp16" (default): fp16 MMA operands, fp32 accumulation — the fast path.
+        "fp32x3": every MMA operand of the axial stack and the LM head (LayerNorm outputs, weights, q, k, v, the tied
+        row-attention and column-attention probabilities, context, FFN hidden) is an fp16 hi + lo pair and every product
+        runs hi*hi + lo*hi + hi*lo into the fp32 accumulator: fp32-grade parity with the reference at several times the
+        tensor work (DESIGN.md sections 4 and 6)."""
+        if name not in self.PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(self.PRECISIONS)}")
+        self.precision = name
+        for layer in self.layers:
+            layer.precision = self.PRECISIONS[name]
+        return self
 
     @property
     def num_layers(self) -> int:
@@ -370,7 +435,8 @@ class MSATransformer(nn.Module):
         dev = tokens.device
         with torch.cuda.device(dev):
             ln = self.emb_layer_norm_after
-            logits = self.lm_head.forward_native(x.view(B, R * C, E), ln.weight, ln.bias, ln.eps).view(B, R, C, -1)
+            logits = self.lm_head.forward_native(x.view(B, R * C, E), ln.weight, ln.bias, ln.eps,
+                                                 self.PRECISIONS[self.precision]).view(B, R, C, -1)
             _lib.check(lib.esmb200_layernorm(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(x), B * R * C, E, ln.eps,
                                              _stream()))
         if N in repr_layers:
@@ -389,7 +455,8 @@ class MSATransformer(nn.Module):
     def _lm_head_rows(self, x_rows: torch.Tensor) -> torch.Tensor:
         """The LM head (msa_transformer.py:204-210) on selected rows [n,E] of the pre-LN stream: fp32 logits [n,V]."""
         ln = self.emb_layer_norm_after
-        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln.weight, ln.bias, ln.eps)[0]
+        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln.weight, ln.bias, ln.eps,
+                                           self.PRECISIONS[self.precision])[0]
 
     def _stack(self, tokens, repr_layers=frozenset(), need_head_weights=False, return_contacts=False):
         """The stack step of `forward` (msa_transformer.py:147-201): embedding prologue and the axial layers.

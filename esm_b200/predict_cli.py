@@ -8,6 +8,7 @@ predict.py:45-104, plus --max-tokens) on the library's batched scorers (esm_b200
   * output: predict.py's table (df.to_csv): a leading unnamed index column, the input columns as read, then one
     column per --model-location named by the location string. It is written with the csv module: the input cells are
     copied unchanged, the scores written with repr. Neither pandas nor Biopython is needed.
+  * --precision fp32x3 runs every model (sequence models and the MSA Transformer) with fp16 hi + lo operand pairs.
   * there is no CPU path: --nogpu raises.
 """
 from __future__ import annotations
@@ -23,11 +24,12 @@ import torch
 from . import pretrained, variants
 
 STRATEGIES = ["wt-marginals", "pseudo-ppl", "masked-marginals"]
+PRECISIONS = ["fp16", "fp32x3"]
 MSA_ONLY_MASKED = "MSA Transformer only supports masked marginal strategy"  # predict.py:163-165
 
 
 def create_parser():
-    """The flags, defaults and choices of predict.py:45-104, plus --max-tokens."""
+    """The flags, defaults and choices of predict.py:45-104, plus --max-tokens and --precision."""
     p = argparse.ArgumentParser(description="Score the single mutants of a deep mutational scan with one or more ESM "
                                             "models on the GPU and write the table back with one score column per "
                                             "model")
@@ -48,6 +50,9 @@ def create_parser():
     p.add_argument("--nogpu", action="store_true", help="accepted for compatibility; raises, as there is no CPU path")
     p.add_argument("--max-tokens", type=int, default=variants.DEFAULT_MAX_TOKENS,
                    help="tokens per batched forward of masked copies (at least one copy per forward)")
+    p.add_argument("--precision", choices=PRECISIONS, default="fp16",
+                   help="fp16: fp16 MMA operands (default, fastest); fp32x3: hi+lo operand pairs, fp32-grade scores "
+                        "(slower); applies to every model location")
     return p
 
 
@@ -132,6 +137,8 @@ def run(args) -> None:
         if getattr(model, "random_init", False):
             raise RuntimeError("refusing to score variants with a random-init model: give --model-location a checkpoint")
         model = model.eval().cuda()
+        if getattr(args, "precision", "fp16") != "fp16":
+            model.set_precision(args.precision)
         scores[location] = score_model(model, alphabet, is_msa, args, mutations)
         del model
         gc.collect()

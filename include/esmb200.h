@@ -74,7 +74,8 @@ typedef struct esmb200_layer_weights {
   int32_t precision;       /* 0 = fp16 MMA operands (default). 1 = "fp32x3": every MMA operand (activations, weights,
                             * q, k, v, P) is an fp16 hi | lo pair and every product runs hi*hi + lo*hi + hi*lo into the
                             * fp32 accumulator (22 significand bits per operand) — fp32-grade results at ~3x the tensor
-                            * work; needs E % 64 == 0 and head_dim <= 64; not available on the MSA axial path */
+                            * work; needs E % 64 == 0 and head_dim <= 64. On the MSA axial path every row and
+                            * column layer of one esmb200_axial_stack_forward call must share the precision */
 } esmb200_layer_weights;
 
 int esmb200_abi_version(void);
@@ -220,8 +221,11 @@ int esmb200_column_attention(const void* qkv_f16, const uint8_t* pad_mask, void*
  * pad_mask [B,R,C] and col_pad_mask [B,C,R] (its transpose): 1 = padding, both NULL for unpadded alignments.
  * row_attn_out: NULL, or n_layers pointers (NULL entries allowed) to fp32 [H,B,C,C] buffers (the reference's
  *   row-attention return layout, axial_attention.py:87,105). Column attention maps are not produced by this call.
- * workspace: esmb200_axial_workspace_bytes(E,F,B,R,C) bytes. */
+ * workspace: esmb200_axial_workspace_bytes(E,F,B,R,C) bytes, or esmb200_axial_workspace_bytes_split(E,F,B,R,C) for
+ *   layers created with precision = 1 (fp32x3: the activations, qkv, ctx and P are stored as fp16 hi | lo pairs).
+ *   All 2 * n_layers layers must share one precision; mixed precision is ESMB200_EINVAL. */
 size_t esmb200_axial_workspace_bytes(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C);
+size_t esmb200_axial_workspace_bytes_split(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C);
 int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer* const* col_layers, int32_t n_layers,
                                 float* x, const uint8_t* pad_mask, const uint8_t* col_pad_mask, int32_t B, int32_t R,
                                 int32_t C, float* const* row_attn_out, void* workspace, size_t workspace_bytes,
@@ -272,12 +276,22 @@ int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
 /* fp32 -> fp16 elementwise */
 int esmb200_convert_f16(const float* src, void* dst_f16, size_t n, void* stream);
 
-/* ---- fp32x3 precision building blocks (operands as fp16 hi | lo pairs along K): the LM head and kernel-level tests.
+/* ---- fp32x3 precision building blocks (operands as fp16 hi | lo pairs along K): the LM head, the MSA layer's
+ * attention-map path (esm_b200/msa.py) and kernel-level tests.
  * esmb200_layernorm_split: fp32 [M,E] -> LayerNorm -> fp16 [M,2E] (hi in columns [0,E), lo = rn(y - hi) in [E,2E)).
  * esmb200_convert_split:   fp32 [rows,K] -> fp16 [rows,2K] the same way (weights).
  * esmb200_gemm_split:      esmb200_gemm_f16 with a [M,2K], w [N,2K]; fp16 outputs (QKV_ROPE, BIAS_GELU) are written as
  *                          [M,2N] hi | lo, fp32 outputs as [M,N].  K % 64 == 0.
- * esmb200_attention_split: esmb200_attention on qkv [B*T, 6E] = [q k v]_hi | [q k v]_lo -> ctx [B*T, 2E] hi | lo. */
+ * esmb200_attention_split: esmb200_attention on qkv [B*T, 6E] = [q k v]_hi | [q k v]_lo -> ctx [B*T, 2E] hi | lo.
+ * esmb200_gemm_qkv_split:  esmb200_gemm_qkv_f16 without rope tables (the MSA axial attention): a [M,2E], w_qkv [3E,2E]
+ *                          (esmb200_convert_split of [Wq;Wk;Wv]), q columns scaled by q_scale -> qkv [M,6E] hi | lo.
+ *                          E % 64 == 0.
+ * esmb200_tied_row_attention_split: esmb200_tied_row_attention on qkv [B*R*C, 6E] -> ctx [B*R*C, 2E] hi | lo; the
+ *                          logits sum each alignment row's 64-wide slab in a fresh fp32 fragment; attn_probs as in
+ *                          the fp16 call. The caller zeroes q_hi AND q_lo at padded positions. scratch:
+ *                          esmb200_tied_row_attention_split_scratch_bytes(B,C,H) (P is stored as hi | lo).
+ * esmb200_column_attention_split: esmb200_column_attention on qkv [B*R*C, 6E] -> ctx [B*R*C, 2E] hi | lo; scratch:
+ *                          esmb200_attention_scratch_bytes(B*C, R). */
 int esmb200_layernorm_split(const float* x, const float* weight, const float* bias, void* out_f16, int32_t M, int32_t E,
                             float eps, void* stream);
 int esmb200_convert_split(const float* src, void* dst_f16, int64_t rows, int32_t K, void* stream);
@@ -286,6 +300,14 @@ int esmb200_gemm_split(int32_t epilogue, const void* a, const void* w, const flo
                        void* stream);
 int esmb200_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,
                             int32_t H, void* scratch, void* stream);
+int esmb200_gemm_qkv_split(const void* a, const void* w_qkv, const float* bias_qkv, void* out, int32_t M, int32_t E,
+                           float q_scale, void* stream);
+size_t esmb200_tied_row_attention_split_scratch_bytes(int32_t B, int32_t C, int32_t H);
+int esmb200_tied_row_attention_split(const void* qkv, const uint8_t* key_pad, void* ctx, float* attn_probs, int32_t B,
+                                     int32_t R, int32_t C, int32_t H, void* scratch, size_t scratch_bytes,
+                                     void* stream);
+int esmb200_column_attention_split(const void* qkv, const uint8_t* pad_mask, void* ctx, int32_t B, int32_t R, int32_t C,
+                                   int32_t H, void* scratch, void* stream);
 
 /* ---- process-wide launch knobs (A/B measurements; the defaults are the product configuration) ----
  * "pdl"       0 (default) | 1: programmatic dependent launch between the layer's kernels        env ESMB200_PDL
