@@ -56,6 +56,9 @@ EXPORTS = (
     "esmb200_tied_row_attention_split_scratch_bytes",
     "esmb200_tied_row_attention_split",
     "esmb200_column_attention_split",
+    "esmb200_layer_packed_bytes",
+    "esmb200_layer_offload",
+    "esmb200_stack_forward_streamed",
 )
 
 ABI_VERSION = 2
@@ -123,6 +126,15 @@ def _declare(lib):
     lib.esmb200_stack_forward.argtypes = [POINTER(c_void_p), c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
                                           c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int64, c_int32,
                                           POINTER(ContactJob), c_void_p, c_size_t, c_void_p]
+    lib.esmb200_layer_packed_bytes.restype = c_size_t
+    lib.esmb200_layer_packed_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32]
+    lib.esmb200_layer_offload.restype = c_int32
+    lib.esmb200_layer_offload.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p]
+    lib.esmb200_stack_forward_streamed.restype = c_int32
+    lib.esmb200_stack_forward_streamed.argtypes = [POINTER(c_void_p), c_int32, c_void_p, c_void_p, c_int32, c_int32,
+                                                   c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int64,
+                                                   c_int32, POINTER(ContactJob), c_void_p, c_size_t, c_void_p,
+                                                   c_size_t, c_void_p, c_void_p]
     lib.esmb200_embed_tokens.restype = c_int32
     lib.esmb200_embed_tokens.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                          c_int32, c_void_p]

@@ -364,6 +364,10 @@ int convert_f16(const float* src, void* dst, size_t rows, int K, bool split, cud
 // ---------------------------------------------------------------------------------------------------------------
 // layer object
 // ---------------------------------------------------------------------------------------------------------------
+struct WeightMaps {
+  CUtensorMap qkv, out, fc1, fc2;  // B operands, box {64, 128 rows}
+};
+
 struct esmb200_layer {
   int E, H, F;
   int d;          // head_dim (<= 128); every head occupies `slots` 64-wide slots of the attention-side tensors
@@ -380,10 +384,42 @@ struct esmb200_layer {
   __half* w_fc1;  // [F,E]
   __half* w_fc2;  // [E,F]
   float* b_qkv;   // [3*Ea]
-  CUtensorMap tm_qkv, tm_out, tm_fc1, tm_fc2;  // B operands, box {64, 128 rows}
+  WeightMaps tm;  // of w_qkv .. w_fc2; zero once offloaded
+  // esmb200_layer_offload: the caller's pinned copy of w_qkv .. w_fc2 in the packed_layout() arrangement; the device
+  // copies are freed and the layer runs only in esmb200_stack_forward_streamed
+  const void* host;
 };
 
 namespace {
+// one layer's packed matrices back to back, 1024-aligned: the layout of its host copy and of one ring slot
+struct PackedLayout {
+  size_t qkv, out, fc1, fc2;  // byte offsets
+  size_t bytes;
+};
+
+PackedLayout packed_layout(int E, int H, int F, int split) {
+  const size_t pf = split ? 2 : 1, Ea = (size_t)64 * head_slots(E, H) * H;
+  PackedLayout p;
+  p.qkv = 0;
+  p.out = align_up(3 * Ea * E * 2 * pf, 1024);
+  p.fc1 = p.out + align_up(Ea * E * 2 * pf, 1024);
+  p.fc2 = p.fc1 + align_up((size_t)F * E * 2 * pf, 1024);
+  p.bytes = p.fc2 + align_up((size_t)E * F * 2 * pf, 1024);
+  return p;
+}
+
+// B-operand maps of a layer's packed matrices (fc1 == nullptr: attention-only layer)
+int make_weight_maps(WeightMaps* m, const __half* qkv, const __half* out, const __half* fc1, const __half* fc2, int E,
+                     int Ea, int F, int split) {
+  const uint64_t pf = split ? 2 : 1;
+  const uint32_t wbox = gemm2_cfg::HALF_N;
+  int rc = make_tmap_f16(&m->qkv, qkv, 3 * (uint64_t)Ea, pf * E, pf * E, wbox);
+  if (!rc) rc = make_tmap_f16(&m->out, out, E, pf * Ea, pf * Ea, wbox);
+  if (!rc && fc1) rc = make_tmap_f16(&m->fc1, fc1, F, pf * E, pf * E, wbox);
+  if (!rc && fc1) rc = make_tmap_f16(&m->fc2, fc2, E, pf * F, pf * F, wbox);
+  return rc;
+}
+
 struct Workspace {
   __half* xn;
   __half* qkv;
@@ -417,31 +453,34 @@ struct ActMaps {
 
 // x += out_proj(attend()) after LN1 -> fp16 and the q,k,v projection (+ bias, q scale, RoPE when rope_cos is given):
 // the self-attention half of an ESM-2 layer (multihead_attention.py:258-261,354-355,395; modules.py:124-134) and each
-// axial attention sub-layer of the MSA stack.  `attend` reads ws.qkv and writes ws.ctx.
+// axial attention sub-layer of the MSA stack.  `attend` reads ws.qkv and writes ws.ctx.  The weights are read through
+// `wm`: the layer's own maps (L->tm), or those of the ring slot its packed matrices were streamed into.
 template <class Attend>
-int attention_block(const esmb200_layer* L, float* x, int M, int T, const float* rope_cos, const float* rope_sin,
-                    float q_scale, const Workspace& ws, const ActMaps& am, cudaStream_t st, Attend attend) {
+int attention_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int M, int T, const float* rope_cos,
+                    const float* rope_sin, float q_scale, const Workspace& ws, const ActMaps& am, cudaStream_t st,
+                    Attend attend) {
   const bool split = L->split != 0;
   int rc = layernorm_f16(x, L->ln1_w, L->ln1_b, ws.xn, M, L->E, L->eps, split, T_LN1, st);
   if (rc) return rc;
   GemmParams g = gemm_params(M, 3 * L->Ea, L->E, L->b_qkv);
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.rope_ld = 32 * L->slots; g.T = T; g.E = L->Ea; g.q_scale = q_scale;
   g.lo_col_off = 3 * L->Ea;
-  if ((rc = launch_gemm(EPI_QKV_ROPE, am.xn, L->tm_qkv, am.qkv_o, g, st, T_QKV, split))) return rc;
+  if ((rc = launch_gemm(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, g, st, T_QKV, split))) return rc;
   if ((rc = attend())) return rc;
-  return launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, L->tm_out, am.x_o, gemm_params(M, L->E, L->Ea, L->out_b), st, T_OUT,
+  return launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, wm.out, am.x_o, gemm_params(M, L->E, L->Ea, L->out_b), st, T_OUT,
                      split);
 }
 
 // x += fc2(GELU(fc1(LN2(x)))) (modules.py:137-140, 413-418)
-int ffn_block(const esmb200_layer* L, float* x, int M, const Workspace& ws, const ActMaps& am, cudaStream_t st) {
+int ffn_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int M, const Workspace& ws, const ActMaps& am,
+              cudaStream_t st) {
   const bool split = L->split != 0;
   int rc = layernorm_f16(x, L->ln2_w, L->ln2_b, ws.xn, M, L->E, L->eps, split, T_LN2, st);
   if (rc) return rc;
   GemmParams g = gemm_params(M, L->F, L->E, L->fc1_b);
   g.lo_col_off = L->F;
-  if ((rc = launch_gemm(EPI_BIAS_GELU, am.xn, L->tm_fc1, am.h_o, g, st, T_FC1, split))) return rc;
-  return launch_gemm(EPI_BIAS_RESIDUAL, am.h, L->tm_fc2, am.x_o, gemm_params(M, L->E, L->F, L->fc2_b), st, T_FC2,
+  if ((rc = launch_gemm(EPI_BIAS_GELU, am.xn, wm.fc1, am.h_o, g, st, T_FC1, split))) return rc;
+  return launch_gemm(EPI_BIAS_RESIDUAL, am.h, wm.fc2, am.x_o, gemm_params(M, L->E, L->F, L->fc2_b), st, T_FC2,
                      split);
 }
 
@@ -527,6 +566,41 @@ AxialWorkspace axial_workspace_layout(void* workspace, int E, int F, int B, int 
   a.bytes = a.ws.bytes + a.tied_bytes + 1024;
   return a;
 }
+
+// esmb200_stack_forward_streamed: two device slots that the offloaded layers' packed matrices are copied into on `copy`
+// (layer i into slot i % 2), with the events that order the copies against the layers reading the slots
+struct WeightRing {
+  cudaStream_t st = nullptr, copy = nullptr;
+  uint8_t* slot[2] = {};
+  size_t bytes = 0;               // one layer's packed matrices
+  WeightMaps maps[2];
+  cudaEvent_t copied[2] = {}, freed[2] = {}, mark = nullptr;
+  // the caller's stream waits for the last copy: an error can leave the layer loop before the wait for a copy that
+  // is still writing the ring, which the caller may free or reuse in stream order once the call returns
+  ~WeightRing() {
+    if (mark && cudaEventRecord(mark, copy) == cudaSuccess) cudaStreamWaitEvent(st, mark, 0);
+    for (cudaEvent_t e : {copied[0], copied[1], freed[0], freed[1], mark})
+      if (e) cudaEventDestroy(e);
+  }
+  int init(uint8_t* ring, size_t layer_bytes, cudaStream_t stream, cudaStream_t copy_stream) {
+    st = stream; copy = copy_stream; bytes = layer_bytes;
+    slot[0] = ring; slot[1] = ring + layer_bytes;
+    for (cudaEvent_t* e : {&copied[0], &copied[1], &freed[0], &freed[1], &mark})
+      CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    // a previous call on `stream` may still be reading a slot of the same ring
+    CK(cudaEventRecord(mark, st));
+    CK(cudaStreamWaitEvent(copy, mark, 0));
+    return ESMB200_OK;
+  }
+  // layer i's packed matrices -> slot i % 2, once layer i - 2 (the last reader of that slot) has run
+  int fetch(const esmb200_layer* L, int i) {
+    const int s = i & 1;
+    if (i >= 2) CK(cudaStreamWaitEvent(copy, freed[s], 0));
+    CK(cudaMemcpyAsync(slot[s], L->host, bytes, cudaMemcpyHostToDevice, copy));
+    CK(cudaEventRecord(copied[s], copy));
+    return ESMB200_OK;
+  }
+};
 }  // namespace
 
 extern "C" {
@@ -616,11 +690,7 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   }
   if (!rc && has_ffn) rc = convert_f16(w->fc1_weight, L->w_fc1, F, E, split, st);
   if (!rc && has_ffn) rc = convert_f16(w->fc2_weight, L->w_fc2, E, F, split, st);
-  const uint32_t wbox = gemm2_cfg::HALF_N;
-  if (!rc) rc = make_tmap_f16(&L->tm_qkv, L->w_qkv, 3 * (uint64_t)Ea, pf * E, pf * E, wbox);
-  if (!rc) rc = make_tmap_f16(&L->tm_out, L->w_out, E, pf * Ea, pf * Ea, wbox);
-  if (!rc && has_ffn) rc = make_tmap_f16(&L->tm_fc1, L->w_fc1, F, pf * E, pf * E, wbox);
-  if (!rc && has_ffn) rc = make_tmap_f16(&L->tm_fc2, L->w_fc2, E, pf * F, pf * F, wbox);
+  if (!rc) rc = make_weight_maps(&L->tm, L->w_qkv, L->w_out, L->w_fc1, L->w_fc2, E, Ea, L->F, split);
   if (rc) {
     esmb200_layer_destroy(L);
     return rc;
@@ -639,12 +709,51 @@ size_t esmb200_workspace_bytes(int32_t E, int32_t H, int32_t F, int32_t B, int32
   return workspace_layout(nullptr, E, H, F, B, T, precision).bytes;
 }
 
-int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
-                          int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
-                          float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
-                          int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
-                          size_t workspace_bytes, void* stream) {
+size_t esmb200_layer_packed_bytes(int32_t E, int32_t H, int32_t F, int32_t precision) {
+  if (E <= 0 || H <= 0 || F <= 0 || E % H != 0 || E / H > 128 || (precision != 0 && precision != 1)) return 0;
+  return packed_layout(E, H, F, precision).bytes;
+}
+
+int esmb200_layer_offload(esmb200_layer* L, void* host_dst, size_t bytes, void* stream) {
+  if (!L || !host_dst) return fail(ESMB200_EINVAL, "null argument");
+  if (L->host) return fail(ESMB200_EINVAL, "layer is already offloaded");
+  if (L->F <= 0) return fail(ESMB200_EINVAL, "attention-only layers cannot be offloaded");
+  const PackedLayout p = packed_layout(L->E, L->H, L->F, L->split);
+  if (bytes < p.bytes) return fail(ESMB200_EINVAL, "host buffer smaller than esmb200_layer_packed_bytes");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaPointerAttributes pa;
+  if (cudaPointerGetAttributes(&pa, host_dst) != cudaSuccess || pa.type != cudaMemoryTypeHost) {
+    cudaGetLastError();
+    return fail(ESMB200_EINVAL, "host_dst must be pinned host memory (cudaHostAlloc / cudaHostRegister)");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* h = static_cast<uint8_t*>(host_dst);
+  const size_t pf = L->split ? 2 : 1, EaE = (size_t)L->Ea * L->E, EF = (size_t)L->E * L->F;
+  CK(cudaMemcpyAsync(h + p.qkv, L->w_qkv, 3 * EaE * 2 * pf, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h + p.out, L->w_out, EaE * 2 * pf, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h + p.fc1, L->w_fc1, EF * 2 * pf, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h + p.fc2, L->w_fc2, EF * 2 * pf, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));  // the copies read what is freed below
+  for (__half** w : {&L->w_qkv, &L->w_out, &L->w_fc1, &L->w_fc2}) {
+    cudaFree(*w);
+    *w = nullptr;
+  }
+  memset(&L->tm, 0, sizeof L->tm);
+  L->host = host_dst;
+  return ESMB200_OK;
+}
+
+// the layer loop of esmb200_stack_forward (ring == nullptr: every layer's weights resident) and of
+// esmb200_stack_forward_streamed (every layer offloaded, its packed matrices copied into `ring` ahead of use)
+static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
+                              int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
+                              float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
+                              int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
+                              size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream, void* stream) {
   if (!layers || n_layers <= 0 || !x || !workspace) return fail(ESMB200_EINVAL, "null argument");
+  for (int i = 0; i < n_layers; ++i)
+    if (!layers[i]) return fail(ESMB200_EINVAL, "null layer");
   if ((rope_cos == nullptr) != (rope_sin == nullptr))  // both NULL: no rotary embedding (ESM-1b / ESM-1v)
     return fail(ESMB200_EINVAL, "rope_cos and rope_sin must both be given or both be NULL");
   if (contact) {
@@ -665,17 +774,46 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
   for (int i = 1; i < n_layers; ++i)
     if (layers[i]->E != E || layers[i]->F != F || layers[i]->H != H || layers[i]->split != layers[0]->split)
       return fail(ESMB200_EINVAL, "layers of one stack must share E, H, F and precision");
+  const bool streamed = ring != nullptr;
+  for (int i = 0; i < n_layers; ++i)
+    if ((layers[i]->host != nullptr) != streamed)
+      return fail(ESMB200_EINVAL, "layer " + std::to_string(i) +
+                                      (streamed ? " is not offloaded: esmb200_stack_forward_streamed runs layers "
+                                                  "whose weights esmb200_layer_offload moved to host memory"
+                                                : " is offloaded to host memory (esmb200_layer_offload): run it with "
+                                                  "esmb200_stack_forward_streamed"));
   const int split = layers[0]->split;
   const Workspace ws = workspace_layout(workspace, E, H, F, B, T, split);
   if (workspace_bytes < ws.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   ActMaps am;
   rc = make_act_maps(&am, ws, x, E, H, F, B * T, split);
   if (rc) return rc;
+  WeightRing wr;
+  if (streamed) {
+    const PackedLayout p = packed_layout(E, H, F, split);
+    if (ring_bytes < 2 * p.bytes) return fail(ESMB200_EINVAL, "ring smaller than 2 * esmb200_layer_packed_bytes");
+    uint8_t* base = static_cast<uint8_t*>(ring);
+    const int Ea = layers[0]->Ea;
+    for (int s = 0; s < 2 && !rc; ++s) {
+      uint8_t* b = base + s * p.bytes;
+      rc = make_weight_maps(&wr.maps[s], reinterpret_cast<__half*>(b + p.qkv), reinterpret_cast<__half*>(b + p.out),
+                            reinterpret_cast<__half*>(b + p.fc1), reinterpret_cast<__half*>(b + p.fc2), E, Ea, F, split);
+    }
+    if (rc) return rc;
+    if ((rc = wr.init(base, p.bytes, st, static_cast<cudaStream_t>(copy_stream)))) return rc;
+    for (int i = 0; i < 2 && i < n_layers && !rc; ++i) rc = wr.fetch(layers[i], i);
+    if (rc) return rc;
+  }
   rc = run_key_bits(pad_mask, ws.as, B, T, st);
   if (rc) return rc;
   const int nt128 = (T + 127) / 128;
   for (int i = 0; i < n_layers; ++i) {
     esmb200_layer* L = layers[i];
+    const WeightMaps* wm = &L->tm;
+    if (streamed) {
+      CK(cudaStreamWaitEvent(st, wr.copied[i & 1], 0));
+      wm = &wr.maps[i & 1];
+    }
     ContactLayer cl;
     if (contact) {
       const int S = contact->hi - contact->lo;
@@ -685,16 +823,42 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
       cl.lo = contact->lo; cl.S = S;
     }
     float* probs = attn_out ? attn_out[i] : nullptr;
-    rc = attention_block(L, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
+    rc = attention_block(L, *wm, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
       return run_attention(ws.qkv, ws.ctx, probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split != 0,
                            contact ? &cl : nullptr, L->slots);  // multihead_attention.py:357-394
     });
-    if (!rc) rc = ffn_block(L, x, B * T, ws, am, st);
+    if (!rc) rc = ffn_block(L, *wm, x, B * T, ws, am, st);
     if (rc) return rc;
+    if (streamed) {  // fc2 was the slot's last reader: layer i + 2 may overwrite it
+      CK(cudaEventRecord(wr.freed[i & 1], st));
+      if (i + 2 < n_layers && (rc = wr.fetch(layers[i + 2], i + 2))) return rc;
+    }
     if (repr_out && repr_out[i])
       CK(cudaMemcpyAsync(repr_out[i], x, (size_t)B * T * E * 4, cudaMemcpyDeviceToDevice, st));
   }
   return ESMB200_OK;
+}
+
+int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
+                          int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
+                          float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
+                          int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  return stack_forward_impl(layers, n_layers, x, pad_mask, B, T, rope_cos, rope_sin, repr_out, attn_out,
+                            attn_batch_stride, attn_flags, contact, workspace, workspace_bytes, nullptr, 0, nullptr,
+                            stream);
+}
+
+int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
+                                   int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
+                                   float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
+                                   int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
+                                   size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream,
+                                   void* stream) {
+  if (!ring) return fail(ESMB200_EINVAL, "null ring");
+  return stack_forward_impl(layers, n_layers, x, pad_mask, B, T, rope_cos, rope_sin, repr_out, attn_out,
+                            attn_batch_stride, attn_flags, contact, workspace, workspace_bytes, ring, ring_bytes,
+                            copy_stream, stream);
 }
 
 int esmb200_layer_forward(esmb200_layer* layer, float* x, const uint8_t* pad_mask, int32_t B, int32_t T,
@@ -951,6 +1115,10 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   for (int i = 0; i < n_layers; ++i)
     if (row_layers[i]->split != split || col_layers[i]->split != split)
       return fail(ESMB200_EINVAL, "the row and column layers of one stack must share one precision");
+  for (int i = 0; i < n_layers; ++i)
+    if (col_layers[i]->host)
+      return fail(ESMB200_EINVAL, "col layer " + std::to_string(i) + " is offloaded to host memory: the MSA axial "
+                                  "stack runs resident layers only");
   const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C, split);
   if (workspace_bytes < aw.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   if (E != 64 * H) return fail(ESMB200_EINVAL, "the MSA axial path needs head_dim 64");
@@ -964,7 +1132,7 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   const float row_scale = 0.125f / sqrtf((float)R);  // axial_attention.py:36-38
   for (int i = 0; i < n_layers; ++i) {
     // tied row attention (modules.py:202-207; axial_attention.py:71-130)
-    rc = attention_block(row_layers[i], x, M, 1, nullptr, nullptr, row_scale, ws, am, st, [&]() -> int {
+    rc = attention_block(row_layers[i], row_layers[i]->tm, x, M, 1, nullptr, nullptr, row_scale, ws, am, st, [&]() -> int {
       if (pad_mask) {
         ProfScope ps(T_KEYBITS, st);
         if (split)
@@ -978,10 +1146,10 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     });
     // column attention (modules.py:208-212; axial_attention.py:182-239)
     if (!rc)
-      rc = attention_block(col_layers[i], x, M, 1, nullptr, nullptr, col_layers[i]->q_scale, ws, am, st,
-                           [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st, split != 0); });
+      rc = attention_block(col_layers[i], col_layers[i]->tm, x, M, 1, nullptr, nullptr, col_layers[i]->q_scale, ws, am,
+                           st, [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st, split != 0); });
     // feed-forward (modules.py:213-214)
-    if (!rc) rc = ffn_block(col_layers[i], x, M, ws, am, st);
+    if (!rc) rc = ffn_block(col_layers[i], col_layers[i]->tm, x, M, ws, am, st);
     if (rc) return rc;
   }
   return ESMB200_OK;

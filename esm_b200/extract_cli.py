@@ -45,6 +45,9 @@ def create_parser():
     p.add_argument("--truncation_seq_length", type=int, default=1022)
     p.add_argument("--precision", choices=["fp16", "fp32x3"], default="fp16",
                    help="fp16: fp16 MMA operands (default, fastest); fp32x3: hi+lo operand pairs, fp32-grade results (~2.6x slower)")
+    p.add_argument("--cpu-offload", action="store_true",
+                   help="keep the transformer layers' weights in pinned host memory and stream them to the GPU layer "
+                        "by layer (ESM-2 15B on one GPU); same outputs")
     return p
 
 
@@ -158,9 +161,10 @@ def run(args) -> int:
     model, alphabet = pretrained.load_model_and_alphabet(args.model_location)
     if getattr(model, "random_init", False):
         raise RuntimeError("refusing to write embeddings of a random-init model: give --model_location a checkpoint")
-    model = model.eval().to(dev)
+    model = model.eval()
     if getattr(args, "precision", "fp16") != "fp16":
         model.set_precision(args.precision)
+    model = model.cpu_offload(dev) if getattr(args, "cpu_offload", False) else model.to(dev)
     n_layers = model.num_layers
     if not all(-(n_layers + 1) <= i <= n_layers for i in args.repr_layers):
         raise ValueError(f"--repr_layers must lie in [-{n_layers + 1}, {n_layers}]")

@@ -106,6 +106,26 @@ class LayerBinding:
         self._handle = None
         self._key = None
         self._keep = None
+        # cpu_offload(): the pinned uint8 slice that holds the packed matrices (esmb200_layer_offload), and the device
+        # the layer is packed and streamed to
+        self.host: Optional[torch.Tensor] = None
+        self.device: Optional[torch.device] = None
+
+    # _params() positions of the vectors an esmb200_layer borrows: LayerNorms, out/fc1/fc2 biases
+    _BORROWED = (0, 1, 9, 10, 11, 13, 15)
+
+    @property
+    def offloaded(self) -> bool:
+        return self.host is not None
+
+    def offload(self, device: torch.device, host: torch.Tensor) -> None:
+        """Pack into `host` (pinned) on the next handle(); the layer then runs in esmb200_stack_forward_streamed."""
+        self.release()
+        self.device, self.host = device, host
+
+    def end_offload(self) -> None:
+        self.release()
+        self.device, self.host = None, None
 
     def _params(self) -> List[torch.Tensor]:
         m, a = self.module, self.module.self_attn
@@ -119,12 +139,15 @@ class LayerBinding:
         if self._handle is not None and key == self._key:
             return self._handle
         self.release()
-        for p in ps:
-            if not p.is_cuda:
-                raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
-                                        "there is no CPU fallback")
+        if self.host is None:
+            for p in ps:
+                if not p.is_cuda:
+                    raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model with .cuda(); "
+                                            "there is no CPU fallback")
+            keep = [_f32(p) for p in ps]
+        else:  # fp32 device copies of the host parameters for as long as the packing takes
+            keep = [p.detach().to(self.device, torch.float32).contiguous() for p in ps]
         lib = _lib.load()
-        keep = [_f32(p) for p in ps]
         w = _lib.LayerWeights()
         w.embed_dim, w.num_heads, w.ffn_dim = self.embed_dim, self.attention_heads, self.ffn_embed_dim
         w.head_dim = self.head_dim
@@ -136,6 +159,12 @@ class LayerBinding:
         out = ctypes.c_void_p()
         with torch.cuda.device(keep[0].device):
             _lib.check(lib.esmb200_layer_create(ctypes.byref(w), _stream(), ctypes.byref(out)))
+            if self.host is not None:
+                rc = lib.esmb200_layer_offload(out, _ptr(self.host), self.host.numel(), _stream())
+                if rc:
+                    lib.esmb200_layer_destroy(out)
+                    _lib.check(rc)
+                keep = [keep[i] for i in self._BORROWED]
         self._handle, self._key, self._keep = out, key, keep  # the library borrows LN weights and biases from `keep`
         return out
 
@@ -183,6 +212,10 @@ class TransformerLayer(nn.Module):
     def precision(self, value: int):
         self._binding.precision = int(value)
 
+    @property
+    def offloaded(self) -> bool:
+        return self._binding.offloaded
+
     # ---- reference-facing forward ------------------------------------------------------------------------------
     def forward(self, x, self_attn_mask=None, self_attn_padding_mask=None, need_head_weights=False):
         """x: (T, B, E) like the reference (modules.py:120-122). Returns (x (T,B,E), attn (H,B,T,T) or None)."""
@@ -222,12 +255,29 @@ def _workspace(nbytes: int, device: torch.device) -> torch.Tensor:
     return ws
 
 
+_rings: Dict[tuple, tuple] = {}
+
+
+def _ring(nbytes: int, device: torch.device):
+    """(ring, copy stream) of esmb200_stack_forward_streamed, cached per (device, CUDA stream) like the workspace: the
+    library orders a call's copies after the work already queued on the stream, and the stream after the copies."""
+    key = (device, torch.cuda.current_stream(device).cuda_stream)
+    hit = _rings.get(key)
+    if hit is None or hit[0].numel() < nbytes:
+        copy = hit[1] if hit is not None else torch.cuda.Stream(device=device)
+        _rings.pop(key, None)
+        hit = (torch.empty(nbytes, dtype=torch.uint8, device=device), copy)
+        _rings[key] = hit
+    return hit
+
+
 def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Tensor],
               rope_cos: Optional[torch.Tensor], rope_sin: Optional[torch.Tensor],
               repr_out: Optional[Dict[int, torch.Tensor]], attn_layers: Sequence[int], zero_pad_rows: bool = False,
               contact_job=None):
     """esmb200_stack_forward on x fp32 (B,T,E) in place. repr_out: {layer index (0-based): (B,T,E) tensor to fill}.
     rope_cos = rope_sin = None: layers without rotary embedding (ESM-1b / ESM-1v).
+    Layers offloaded by cpu_offload() run through esmb200_stack_forward_streamed instead, with the same results.
     Returns {layer index: (B,H,T,T) fp32} for the indices in attn_layers."""
     if not x.is_cuda:
         raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
@@ -236,9 +286,10 @@ def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Te
     B, T, E = x.shape
     n = len(layers)
     Fdim, H = layers[0].ffn_embed_dim, layers[0].attention_heads
+    precision = getattr(layers[0], "precision", 0)
     with torch.cuda.device(x.device):
         handles = (ctypes.c_void_p * n)(*[l.handle() for l in layers])
-        nbytes = lib.esmb200_workspace_bytes(E, H, Fdim, B, T, getattr(layers[0], "precision", 0))
+        nbytes = lib.esmb200_workspace_bytes(E, H, Fdim, B, T, precision)
         ws = _workspace(nbytes, x.device)
         mask = None
         if padding_mask is not None:
@@ -261,12 +312,16 @@ def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Te
                 attn_t[i] = a
                 attns[i] = a.data_ptr()
         keep.append(mask)
-        _lib.check(lib.esmb200_stack_forward(handles, n, _ptr(x), _ptr(mask), B, T, _ptr(rope_cos), _ptr(rope_sin),
-                                             reprs if repr_out else None, attns if attn_layers else None,
-                                             (len(attn_layers) * H * T * T) if attn_layers else 0,
-                                             1 if zero_pad_rows else 0,
-                                             ctypes.byref(contact_job) if contact_job is not None else None,
-                                             _ptr(ws), ws.numel(), _stream()))
+        args = (handles, n, _ptr(x), _ptr(mask), B, T, _ptr(rope_cos), _ptr(rope_sin),
+                reprs if repr_out else None, attns if attn_layers else None,
+                (len(attn_layers) * H * T * T) if attn_layers else 0, 1 if zero_pad_rows else 0,
+                ctypes.byref(contact_job) if contact_job is not None else None, _ptr(ws), ws.numel())
+        if getattr(layers[0], "offloaded", False):
+            ring, copy = _ring(2 * lib.esmb200_layer_packed_bytes(E, H, Fdim, precision), x.device)
+            _lib.check(lib.esmb200_stack_forward_streamed(*args, _ptr(ring), ring.numel(),
+                                                          ctypes.c_void_p(copy.cuda_stream), _stream()))
+        else:
+            _lib.check(lib.esmb200_stack_forward(*args, _stream()))
     if stacked is not None:
         attn_t["stacked"] = stacked
     return attn_t
@@ -508,8 +563,59 @@ class ProteinLanguageModel(nn.Module):
         self.lm_head = RobertaLMHead(embed_dim, self.alphabet_size, self.embed_tokens.weight)
         self._mirrors: Dict[str, tuple] = {}
         self.precision = "fp16"
+        self._offload = None  # cpu_offload(): (device, pinned arena)
 
     PRECISIONS = {"fp16": 0, "fp32x3": 1}
+
+    def cpu_offload(self, device=None) -> "ProteinLanguageModel":
+        """Run on `device` (default: the current CUDA device) with the transformer layers' weights in host memory, the
+        way the reference runs ESM-2 15B on one GPU (examples/esm2_infer_fairscale_fsdp_cpu_offloading.py,
+        scripts/fold.py --cpu-offload).  The layers' parameters stay on the host, in any dtype; every other module moves
+        to `device`.  Each distinct layer is packed once by the library (its parameters staged on the device as fp32
+        one layer at a time) and its fp16 matrices moved into one pinned host arena.  From then on every forward
+        streams them to the device through a two-slot ring, the copy of layer i + 1 overlapping the kernels of layer i,
+        with results bit-identical to the resident model.  At 15B the device then holds two layers' matrices (1.26 GB)
+        instead of 30 GB.  set_precision() and in-place changes of a host parameter re-pack as usual; model.cuda(),
+        .to() or any other module conversion ends the mode and frees the arena."""
+        if not torch.cuda.is_available():
+            raise _lib.Esmb200Error("cpu_offload() streams the layers to a CUDA (sm_90a) device; none is available")
+        device = torch.device("cuda") if device is None else torch.device(device)
+        if device.type != "cuda":
+            raise _lib.Esmb200Error(f"cpu_offload() needs a CUDA device, got {device}")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        lib = _lib.load()
+        self._end_offload()
+        for name, child in self.named_children():
+            if name != "layers":
+                child.to(device)
+        layers = list({id(l): l for l in self.layers}.values())  # a module repeated in the list is packed once
+        for layer in layers:
+            layer.cpu()
+            if layer.self_attn.rot_emb is not None:  # rope tables are built on the device
+                layer.self_attn.rot_emb.to(device)
+        nbytes = lib.esmb200_layer_packed_bytes(self.embed_dim, self.attention_heads, layers[0].ffn_embed_dim,
+                                                self.PRECISIONS[self.precision])
+        # one arena: torch's pinned allocator rounds every allocation up to a power of two
+        arena = torch.empty(len(layers) * nbytes, dtype=torch.uint8, pin_memory=True)
+        self._offload = (device, arena)
+        for i, layer in enumerate(layers):
+            layer._binding.offload(device, arena[i * nbytes:(i + 1) * nbytes])
+            layer.handle()
+        torch.cuda.empty_cache()  # return the fp32 staging of the packing to the device
+        return self
+
+    def _end_offload(self) -> None:
+        if getattr(self, "_offload", None) is None:
+            return
+        torch.cuda.synchronize(self._offload[0])  # a streamed forward may still be copying from the arena
+        for layer in self.layers:
+            layer._binding.end_offload()
+        self._offload = None
+
+    def _apply(self, fn, *args, **kwargs):
+        self._end_offload()  # model.cuda() / .to() / .half() after cpu_offload(): the resident path again
+        return super()._apply(fn, *args, **kwargs)
 
     def set_precision(self, name: str) -> "ProteinLanguageModel":
         """"fp16" (default): fp16 MMA operands, fp32 accumulation — the fast path bench.py measures.
@@ -521,9 +627,12 @@ class ProteinLanguageModel(nn.Module):
             raise ValueError(f"precision must be one of {sorted(self.PRECISIONS)}")
         if name == "fp32x3" and (self.embed_dim % 64 != 0 or self.embed_dim // self.attention_heads > 64):
             raise ValueError("fp32x3 precision needs embed_dim % 64 == 0 and head_dim <= 64")
+        changed = name != self.precision
         self.precision = name
         for layer in self.layers:
             layer.precision = self.PRECISIONS[name]
+        if changed and self._offload is not None:
+            self.cpu_offload(self._offload[0])  # the packed size depends on the precision: a new arena
         return self
 
     def _rope_tables(self, T: int):

@@ -53,6 +53,10 @@ def create_parser():
     p.add_argument("--precision", choices=PRECISIONS, default="fp16",
                    help="fp16: fp16 MMA operands (default, fastest); fp32x3: hi+lo operand pairs, fp32-grade scores "
                         "(slower); applies to every model location")
+    p.add_argument("--cpu-offload", action="store_true",
+                   help="keep the transformer layers' weights of ESM-2 / ESM-1b / ESM-1v models in pinned host memory "
+                        "and stream them to the GPU layer by layer (ESM-2 15B on one GPU); same scores. The MSA "
+                        "Transformer stays resident")
     return p
 
 
@@ -136,9 +140,10 @@ def run(args) -> None:
         model, alphabet, is_msa = load_model(location)
         if getattr(model, "random_init", False):
             raise RuntimeError("refusing to score variants with a random-init model: give --model-location a checkpoint")
-        model = model.eval().cuda()
+        model = model.eval()
         if getattr(args, "precision", "fp16") != "fp16":
             model.set_precision(args.precision)
+        model = model.cpu_offload() if getattr(args, "cpu_offload", False) and not is_msa else model.cuda()
         scores[location] = score_model(model, alphabet, is_msa, args, mutations)
         del model
         gc.collect()

@@ -134,6 +134,31 @@ int esmb200_stack_forward(esmb200_layer* const* layers, int32_t n_layers, float*
                           int32_t attn_flags, const esmb200_contact_job* contact /* nullable */, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---- streamed weights: a stack whose packed matrices live in pinned host memory (ESM-2 15B on one GPU; the
+ * reference's CPU offloading, examples/esm2_infer_fairscale_fsdp_cpu_offloading.py, scripts/fold.py --cpu-offload) ----
+ * esmb200_layer_packed_bytes: bytes of one layer's packed matrices (w_qkv, w_out, w_fc1, w_fc2, each 1024-aligned,
+ *   back to back): the size of its host copy and of one ring slot. Pure host arithmetic; 0 for an unsupported shape.
+ * esmb200_layer_offload: copies the packed matrices into host_dst (pinned, caller-owned, at least
+ *   esmb200_layer_packed_bytes; it must outlive the layer) after the work queued on `stream` (esmb200_layer_create's
+ *   packing), synchronises `stream`, and frees their device copies. The packed q/k/v bias and the borrowed LayerNorm
+ *   vectors and biases stay on the device. From then on esmb200_layer_forward and esmb200_stack_forward return
+ *   ESMB200_EINVAL for the layer and launch nothing; esmb200_stack_forward_streamed runs it.
+ * esmb200_stack_forward_streamed: esmb200_stack_forward (same arguments and results, bit-identical) on layers that are
+ *   all offloaded and share E, H, F and precision; a handle may appear more than once. ring: a device buffer of at
+ *   least 2 * esmb200_layer_packed_bytes (16-byte aligned). Layer i's matrices are copied into slot i % 2 on
+ *   copy_stream (a stream other than `stream`, so that the copies run on the copy engine under the previous layer's
+ *   kernels), once layer i - 2's fc2 GEMM has run; layer i's QKV GEMM waits for its copy. copy_stream first waits
+ *   for the work already queued on `stream`, and `stream` waits for every copy of the call, so calls that share a
+ *   ring on one stream, and the caller's stream-ordered reuse of the ring, are safe. */
+size_t esmb200_layer_packed_bytes(int32_t embed_dim, int32_t num_heads, int32_t ffn_dim, int32_t precision);
+int esmb200_layer_offload(esmb200_layer* layer, void* host_dst, size_t bytes, void* stream);
+int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
+                                   int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
+                                   float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
+                                   int32_t attn_flags, const esmb200_contact_job* contact /* nullable */,
+                                   void* workspace, size_t workspace_bytes, void* ring, size_t ring_bytes,
+                                   void* copy_stream, void* stream);
+
 /* Embedding prologue of ESM2.forward (esm2.py:84-95): gather from table [V,E], zero <mask> rows and rescale by
  * 0.88/(1 - n_mask/n_nonpad) when token_dropout, zero pad rows. tokens int64 [B,T] -> x fp32 [B,T,E]. */
 int esmb200_embed_tokens(const int64_t* tokens, const float* table, float* x, int32_t B, int32_t T, int32_t E,
