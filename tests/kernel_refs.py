@@ -1,0 +1,163 @@
+"""float64 references of single kernels, shared by the kernel-level GPU tests and checked on the CPU by
+tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test pass).
+
+  * contact_partials: the accumulators of the fused probability + contact pass (csrc/attention_contact.cuh) in the
+    kernel's own layout: acc [B,S,S], row_part / col_part [B,H,4*ceil(T/128),S], one partial per 32-key / 32-query
+    quarter of each 128-wide tile;
+  * gemm_launches: every (epilogue, N, K) GEMM a model's forward launches (api.cu attention_block / ffn_block, the LM
+    head of model.py RobertaLMHead.forward_native, the MSA Transformer's layer in msa.py);
+  * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf).
+"""
+from __future__ import annotations
+
+import math
+from typing import Dict, List, Optional, Tuple
+
+import torch
+
+EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32 = range(5)
+
+U32 = 2.0 ** -24  # unit roundoff of fp32
+
+
+# ---- contact head ---------------------------------------------------------------------------------------------------
+def contact_mask(keep: Optional[torch.Tensor], T: int, lo: int, hi: int, device=None) -> torch.Tensor:
+    """[B or 1, T] float64: 1 at positions inside the crop [lo, hi) that are not <eos> (keep = tokens != eos)."""
+    crop = torch.zeros(T, dtype=torch.float64, device=device)
+    crop[lo:hi] = 1
+    if keep is None:
+        return crop[None]
+    return keep.to(device=device, dtype=torch.float64) * crop[None]
+
+
+def masked_maps(attn: torch.Tensor, keep: Optional[torch.Tensor], lo: int, hi: int) -> torch.Tensor:
+    """attn [B,H,T,T] (one layer) -> float64 A_h with the rows and columns outside the crop or at <eos> zeroed."""
+    B, H, T, _ = attn.shape
+    m = contact_mask(keep, T, lo, hi, attn.device)
+    m = m.expand(B, T)
+    return attn.double() * (m[:, None, :, None] * m[:, None, None, :])
+
+
+def quarter_sums(x: torch.Tensor, dim: int) -> torch.Tensor:
+    """Sum `x` over consecutive 32-wide groups along `dim` (padded with zeros to a multiple of 128): the group g holds
+    indices [32 g, 32 g + 32), i.e. quarter g % 4 of 128-wide tile g // 4."""
+    n = x.shape[dim]
+    nt = (n + 127) // 128
+    pad = [0, 0] * (x.ndim - 1 - (dim % x.ndim)) + [0, 128 * nt - n]
+    xp = torch.nn.functional.pad(x, pad)
+    shape = list(xp.shape)
+    d = dim % x.ndim
+    shape[d:d + 1] = [4 * nt, 32]
+    return xp.reshape(shape).sum(d + 1)
+
+
+def contact_partials(attn: torch.Tensor, w: torch.Tensor, keep: Optional[torch.Tensor], lo: int, hi: int):
+    """One layer's share of the fused contact accumulators, float64.
+    attn [B,H,T,T], w [H] -> (acc [B,S,S] = sum_h w_h A_h, row_part [B,H,4nt,S], col_part [B,H,4nt,S]) with
+    row_part[b,h,4kt+q,i-lo] = sum of A_h[i, j] over the keys j of quarter q of key tile kt, and
+    col_part[b,h,4qt+r,j-lo] = sum of A_h[i, j] over the queries i of quarter r of query tile qt."""
+    a = masked_maps(attn, keep, lo, hi)
+    acc = torch.einsum("bhij,h->bij", a, w.double().to(a.device))[:, lo:hi, lo:hi]
+    row = quarter_sums(a, -1)[:, :, lo:hi, :].transpose(-1, -2)  # [B,H,4nt,S]
+    col = quarter_sums(a, -2)[:, :, :, lo:hi]                     # [B,H,4nt,S]
+    return acc, row, col
+
+
+def contacts_from_partials(acc: torch.Tensor, row: torch.Tensor, col: torch.Tensor, w: torch.Tensor,
+                           bias: Optional[float]) -> torch.Tensor:
+    """The contact head from the accumulators of all layers, float64: row/col [L,B,H,4nt,S], w [L,H], acc [B,S,S].
+    logit = acc + acc^T - sum_c (w_c / a12_c) a1_c a1_c^T + bias, a1_c = rowsum + colsum (model.py
+    ContactPredictionHead.forward)."""
+    L, B, H, _, S = row.shape
+    a1 = (row.double().sum(3) + col.double().sum(3)).permute(1, 0, 2, 3).reshape(B, L * H, S)
+    wl = w.double().reshape(1, L * H, 1).to(a1.device)
+    u = a1 * wl / a1.sum(-1, keepdim=True)
+    acc = acc.double()
+    logits = acc + acc.transpose(-1, -2) - torch.einsum("bci,bcj->bij", u, a1)
+    if bias is not None:
+        logits = logits + bias
+    return torch.sigmoid(logits)
+
+
+def sum_bound(terms_abs: torch.Tensor, n: int) -> torch.Tensor:
+    """Bound of an n-term fp32 recursive sum (any order) of values with absolute sum `terms_abs`: (n - 1) u sum|x|."""
+    return (n - 1) * U32 * terms_abs
+
+
+# ---- GEMM launch table ----------------------------------------------------------------------------------------------
+# (name, layers, embed_dim, heads, ffn_dim, rotary, msa)
+MODELS: Dict[str, Tuple[int, int, int, int, bool, bool]] = {
+    "esm2_t6_8M": (6, 320, 20, 1280, True, False),
+    "esm2_t12_35M": (12, 480, 20, 1920, True, False),
+    "esm2_t30_150M": (30, 640, 20, 2560, True, False),
+    "esm2_t33_650M": (33, 1280, 20, 5120, True, False),
+    "esm2_t36_3B": (36, 2560, 40, 10240, True, False),
+    "esm2_t48_15B": (48, 5120, 40, 20480, True, False),
+    "esm1b_t33_650M": (33, 1280, 20, 5120, False, False),
+    "esm_msa1b_t12_100M": (12, 768, 12, 3072, False, True),
+}
+VOCAB = 33
+
+
+def head_slots(E: int, H: int) -> int:
+    """64-wide column slots per head on the attention side (api.cu head_slots)."""
+    return 2 if E // H > 64 else 1
+
+
+def gemm_launches(name: str) -> List[Tuple[str, int, int, int]]:
+    """[(role, epilogue, N, K)] of one forward of the model: the transformer layer's four GEMMs (the MSA layer has a
+    row and a column attention block, each with its QKV and out-projection), then the LM head's dense layer
+    (erf-GELU into fp32) and its projection onto the vocabulary padded to 64 columns."""
+    _, E, H, F, _, msa = MODELS[name]
+    Ea = 64 * head_slots(E, H) * H
+    attn = [("qkv", EPI_QKV_ROPE, 3 * Ea, E), ("out_proj", EPI_BIAS_RESIDUAL, E, Ea)]
+    ffn = [("fc1", EPI_BIAS_GELU, F, E), ("fc2", EPI_BIAS_RESIDUAL, E, F)]
+    layer = (attn + attn if msa else attn) + ffn
+    npad = (VOCAB + 63) // 64 * 64
+    return layer + [("lm_dense", EPI_BIAS_GELU_F32, E, E), ("lm_out", EPI_BIAS_F32, npad, E)]
+
+
+def packed_bytes_from_launches(name: str) -> int:
+    """esmb200_layer_packed_bytes of the model's transformer layer, from the B operands [N, K] fp16 of its four
+    GEMMs, each 1024-byte aligned (api.cu packed_layout)."""
+    launches = gemm_launches(name)[:4]
+    return sum((n * k * 2 + 1023) // 1024 * 1024 for _, _, n, k in launches)
+
+
+# ---- erf-GELU -------------------------------------------------------------------------------------------------------
+AS_ERF = 1.5e-7  # Abramowitz & Stegun 7.1.26: |erf(z) - approx| <= 1.5e-7 for z >= 0
+
+
+def gelu64(x: torch.Tensor) -> torch.Tensor:
+    x = x.double()
+    return x * 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def gelu_bound(x: torch.Tensor) -> torch.Tensor:
+    """|gelu_erf(x) - gelu(x)| bound for the fp32 epilogue, x the fp32 pre-activation (float64 tensor).
+    gelu_erf computes q = 0.5 erfc(|x|/sqrt2) as 0.5 poly(t) exp(-z^2) and returns x (1 - q) or x q:
+      * the A&S truncation: |dq| <= 0.5 * 1.5e-7;
+      * rcp.approx (t, 1 ulp), the four fmas of the Horner chain, ex2.approx (2 ulp) and the rounding of its argument
+        -z^2 log2(e) (|arg| ulp, times ln 2) perturb q relatively by at most 32 u + 2 u |arg|, with the Horner
+        chain's condition number (|t P'(t) / P(t)| <= 3.5 on t in (0, 1], P = t (a1 + a2 t + ...)) folded in;
+      * the final 1 - q and x * (...) roundings: 2 u |y|.
+    Tightening any term below what the kernel computes makes the test fail on a correct kernel."""
+    x = x.double()
+    z = x.abs() / math.sqrt(2.0)
+    q = 0.5 * torch.erfc(z)
+    arg = z * z / math.log(2.0)
+    return x.abs() * (0.5 * AS_ERF + q * (32 + 2 * arg) * U32) + 2 * U32 * gelu64(x).abs() + 1e-30
+
+
+def horner_condition() -> float:
+    """max over t in (0, 1] of |t P'(t) / P(t)| for the A&S polynomial P (the factor folded into gelu_bound)."""
+    a = [0.254829592, -0.284496736, 1.421413741, -1.453152027, 1.061405429]
+    t = torch.linspace(1e-6, 1.0, 100001, dtype=torch.float64)
+    p = sum(c * t ** (i + 1) for i, c in enumerate(a))
+    dp = sum((i + 1) * c * t ** i for i, c in enumerate(a))
+    return float((t * dp / p).abs().max())
+
+
+# ---- LayerNorm ------------------------------------------------------------------------------------------------------
+def layer_norm64(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    return torch.nn.functional.layer_norm(x.double(), (x.shape[-1],), w.double(), b.double(), eps)

@@ -179,8 +179,9 @@ def test_narrow_heads_vs_oracle(L, E, H):
 @pytest.mark.parametrize("L,E,H", [(3, 256, 2), (2, 640, 5), (2, 192, 2)])
 def test_wide_heads_vs_oracle(L, E, H):
     """head_dim 128 — esm2_t48_15B's head width (pretrained.py:390-397), at small widths — and 96: two 64-wide column
-    slots per head, 64-column rope tables; ragged batch with <mask> tokens, attentions and contacts (the separate
-    probability + accumulation kernels: the fused contact pass is a head_dim <= 64 kernel)."""
+    slots per head, 64-column rope tables; ragged batch with <mask> tokens, attentions and contacts (the fused
+    probability + contact pass in its two-slot DS = 2 instance; tests/test_gpu_contact_fused.py checks its
+    accumulators)."""
     from oracle import esm2_oracle
     from oracle.weights import make_tokens
     model, sd = build_model(L, E, H)
