@@ -6,7 +6,9 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
     quarter of each 128-wide tile;
   * gemm_launches: every (epilogue, N, K) GEMM a model's forward launches (api.cu attention_block / ffn_block, the LM
     head of model.py RobertaLMHead.forward_native, the MSA Transformer's layer in msa.py);
-  * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf).
+  * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf);
+  * split16 / join64 / split_rep_bound / split_acc_bound / FP32X3_MODELS: the fp32x3 precision's hi | lo operand pairs,
+    the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs.
 """
 from __future__ import annotations
 
@@ -117,11 +119,65 @@ def gemm_launches(name: str) -> List[Tuple[str, int, int, int]]:
     return layer + [("lm_dense", EPI_BIAS_GELU_F32, E, E), ("lm_out", EPI_BIAS_F32, npad, E)]
 
 
+def fp32x3_accepts(E: int, H: int) -> bool:
+    """The layers run precision 1 (fp32x3) when E % 64 == 0 (every GEMM K a whole number of 64-wide slabs) and the
+    heads fit one 64-wide slot (model.py ProteinLanguageModel.set_precision; the MSA layers have head_dim 64)."""
+    return E % 64 == 0 and E // H <= 64
+
+
+# 8M, 150M, 650M, 3B, ESM-1b and MSA-1b; 35M fails E % 64 (480) and 15B has 128-wide heads
+FP32X3_MODELS: List[str] = [n for n, (_, E, H, _, _, _) in MODELS.items() if fp32x3_accepts(E, H)]
+
+
 def packed_bytes_from_launches(name: str) -> int:
     """esmb200_layer_packed_bytes of the model's transformer layer, from the B operands [N, K] fp16 of its four
     GEMMs, each 1024-byte aligned (api.cu packed_layout)."""
     launches = gemm_launches(name)[:4]
     return sum((n * k * 2 + 1023) // 1024 * 1024 for _, _, n, k in launches)
+
+
+# ---- fp32x3 operands ------------------------------------------------------------------------------------------------
+F16_HALF_QUANTUM = 2.0 ** -25  # half the smallest fp16 subnormal (2^-24): the absolute rounding error below 2^-14
+
+
+def split16(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp32 x -> fp16 (hi, lo) with hi = rn16(x), lo = rn16(x - hi) (esmb200_convert_split; the GEMM epilogues and the
+    attention kernels split their fp32 results the same way).  x - hi is exact in fp32."""
+    x = x.float()
+    hi = x.half()
+    return hi, (x - hi.float()).half()
+
+
+def join64(hi: torch.Tensor, lo: torch.Tensor) -> torch.Tensor:
+    """The value a hi | lo pair stands for, in float64 (exact)."""
+    return hi.double() + lo.double()
+
+
+def split_rep_bound(x: torch.Tensor) -> torch.Tensor:
+    """|x - (hi + lo)| for (hi, lo) = split16(x): r = x - hi is exact and |r| <= 2^-11 |x| (or <= 2^-25 when hi is
+    subnormal); rn16(r) is within 2^-11 |r| + 2^-25 of r, the 2^-25 being the subnormal half-quantum, which applies to
+    the lo half of every |x| below ~2^-3.  Hence <= 2^-22 |x| + 2^-25."""
+    return 2.0 ** -22 * x.double().abs() + F16_HALF_QUANTUM
+
+
+def split_acc_bound(a_hi: torch.Tensor, a_lo: torch.Tensor, w_hi: torch.Tensor, w_lo: torch.Tensor, K: int,
+                    y: torch.Tensor) -> torch.Tensor:
+    """|out - y| for the split GEMM (gemm2_f16_kernel<EPI, true>) before any epilogue function, y = (a_hi + a_lo)
+    (w_hi + w_lo)^T + bias in float64 (a [M, K], w [N, K] fp16 halves):
+      * the three passes hi*hi, lo*hi, hi*lo feed one fp32 accumulator, 3K/16 k16 steps; each step adds its exact
+        products with truncation (one ulp, 2^-23 of a partial sum bounded by the absolute sum of all three passes),
+        doubled for slack and given 4 steps of headroom as for the fp16 kernel: (3K/16 + 4) 2^-22 sum|a w|;
+      * the dropped lo*lo term, bounded by sum_k |a_lo w_lo| (computed exactly, <= 2^-22 sum|a w|);
+      * the bias add and the fp32 result: 2 u |y|."""
+    ah, al, wh, wl = (t.double().abs() for t in (a_hi, a_lo, w_hi, w_lo))
+    passes = ah @ wh.t() + al @ wh.t() + ah @ wl.t()
+    return (3 * K / 16 + 4) * 2.0 ** -22 * passes + al @ wl.t() + 2 * U32 * y.abs()
+
+
+def split_box_scale(K: int) -> float:
+    """(3K/16 + 4) 2^-25: the scale of the per-output-box rel-Frobenius gate of the split GEMM (the accumulation drift
+    of DESIGN.md section 4, per unit of relative size)."""
+    return (3 * K / 16 + 4) * 2.0 ** -25
 
 
 # ---- erf-GELU -------------------------------------------------------------------------------------------------------

@@ -330,7 +330,8 @@ def test_msa_transformer_masked_marginals_against_the_reference(esm_ref):
           f"centered rel_fro={r:.3e}; forward logits of row 0 without a mask: centered rel_fro={rf:.3e}", flush=True)
     # Since the scorer is the forward bit for bit, the remaining difference is the fp16-mode error of the 12-layer axial
     # stack with 64 tied rows on these random weights (measured at 1.0e-2 on an H100), which the unmasked forward shows
-    # as well; the MSA path has no fp32x3 mode to tighten it. Held to that level, not to the 4e-3 of the sequence models.
+    # as well (test_masked_marginals_fp32x3_against_the_reference in test_gpu_msa_precision.py runs the same comparison
+    # in the fp32x3 mode). Held to that level, not to the 4e-3 of the sequence models.
     assert r <= 2e-2 and rf <= 2e-2
 
 

@@ -104,6 +104,88 @@ def test_gemm_launch_table_matches_the_modules(name):
     assert launches["lm_dense"] == (E, E) and launches["lm_out"] == (64, E)
 
 
+def test_split16_is_exact_hi_plus_rounded_residue():
+    g = torch.Generator().manual_seed(0)
+    x = torch.randn(10000, generator=g) * torch.logspace(-8, 4, 10000)  # below the fp16 overflow at 65520
+    hi, lo = kr.split16(x)
+    assert hi.dtype == lo.dtype == torch.float16
+    assert torch.equal(hi, x.half())
+    assert torch.equal(lo, (x.double() - hi.double()).float().half())  # x - hi is exact in fp32
+    assert torch.equal(kr.join64(hi, lo), hi.double() + lo.double())
+
+
+def test_split_representation_bound_holds_and_is_tight():
+    """|x - (hi + lo)| <= 2^-22 |x| + 2^-25 from 1e-8 to 6e4, and the bound is attained to within 2x: overall (lo
+    subnormal) and on the normal range alone (where the largest error is half the 2^-22 term)."""
+    g = torch.Generator().manual_seed(1)
+    mag = torch.logspace(-8, math.log10(6e4), 400001, dtype=torch.float64)
+    x = (mag * torch.where(torch.rand(mag.shape, generator=g) < 0.5, -1.0, 1.0)).float()
+    hi, lo = kr.split16(x)
+    assert bool(torch.isfinite(hi).all())
+    err = (x.double() - kr.join64(hi, lo)).abs()
+    ratio = err / kr.split_rep_bound(x)
+    assert float(ratio.max()) <= 1.0
+    assert float(ratio.max()) >= 0.5
+    big = x.abs() >= 1.0
+    assert float(ratio[big].max()) >= 0.45
+    assert float(ratio[x.abs() < 2.0 ** -3].max()) >= 0.5  # the subnormal half-quantum is needed
+    assert float((err / (2.0 ** -22 * x.double().abs()))[x.abs() < 2.0 ** -3].max()) > 1.0
+
+
+def test_fp32x3_models_follow_set_precision():
+    """kr.FP32X3_MODELS are exactly the table's models whose set_precision("fp32x3") succeeds (the MSA layers have
+    head_dim 64 by construction)"""
+    from types import SimpleNamespace
+    from esm_b200.model import ProteinLanguageModel
+    assert kr.FP32X3_MODELS == ["esm2_t6_8M", "esm2_t30_150M", "esm2_t33_650M", "esm2_t36_3B", "esm1b_t33_650M",
+                                "esm_msa1b_t12_100M"]
+    for name, (_, E, H, _, _, msa) in kr.MODELS.items():
+        if msa:
+            assert E == 64 * H and name in kr.FP32X3_MODELS
+            continue
+        stub = SimpleNamespace(embed_dim=E, attention_heads=H, PRECISIONS=ProteinLanguageModel.PRECISIONS,
+                               precision="fp16", layers=[SimpleNamespace(precision=0)], _offload=None)
+        try:
+            ProteinLanguageModel.set_precision(stub, "fp32x3")
+            ok = True
+        except ValueError:
+            ok = False
+        assert ok == (name in kr.FP32X3_MODELS), name
+        assert not ok or stub.layers[0].precision == 1
+
+
+def test_split_acc_bound_covers_an_emulated_three_pass_product():
+    """The three-pass product with fp32 accumulation in k16 steps truncated toward zero (the tensor core's behaviour,
+    emulated in float64 then chopped to fp32) stays inside kr.split_acc_bound, and dropping a pass does not."""
+    g = torch.Generator().manual_seed(2)
+    M, N, K = 16, 24, 640
+    a, w = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g) * K ** -0.5
+    ah, al = kr.split16(a)
+    wh, wl = kr.split16(w)
+    y = kr.join64(ah, al) @ kr.join64(wh, wl).t()
+
+    def chop(t):  # round toward zero to fp32
+        f = t.float()
+        over = f.double().abs() > t.abs()
+        return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f).double()
+
+    def run(passes):
+        acc = torch.zeros(M, N, dtype=torch.float64)
+        for k0 in range(0, K, 64):
+            for pa, pw in passes:
+                for s in range(k0, k0 + 64, 16):
+                    acc = chop(acc + pa[:, s:s + 16].double() @ pw[:, s:s + 16].double().t())
+        return acc
+
+    b = kr.split_acc_bound(ah, al, wh, wl, K, y)
+    good = run([(ah, wh), (al, wh), (ah, wl)])
+    assert float(((good - y).abs() / b).max()) <= 1.0
+    bad = run([(ah, wh), (ah, wh), (ah, wl)])  # lo*hi read as hi*hi
+    assert float(((bad - y).abs() / b).max()) > 1.0
+    dropped = run([(ah, wh), (ah, wl)])        # lo*hi missing
+    assert float(((dropped - y).abs() / b).max()) > 1.0
+
+
 def test_gelu_bound_covers_an_fp32_restatement():
     """The epilogue's formula evaluated in fp32 with correctly rounded reciprocal and exponential stays inside the bound
     (the approximate MUFU instructions' share of the bound is not exercised here; the GPU test does that)."""
