@@ -59,10 +59,13 @@ EXPORTS = (
     "esmb200_layer_packed_bytes",
     "esmb200_layer_offload",
     "esmb200_stack_forward_streamed",
+    "esmb200_layernorm_fp8",
+    "esmb200_quantize_fp8",
+    "esmb200_gemm_fp8",
 )
 
 ABI_VERSION = 2
-EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32 = range(5)
+EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32, EPI_GELU_FP8 = range(6)
 
 
 class LayerWeights(ctypes.Structure):
@@ -216,6 +219,14 @@ def _declare(lib):
                                                    c_void_p, c_void_p]
     lib.esmb200_set_option.restype = c_int32
     lib.esmb200_set_option.argtypes = [c_char_p, c_int32]
+    lib.esmb200_layernorm_fp8.restype = c_int32
+    lib.esmb200_layernorm_fp8.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float,
+                                          c_void_p]
+    lib.esmb200_quantize_fp8.restype = c_int32
+    lib.esmb200_quantize_fp8.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]
+    lib.esmb200_gemm_fp8.restype = c_int32
+    lib.esmb200_gemm_fp8.argtypes = [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p]
     lib.esmb200_convert_f16.restype = c_int32
     lib.esmb200_convert_f16.argtypes = [c_void_p, c_void_p, c_size_t, c_void_p]
 

@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "elementwise.cuh"
 #include "gemm2.cuh"
+#include "gemm_fp8.cuh"
 #include "tied_attention.cuh"
 
 using namespace esmb200;
@@ -100,7 +101,7 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2D row-major [rows, cols] (cols contiguous) of fp16 (esize 2) or fp32 (esize 4);
+// 2D row-major [rows, cols] (cols contiguous) of e4m3 (esize 1), fp16 (esize 2) or fp32 (esize 4);
 // box = {128 bytes of columns, box_rows}, 128B swizzle.
 int make_tmap_2d(CUtensorMap* map, const void* ptr, int esize, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                  uint32_t box_rows) {
@@ -112,7 +113,10 @@ int make_tmap_2d(CUtensorMap* map, const void* ptr, int esize, uint64_t rows, ui
   cuuint64_t strides[1] = {ld_elems * (uint64_t)esize};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esize), box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+  const CUtensorMapDataType dt = esize == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                 : esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                              : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUresult r = enc(map, dt, 2,
                    const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -191,6 +195,24 @@ int launch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   if (e != cudaSuccess) return fail_cuda(e, split ? "gemm launch (fp32x3)" : "gemm launch");
   return ESMB200_OK;
 }
+
+// fp8 precision (gemm_fp8.cuh): epilogues EPI_QKV_ROPE (fp16 out), EPI_BIAS_RESIDUAL (fp32 x += y), EPI_GELU_FP8 (e4m3
+// out + scales)
+int launch_gemm_fp8(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const Fp8GemmParams& p,
+                    cudaStream_t st, int tag = T_GEMM_OTHER) {
+  ProfScope ps(tag, st);
+  cudaError_t e;
+  switch (epi) {
+    case EPI_QKV_ROPE: e = launch_gemm_fp8_epi<EPI_QKV_ROPE>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_BIAS_RESIDUAL: e = launch_gemm_fp8_epi<EPI_BIAS_RESIDUAL>(ta, tb, to, p, num_sms(), st); break;
+    case EPI_GELU_FP8: e = launch_gemm_fp8_epi<EPI_GELU_FP8>(ta, tb, to, p, num_sms(), st); break;
+    default: return fail(ESMB200_EINVAL, "fp8 gemm epilogue must be 0 (qkv), 1 (residual) or 5 (gelu -> fp8)");
+  }
+  if (e != cudaSuccess) return fail_cuda(e, "gemm launch (fp8)");
+  return ESMB200_OK;
+}
+
+inline int kblocks(int K) { return (K + 127) / 128; }  // 128-wide K blocks of the fp8 scales
 
 // every GemmParams field an epilogue does not read stays zero
 GemmParams gemm_params(int M, int N, int K, const float* bias) {
@@ -345,6 +367,27 @@ int layernorm_f16(const float* x, const float* w, const float* b, void* out, int
   return ESMB200_OK;
 }
 
+// LayerNorm -> e4m3 GEMM operand [M, E] and its scales [ceil(E/128), M]
+int layernorm_fp8(const float* x, const float* w, const float* b, void* out, float* scales, int M, int E, float eps,
+                  int tag, cudaStream_t st) {
+  cudaError_t e;
+  {
+    ProfScope ps(tag, st);
+    e = launch_layernorm<3>(x, w, b, out, M, E, eps, st, scales);
+  }
+  if (e != cudaSuccess) return fail_cuda(e, "layernorm_fp8");
+  return ESMB200_OK;
+}
+
+// fp32 [rows, K] -> e4m3 [rows, K] + scales per block_rows x 128 block (quantize_fp8_kernel)
+int quantize_fp8(const float* src, uint8_t* dst, float* scales, int rows, int K, int block_rows, cudaStream_t st) {
+  ProfScope ps(T_CONVERT, st);
+  quantize_fp8_kernel<<<dim3(kblocks(K), (rows + block_rows - 1) / block_rows), 256, 0, st>>>(src, dst, scales, rows, K,
+                                                                                               block_rows);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
 // fp32 [rows, K] -> fp16 [rows, K], or with split the fp32x3 hi | lo halves [rows, 2K]
 int convert_f16(const float* src, void* dst, size_t rows, int K, bool split, cudaStream_t st) {
   const size_t n = rows * (size_t)K;
@@ -375,6 +418,7 @@ struct esmb200_layer {
   int Ea;         // 64 * slots * H: width of q / k / v / ctx
   float q_scale;  // d^-1/2 (multihead_attention.py:100)
   int split;      // 1: fp32x3 precision — weights packed as fp16 hi | lo along K, activations likewise
+  int fp8;        // 1: fp8 precision — QKV, fc1 and fc2 run the e4m3 GEMM from w8; out_proj stays fp16 (w_out)
   float eps;
   // borrowed fp32 parameters (owned by the caller, must outlive the layer)
   const float *ln1_w, *ln1_b, *ln2_w, *ln2_b, *out_b, *fc1_b, *fc2_b;
@@ -384,6 +428,11 @@ struct esmb200_layer {
   __half* w_fc1;  // [F,E]
   __half* w_fc2;  // [E,F]
   float* b_qkv;   // [3*Ea]
+  // fp8 precision: one allocation holding the e4m3 matrices ([Wq;Wk;Wv] in head slots, fc1, fc2) and their 128 x 128
+  // block scales (Fp8Layout); w_qkv, w_fc1 and w_fc2 stay NULL
+  uint8_t* w8;
+  uint8_t *q_qkv, *q_fc1, *q_fc2;
+  float *s_qkv, *s_fc1, *s_fc2;
   WeightMaps tm;  // of w_qkv .. w_fc2; zero once offloaded
   // esmb200_layer_offload: the caller's pinned copy of w_qkv .. w_fc2 in the packed_layout() arrangement; the device
   // copies are freed and the layer runs only in esmb200_stack_forward_streamed
@@ -408,6 +457,39 @@ PackedLayout packed_layout(int E, int H, int F, int split) {
   return p;
 }
 
+// fp8 precision: the e4m3 matrices and their block scales [ceil(rows/128), ceil(K/128)] back to back, 1024-aligned
+struct Fp8Layout {
+  size_t qkv, fc1, fc2, s_qkv, s_fc1, s_fc2;  // byte offsets
+  size_t bytes;
+};
+
+Fp8Layout fp8_layout(int E, int Ea, int F) {
+  Fp8Layout l;
+  size_t o = 0;
+  auto take = [&](size_t n) {
+    const size_t at = o;
+    o += align_up(n, 1024);
+    return at;
+  };
+  l.qkv = take((size_t)3 * Ea * E);
+  l.fc1 = take((size_t)F * E);
+  l.fc2 = take((size_t)E * F);
+  l.s_qkv = take((size_t)kblocks(3 * Ea) * kblocks(E) * 4);
+  l.s_fc1 = take((size_t)kblocks(F) * kblocks(E) * 4);
+  l.s_fc2 = take((size_t)kblocks(E) * kblocks(F) * 4);
+  l.bytes = o;
+  return l;
+}
+
+// B-operand maps of a layer's fp8 matrices and its fp16 out_proj
+int make_weight_maps_fp8(WeightMaps* m, const esmb200_layer* L) {
+  int rc = make_tmap_2d(&m->qkv, L->q_qkv, 1, 3 * (uint64_t)L->Ea, L->E, L->E, gemm_fp8_cfg::BOX_ROWS);
+  if (!rc) rc = make_tmap_f16(&m->out, L->w_out, L->E, L->Ea, L->Ea, gemm2_cfg::HALF_N);
+  if (!rc) rc = make_tmap_2d(&m->fc1, L->q_fc1, 1, L->F, L->E, L->E, gemm_fp8_cfg::BOX_ROWS);
+  if (!rc) rc = make_tmap_2d(&m->fc2, L->q_fc2, 1, L->E, L->F, L->F, gemm_fp8_cfg::BOX_ROWS);
+  return rc;
+}
+
 // B-operand maps of a layer's packed matrices (fc1 == nullptr: attention-only layer)
 int make_weight_maps(WeightMaps* m, const __half* qkv, const __half* out, const __half* fc1, const __half* fc2, int E,
                      int Ea, int F, int split) {
@@ -421,26 +503,34 @@ int make_weight_maps(WeightMaps* m, const __half* qkv, const __half* out, const 
 }
 
 struct Workspace {
-  __half* xn;
+  __half* xn;    // fp8 precision: e4m3 [M,E], followed by its scales xn_s [ceil(E/128), M]
   __half* qkv;
   __half* ctx;
-  __half* h;     // aliases qkv + ctx
+  __half* h;     // aliases qkv + ctx; fp8 precision: e4m3 [M,F], followed by its scales h_s [F/128, M]
+  float* xn_s;
+  float* h_s;
   AttnScratch as;
   size_t bytes;  // size of the whole layout, including 1024 bytes to align the caller's pointer
 };
 
-// the one definition of the layer workspace: nullptr measures it (esmb200_workspace_bytes), a device pointer carves it
-Workspace workspace_layout(void* workspace, int E, int H, int F, int B, int T, int split) {
-  const size_t M = (size_t)B * T, Ea = (size_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;
+// the one definition of the layer workspace: nullptr measures it (esmb200_workspace_bytes), a device pointer carves it.
+// precision 2 (fp8): xn and h are e4m3 with their scale arrays behind them; q, k, v and ctx stay fp16.
+Workspace workspace_layout(void* workspace, int E, int H, int F, int B, int T, int precision) {
+  const bool fp8 = precision == 2;
+  const size_t M = (size_t)B * T, Ea = (size_t)64 * head_slots(E, H) * H, pf = precision && !fp8 ? 2 : 1;
   const uintptr_t base = workspace ? align_up(reinterpret_cast<uintptr_t>(workspace), 1024) : 0;
-  const size_t xn = align_up(M * E * 2 * pf, 1024);  // fp16 [M,E] (hi | lo)
+  const size_t xn_q = fp8 ? align_up(M * E, 1024) : 0, h_q = fp8 ? align_up(M * F, 1024) : 0;
+  const size_t xn = fp8 ? xn_q + align_up((size_t)kblocks(E) * M * 4, 1024)
+                        : align_up(M * E * 2 * pf, 1024);  // fp16 [M,E] (hi | lo)
   const size_t qkv = align_up(M * 3 * Ea * 2 * pf, 1024), ctx = align_up(M * Ea * 2 * pf, 1024);
-  const size_t h = align_up(M * F * 2 * pf, 1024);
+  const size_t h = fp8 ? h_q + align_up((size_t)kblocks(F) * M * 4, 1024) : align_up(M * F * 2 * pf, 1024);
   const size_t scratch = xn + (qkv + ctx > h ? qkv + ctx : h);
   Workspace ws;
   ws.xn = reinterpret_cast<__half*>(base);
   ws.qkv = ws.h = reinterpret_cast<__half*>(base + xn);
   ws.ctx = reinterpret_cast<__half*>(base + xn + qkv);
+  ws.xn_s = fp8 ? reinterpret_cast<float*>(base + xn_q) : nullptr;
+  ws.h_s = fp8 ? reinterpret_cast<float*>(base + xn + h_q) : nullptr;
   ws.as = attn_scratch_layout(base + scratch, B, T, H);
   ws.bytes = scratch + ws.as.bytes + 1024;
   return ws;
@@ -460,12 +550,15 @@ int attention_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int 
                     const float* rope_sin, float q_scale, const Workspace& ws, const ActMaps& am, cudaStream_t st,
                     Attend attend) {
   const bool split = L->split != 0;
-  int rc = layernorm_f16(x, L->ln1_w, L->ln1_b, ws.xn, M, L->E, L->eps, split, T_LN1, st);
+  int rc = L->fp8 ? layernorm_fp8(x, L->ln1_w, L->ln1_b, ws.xn, ws.xn_s, M, L->E, L->eps, T_LN1, st)
+                  : layernorm_f16(x, L->ln1_w, L->ln1_b, ws.xn, M, L->E, L->eps, split, T_LN1, st);
   if (rc) return rc;
   GemmParams g = gemm_params(M, 3 * L->Ea, L->E, L->b_qkv);
   g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.rope_ld = 32 * L->slots; g.T = T; g.E = L->Ea; g.q_scale = q_scale;
   g.lo_col_off = 3 * L->Ea;
-  if ((rc = launch_gemm(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, g, st, T_QKV, split))) return rc;
+  rc = L->fp8 ? launch_gemm_fp8(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, {g, ws.xn_s, L->s_qkv, nullptr}, st, T_QKV)
+              : launch_gemm(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, g, st, T_QKV, split);
+  if (rc) return rc;
   if ((rc = attend())) return rc;
   return launch_gemm(EPI_BIAS_RESIDUAL, am.ctx, wm.out, am.x_o, gemm_params(M, L->E, L->Ea, L->out_b), st, T_OUT,
                      split);
@@ -475,6 +568,16 @@ int attention_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int 
 int ffn_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int M, const Workspace& ws, const ActMaps& am,
               cudaStream_t st) {
   const bool split = L->split != 0;
+  if (L->fp8) {
+    int rc = layernorm_fp8(x, L->ln2_w, L->ln2_b, ws.xn, ws.xn_s, M, L->E, L->eps, T_LN2, st);
+    if (!rc)
+      rc = launch_gemm_fp8(EPI_GELU_FP8, am.xn, wm.fc1, am.h_o, {gemm_params(M, L->F, L->E, L->fc1_b), ws.xn_s,
+                                                                  L->s_fc1, ws.h_s}, st, T_FC1);
+    if (!rc)
+      rc = launch_gemm_fp8(EPI_BIAS_RESIDUAL, am.h, wm.fc2, am.x_o, {gemm_params(M, L->E, L->F, L->fc2_b), ws.h_s,
+                                                                      L->s_fc2, nullptr}, st, T_FC2);
+    return rc;
+  }
   int rc = layernorm_f16(x, L->ln2_w, L->ln2_b, ws.xn, M, L->E, L->eps, split, T_LN2, st);
   if (rc) return rc;
   GemmParams g = gemm_params(M, L->F, L->E, L->fc1_b);
@@ -484,13 +587,18 @@ int ffn_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int M, con
                      split);
 }
 
-int make_act_maps(ActMaps* am, const Workspace& ws, float* x, int E, int H, int F, int M, int split = 0) {
-  const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = split ? 2 : 1;  // fp32x3: activations are [rows, 2 * width]
-  int rc = make_tmap_f16(&am->xn, ws.xn, M, pf * E, pf * E, gemm2_cfg::BOX_M);
+// precision 0 fp16, 1 fp32x3, 2 fp8 (xn and h e4m3)
+int make_act_maps(ActMaps* am, const Workspace& ws, float* x, int E, int H, int F, int M, int precision = 0) {
+  // fp32x3: activations are [rows, 2 * width]
+  const uint64_t Ea = (uint64_t)64 * head_slots(E, H) * H, pf = precision == 1 ? 2 : 1;
+  const int es = precision == 2 ? 1 : 2;  // element bytes of xn and h
+  // xn and h feed the fp8 GEMM in precision 2: its producer expects boxes of gemm_fp8_cfg::BOX_ROWS rows
+  const uint32_t box = precision == 2 ? gemm_fp8_cfg::BOX_ROWS : gemm2_cfg::BOX_M;
+  int rc = make_tmap_2d(&am->xn, ws.xn, es, M, pf * E, pf * E, box);
   if (!rc) rc = make_tmap_f16(&am->ctx, ws.ctx, M, pf * Ea, pf * Ea, gemm2_cfg::BOX_M);
-  if (!rc) rc = make_tmap_f16(&am->h, ws.h, M, pf * F, pf * F, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_tmap_2d(&am->h, ws.h, es, M, pf * F, pf * F, box);
   if (!rc) rc = make_gemm_out_map(&am->qkv_o, ws.qkv, 2, M, pf * 3 * Ea);
-  if (!rc) rc = make_gemm_out_map(&am->h_o, ws.h, 2, M, pf * F);
+  if (!rc) rc = make_gemm_out_map(&am->h_o, ws.h, es, M, pf * F);
   if (!rc) rc = make_gemm_out_map(&am->x_o, x, 4, M, E);
   return rc;
 }
@@ -621,6 +729,7 @@ int esmb200_layer_destroy(esmb200_layer* L) {
   cudaFree(L->w_fc1);
   cudaFree(L->w_fc2);
   cudaFree(L->b_qkv);
+  cudaFree(L->w8);
   delete L;
   return ESMB200_OK;
 }
@@ -637,9 +746,13 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   if (E % 16 != 0) return fail(ESMB200_EINVAL, "embed_dim must be a multiple of 16");
   const bool has_ffn = w->fc1_weight != nullptr;  // NULL fc1_weight: attention-only layer (MSA row-attention sub-layer)
   if (has_ffn && (F <= 0 || F % 64 != 0)) return fail(ESMB200_EINVAL, "ffn_dim must be a positive multiple of 64");
-  if (w->precision != 0 && w->precision != 1)
-    return fail(ESMB200_EINVAL, "precision must be 0 (fp16 operands) or 1 (fp32x3: fp16 hi|lo operands)");
-  const int split = w->precision;
+  if (w->precision < 0 || w->precision > 2)
+    return fail(ESMB200_EINVAL,
+                "precision must be 0 (fp16 operands), 1 (fp32x3: fp16 hi|lo operands) or 2 (fp8: e4m3 QKV/fc1/fc2)");
+  if (w->precision == 2 && (!has_ffn || F % 128 != 0))
+    return fail(ESMB200_EINVAL, "fp8 precision needs a feed-forward layer with ffn_dim % 128 == 0 (ESM-2, ESM-1b/1v)");
+  const int split = w->precision == 1;
+  const int fp8 = w->precision == 2;
   const int slots = head_slots(E, H);
   if (split && slots == 2) return fail(ESMB200_EINVAL, "fp32x3 precision is not available for head_dim > 64");
   if (split && E % 64 != 0)
@@ -653,6 +766,7 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   L->ln1_w = w->ln1_weight; L->ln1_b = w->ln1_bias; L->ln2_w = w->ln2_weight; L->ln2_b = w->ln2_bias;
   L->out_b = w->out_bias; L->fc1_b = w->fc1_bias; L->fc2_b = w->fc2_bias;
   L->split = split;
+  L->fp8 = fp8;
   const size_t pf = split ? 2 : 1;  // fp32x3: every K extent doubles (hi | lo)
   const size_t EaE = (size_t)Ea * E, EF = (size_t)E * F;
   cudaError_t e;
@@ -661,23 +775,49 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
     esmb200_layer_destroy(L);                                          \
     return fail_cuda(e, "cudaMalloc(packed weights)");                 \
   }
-  ALLOC(L->w_qkv, 3 * EaE * 2 * pf);
+  const Fp8Layout fl = fp8_layout(E, Ea, F);
+  if (fp8) {
+    ALLOC(L->w8, fl.bytes);
+    L->q_qkv = L->w8 + fl.qkv; L->q_fc1 = L->w8 + fl.fc1; L->q_fc2 = L->w8 + fl.fc2;
+    L->s_qkv = reinterpret_cast<float*>(L->w8 + fl.s_qkv);
+    L->s_fc1 = reinterpret_cast<float*>(L->w8 + fl.s_fc1);
+    L->s_fc2 = reinterpret_cast<float*>(L->w8 + fl.s_fc2);
+  } else {
+    ALLOC(L->w_qkv, 3 * EaE * 2 * pf);
+  }
   ALLOC(L->w_out, EaE * 2 * pf);
-  if (has_ffn) {
+  if (has_ffn && !fp8) {
     ALLOC(L->w_fc1, EF * 2 * pf);
     ALLOC(L->w_fc2, EF * 2 * pf);
   }
   ALLOC(L->b_qkv, (size_t)3 * Ea * 4);
 #undef ALLOC
   // every head goes into its zero-padded 64-wide slot(s) (elementwise.cuh head_slot; for head_dim 64 the identity)
-  e = cudaMemsetAsync(L->w_qkv, 0, 3 * EaE * 2 * pf, st);
+  e = fp8 ? cudaSuccess : cudaMemsetAsync(L->w_qkv, 0, 3 * EaE * 2 * pf, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(L->w_out, 0, EaE * 2 * pf, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(L->b_qkv, 0, (size_t)3 * Ea * 4, st);
   if (e != cudaSuccess) rc = fail_cuda(e, "memset(packed weights)");
   const float* ws3[3] = {w->q_weight, w->k_weight, w->v_weight};
   const float* bs3[3] = {w->q_bias, w->k_bias, w->v_bias};
   const unsigned blocks = (unsigned)(((size_t)E * E + 255) / 256);
-  for (int s3 = 0; s3 < 3 && !rc; ++s3) {
+  if (fp8 && !rc) {
+    // [Wq;Wk;Wv] into their head slots as fp32, then 128 x 128 block quantisation; fc1 and fc2 straight from the caller
+    float* staged = nullptr;
+    e = cudaMallocAsync(reinterpret_cast<void**>(&staged), 3 * EaE * 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(staged, 0, 3 * EaE * 4, st);
+    for (int s3 = 0; s3 < 3 && e == cudaSuccess; ++s3) {
+      ProfScope ps(T_CONVERT, st);
+      pack_head_rows_f32_kernel<<<blocks, 256, 0, st>>>(ws3[s3], bs3[s3], staged + (size_t)s3 * EaE,
+                                                        L->b_qkv + s3 * Ea, E, d);
+      e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) rc = fail_cuda(e, "pack_head_rows (fp8)");
+    if (!rc) rc = quantize_fp8(staged, L->q_qkv, L->s_qkv, 3 * Ea, E, 128, st);
+    if (staged) cudaFreeAsync(staged, st);
+    if (!rc) rc = quantize_fp8(w->fc1_weight, L->q_fc1, L->s_fc1, F, E, 128, st);
+    if (!rc) rc = quantize_fp8(w->fc2_weight, L->q_fc2, L->s_fc2, E, F, 128, st);
+  }
+  for (int s3 = 0; s3 < 3 && !rc && !fp8; ++s3) {
     ProfScope ps(T_CONVERT, st);
     pack_head_rows_kernel<<<blocks, 256, 0, st>>>(ws3[s3], bs3[s3], L->w_qkv + (size_t)s3 * EaE * pf, L->b_qkv + s3 * Ea,
                                                   E, d, split);
@@ -688,9 +828,10 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
     pack_head_cols_kernel<<<blocks, 256, 0, st>>>(w->out_weight, L->w_out, E, Ea, d, split);
     if ((e = cudaGetLastError()) != cudaSuccess) rc = fail_cuda(e, "pack_head_cols");
   }
-  if (!rc && has_ffn) rc = convert_f16(w->fc1_weight, L->w_fc1, F, E, split, st);
-  if (!rc && has_ffn) rc = convert_f16(w->fc2_weight, L->w_fc2, E, F, split, st);
-  if (!rc) rc = make_weight_maps(&L->tm, L->w_qkv, L->w_out, L->w_fc1, L->w_fc2, E, Ea, L->F, split);
+  if (!rc && has_ffn && !fp8) rc = convert_f16(w->fc1_weight, L->w_fc1, F, E, split, st);
+  if (!rc && has_ffn && !fp8) rc = convert_f16(w->fc2_weight, L->w_fc2, E, F, split, st);
+  if (!rc) rc = fp8 ? make_weight_maps_fp8(&L->tm, L)
+                    : make_weight_maps(&L->tm, L->w_qkv, L->w_out, L->w_fc1, L->w_fc2, E, Ea, L->F, split);
   if (rc) {
     esmb200_layer_destroy(L);
     return rc;
@@ -718,6 +859,7 @@ int esmb200_layer_offload(esmb200_layer* L, void* host_dst, size_t bytes, void* 
   if (!L || !host_dst) return fail(ESMB200_EINVAL, "null argument");
   if (L->host) return fail(ESMB200_EINVAL, "layer is already offloaded");
   if (L->F <= 0) return fail(ESMB200_EINVAL, "attention-only layers cannot be offloaded");
+  if (L->fp8) return fail(ESMB200_EINVAL, "fp8 layers cannot be offloaded: streamed layers run fp16 or fp32x3");
   const PackedLayout p = packed_layout(L->E, L->H, L->F, L->split);
   if (bytes < p.bytes) return fail(ESMB200_EINVAL, "host buffer smaller than esmb200_layer_packed_bytes");
   int rc = check_device();
@@ -772,7 +914,8 @@ static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, fl
   const int E = layers[0]->E, F = layers[0]->F, H = layers[0]->H;
   if (F <= 0) return fail(ESMB200_EINVAL, "attention-only layers belong to esmb200_axial_stack_forward");
   for (int i = 1; i < n_layers; ++i)
-    if (layers[i]->E != E || layers[i]->F != F || layers[i]->H != H || layers[i]->split != layers[0]->split)
+    if (layers[i]->E != E || layers[i]->F != F || layers[i]->H != H || layers[i]->split != layers[0]->split ||
+        layers[i]->fp8 != layers[0]->fp8)
       return fail(ESMB200_EINVAL, "layers of one stack must share E, H, F and precision");
   const bool streamed = ring != nullptr;
   for (int i = 0; i < n_layers; ++i)
@@ -783,10 +926,11 @@ static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, fl
                                                 : " is offloaded to host memory (esmb200_layer_offload): run it with "
                                                   "esmb200_stack_forward_streamed"));
   const int split = layers[0]->split;
-  const Workspace ws = workspace_layout(workspace, E, H, F, B, T, split);
+  const int precision = layers[0]->fp8 ? 2 : split;
+  const Workspace ws = workspace_layout(workspace, E, H, F, B, T, precision);
   if (workspace_bytes < ws.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   ActMaps am;
-  rc = make_act_maps(&am, ws, x, E, H, F, B * T, split);
+  rc = make_act_maps(&am, ws, x, E, H, F, B * T, precision);
   if (rc) return rc;
   WeightRing wr;
   if (streamed) {
@@ -927,6 +1071,47 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
                           float eps, void* stream) {
   if (!x || !weight || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
   return layernorm_f16(x, weight, bias, out, M, E, eps, false, T_LN1, static_cast<cudaStream_t>(stream));
+}
+
+int esmb200_layernorm_fp8(const float* x, const float* weight, const float* bias, void* out_e4m3, float* scales,
+                          int32_t M, int32_t E, float eps, void* stream) {
+  if (!x || !weight || !bias || !out_e4m3 || !scales) return fail(ESMB200_EINVAL, "null argument");
+  if (M <= 0 || E <= 0 || E % 4 != 0 || E > 40 * 128) return fail(ESMB200_EINVAL, "bad shape");
+  return layernorm_fp8(x, weight, bias, out_e4m3, scales, M, E, eps, T_LN1, static_cast<cudaStream_t>(stream));
+}
+
+int esmb200_quantize_fp8(const float* src, void* dst_e4m3, float* scales, int32_t rows, int32_t K, int32_t block_rows,
+                         void* stream) {
+  if (!src || !dst_e4m3 || !scales) return fail(ESMB200_EINVAL, "null argument");
+  if (rows <= 0 || K <= 0 || (block_rows != 1 && block_rows != 128) || rows / block_rows > 65535)
+    return fail(ESMB200_EINVAL, "quantize_fp8 needs rows, K > 0 and block_rows 1 or 128");
+  return quantize_fp8(src, static_cast<uint8_t*>(dst_e4m3), scales, rows, K, block_rows,
+                      static_cast<cudaStream_t>(stream));
+}
+
+int esmb200_gemm_fp8(int32_t epilogue, const void* a, const float* a_scales, const void* w, const float* w_scales,
+                     const float* bias, void* out, float* out_scales, int32_t M, int32_t N, int32_t K,
+                     const float* rope_cos, const float* rope_sin, int32_t T, int32_t E, void* stream) {
+  if (!a || !a_scales || !w || !w_scales || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
+  if (M <= 0 || N <= 0 || K <= 0 || K % 16 != 0) return fail(ESMB200_EINVAL, "fp8 gemm needs M, N > 0 and K % 16 == 0");
+  if (epilogue == EPI_QKV_ROPE &&
+      (N % 64 != 0 || !rope_cos || !rope_sin || T <= 0 || E <= 0 || E % 64 != 0 || N != 3 * E))
+    return fail(ESMB200_EINVAL, "qkv epilogue needs rope tables, T and N == 3E, E % 64 == 0");
+  if (epilogue == EPI_BIAS_RESIDUAL && N % 32 != 0) return fail(ESMB200_EINVAL, "residual epilogue needs N % 32 == 0");
+  if (epilogue == EPI_GELU_FP8 && (N % 128 != 0 || !out_scales))
+    return fail(ESMB200_EINVAL, "gelu -> fp8 epilogue needs N % 128 == 0 and out_scales");
+  if (epilogue != EPI_QKV_ROPE && epilogue != EPI_BIAS_RESIDUAL && epilogue != EPI_GELU_FP8)
+    return fail(ESMB200_EINVAL, "fp8 gemm epilogue must be 0 (qkv), 1 (residual) or 5 (gelu -> fp8)");
+  int rc = check_device();
+  if (rc) return rc;
+  CUtensorMap ta, tb, to;
+  rc = make_tmap_2d(&ta, a, 1, M, K, K, gemm_fp8_cfg::BOX_ROWS);
+  if (!rc) rc = make_tmap_2d(&tb, w, 1, N, K, K, gemm_fp8_cfg::BOX_ROWS);
+  if (!rc) rc = make_gemm_out_map(&to, out, epilogue == EPI_QKV_ROPE ? 2 : epilogue == EPI_GELU_FP8 ? 1 : 4, M, N);
+  if (rc) return rc;
+  GemmParams g = gemm_params(M, N, K, bias);
+  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.T = T; g.E = E; g.q_scale = 0.125f;
+  return launch_gemm_fp8(epilogue, ta, tb, to, {g, a_scales, w_scales, out_scales}, static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_gemm_f16(int32_t epilogue, const void* a, const void* w, const float* bias, void* out, int32_t M,
@@ -1105,6 +1290,9 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   int rc = check_device();
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int i = 0; i < n_layers; ++i)
+    if ((row_layers[i] && row_layers[i]->fp8) || (col_layers[i] && col_layers[i]->fp8))
+      return fail(ESMB200_EINVAL, "the MSA axial stack runs fp16 or fp32x3 layers, not fp8");
   const int E = col_layers[0]->E, F = col_layers[0]->F, H = col_layers[0]->H;
   if (F <= 0) return fail(ESMB200_EINVAL, "col_layers carry the feed-forward weights");
   const int split = col_layers[0]->split;

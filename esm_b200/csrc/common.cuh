@@ -456,6 +456,30 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// ---------------------------------------------------------------------------------------------
+// fp8 (e4m3) block scaling: q = e4m3(x / s) with s a power of two per block, so x / s and q * s are exact
+// ---------------------------------------------------------------------------------------------
+// The smallest power of two s with amax / s <= 448 (e4m3's largest finite value), from the exponent bits: amax = m 2^e
+// with m in [1, 2) needs s = 2^(e - 8) when m <= 1.75 (448 = 1.75 * 2^8), else 2^(e - 7).  1 for amax == 0; never
+// below 2^-126, so s is a normal float (an amax under 2^-118 then gives amax / s < 256).
+__device__ __forceinline__ float fp8_block_scale(float amax) {
+  if (amax == 0.f) return 1.0f;
+  const uint32_t b = __float_as_uint(amax);
+  const int e = (int)(b >> 23) - 8 + ((b & 0x7fffffu) > 0x600000u ? 1 : 0);
+  return __uint_as_float((uint32_t)(e < 1 ? 1 : e) << 23);
+}
+// two fp32 values -> e4m3 (round to nearest even, saturating), lo in the low byte
+__device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 // named barrier for a subset of warps (id 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -18,11 +18,13 @@ namespace esmb200 {
 
 // Each lane owns float4 chunks lane, lane+32, ... of the row. MAXV bounds E <= MAXV*128.
 // OUT: 0 = fp32 [M,E]; 1 = fp16 [M,E] (GEMM A operand); 2 = fp16 hi | lo [M,2E] (A operand of the fp32x3 GEMMs:
-// hi = rn(y) in columns [0,E), lo = rn(y - hi) in columns [E,2E)).
+// hi = rn(y) in columns [0,E), lo = rn(y - hi) in columns [E,2E)); 3 = e4m3 [M,E] and one power-of-two scale per row
+// and 128 columns, scales[kb * M + row] (A operand of the fp8 GEMMs: a lane's float4 chunk i lies in 128-column block i,
+// so a block's amax is one warp reduction).
 template <int MAXV, int OUT>
 __global__ void __launch_bounds__(256)
 layernorm_rows_kernel(const float* x, const float* __restrict__ gamma, const float* __restrict__ beta, void* out, int M,
-                      int E, float eps) {  // x and out may alias (in-place final LayerNorm): a warp reads its whole row first
+                      int E, float eps, float* scales) {  // x and out may alias (in-place final LayerNorm): a warp reads its whole row first
   const int warps_per_block = blockDim.x / 32;
   const int row = blockIdx.x * warps_per_block + threadIdx.x / 32;
   if (row >= M) return;
@@ -54,6 +56,28 @@ layernorm_rows_kernel(const float* x, const float* __restrict__ gamma, const flo
   const float rstd = rsqrtf(warp_sum(q) / (float)E + eps);
   const float4* g4 = reinterpret_cast<const float4*>(gamma);
   const float4* b4 = reinterpret_cast<const float4*>(beta);
+  if constexpr (OUT == 3) {
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      if (i * 128 >= E) break;  // warp-uniform: every lane takes part in the block's reduction
+      const int idx = lane + i * 32;
+      float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (idx < nvec) {
+        const float4 g = __ldg(g4 + idx), b = __ldg(b4 + idx);
+        o.x = (v[i].x - mean) * rstd * g.x + b.x;
+        o.y = (v[i].y - mean) * rstd * g.y + b.y;
+        o.z = (v[i].z - mean) * rstd * g.z + b.z;
+        o.w = (v[i].w - mean) * rstd * g.w + b.w;
+      }
+      const float sc = fp8_block_scale(warp_max(fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w)))));
+      const float inv = __frcp_rn(sc);  // o * inv == o / sc exactly
+      if (idx < nvec)
+        reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(out) + (size_t)row * E)[idx] =
+            (uint32_t)cvt_e4m3x2(o.x * inv, o.y * inv) | ((uint32_t)cvt_e4m3x2(o.z * inv, o.w * inv) << 16);
+      if (lane == 0) scales[(size_t)i * M + row] = sc;
+    }
+    return;
+  }
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
     const int idx = lane + i * 32;
@@ -89,16 +113,19 @@ layernorm_rows_kernel(const float* x, const float* __restrict__ gamma, const flo
 
 template <int OUT>
 inline cudaError_t launch_layernorm(const float* x, const float* gamma, const float* beta, void* out, int M, int E,
-                                    float eps, cudaStream_t stream) {
+                                    float eps, cudaStream_t stream, float* scales = nullptr) {
   if (E % 4 != 0 || E > 40 * 128) return cudaErrorInvalidValue;
   const int wpb = 8;
   const int grid = (M + wpb - 1) / wpb;
   if (grid == 0) return cudaSuccess;
   const dim3 g(grid), b(wpb * 32);
-  if (E <= 4 * 128) return launch_pdl(layernorm_rows_kernel<4, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps);
-  if (E <= 10 * 128) return launch_pdl(layernorm_rows_kernel<10, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps);
-  if (E <= 20 * 128) return launch_pdl(layernorm_rows_kernel<20, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps);
-  return launch_pdl(layernorm_rows_kernel<40, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps);
+  if (E <= 4 * 128) return launch_pdl(layernorm_rows_kernel<4, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps,
+                                         scales);
+  if (E <= 10 * 128) return launch_pdl(layernorm_rows_kernel<10, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps,
+                                         scales);
+  if (E <= 20 * 128) return launch_pdl(layernorm_rows_kernel<20, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps,
+                                         scales);
+  return launch_pdl(layernorm_rows_kernel<40, OUT>, g, b, 0, stream, x, gamma, beta, out, M, E, eps, scales);
 }
 
 // grid (row chunks, B): every block counts the <mask>/<pad> tokens of its sequence (T 8-byte reads, cheaper than a
@@ -296,6 +323,45 @@ __global__ void pack_head_cols_kernel(const float* __restrict__ w, __half* __res
   const size_t pitch = split ? 2 * (size_t)Ea : (size_t)Ea;
   dst[(size_t)n * pitch + head_slot(k, d)] = h;
   if (split) dst[(size_t)n * pitch + Ea + head_slot(k, d)] = __float2half_rn(w[i] - __half2float(h));
+}
+
+// fp8 precision: the QKV weight rows in their head slots as fp32 (w [E,E] -> dst [Ea, E], zero-filled by the caller), so
+// that the 128 x 128 block quantisation sees exactly the fp32 weights
+__global__ void pack_head_rows_f32_kernel(const float* __restrict__ w, const float* __restrict__ b, float* __restrict__ dst,
+                                          float* __restrict__ bdst, int E, int d) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)E * E) return;
+  const int n = (int)(i / E), k = (int)(i % E);
+  const int r = head_slot(n, d);
+  dst[(size_t)r * E + k] = w[i];
+  if (k == 0) bdst[r] = b[n];
+}
+
+// fp32 [rows, K] -> e4m3 [rows, K], one power-of-two scale (fp8_block_scale) per block of block_rows x 128 columns:
+// block_rows 1 (activations; scales [ceil(K/128), rows]) or 128 (weights; scales [ceil(rows/128), ceil(K/128)]).
+// A partial block takes its scale over its valid elements.  Grid (ceil(K/128), ceil(rows/block_rows)), 256 threads.
+__global__ void __launch_bounds__(256)
+quantize_fp8_kernel(const float* __restrict__ src, uint8_t* __restrict__ dst, float* __restrict__ scales, int rows, int K,
+                    int block_rows) {
+  __shared__ float red[8];
+  const int kb = blockIdx.x, r_lo = blockIdx.y * block_rows, k0 = kb * 128;
+  const int nr = min(block_rows, rows - r_lo), nk = min(128, K - k0);
+  float m = 0.f;
+  for (int e = threadIdx.x; e < nr * 128; e += 256)
+    if (e % 128 < nk) m = fmaxf(m, fabsf(src[(size_t)(r_lo + e / 128) * K + k0 + e % 128]));
+  m = warp_max(m);
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = m;
+  __syncthreads();
+  m = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) m = fmaxf(m, red[w]);
+  const float sc = fp8_block_scale(m), inv = __frcp_rn(sc);
+  for (int e = threadIdx.x; e < nr * 128; e += 256)
+    if (e % 128 < nk) {
+      const size_t at = (size_t)(r_lo + e / 128) * K + k0 + e % 128;
+      dst[at] = (uint8_t)(cvt_e4m3x2(src[at] * inv, 0.f) & 0xffu);
+    }
+  if (threadIdx.x == 0) scales[block_rows == 1 ? (size_t)kb * rows + r_lo : (size_t)blockIdx.y * gridDim.x + kb] = sc;
 }
 
 // MSA row attention: q is zeroed at padded positions before the logits are summed over the alignment rows

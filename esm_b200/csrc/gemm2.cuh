@@ -34,17 +34,6 @@ constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: 
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * OUT_BUFS * OUT_BOX_BYTES + 1024 + 256;  // 230656 B
 }  // namespace gemm2_cfg
 
-// An fp16 64 x 64 output box of one MMA warpgroup into a 128B-swizzled staging buffer (the layout the output TMA map
-// reads): h[2 b + hr] holds the warp's rows g + 8 hr, columns 8 b + 2 c ..+1 (the accumulator fragment layout, which is
-// stmatrix's).  Each x4 writes blocks 2s, 2s + 1 for both row halves; 8 rows x 16 bytes per matrix, conflict-free.
-__device__ __forceinline__ void stage_box_f16(uint32_t buf, uint32_t warp, uint32_t lane, const uint32_t (&h)[16]) {
-  const uint32_t m = lane / 8;  // matrix this lane addresses: block 2s + m / 2, row half m % 2
-#pragma unroll
-  for (int s = 0; s < 4; ++s)
-    stsm_x4(sw128(buf, warp * 16 + (m % 2) * 8 + lane % 8, 2 * s + m / 2), h[4 * s], h[4 * s + 1], h[4 * s + 2],
-            h[4 * s + 3]);
-}
-
 // SPLIT ("fp32x3" precision): both operands are stored as fp16 hi | lo halves along K (A [M,2K], B [N,2K]); the K loop
 // runs hi*hi + lo*hi + hi*lo (three passes over the same fp32 accumulator: 22 significand bits per operand, the
 // dropped lo*lo term is 2^-22 relative), and fp16 outputs are written as hi | lo pairs as well (lo part p.lo_col_off
@@ -175,56 +164,8 @@ gemm2_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         const int col0 = n0 + gi * 64;
         if (col0 >= p.N) break;
         uint32_t hi[16], lo[16];  // [2 b + hr]: 8-column block b of the box, rows r0 + 8 hr
-        if constexpr (EPI == EPI_QKV_ROPE) {  // column j pairs with j + 32 (same thread)
-          const int sect = col0 / p.E;  // 0 q, 1 k, 2 v
-          const float sc = (sect == 0) ? p.q_scale : 1.0f;
-          // Every bias / table load of the box is issued before the first is used: one memory latency per box rather
-          // than one per column pair (the rotation's branch would otherwise split them into dependent steps).
-          float2 bl[4], bh[4], cs[2][4], sn[2][4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            bl[q] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * q + 2 * (int)c));
-            bh[q] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 32 + 8 * q + 2 * (int)c));
-          }
-          const bool rotate = sect < 2 && p.rope_cos != nullptr;  // uniform over the box
-          if (rotate) {
-            const int ld = p.rope_ld == 64 ? 64 : 32;
-            const int slot = p.rope_ld == 64 ? ((col0 >> 6) & 1) : 0;
-#pragma unroll
-            for (int hr = 0; hr < 2; ++hr) {
-              const int t = (r0 + 8 * hr) % p.T;  // rows >= M read a valid table row too; TMA drops them
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const size_t at = (size_t)t * ld + slot * 32 + 8 * q + 2 * (int)c;
-                cs[hr][q] = __ldg(reinterpret_cast<const float2*>(p.rope_cos + at));
-                sn[hr][q] = __ldg(reinterpret_cast<const float2*>(p.rope_sin + at));
-              }
-            }
-          }
-#pragma unroll
-          for (int hr = 0; hr < 2; ++hr) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {  // column pair (j, j + 1) and (j + 32, j + 33) of the box, j = 8 q + 2 c
-              float a0 = (acc[4 * (8 * gi + q) + 2 * hr] + bl[q].x) * sc;
-              float a1 = (acc[4 * (8 * gi + q) + 2 * hr + 1] + bl[q].y) * sc;
-              float b0 = (acc[4 * (8 * gi + q + 4) + 2 * hr] + bh[q].x) * sc;
-              float b1 = (acc[4 * (8 * gi + q + 4) + 2 * hr + 1] + bh[q].y) * sc;
-              if (rotate) {  // rotary_embedding.py:16-20, rotate_half = cat(-x2, x1)
-                const float2 co = cs[hr][q], si = sn[hr][q];
-                const float ra0 = a0 * co.x - b0 * si.x, rb0 = b0 * co.x + a0 * si.x;
-                const float ra1 = a1 * co.y - b1 * si.y, rb1 = b1 * co.y + a1 * si.y;
-                a0 = ra0; b0 = rb0; a1 = ra1; b1 = rb1;
-              }
-              hi[2 * q + hr] = pack_half2(a0, a1);
-              hi[2 * (q + 4) + hr] = pack_half2(b0, b1);
-              if constexpr (SPLIT) {
-                const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * q + hr]));
-                const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * (q + 4) + hr]));
-                lo[2 * q + hr] = pack_half2(a0 - fa.x, a1 - fa.y);
-                lo[2 * (q + 4) + hr] = pack_half2(b0 - fb.x, b1 - fb.y);
-              }
-            }
-          }
+        if constexpr (EPI == EPI_QKV_ROPE) {
+          epi_qkv_box<SPLIT>(acc + 32 * gi, p, col0, r0, c, hi, lo);
         } else {
 #pragma unroll
           for (int b = 0; b < 8; ++b) {

@@ -43,8 +43,9 @@ def create_parser():
     p.add_argument("--repr_layers", type=int, default=[-1], nargs="+")
     p.add_argument("--include", type=str, nargs="+", choices=list(INCLUDE_CHOICES), required=True)
     p.add_argument("--truncation_seq_length", type=int, default=1022)
-    p.add_argument("--precision", choices=["fp16", "fp32x3"], default="fp16",
-                   help="fp16: fp16 MMA operands (default, fastest); fp32x3: hi+lo operand pairs, fp32-grade results (~2.6x slower)")
+    p.add_argument("--precision", choices=["fp16", "fp32x3", "fp8"], default="fp16",
+                   help="fp16: fp16 MMA operands (default); fp32x3: hi+lo operand pairs, fp32-grade results (~2.6x "
+                        "slower); fp8: e4m3 QKV/fc1/fc2 projections with block scales (faster, less accurate)")
     p.add_argument("--cpu-offload", action="store_true",
                    help="keep the transformer layers' weights in pinned host memory and stream them to the GPU layer "
                         "by layer (ESM-2 15B on one GPU); same outputs")

@@ -102,7 +102,7 @@ class LayerBinding:
         if self.head_dim * self.attention_heads != self.embed_dim or self.head_dim > 128 or self.head_dim % 2:
             raise ValueError("esm_b200 supports even head_dim <= 128 (every ESM-2 model); "
                              f"got embed_dim={self.embed_dim}, heads={self.attention_heads}")
-        self.precision = 0  # 0 = fp16 MMA operands, 1 = "fp32x3" (esmb200.h: esmb200_layer_weights.precision)
+        self.precision = 0  # 0 = fp16 MMA operands, 1 = "fp32x3", 2 = "fp8" (esmb200.h: esmb200_layer_weights.precision)
         self._handle = None
         self._key = None
         self._keep = None
@@ -565,7 +565,9 @@ class ProteinLanguageModel(nn.Module):
         self.precision = "fp16"
         self._offload = None  # cpu_offload(): (device, pinned arena)
 
-    PRECISIONS = {"fp16": 0, "fp32x3": 1}
+    PRECISIONS = {"fp16": 0, "fp32x3": 1}  # the precisions the MSA Transformer shares
+    # every precision of the ESM-2 / ESM-1b layer stack (esmb200_layer_weights.precision): PRECISIONS and "fp8"
+    LAYER_PRECISIONS = {**PRECISIONS, "fp8": 2}
 
     def cpu_offload(self, device=None) -> "ProteinLanguageModel":
         """Run on `device` (default: the current CUDA device) with the transformer layers' weights in host memory, the
@@ -577,6 +579,8 @@ class ProteinLanguageModel(nn.Module):
         with results bit-identical to the resident model.  At 15B the device then holds two layers' matrices (1.26 GB)
         instead of 30 GB.  set_precision() and in-place changes of a host parameter re-pack as usual; model.cuda(),
         .to() or any other module conversion ends the mode and frees the arena."""
+        if self.precision == "fp8":
+            raise _lib.Esmb200Error("cpu_offload() streams fp16 or fp32x3 layers; fp8 layers stay resident")
         if not torch.cuda.is_available():
             raise _lib.Esmb200Error("cpu_offload() streams the layers to a CUDA (sm_90a) device; none is available")
         device = torch.device("cuda") if device is None else torch.device(device)
@@ -595,7 +599,7 @@ class ProteinLanguageModel(nn.Module):
             if layer.self_attn.rot_emb is not None:  # rope tables are built on the device
                 layer.self_attn.rot_emb.to(device)
         nbytes = lib.esmb200_layer_packed_bytes(self.embed_dim, self.attention_heads, layers[0].ffn_embed_dim,
-                                                self.PRECISIONS[self.precision])
+                                                self.LAYER_PRECISIONS[self.precision])
         # one arena: torch's pinned allocator rounds every allocation up to a power of two
         arena = torch.empty(len(layers) * nbytes, dtype=torch.uint8, pin_memory=True)
         self._offload = (device, arena)
@@ -622,15 +626,23 @@ class ProteinLanguageModel(nn.Module):
         "fp32x3": every MMA operand (LayerNorm output, weights, q, k, v, softmax probabilities, context, FFN hidden) is
         an fp16 hi + lo pair and every product runs hi*hi + lo*hi + hi*lo into the fp32 accumulator: 22 significand bits
         per operand, fp32-grade parity with the reference at ~3x the tensor work (DESIGN.md section 4).  Needs
-        embed_dim % 64 == 0."""
-        if name not in self.PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(self.PRECISIONS)}")
+        embed_dim % 64 == 0.
+        "fp8": the QKV, fc1 and fc2 projections run e4m3 GEMMs with power-of-two block scales (activations one per row
+        and 128 columns, weights one per 128 x 128 block) and fp32 accumulation; attention, out_proj, LayerNorm
+        statistics, the residual stream and the LM head stay as in "fp16" (DESIGN.md section 4).  Not available on a
+        cpu_offload() model."""
+        ids = ProteinLanguageModel.LAYER_PRECISIONS
+        if name not in ids:
+            raise ValueError(f"precision must be one of {sorted(ids)}")
+        if name == "fp8" and self._offload is not None:
+            raise _lib.Esmb200Error("fp8 layers cannot be streamed from host memory: undo cpu_offload() (model.cuda()) "
+                                    "first")
         if name == "fp32x3" and (self.embed_dim % 64 != 0 or self.embed_dim // self.attention_heads > 64):
             raise ValueError("fp32x3 precision needs embed_dim % 64 == 0 and head_dim <= 64")
         changed = name != self.precision
         self.precision = name
         for layer in self.layers:
-            layer.precision = self.PRECISIONS[name]
+            layer.precision = ids[name]
         if changed and self._offload is not None:
             self.cpu_offload(self._offload[0])  # the packed size depends on the precision: a new arena
         return self
@@ -688,9 +700,10 @@ class ProteinLanguageModel(nn.Module):
             # esm2.py:111-121 layer loop (intermediate representations are copied out by the library)
             repr_out = {i - 1: torch.empty_like(x) for i in repr_layers if 0 < i < N}
             cos, sin = self._rope_tables(T)
-            # contacts: folded into the probability pass (fp16 mode; fp32x3 runs the separate kernels afterwards)
+            # contacts: folded into the probability pass (fp16 and fp8 modes, whose attention is the fp16 kernel; fp32x3
+            # runs the separate kernels afterwards)
             cjob = (self.contact_head.begin_job(tokens, N, self.attention_heads)
-                    if return_contacts and self.precision == "fp16" else None)
+                    if return_contacts and self.precision in ("fp16", "fp8") else None)
             attn_t = run_stack(list(self.layers), x, mask, cos, sin, repr_out,
                                list(range(N)) if need_head_weights else [], zero_pad_rows=True,
                                contact_job=cjob["job"] if cjob else None)
@@ -703,7 +716,11 @@ class ProteinLanguageModel(nn.Module):
         model.half()."""
         ln = self.emb_layer_norm_after
         ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)
-        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln_w, ln_b, ln.eps, self.PRECISIONS[self.precision])[0]
+        return self.lm_head.forward_native(x_rows.unsqueeze(0), ln_w, ln_b, ln.eps, self._lm_head_precision())[0]
+
+    def _lm_head_precision(self) -> int:
+        """RobertaLMHead.forward_native's precision id: 1 for fp32x3, else 0 (the fp8 mode's head runs fp16)."""
+        return int(self.precision == "fp32x3")
 
     @torch.no_grad()
     def forward(self, tokens, repr_layers=[], need_head_weights=False, return_contacts=False):
@@ -721,7 +738,7 @@ class ProteinLanguageModel(nn.Module):
             # esm2.py:129 LM head, from the pre-LN stream (its first step is the same emb_layer_norm_after)
             ln = self.emb_layer_norm_after
             ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)
-            logits = cast(self.lm_head.forward_native(x, ln_w, ln_b, ln.eps, self.PRECISIONS[self.precision]))
+            logits = cast(self.lm_head.forward_native(x, ln_w, ln_b, ln.eps, self._lm_head_precision()))
             # esm2.py:123-128 final LayerNorm; the last representation is post-LN
             _lib.check(lib.esmb200_layernorm(_ptr(x), _ptr(ln_w), _ptr(ln_b), _ptr(x), B * T, E, ln.eps, _stream()))
         if N in repr_layers:

@@ -75,7 +75,14 @@ typedef struct esmb200_layer_weights {
                             * q, k, v, P) is an fp16 hi | lo pair and every product runs hi*hi + lo*hi + hi*lo into the
                             * fp32 accumulator (22 significand bits per operand) — fp32-grade results at ~3x the tensor
                             * work; needs E % 64 == 0 and head_dim <= 64. On the MSA axial path every row and
-                            * column layer of one esmb200_axial_stack_forward call must share the precision */
+                            * column layer of one esmb200_axial_stack_forward call must share the precision.
+                            * 2 = "fp8": the QKV, fc1 and fc2 projections run e4m3 x e4m3 wgmma GEMMs with power-of-two
+                            * block scales (activations one per row and 128 columns, weights one per 128 x 128 block)
+                            * and an fp32 promotion per 128-wide K block; LayerNorm writes e4m3 + scales, fc1's
+                            * epilogue writes fc2's e4m3 operand + scales. Attention, out_proj, the residual stream
+                            * and the contact pass are those of precision 0. Needs a feed-forward layer with
+                            * ffn_dim % 128 == 0; not for the MSA axial stack (ESMB200_EINVAL) and not offloadable
+                            * (esmb200_layer_packed_bytes is 0, esmb200_layer_offload ESMB200_EINVAL) */
 } esmb200_layer_weights;
 
 int esmb200_abi_version(void);
@@ -297,6 +304,25 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
+
+/* ---- fp8 precision building blocks (e4m3 operands, power-of-two scales s: q = e4m3_rn(x / s), x ~ q * s; s is the
+ * smallest power of two with amax / s <= 448 over its block, at least 2^-126, and 1 for an all-zero block; a partial
+ * block takes its amax over its valid elements). Used by the fp8 layers and kernel-level tests.
+ * esmb200_layernorm_fp8: fp32 [M,E] -> LayerNorm -> e4m3 [M,E] + scales [ceil(E/128), M] (scales[kb * M + row]).
+ * esmb200_quantize_fp8:  fp32 [rows,K] -> e4m3 [rows,K]; block_rows 1: scales [ceil(K/128), rows] as above;
+ *                        block_rows 128 (weights): scales [ceil(rows/128), ceil(K/128)]. Deterministic.
+ * esmb200_gemm_fp8:      A [M,K] e4m3 with 1 x 128 scales (a_scales [ceil(K/128), M]), W [N,K] e4m3 with 128 x 128
+ *                        scales (w_scales [ceil(N/128), ceil(K/128)]), fp32 accumulation promoted per 128-wide K block.
+ *                        epilogue 0: qkv + rope -> fp16 [M,N] as esmb200_gemm_f16 (q_scale 0.125, N == 3E);
+ *                        1: out fp32 [M,N] += y + bias (N % 32 == 0); 5: erf-GELU(y + bias) -> e4m3 [M,N] with
+ *                        out_scales [N/128, M] (N % 128 == 0). K % 16 == 0. */
+int esmb200_layernorm_fp8(const float* x, const float* weight, const float* bias, void* out_e4m3, float* scales,
+                          int32_t M, int32_t E, float eps, void* stream);
+int esmb200_quantize_fp8(const float* src, void* dst_e4m3, float* scales, int32_t rows, int32_t K, int32_t block_rows,
+                         void* stream);
+int esmb200_gemm_fp8(int32_t epilogue, const void* a_e4m3, const float* a_scales, const void* w_e4m3,
+                     const float* w_scales, const float* bias, void* out, float* out_scales, int32_t M, int32_t N,
+                     int32_t K, const float* rope_cos, const float* rope_sin, int32_t T, int32_t E, void* stream);
 
 /* fp32 -> fp16 elementwise */
 int esmb200_convert_f16(const float* src, void* dst_f16, size_t n, void* stream);
