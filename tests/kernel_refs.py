@@ -8,7 +8,10 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
     head of model.py RobertaLMHead.forward_native, the MSA Transformer's layer in msa.py);
   * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf);
   * split16 / join64 / split_rep_bound / split_acc_bound / FP32X3_MODELS: the fp32x3 precision's hi | lo operand pairs,
-    the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs.
+    the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs;
+  * attention64 / attn_ctx_bound / attn_relfro_gate / attn_probs_bound / attn_rowsum_bound / attn_max_bound /
+    attn_sum_bound: float64 softmax attention on fp16 q, k, v and the first-order error model of the fp16 attention
+    kernels (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2).
 """
 from __future__ import annotations
 
@@ -178,6 +181,157 @@ def split_box_scale(K: int) -> float:
     """(3K/16 + 4) 2^-25: the scale of the per-output-box rel-Frobenius gate of the split GEMM (the accumulation drift
     of DESIGN.md section 4, per unit of relative size)."""
     return (3 * K / 16 + 4) * 2.0 ** -25
+
+
+# ---- fp16 attention -------------------------------------------------------------------------------------------------
+# The fp16 attention kernels, per key block of `block` keys (128: attention_wg_kernel, 64: attention_fwd_kernel<false,
+# 2>): S = q k^T on the tensor cores (fp32, truncating k16 steps over the head's D = 64 or 128 columns, both slots into
+# one accumulator); the exact running maximum m; e = ex2.approx(fma(s, log2e, -m log2e)) in fp32; l = alpha l + sum e
+# (fp32); O = alpha O + fp16(e) V (fp32, truncating k16 steps); ctx = fp16(O * (1 / l)).  alpha = ex2.approx((m_old - m)
+# log2e) multiplies O and l alike, so its own error cancels in ctx.  The probability kernel recomputes S (mma.sync,
+# another accumulation order than the wgmma forward) and writes ex2.approx(fma(s, log2e, -m log2e)) * (1 / l) with the
+# forward's saved m and l.
+F16_U = 2.0 ** -11  # unit roundoff of fp16
+
+
+def attention64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, padded: Optional[torch.Tensor], block: int) -> Dict:
+    """float64 softmax attention of fp16 q, k, v [B, H, T, D] (D = 64 or 128) under the key-padding mask `padded`
+    [B, T] (True: padded key; None: none), with what the error bounds below need.  Rows of an all-padding sequence are 0
+    (ctx, p, m and l).
+      * lerr [B,H,T,T]: the absolute error bound of each logit, (D/16 + 4) 2^-22 sum_d |q_d k_d| (the GEMM's
+        accumulation bound: D/16 truncating k16 steps, one ulp of a partial sum bounded by sum|q k| each, doubled,
+        plus 4 steps);
+      * delta [B,H,T,T]: the relative error bound Delta_j of key j's unnormalised weight e^(s_j - m): its logit (lerr),
+        ex2.approx (2 ulp = 2^-22, doubled) and the fp32 roundings of log2e, s log2e and -m log2e (2^-23 (|s| + 3 |m|));
+      * nblk [B,1,1,1]: the key blocks the kernel walks, ceil(kvlen / block), kvlen = 1 + the last attendable key."""
+    q, k, v = q.double(), k.double(), v.double()
+    B, H, T, D = q.shape
+    if padded is None:
+        padded = torch.zeros(B, T, dtype=torch.bool, device=q.device)
+    padded = padded.bool()
+    km = padded[:, None, None, :]
+    s = q @ k.transpose(-1, -2)
+    sm = s.masked_fill(km, float("-inf"))
+    m = sm.amax(-1, keepdim=True)
+    m = torch.where(torch.isinf(m), torch.zeros_like(m), m)
+    e = torch.exp(sm - m)
+    l = e.sum(-1, keepdim=True)
+    p = e / torch.where(l > 0, l, torch.ones_like(l))
+    lerr = ((D / 16 + 4) * 2.0 ** -22 * (q.abs() @ k.abs().transpose(-1, -2))).masked_fill(km, 0.0)
+    delta = (lerr + 2.0 ** -21 + 2.0 ** -23 * (s.abs() + 3 * m.abs())).masked_fill(km, 0.0)
+    idx = torch.arange(1, T + 1, device=q.device)
+    kvlen = torch.where(padded, torch.zeros_like(idx), idx).amax(-1)
+    nblk = ((kvlen + block - 1) // block).double()[:, None, None, None]
+    return dict(q=q, k=k, v=v, s=s, m=m, l=l, p=p, ctx=p @ v, lerr=lerr, delta=delta, nblk=nblk, km=km, block=block)
+
+
+def _vsum(r, f) -> torch.Tensor:
+    """[B,H,1,D]: sum over the attendable keys of f(v)"""
+    return f(r["v"]).masked_fill(r["km"].transpose(-1, -2), 0.0).sum(-2, keepdim=True)
+
+
+def _safe(l: torch.Tensor) -> torch.Tensor:
+    return torch.where(l > 0, l, torch.ones_like(l))
+
+
+def attn_weights(r) -> torch.Tensor:
+    """The weights' share of the ctx bound, element-wise: ctx moves by sum_j p_j Delta_j (v_j - ctx), at most
+    (p Delta) |v| + (sum_j p_j Delta_j) |ctx|."""
+    pd = r["p"] * r["delta"]
+    return pd @ r["v"].abs() + pd.sum(-1, keepdim=True) * r["ctx"].abs()
+
+
+def attn_acc(r) -> torch.Tensor:
+    """The accumulations' share of the ctx bound, element-wise:
+      * P . V: nblk block/16 truncating k16 steps into one fp32 accumulator, each within 2^-22 of a partial sum bounded
+        by sum_j P_j |v_j| (P = fp16(e) <= (1 + 2^-11) e), plus 4 steps, as for the GEMM; and the rescale of O once per
+        block (u each);
+      * the row sum: at most 10 fp32 roundings per block on any path of l (the pair sum, up to 8 running adds, the
+        rescale), the quad shuffle sum (2), 1 / l and O * (1 / l): (10 nblk + 8) u relative."""
+    nblk = r["nblk"]
+    pv = r["p"] @ r["v"].abs()
+    b = ((nblk * r["block"] / 16 + 4) * 2.0 ** -22 * (1 + F16_U) + nblk * U32) * pv
+    return b + (10 * nblk + 8) * U32 * r["ctx"].abs()
+
+
+def attn_ctx_bound(r) -> torch.Tensor:
+    """|ctx - ctx64| element-wise: attn_weights, attn_acc, P rounded to fp16 relative to the running maximum (2^-11 e_j,
+    or the subnormal half-quantum 2^-25 below 2^-14, per key: 2^-11 p |v| + 2^-25 sum_j |v_j| / l after normalisation,
+    the rescales only shrinking it; not normalised away, since l sums the fp32 e, not fp16(e)), and the fp16 output
+    (2^-11 |ctx| + 2^-25)."""
+    p, v, ctx, l = r["p"], r["v"], r["ctx"], r["l"]
+    b = attn_weights(r) + attn_acc(r) + F16_U * (p @ v.abs()) + F16_HALF_QUANTUM * _vsum(r, torch.abs) / _safe(l)
+    return b + F16_U * ctx.abs() + F16_HALF_QUANTUM
+
+
+def half_ulp16(y: torch.Tensor) -> torch.Tensor:
+    """half an fp16 ulp at |y| (2^-25 in the subnormal range)"""
+    _, ex = torch.frexp(y.double().abs())
+    return torch.pow(2.0, (ex - 1).clamp_min(-14).double() - 11)
+
+
+GATE_SIGMAS = 3.0
+
+
+def attn_relfro_gate(r) -> torch.Tensor:
+    """[B, H]: the per-(sequence, head) bound of ||ctx - ctx64||_F / ||ctx64||_F.
+    The errors that do not depend on the sign of v are modelled as independent and zero-mean:
+      * the fp16 roundings of P and of the output, uniform within half an ulp (variance ulp^2 / 12): P's half ulp taken
+        at its upper bound 2^-11 e_j (2^-25 below 2^-14), the output's as the exact half ulp of ctx64;
+      * each weight's error, at most Delta_j in size with a sign set by q and k alone (the logit's accumulation,
+        ex2.approx, the exponent's roundings), so independent of v_j's: variance p_j^2 Delta_j^2 (|v_j| + |ctx|)^2.
+    The squared error norm sums at least 64 T such terms, so it concentrates within a few per cent of its mean sigma^2;
+    GATE_SIGMAS = 3 sigma covers what the model approximates (errors that are not quite uniform or independent).  The
+    accumulations truncate, a bias rather than noise: attn_acc is added at its worst case.
+    Diffuse heads give a gate of ~1.3e-3 (P and the output each ~2^-11 / sqrt(3) relative); ctx scaled by 1 + 2^-9
+    (1.95e-3) is outside it."""
+    p, v, ctx, l = r["p"], r["v"], r["ctx"], r["l"]
+    var = (F16_U ** 2 / 3) * ((p * p) @ (v * v)) + (F16_HALF_QUANTUM ** 2 / 3) * _vsum(r, torch.square) / _safe(l) ** 2
+    var = var + half_ulp16(ctx) ** 2 / 3
+    w2 = (p * r["delta"]).pow(2)
+    var = var + w2 @ (v * v) + 2 * (w2 @ v.abs()) * ctx.abs() + w2.sum(-1, keepdim=True) * ctx * ctx
+    sigma = var.sum((-1, -2)).sqrt()
+    acc = attn_acc(r).pow(2).sum((-1, -2)).sqrt()
+    return (GATE_SIGMAS * sigma + acc) / ctx.pow(2).sum((-1, -2)).sqrt().clamp_min(1e-300)
+
+
+def attn_probs_bound(r) -> torch.Tensor:
+    """|p - p64| of the probability kernel: p_j off by Delta_j (its own, recomputed logit, ex2.approx and argument
+    roundings), the saved row sum off by sum_i p_i Delta_i <= max Delta (the forward's logits) plus the roundings of
+    its rescale chain: the exponents (m_old - m) log2e, 3 u sum |m_old - m| <= 3 u (|m| + |m_first|) <= max Delta (Delta
+    of the first block's maximum alone holds 34 u |m_first| + 6 u |m|), and ex2.approx of alpha (8 u per block); the row
+    sum's own (10 nblk + 8) u, 1 / l, the product and the fp32 store (4 u).  ex2.approx flushes results below 2^-126 to
+    zero.  The saved maximum's error cancels: it enters the forward's l and the probability alike."""
+    p, delta, nblk = r["p"], r["delta"], r["nblk"]
+    dmax = delta.amax(-1, keepdim=True)
+    return p * (delta + 2 * dmax + (18 * nblk + 12) * U32) + 2.0 ** -126
+
+
+def attn_rowsum_bound(r) -> torch.Tensor:
+    """[B,H,T]: |sum_j p_j - 1| of the probability kernel's rows.  Row j's numerator and the saved row sum carry the
+    same weights, each off by its own Delta (the probability kernel's recomputed logit and the forward's), so the
+    weight errors cost sum_j p_j (Delta'_j + Delta_j) <= 2 sum_j p_j Delta_j rather than max Delta; what the row sum
+    alone carries is its rescale chain, the exponents 3 u sum |m_old - m| <= 6 u max|s| over the valid keys and
+    ex2.approx of alpha (8 u per block), its own (10 nblk + 8) u, and 1 / l, the product and the fp32 stores (4 u).
+    Unlike the sum of the element bounds this is tighter than a common rescale of the row: on diffuse heads
+    p (1 + 2^-13) leaves it."""
+    p, delta, nblk = r["p"], r["delta"], r["nblk"][..., 0]
+    smax = r["s"].abs().masked_fill(r["km"], 0.0).amax(-1)
+    return 2 * (p * delta).sum(-1) + 6 * U32 * smax + (18 * nblk + 12) * U32
+
+
+def attn_max_bound(r) -> torch.Tensor:
+    """[B,H,T]: |saved row max - m64|: the saved maximum is the largest of the kernel's own fp32 logits, so within the
+    row's largest logit error"""
+    return r["lerr"].amax(-1) + 1e-30
+
+
+def attn_sum_bound(r, l_at: torch.Tensor) -> torch.Tensor:
+    """[B,H,T]: |saved row sum - l_at|, l_at = sum_j e^(s_j - m_saved) in float64: the weights' Delta (<= max Delta),
+    the rescale chain's exponents (<= max Delta, see attn_probs_bound) and ex2.approx (8 u per block), and the sum's
+    (10 nblk + 8) u"""
+    dmax = r["delta"].amax(-1)
+    return l_at * (2 * dmax + (18 * r["nblk"][..., 0] + 8) * U32) + 1e-30
 
 
 # ---- erf-GELU -------------------------------------------------------------------------------------------------------

@@ -1,7 +1,7 @@
 """GPU (-m gpu): the warpgroup-MMA attention forward (csrc/attention_wg.cuh), which runs every fp16 attention with
-64-wide heads: esmb200_attention and esmb200_column_attention against an fp32 PyTorch softmax attention of the same
-fp16 inputs.  Tolerances as in test_gpu_kernels.py: P is rounded to fp16 before P.V (ctx 4e-3), the statistics are
-fp32 (compared through the probabilities the probability kernel forms from them, and directly)."""
+64-wide heads: esmb200_attention and esmb200_column_attention against float64 softmax attention of the same fp16
+inputs, through test_gpu_attention_f16.check16 (ctx element-wise and per (sequence, head), the probabilities and the
+saved statistics, each within its derived bound in kernel_refs)."""
 import ctypes
 import os
 import shutil
@@ -9,6 +9,8 @@ import subprocess
 
 import pytest
 import torch
+
+import test_gpu_attention_f16 as f16
 
 pytestmark = pytest.mark.gpu
 
@@ -36,23 +38,6 @@ def _pad(B, T, lengths, dev):
     for b, n in enumerate(lengths):
         pad[b, n:] = 1
     return pad.to(dev)
-
-
-def _ref(qkv, pad, B, T, H):
-    """ctx [B*T, 64H], probabilities [B,H,T,T], row max of the scaled scores and sum of exp(s - max) [B,H,T]."""
-    E = 64 * H
-    y = qkv.float().view(B, T, 3, H, 64)
-    q, k, v = (y[:, :, i].transpose(1, 2) for i in range(3))
-    s = q @ k.transpose(-1, -2)
-    if pad is not None:
-        s = s.masked_fill(pad[:, None, None, :].bool(), float("-inf"))
-    m = s.amax(-1)
-    m0 = torch.where(torch.isinf(m), torch.zeros_like(m), m)
-    e = torch.exp(s - m0[..., None])
-    l = e.sum(-1)
-    p = e / torch.where(l > 0, l, torch.ones_like(l))[..., None]
-    o = (p @ v).transpose(1, 2).reshape(B * T, E)
-    return o, p, m0, l
 
 
 def _run(L, qkv, pad, B, T, H, probs=True):
@@ -92,18 +77,7 @@ def test_lengths_context_probs_and_stats(L, T):
     B, H = 3, 2
     lengths = [T, max(1, T // 2), max(1, (2 * T) // 3 - 1)]
     qkv = _qkv(B, T, H, 100 + T)
-    pad = _pad(B, T, lengths, qkv.device)
-    ctx, pr, scratch = _run(L, qkv, pad, B, T, H)
-    ref_o, ref_p, ref_m, ref_l = _ref(qkv, pad, B, T, H)
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(pr, ref_p, atol=2e-5, rtol=2e-4)
-    mx, sm = _stats(scratch, B, T, H)
-    torch.testing.assert_close(mx, ref_m, atol=2e-5, rtol=2e-5)
-    torch.testing.assert_close(sm, ref_l, atol=1e-4, rtol=2e-5)
-    ctx2, _, _ = _run(L, qkv, pad, B, T, H, probs=False)
-    assert torch.equal(ctx, ctx2)  # with and without probabilities
-    ctx3, _, _ = _run(L, qkv, pad, B, T, H, probs=False)
-    assert torch.equal(ctx2, ctx3)  # two identical calls
+    f16.check16(f"lengths={lengths}", qkv, _pad(B, T, lengths, qkv.device), B, T, H, 64)
 
 
 def test_all_padding_sequence_gives_zero(L):
@@ -111,13 +85,12 @@ def test_all_padding_sequence_gives_zero(L):
     qkv = _qkv(B, T, H, 7)
     pad = _pad(B, T, [300, 0, 131], qkv.device)
     ctx, pr, scratch = _run(L, qkv, pad, B, T, H)
-    ref_o, _, ref_m, ref_l = _ref(qkv, pad, B, T, H)
-    assert torch.equal(ctx[T:2 * T], torch.zeros_like(ctx[T:2 * T]))
     mx, sm = _stats(scratch, B, T, H)
-    assert torch.equal(mx[1], torch.zeros_like(mx[1])) and torch.equal(sm[1], torch.zeros_like(sm[1]))
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(mx, ref_m, atol=2e-5, rtol=2e-5)
-    torch.testing.assert_close(sm, ref_l, atol=1e-4, rtol=2e-5)
+    name = f"attention_f16 D=64 all-padding sequence B={B} T={T} H={H}"
+    assert f16.exact(name + " ctx", ctx[T:2 * T], torch.zeros_like(ctx[T:2 * T]))
+    assert f16.exact(name + " row max", mx[1], torch.zeros_like(mx[1]))
+    assert f16.exact(name + " row sum", sm[1], torch.zeros_like(sm[1]))
+    f16.check16("all padding", qkv, pad, B, T, H, 64)
 
 
 def test_left_padding_and_interior_gap_at_minus_40(L):
@@ -138,15 +111,8 @@ def test_left_padding_and_interior_gap_at_minus_40(L):
     pad[0, :260] = 1          # blocks 0 and 1 fully masked, block 2 partially
     pad[1, 64:300] = 1        # interior gap across a block boundary
     pad[1, 490:] = 1
-    pad = pad.cuda()
-    ctx, pr, scratch = _run(L, qkv, pad, B, T, H)
-    ref_o, ref_p, ref_m, ref_l = _ref(qkv, pad, B, T, H)
-    assert float(ref_o.abs().max()) > 0.05
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(pr, ref_p, atol=2e-5, rtol=1e-3)
-    mx, sm = _stats(scratch, B, T, H)
-    torch.testing.assert_close(mx, ref_m, atol=1e-4, rtol=2e-5)
-    torch.testing.assert_close(sm, ref_l, atol=1e-4, rtol=1e-4)
+    out = f16.check16("left padding, gap, logits ~-40", qkv, pad.cuda(), B, T, H, 64)
+    assert out["ctx_absmax"] > 0.05
 
 
 def test_running_maximum_rises_every_block(L):
@@ -162,14 +128,7 @@ def test_running_maximum_rises_every_block(L):
     for h in range(H):
         qkv[:, h * 64:(h + 1) * 64] = u + 0.1 * torch.randn(B * T, 64, generator=g)
         qkv[:, E + h * 64:E + (h + 1) * 64] = u * (0.8 * blk[:, None]) + 0.3 * torch.randn(B * T, 64, generator=g)
-    qkv = qkv.half().cuda()
-    ctx, pr, scratch = _run(L, qkv, None, B, T, H)
-    ref_o, ref_p, ref_m, ref_l = _ref(qkv, None, B, T, H)
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(pr, ref_p, atol=1e-4, rtol=1e-3)
-    mx, sm = _stats(scratch, B, T, H)
-    torch.testing.assert_close(mx, ref_m, atol=1e-4, rtol=2e-5)
-    torch.testing.assert_close(sm, ref_l, atol=1e-4, rtol=1e-4)
+    f16.check16("rising maximum", qkv.half().cuda(), None, B, T, H, 64)
 
 
 def test_one_hot_rows_read_every_value_exactly(L):
@@ -190,39 +149,30 @@ def test_one_hot_rows_read_every_value_exactly(L):
     top2 = s.topk(2, dim=1).values
     assert float((top2[:, 0] - top2[:, 1]).min()) > 25.0  # exp(-25) is below the smallest fp16 subnormal
     ctx, _, _ = _run(L, qkv, None, B, T, H, probs=False)
-    assert torch.equal(ctx, qkv[perm.cuda(), 128:])
+    assert f16.exact(f"attention_f16 D=64 one-hot rows B={B} T={T} H={H}", ctx, qkv[perm.cuda(), 128:])
 
 
 @pytest.mark.parametrize("B,R,C,H,ragged", [(1, 128, 8, 2, False), (2, 77, 5, 3, True), (1, 200, 3, 12, True)])
 def test_column_attention(L, B, R, C, H, ragged):
-    """MSA column attention (cols > 1: the R tokens of a column are C rows of qkv apart) against torch on the
+    """MSA column attention (cols > 1: the R tokens of a column are C rows of qkv apart) against float64 on the
     regrouped tensor [B*C, R, 3E]; R not a multiple of 128 and padded rows."""
-    lib = L.load()
     E = 64 * H
     g = torch.Generator(device="cpu").manual_seed(B * 31 + R + C)
     qkv = torch.randn(B, R, C, 3 * E, generator=g)
     qkv[..., :E] *= 0.5
-    qkv = qkv.half().cuda()
+    qkv = qkv.half().cuda().view(B * R * C, 3 * E)
     pad = torch.zeros(B, C, R, dtype=torch.uint8)
     if ragged:
         for b in range(B):
             for c in range(C):
                 pad[b, c, (R * (c + 1)) // (C + 1) + 1:] = 1
         pad[0, 0, :] = 1  # a column that is all padding
-    pad = pad.cuda()
-    ctx = torch.full((B * R * C, E), float("nan"), dtype=torch.float16, device="cuda")
-    scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B * C, R), dtype=torch.uint8, device="cuda")
-    L.check(lib.esmb200_column_attention(P(qkv), P(pad), P(ctx), B, R, C, H, P(scratch), S()))
-    torch.cuda.synchronize()
-    reg = qkv.permute(0, 2, 1, 3).reshape(B * C * R, 3 * E).contiguous()
-    ref_o, _, _, _ = _ref(reg, pad.view(B * C, R), B * C, R, H)
-    ref_o = ref_o.view(B, C, R, E).permute(0, 2, 1, 3).reshape(B * R * C, E)
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
+    f16.check_column("ragged" if ragged else "full", qkv, pad.cuda(), B, R, C, H)
 
 
 def test_many_more_items_than_sms_at_full_size(L):
     """The configs[1] shape (256 x 1024 tokens, 20 heads): ~40k work items, so every persistent CTA walks hundreds;
-    ragged lengths; checked against torch in chunks of sequences."""
+    ragged lengths; ctx element-wise and per (sequence, head) against float64, checked in chunks of sequences."""
     B, T, H = 256, 1024, 20
     E = 64 * H
     g = torch.Generator(device="cpu").manual_seed(11)
@@ -234,10 +184,8 @@ def test_many_more_items_than_sms_at_full_size(L):
     ctx, _, _ = _run(L, qkv, pad, B, T, H, probs=False)
     ctx2, _, _ = _run(L, qkv, pad, B, T, H, probs=False)
     assert torch.equal(ctx, ctx2)
-    for b0 in range(0, B, 32):
-        rows = slice(b0 * T, (b0 + 32) * T)
-        ref_o, _, _, _ = _ref(qkv[rows], pad[b0:b0 + 32], 32, T, H)
-        torch.testing.assert_close(ctx[rows].float(), ref_o, atol=4e-3, rtol=4e-3)
+    out = f16.measure(qkv, pad, B, T, H, 64, ctx)
+    f16.assert_within(f"attention_f16 D=64 many items B={B} T={T} H={H}", out)
 
 
 def test_kernel_runs_on_warpgroup_mma(L):

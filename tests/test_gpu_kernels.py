@@ -1,11 +1,14 @@
 """GPU (-m gpu): each sm_90a kernel, called through the C ABI, against a plain PyTorch fp32 evaluation of the same
 op on the same device.  Inputs to the tensor-core kernels are rounded to fp16 first, so the comparison isolates the
-kernel (fp32 accumulation order) from the operand-precision choice; tolerances are stated per test."""
+kernel (fp32 accumulation order) from the operand-precision choice; tolerances are stated per test.  The attention
+cases run through test_gpu_attention_f16.check16, against float64 within the derived bounds of kernel_refs."""
 import ctypes
 import math
 
 import pytest
 import torch
+
+import test_gpu_attention_f16 as f16
 
 pytestmark = pytest.mark.gpu
 
@@ -116,49 +119,18 @@ def test_gemm_qkv_rope(dev, B, T, H):
     torch.testing.assert_close(out.float(), ref, atol=3e-3, rtol=2e-3)
 
 
-def _attention_ref(qkv, pad, B, T, H, D=64):
-    E = D * H
-    y = qkv.float().view(B, T, 3, H, D)
-    q, k, v = (y[:, :, i].transpose(1, 2) for i in range(3))
-    s = q @ k.transpose(-1, -2)
-    if pad is not None:
-        s = s.masked_fill(pad[:, None, None, :].bool(), float("-inf"))
-    p = torch.softmax(s, -1)
-    o = (p @ v).transpose(1, 2).reshape(B * T, E)
-    return o, p
-
-
 @pytest.mark.parametrize("B,T,H,lengths", [
     (1, 128, 1, None), (2, 40, 2, [40, 23]), (3, 200, 4, [200, 150, 7]), (2, 300, 2, None),
     (2, 1024, 20, [1024, 517]), (1, 129, 1, [129]), (2, 256, 1, [256, 128]),
 ])
 def test_attention_forward_and_probs(dev, B, T, H, lengths):
     """softmax(QK^T + key-padding mask) V (multihead_attention.py:357-394) incl. ragged lengths, T not a multiple of
-    128, fully padded key blocks; and the need_head_weights probabilities (:397-400)."""
-    L = _lib(); lib = L.load()
-    E = 64 * H
+    128, fully padded key blocks; and the need_head_weights probabilities (:397-400).  Against float64 on the same fp16
+    q, k, v within the bounds of kernel_refs (test_gpu_attention_f16.check16)."""
     g = torch.Generator(device="cpu").manual_seed(B * 1000 + T)
-    qkv = torch.randn(B * T, 3 * E, generator=g)
-    qkv[:, :E] *= 0.5  # q is pre-scaled in the real pipeline; keep logits O(1..10)
-    qkv = qkv.half().to(dev)
-    pad = None
-    if lengths is not None:
-        pad = torch.zeros(B, T, dtype=torch.uint8)
-        for b, n in enumerate(lengths):
-            pad[b, n:] = 1
-        pad = pad.to(dev)
-    ctx = torch.full((B * T, E), float("nan"), dtype=torch.float16, device=dev)
-    probs = torch.full((B, H, T, T), float("nan"), device=dev)
-    scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
-    L.check(lib.esmb200_attention(P(qkv), P(pad), P(ctx), P(probs), B, T, H, P(scratch), S()))
-    ref_o, ref_p = _attention_ref(qkv, pad, B, T, H)
-    # P is rounded to fp16 before the PV product: |dO| <~ 2^-11 * max|v| ~ 2e-3
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(probs, ref_p, atol=2e-5, rtol=2e-4)
-    # same call without probabilities must give the identical context
-    ctx2 = torch.empty_like(ctx)
-    L.check(lib.esmb200_attention(P(qkv), P(pad), P(ctx2), None, B, T, H, P(scratch), S()))
-    assert torch.equal(ctx, ctx2)
+    qkv = torch.randn(B * T, 3 * 64 * H, generator=g)
+    qkv[:, :64 * H] *= 0.5  # q is pre-scaled in the real pipeline; keep logits O(1..10)
+    f16.check16("forward and probs", qkv.half().to(dev), f16.pad_of(B, T, lengths), B, T, H, 64)
 
 
 @pytest.mark.parametrize("B,T,H,lengths", [(1, 128, 1, None), (2, 200, 3, [200, 61]), (2, 1024, 4, [1024, 517]),
@@ -166,28 +138,10 @@ def test_attention_forward_and_probs(dev, B, T, H, lengths):
 def test_attention_head_dim_128(dev, B, T, H, lengths):
     """esm2_t48_15B's head width (pretrained.py:390-397): the same contract as above on 128-wide heads (two 64-wide
     column slots per head: QK^T sums both, P.V runs once per slot), context and probabilities."""
-    L = _lib(); lib = L.load()
-    E = 128 * H
     g = torch.Generator(device="cpu").manual_seed(B * 977 + T)
-    qkv = torch.randn(B * T, 3 * E, generator=g)
-    qkv[:, :E] *= 0.35
-    qkv = qkv.half().to(dev)
-    pad = None
-    if lengths is not None:
-        pad = torch.zeros(B, T, dtype=torch.uint8)
-        for b, n in enumerate(lengths):
-            pad[b, n:] = 1
-        pad = pad.to(dev)
-    ctx = torch.full((B * T, E), float("nan"), dtype=torch.float16, device=dev)
-    probs = torch.full((B, H, T, T), float("nan"), device=dev)
-    scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
-    L.check(lib.esmb200_attention128(P(qkv), P(pad), P(ctx), P(probs), B, T, H, P(scratch), S()))
-    ref_o, ref_p = _attention_ref(qkv, pad, B, T, H, 128)
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(probs, ref_p, atol=2e-5, rtol=2e-4)
-    ctx2 = torch.empty_like(ctx)
-    L.check(lib.esmb200_attention128(P(qkv), P(pad), P(ctx2), None, B, T, H, P(scratch), S()))
-    assert torch.equal(ctx, ctx2)
+    qkv = torch.randn(B * T, 3 * 128 * H, generator=g)
+    qkv[:, :128 * H] *= 0.35
+    f16.check16("head dim 128", qkv.half().to(dev), f16.pad_of(B, T, lengths), B, T, H, 128)
 
 
 @pytest.mark.parametrize("D,B,H", [(64, 1, 2), (128, 1, 2), (128, 3, 40)])
@@ -196,7 +150,6 @@ def test_attention_reference_max_raise(dev, D, B, H):
     the lazy-rescale threshold) force the O-rescale / block-redo path; result must still be the exact softmax.
     (D = 128: the double-buffered two-slot kernel, whose rescale waits for the previous P.V; the 3 x 40-head case keeps
     every CTA of the GPU busy with several tiles.)"""
-    L = _lib(); lib = L.load()
     T = 640
     E = D * H
     g = torch.Generator(device="cpu").manual_seed(5)
@@ -208,15 +161,7 @@ def test_attention_reference_max_raise(dev, D, B, H):
         qkv[:, h * D:(h + 1) * D] = u + 0.1 * torch.randn(B * T, D, generator=g)
         # logits ~ 8 * 0.8 * block index: every block tops the previous maximum by ~6.4 > tau (5.5)
         qkv[:, E + h * D:E + (h + 1) * D] = u * (0.8 * blk[:, None]) + 0.3 * torch.randn(B * T, D, generator=g)
-    qkv = qkv.half().to(dev)
-    ctx = torch.empty(B * T, E, dtype=torch.float16, device=dev)
-    probs = torch.empty(B, H, T, T, device=dev)
-    scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
-    fn = lib.esmb200_attention if D == 64 else lib.esmb200_attention128
-    L.check(fn(P(qkv), None, P(ctx), P(probs), B, T, H, P(scratch), S()))
-    ref_o, ref_p = _attention_ref(qkv, None, B, T, H, D)
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(probs, ref_p, atol=1e-4, rtol=1e-3)
+    f16.check16("max raise", qkv.half().to(dev), None, B, T, H, D)
 
 
 @pytest.mark.parametrize("D", [64, 128])
@@ -224,7 +169,6 @@ def test_attention_left_and_interior_padding_with_very_negative_scores(dev, D):
     """ADVICE r1: when the first key block is fully padded the reference maximum must be seeded from the first block that
     has an attendable key — with scores around -40 a reference of 0 would round every probability to 0 in fp16.  Left
     padding (first 130 keys) and an interior gap, all valid logits ~ -40."""
-    L = _lib(); lib = L.load()
     B, T, H = 2, 400, 2
     E = D * H
     g = torch.Generator(device="cpu").manual_seed(17)
@@ -235,21 +179,12 @@ def test_attention_left_and_interior_padding_with_very_negative_scores(dev, D):
         qkv[:, h * D:(h + 1) * D] += u
         qkv[:, E + h * D:E + (h + 1) * D] -= u
     qkv[:, 2 * E:] = torch.randn(B * T, E, generator=g)
-    qkv = qkv.half().to(dev)
     pad = torch.zeros(B, T, dtype=torch.uint8)
     pad[0, :130] = 1            # left padding: blocks 0 and 1 (64-key blocks) fully masked, block 2 partially
     pad[1, 64:200] = 1          # interior gap
     pad[1, 390:] = 1
-    pad = pad.to(dev)
-    ctx = torch.full((B * T, E), float("nan"), dtype=torch.float16, device=dev)
-    probs = torch.full((B, H, T, T), float("nan"), device=dev)
-    scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
-    fn = lib.esmb200_attention if D == 64 else lib.esmb200_attention128
-    L.check(fn(P(qkv), P(pad), P(ctx), P(probs), B, T, H, P(scratch), S()))
-    ref_o, ref_p = _attention_ref(qkv, pad, B, T, H, D)
-    assert float(ref_o.abs().max()) > 0.05
-    torch.testing.assert_close(ctx.float(), ref_o, atol=4e-3, rtol=4e-3)
-    torch.testing.assert_close(probs, ref_p, atol=2e-5, rtol=1e-3)
+    out = f16.check16("left padding, gap, logits ~-40", qkv.half().to(dev), pad.to(dev), B, T, H, D)
+    assert out["ctx_absmax"] > 0.05
 
 
 def test_embed_tokens(dev):

@@ -4,7 +4,9 @@
     each partial is the sum over its own 32-wide quarter (a swapped quarter or tile index in the reference fails here);
   * the per-model GEMM launch table reproduces the packed layer size the library reports and the shapes of the models'
     own modules;
-  * the erf-GELU bound holds for an fp32 restatement of the epilogue's formula."""
+  * the erf-GELU bound holds for an fp32 restatement of the epilogue's formula;
+  * the fp16 attention bounds hold for a float64 emulation of the kernels' arithmetic, are not vacuous, and refuse the
+    same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9."""
 import math
 
 import numpy as np
@@ -207,3 +209,137 @@ def test_gelu_bound_covers_an_fp32_restatement():
     assert bool((err <= bound).all()), float((err / bound).max())
     assert float((err / bound).max()) > 0.05  # the bound is not vacuous
     assert math.isclose(float(kr.gelu64(torch.tensor(1.0))), 0.8413447460685429, rel_tol=1e-15)
+
+
+# ---- fp16 attention -------------------------------------------------------------------------------------------------
+LOG2E32 = float(torch.tensor(1.4426950408889634, dtype=torch.float32))
+
+
+def _f32(t):
+    return t.float().double()
+
+
+def _chop(t):  # round toward zero to fp32: the tensor core's accumulation
+    f = t.float()
+    over = f.double().abs() > t.abs()
+    return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f).double()
+
+
+def _emulate_attention(q, k, v, padded, block, count_key=None, skip_rescale=None):
+    """float64 emulation of the fp16 attention kernels' arithmetic on one head: q, k, v [T, D] fp16, padded [T] bool.
+    Logits in fp32 truncating k16 steps; per `block`-key block the exact running maximum,
+    e = 2^(fp32(s log2e - m log2e)) (correctly rounded: ex2.approx's own error is not emulated),
+    l = fp32(alpha l + fp32 sum e), P = fp16(e), O = fp32(alpha O) + P V in truncating k16 steps;
+    ctx = fp16(O * fp32(1 / l)).  Returns ctx, the saved row max and row sum, and the probability kernel's output from
+    the same logits.  Faults: count_key (a padded key index counted as attendable), skip_rescale (a block index whose O
+    rescale is left out)."""
+    T, D = q.shape
+    live = ~padded
+    if count_key is not None:
+        live = live.clone()
+        live[count_key] = True
+    kvlen = int(torch.nonzero(live).max()) + 1 if bool(live.any()) else 0
+    s = torch.zeros(T, T, dtype=torch.float64)
+    for d0 in range(0, D, 16):
+        s = _chop(s + q[:, d0:d0 + 16].double() @ k[:, d0:d0 + 16].double().t())
+    s = s.masked_fill(~live[None, :], float("-inf"))
+    m = torch.full((T, 1), float("-inf"), dtype=torch.float64)
+    l = torch.zeros(T, 1, dtype=torch.float64)
+    o = torch.zeros(T, D, dtype=torch.float64)
+    for j0 in range(0, kvlen, block):
+        sb = s[:, j0:j0 + block]
+        mn = torch.maximum(m, sb.amax(-1, keepdim=True))
+        alpha = torch.where(torch.isinf(mn), torch.ones_like(mn), torch.exp2(_f32(_f32(m - mn) * LOG2E32)))
+        ref = torch.where(torch.isinf(mn), torch.zeros_like(mn), _f32(-mn * LOG2E32))
+        e = _f32(torch.exp2(_f32(sb * LOG2E32 + ref)))
+        m = mn
+        l = _f32(_f32(l * alpha) + _f32(e.float().sum(-1, keepdim=True)))
+        if j0 // block != skip_rescale:
+            o = _f32(o * alpha)
+        ph = e.half().double()
+        vb = v[j0:j0 + block].double()
+        for k0 in range(0, ph.shape[1], 16):
+            o = _chop(o + ph[:, k0:k0 + 16] @ vb[k0:k0 + 16])
+    inv = torch.where(l > 0, _f32(1.0 / torch.where(l > 0, l, torch.ones_like(l))), torch.zeros_like(l))
+    ctx = _f32(o * inv).half().double()
+    mx = torch.where(torch.isinf(m), torch.zeros_like(m), m)
+    probs = _f32(_f32(torch.exp2(_f32(s * LOG2E32 + _f32(-mx * LOG2E32)))) * inv)
+    return ctx, mx[:, 0], l[:, 0], probs
+
+
+def _attention_inputs(T, D, std, seed, rise=False):
+    """fp16 q, k, v [T, D] with logits of std `std` (diffuse at 1, sharp at 8); rise: every 64 keys score ~3 higher"""
+    g = torch.Generator().manual_seed(seed)
+    q = torch.randn(T, D, generator=g, dtype=torch.float64) * std / math.sqrt(D)
+    k = torch.randn(T, D, generator=g, dtype=torch.float64)
+    if rise:
+        u = q.mean(0)
+        k = k + (torch.arange(T, dtype=torch.float64) // 64)[:, None] * 3.0 * u / float(u @ u)
+    v = torch.randn(T, D, generator=g, dtype=torch.float64)
+    return q.half(), k.half(), v.half()
+
+
+def _ratios(q, k, v, padded, block, ctx, mx=None, sm=None, probs=None):
+    r = kr.attention64(q[None, None], k[None, None], v[None, None], padded[None], block)
+    out = {"ctx": float(((ctx - r["ctx"][0, 0]).abs() / kr.attn_ctx_bound(r)[0, 0]).max())}
+    num = (ctx - r["ctx"][0, 0]).pow(2).sum().sqrt()
+    out["gate"] = float(num / r["ctx"].pow(2).sum().sqrt() / kr.attn_relfro_gate(r)[0, 0])
+    if mx is not None:
+        out["max"] = float(((mx - r["m"][0, 0, :, 0]).abs() / kr.attn_max_bound(r)[0, 0]).max())
+        l_at = torch.exp(r["s"].masked_fill(r["km"], float("-inf")) - mx[None, None, :, None]).sum(-1)
+        out["sum"] = float(((sm - l_at[0, 0]).abs() / kr.attn_sum_bound(r, l_at)[0, 0]).max())
+        out["probs"] = float(((probs - r["p"][0, 0]).abs() / kr.attn_probs_bound(r)[0, 0]).max())
+        live = ~padded.all()
+        dev = (probs.sum(-1) - 1).abs() if bool(live) else torch.zeros(probs.shape[0], dtype=torch.float64)
+        out["rowsum"] = float((dev / kr.attn_rowsum_bound(r)[0, 0]).max())
+    return out
+
+
+ATTN_EMU_CASES = [(300, 64, 128, 1.0, False), (300, 64, 128, 8.0, False), (1024, 64, 128, 1.0, False),
+                  (300, 128, 64, 1.0, False), (300, 128, 64, 8.0, False), (400, 128, 64, 2.0, True),
+                  (400, 64, 128, 2.0, True)]
+
+
+@pytest.mark.parametrize("T,D,block,std,rise", ATTN_EMU_CASES)
+def test_attention_bounds_cover_an_emulated_kernel(T, D, block, std, rise):
+    """The emulated kernel, on a ragged mask with the last key padded, stays inside every bound; the bounds are not
+    vacuous: the worst element of ctx reaches 0.1 of its bound and the gate 0.1 (diffuse heads, where neither term is
+    dominated by exact one-hot rows)."""
+    q, k, v = _attention_inputs(T, D, std, seed=T + D + int(std))
+    padded = torch.zeros(T, dtype=torch.bool)
+    padded[T - 37:] = True
+    padded[5:9] = True
+    ctx, mx, sm, probs = _emulate_attention(q, k, v, padded, block)
+    out = _ratios(q, k, v, padded, block, ctx, mx, sm, probs)
+    assert max(out.values()) <= 1.0, out
+    if std == 1.0:
+        assert out["ctx"] >= 0.1 and out["gate"] >= 0.1, out
+
+
+@pytest.mark.parametrize("D,block", [(64, 128), (128, 64)])
+def test_attention_bounds_refuse_emulated_faults(D, block):
+    """The same emulation with one padded key counted, one block's O rescale skipped, or ctx scaled by 1 + 2^-9
+    leaves the element bound or the per-head gate; probabilities scaled by 1 + 2^-13 leave the row-sum bound, which is
+    tighter than the sum of the element bounds (that sum is implied by the element check and refuses nothing on its
+    own)."""
+    T = 300
+    q, k, v = _attention_inputs(T, D, 2.0, seed=7, rise=True)
+    padded = torch.zeros(T, dtype=torch.bool)
+    padded[T - 37:] = True
+    good, _, _, _ = _emulate_attention(q, k, v, padded, block)
+    assert max(_ratios(q, k, v, padded, block, good).values()) <= 1.0
+    counted, _, _, _ = _emulate_attention(q, k, v, padded, block, count_key=T - 20)
+    skipped, _, _, _ = _emulate_attention(q, k, v, padded, block, skip_rescale=1)
+    for bad in (counted, skipped):
+        assert max(_ratios(q, k, v, padded, block, bad).values()) > 1.0
+    qd, kd, vd = _attention_inputs(1024, D, 1.0, seed=8)
+    pd = torch.zeros(1024, dtype=torch.bool)
+    ctx, mx, sm, probs = _emulate_attention(qd, kd, vd, pd, block)
+    scaled = (ctx * (1 + 2.0 ** -9)).half().double()
+    assert _ratios(qd, kd, vd, pd, block, scaled)["gate"] > 1.0
+    up = _f32(probs * (1 + 2.0 ** -13))
+    assert _ratios(qd, kd, vd, pd, block, ctx, mx, sm, up)["rowsum"] > 1.0
+    r = kr.attention64(qd[None, None], kd[None, None], vd[None, None], pd[None], block)
+    dev = (up.sum(-1) - 1).abs()
+    summed = float((dev / kr.attn_probs_bound(r)[0, 0].sum(-1)).max())
+    assert float((dev / kr.attn_rowsum_bound(r)[0, 0]).max()) > 1.3 * summed  # tighter than the summed element bounds
