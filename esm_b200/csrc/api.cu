@@ -1041,6 +1041,7 @@ int esmb200_esm1b_embed(const int64_t* tokens, const float* embed_table, const f
   ProfScope ps(T_EMBED, st);
   int chunks = (8 * num_sms() + B - 1) / B;  // >= 8 blocks per SM over the batch, at least 8 rows (one per warp) per block
   if (chunks > (T + 7) / 8) chunks = (T + 7) / 8;
+  if (chunks < (T + 8191) / 8192) chunks = (T + 8191) / 8192;  // a chunk's positions (4 bytes a row) stay within 48 KB
   if (chunks < 1) chunks = 1;
   const int rows = (T + chunks - 1) / chunks;
   const dim3 grid(chunks, B);
@@ -1347,7 +1348,9 @@ int esmb200_msa_embed(const int64_t* tokens, const float* embed_table, const flo
                       int32_t msa_pos_dim, const float* ln_weight, const float* ln_bias, float eps, float* x,
                       int32_t B, int32_t R, int32_t C, int32_t E, int32_t padding_idx, void* stream) {
   if (!tokens || !embed_table || !pos_table || !ln_weight || !ln_bias || !x) return fail(ESMB200_EINVAL, "null argument");
-  if (B <= 0 || R <= 0 || C <= 0 || E <= 0 || E % 4 != 0 || E > 20 * 128) return fail(ESMB200_EINVAL, "bad shape");
+  // C <= 12288: a row's positions (4 bytes a column) are held in 48 KB of shared memory
+  if (B <= 0 || R <= 0 || C <= 0 || C > 12288 || E <= 0 || E % 4 != 0 || E > 20 * 128)
+    return fail(ESMB200_EINVAL, "bad shape");
   if (msa_pos && msa_pos_dim != E && msa_pos_dim != 1)
     return fail(ESMB200_EINVAL, "msa_position_embedding width must be E or 1");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1406,9 +1409,9 @@ int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_
                       void* stream) {
   if (!x || !lengths || !out) return fail(ESMB200_EINVAL, "null argument");
   if (B <= 0 || T < 2 || E <= 0 || B > 65535) return fail(ESMB200_EINVAL, "bad shape");
+  if (E % 4 != 0) return fail(ESMB200_EINVAL, "mean_pool needs E % 4 == 0");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ProfScope ps(T_MEANPOOL, st);
-  if (E % 4 != 0) return fail(ESMB200_EINVAL, "mean_pool needs E % 4 == 0");
   dim3 grid((E + 127) / 128, B);
   mean_pool_kernel<<<grid, 256, 0, st>>>(x, lengths, out, T, E);
   CK(cudaGetLastError());

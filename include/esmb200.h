@@ -167,7 +167,10 @@ int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layer
                                    void* copy_stream, void* stream);
 
 /* Embedding prologue of ESM2.forward (esm2.py:84-95): gather from table [V,E], zero <mask> rows and rescale by
- * 0.88/(1 - n_mask/n_nonpad) when token_dropout, zero pad rows. tokens int64 [B,T] -> x fp32 [B,T,E]. */
+ * 0.88/(1 - n_mask/n_nonpad) when token_dropout, zero pad rows. tokens int64 [B,T] -> x fp32 [B,T,E].
+ * E % 4 == 0, B <= 65535. Pad rows are written as zeros whatever the scale: a sequence of pads only (scale 0/0) gives
+ * zeros where the reference's x * (1 - padding_mask) keeps NaN. A sequence whose non-pad tokens are all <mask> (scale
+ * 0.88/0) gives NaN at its non-pad rows, as the reference does. */
 int esmb200_embed_tokens(const int64_t* tokens, const float* table, float* x, int32_t B, int32_t T, int32_t E,
                          int32_t padding_idx, int32_t mask_idx, int32_t token_dropout, void* stream);
 
@@ -189,7 +192,9 @@ int esmb200_layernorm(const float* x, const float* weight, const float* bias, fl
                       float eps, void* stream);
 
 /* Per-sequence mean representation, scripts/extract.py:116-119: out[b] = mean_t x[b, 1 : 1+lengths[b]] (residues only,
- * <cls> at position 0 excluded). x fp32 [B,T,E], lengths int32 [B] (device), out fp32 [B,E]. */
+ * <cls> at position 0 excluded). x fp32 [B,T,E], lengths int32 [B] (device), out fp32 [B,E]. T >= 2, E % 4 == 0.
+ * lengths[b] is clamped to [0, T-1] as the slice clamps it; 0 gives NaN (the mean of an empty slice). Rows past the
+ * length and the <cls> row are not read. Deterministic. */
 int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_t B, int32_t T, int32_t E,
                       void* stream);
 
@@ -266,7 +271,8 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
 /* MSA Transformer embedding prologue, esm/model/msa_transformer.py:155-172 (+ LearnedPositionalEmbedding.forward,
  * esm/modules.py:241-257): x[B,R,C,E] fp32 = LayerNorm(embed_tokens[tok] + embed_positions[pos] +
  * msa_position_embedding[r]) * (1 - is_pad). tokens int64 [B,R,C]; pos_table [max_positions + padding_idx + 1, E];
- * msa_pos [>=R, msa_pos_dim] or NULL, msa_pos_dim = E or 1 (the initial esm_msa1 release, pretrained.py:123-125). */
+ * msa_pos [>=R, msa_pos_dim] or NULL, msa_pos_dim = E or 1 (the initial esm_msa1 release, pretrained.py:123-125).
+ * E % 4 == 0, E <= 2560, C <= 12288 (one alignment row's positions are held in shared memory). */
 int esmb200_msa_embed(const int64_t* tokens, const float* embed_table, const float* pos_table, const float* msa_pos,
                       int32_t msa_pos_dim, const float* ln_weight, const float* ln_bias, float eps, float* x,
                       int32_t B, int32_t R, int32_t C, int32_t E, int32_t padding_idx, void* stream);

@@ -11,7 +11,13 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
     the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs;
   * attention64 / attn_ctx_bound / attn_relfro_gate / attn_probs_bound / attn_rowsum_bound / attn_max_bound /
     attn_sum_bound: float64 softmax attention on fp16 q, k, v and the first-order error model of the fp16 attention
-    kernels (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2).
+    kernels (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2);
+  * positions / embed_esm2_64 / embed_esm1b_64 / embed_msa_64 / embed_scale_bound / ln_tol / ln_scale: the three
+    embedding prologues (csrc/elementwise.cuh embed_tokens_kernel, esm1b_embed_kernel, msa_embed_kernel);
+  * mean_pool64 / mean_pool_bound, log_softmax64 / log_softmax_bound: the per-sequence mean representation and the
+    log-softmax rows of variant scoring;
+  * contact_stripes: the accumulators of the standalone contact pass (contact_accumulate_kernel) in its own layout;
+  * layer64: one ESM-2 TransformerLayer in float64 at any even head width.
 """
 from __future__ import annotations
 
@@ -371,3 +377,167 @@ def horner_condition() -> float:
 # ---- LayerNorm ------------------------------------------------------------------------------------------------------
 def layer_norm64(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
     return torch.nn.functional.layer_norm(x.double(), (x.shape[-1],), w.double(), b.double(), eps)
+
+
+def ln_tol(E: int, cond: float = 1.0) -> float:
+    """Bound of an fp32 two-pass LayerNorm row, relative to ln_scale: the mean and variance of E fp32 values (a rounding
+    walk of ~sqrt(E) steps, so |d mean| / std <~ sqrt(E) u cond with cond = |mean| / std of the row), rsqrt (2 ulp) and
+    the affine step (3 roundings), with a factor 4 of room (the bound of tests/test_gpu_row_kernels.py)."""
+    return 4 * U32 * (8 + 2 * E ** 0.5 * (1 + cond))
+
+
+def ln_scale(want: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """|g| (|xhat| + 1) + |b| for want = g xhat + b: what ln_tol is relative to"""
+    return (want - b.double()).abs() + w.double().abs() + b.double().abs()
+
+
+# ---- embedding prologues --------------------------------------------------------------------------------------------
+KEEP_SCALE = 1 - 0.15 * 0.8  # esm2.py:90: the share of tokens the training-time dropout left in place
+
+
+def positions(tokens: torch.Tensor, padding_idx: int) -> torch.Tensor:
+    """LearnedPositionalEmbedding.forward (esm/modules.py:247-248) over the last dim: the count of non-pad tokens up to
+    and including this one, plus padding_idx; padding_idx at the pads themselves."""
+    nonpad = tokens.ne(padding_idx).long()
+    return torch.cumsum(nonpad, -1) * nonpad + padding_idx
+
+
+def mask_ratio(tokens: torch.Tensor, padding_idx: int, mask_idx: int) -> torch.Tensor:
+    """[B] float64: n_mask / n_nonpad (0 / 0 = NaN for a sequence of pads only)"""
+    return tokens.eq(mask_idx).sum(-1).double() / tokens.ne(padding_idx).sum(-1).double()
+
+
+def embed_esm2_64(tokens: torch.Tensor, table: torch.Tensor, padding_idx: int, mask_idx: int,
+                  token_dropout: bool) -> torch.Tensor:
+    """esm/model/esm2.py:84-95 in float64: gather, <mask> rows zeroed and (x 0.88) / (1 - n_mask / n_nonpad) only under
+    token_dropout, pad rows multiplied by zero (so a NaN scale stays NaN there, as in the reference).
+    tokens [B,T] -> [B,T,E]."""
+    x = table.double()[tokens]
+    if token_dropout:
+        x = x.masked_fill(tokens.eq(mask_idx)[..., None], 0.0)
+        x = x * KEEP_SCALE / (1 - mask_ratio(tokens, padding_idx, mask_idx))[:, None, None]
+    return x * tokens.ne(padding_idx)[..., None].double()
+
+
+def embed_scale_bound(tokens: torch.Tensor, padding_idx: int, mask_idx: int, token_dropout: bool) -> torch.Tensor:
+    """[B,1,1]: the relative error of the fp32 token-dropout scale. 0.88 as an fp32 constant, the product and the
+    quotient are one rounding each; the ratio r and 1 - r are one each, and the ratio's reaches 1 - r magnified by
+    r / (1 - r): u (4 + r / (1 - r)).  Without token_dropout the gather is exact."""
+    if not token_dropout:
+        return torch.zeros(tokens.shape[0], 1, 1, dtype=torch.float64)
+    r = mask_ratio(tokens, padding_idx, mask_idx).cpu()
+    return (U32 * (4 + r / (1 - r)))[:, None, None].nan_to_num(nan=0.0, posinf=0.0)
+
+
+def embed_esm1b_64(tokens, table, pos_table, ln_w, ln_b, padding_idx: int, mask_idx: int, token_dropout: bool,
+                   eps: float = 1e-5):
+    """esm/model/esm1.py:121-139 in float64: the ESM-2 scaling of the token embedding, plus the learned position, then
+    emb_layer_norm_before when ln_w is given, then pad rows multiplied by zero.  Returns (x, the rows before the
+    LayerNorm and the pad zeroing)."""
+    x = table.double()[tokens]
+    if token_dropout:
+        x = x.masked_fill(tokens.eq(mask_idx)[..., None], 0.0)
+        x = x * KEEP_SCALE / (1 - mask_ratio(tokens, padding_idx, mask_idx))[:, None, None]
+    pre = x + pos_table.double()[positions(tokens, padding_idx)]
+    x = layer_norm64(pre, ln_w, ln_b, eps) if ln_w is not None else pre
+    return x * tokens.ne(padding_idx)[..., None].double(), pre
+
+
+def embed_msa_64(tokens, table, pos_table, msa_pos, ln_w, ln_b, padding_idx: int, eps: float = 1e-5):
+    """esm/model/msa_transformer.py:155-172 in float64: tokens [B,R,C]; msa_pos None or [>= R, E or 1] (row r of the
+    alignment takes msa_pos[r]).  Returns (x [B,R,C,E], the rows before the LayerNorm)."""
+    B, R, C = tokens.shape
+    pre = table.double()[tokens] + pos_table.double()[positions(tokens, padding_idx)]
+    if msa_pos is not None:
+        pre = pre + msa_pos.double()[None, :R, None, :]
+    x = layer_norm64(pre, ln_w, ln_b, eps)
+    return x * tokens.ne(padding_idx)[..., None].double(), pre
+
+
+def row_cond(pre: torch.Tensor, tokens: torch.Tensor, padding_idx: int) -> float:
+    """max over the non-pad rows of |mean| / std: the conditioning ln_tol takes (a pad row may be constant; its output
+    is multiplied by zero)"""
+    c = pre.mean(-1).abs() / pre.std(-1, unbiased=False).clamp_min(1e-30)
+    return float(c[tokens.ne(padding_idx)].max())
+
+
+# ---- mean pool and log-softmax rows ---------------------------------------------------------------------------------
+def mean_pool64(x: torch.Tensor, lengths: torch.Tensor) -> torch.Tensor:
+    """scripts/extract.py:116-119 in float64: out[b] = x[b, 1 : 1 + n].mean(0) with n = lengths[b] clamped to
+    [0, T - 1] (the slice's own clamp); NaN for the empty slice.  x [B,T,E] -> [B,E]."""
+    B, T, E = x.shape
+    rows = []
+    for b in range(B):
+        n = min(max(int(lengths[b]), 0), T - 1)
+        rows.append(x[b, 1:1 + n].double().mean(0))
+    return torch.stack(rows)
+
+
+def mean_pool_bound(x: torch.Tensor, lengths: torch.Tensor) -> torch.Tensor:
+    """|out - mean_pool64|: an n-term fp32 sum in any order (sum_bound), then 1 / n and the product (2 u |mean|)"""
+    B, T, E = x.shape
+    rows = []
+    for b in range(B):
+        n = min(max(int(lengths[b]), 0), T - 1)
+        a = x[b, 1:1 + n].double().abs().sum(0)
+        rows.append((sum_bound(a, max(n, 1)) + 2 * U32 * a) / max(n, 1))
+    return torch.stack(rows) + 1e-45
+
+
+def log_softmax64(x: torch.Tensor) -> torch.Tensor:
+    """x - max - log sum exp(x - max) over the last dim in float64; -inf stays -inf, a row of -inf only is NaN"""
+    x = x.double()
+    m = x.amax(-1, keepdim=True)
+    return (x - m) - torch.log(torch.exp(x - m).sum(-1, keepdim=True))
+
+
+def log_softmax_bound(x: torch.Tensor) -> torch.Tensor:
+    """|out - log_softmax64| for the fp32 kernel: x - m and the last subtraction are a rounding each of at most
+    u (|x - m| + |lse|); expf (2 ulp), the sum (two terms per lane, five butterfly levels) and logf (1 ulp of |lse|)
+    move lse by at most 9 u + u |lse|, taken as 16 u absolute (s >= 1: lse >= 0 is well conditioned)."""
+    x = x.double()
+    m = x.amax(-1, keepdim=True)
+    lse = torch.log(torch.exp(x - m).sum(-1, keepdim=True))
+    d = (x - m).abs()
+    d = torch.where(torch.isinf(d), torch.zeros_like(d), d)
+    return U32 * (2 * d + 2 * lse.abs() + 16)
+
+
+# ---- standalone contact pass ----------------------------------------------------------------------------------------
+def contact_stripes(attn: torch.Tensor, w: torch.Tensor, keep: Optional[torch.Tensor], lo: int, hi: int):
+    """One layer's share of the accumulators of esmb200_contact_accumulate, float64: attn [B,H,T,T], w [H] ->
+    (acc [B,S,S] = sum_h w_h A_h, row_sum [B,H,S], col_part [B,H,ceil(S/16),S]: the column sums of each stripe of 16
+    cropped query rows).  row_sum[:, :, None] and col_part feed contacts_from_partials like the fused pass's partials."""
+    a = masked_maps(attn, keep, lo, hi)[:, :, lo:hi, lo:hi]
+    B, H, S, _ = a.shape
+    acc = torch.einsum("bhij,h->bij", a, w.double().to(a.device))
+    nt = (S + 15) // 16
+    ap = torch.nn.functional.pad(a, [0, 0, 0, 16 * nt - S])
+    return acc, a.sum(-1), ap.reshape(B, H, nt, 16, S).sum(3)
+
+
+# ---- one transformer layer ------------------------------------------------------------------------------------------
+def layer64(x: torch.Tensor, sd: Dict[str, torch.Tensor], pre: str, H: int, pad: torch.Tensor):
+    """oracle.esm2_oracle.transformer_layer kept in float64 throughout (the oracle's softmax runs in fp32, as the
+    reference's does), at any even head width d = E / H (the rotation pairs dimension j with j + d/2 under table column
+    j < d/2, whatever d): x [B,T,E] float64, sd float64, pad [B,T] bool -> (x', probabilities [B,H,T,T])"""
+    from oracle import esm2_oracle as o
+    F = torch.nn.functional
+    B, T, E = x.shape
+    d = E // H
+    assert d * H == E and d % 2 == 0
+    h = o.layer_norm(x, sd[pre + "self_attn_layer_norm.weight"], sd[pre + "self_attn_layer_norm.bias"])
+    a = pre + "self_attn."
+    q = (F.linear(h, sd[a + "q_proj.weight"], sd[a + "q_proj.bias"]) * d ** -0.5).view(B, T, H, d).transpose(1, 2)
+    k = F.linear(h, sd[a + "k_proj.weight"], sd[a + "k_proj.bias"]).view(B, T, H, d).transpose(1, 2)
+    v = F.linear(h, sd[a + "v_proj.weight"], sd[a + "v_proj.bias"]).view(B, T, H, d).transpose(1, 2)
+    cos, sin = o.rope_tables(sd[a + "rot_emb.inv_freq"], T)
+    assert cos.shape == (T, d // 2)
+    q, k = o.apply_rope(q, cos, sin), o.apply_rope(k, cos, sin)
+    s = (q @ k.transpose(-1, -2)).masked_fill(pad[:, None, None, :], float("-inf"))
+    p = torch.softmax(s, -1)
+    ctx = (p @ v).transpose(1, 2).reshape(B, T, E)
+    x = x + F.linear(ctx, sd[a + "out_proj.weight"], sd[a + "out_proj.bias"])
+    h = o.layer_norm(x, sd[pre + "final_layer_norm.weight"], sd[pre + "final_layer_norm.bias"])
+    h = o.gelu(F.linear(h, sd[pre + "fc1.weight"], sd[pre + "fc1.bias"]))
+    return x + F.linear(h, sd[pre + "fc2.weight"], sd[pre + "fc2.bias"]), p

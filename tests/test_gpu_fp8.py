@@ -189,7 +189,8 @@ def check_against_emulation(model, tok, name):
         assert math.isfinite(spread) and err <= 2 * spread, (name, i)
 
 
-@pytest.mark.parametrize("E,H", [(256, 4), (320, 20), (256, 2)], ids=["d64", "d16-partialK", "d128-two-slots"])
+@pytest.mark.parametrize("E,H", [(256, 4), (320, 20), (256, 2), (480, 20), (384, 4)],
+                         ids=["d64", "d16-partialK", "d128-two-slots", "d24", "d96-partial-second-slot"])
 def test_layer_against_float64_emulation(E, H):
     """Two fp8 layers whose matrices have block scales several powers of two apart (so that a scale array handed to the
     wrong GEMM, or a weight packed into the wrong slot, moves outputs far outside the bound)."""

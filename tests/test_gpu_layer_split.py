@@ -10,6 +10,8 @@
 import pytest
 import torch
 
+from kernel_refs import layer64
+
 pytestmark = pytest.mark.gpu
 
 # Gates of the narrow-head layer test (DESIGN.md section 4 gives the measured maxima).  A lo weight half dropped or
@@ -22,29 +24,6 @@ LAYER_PROBS_MAX_ABS = 7e-5  # attention probabilities, valid query rows
 
 def report(name, **kv):
     print("PARITY", name, " ".join(f"{k}={v:.3e}" for k, v in kv.items()), flush=True)
-
-
-def layer64(x, sd, pre, H, pad):
-    """oracle.esm2_oracle.transformer_layer kept in float64 throughout (the oracle's softmax runs in fp32, as the
-    reference's does): x [B,T,E] float64 -> (x', probabilities [B,H,T,T])"""
-    from oracle import esm2_oracle as o
-    F = torch.nn.functional
-    B, T, E = x.shape
-    d = E // H
-    h = o.layer_norm(x, sd[pre + "self_attn_layer_norm.weight"], sd[pre + "self_attn_layer_norm.bias"])
-    a = pre + "self_attn."
-    q = (F.linear(h, sd[a + "q_proj.weight"], sd[a + "q_proj.bias"]) * d ** -0.5).view(B, T, H, d).transpose(1, 2)
-    k = F.linear(h, sd[a + "k_proj.weight"], sd[a + "k_proj.bias"]).view(B, T, H, d).transpose(1, 2)
-    v = F.linear(h, sd[a + "v_proj.weight"], sd[a + "v_proj.bias"]).view(B, T, H, d).transpose(1, 2)
-    cos, sin = o.rope_tables(sd[a + "rot_emb.inv_freq"], T)
-    q, k = o.apply_rope(q, cos, sin), o.apply_rope(k, cos, sin)
-    s = (q @ k.transpose(-1, -2)).masked_fill(pad[:, None, None, :], float("-inf"))
-    p = torch.softmax(s, -1)
-    ctx = (p @ v).transpose(1, 2).reshape(B, T, E)
-    x = x + F.linear(ctx, sd[a + "out_proj.weight"], sd[a + "out_proj.bias"])
-    h = o.layer_norm(x, sd[pre + "final_layer_norm.weight"], sd[pre + "final_layer_norm.bias"])
-    h = o.gelu(F.linear(h, sd[pre + "fc1.weight"], sd[pre + "fc1.bias"]))
-    return x + F.linear(h, sd[pre + "fc2.weight"], sd[pre + "fc2.bias"]), p
 
 
 @pytest.mark.parametrize("E,H", [(320, 20), (640, 20), (1280, 20)], ids=["8M", "150M", "650M"])

@@ -6,7 +6,11 @@
     own modules;
   * the erf-GELU bound holds for an fp32 restatement of the epilogue's formula;
   * the fp16 attention bounds hold for a float64 emulation of the kernels' arithmetic, are not vacuous, and refuse the
-    same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9."""
+    same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9;
+  * the embedding references give the oracles' embeddings (oracle.esm2_oracle.embed, the embedding lines of
+    oracle.msa_oracle.msa_transformer_forward, its representation 0), positions a hand-written example, mean_pool64 and
+    log_softmax64 torch's float64 results, contact_stripes the reference contact head, and layer64 the oracle's layer;
+    torch's fp32 log-softmax stays inside log_softmax_bound and a row summed over its first 32 columns only does not."""
 import math
 
 import numpy as np
@@ -343,3 +347,178 @@ def test_attention_bounds_refuse_emulated_faults(D, block):
     dev = (up.sum(-1) - 1).abs()
     summed = float((dev / kr.attn_probs_bound(r)[0, 0].sum(-1)).max())
     assert float((dev / kr.attn_rowsum_bound(r)[0, 0]).max()) > 1.3 * summed  # tighter than the summed element bounds
+
+
+# ---- embedding prologues, mean pool, log-softmax, standalone contact pass, layer ------------------------------------
+def _tokens(B, T, seed, pad=1, mask=32):
+    """[B,T] residues with leading, interior and trailing pads and a few <mask>; row 1 has neither"""
+    g = torch.Generator().manual_seed(seed)
+    tok = torch.randint(4, 24, (B, T), generator=g)
+    tok[:, 0] = 0
+    tok[0, T - 3:] = pad
+    tok[0, 2] = tok[0, T // 2] = mask
+    if B > 2:
+        tok[2, :2] = pad
+        tok[2, T // 3] = pad
+        tok[2, 5] = mask
+    return tok
+
+
+def test_positions_hand_written_example():
+    tok = torch.tensor([[1, 1, 0, 5, 1, 6, 1, 7, 2, 1], [0, 5, 6, 7, 8, 9, 2, 1, 1, 1]])
+    want = torch.tensor([[1, 1, 2, 3, 1, 4, 1, 5, 6, 1], [2, 3, 4, 5, 6, 7, 8, 1, 1, 1]])
+    assert torch.equal(kr.positions(tok, 1), want)
+    assert torch.equal(kr.positions(tok[None], 1), want[None])  # over the last dim, whatever is in front
+    # another padding index shifts every position and moves the pads
+    assert torch.equal(kr.positions(torch.tensor([[0, 3, 5, 3, 6]]), 3), torch.tensor([[4, 3, 5, 3, 6]]))
+
+
+@pytest.mark.parametrize("token_dropout", [True, False])
+def test_embed_esm2_64_matches_the_oracle(token_dropout):
+    from oracle import esm2_oracle
+    from oracle.weights import make_state_dict
+    table = make_state_dict(0, 64, 2, seed=1)["embed_tokens.weight"].double()
+    tok = _tokens(3, 40, seed=2)
+    want = esm2_oracle.embed(tok, {"embed_tokens.weight": table}, token_dropout)
+    got = kr.embed_esm2_64(tok, table, 1, 32, token_dropout)
+    torch.testing.assert_close(got, want, atol=0, rtol=1e-15)
+    assert (float(got[0, 2].abs().max()) == 0.0) == token_dropout  # a <mask> row
+    assert float(got[0, -1].abs().max()) == 0.0 and float(got[1].abs().min()) > 0.0
+    if token_dropout:  # row 0: 2 <mask> of 37 non-pad tokens; row 1: none
+        torch.testing.assert_close(got[0, 1], table[tok[0, 1]] * 0.88 / (1 - 2 / 37), rtol=1e-15, atol=0)
+        torch.testing.assert_close(got[1, 1], table[tok[1, 1]] * 0.88, rtol=1e-15, atol=0)
+
+
+def test_embed_esm2_64_non_finite_scales():
+    """pads only: 0 / 0, NaN everywhere (the reference multiplies the pad rows by zero); every non-pad token a <mask>:
+    0.88 * 0 / 0 = NaN"""
+    table = torch.randn(33, 8, generator=torch.Generator().manual_seed(0))
+    tok = torch.tensor([[1, 1, 1, 1], [32, 32, 32, 1], [0, 5, 32, 1]])
+    got = kr.embed_esm2_64(tok, table, 1, 32, True)
+    assert bool(got[0].isnan().all()) and bool(got[1].isnan().all()) and bool(got[2].isfinite().all())
+    assert bool(kr.embed_esm2_64(tok, table, 1, 32, False).isfinite().all())
+    b = kr.embed_scale_bound(tok, 1, 32, True)
+    assert b.shape == (3, 1, 1) and float(b[0]) == 0.0 and float(b[1]) == 0.0
+    assert math.isclose(float(b[2]), kr.U32 * (4 + (1 / 3) / (2 / 3)))
+    assert float(kr.embed_scale_bound(tok, 1, 32, False).abs().max()) == 0.0
+
+
+@pytest.mark.parametrize("token_dropout", [True, False])
+def test_embed_esm1b_64_is_the_esm2_scaling_plus_positions(token_dropout):
+    from oracle import esm2_oracle
+    g = torch.Generator().manual_seed(3)
+    E, T = 32, 40
+    table = torch.randn(33, E, generator=g, dtype=torch.float64)
+    pos = torch.randn(T + 2, E, generator=g, dtype=torch.float64)
+    w, b = 1 + 0.2 * torch.randn(E, generator=g, dtype=torch.float64), torch.randn(E, generator=g, dtype=torch.float64)
+    tok = _tokens(3, T, seed=4)
+    keep = tok.ne(1)[..., None]
+    scaled = esm2_oracle.embed(tok, {"embed_tokens.weight": table}, token_dropout)
+    x, pre = kr.embed_esm1b_64(tok, table, pos, None, None, 1, 32, token_dropout)
+    assert torch.equal(x, pre * keep)
+    p = torch.zeros(3, T, dtype=torch.long)
+    for i in range(3):  # the count of non-pad tokens so far, written as a loop
+        n = 0
+        for t in range(T):
+            n += int(tok[i, t] != 1)
+            p[i, t] = n + 1 if tok[i, t] != 1 else 1
+    torch.testing.assert_close(x, (scaled + pos[p]) * keep, atol=0, rtol=1e-15)
+    y, pre2 = kr.embed_esm1b_64(tok, table, pos, w, b, 1, 32, token_dropout)
+    assert torch.equal(pre, pre2)
+    torch.testing.assert_close(y, torch.nn.functional.layer_norm(pre, (E,), w, b, 1e-5) * keep, atol=0, rtol=1e-15)
+    assert float(y[0, -1].abs().max()) == 0.0
+
+
+@pytest.mark.parametrize("msa_pos_dim", [None, 1, 0], ids=["E", "1", "none"])
+def test_embed_msa_64_matches_the_oracle_embedding(msa_pos_dim):
+    from oracle.msa_oracle import make_msa_state_dict, make_msa_tokens, msa_transformer_forward
+    E, H, B, R, C = 64, 2, 2, 5, 40
+    sd = make_msa_state_dict(1, E, 128, H, seed=5, msa_pos_dim=msa_pos_dim or None)
+    if msa_pos_dim == 0:
+        del sd["msa_position_embedding"]
+    sd = {k: v.double() for k, v in sd.items()}
+    tok = make_msa_tokens(B, R, C, seed=6, pad_cols=4, pad_rows_last=2)
+    tok[0, 1, 3] = tok[0, 2, 0] = 1  # interior and leading pads
+    # representation 0 of a one-layer model: the embedding (with no layer at all it would be the final LayerNorm's)
+    want = msa_transformer_forward(sd, 1, H, tok, repr_layers=[0])["representations"][0]
+    mp = sd["msa_position_embedding"][0, :, 0] if "msa_position_embedding" in sd else None  # [1024, E or 1]
+    got, pre = kr.embed_msa_64(tok, sd["embed_tokens.weight"], sd["embed_positions.weight"], mp,
+                               sd["emb_layer_norm_before.weight"], sd["emb_layer_norm_before.bias"], 1)
+    torch.testing.assert_close(got, want, atol=1e-13, rtol=1e-13)
+    assert pre.shape == (B, R, C, E) and kr.row_cond(pre, tok, 1) < 10
+
+
+def test_mean_pool64_clamps_and_gives_nan_for_the_empty_slice():
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(6, 10, 8, generator=g)
+    lengths = torch.tensor([9, 4, 0, -3, 12, 1], dtype=torch.int32)
+    got = kr.mean_pool64(x, lengths)
+    for b, n in enumerate([9, 4, 0, 0, 9, 1]):
+        assert bool(got[b].isnan().all()) == (n == 0)
+        if n:
+            assert torch.equal(got[b], x[b, 1:1 + n].double().mean(0))
+    assert torch.equal(got[4], x[4, 1:1 + 12].double().mean(0))  # the slice's own clamp
+    bound = kr.mean_pool_bound(x, lengths)
+    f32 = torch.stack([x[b, 1:1 + n].sum(0) / n for b, n in ((0, 9), (1, 4), (4, 9), (5, 1))]).double()
+    ok = torch.tensor([0, 1, 4, 5])
+    assert bool(((f32 - got[ok]).abs() <= bound[ok]).all()) and float(bound[ok].max()) < 1e-6
+
+
+def test_log_softmax64_matches_torch_and_its_bound_holds_in_fp32():
+    g = torch.Generator().manual_seed(8)
+    x = (torch.rand(50, 33, generator=g) * 160 - 80)
+    x[3, 5] = float("-inf")
+    x[4] = float("-inf")
+    x[5, 7] = 300.0  # dominant: lse ~ 0
+    got = kr.log_softmax64(x)
+    want = torch.log_softmax(x.double(), -1)
+    fin = torch.ones(50, dtype=torch.bool)
+    fin[4] = False
+    torch.testing.assert_close(got[fin], want[fin], atol=1e-12, rtol=1e-13)
+    assert bool(got[4].isnan().all()) and got[3, 5] == float("-inf") and float(got[5, 7]) == 0.0
+    bound = kr.log_softmax_bound(x)
+    live = got.isfinite()
+    assert bool(((torch.log_softmax(x, -1).double() - got).abs()[live] <= bound[live]).all())
+    # a fault: column 32 left out of the sum, on the rows where it carries weight
+    m = x[:, :32].amax(-1, keepdim=True)
+    half = ((x - m) - torch.log(torch.exp(x[:, :32] - m).sum(-1, keepdim=True))).double()
+    rows = x[:, 32] > x[:, :32].amax(-1) - 5
+    assert bool(rows.any()) and bool(((half - got).abs()[rows][:, :32] > bound[rows][:, :32]).all())
+
+
+def test_contact_stripes_sum_to_the_reference_contact_head():
+    from oracle import esm2_oracle
+    from oracle.weights import make_tokens
+    L, H, T = 2, 3, 40
+    tokens = make_tokens([38, 20], T, seed=9)
+    attn = _random_maps(L, 2, H, T, seed=10)
+    g = torch.Generator().manual_seed(11)
+    sd = {"contact_head.regression.weight": torch.randn(1, L * H, generator=g, dtype=torch.float64),
+          "contact_head.regression.bias": torch.randn(1, generator=g, dtype=torch.float64)}
+    want = esm2_oracle.contact_head(tokens, attn, sd)
+    w = sd["contact_head.regression.weight"].view(L, H)
+    parts = [kr.contact_stripes(attn[:, l], w[l], tokens.ne(2), 1, T - 1) for l in range(L)]
+    assert parts[0][1].shape == (2, H, 38) and parts[0][2].shape == (2, H, 3, 38)
+    a = kr.masked_maps(attn[:, 0], tokens.ne(2), 1, T - 1)[:, :, 1:T - 1, 1:T - 1]
+    torch.testing.assert_close(parts[0][2][:, :, 2], a[:, :, 32:38].sum(-2), atol=0, rtol=1e-14)  # the partial stripe
+    torch.testing.assert_close(parts[0][2][:, :, 1], a[:, :, 16:32].sum(-2), atol=0, rtol=1e-14)
+    got = kr.contacts_from_partials(sum(p[0] for p in parts), torch.stack([p[1][:, :, None] for p in parts]),
+                                    torch.stack([p[2] for p in parts]), w, float(sd["contact_head.regression.bias"]))
+    torch.testing.assert_close(got, want, atol=1e-12, rtol=1e-12)
+
+
+@pytest.mark.parametrize("E,H", [(128, 2), (144, 2)], ids=["d64", "d72"])
+def test_layer64_matches_the_oracle_layer(E, H):
+    from oracle import esm2_oracle
+    from oracle.weights import make_state_dict
+    sd = {k: v.double() for k, v in make_state_dict(1, E, H, seed=12).items()}
+    g = torch.Generator().manual_seed(13)
+    x = torch.randn(2, 30, E, generator=g, dtype=torch.float64)
+    pad = torch.zeros(2, 30, dtype=torch.bool)
+    pad[1, 21:] = True
+    sd32 = {k: v.float() for k, v in sd.items()}
+    want, wp = esm2_oracle.transformer_layer(x.float(), sd32, "layers.0.", H, pad, True)  # the fp32 oracle
+    got, gp = kr.layer64(x, sd, "layers.0.", H, pad)
+    torch.testing.assert_close(gp, wp.double(), atol=2e-6, rtol=0)
+    torch.testing.assert_close(got, want.double(), atol=3e-5, rtol=0)
+    assert float(gp[1, :, :, 21:].abs().max()) == 0.0
