@@ -255,7 +255,9 @@ int esmb200_column_attention(const void* qkv_f16, const uint8_t* pad_mask, void*
  * row_layers[i]: an esmb200_layer created with fc1_weight == NULL (attention-only) from row_self_attention's
  *   layer_norm + q/k/v/out projections; col_layers[i]: column_self_attention's layer_norm + projections as ln1/q/k/v/out
  *   and feed_forward_layer's layer_norm + fc1/fc2 as ln2/fc1/fc2.
- * pad_mask [B,R,C] and col_pad_mask [B,C,R] (its transpose): 1 = padding, both NULL for unpadded alignments.
+ * pad_mask [B,R,C] and col_pad_mask [B,C,R] (its transpose): 1 = padding, both NULL for unpadded alignments. As in
+ *   the reference (axial_attention.py:82-97), the row attention zeroes q at every padded token, and its padded key
+ *   columns are those of row 0 of each alignment (pad_mask[b, 0, :]).
  * row_attn_out: NULL, or n_layers pointers (NULL entries allowed) to fp32 [H,B,C,C] buffers (the reference's
  *   row-attention return layout, axial_attention.py:87,105). Column attention maps are not produced by this call.
  * workspace: esmb200_axial_workspace_bytes(E,F,B,R,C) bytes, or esmb200_axial_workspace_bytes_split(E,F,B,R,C) for

@@ -12,6 +12,9 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
   * attention64 / attn_ctx_bound / attn_relfro_gate / attn_probs_bound / attn_rowsum_bound / attn_max_bound /
     attn_sum_bound: float64 softmax attention on fp16 q, k, v and the first-order error model of the fp16 attention
     kernels (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2);
+  * tied64 / tied_softmax64 / tied_probs_bound / tied_P_bound / tied_rowsum_bound / tied_pv / tied_ctx_bound /
+    tied_relfro_gate: the MSA Transformer's tied row attention (csrc/tied_attention.cuh, fp16 and fp32x3) end to end
+    and stage by stage, each stage on the kernel's own inputs (logits, softmax of its logits, P V of its P);
   * positions / embed_esm2_64 / embed_esm1b_64 / embed_msa_64 / embed_scale_bound / ln_tol / ln_scale: the three
     embedding prologues (csrc/elementwise.cuh embed_tokens_kernel, esm1b_embed_kernel, msa_embed_kernel);
   * mean_pool64 / mean_pool_bound, log_softmax64 / log_softmax_bound: the per-sequence mean representation and the
@@ -273,7 +276,7 @@ def attn_ctx_bound(r) -> torch.Tensor:
 def half_ulp16(y: torch.Tensor) -> torch.Tensor:
     """half an fp16 ulp at |y| (2^-25 in the subnormal range)"""
     _, ex = torch.frexp(y.double().abs())
-    return torch.pow(2.0, (ex - 1).clamp_min(-14).double() - 11)
+    return torch.ldexp(torch.ones_like(y, dtype=torch.float64), (ex - 1).clamp_min(-14) - 11)  # exact, unlike pow
 
 
 GATE_SIGMAS = 3.0
@@ -338,6 +341,169 @@ def attn_sum_bound(r, l_at: torch.Tensor) -> torch.Tensor:
     (10 nblk + 8) u"""
     dmax = r["delta"].amax(-1)
     return l_at * (2 * dmax + (18 * r["nblk"][..., 0] + 8) * U32) + 1e-30
+
+
+# ---- tied row attention (MSA Transformer) ---------------------------------------------------------------------------
+# csrc/tied_attention.cuh, <false> (fp16) and <true> (fp32x3): tied_scores_kernel S = sum_r q_r k_r^T on the tensor
+# cores (fp16: one fp32 accumulator carried over all R alignment rows, 4 truncating k16 steps per row; fp32x3: each
+# row's 64-wide slab in a fresh fragment, 3 passes q_lo k_hi, q_hi k_lo, q_hi k_hi per k16 step, then one fp32 add into
+# the running sum); tied_softmax_kernel, one warp per row: -10000 at padded key columns, the exact row max m,
+# e = __expf(x - m) (ex2.approx of fp32 (x - m) log2e), a row sum of ceil(C/32) serial terms per lane then 5 shuffle
+# levels, q = e * (1.0f / sum) (a correctly rounded divide: no --use_fast_math), P = fp16(q) or hi | lo of q, zero in
+# columns [C, Cp); tied_pv_kernel ctx = P V over Cp/16 truncating k16 steps (fp32x3: P_hi v_hi, P_lo v_hi, P_hi v_lo per
+# step), fp16 or hi | lo output.
+def tied_operands(qkv: torch.Tensor, B: int, R: int, C: int, H: int, split: bool):
+    """The kernel's operands in float64, [B,R,C,3,H,64] (sections q, k, v): (value, hi, lo); fp16: (x, x, None)."""
+    y = qkv.double().view(B, R, C, 6 if split else 3, H, 64)
+    if split:
+        return y[:, :, :, :3] + y[:, :, :, 3:], y[:, :, :, :3], y[:, :, :, 3:]
+    return y, y, None
+
+
+def _qk(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    return torch.einsum("brihd,brjhd->hbij", a, b)
+
+
+def _pv(p: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    return torch.einsum("hbij,brjhd->brihd", p, v)
+
+
+def tied_depth(C: int) -> int:
+    """rounding depth of tied_softmax_kernel's row sum: ceil(C/32) - 1 serial adds per lane, then 5 shuffle levels"""
+    return (C + 31) // 32 + 4
+
+
+def tied_pad(key_pad: Optional[torch.Tensor], B: int, C: int, device) -> torch.Tensor:
+    """[1,B,1,C] bool: padded key columns (key_pad [B,C], 1 = padded; None: none)"""
+    if key_pad is None:
+        return torch.zeros(1, B, 1, C, dtype=torch.bool, device=device)
+    return key_pad.bool().view(1, B, 1, C)
+
+
+def tied64(qkv: torch.Tensor, key_pad: Optional[torch.Tensor], B: int, R: int, C: int, H: int, split: bool) -> Dict:
+    """float64 tied row attention on the kernel's own operands (qkv [B*R*C, 3E] fp16, or [B*R*C, 6E] hi | lo):
+    S = sum_r q_r k_r^T [H,B,C,C], -10000 at padded key columns, P = softmax, ctx = P v_r [B,R,C,H,64]; and lerr, the
+    bound of each of the kernel's fp32 logits:
+      * fp16: 4R truncating k16 steps into one accumulator, (4R + 4) 2^-22 sum|q k| (attention64's lerr, D = 64 R);
+      * fp32x3: per alignment row a fresh fragment of 12 steps, (12 + 4) 2^-22 times the slab's
+        sum(|q_hi k_hi| + |q_lo k_hi| + |q_hi k_lo|), the dropped sum|q_lo k_lo|, and the R fp32 adds of the slabs into
+        the running sum, sum_bound over the slabs' absolute sums (each within 2^-10 of sum|q k|)."""
+    x, hi, lo = tied_operands(qkv, B, R, C, H, split)
+    q, k, v = x[:, :, :, 0], x[:, :, :, 1], x[:, :, :, 2]
+    s = _qk(q, k)
+    qk_abs = _qk(q.abs(), k.abs())
+    if split:
+        qh, kh, ql, kl = hi[:, :, :, 0].abs(), hi[:, :, :, 1].abs(), lo[:, :, :, 0].abs(), lo[:, :, :, 1].abs()
+        passes = _qk(qh, kh) + _qk(ql, kh) + _qk(qh, kl)
+        lerr = 16 * 2.0 ** -22 * passes + _qk(ql, kl) + sum_bound(qk_abs * (1 + 2.0 ** -10), R)
+    else:
+        lerr = (4 * R + 4) * 2.0 ** -22 * qk_abs
+    km = tied_pad(key_pad, B, C, qkv.device)
+    sm = s.masked_fill(km, -10000.0)
+    m = sm.amax(-1, keepdim=True)
+    p = torch.softmax(sm, -1)
+    return dict(s=s, sm=sm, m=m, p=p, v=v, ctx=_pv(p, v), lerr=lerr, km=km, split=split, R=R, C=C,
+                Cp=(C + 63) // 64 * 64)
+
+
+def tied_softmax64(S: torch.Tensor, key_pad: Optional[torch.Tensor]) -> Dict:
+    """float64 softmax of the kernel's own fp32 logits S [H,B,C,C] (-10000 at padded key columns), with Delta_j, the
+    relative error bound of the kernel's e_j = __expf(x_j - m): the fp32 roundings of x - m, of the product with log2e
+    and of log2e itself (3 u |x - m|), and ex2.approx (2^-22, doubled)."""
+    H, B, C, _ = S.shape
+    x = S.double().masked_fill(tied_pad(key_pad, B, C, S.device), -10000.0)
+    m = x.amax(-1, keepdim=True)
+    return dict(p=torch.softmax(x, -1), delta=3 * U32 * (x - m).abs() + 2.0 ** -21, C=C)
+
+
+def tied_probs_bound(sr: Dict) -> torch.Tensor:
+    """|q - p| for the kernel's fp32 q = e_j * (1 / sum) (the attn_probs output) against p = softmax(S_kernel): its own
+    weight's Delta_j, the row sum's weights sum_i p_i Delta_i, the sum's tied_depth(C) roundings, 1 / sum and the
+    product (u each); results of ex2.approx below 2^-126 may be subnormal or flushed to zero (2^-126 absolute)."""
+    p, d = sr["p"], sr["delta"]
+    return p * (d + (p * d).sum(-1, keepdim=True) + (tied_depth(sr["C"]) + 2) * U32) + 2.0 ** -126
+
+
+def tied_P_bound(sr: Dict, split: bool) -> torch.Tensor:
+    """|P - p| for the kernel's P: tied_probs_bound, then fp16(q) (half an ulp, at most 2^-11 |q| or the subnormal
+    half-quantum 2^-25) or the hi | lo pair of q (split_rep_bound)."""
+    b = tied_probs_bound(sr)
+    q = sr["p"] + b
+    return b + (split_rep_bound(q) if split else F16_U * q + F16_HALF_QUANTUM)
+
+
+def tied_rowsum_bound(C: int) -> float:
+    """|sum_j q_j - 1| for a row of the fp32 probabilities.  Every q_j is e_j (1 + e_mul) / (sum_i e_i (1 + e_sum)) with
+    the kernel's own e_i in numerator and sum alike, so the weights' errors cancel: what is left is the sum's tied_depth(C)
+    roundings, 1 / sum and the product (u each), and C flushed terms below 2^-126.  A uniform rescale of the row by
+    1 + 2^-13 is ~30 times outside it at C = 1024."""
+    return (tied_depth(C) + 2) * U32 + C * 2.0 ** -126
+
+
+def tied_pv(P_hi: torch.Tensor, P_lo: Optional[torch.Tensor], v_hi: torch.Tensor, v_lo: Optional[torch.Tensor],
+            Cp: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """float64 P V on the kernel's own P ([H,B,C,C] halves, the columns [C, Cp) being zero) and v ([B,R,C,H,64] halves)
+    -> (ctx [B,R,C,H,64], bound of the kernel's ctx):
+      * fp16: Cp/16 truncating k16 steps, (Cp/16 + 4) 2^-22 sum_j P_j |v_j|, and half an fp16 ulp of the output;
+      * fp32x3: three passes, (3 Cp/16 + 4) 2^-22 sum_j (|P_hi v_hi| + |P_lo v_hi| + |P_hi v_lo|), the dropped
+        sum_j |P_lo v_lo|, and the hi | lo output (split_rep_bound)."""
+    if P_lo is None:
+        ref = _pv(P_hi, v_hi)
+        acc = (Cp / 16 + 4) * 2.0 ** -22 * _pv(P_hi.abs(), v_hi.abs())
+        return ref, acc + half_ulp16(ref.abs() + acc)
+    ph, pl, vh, vl = P_hi.abs(), P_lo.abs(), v_hi.abs(), v_lo.abs()
+    ref = _pv(P_hi + P_lo, v_hi + v_lo)
+    acc = (3 * Cp / 16 + 4) * 2.0 ** -22 * (_pv(ph, vh) + _pv(pl, vh) + _pv(ph, vl)) + _pv(pl, vl)
+    return ref, acc + split_rep_bound(ref.abs() + acc)
+
+
+def _tied_delta(r: Dict) -> torch.Tensor:
+    """relative error bound of each weight e_j: its logit (lerr; none at a padded column, whose logit is replaced) and
+    the softmax's own Delta_j"""
+    return r["lerr"].masked_fill(r["km"], 0.0) + 3 * U32 * (r["sm"] - r["m"]).abs() + 2.0 ** -21
+
+
+def _tied_acc(r: Dict) -> torch.Tensor:
+    """the accumulations' worst case, element-wise: P V (tied_pv's accumulation, on P within 2^-10 of p; fp32x3 also
+    its dropped lo*lo), and the row sum, 1 / sum and the product (tied_depth(C) + 2) u of sum_j p_j |v_j|"""
+    pv = _pv(r["p"], r["v"].abs())
+    steps = (3 if r["split"] else 1) * r["Cp"] / 16 + 4
+    rel = steps * 2.0 ** -22 * (1 + 2.0 ** -10) + (tied_depth(r["C"]) + 2) * U32
+    if r["split"]:
+        rel = rel + 2.0 ** -22
+    return rel * pv
+
+
+def tied_ctx_bound(r: Dict) -> torch.Tensor:
+    """|ctx - ctx64| element-wise ([B,R,C,H,64]) from tied64, in attn_ctx_bound's structure: the weights' errors
+    sum_j p_j Delta_j (v_j - ctx) (Delta_j the logit bound plus the softmax's), _tied_acc, P's representation (fp16:
+    2^-11 p_j or 2^-25 per key; fp32x3: 2^-22 p_j + 2^-25) and the output's (fp16: 2^-11 |ctx| + 2^-25; fp32x3:
+    split_rep_bound).  Loose for fp16 at large R, where the logit bound grows as R^1.5."""
+    p, v, ctx = r["p"], r["v"], r["ctx"]
+    pd = p * _tied_delta(r)
+    va = v.abs()
+    b = _pv(pd, va) + pd.sum(-1).permute(1, 2, 0)[:, None, :, :, None] * ctx.abs() + _tied_acc(r)
+    vsum = va.sum(2, keepdim=True)  # [B,R,1,H,64]: sum over the keys of |v_j|
+    rep = (2.0 ** -22 if r["split"] else F16_U) * _pv(p, va) + F16_HALF_QUANTUM * vsum
+    out = split_rep_bound(ctx) if r["split"] else F16_U * ctx.abs() + F16_HALF_QUANTUM
+    return b + rep + out
+
+
+def tied_relfro_gate(r: Dict) -> torch.Tensor:
+    """[B, H]: the per-(alignment, head) bound of ||ctx - ctx64||_F / ||ctx64||_F over the alignment's R x C x 64
+    outputs, in attn_relfro_gate's model: P's and the output's roundings uniform and independent (variance ulp^2 / 12
+    at their upper bounds), each weight's error at most Delta_j with a sign independent of v_j, GATE_SIGMAS sigma of
+    that, plus _tied_acc at its worst case."""
+    p, v, ctx = r["p"], r["v"], r["ctx"]
+    rel = 2.0 ** -22 if r["split"] else F16_U
+    var = (rel ** 2 / 3) * _pv(p * p, v * v) + (F16_HALF_QUANTUM ** 2 / 3) * (v * v).sum(2, keepdim=True)
+    var = var + (split_rep_bound(ctx) if r["split"] else half_ulp16(ctx)) ** 2 / 3
+    w2 = (p * _tied_delta(r)).pow(2)
+    w2sum = w2.sum(-1).permute(1, 2, 0)[:, None, :, :, None]
+    var = var + _pv(w2, v * v) + 2 * _pv(w2, v.abs()) * ctx.abs() + w2sum * ctx * ctx
+    sigma = var.sum((1, 2, 4)).sqrt()
+    acc = _tied_acc(r).pow(2).sum((1, 2, 4)).sqrt()
+    return (GATE_SIGMAS * sigma + acc) / ctx.pow(2).sum((1, 2, 4)).sqrt().clamp_min(1e-300)
 
 
 # ---- erf-GELU -------------------------------------------------------------------------------------------------------

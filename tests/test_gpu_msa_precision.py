@@ -22,6 +22,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 if HERE not in sys.path:
     sys.path.insert(0, HERE)  # variant_fixtures
 
+import test_gpu_tied_attention as tied  # noqa: E402
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(HERE)
@@ -101,12 +103,17 @@ def run_tied(q, k, v, pad, split):
 @pytest.mark.parametrize("B,R,C,H", [(2, 64, 130, 4), (1, 5, 300, 2), (1, 1024, 64, 2)])
 def test_split_tied_row_attention_against_float64(B, R, C, H):
     """Sharp logits (std 8 after the sum over R*64 products) with key padding. At R = 1024 the logits are sums of
-    65,536 products: the split kernel adds each alignment row's 64-wide slab into the running sum in fp32."""
+    65,536 products: the split kernel adds each alignment row's 64-wide slab into the running sum in fp32.  Every stage
+    is held to its float64 bound by test_gpu_tied_attention.check_tied; the PARITY line also gives torch's fp32 and the
+    fp16 entry point on the same inputs."""
     torch.backends.cuda.matmul.allow_tf32 = False
     q, k, v, pad = tied_inputs(B, R, C, H, sharp=8.0, seed=B * 1000 + R + C)
     want, pwant = tied_torch(q, k, v, pad, torch.float64)
     f32, p32 = tied_torch(q, k, v, pad, torch.float32)
-    got, pgot = run_tied(q, k, v, pad, True)
+    qkv = tied.pack(torch.stack([q, k, v], 3), True)
+    key_pad = pad.to(torch.uint8).contiguous()
+    ctx, pgot = tied.check_tied("msa_precision sharp", qkv, key_pad, B, R, C, H, True)
+    got = join16(ctx, H * 64).float().view(B, R, C, H, 64)
     g16, p16 = run_tied(q, k, v, pad, False)
     keep = ~pad[:, None, :].expand(B, R, C)       # query positions that are not padding
     r, m = rel_fro(got[keep], want[keep]), max_abs(pgot, pwant)

@@ -7,6 +7,9 @@
   * the erf-GELU bound holds for an fp32 restatement of the epilogue's formula;
   * the fp16 attention bounds hold for a float64 emulation of the kernels' arithmetic, are not vacuous, and refuse the
     same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9;
+  * the tied row attention's stage and end-to-end bounds hold for a float64 emulation of its three kernels in fp16 and
+    fp32x3, and refuse P x (1 + 2^-13), ctx x (1 + 2^-9), an alignment row's slab dropped from the logits, the split
+    slab's q_lo k_hi pass dropped, and V read from the next alignment row;
   * the embedding references give the oracles' embeddings (oracle.esm2_oracle.embed, the embedding lines of
     oracle.msa_oracle.msa_transformer_forward, its representation 0), positions a hand-written example, mean_pool64 and
     log_softmax64 torch's float64 results, contact_stripes the reference contact head, and layer64 the oracle's layer;
@@ -347,6 +350,140 @@ def test_attention_bounds_refuse_emulated_faults(D, block):
     dev = (up.sum(-1) - 1).abs()
     summed = float((dev / kr.attn_probs_bound(r)[0, 0].sum(-1)).max())
     assert float((dev / kr.attn_rowsum_bound(r)[0, 0]).max()) > 1.3 * summed  # tighter than the summed element bounds
+
+
+# ---- tied row attention ---------------------------------------------------------------------------------------------
+def _tied_qkv(B, R, C, H, std, seed, split):
+    """qkv [B*R*C, 3E] fp16 (or [B*R*C, 6E] hi | lo) with summed logits of std `std`"""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, R, C, 3, H, 64, generator=g, dtype=torch.float64)
+    x[:, :, :, 0] *= std / math.sqrt(64 * R)
+    x = x.reshape(B * R * C, 3 * 64 * H)
+    if split:
+        return torch.cat(kr.split16(x), 1)
+    return x.half()
+
+
+def _emulate_tied(qkv, key_pad, B, R, C, H, split, drop_slab=None, drop_lohi=False, p_scale=1.0, ctx_scale=1.0,
+                  v_shift=0):
+    """float64 emulation of tied_scores / tied_softmax / tied_pv: logits in truncating k16 steps (fp16: one accumulator
+    over all rows; split: a fresh fragment per row, q_lo k_hi, q_hi k_lo, q_hi k_hi per step, then an fp32 add), the
+    softmax with fp32 roundings (exp2 correctly rounded, flushed below 2^-126) and the lane / shuffle sum order, P V in
+    truncating k16 steps.  Returns S [H,B,C,C], P halves [H,B,C,Cp], the fp32 probabilities and ctx halves
+    [B,R,C,H,64].  Faults: drop_slab (an alignment row left out of the logits), drop_lohi (the split slab's q_lo k_hi
+    pass left out), p_scale (q scaled before it is stored), ctx_scale (the accumulator scaled before the output),
+    v_shift (V read from alignment row r + v_shift)."""
+    _, hi, lo = kr.tied_operands(qkv, B, R, C, H, split)
+    Cp = (C + 63) // 64 * 64
+    S = torch.zeros(H, B, C, C, dtype=torch.float64)
+    for r in range(R):
+        if r == drop_slab:
+            continue
+        part = torch.zeros_like(S) if split else S
+        for d0 in range(0, 64, 16):
+            sl = slice(d0, d0 + 16)
+            terms = [(hi, hi)]
+            if split:
+                terms = ([] if drop_lohi else [(lo, hi)]) + [(hi, lo), (hi, hi)]
+            for a, b in terms:
+                part = _chop(part + kr._qk(a[:, r:r + 1, :, 0, :, sl], b[:, r:r + 1, :, 1, :, sl]))
+        S = _f32(S + part) if split else part
+    x = S.masked_fill(kr.tied_pad(key_pad, B, C, S.device), -10000.0)
+    m = x.amax(-1, keepdim=True)
+    t = _f32(_f32(x - m) * LOG2E32)
+    e = _f32(torch.exp2(t))
+    e = torch.where(e < 2.0 ** -126, torch.zeros_like(e), e)
+    lanes = torch.nn.functional.pad(e, (0, 1024 - C)).view(H, B, C, 32, 32)  # [.., i, lane]: column 32 i + lane
+    acc = torch.zeros(H, B, C, 32, dtype=torch.float64)
+    for i in range(32):
+        acc = _f32(acc + lanes[..., i, :])
+    for o in (16, 8, 4, 2, 1):
+        acc = _f32(acc + acc[..., torch.arange(32) ^ o])
+    inv = _f32(1.0 / acc[..., :1])
+    q = _f32(_f32(e * inv) * p_scale)
+    qp = torch.nn.functional.pad(q, (0, Cp - C))
+    P_hi = qp.half().double()
+    P_lo = _f32(qp - P_hi).half().double() if split else None
+    vh = torch.roll(hi[:, :, :, 2], -v_shift, 1)
+    vl = torch.roll(lo[:, :, :, 2], -v_shift, 1) if split else None
+    vpad = lambda w: torch.nn.functional.pad(w, (0, 0, 0, 0, 0, Cp - C))  # noqa: E731  keys C .. Cp: zero
+    vh, vl = vpad(vh), (vpad(vl) if split else None)
+    out = torch.zeros(B, R, C, H, 64, dtype=torch.float64)
+    for s0 in range(0, Cp, 16):
+        sl = slice(s0, s0 + 16)
+        terms = [(P_hi, vh)] + ([(P_lo, vh), (P_hi, vl)] if split else [])
+        for a, w in terms:
+            out = _chop(out + kr._pv(a[..., sl], w[:, :, sl]))
+    out = _f32(out * ctx_scale)
+    c_hi = out.half().double()
+    c_lo = _f32(out - c_hi).half().double() if split else None
+    return S, (P_hi, P_lo), q, (c_hi, c_lo)
+
+
+def _tied_ratios(qkv, key_pad, B, R, C, H, split, em):
+    """worst ratio of each stage and of the end-to-end checks to its kernel_refs bound"""
+    S, (P_hi, P_lo), q, (c_hi, c_lo) = em
+    r = kr.tied64(qkv, key_pad, B, R, C, H, split)
+    sr = kr.tied_softmax64(S.float(), key_pad)
+    P = P_hi if P_lo is None else P_hi + P_lo
+    _, hi, lo = kr.tied_operands(qkv, B, R, C, H, split)
+    pv_ref, pv_b = kr.tied_pv(P_hi[..., :C], None if P_lo is None else P_lo[..., :C], hi[:, :, :, 2],
+                              None if lo is None else lo[:, :, :, 2], r["Cp"])
+    ctx = c_hi if c_lo is None else c_hi + c_lo
+    out = dict(logits=float(((S - r["s"]).abs() / r["lerr"]).max()),
+               P=float(((P[..., :C] - sr["p"]).abs() / kr.tied_P_bound(sr, split)).max()),
+               probs=float(((q - sr["p"]).abs() / kr.tied_probs_bound(sr)).max()),
+               rowsum=float(((q.sum(-1) - 1).abs() / kr.tied_rowsum_bound(C)).max()),
+               pv=float(((ctx - pv_ref).abs() / pv_b).max()),
+               ctx=float(((ctx - r["ctx"]).abs() / kr.tied_ctx_bound(r)).max()))
+    rf = (ctx - r["ctx"]).pow(2).sum((1, 2, 4)).sqrt() / r["ctx"].pow(2).sum((1, 2, 4)).sqrt()
+    out["gate"] = float((rf / kr.tied_relfro_gate(r)).max())
+    return out
+
+
+def _tied_pad(B, C):
+    pad = torch.zeros(B, C, dtype=torch.uint8)
+    pad[0, C - C // 7:] = 1
+    pad[B - 1, C // 3] = 1
+    return pad
+
+
+TIED_EMU_CASES = [(1, 33, 1.0, False), (5, 97, 1.0, False), (3, 300, 3.0, False), (2, 129, 8.0, False),
+                  (1, 33, 1.0, True), (5, 97, 1.0, True), (3, 300, 3.0, True), (2, 129, 8.0, True)]
+
+
+@pytest.mark.parametrize("R,C,std,split", TIED_EMU_CASES)
+def test_tied_bounds_cover_an_emulated_kernel(R, C, std, split):
+    """The emulated kernels on two alignments with different padded key columns stay inside every stage and
+    end-to-end bound, and the bounds are not vacuous: P reaches 0.1 of its bound, and with fp16 so do P V and the
+    end-to-end ctx.  (With fp32x3 the end-to-end bound is led by ex2.approx's 2^-22, which the emulation, rounding
+    exp2 correctly, does not reproduce.)"""
+    B, H = 2, 2
+    qkv = _tied_qkv(B, R, C, H, std, seed=R * 1000 + C, split=split)
+    pad = _tied_pad(B, C)
+    out = _tied_ratios(qkv, pad, B, R, C, H, split, _emulate_tied(qkv, pad, B, R, C, H, split))
+    print("tied emulation", R, C, std, split, {k: f"{v:.3f}" for k, v in out.items()})
+    assert max(out.values()) <= 1.0, out
+    assert out["P"] >= 0.1 and (split or (out["pv"] >= 0.1 and out["ctx"] >= 0.1)), out
+
+
+@pytest.mark.parametrize("split", [False, True], ids=["fp16", "fp32x3"])
+def test_tied_bounds_refuse_emulated_faults(split):
+    """P x (1 + 2^-13) leaves the probabilities' row-sum bound; ctx x (1 + 2^-9) and V read from the next alignment
+    row leave the P V bound; an alignment row's slab dropped from the logits, and with fp32x3 the slab's q_lo k_hi
+    pass, leave the logit bound."""
+    B, R, C, H = 2, 5, 97, 2
+    qkv = _tied_qkv(B, R, C, H, 1.0, seed=3, split=split)
+    pad = _tied_pad(B, C)
+    ratios = lambda **f: _tied_ratios(qkv, pad, B, R, C, H, split,  # noqa: E731
+                                      _emulate_tied(qkv, pad, B, R, C, H, split, **f))
+    assert max(ratios().values()) <= 1.0
+    assert ratios(p_scale=1 + 2.0 ** -13)["rowsum"] > 1.0
+    assert ratios(ctx_scale=1 + 2.0 ** -9)["pv"] > 1.0
+    assert ratios(v_shift=1)["pv"] > 1.0
+    assert ratios(drop_slab=R // 2)["logits"] > 1.0
+    if split:
+        assert ratios(drop_lohi=True)["logits"] > 1.0
 
 
 # ---- embedding prologues, mean pool, log-softmax, standalone contact pass, layer ------------------------------------

@@ -1,6 +1,7 @@
 """CPU: host-side logic of the MSA Transformer mirror — state-dict layout, the checkpoint upgrade rule of
 /root/reference/esm/pretrained.py:104-125 (fairseq prefixes stripped, "row" <-> "column" swapped, width of
 msa_position_embedding taken from the tensor), constructor defaults, and the no-CPU-fallback contract."""
+import ctypes
 from argparse import Namespace
 
 import pytest
@@ -109,3 +110,33 @@ def test_factories_raise_without_checkpoint_unless_random_init_is_requested(tmp_
     torch.save({"cfg": cfg, "model": dict(full, **{"encoder.sentence_encoder.bogus": torch.zeros(1)})}, tmp_path / "extra.pt")
     with pytest.raises(RuntimeError, match="Unexpected key"):
         pretrained.load_model_and_alphabet(str(tmp_path / "extra.pt"))
+
+
+# ---- argument refusals of the tied row attention: every check below returns before the device is touched -----------
+# Placeholder pointers, which a refused call never dereferences; run only where no CUDA device is present, so that a
+# refusal lost from the library can never turn into a launch on a bad address.  With a device,
+# tests/test_gpu_tied_attention.py checks the same refusals with real buffers.
+_FAKE = ctypes.c_void_p(4096)
+no_device = pytest.mark.skipif(torch.cuda.is_available(), reason="placeholder pointers: only where nothing can launch")
+
+
+@no_device
+@pytest.mark.parametrize("split", [False, True], ids=["fp16", "fp32x3"])
+@pytest.mark.parametrize("case,shape,rc,msg", [
+    ("C=1025", (1, 1, 1025, 1), -1, b"1024"), ("BH=65536", (1024, 1, 1, 64), -1, b"bad shape"),
+    ("H=65", (1, 1, 1, 65), -1, b"bad shape"), ("scratch-short", (2, 3, 5, 2), -4, b"scratch too small"),
+    ("null-qkv", (2, 3, 5, 2), -1, b"null argument"), ("null-ctx", (2, 3, 5, 2), -1, b"null argument"),
+    ("null-scratch", (2, 3, 5, 2), -1, b"null argument")])
+def test_tied_row_attention_refusals(case, shape, rc, msg, split):
+    from esm_b200 import _lib
+    lib = _lib.load()
+    B, R, C, H = shape
+    nbytes = (lib.esmb200_tied_row_attention_split_scratch_bytes if split else
+              lib.esmb200_tied_row_attention_scratch_bytes)(B, C, H)
+    fn = lib.esmb200_tied_row_attention_split if split else lib.esmb200_tied_row_attention
+    args = [_FAKE, None, _FAKE, None, B, R, C, H, _FAKE, nbytes - (case == "scratch-short"), None]
+    if case.startswith("null"):
+        args[{"null-qkv": 0, "null-ctx": 2, "null-scratch": 8}[case]] = None
+    before = lib.esmb200_launch_count()
+    assert fn(*args) == rc and msg in lib.esmb200_last_error(), lib.esmb200_last_error()
+    assert lib.esmb200_launch_count() == before
