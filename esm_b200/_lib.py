@@ -62,6 +62,8 @@ EXPORTS = (
     "esmb200_layernorm_fp8",
     "esmb200_quantize_fp8",
     "esmb200_gemm_fp8",
+    "esmb200_stack_contacts_bytes",
+    "esmb200_stack_contacts",
 )
 
 ABI_VERSION = 2
@@ -138,6 +140,13 @@ def _declare(lib):
                                                    c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int64,
                                                    c_int32, POINTER(ContactJob), c_void_p, c_size_t, c_void_p,
                                                    c_size_t, c_void_p, c_void_p]
+    lib.esmb200_stack_contacts_bytes.restype = c_int32
+    lib.esmb200_stack_contacts_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                                 POINTER(c_size_t), POINTER(c_size_t), POINTER(c_size_t)]
+    lib.esmb200_stack_contacts.restype = c_int32
+    lib.esmb200_stack_contacts.argtypes = [POINTER(c_void_p), c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                           c_void_p, POINTER(c_void_p), POINTER(ContactJob), c_void_p, c_size_t,
+                                           c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]
     lib.esmb200_embed_tokens.restype = c_int32
     lib.esmb200_embed_tokens.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                          c_int32, c_void_p]

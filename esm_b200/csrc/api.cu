@@ -171,6 +171,10 @@ int check_device() {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// esmb200_contact_accumulate's limit (its shared memory holds 8 rows of S floats)
+constexpr int kContactMaxS = 1024;
+const char* const kContactMaxSMsg = "contact head supports at most 1024 positions";
+
 template <bool SPLIT>
 cudaError_t launch_gemm_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to,
                             const GemmParams& p, cudaStream_t st) {
@@ -279,8 +283,8 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
   ap.slots = slots;
   ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
   ap.ctx = static_cast<__half*>(ctx);
-  ap.row_max = probs ? s.row_max : nullptr;
-  ap.row_sum = probs ? s.row_sum : nullptr;
+  ap.row_max = probs || contact ? s.row_max : nullptr;  // the contact pass reads them, with or without probs
+  ap.row_sum = probs || contact ? s.row_sum : nullptr;
   cudaError_t e;
   {
     CUtensorMap tkv;
@@ -290,8 +294,9 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
     e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "attention launch");
-  if (probs && contact && !split) {
-    // probabilities written once and folded into the contact accumulators in the same pass (attention_contact.cuh)
+  if (contact && !split) {
+    // probabilities written once and folded into the contact accumulators in the same pass (attention_contact.cuh);
+    // probs == nullptr: the same pass without the stores (esmb200_stack_contacts)
     if (B > 65535) return fail(ESMB200_EINVAL, "return_contacts: B must be <= 65535");
     ContactFuseParams cp;
     cp.B = B; cp.T = T; cp.H = H; cp.E = E; cp.slots = slots;
@@ -324,6 +329,22 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
     }
     if (e != cudaSuccess) return fail_cuda(e, "attention probs launch");
   }
+  return ESMB200_OK;
+}
+
+// contact_accumulate_kernel on one layer's maps (arguments validated by the caller: S = hi - lo <= 1024, B <= 65535)
+int run_contact_accumulate(const float* attn, long long batch_stride, const float* w, const uint8_t* keep, float* acc,
+                           float* row_sum, float* col_part, int B, int H, int T, int lo, int S, cudaStream_t st) {
+  ProfScope ps(T_PROBS, st);
+  const size_t smem = (size_t)8 * S * sizeof(float);
+  dim3 grid((S + 15) / 16, B);  // 8 warps x 2 rows
+  if (S <= 512)
+    contact_accumulate_kernel<2, 16, 2><<<grid, 256, smem, st>>>(attn, batch_stride, w, keep, acc, row_sum, col_part, H, T,
+                                                                  lo, S);
+  else
+    contact_accumulate_kernel<2, 32, 1><<<grid, 256, smem, st>>>(attn, batch_stride, w, keep, acc, row_sum, col_part, H, T,
+                                                                  lo, S);
+  CK(cudaGetLastError());
   return ESMB200_OK;
 }
 
@@ -886,21 +907,43 @@ int esmb200_layer_offload(esmb200_layer* L, void* host_dst, size_t bytes, void* 
   return ESMB200_OK;
 }
 
-// the layer loop of esmb200_stack_forward (ring == nullptr: every layer's weights resident) and of
-// esmb200_stack_forward_streamed (every layer offloaded, its packed matrices copied into `ring` ahead of use)
+// esmb200_stack_contacts: the partial buffers of a contact job and the fp32x3 probability scratch, in bytes
+struct ContactSizes {
+  size_t row_part, col_part, scratch;
+};
+
+static ContactSizes contact_sizes(int n_layers, int H, int B, int T, int S, int precision) {
+  const size_t lbh = (size_t)n_layers * B * H;
+  ContactSizes c;
+  if (precision == 1) {  // fp32x3: contact_accumulate_kernel's row sums and 16-row column stripes, one layer's maps
+    c.row_part = lbh * S * 4;
+    c.col_part = lbh * ((S + 15) / 16) * S * 4;
+    c.scratch = (size_t)B * H * T * T * 4;
+  } else {  // the fused pass: one partial per 32-key / 32-query quarter of each 128-wide tile
+    c.row_part = c.col_part = lbh * 4 * ((T + 127) / 128) * S * 4;
+    c.scratch = 0;
+  }
+  return c;
+}
+
+// the layer loop of esmb200_stack_forward (ring == nullptr: every layer's weights resident), of
+// esmb200_stack_forward_streamed (every layer offloaded, its packed matrices copied into `ring` ahead of use) and, with
+// contacts_only, of esmb200_stack_contacts (attn_out == nullptr; fp32x3 maps go through `scratch` one layer at a time)
 static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask,
                               int32_t B, int32_t T, const float* rope_cos, const float* rope_sin,
                               float* const* repr_out, float* const* attn_out, int64_t attn_batch_stride,
                               int32_t attn_flags, const esmb200_contact_job* contact, void* workspace,
-                              size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream, void* stream) {
+                              size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream, void* stream,
+                              bool contacts_only = false, void* scratch = nullptr, size_t scratch_bytes = 0) {
   if (!layers || n_layers <= 0 || !x || !workspace) return fail(ESMB200_EINVAL, "null argument");
   for (int i = 0; i < n_layers; ++i)
     if (!layers[i]) return fail(ESMB200_EINVAL, "null layer");
   if ((rope_cos == nullptr) != (rope_sin == nullptr))  // both NULL: no rotary embedding (ESM-1b / ESM-1v)
     return fail(ESMB200_EINVAL, "rope_cos and rope_sin must both be given or both be NULL");
+  if (contacts_only && !contact) return fail(ESMB200_EINVAL, "null contact job");
   if (contact) {
-    if (!attn_out) return fail(ESMB200_EINVAL, "a contact job needs attn_out for every layer");
-    for (int i = 0; i < n_layers; ++i)
+    if (!contacts_only && !attn_out) return fail(ESMB200_EINVAL, "a contact job needs attn_out for every layer");
+    for (int i = 0; i < n_layers && !contacts_only; ++i)
       if (!attn_out[i]) return fail(ESMB200_EINVAL, "a contact job needs attn_out for every layer");
     if (!contact->weights || !contact->acc || !contact->row_part || !contact->col_part || contact->lo < 0 ||
         contact->hi > T || contact->hi <= contact->lo)
@@ -929,6 +972,18 @@ static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, fl
   const int precision = layers[0]->fp8 ? 2 : split;
   const Workspace ws = workspace_layout(workspace, E, H, F, B, T, precision);
   if (workspace_bytes < ws.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
+  const int S = contact ? contact->hi - contact->lo : 0;
+  if (contacts_only) {  // refused before anything is launched
+    if (B > 65535) return fail(ESMB200_EINVAL, "return_contacts: B must be <= 65535");
+    if (split) {
+      if (S > kContactMaxS) return fail(ESMB200_EINVAL, kContactMaxSMsg);
+      if ((size_t)B * H > 65535) return fail(ESMB200_EINVAL, "need_head_weights: B*H must be <= 65535");
+      if (!scratch || scratch_bytes < contact_sizes(n_layers, H, B, T, S, precision).scratch)
+        return fail(ESMB200_EWORKSPACE, "probability scratch smaller than esmb200_stack_contacts_bytes");
+      if (reinterpret_cast<uintptr_t>(scratch) % 16 != 0)
+        return fail(ESMB200_EINVAL, "probability scratch must be 16-byte aligned");
+    }
+  }
   ActMaps am;
   rc = make_act_maps(&am, ws, x, E, H, F, B * T, precision);
   if (rc) return rc;
@@ -960,17 +1015,32 @@ static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, fl
     }
     ContactLayer cl;
     if (contact) {
-      const int S = contact->hi - contact->lo;
       const size_t part = (size_t)B * H * nt128 * S;
       cl.w = contact->weights + (size_t)i * H; cl.keep = contact->keep; cl.acc = contact->acc;
       cl.row_part = contact->row_part + (size_t)i * 4 * part; cl.col_part = contact->col_part + (size_t)i * 4 * part;
       cl.lo = contact->lo; cl.S = S;
     }
     float* probs = attn_out ? attn_out[i] : nullptr;
-    rc = attention_block(L, *wm, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
-      return run_attention(ws.qkv, ws.ctx, probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split != 0,
-                           contact ? &cl : nullptr, L->slots);  // multihead_attention.py:357-394
-    });
+    if (contacts_only && split) {
+      // fp32x3: this layer's maps into the scratch with the split probability kernel (padded query rows zeroed, as
+      // the forward writes them), then contact_accumulate_kernel, as ContactPredictionHead.forward runs it on the stack
+      rc = attention_block(L, *wm, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
+        const size_t lbh = (size_t)i * B * H;
+        int r = run_attention(ws.qkv, ws.ctx, static_cast<float*>(scratch), 0, 1, ws.as, B, T, H, st, true, nullptr,
+                              L->slots);
+        if (!r)
+          r = run_contact_accumulate(static_cast<const float*>(scratch), (long long)H * T * T, cl.w, contact->keep,
+                                     contact->acc, contact->row_part + lbh * S,
+                                     contact->col_part + lbh * ((S + 15) / 16) * S, B, H, T, contact->lo, S, st);
+        return r;
+      });
+    } else {
+      rc = attention_block(L, *wm, x, B * T, T, rope_cos, rope_sin, L->q_scale, ws, am, st, [&] {
+        // contacts_only: probs == nullptr and attn_flags bit 0 set, the store-free fused pass
+        return run_attention(ws.qkv, ws.ctx, probs, attn_batch_stride, attn_flags, ws.as, B, T, H, st, split != 0,
+                             contact ? &cl : nullptr, L->slots);  // multihead_attention.py:357-394
+      });
+    }
     if (!rc) rc = ffn_block(L, *wm, x, B * T, ws, am, st);
     if (rc) return rc;
     if (streamed) {  // fc2 was the slot's last reader: layer i + 2 may overwrite it
@@ -1003,6 +1073,28 @@ int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layer
   return stack_forward_impl(layers, n_layers, x, pad_mask, B, T, rope_cos, rope_sin, repr_out, attn_out,
                             attn_batch_stride, attn_flags, contact, workspace, workspace_bytes, ring, ring_bytes,
                             copy_stream, stream);
+}
+
+int esmb200_stack_contacts_bytes(int32_t n_layers, int32_t num_heads, int32_t B, int32_t T, int32_t S,
+                                 int32_t precision, size_t* row_part_bytes, size_t* col_part_bytes,
+                                 size_t* scratch_bytes) {
+  if (n_layers <= 0 || num_heads <= 0 || B <= 0 || T <= 0 || S <= 0 || S > T || precision < 0 || precision > 2)
+    return fail(ESMB200_EINVAL, "bad shape");
+  const ContactSizes c = contact_sizes(n_layers, num_heads, B, T, S, precision);
+  if (row_part_bytes) *row_part_bytes = c.row_part;
+  if (col_part_bytes) *col_part_bytes = c.col_part;
+  if (scratch_bytes) *scratch_bytes = c.scratch;
+  return ESMB200_OK;
+}
+
+int esmb200_stack_contacts(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask, int32_t B,
+                           int32_t T, const float* rope_cos, const float* rope_sin, float* const* repr_out,
+                           const esmb200_contact_job* contact, void* probs_scratch, size_t probs_scratch_bytes,
+                           void* workspace, size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream,
+                           void* stream) {
+  return stack_forward_impl(layers, n_layers, x, pad_mask, B, T, rope_cos, rope_sin, repr_out, nullptr, 0,
+                            1 /* padded query rows zero, as in ESM2.forward */, contact, workspace, workspace_bytes,
+                            ring, ring_bytes, copy_stream, stream, true, probs_scratch, probs_scratch_bytes);
 }
 
 int esmb200_layer_forward(esmb200_layer* layer, float* x, const uint8_t* pad_mask, int32_t B, int32_t T,
@@ -1377,19 +1469,9 @@ int esmb200_contact_accumulate(const float* attn, int64_t batch_stride, const fl
   if (!attn || !w || !acc || !row_sum || !col_part) return fail(ESMB200_EINVAL, "null argument");
   const int S = hi - lo;
   if (B <= 0 || H <= 0 || T <= 0 || lo < 0 || hi > T || S <= 0 || B > 65535) return fail(ESMB200_EINVAL, "bad shape");
-  if (S > 1024) return fail(ESMB200_EINVAL, "contact head supports at most 1024 positions");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  ProfScope ps(T_PROBS, st);
-  const size_t smem = (size_t)8 * S * sizeof(float);
-  dim3 grid((S + 15) / 16, B);  // 8 warps x 2 rows
-  if (S <= 512)
-    contact_accumulate_kernel<2, 16, 2><<<grid, 256, smem, st>>>(attn, batch_stride, w, keep, acc, row_sum, col_part, H, T,
-                                                                  lo, S);
-  else
-    contact_accumulate_kernel<2, 32, 1><<<grid, 256, smem, st>>>(attn, batch_stride, w, keep, acc, row_sum, col_part, H, T,
-                                                                  lo, S);
-  CK(cudaGetLastError());
-  return ESMB200_OK;
+  if (S > kContactMaxS) return fail(ESMB200_EINVAL, kContactMaxSMsg);
+  return run_contact_accumulate(attn, batch_stride, w, keep, acc, row_sum, col_part, B, H, T, lo, S,
+                                static_cast<cudaStream_t>(stream));
 }
 
 int esmb200_contact_finalize(const float* acc, const float* u, const float* a1, const float* bias, float* out, int32_t B,

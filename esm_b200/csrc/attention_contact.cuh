@@ -1,6 +1,9 @@
 // esm_b200 — need_head_weights + return_contacts in ONE pass (sm_90a, head_dim <= 64, or <= 128 with DS = 2): the
 // attention probabilities of a layer are written to the stacked [B,L,H,T,T] result AND folded into the contact head's
 // accumulators while they are still in registers, so the 4*B*L*H*T^2-byte stack is written once and never read back.
+// The STORE = false instantiation (esmb200_stack_contacts: contacts without the stack) is the same pass without the
+// probability stores: same tiles, same masked_prob arithmetic, same accumulation order, so its acc, row_part and
+// col_part are bit-identical to the storing pass's, and the caller never allocates the stack.
 //
 // Replaces esm/multihead_attention.py:397-400 (per-head probabilities) and the per-layer share of
 // ContactPredictionHead.forward, esm/modules.py:338-357 (eos masking, bos/eos crop, symmetrize :27-29, apc :32-41), in
@@ -27,7 +30,8 @@ struct ContactFuseParams {
   int words;
   const float* row_max;      // [B,H,T] reference max / row sum of the forward kernel
   const float* row_sum;
-  float* probs;              // this layer's slice of the stacked result: batch b at probs + b * batch_stride
+  float* probs;              // this layer's slice of the stacked result: batch b at probs + b * batch_stride; NULL:
+                             // contacts only (the STORE = false instantiation)
   long long batch_stride;
   int zero_pad_rows;
   // contact head
@@ -49,7 +53,7 @@ constexpr int smem_bytes(int ds) {  // ds operand tiles per Q and per K stage
 }
 }  // namespace cfuse_cfg
 
-template <int DS>
+template <int DS, bool STORE>  // STORE = false: p.probs and p.batch_stride are not read, no probability is written
 __global__ void __launch_bounds__(cfuse_cfg::NUM_THREADS, 1)
 attention_probs_contact_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const ContactFuseParams p) {
   using namespace cfuse_cfg;
@@ -143,14 +147,15 @@ attention_probs_contact_kernel(const __grid_constant__ CUtensorMap tmap_qkv, con
         const float l = p.row_sum[si];
         inv = (l > 0.f && !qpad[r]) ? 1.0f / l : 0.f;  // esm2.py:135-139: rows of padded query tokens are zero
       }
-      float* dst = p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + (size_t)t[r] * p.T + k0;
+      float* dst = STORE ? p.probs + (size_t)b * p.batch_stride + (size_t)h * p.T * p.T + (size_t)t[r] * p.T + k0
+                         : nullptr;
 #pragma unroll
       for (int nb = 0; nb < 16; ++nb)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int key = nb * 8 + 2 * (int)c + e;
           const float pr = live ? masked_prob(sc[nb][2 * r + e], kw[nb / 4], key, mneg, inv) : 0.f;
-          if (row_ok[r] && key < ncols) dst[key] = pr;
+          if (STORE && row_ok[r] && key < ncols) dst[key] = pr;
           const float x = (ri[r] && ((cmask >> (2 * nb + e)) & 1u)) ? pr : 0.f;
           acc[nb][2 * r + e] = fmaf(wh, x, acc[nb][2 * r + e]);
           rs[r][nb / 4] += x;
@@ -204,21 +209,26 @@ attention_probs_contact_kernel(const __grid_constant__ CUtensorMap tmap_qkv, con
   }
 }
 
-template <int DS>
+template <int DS, bool STORE>
 inline cudaError_t launch_attention_probs_contact_ds(const CUtensorMap& tmap_qkv, const ContactFuseParams& p,
                                                      cudaStream_t stream) {
   using namespace cfuse_cfg;
   constexpr int smem = smem_bytes(DS);
-  cudaError_t e = cudaFuncSetAttribute(attention_probs_contact_kernel<DS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaError_t e = cudaFuncSetAttribute(attention_probs_contact_kernel<DS, STORE>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   dim3 grid((p.T + BLOCK - 1) / BLOCK, (p.T + BLOCK - 1) / BLOCK, p.B);
-  return launch_pdl(attention_probs_contact_kernel<DS>, grid, dim3(NUM_THREADS), smem, stream, tmap_qkv, p);
+  return launch_pdl(attention_probs_contact_kernel<DS, STORE>, grid, dim3(NUM_THREADS), smem, stream, tmap_qkv, p);
 }
 
+// p.probs == NULL: the store-free pass (contacts only)
 inline cudaError_t launch_attention_probs_contact(const CUtensorMap& tmap_qkv, const ContactFuseParams& p,
                                                   cudaStream_t stream) {
-  return p.slots == 2 ? launch_attention_probs_contact_ds<2>(tmap_qkv, p, stream)
-                      : launch_attention_probs_contact_ds<1>(tmap_qkv, p, stream);
+  if (p.probs)
+    return p.slots == 2 ? launch_attention_probs_contact_ds<2, true>(tmap_qkv, p, stream)
+                        : launch_attention_probs_contact_ds<1, true>(tmap_qkv, p, stream);
+  return p.slots == 2 ? launch_attention_probs_contact_ds<2, false>(tmap_qkv, p, stream)
+                      : launch_attention_probs_contact_ds<1, false>(tmap_qkv, p, stream);
 }
 
 }  // namespace esmb200

@@ -6,6 +6,8 @@ command line and the output files of the reference's `esm-extract` (/root/refere
 What differs from the reference's loop (which runs the model, copies whole padded batches to the host and calls
 torch.save in line, so the GPU idles during the copies and the pickling):
   * the model runs through libesmb200.so (GPU required; there is no --nogpu path);
+  * --include contacts runs the forward without the [B,L,H,T,T] attention stack (same contacts, bit for bit), so the
+    default token budget fits long sequences;
   * the per-sequence mean (extract.py:116-119) is reduced on the device (`esmb200_mean_pool`), `bos` is sliced on the
     device: only what was asked for crosses PCIe;
   * device->host copies go to pinned staging buffers on a side stream and are overlapped with the next batch's forward
@@ -188,7 +190,10 @@ def run(args) -> int:
                 labels, strs, toks = to_tokens([dataset[i] for i in idxs])
                 lengths = [min(args.truncation_seq_length, len(s)) for s in strs]
                 toks_dev = toks.pin_memory().to(dev, non_blocking=True)
-                out = model(toks_dev, repr_layers=layers, return_contacts=want_contacts)
+                # contacts: the forward without the attention stack (ProteinLanguageModel._contacts_forward), so only
+                # the representations and the [B,S,S] contacts stay alive with the batch while its copies run
+                out = (model._contacts_forward(toks_dev, repr_layers=layers) if want_contacts
+                       else model(toks_dev, repr_layers=layers))
                 reps = out["representations"]
                 B, T, E = next(iter(reps.values())).shape
                 computed = torch.cuda.Event()

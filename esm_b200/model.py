@@ -274,10 +274,12 @@ def _ring(nbytes: int, device: torch.device):
 def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Tensor],
               rope_cos: Optional[torch.Tensor], rope_sin: Optional[torch.Tensor],
               repr_out: Optional[Dict[int, torch.Tensor]], attn_layers: Sequence[int], zero_pad_rows: bool = False,
-              contact_job=None):
+              contact_job=None, contacts_only: bool = False, probs_scratch: Optional[torch.Tensor] = None):
     """esmb200_stack_forward on x fp32 (B,T,E) in place. repr_out: {layer index (0-based): (B,T,E) tensor to fill}.
     rope_cos = rope_sin = None: layers without rotary embedding (ESM-1b / ESM-1v).
     Layers offloaded by cpu_offload() run through esmb200_stack_forward_streamed instead, with the same results.
+    contacts_only: esmb200_stack_contacts with `contact_job` (ContactPredictionHead.begin_contacts) and no attention
+    maps; probs_scratch is its fp32x3 scratch.
     Returns {layer index: (B,H,T,T) fp32} for the indices in attn_layers."""
     if not x.is_cuda:
         raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
@@ -312,11 +314,24 @@ def run_stack(layers: Sequence, x: torch.Tensor, padding_mask: Optional[torch.Te
                 attn_t[i] = a
                 attns[i] = a.data_ptr()
         keep.append(mask)
+        offloaded = getattr(layers[0], "offloaded", False)
+        if contacts_only:
+            assert contact_job is not None and not attn_layers
+            args = (handles, n, _ptr(x), _ptr(mask), B, T, _ptr(rope_cos), _ptr(rope_sin),
+                    reprs if repr_out else None, ctypes.byref(contact_job), _ptr(probs_scratch),
+                    probs_scratch.nbytes if probs_scratch is not None else 0, _ptr(ws), ws.numel())
+            if offloaded:
+                ring, copy = _ring(2 * lib.esmb200_layer_packed_bytes(E, H, Fdim, precision), x.device)
+                _lib.check(lib.esmb200_stack_contacts(*args, _ptr(ring), ring.numel(),
+                                                      ctypes.c_void_p(copy.cuda_stream), _stream()))
+            else:
+                _lib.check(lib.esmb200_stack_contacts(*args, None, 0, None, _stream()))
+            return {}
         args = (handles, n, _ptr(x), _ptr(mask), B, T, _ptr(rope_cos), _ptr(rope_sin),
                 reprs if repr_out else None, attns if attn_layers else None,
                 (len(attn_layers) * H * T * T) if attn_layers else 0, 1 if zero_pad_rows else 0,
                 ctypes.byref(contact_job) if contact_job is not None else None, _ptr(ws), ws.numel())
-        if getattr(layers[0], "offloaded", False):
+        if offloaded:
             ring, copy = _ring(2 * lib.esmb200_layer_packed_bytes(E, H, Fdim, precision), x.device)
             _lib.check(lib.esmb200_stack_forward_streamed(*args, _ptr(ring), ring.numel(),
                                                           ctypes.c_void_p(copy.cuda_stream), _stream()))
@@ -482,16 +497,34 @@ class ContactPredictionHead(nn.Module):
     def begin_job(self, tokens: torch.Tensor, num_layers: int, num_heads: int):
         """Buffers + esmb200_contact_job for a [B,T] batch (attention_contact.cuh); finish_job() turns them into contacts."""
         B, T = tokens.shape
+        nt = (T + 127) // 128
+        shape = lambda S: (num_layers, B, num_heads, 4 * nt, S)
+        return self._job(tokens, num_layers, num_heads, shape, shape)
+
+    def begin_contacts(self, tokens: torch.Tensor, num_layers: int, num_heads: int, precision: int):
+        """Buffers + esmb200_contact_job for esmb200_stack_contacts (contacts without the attention stack); precision
+        as esmb200_layer_weights.precision. fp16 and fp8: begin_job's. fp32x3: per layer the row sums and 16-row
+        column stripes of esmb200_contact_accumulate, plus one layer's [B,H,T,T] probability scratch.
+        finish_contacts() turns them into contacts."""
+        if precision != 1:
+            return self.begin_job(tokens, num_layers, num_heads)
+        B, T = tokens.shape
+        st = self._job(tokens, num_layers, num_heads, lambda S: (num_layers, B, num_heads, S),
+                       lambda S: (num_layers, B, num_heads, (S + 15) // 16, S))
+        st["scratch"] = torch.empty((B, num_heads, T, T), dtype=torch.float32, device=tokens.device)
+        return st
+
+    def _job(self, tokens, num_layers, num_heads, row_shape, col_shape):
+        B, T = tokens.shape
         lo = 1 if self.prepend_bos else 0
         hi = T - 1 if self.append_eos else T
         S = hi - lo
         dev = tokens.device
-        nt = (T + 127) // 128
         st = {
             "keep": tokens.ne(self.eos_idx).to(torch.uint8).contiguous() if self.append_eos else None,
             "acc": torch.zeros((B, S, S), dtype=torch.float32, device=dev),
-            "row": torch.empty((num_layers, B, num_heads, 4 * nt, S), dtype=torch.float32, device=dev),
-            "col": torch.empty((num_layers, B, num_heads, 4 * nt, S), dtype=torch.float32, device=dev),
+            "row": torch.empty(row_shape(S), dtype=torch.float32, device=dev),
+            "col": torch.empty(col_shape(S), dtype=torch.float32, device=dev),
             "w": _f32(self.regression.weight).view(num_layers, num_heads).contiguous(),
         }
         job = _lib.ContactJob()
@@ -505,6 +538,16 @@ class ContactPredictionHead(nn.Module):
         L, B, H, _, S = st["row"].shape
         a1 = st["row"].sum(3) + st["col"].sum(3)                          # [L,B,H,S], fixed summation order
         return self._finalize(st["acc"], a1.permute(1, 0, 2, 3).reshape(B, L * H, S), st["w"])
+
+    def finish_contacts(self, st) -> torch.Tensor:
+        """Contacts from begin_contacts' buffers once esmb200_stack_contacts has filled them."""
+        if st["row"].dim() == 5:
+            return self.finish_job(st)
+        L, B, H, S = st["row"].shape  # fp32x3: a1 exactly as forward() builds it from the per-layer accumulations
+        a1 = torch.empty((B, L, H, S), dtype=torch.float32, device=st["acc"].device)
+        for l in range(L):
+            torch.add(st["row"][l], st["col"][l].sum(2), out=a1[:, l])
+        return self._finalize(st["acc"], a1.view(B, L * H, S), st["w"])
 
     def _forward_torch(self, tokens, attentions, w, lo, hi):
         """The same formula with PyTorch ops (non-CUDA or non-fp32 inputs; cross-check in the tests)."""
@@ -667,11 +710,12 @@ class ProteinLanguageModel(nn.Module):
         return hit[1]
 
     def _stack(self, tokens, repr_layers=frozenset(), need_head_weights=False, return_contacts=False,
-               cast=lambda t: t):
+               cast=lambda t: t, contacts_only=False):
         """The stack step of `forward` (esm2.py:82-121): embedding prologue and one esmb200_stack_forward.
         Returns (tokens int64 contiguous, x, hidden, attn_t, cjob): x is the fp32 residual stream [B,T,E] BEFORE
         emb_layer_norm_after, hidden {i: cast(representation)} for the requested layers below num_layers, attn_t
-        run_stack's attention maps, cjob the fused contact job or None.  Runs under torch.cuda.device(tokens.device)."""
+        run_stack's attention maps, cjob the fused contact job or None.  Runs under torch.cuda.device(tokens.device).
+        contacts_only: esmb200_stack_contacts instead, no attention maps; cjob is begin_contacts' job."""
         assert tokens.ndim == 2
         if not tokens.is_cuda:
             raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
@@ -702,11 +746,17 @@ class ProteinLanguageModel(nn.Module):
             cos, sin = self._rope_tables(T)
             # contacts: folded into the probability pass (fp16 and fp8 modes, whose attention is the fp16 kernel; fp32x3
             # runs the separate kernels afterwards)
-            cjob = (self.contact_head.begin_job(tokens, N, self.attention_heads)
-                    if return_contacts and self.precision in ("fp16", "fp8") else None)
-            attn_t = run_stack(list(self.layers), x, mask, cos, sin, repr_out,
-                               list(range(N)) if need_head_weights else [], zero_pad_rows=True,
-                               contact_job=cjob["job"] if cjob else None)
+            if contacts_only:
+                cjob = self.contact_head.begin_contacts(tokens, N, self.attention_heads,
+                                                        self.LAYER_PRECISIONS[self.precision])
+                attn_t = run_stack(list(self.layers), x, mask, cos, sin, repr_out, [], zero_pad_rows=True,
+                                   contact_job=cjob["job"], contacts_only=True, probs_scratch=cjob.pop("scratch", None))
+            else:
+                cjob = (self.contact_head.begin_job(tokens, N, self.attention_heads)
+                        if return_contacts and self.precision in ("fp16", "fp8") else None)
+                attn_t = run_stack(list(self.layers), x, mask, cos, sin, repr_out,
+                                   list(range(N)) if need_head_weights else [], zero_pad_rows=True,
+                                   contact_job=cjob["job"] if cjob else None)
             for i, t in repr_out.items():
                 hidden[i + 1] = cast(t)
         return tokens, x, hidden, attn_t, cjob
@@ -756,7 +806,30 @@ class ProteinLanguageModel(nn.Module):
         return result
 
     def predict_contacts(self, tokens):
-        return self(tokens, return_contacts=True)["contacts"]
+        """forward(tokens, return_contacts=True)["contacts"], bit for bit, without the [B,L,H,T,T] attention stack:
+        its peak memory is the contact partials (about 1/16 of the stack) instead of the stack."""
+        return self._contacts_forward(tokens)["contacts"]
+
+    @torch.no_grad()
+    def _contacts_forward(self, tokens, repr_layers=()):
+        """forward(tokens, repr_layers, return_contacts=True) without the attention stack and the LM head:
+        {"representations", "contacts"}, each bit-identical to forward's (the last layer post-LN, every tensor in
+        forward's dtype). Runs esmb200_stack_contacts (esmb200_stack_forward's layer loop, store-free contact pass)."""
+        dtype = self.embed_tokens.weight.dtype
+        repr_layers = set(repr_layers)
+        cast = (lambda t: t) if dtype == torch.float32 else (lambda t: t.to(dtype))
+        tokens, x, hidden, _, cjob = self._stack(tokens, repr_layers, cast=cast, contacts_only=True)
+        B, T = tokens.shape
+        E, N = self.embed_dim, self.num_layers
+        with torch.cuda.device(tokens.device):
+            contacts = cast(self.contact_head.finish_contacts(cjob))
+            if N in repr_layers:  # esm2.py:123-128 final LayerNorm, as forward applies it
+                ln = self.emb_layer_norm_after
+                ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)
+                _lib.check(_lib.load().esmb200_layernorm(_ptr(x), _ptr(ln_w), _ptr(ln_b), _ptr(x), B * T, E, ln.eps,
+                                                         _stream()))
+                hidden[N] = cast(x)
+        return {"representations": hidden, "contacts": contacts}
 
 
 class ESM2(ProteinLanguageModel):

@@ -166,6 +166,33 @@ int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layer
                                    void* workspace, size_t workspace_bytes, void* ring, size_t ring_bytes,
                                    void* copy_stream, void* stream);
 
+/* ---- contacts without the attention stack (ProteinLanguageModel.predict_contacts) ----
+ * esmb200_stack_contacts: the layer loop of esmb200_stack_forward with a contact job and no attn_out. x, repr_out and
+ *   the contacts are bit-identical to those of esmb200_stack_forward with attn_out for every layer, attn_flags = 1
+ *   (padded query rows zero, as ESM2.forward asks) and the same job; the [B,L,H,T,T] stack is neither written nor
+ *   needed. contact: required (NULL is ESMB200_EINVAL); acc zeroed by the caller. ring == NULL: every layer resident;
+ *   otherwise every layer offloaded, with the ring, copy_stream and event protocol of esmb200_stack_forward_streamed.
+ *   Mixed precision, or resident and offloaded layers mixed, is ESMB200_EINVAL.
+ *   fp16 and fp8 layers: the fused pass without its probability stores (attention_contact.cuh); row_part and col_part
+ *     have the esmb200_contact_job layout [n_layers,B,H,4*nt,S]. probs_scratch is not used and may be NULL.
+ *   fp32x3 layers: per layer, the split probability kernel writes the maps into probs_scratch (fp32 [B,H,T,T], 16-byte
+ *     aligned), then esmb200_contact_accumulate's kernel reads them: row_part is row_sum [n_layers,B,H,S] and col_part
+ *     is col_part [n_layers,B,H,ceil(S/16),S] of that entry, layer l at offset l*B*H*S and l*B*H*ceil(S/16)*S.
+ *     a1 of layer l = row_part[l] + col_part[l] summed over its stripe axis. S <= 1024, B*H <= 65535.
+ *   A probs_scratch or workspace smaller than its size is ESMB200_EWORKSPACE. Every refusal comes before any launch.
+ * esmb200_stack_contacts_bytes: bytes of row_part, col_part and probs_scratch for n_layers layers of num_heads heads,
+ *   a [B,T] batch and S = hi - lo cropped positions in `precision` (0 fp16, 1 fp32x3, 2 fp8); scratch is 0 for 0 and 2.
+ *   Pure host arithmetic; ESMB200_EINVAL for a non-positive size, S > T or an unknown precision. Out pointers may be
+ *   NULL. */
+int esmb200_stack_contacts_bytes(int32_t n_layers, int32_t num_heads, int32_t B, int32_t T, int32_t S,
+                                 int32_t precision, size_t* row_part_bytes, size_t* col_part_bytes,
+                                 size_t* scratch_bytes);
+int esmb200_stack_contacts(esmb200_layer* const* layers, int32_t n_layers, float* x, const uint8_t* pad_mask, int32_t B,
+                           int32_t T, const float* rope_cos, const float* rope_sin, float* const* repr_out,
+                           const esmb200_contact_job* contact, void* probs_scratch, size_t probs_scratch_bytes,
+                           void* workspace, size_t workspace_bytes, void* ring, size_t ring_bytes, void* copy_stream,
+                           void* stream);
+
 /* Embedding prologue of ESM2.forward (esm2.py:84-95): gather from table [V,E], zero <mask> rows and rescale by
  * 0.88/(1 - n_mask/n_nonpad) when token_dropout, zero pad rows. tokens int64 [B,T] -> x fp32 [B,T,E].
  * E % 4 == 0, B <= 65535. Pad rows are written as zeros whatever the scale: a sequence of pads only (scale 0/0) gives
