@@ -9,9 +9,10 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
   * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf);
   * split16 / join64 / split_rep_bound / split_acc_bound / FP32X3_MODELS: the fp32x3 precision's hi | lo operand pairs,
     the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs;
-  * attention64 / attn_ctx_bound / attn_relfro_gate / attn_probs_bound / attn_rowsum_bound / attn_max_bound /
-    attn_sum_bound: float64 softmax attention on fp16 q, k, v and the first-order error model of the fp16 attention
-    kernels (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2);
+  * attention64 / attention64_rows / attn_ctx_bound / attn_relfro_gate / attn_probs_bound / attn_rowsum_bound /
+    attn_max_bound / attn_sum_bound: float64 softmax attention on fp16 q, k, v (whole heads, or slices of their query
+    rows so that T = 16384 fits a few GB) and the first-order error model of the fp16 attention kernels
+    (csrc/attention_wg.cuh, attention8.cuh <false, 2>, attention_probs.cuh modes 0 and 2);
   * tied64 / tied_softmax64 / tied_probs_bound / tied_P_bound / tied_rowsum_bound / tied_pv / tied_ctx_bound /
     tied_relfro_gate: the MSA Transformer's tied row attention (csrc/tied_attention.cuh, fp16 and fp32x3) end to end
     and stage by stage, each stage on the kernel's own inputs (logits, softmax of its logits, P V of its P);
@@ -204,17 +205,19 @@ F16_U = 2.0 ** -11  # unit roundoff of fp16
 
 
 def attention64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, padded: Optional[torch.Tensor], block: int) -> Dict:
-    """float64 softmax attention of fp16 q, k, v [B, H, T, D] (D = 64 or 128) under the key-padding mask `padded`
-    [B, T] (True: padded key; None: none), with what the error bounds below need.  Rows of an all-padding sequence are 0
-    (ctx, p, m and l).
-      * lerr [B,H,T,T]: the absolute error bound of each logit, (D/16 + 4) 2^-22 sum_d |q_d k_d| (the GEMM's
+    """float64 softmax attention of fp16 queries q [B, H, Tq, D] on keys and values k, v [B, H, T, D] (D = 64 or 128)
+    under the key-padding mask `padded` [B, T] (True: padded key; None: none), with what the error bounds below need.
+    q may be any slice of a head's query rows (attention64_rows): every row's values depend on that row and the keys
+    alone.  Rows of an all-padding sequence are 0 (ctx, p, m and l).
+      * lerr [B,H,Tq,T]: the absolute error bound of each logit, (D/16 + 4) 2^-22 sum_d |q_d k_d| (the GEMM's
         accumulation bound: D/16 truncating k16 steps, one ulp of a partial sum bounded by sum|q k| each, doubled,
         plus 4 steps);
-      * delta [B,H,T,T]: the relative error bound Delta_j of key j's unnormalised weight e^(s_j - m): its logit (lerr),
-        ex2.approx (2 ulp = 2^-22, doubled) and the fp32 roundings of log2e, s log2e and -m log2e (2^-23 (|s| + 3 |m|));
+      * delta [B,H,Tq,T]: the relative error bound Delta_j of key j's unnormalised weight e^(s_j - m): its logit
+        (lerr), ex2.approx (2 ulp = 2^-22, doubled) and the fp32 roundings of log2e, s log2e and -m log2e
+        (2^-23 (|s| + 3 |m|));
       * nblk [B,1,1,1]: the key blocks the kernel walks, ceil(kvlen / block), kvlen = 1 + the last attendable key."""
     q, k, v = q.double(), k.double(), v.double()
-    B, H, T, D = q.shape
+    B, H, T, D = k.shape
     if padded is None:
         padded = torch.zeros(B, T, dtype=torch.bool, device=q.device)
     padded = padded.bool()
@@ -232,6 +235,19 @@ def attention64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, padded: Optio
     kvlen = torch.where(padded, torch.zeros_like(idx), idx).amax(-1)
     nblk = ((kvlen + block - 1) // block).double()[:, None, None, None]
     return dict(q=q, k=k, v=v, s=s, m=m, l=l, p=p, ctx=p @ v, lerr=lerr, delta=delta, nblk=nblk, km=km, block=block)
+
+
+def attention64_rows(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, padded: Optional[torch.Tensor], block: int,
+                     max_elems: int = 1 << 23):
+    """attention64 over consecutive slices of the query rows, so that one head at T = 16384 fits a few GB: yields
+    (i0, r), r = attention64(q[..., i0:i0 + n, :], k, v, padded, block), with n rows per slice (the last may have
+    fewer) such that a [B, H, n, T] tensor holds at most max_elems elements (at least one row).  The element-wise
+    values and bounds of a slice are those of the same rows of the whole-head reference; the per-head gate is
+    attn_relfro_combine of the slices' attn_relfro_terms, summed."""
+    B, H, Tq, _ = q.shape
+    n = max(1, max_elems // (B * H * k.shape[-2]))
+    for i0 in range(0, Tq, n):
+        yield i0, attention64(q[..., i0:i0 + n, :], k, v, padded, block)
 
 
 def _vsum(r, f) -> torch.Tensor:
@@ -283,7 +299,8 @@ GATE_SIGMAS = 3.0
 
 
 def attn_relfro_gate(r) -> torch.Tensor:
-    """[B, H]: the per-(sequence, head) bound of ||ctx - ctx64||_F / ||ctx64||_F.
+    """[B, H]: the per-(sequence, head) bound of ||ctx - ctx64||_F / ||ctx64||_F over r's query rows,
+    attn_relfro_combine(*attn_relfro_terms(r)).
     The errors that do not depend on the sign of v are modelled as independent and zero-mean:
       * the fp16 roundings of P and of the output, uniform within half an ulp (variance ulp^2 / 12): P's half ulp taken
         at its upper bound 2^-11 e_j (2^-25 below 2^-14), the output's as the exact half ulp of ctx64;
@@ -294,14 +311,23 @@ def attn_relfro_gate(r) -> torch.Tensor:
     accumulations truncate, a bias rather than noise: attn_acc is added at its worst case.
     Diffuse heads give a gate of ~1.3e-3 (P and the output each ~2^-11 / sqrt(3) relative); ctx scaled by 1 + 2^-9
     (1.95e-3) is outside it."""
+    return attn_relfro_combine(*attn_relfro_terms(r))
+
+
+def attn_relfro_terms(r) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """([B, H] each) the sums over r's query rows and head dimensions of the gate's variance sigma^2 (the model of
+    attn_relfro_gate), of attn_acc^2 and of ctx64^2.  Sums over the row slices of a head give the whole head's."""
     p, v, ctx, l = r["p"], r["v"], r["ctx"], r["l"]
     var = (F16_U ** 2 / 3) * ((p * p) @ (v * v)) + (F16_HALF_QUANTUM ** 2 / 3) * _vsum(r, torch.square) / _safe(l) ** 2
     var = var + half_ulp16(ctx) ** 2 / 3
     w2 = (p * r["delta"]).pow(2)
     var = var + w2 @ (v * v) + 2 * (w2 @ v.abs()) * ctx.abs() + w2.sum(-1, keepdim=True) * ctx * ctx
-    sigma = var.sum((-1, -2)).sqrt()
-    acc = attn_acc(r).pow(2).sum((-1, -2)).sqrt()
-    return (GATE_SIGMAS * sigma + acc) / ctx.pow(2).sum((-1, -2)).sqrt().clamp_min(1e-300)
+    return var.sum((-1, -2)), attn_acc(r).pow(2).sum((-1, -2)), ctx.pow(2).sum((-1, -2))
+
+
+def attn_relfro_combine(var: torch.Tensor, acc2: torch.Tensor, ctx2: torch.Tensor) -> torch.Tensor:
+    """the gate (GATE_SIGMAS sigma + ||attn_acc||_F) / ||ctx64||_F from the sums of attn_relfro_terms"""
+    return (GATE_SIGMAS * var.sqrt() + acc2.sqrt()) / ctx2.sqrt().clamp_min(1e-300)
 
 
 def attn_probs_bound(r) -> torch.Tensor:

@@ -66,28 +66,17 @@ CASES = [
 ]
 
 
-@pytest.mark.parametrize("L,E,H,T,lengths", CASES)
-def test_fused_contact_pass_against_float64(L, E, H, T, lengths):
-    from oracle.weights import make_tokens
-    model = build_model(L, E, H, seed=T + E)
-    tokens = make_tokens(lengths, T, seed=T, n_mask=1).cuda()
-    B = len(lengths)
-    with torch.no_grad():
-        probs, st = fused_stack(model, tokens)
-        # the separate probability kernel (no contact job) must write the same bits
-        _, _, _, attn_sep, _ = model._stack(tokens, need_head_weights=True, return_contacts=False)
-    assert torch.equal(probs, attn_sep["stacked"])
-
-    head = model.contact_head
-    lo, hi = 1, T - 1
+def check_partials(probs, st, keep, lo, hi):
+    """A contact job's row / column partials and accumulator against float64 sums of the maps probs [B,L,H,T,T]
+    (kernel_refs.contact_partials with the job's own weights st["w"]); returns the worst error / bound ratios."""
+    B, L, H, T, _ = probs.shape
     S = hi - lo
-    keep = tokens.ne(head.eos_idx)
-    w = st["w"]
     nt = (T + 127) // 128
     assert st["row"].shape == st["col"].shape == (L, B, H, 4 * nt, S)
     acc_ref = torch.zeros(B, S, S, dtype=torch.float64, device="cuda")
     acc_abs = torch.zeros_like(acc_ref)
     worst = {"row": 0.0, "col": 0.0}
+    w = st["w"]
     for l in range(L):
         acc_l, row, col = kr.contact_partials(probs[:, l], w[l], keep, lo, hi)
         acc_ref += acc_l
@@ -100,26 +89,58 @@ def test_fused_contact_pass_against_float64(L, E, H, T, lengths):
             bound = kr.sum_bound(ref, 32) + 1e-30
             worst[name] = max(worst[name], float((err / bound).max()))
             assert bool((err <= bound).all()), (l, name, float((err - bound).max()))
+        del acc_l, row, col
     # acc: one fma per head in each layer's launch, then one add into the running sum per layer:
     # |err| <= (L * H + L) u sum_l sum_h |w| A
     err = (st["acc"].double() - acc_ref).abs()
     bound = (L * H + L) * U * acc_abs + 1e-30
     acc_ratio = float((err / bound).max())
     assert bool((err <= bound).all())
+    return dict(row_err_over_bound=worst["row"], col_err_over_bound=worst["col"], acc_err_over_bound=acc_ratio)
+
+
+def check_fused(L, E, H, T, lengths):
+    """The fused pass of a 2-layer model on make_tokens(lengths, T) against float64 (check_partials), its
+    probabilities against the separate probability kernel's bit for bit, and its contacts against the head in float64
+    on the same maps (and, up to T = 1024, against the non-fused accumulation kernel).  Returns (model, tokens, probs,
+    ratios)."""
+    from oracle.weights import make_tokens
+    model = build_model(L, E, H, seed=T + E)
+    tokens = make_tokens(lengths, T, seed=T, n_mask=1).cuda()
+    with torch.no_grad():
+        probs, st = fused_stack(model, tokens)
+        # the separate probability kernel (no contact job) must write the same bits
+        _, _, _, attn_sep, _ = model._stack(tokens, need_head_weights=True, return_contacts=False)
+    assert torch.equal(probs, attn_sep["stacked"])
+    del attn_sep
+
+    head = model.contact_head
+    lo, hi = 1, T - 1
+    keep = tokens.ne(head.eos_idx)
+    out = check_partials(probs, st, keep, lo, hi)
 
     # contacts: finish_job (fp32 APC + finalize kernel) against the head in float64 on the same maps; the logits are
     # O(1) sums whose fp32 evaluation is good to ~1e-6, the sigmoid halves that
     with torch.no_grad():
         got = head.finish_job(st)
-        want = head._forward_torch(tokens, probs.double(), w.double(), lo, hi)
-        nonfused = head(tokens, probs)
-    c_abs = float((got.double() - want).abs().max())
-    n_abs = float((nonfused.double() - want).abs().max())
-    report(f"contact_fused L{L}_E{E}_H{H}_T{T}", row_err_over_bound=worst["row"], col_err_over_bound=worst["col"],
-           acc_err_over_bound=acc_ratio, contacts_max_abs=c_abs, nonfused_contacts_max_abs=n_abs)
-    assert c_abs <= 1e-5 and n_abs <= 1e-5
-    # and both paths' contacts against each other
-    torch.testing.assert_close(got, nonfused, atol=1e-5, rtol=0)
+        want = head._forward_torch(tokens, probs.double(), st["w"].double(), lo, hi)
+    out["contacts_max_abs"] = float((got.double() - want).abs().max())
+    if T <= 1024:  # esmb200_contact_accumulate's limit
+        with torch.no_grad():
+            nonfused = head(tokens, probs)
+        out["nonfused_contacts_max_abs"] = float((nonfused.double() - want).abs().max())
+    report(f"contact_fused L{L}_E{E}_H{H}_T{T}", **out)
+    assert out["contacts_max_abs"] <= 1e-5
+    if T <= 1024:
+        assert out["nonfused_contacts_max_abs"] <= 1e-5
+        # and both paths' contacts against each other
+        torch.testing.assert_close(got, nonfused, atol=1e-5, rtol=0)
+    return model, tokens, probs, out
+
+
+@pytest.mark.parametrize("L,E,H,T,lengths", CASES)
+def test_fused_contact_pass_against_float64(L, E, H, T, lengths):
+    check_fused(L, E, H, T, lengths)
 
 
 def test_row_partials_are_per_quarter_not_only_per_row():

@@ -162,7 +162,12 @@ def test_accumulate_is_deterministic_and_checks_its_arguments():
 @pytest.mark.parametrize("C,S,with_bias", [(1, 65, True), (15, 130, False), (16, 64, True), (17, 130, True),
                                            (660, 130, False), (660, 1024, True)])
 def test_finalize_against_float64(C, S, with_bias):
-    B = 2
+    check_finalize(C, S, with_bias)
+
+
+def check_finalize(C, S, with_bias, B=2):
+    """esmb200_contact_finalize on random acc, u and a1 against float64, gated on the logit rebuilt from the output;
+    returns the worst logit error over its bound"""
     g = torch.Generator().manual_seed(C + S)
     acc = torch.randn(B, S, S, generator=g) * 2
     acc[:, :8] *= 20   # logits out to |z| ~ 90 and beyond
@@ -194,3 +199,4 @@ def test_finalize_against_float64(C, S, with_bias):
            probs_max_abs=float((out.double() - sig).abs().max()), z_absmax=float(z.abs().max()))
     assert r <= 1.0
     assert bool(((zgot - zgot.transpose(-1, -2)).abs() <= bound + bound.transpose(-1, -2))[mid & mid.transpose(-1, -2)].all())
+    return r

@@ -221,9 +221,14 @@ def test_qkv_rope_two_slots_per_head():
     with table columns [32, 64).  The standalone entry point has no rope_ld, so this runs one layer and compares its
     attention probabilities with float64 attention on q, k rebuilt from the layer's own fp16 LayerNorm output and
     weights; a wrong slot would rotate half of every head's dimensions by the wrong angles."""
+    check_two_slot_rope(160, 2)
+
+
+def check_two_slot_rope(T, B, label="(via one layer)"):
+    """test_qkv_rope_two_slots_per_head at T positions and B sequences; returns the probabilities' max-abs error"""
     from esm_b200.model import TransformerLayer, rope_tables
     from oracle.weights import make_state_dict
-    E, H, T, B = 256, 2, 160, 2
+    E, H = 256, 2
     d = E // H
     sd = make_state_dict(1, E, H, seed=4)
     layer = TransformerLayer(E, 4 * E, H)
@@ -254,8 +259,9 @@ def test_qkv_rope_two_slots_per_head():
     # q, k are stored as fp16 (the reference rounds them too); what remains is the fp32 accumulation and a rounding
     # of q or k landing on the other side of an fp16 tie (|ds| <~ 2^-11 |q||k|, ~1e-3 here): max-abs 5e-3
     e = float((attn.double() - p).abs().max())
-    report("gemm qkv rope two slots per head (via one layer)", probs_max_abs=e)
+    report(f"gemm qkv rope two slots per head {label}", probs_max_abs=e)
     assert e <= 5e-3
+    return e
 
 
 # ---- GELU -----------------------------------------------------------------------------------------------------------

@@ -37,11 +37,18 @@ def report(name, **kv):
 
 @pytest.mark.parametrize("d,precision", CASES)
 def test_layer_at_head_width_against_float64(d, precision):
+    check_layer(d, precision, 130, [130, 97])
+
+
+def check_layer(d, precision, T, lengths, gates=None):
+    """One layer of head width d (SHAPES) on B = len(lengths) sequences of T positions, sequence b padded from
+    lengths[b] on, against layer64; held to `gates` (default GATES[precision]).  Returns (update rel-Fro, probs
+    max-abs)."""
     from esm_b200.model import TransformerLayer
     from oracle.weights import make_state_dict
     E, H = SHAPES[d]
     assert E // H == d
-    T, B = 130, 2
+    B = len(lengths)
     sd = make_state_dict(1, E, H, seed=d)
     layer = TransformerLayer(E, 4 * E, H)
     layer.load_state_dict({k[len("layers.0."):]: v for k, v in sd.items() if k.startswith("layers.0.")}, strict=True)
@@ -49,7 +56,8 @@ def test_layer_at_head_width_against_float64(d, precision):
     layer.precision = precision
     x = torch.randn(T, B, E, generator=torch.Generator().manual_seed(d + 1))
     pad = torch.zeros(B, T, dtype=torch.bool)
-    pad[1, 97:] = True
+    for b, n in enumerate(lengths):
+        pad[b, n:] = True
     with torch.no_grad():
         out, attn = layer(x.cuda(), self_attn_padding_mask=pad.cuda(), need_head_weights=True)  # (T,B,E), (H,B,T,T)
     torch.cuda.synchronize()
@@ -61,9 +69,10 @@ def test_layer_at_head_width_against_float64(d, precision):
     r = float((d_got - d_ref).norm() / d_ref.norm())
     pa = float((attn.transpose(0, 1).double().cpu() - p).abs()[keep[:, None, :, None].expand_as(p)].max())
     report(f"layer head width d={d} E={E} H={H} precision={precision} T={T}", delta_rel_fro=r, probs_max_abs=pa)
-    gate_r, gate_p = GATES[precision]
+    gate_r, gate_p = gates or GATES[precision]
     assert r <= gate_r and pa <= gate_p
     layer.release()
+    return r, pa
 
 
 @pytest.mark.parametrize("E,H,precision,message", [

@@ -6,7 +6,9 @@
     own modules;
   * the erf-GELU bound holds for an fp32 restatement of the epilogue's formula;
   * the fp16 attention bounds hold for a float64 emulation of the kernels' arithmetic, are not vacuous, and refuse the
-    same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9;
+    same emulation with a padded key counted, a block's O rescale skipped or ctx scaled by 1 + 2^-9; the reference
+    over slices of query rows equals the whole-head reference bit for bit; the bounds hold with up to 64 key blocks
+    (T = 4096 and 8192) and refuse the O rescale skipped from the 9th block on;
   * the tied row attention's stage and end-to-end bounds hold for a float64 emulation of its three kernels in fp16 and
     fp32x3, and refuse P x (1 + 2^-13), ctx x (1 + 2^-9), an alignment row's slab dropped from the logits, the split
     slab's q_lo k_hi pass dropped, and V read from the next alignment row;
@@ -232,27 +234,28 @@ def _chop(t):  # round toward zero to fp32: the tensor core's accumulation
     return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f).double()
 
 
-def _emulate_attention(q, k, v, padded, block, count_key=None, skip_rescale=None):
-    """float64 emulation of the fp16 attention kernels' arithmetic on one head: q, k, v [T, D] fp16, padded [T] bool.
-    Logits in fp32 truncating k16 steps; per `block`-key block the exact running maximum,
-    e = 2^(fp32(s log2e - m log2e)) (correctly rounded: ex2.approx's own error is not emulated),
+def _emulate_attention(q, k, v, padded, block, count_key=None, skip_rescale=None, skip_rescale_from=None):
+    """float64 emulation of the fp16 attention kernels' arithmetic on one head: q [Tq, D] (any Tq of the head's query
+    rows), k, v [T, D] fp16, padded [T] bool.  Logits in fp32 truncating k16 steps; per `block`-key block the exact
+    running maximum, e = 2^(fp32(s log2e - m log2e)) (correctly rounded: ex2.approx's own error is not emulated),
     l = fp32(alpha l + fp32 sum e), P = fp16(e), O = fp32(alpha O) + P V in truncating k16 steps;
     ctx = fp16(O * fp32(1 / l)).  Returns ctx, the saved row max and row sum, and the probability kernel's output from
     the same logits.  Faults: count_key (a padded key index counted as attendable), skip_rescale (a block index whose O
-    rescale is left out)."""
-    T, D = q.shape
+    rescale is left out), skip_rescale_from (the O rescale left out from this block index on)."""
+    Tq, D = q.shape
+    T = k.shape[0]
     live = ~padded
     if count_key is not None:
         live = live.clone()
         live[count_key] = True
     kvlen = int(torch.nonzero(live).max()) + 1 if bool(live.any()) else 0
-    s = torch.zeros(T, T, dtype=torch.float64)
+    s = torch.zeros(Tq, T, dtype=torch.float64)
     for d0 in range(0, D, 16):
         s = _chop(s + q[:, d0:d0 + 16].double() @ k[:, d0:d0 + 16].double().t())
     s = s.masked_fill(~live[None, :], float("-inf"))
-    m = torch.full((T, 1), float("-inf"), dtype=torch.float64)
-    l = torch.zeros(T, 1, dtype=torch.float64)
-    o = torch.zeros(T, D, dtype=torch.float64)
+    m = torch.full((Tq, 1), float("-inf"), dtype=torch.float64)
+    l = torch.zeros(Tq, 1, dtype=torch.float64)
+    o = torch.zeros(Tq, D, dtype=torch.float64)
     for j0 in range(0, kvlen, block):
         sb = s[:, j0:j0 + block]
         mn = torch.maximum(m, sb.amax(-1, keepdim=True))
@@ -261,7 +264,7 @@ def _emulate_attention(q, k, v, padded, block, count_key=None, skip_rescale=None
         e = _f32(torch.exp2(_f32(sb * LOG2E32 + ref)))
         m = mn
         l = _f32(_f32(l * alpha) + _f32(e.float().sum(-1, keepdim=True)))
-        if j0 // block != skip_rescale:
+        if j0 // block != skip_rescale and (skip_rescale_from is None or j0 // block < skip_rescale_from):
             o = _f32(o * alpha)
         ph = e.half().double()
         vb = v[j0:j0 + block].double()
@@ -350,6 +353,99 @@ def test_attention_bounds_refuse_emulated_faults(D, block):
     dev = (up.sum(-1) - 1).abs()
     summed = float((dev / kr.attn_probs_bound(r)[0, 0].sum(-1)).max())
     assert float((dev / kr.attn_rowsum_bound(r)[0, 0]).max()) > 1.3 * summed  # tighter than the summed element bounds
+
+
+# ---- long heads: row slices and up to 64 key blocks ------------------------------------------------------------------
+def test_row_slices_equal_the_whole_head():
+    """attention64_rows gives every row-indexed value and bound of attention64 on the whole head bit for bit (rows
+    are independent), the same nblk, and the whole head's gate from the slices' summed terms; slices of 37 rows leave
+    a short last one, and one sequence is all padding."""
+    g = torch.Generator().manual_seed(11)
+    B, H, T, D = 3, 2, 300, 64
+    q, k, v = (torch.randn(B, H, T, D, generator=g).half() for _ in range(3))
+    padded = torch.zeros(B, T, dtype=torch.bool)
+    padded[1, 171:] = True
+    padded[2] = True
+    whole = kr.attention64(q, k, v, padded, 128)
+    l_at = torch.exp(whole["s"].masked_fill(whole["km"], float("-inf")) - whole["m"]).sum(-1)
+    bounds = {"ctx": kr.attn_ctx_bound(whole), "probs": kr.attn_probs_bound(whole),
+              "rowsum": kr.attn_rowsum_bound(whole), "max": kr.attn_max_bound(whole),
+              "sum": kr.attn_sum_bound(whole, l_at)}
+    terms = [torch.zeros(B, H, dtype=torch.float64) for _ in range(3)]
+    starts = []
+    for i0, r in kr.attention64_rows(q, k, v, padded, 128, max_elems=B * H * T * 37):
+        n = r["q"].shape[-2]
+        starts.append((i0, n))
+        rows = slice(i0, i0 + n)
+        for name in ("s", "m", "l", "p", "ctx", "lerr", "delta"):
+            assert torch.equal(r[name], whole[name][:, :, rows]), name
+        assert torch.equal(r["nblk"], whole["nblk"])
+        la = torch.exp(r["s"].masked_fill(r["km"], float("-inf")) - r["m"]).sum(-1)
+        got = {"ctx": kr.attn_ctx_bound(r), "probs": kr.attn_probs_bound(r), "rowsum": kr.attn_rowsum_bound(r),
+               "max": kr.attn_max_bound(r), "sum": kr.attn_sum_bound(r, la)}
+        for name, b in got.items():
+            assert torch.equal(b, bounds[name][:, :, rows]), name
+        for acc, t in zip(terms, kr.attn_relfro_terms(r)):
+            acc += t
+    assert starts[0] == (0, 37) and starts[-1] == (296, 4) and len(starts) == 9
+    torch.testing.assert_close(kr.attn_relfro_combine(*terms), kr.attn_relfro_gate(whole), rtol=1e-13, atol=0)
+    assert [int(x) for x in whole["nblk"].flatten()] == [3, 2, 0]
+
+
+def _rising_inputs(T, D, seed):
+    """fp16 q, k, v [T, D] whose logits rise by ~3.2 every 64 keys (tests/test_gpu_attention_f16.py rising_qkv):
+    every 64-key step of every row raises the running maximum, so every block rescales O and l"""
+    g = torch.Generator().manual_seed(seed)
+    u = torch.randn(D, generator=g, dtype=torch.float64)
+    u = u / u.norm() * 8.0 ** 0.5
+    blk = (torch.arange(T, dtype=torch.float64) // 64)[:, None]
+    q = u + 0.1 * torch.randn(T, D, generator=g, dtype=torch.float64)
+    k = u * (0.4 * blk) + 0.3 * torch.randn(T, D, generator=g, dtype=torch.float64)
+    v = torch.randn(T, D, generator=g, dtype=torch.float64)
+    return q.half(), k.half(), v.half()
+
+
+def _long_inputs(T, D, std, rise, seed):
+    """(q rows, k, v, padded): 96 query rows spread over the head (rows are independent, so they stand for all T),
+    keys padded at the tail and in one interior run"""
+    q, k, v = _rising_inputs(T, D, seed) if rise else _attention_inputs(T, D, std, seed)
+    padded = torch.zeros(T, dtype=torch.bool)
+    padded[T - 37:] = True
+    padded[T // 3:T // 3 + 5] = True
+    return q[torch.arange(0, T, T // 96)], k, v, padded
+
+
+LONG_EMU_CASES = [(64, 128, 8192, 1.0, False), (64, 128, 8192, 8.0, False), (64, 128, 4096, 2.0, True),
+                  (128, 64, 4096, 1.0, False), (128, 64, 4096, 8.0, False), (128, 64, 4096, 2.0, True)]
+
+
+@pytest.mark.parametrize("D,block,T,std,rise", LONG_EMU_CASES)
+def test_attention_bounds_cover_an_emulated_kernel_to_64_blocks(D, block, T, std, rise):
+    """nblk up to 64 (the wg kernel at T = 8192, the two-slot kernel at 4096): the bounds' nblk terms still cover the
+    emulated kernel.  They are worst cases linear in nblk, so the worst ratio of a diffuse head falls with T (0.05 for
+    ctx and the gate at 64 blocks of 128 keys, against 0.1 .. 0.3 at T <= 1024); 0.03 keeps them from going vacuous."""
+    q, k, v, padded = _long_inputs(T, D, std, rise, seed=T + D + int(std))
+    ctx, mx, sm, probs = _emulate_attention(q, k, v, padded, block)
+    r = kr.attention64(q[None, None], k[None, None], v[None, None], padded[None], block)
+    assert int(r["nblk"]) == (T - 37 + block - 1) // block
+    out = _ratios(q, k, v, padded, block, ctx, mx, sm, probs)
+    assert max(out.values()) <= 1.0, out
+    if std == 1.0:
+        assert out["ctx"] >= 0.03 and out["gate"] >= 0.03, out
+
+
+@pytest.mark.parametrize("D,block,T", [(64, 128, 4096), (128, 64, 2048)])
+def test_attention_bounds_refuse_a_rescale_skipped_after_block_8(D, block, T):
+    """The O rescale left out from the 9th key block on (a kernel that only rescales the first 8 blocks, all that
+    T <= 1024 walks at 128-key blocks) leaves the element bound and the gate on diffuse and on rising logits, while
+    the correct emulation of the same rows stays inside"""
+    for std, rise in ((1.0, False), (2.0, True)):
+        q, k, v, padded = _long_inputs(T, D, std, rise, seed=3 * T + D)
+        good, _, _, _ = _emulate_attention(q, k, v, padded, block)
+        assert max(_ratios(q, k, v, padded, block, good).values()) <= 1.0
+        bad, _, _, _ = _emulate_attention(q, k, v, padded, block, skip_rescale_from=8)
+        out = _ratios(q, k, v, padded, block, bad)
+        assert out["ctx"] > 1.0 and out["gate"] > 1.0, (std, rise, out)
 
 
 # ---- tied row attention ---------------------------------------------------------------------------------------------
