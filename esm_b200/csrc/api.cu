@@ -783,7 +783,9 @@ int esmb200_layer_create(const esmb200_layer_weights* w, void* stream, esmb200_l
   memset(static_cast<void*>(L), 0, sizeof(*L));
   const int Ea = 64 * slots * H;
   L->E = E; L->H = H; L->F = has_ffn ? F : 0; L->d = d; L->slots = slots; L->Ea = Ea; L->eps = w->ln_eps;
-  L->q_scale = 1.0f / sqrtf((float)d);
+  // the reference's head_dim ** -0.5 is a Python double, rounded to fp32 by `q *= scaling`; 1.0f / sqrtf(d) in fp32
+  // is one ulp off at d = 6, 18, 24 (esm2_t12_35M), 28, 34, 58, 68, 72, ... (DESIGN.md section 4)
+  L->q_scale = (float)pow((double)d, -0.5);
   L->ln1_w = w->ln1_weight; L->ln1_b = w->ln1_bias; L->ln2_w = w->ln2_weight; L->ln2_b = w->ln2_bias;
   L->out_b = w->out_bias; L->fc1_b = w->fc1_bias; L->fc2_b = w->fc2_bias;
   L->split = split;
@@ -1410,7 +1412,9 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   if (rc) return rc;
   rc = run_key_bits(col_pad_mask, ws.as, B * C, R, st);  // column attention: B*C sequences of R keys
   if (rc) return rc;
-  const float row_scale = 0.125f / sqrtf((float)R);  // axial_attention.py:36-38
+  // axial_attention.py:36-38: scaling / math.sqrt(num_rows) in double, rounded to fp32 by `q *= ...` (0.125f /
+  // sqrtf(R) in fp32 is one ulp off at 242 of the depths R = 1 ... 1024, the first R = 6, 7 and 17)
+  const float row_scale = (float)(pow(64.0, -0.5) / sqrt((double)R));
   for (int i = 0; i < n_layers; ++i) {
     // tied row attention (modules.py:202-207; axial_attention.py:71-130)
     rc = attention_block(row_layers[i], row_layers[i]->tm, x, M, 1, nullptr, nullptr, row_scale, ws, am, st, [&]() -> int {

@@ -110,7 +110,7 @@ def acc_bound(A, W, per_block=2.0 ** -11):
 
 
 # ---- checkers of e4m3 outputs against a float64 reference ------------------------------------------------------------
-def check_codes(q8, s, y, ybnd):
+def check_codes(q8, s, y, ybnd, device="cpu"):
     """An e4m3 output q8 [R, N] with its scales s [ceil(N/128), R] (one per row and 128 columns) against the float64
     values y [R, N] it quantises, where the kernel computed each value within ybnd [R, N] of y.  Returns a dict:
       bad_scale  scales that differ from the reference's by other than one power of two, or whose block's float64 amax
@@ -122,8 +122,8 @@ def check_codes(q8, s, y, ybnd):
                  round a value within the bound of y;
       flips      code mismatches under an equal scale (all of them boundary flips when bad_code is 0);
       scale_flips, n.
-    All on the CPU."""
-    q8, s, y, ybnd = q8.cpu(), s.cpu().float(), y.cpu().double(), ybnd.cpu().double()
+    On the CPU, or on `device`."""
+    q8, s, y, ybnd = q8.to(device), s.to(device).float(), y.to(device).double(), ybnd.to(device).double()
     R, N = y.shape
     kb = -(-N // 128)
     qr, sr = quantize(y.float(), 1)
@@ -136,7 +136,7 @@ def check_codes(q8, s, y, ybnd):
     bad_code = (y - deq).abs() > half_ulp * (1 + 1e-6) + ybnd
     mism = q8.view(torch.uint8) != qr.view(torch.uint8)
     flips = mism & ~sflip_full
-    pad = torch.zeros(R, kb * 128, dtype=torch.float64)
+    pad = torch.zeros(R, kb * 128, dtype=torch.float64, device=y.device)
     pad[:, :N] = y.abs()
     am = pad.view(R, kb, 128).amax(-1).t()
     pad[:, :N] = ybnd

@@ -6,6 +6,8 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
     quarter of each 128-wide tile;
   * gemm_launches: every (epilogue, N, K) GEMM a model's forward launches (api.cu attention_block / ffn_block, the LM
     head of model.py RobertaLMHead.forward_native, the MSA Transformer's layer in msa.py);
+  * gemm_exact / gemm_acc_bound / f16_bound / residual_bound / qkv_ref / qkv_bound: the fp16 GEMM's float64 reference
+    and the bounds of its epilogues (residual add, q scale and RoPE);
   * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf);
   * split16 / join64 / split_rep_bound / split_acc_bound / FP32X3_MODELS: the fp32x3 precision's hi | lo operand pairs,
     the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs;
@@ -97,6 +99,56 @@ def contacts_from_partials(acc: torch.Tensor, row: torch.Tensor, col: torch.Tens
 def sum_bound(terms_abs: torch.Tensor, n: int) -> torch.Tensor:
     """Bound of an n-term fp32 recursive sum (any order) of values with absolute sum `terms_abs`: (n - 1) u sum|x|."""
     return (n - 1) * U32 * terms_abs
+
+
+# ---- fp16 GEMM epilogues (csrc/gemm2.cuh) ---------------------------------------------------------------------------
+def gemm_exact(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(a w^T + bias in float64, sum_k |a_k w_k|) on the kernel's own operands"""
+    ad, wd = a.double(), w.double()
+    return ad @ wd.t() + bias.double(), ad.abs() @ wd.abs().t()
+
+
+def gemm_acc_bound(absdot: torch.Tensor, K: int, y: torch.Tensor) -> torch.Tensor:
+    """|out - y| of the fp16 GEMM before any epilogue function: the tensor core sums each k16 step's exact products into
+    the fp32 accumulator with truncation, (K/16 + 4) 2^-22 sum_k |a_k w_k| (one ulp per step, doubled for slack), plus
+    the bias add and the fp32 result (2 u |y|)."""
+    return (K / 16 + 4) * 2.0 ** -22 * absdot + 2 * U32 * y.abs()
+
+
+def f16_bound(y: torch.Tensor) -> torch.Tensor:
+    """rounding of a finite fp32 value to fp16: half an ulp, 2^-11 relative, 2^-25 absolute below the normal range."""
+    return 2.0 ** -11 * y.abs() + 2.0 ** -25
+
+
+def residual_bound(acc: torch.Tensor, want: torch.Tensor) -> torch.Tensor:
+    """|x' - want| for the residual epilogue x' = x + y (EPI_BIAS_RESIDUAL, the fp32 add in the L2), want = x + y64:
+    the update's own bound `acc` (gemm_acc_bound, split_acc_bound or fp8_refs.acc_bound) and the fp32 add (u |want|)."""
+    return acc + U32 * want.abs()
+
+
+def qkv_ref(a, w, bias, q_scale, E, T=None, cos=None, sin=None):
+    """[q*scale | k | v] in float64 (the bias added before the scale), with rotate-half RoPE on every 64-column group
+    of q and k: pair (c, c + 32) rotated by table column c of a [T, 32] table (row r at position r % T).  Returns
+    (y, absdot) with absdot the matching sum of |products| (rotated pairs: both members' sums, |cos|, |sin| <= 1)."""
+    y, absdot = gemm_exact(a, w, bias)
+    y[:, :E] *= q_scale
+    absdot[:, :E] *= q_scale
+    if cos is not None:
+        M = y.shape[0]
+        t = torch.arange(M, device=y.device) % T
+        c, s = cos.double()[t][:, :32], sin.double()[t][:, :32]
+        for g0 in range(0, 2 * E, 64):
+            x1, x2 = y[:, g0:g0 + 32].clone(), y[:, g0 + 32:g0 + 64].clone()
+            y[:, g0:g0 + 32], y[:, g0 + 32:g0 + 64] = x1 * c - x2 * s, x2 * c + x1 * s
+            d1, d2 = absdot[:, g0:g0 + 32].clone(), absdot[:, g0 + 32:g0 + 64].clone()
+            absdot[:, g0:g0 + 32] = absdot[:, g0 + 32:g0 + 64] = d1 + d2
+    return y, absdot
+
+
+def qkv_bound(y: torch.Tensor, absdot: torch.Tensor, K: int) -> torch.Tensor:
+    """|out - y| of the fp16 QKV epilogue: gemm_acc_bound, the q scale and the rotation's products and add (4 u |y|),
+    and the fp16 output"""
+    return gemm_acc_bound(absdot, K, y) + 4 * U32 * y.abs() + f16_bound(y)
 
 
 # ---- GEMM launch table ----------------------------------------------------------------------------------------------

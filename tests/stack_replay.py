@@ -1,0 +1,567 @@
+"""Layer-by-layer replay of the library's layer stacks through the single-kernel C-ABI entry points, with every
+intermediate kept, and the float64 checks of each stage on its own inputs (tests/test_gpu_stack_stages.py).
+
+The replay packs the weights itself from the module parameters (`.half()`, esmb200_convert_split hi | lo, [Wq;Wk;Wv]
+quantised by esmb200_quantize_fp8) and takes every parameter from the reference's definition rather than from the
+library: the module's LayerNorm eps, the q scale fp32(d ** -0.5) (fp32(d ** -0.5 / sqrt(R)) for the MSA row attention),
+and the rotary tables of rotary_embedding.py:47-61.  A stack that packs, scales or wires one of them differently gives
+other bits than the replay.
+
+  * pack_esm / replay_esm: one ESM-2 / ESM-1b layer in precision 0 (fp16), 1 (fp32x3) or 2 (fp8), head_dim 64;
+  * check_esm_stages / check_fp8_stages: each stage of one replayed layer against float64, worst ratios per stage;
+  * pack_axial / replay_axial / check_axial_stages: one MSA Transformer AxialTransformerLayer in fp16 or fp32x3, and its
+    stages against float64;
+  * packed_arena: the bytes esmb200_layer_offload writes (api.cu packed_layout) at any head width.
+"""
+from __future__ import annotations
+
+import ctypes
+import math
+from typing import Dict, Optional
+
+import numpy as np
+import torch
+
+import fp8_refs
+import kernel_refs as kr
+
+
+def P(t: Optional[torch.Tensor]):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def S():
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def lib():
+    from esm_b200 import _lib
+    return _lib.load()
+
+
+def check(rc):
+    from esm_b200 import _lib
+    _lib.check(rc)
+
+
+def q_scale(d: int, rows: int = 0) -> float:
+    """The reference's q scale as the fp32 value `q *= scaling` multiplies by: head_dim ** -0.5 (multihead_attention.py
+    :100), or for the MSA row attention head_dim ** -0.5 / math.sqrt(num_rows) (axial_attention.py:36-38), both Python
+    doubles rounded to fp32."""
+    s = d ** -0.5
+    if rows:
+        s = s / math.sqrt(rows)
+    return float(np.float32(s))
+
+
+def rope_ref(inv_freq: torch.Tensor, T: int):
+    """rotary_embedding.py:47-61 on the device: cos / sin of t * inv_freq, the first d/2 columns of the reference's
+    duplicated table ([T, 32] for d = 64)"""
+    t = torch.arange(T, device=inv_freq.device).type_as(inv_freq)
+    freqs = torch.einsum("i,j->ij", t, inv_freq)
+    emb = torch.cat((freqs, freqs), dim=-1)
+    h = inv_freq.numel()
+    return emb.cos()[:, :h].contiguous(), emb.sin()[:, :h].contiguous()
+
+
+def split_dev(w: torch.Tensor) -> torch.Tensor:
+    """esmb200_convert_split: fp32 [N, K] -> fp16 [N, 2K] hi | lo"""
+    w = w.detach().float().contiguous()
+    N, K = w.shape
+    out = torch.empty(N, 2 * K, dtype=torch.float16, device=w.device)
+    check(lib().esmb200_convert_split(P(w), P(out), N, K, S()))
+    return out
+
+
+def _pack_matrix(w: torch.Tensor, precision: int):
+    if precision == 1:
+        return split_dev(w)
+    return w.detach().half().contiguous()
+
+
+# ---- ESM-2 / ESM-1b layer -------------------------------------------------------------------------------------------
+def pack_esm(layer, precision: int) -> Dict:
+    """The GEMM operands of one TransformerLayer (head_dim 64: the head slots are the identity)."""
+    a = layer.self_attn
+    wqkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight]).detach().float().contiguous()
+    pk = dict(b_qkv=torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]).detach().float().contiguous(),
+              w_out=_pack_matrix(a.out_proj.weight, 1 if precision == 1 else 0))
+    if precision == 2:
+        pk["q_qkv"], pk["s_qkv"] = fp8_refs.quantize_dev(wqkv, 128)
+        pk["q_fc1"], pk["s_fc1"] = fp8_refs.quantize_dev(layer.fc1.weight.detach().float().contiguous(), 128)
+        pk["q_fc2"], pk["s_fc2"] = fp8_refs.quantize_dev(layer.fc2.weight.detach().float().contiguous(), 128)
+    else:
+        pk["w_qkv"] = _pack_matrix(wqkv, precision)
+        pk["w_fc1"] = _pack_matrix(layer.fc1.weight, precision)
+        pk["w_fc2"] = _pack_matrix(layer.fc2.weight, precision)
+    return pk
+
+
+def _ln(x, ln, out, precision, scales=None):
+    M, E = x.shape
+    L = lib()
+    if precision == 2:
+        check(L.esmb200_layernorm_fp8(P(x), P(ln.weight), P(ln.bias), P(out), P(scales), M, E, ln.eps, S()))
+    else:
+        fn = L.esmb200_layernorm_split if precision == 1 else L.esmb200_layernorm_f16
+        check(fn(P(x), P(ln.weight), P(ln.bias), P(out), M, E, ln.eps, S()))
+
+
+def _gemm(epi, a, w, bias, out, M, N, K, precision, cos=None, sin=None, T=0, E=0):
+    fn = lib().esmb200_gemm_split if precision == 1 else lib().esmb200_gemm_f16
+    check(fn(epi, P(a), P(w), P(bias), P(out), M, N, K, P(cos), P(sin), T, E, S()))
+
+
+def _gemm8(epi, a, sa, w, sw, bias, out, out_s, M, N, K, cos=None, sin=None, T=0, E=0):
+    check(lib().esmb200_gemm_fp8(epi, P(a), P(sa), P(w), P(sw), P(bias), P(out), P(out_s), M, N, K, P(cos), P(sin), T, E,
+                                 S()))
+
+
+def replay_esm(layer, pk: Dict, x: torch.Tensor, pad8: torch.Tensor, B: int, T: int, cos, sin, precision: int,
+               probs: Optional[torch.Tensor] = None) -> Dict:
+    """One layer in place on x fp32 [B*T, E], kernel by kernel as api.cu attention_block / ffn_block launch them.
+    cos = sin = None: no rotary embedding (ESM-1b).  probs: fp32 [B,H,T,T] to fill, or None.  Returns the stages:
+    x0 (input), xn1, qkv, ctx, x1 (after out_proj), xn2, h, x (output), the fp8 scales xs1 / xs2 / hs."""
+    E, H, F = layer.embed_dim, layer.attention_heads, layer.ffn_embed_dim
+    M = B * T
+    d = E // H
+    pf = 2 if precision == 1 else 1
+    dev = x.device
+    L = lib()
+    st = dict(x0=x.clone())
+    qs = q_scale(d)
+    if precision == 2:
+        xn = torch.empty(M, E, dtype=torch.uint8, device=dev)
+        xs = torch.empty((E + 127) // 128, M, device=dev)
+    else:
+        xn, xs = torch.empty(M, pf * E, dtype=torch.float16, device=dev), None
+    _ln(x, layer.self_attn_layer_norm, xn, precision, xs)
+    st.update(xn1=xn.clone(), xs1=None if xs is None else xs.clone())
+    qkv = torch.empty(M, pf * 3 * E, dtype=torch.float16, device=dev)
+    if precision == 2:
+        # esmb200_gemm_fp8 takes rope tables only; cos = 1, sin = 0 rotates by nothing (x1 * 1 - x2 * 0 == x1)
+        assert qs == 0.125, "esmb200_gemm_fp8 scales q by 0.125"
+        c, s_ = (cos, sin) if cos is not None else (torch.ones(T, 32, device=dev), torch.zeros(T, 32, device=dev))
+        _gemm8(kr.EPI_QKV_ROPE, xn, xs, pk["q_qkv"], pk["s_qkv"], pk["b_qkv"], qkv, None, M, 3 * E, E, c, s_, T, E)
+    elif precision == 1 and cos is not None:
+        assert qs == 0.125, "esmb200_gemm_split scales q by 0.125"
+        _gemm(kr.EPI_QKV_ROPE, xn, pk["w_qkv"], pk["b_qkv"], qkv, M, 3 * E, E, 1, cos, sin, T, E)
+    elif precision == 1:
+        check(L.esmb200_gemm_qkv_split(P(xn), P(pk["w_qkv"]), P(pk["b_qkv"]), P(qkv), M, E, qs, S()))
+    else:
+        check(L.esmb200_gemm_qkv_f16(P(xn), P(pk["w_qkv"]), P(pk["b_qkv"]), P(qkv), M, E, qs, P(cos), P(sin),
+                                     T if cos is not None else 0, S()))
+    st["qkv"] = qkv.clone()
+    ctx = torch.empty(M, pf * E, dtype=torch.float16, device=dev)
+    scratch = torch.empty(L.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
+    att = L.esmb200_attention_split if precision == 1 else L.esmb200_attention
+    check(att(P(qkv), P(pad8), P(ctx), P(probs), B, T, H, P(scratch), S()))
+    st["ctx"] = ctx.clone()
+    _gemm(kr.EPI_BIAS_RESIDUAL, ctx, pk["w_out"], layer.self_attn.out_proj.bias, x, M, E, E, 1 if precision == 1 else 0)
+    st["x1"] = x.clone()
+    _ln(x, layer.final_layer_norm, xn, precision, xs)
+    st.update(xn2=xn.clone(), xs2=None if xs is None else xs.clone())
+    if precision == 2:
+        h = torch.empty(M, F, dtype=torch.uint8, device=dev)
+        hs = torch.empty(F // 128, M, device=dev)
+        _gemm8(fp8_refs_epi_gelu(), xn, xs, pk["q_fc1"], pk["s_fc1"], layer.fc1.bias, h, hs, M, F, E)
+        st.update(h=h.clone(), hs=hs.clone())
+        _gemm8(kr.EPI_BIAS_RESIDUAL, h, hs, pk["q_fc2"], pk["s_fc2"], layer.fc2.bias, x, None, M, E, F)
+    else:
+        h = torch.empty(M, pf * F, dtype=torch.float16, device=dev)
+        _gemm(kr.EPI_BIAS_GELU, xn, pk["w_fc1"], layer.fc1.bias, h, M, F, E, precision)
+        st["h"] = h.clone()
+        _gemm(kr.EPI_BIAS_RESIDUAL, h, pk["w_fc2"], layer.fc2.bias, x, M, E, F, precision)
+    st["x"] = x
+    return st
+
+
+def fp8_refs_epi_gelu() -> int:
+    from esm_b200 import _lib
+    return _lib.EPI_GELU_FP8
+
+
+# ---- float64 stages -------------------------------------------------------------------------------------------------
+def _worst(worst: Dict, name: str, ratio: float):
+    assert ratio == ratio, f"NaN ratio in stage {name}"
+    worst[name] = max(worst.get(name, 0.0), ratio)
+
+
+def _ratio(err: torch.Tensor, bound: torch.Tensor) -> float:
+    assert not bool(err.isnan().any()), "NaN in a stage"
+    r = float((err / bound).max())
+    assert r == r, "NaN ratio in a stage (a zero bound at a zero error)"
+    return r
+
+
+def _ln_stage(x, ln, got, split):
+    """(error, bound) of a LayerNorm -> fp16 (or hi | lo) output against float64 on the kernel's fp32 input"""
+    want, b = _ln_want(x, ln)
+    E = x.shape[-1]
+    if split:
+        g = kr.join64(got[:, :E], got[:, E:])
+        b = b + kr.split_rep_bound(want.abs() + b)
+    else:
+        g = got.double()
+        b = b + kr.f16_bound(want.abs() + b)
+    return (g - want).abs(), b
+
+
+def _ln_want(x, ln):
+    """(float64 LayerNorm of the kernel's fp32 input, the fp32 kernel's bound ln_tol at the row's |mean|/std)"""
+    E = x.shape[-1]
+    xd = x.double()
+    want = kr.layer_norm64(xd, ln.weight, ln.bias, ln.eps)
+    cond = (xd.mean(-1, keepdim=True).abs() / xd.std(-1, unbiased=False, keepdim=True).clamp_min(1e-30))
+    return want, kr.ln_tol(E, cond) * kr.ln_scale(want, ln.weight, ln.bias)
+
+
+def ln_stage(worst, name, x, ln, got, split):
+    err, b = _ln_stage(x, ln, got, split)
+    _worst(worst, name, _ratio(err, b))
+
+
+def _heads(t: torch.Tensor, B: int, T: int, H: int, i: int) -> torch.Tensor:
+    """section i (0 q, 1 k, 2 v) of [B*T, 3E] as [B, H, T, 64]"""
+    E = 64 * H
+    return t[:, i * E:(i + 1) * E].reshape(B, T, H, 64).transpose(1, 2)
+
+
+def qkv_stage(worst, xn, w_qkv, bqkv, qkv, E, qs, T, cos, sin, split, zero_rows=None):
+    """the QKV projection (q scale, RoPE when cos is given) on the kernel's own operands; zero_rows [M] bool: rows whose
+    q the caller zeroed (the MSA row attention's padded tokens)"""
+    if split:
+        from test_gpu_gemm_split import split_qkv_bound
+        xh, xl, wh, wl = xn[:, :E], xn[:, E:], w_qkv[:, :E], w_qkv[:, E:]
+        aj, wj = kr.join64(xh, xl), kr.join64(wh, wl)
+        y_pre = aj @ wj.t() + bqkv.double()
+        y_pre[:, :E] *= qs
+        y, _ = kr.qkv_ref(aj, wj, bqkv, qs, E, T, cos, sin)
+        b = split_qkv_bound(xh, xl, wh, wl, E, y_pre, E, qs, cos) + kr.split_rep_bound(y)
+        got = kr.join64(qkv[:, :3 * E], qkv[:, 3 * E:])
+    else:
+        y, absdot = kr.qkv_ref(xn, w_qkv, bqkv, qs, E, T, cos, sin)
+        b = kr.qkv_bound(y, absdot, E)
+        got = qkv.double()
+    if zero_rows is not None:
+        y[zero_rows, :E] = 0.0
+    _worst(worst, "qkv", _ratio((got - y).abs(), b))
+
+
+def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,), prefix=""):
+    """fp16 attention on the kernel's q, k, v (qkv [B*T, 3E], sequences of T tokens, pad [B, T] bool): ctx element-wise
+    (attn_ctx_bound) and per (sequence, head) rel-Fro (attn_relfro_gate), probabilities and row sums of the valid query
+    rows.  blocks: the key-block sizes the kernel may walk; the bound is the largest over them."""
+    q, k, v = (_heads(qkv, B, T, H, i) for i in range(3))
+    got = _heads(ctx, B, T, H, 0).double()
+    terms = {bl: [0, 0, 0] for bl in blocks}
+    err2 = 0
+    for i0, r0 in kr.attention64_rows(q, k, v, pad, blocks[0]):
+        rs = [r0] + [kr.attention64(q[..., i0:i0 + r0["ctx"].shape[-2], :], k, v, pad, bl) for bl in blocks[1:]]
+        n = r0["ctx"].shape[-2]
+        g = got[..., i0:i0 + n, :]
+        e = (g - r0["ctx"]).abs()
+        _worst(worst, prefix + "ctx", _ratio(e, torch.stack([kr.attn_ctx_bound(r) for r in rs]).amax(0)))
+        for bl, r in zip(blocks, rs):
+            t = kr.attn_relfro_terms(r)
+            terms[bl] = [a + b for a, b in zip(terms[bl], t)]
+        err2 = err2 + e.pow(2).sum((-1, -2))
+        if probs is not None:
+            rows = ~pad.bool()[:, i0:i0 + n]
+            m = rows[:, None, :, None].expand_as(r0["p"])
+            pr = probs[:, :, i0:i0 + n].double()
+            _worst(worst, prefix + "probs", _ratio((pr - r0["p"]).abs()[m], kr.attn_probs_bound(r0)[m]))
+            mr = rows[:, None, :].expand(B, H, n)
+            _worst(worst, prefix + "rowsum", _ratio((pr.sum(-1) - 1).abs()[mr], kr.attn_rowsum_bound(r0)[mr]))
+        del rs, r0
+    gate = torch.stack([kr.attn_relfro_combine(*terms[bl]) for bl in blocks]).amax(0)
+    ctx2 = terms[blocks[0]][2]
+    live = ctx2 > 0  # a sequence of padding only has ctx 0, written as 0 (checked element-wise above)
+    fro = err2.sqrt() / ctx2.sqrt().clamp_min(1e-300)
+    _worst(worst, prefix + "ctx_relfro_gate", float((fro[live] / gate[live]).max()))
+
+
+def attention_stage_split(worst, qkv, ctx, pad, B, T, H, probs=None, prefix=""):
+    """fp32x3 attention on the kernel's q, k, v hi | lo (qkv [B*T, 6E]): the split attention tests' element bound and
+    per-head gate, and the probabilities of the valid query rows"""
+    import test_gpu_attention_split as tas
+    E = 64 * H
+    r = tas.reference(qkv[:, :3 * E], qkv[:, 3 * E:], pad, B, T, H)
+    got = _heads(ctx[:, :E].double(), B, T, H, 0) + _heads(ctx[:, E:].double(), B, T, H, 0)
+    err = (got - r["ctx"]).abs()
+    _worst(worst, prefix + "ctx", _ratio(err, tas.ctx_bound(r)))
+    fro = (err.pow(2).sum((-1, -2)) / r["ctx"].pow(2).sum((-1, -2)).clamp_min(1e-300)).sqrt()
+    _worst(worst, prefix + "ctx_relfro_gate", float((fro / tas.relfro_gate(r)).max()))
+    if probs is not None:
+        m = (~pad.bool())[:, None, :, None].expand_as(r["p"])
+        _worst(worst, prefix + "probs", _ratio((probs.double() - r["p"]).abs()[m], tas.probs_bound(r)[m]))
+
+
+def residual_stage(worst, name, a_op, w_op, bias, x_in, x_out, K, split):
+    """x_out = x_in + a w^T + bias (fp16 or hi | lo operands) within residual_bound"""
+    if split:
+        ah, al, wh, wl = a_op[:, :K], a_op[:, K:], w_op[:, :K], w_op[:, K:]
+        upd = kr.join64(ah, al) @ kr.join64(wh, wl).t() + bias.double()
+        acc = kr.split_acc_bound(ah, al, wh, wl, K, upd)
+    else:
+        upd, absdot = kr.gemm_exact(a_op, w_op, bias)
+        acc = kr.gemm_acc_bound(absdot, K, upd)
+    want = x_in.double() + upd
+    _worst(worst, name, _ratio((x_out.double() - want).abs(), kr.residual_bound(acc, want)))
+
+
+def fc1_stage(worst, xn, w, bias, h, E, F, split):
+    """h = GELU(xn w^T + bias) in fp16 or hi | lo: 1.13 x the GEMM bound (|GELU'| <= 1.13), gelu_bound, output rounding"""
+    if split:
+        ah, al, wh, wl = xn[:, :E], xn[:, E:], w[:, :E], w[:, E:]
+        y = kr.join64(ah, al) @ kr.join64(wh, wl).t() + bias.double()
+        acc = kr.split_acc_bound(ah, al, wh, wl, E, y)
+        got = kr.join64(h[:, :F], h[:, F:])
+        want = kr.gelu64(y)
+        b = 1.13 * acc + kr.gelu_bound(y) + kr.split_rep_bound(want.abs() + 1.13 * acc)
+    else:
+        y, absdot = kr.gemm_exact(xn, w, bias)
+        acc = kr.gemm_acc_bound(absdot, E, y)
+        got = h.double()
+        want = kr.gelu64(y)
+        b = 1.13 * acc + kr.gelu_bound(y) + kr.f16_bound(want.abs() + 1.13 * acc)
+    _worst(worst, "fc1", _ratio((got - want).abs(), b))
+
+
+def check_esm_stages(layer, pk: Dict, st: Dict, pad: torch.Tensor, B: int, T: int, cos, precision: int, worst: Dict,
+                     probs: Optional[torch.Tensor] = None, sin=None):
+    """Every stage of one replayed layer against float64 on that stage's own inputs; the largest error / bound of each
+    stage is folded into `worst`.  fp16 and fp32x3 (fp8: check_fp8_stages)."""
+    E, H, F = layer.embed_dim, layer.attention_heads, layer.ffn_embed_dim
+    split = precision == 1
+    a = layer.self_attn
+    ln_stage(worst, "ln1", st["x0"], layer.self_attn_layer_norm, st["xn1"], split)
+    ln_stage(worst, "ln2", st["x1"], layer.final_layer_norm, st["xn2"], split)
+    qkv_stage(worst, st["xn1"], pk["w_qkv"], pk["b_qkv"], st["qkv"], E, q_scale(E // H), T, cos, sin, split)
+    if split:
+        attention_stage_split(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
+    else:
+        attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
+    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], E, split)
+    fc1_stage(worst, st["xn2"], pk["w_fc1"], layer.fc1.bias, st["h"], E, F, split)
+    residual_stage(worst, "fc2", st["h"], pk["w_fc2"], layer.fc2.bias, st["x1"], st["x"], F, split)
+
+
+# ---- fp8 stages (fp8_refs' bounds on the dequantised operands) -----------------------------------------------------
+def _e4m3(q: torch.Tensor) -> torch.Tensor:
+    return q.view(torch.float8_e4m3fn)
+
+
+def _codes_stage(worst, name, q8, s, y, ybnd):
+    """an e4m3 output with its 1 x 128 scales against float64 (fp8_refs.check_codes): no scale off by more than the
+    edge case, no code farther from y than half an e4m3 ulp plus the bound, boundary flips under 2 %"""
+    r = fp8_refs.check_codes(_e4m3(q8), s, y, ybnd, device=y.device)
+    assert r["bad_scale"] == 0 and r["bad_code"] == 0 and r["flips"] <= max(64, r["n"] // 50), (name, r)
+    _worst(worst, name + "_flip_share", r["flips"] / r["n"])
+
+
+def check_fp8_stages(layer, pk: Dict, st: Dict, pad: torch.Tensor, B: int, T: int, cos, sin, worst: Dict,
+                     probs: Optional[torch.Tensor] = None):
+    """The stages of one replayed fp8 layer: LayerNorm -> e4m3 codes and scales, the QKV, fc1 (GELU -> e4m3) and fc2
+    (residual) GEMMs on the dequantised operands with fp8_refs.acc_bound (2^-11 per K block), and the stages the fp8
+    layer shares with fp16 (attention, out_proj)."""
+    E, H, F = layer.embed_dim, layer.attention_heads, layer.ffn_embed_dim
+    a = layer.self_attn
+    for name, x, ln, q8, s in (("ln1_codes", st["x0"], layer.self_attn_layer_norm, st["xn1"], st["xs1"]),
+                               ("ln2_codes", st["x1"], layer.final_layer_norm, st["xn2"], st["xs2"])):
+        want, b = _ln_want(x, ln)
+        _codes_stage(worst, name, q8, s, want, b + 2.0 ** -24 * want.abs())
+    A = fp8_refs.dequantize(_e4m3(st["xn1"]), st["xs1"], 1)
+    W = fp8_refs.dequantize(_e4m3(pk["q_qkv"]), pk["s_qkv"], 128)
+    y, absdot = kr.qkv_ref(A, W, pk["b_qkv"], 0.125, E, T, cos, sin)
+    acc = absdot * (2.0 ** -11 + 2.0 ** -24 * math.ceil(E / 128))
+    _worst(worst, "qkv", _ratio((st["qkv"].double() - y).abs(), acc + 6 * kr.U32 * y.abs() + kr.f16_bound(y)))
+    del A, W, y, absdot, acc
+    attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
+    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], E, False)
+    A = fp8_refs.dequantize(_e4m3(st["xn2"]), st["xs2"], 1)
+    W = fp8_refs.dequantize(_e4m3(pk["q_fc1"]), pk["s_fc1"], 128)
+    ref = A @ W.t() + layer.fc1.bias.double()
+    y = kr.gelu64(ref)
+    ybnd = 1.13 * fp8_refs.acc_bound(A, W) + 1e-7 * ref.abs() + 2.0 ** -20 * y.abs()
+    _codes_stage(worst, "fc1_codes", st["h"], st["hs"], y, ybnd)
+    del A, W, ref, y, ybnd
+    A = fp8_refs.dequantize(_e4m3(st["h"]), st["hs"], 1)
+    W = fp8_refs.dequantize(_e4m3(pk["q_fc2"]), pk["s_fc2"], 128)
+    upd = A @ W.t() + layer.fc2.bias.double()
+    want = st["x1"].double() + upd
+    acc = fp8_refs.acc_bound(A, W) + 2 * kr.U32 * upd.abs()
+    _worst(worst, "fc2", _ratio((st["x"].double() - want).abs(), kr.residual_bound(acc, want)))
+
+
+# ---- MSA Transformer axial layer ------------------------------------------------------------------------------------
+def pack_axial(layer, precision: int) -> Dict:
+    out = {}
+    for key, blk in (("row", layer.row_self_attention.layer), ("col", layer.column_self_attention.layer)):
+        w = torch.cat([blk.q_proj.weight, blk.k_proj.weight, blk.v_proj.weight]).detach().float().contiguous()
+        out[key + "_qkv"] = _pack_matrix(w, precision)
+        out[key + "_b"] = torch.cat([blk.q_proj.bias, blk.k_proj.bias, blk.v_proj.bias]).detach().float().contiguous()
+        out[key + "_out"] = _pack_matrix(blk.out_proj.weight, precision)
+    ffn = layer.feed_forward_layer.layer
+    out["fc1"], out["fc2"] = _pack_matrix(ffn.fc1.weight, precision), _pack_matrix(ffn.fc2.weight, precision)
+    return out
+
+
+def replay_axial(layer, pk: Dict, x: torch.Tensor, pad: Optional[torch.Tensor], B: int, R: int, C: int,
+                 precision: int, row_probs: Optional[torch.Tensor] = None) -> Dict:
+    """One AxialTransformerLayer in place on x fp32 [B*R*C, E]: tied row attention (q zeroed at padded tokens, key
+    padding from row 0 of each alignment), column attention, feed-forward.  pad [B,R,C] bool or None.  Returns the
+    stages: x0, row_xn, row_qkv (q zeroed), row_ctx, x_row, col_xn, col_qkv, col_ctx, x_col, ffn_xn, h, x."""
+    E, H, F = layer.embedding_dim, layer.num_heads, layer.ffn_embedding_dim
+    M = B * R * C
+    pf = 2 if precision == 1 else 1
+    split = precision == 1
+    dev = x.device
+    L = lib()
+    xn = torch.empty(M, pf * E, dtype=torch.float16, device=dev)
+    qkv = torch.empty(M, pf * 3 * E, dtype=torch.float16, device=dev)
+    ctx = torch.empty(M, pf * E, dtype=torch.float16, device=dev)
+    key_pad = col_pad = None
+    if pad is not None:
+        key_pad = pad[:, 0].contiguous().to(torch.uint8)
+        col_pad = pad.permute(0, 2, 1).contiguous().to(torch.uint8)
+    st = dict(x0=x.clone())
+
+    def qkv_proj(w, b, scale):
+        if split:
+            check(L.esmb200_gemm_qkv_split(P(xn), P(w), P(b), P(qkv), M, E, scale, S()))
+        else:
+            check(L.esmb200_gemm_qkv_f16(P(xn), P(w), P(b), P(qkv), M, E, scale, None, None, 0, S()))
+
+    blk = layer.row_self_attention
+    _ln(x, blk.layer_norm, xn, precision)
+    st["row_xn"] = xn.clone()
+    qkv_proj(pk["row_qkv"], pk["row_b"], q_scale(64, R))
+    if pad is not None:
+        q5 = qkv.view(B, R, C, 3 * pf, E)
+        q5[:, :, :, 0].masked_fill_(pad[..., None], 0)
+        if split:
+            q5[:, :, :, 3].masked_fill_(pad[..., None], 0)
+    st["row_qkv"] = qkv.clone()
+    if split:
+        nbytes, tied = L.esmb200_tied_row_attention_split_scratch_bytes(B, C, H), L.esmb200_tied_row_attention_split
+    else:
+        nbytes, tied = L.esmb200_tied_row_attention_scratch_bytes(B, C, H), L.esmb200_tied_row_attention
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    check(tied(P(qkv), P(key_pad), P(ctx), P(row_probs), B, R, C, H, P(scratch), nbytes, S()))
+    st["row_ctx"] = ctx.clone()
+    _gemm(kr.EPI_BIAS_RESIDUAL, ctx, pk["row_out"], blk.layer.out_proj.bias, x, M, E, E, precision)
+    st["x_row"] = x.clone()
+    blk = layer.column_self_attention
+    _ln(x, blk.layer_norm, xn, precision)
+    st["col_xn"] = xn.clone()
+    qkv_proj(pk["col_qkv"], pk["col_b"], q_scale(64))
+    st["col_qkv"] = qkv.clone()
+    scratch = torch.empty(L.esmb200_attention_scratch_bytes(B * C, R), dtype=torch.uint8, device=dev)
+    col = L.esmb200_column_attention_split if split else L.esmb200_column_attention
+    check(col(P(qkv), P(col_pad), P(ctx), B, R, C, H, P(scratch), S()))
+    st["col_ctx"] = ctx.clone()
+    _gemm(kr.EPI_BIAS_RESIDUAL, ctx, pk["col_out"], blk.layer.out_proj.bias, x, M, E, E, precision)
+    st["x_col"] = x.clone()
+    blk = layer.feed_forward_layer
+    _ln(x, blk.layer_norm, xn, precision)
+    st["ffn_xn"] = xn.clone()
+    h = torch.empty(M, pf * F, dtype=torch.float16, device=dev)
+    _gemm(kr.EPI_BIAS_GELU, xn, pk["fc1"], blk.layer.fc1.bias, h, M, F, E, precision)
+    st["h"] = h.clone()
+    _gemm(kr.EPI_BIAS_RESIDUAL, h, pk["fc2"], blk.layer.fc2.bias, x, M, E, F, precision)
+    st["x"] = x
+    return st
+
+
+def _column_major(t: torch.Tensor, B: int, R: int, C: int) -> torch.Tensor:
+    """[B*R*C, w] row-major alignment tensor -> [B*C*R, w]: the column sequences of R tokens, one after another"""
+    w = t.shape[-1]
+    return t.view(B, R, C, w).permute(0, 2, 1, 3).reshape(B * C * R, w)
+
+
+def check_axial_stages(layer, pk: Dict, st: Dict, pad: Optional[torch.Tensor], B: int, R: int, C: int,
+                       precision: int, worst: Dict):
+    """Every stage of one replayed AxialTransformerLayer against float64 on its own inputs: the three LayerNorms, the
+    row and column QKV (row q scale fp32(d^-1/2 / sqrt(R)), q zero at padded tokens), the tied row attention end to
+    end (tied_ctx_bound, tied_relfro_gate), the column attention (the fp16 or split attention bounds, per column
+    sequence of R tokens, over both key-block sizes of the fp16 kernels), the two out-projections and the
+    feed-forward."""
+    E, H, F = layer.embedding_dim, layer.num_heads, layer.ffn_embedding_dim
+    split = precision == 1
+    pf = 2 if split else 1
+    ln_stage(worst, "row_ln", st["x0"], layer.row_self_attention.layer_norm, st["row_xn"], split)
+    ln_stage(worst, "col_ln", st["x_row"], layer.column_self_attention.layer_norm, st["col_xn"], split)
+    ln_stage(worst, "ffn_ln", st["x_col"], layer.feed_forward_layer.layer_norm, st["ffn_xn"], split)
+    zero = pad.reshape(-1) if pad is not None else None
+    w_sub = {}
+    qkv_stage(w_sub, st["row_xn"], pk["row_qkv"], pk["row_b"], st["row_qkv"], E, q_scale(64, R), 1, None, None,
+              split, zero)
+    _worst(worst, "row_qkv", w_sub.pop("qkv"))
+    qkv_stage(w_sub, st["col_xn"], pk["col_qkv"], pk["col_b"], st["col_qkv"], E, q_scale(64), 1, None, None, split)
+    _worst(worst, "col_qkv", w_sub.pop("qkv"))
+    # tied row attention on its own (q-zeroed) q, k, v
+    key_pad = pad[:, 0] if pad is not None else None
+    r = kr.tied64(st["row_qkv"], key_pad, B, R, C, H, split)
+    cv = st["row_ctx"].double().view(B, R, C, pf * E)
+    got = (cv[..., :E] + cv[..., E:] if split else cv).reshape(B, R, C, H, 64)
+    err = (got - r["ctx"]).abs()
+    _worst(worst, "tied_ctx", _ratio(err, kr.tied_ctx_bound(r)))
+    fro = (err.pow(2).sum((1, 2, 4)) / r["ctx"].pow(2).sum((1, 2, 4)).clamp_min(1e-300)).sqrt()
+    _worst(worst, "tied_relfro_gate", float((fro / kr.tied_relfro_gate(r)).max()))
+    del r, err, got
+    # column attention: B*C sequences of R tokens
+    cq, cc = _column_major(st["col_qkv"], B, R, C), _column_major(st["col_ctx"], B, R, C)
+    cpad = pad.permute(0, 2, 1).reshape(B * C, R) if pad is not None else torch.zeros(B * C, R, dtype=torch.bool,
+                                                                                         device=cq.device)
+    if split:
+        attention_stage_split(worst, cq, cc, cpad, B * C, R, H, prefix="col_")
+    else:
+        attention_stage_f16(worst, cq, cc, cpad, B * C, R, H, blocks=(64, 128), prefix="col_")
+    residual_stage(worst, "row_out_proj", st["row_ctx"], pk["row_out"], layer.row_self_attention.layer.out_proj.bias,
+                   st["x0"], st["x_row"], E, split)
+    residual_stage(worst, "col_out_proj", st["col_ctx"], pk["col_out"],
+                   layer.column_self_attention.layer.out_proj.bias, st["x_row"], st["x_col"], E, split)
+    ffn = layer.feed_forward_layer.layer
+    fc1_stage(worst, st["ffn_xn"], pk["fc1"], ffn.fc1.bias, st["h"], E, F, split)
+    residual_stage(worst, "fc2", st["h"], pk["fc2"], ffn.fc2.bias, st["x_col"], st["x"], F, split)
+
+
+# ---- the packed matrices of esmb200_layer_offload -------------------------------------------------------------------
+def _align(n: int, a: int = 1024) -> int:
+    return (n + a - 1) // a * a
+
+
+def packed_arena(layer, split: bool) -> torch.Tensor:
+    """uint8 bytes of api.cu packed_layout for one TransformerLayer of any head width, built on the host from the
+    module's parameters: [Wq;Wk;Wv] rows and out_proj columns in their zero-padded 64-wide head slots
+    (fp8_refs.head_slot), fc1 and fc2 as they are; fp16, or with split the hi | lo halves side by side along K, each
+    matrix 1024-byte aligned."""
+    a = layer.self_attn
+    E, H = layer.embed_dim, layer.attention_heads
+    d = E // H
+    Ea = 64 * kr.head_slots(E, H) * H
+    slot = fp8_refs.head_slot(torch.arange(E), d)
+
+    def enc(w32):  # fp32 [N, K] -> fp16 [N, K] or [N, 2K]
+        w32 = w32.detach().float().cpu()
+        if not split:
+            return w32.half()
+        hi, lo = kr.split16(w32)
+        return torch.cat([hi, lo], 1)
+
+    pf = 2 if split else 1
+    qkv = torch.zeros(3 * Ea, pf * E, dtype=torch.float16)
+    for s3, w in enumerate((a.q_proj.weight, a.k_proj.weight, a.v_proj.weight)):
+        qkv[s3 * Ea + slot] = enc(w)
+    out = torch.zeros(E, pf * Ea, dtype=torch.float16)
+    wo = enc(a.out_proj.weight)
+    out[:, slot] = wo[:, :E]
+    if split:
+        out[:, Ea + slot] = wo[:, E:]
+    parts = [qkv, out, enc(layer.fc1.weight), enc(layer.fc2.weight)]
+    chunks = []
+    for p in parts:
+        b = p.contiguous().view(torch.uint8).reshape(-1)
+        chunks.append(torch.cat([b, torch.zeros(_align(b.numel()) - b.numel(), dtype=torch.uint8)]))
+    return torch.cat(chunks)

@@ -42,19 +42,7 @@ def operands(M, N, K, seed, scale=1.0):
     return a, w, bias
 
 
-def exact(a, w, bias):
-    """(a w^T + bias in float64, sum_k |a_k w_k|)"""
-    ad, wd = a.double(), w.double()
-    return ad @ wd.t() + bias.double(), ad.abs() @ wd.abs().t()
-
-
-def acc_bound(absdot, K, y):
-    return (K / 16 + 4) * 2.0 ** -22 * absdot + 2 * kr.U32 * y.abs()
-
-
-def f16_bound(y):
-    """rounding of a finite fp32 value to fp16: half an ulp, 2^-11 relative, 2^-25 absolute below the normal range."""
-    return 2.0 ** -11 * y.abs() + 2.0 ** -25
+exact, acc_bound, f16_bound, qkv_ref = kr.gemm_exact, kr.gemm_acc_bound, kr.f16_bound, kr.qkv_ref
 
 
 def run_gemm(epi, a, w, bias, out, M, N, K, cos=None, sin=None, T=0, E=0):
@@ -94,29 +82,8 @@ def check_plain(epi, M, N, K, seed):
     return ratio
 
 
-def qkv_ref(a, w, bias, q_scale, E, T=None, cos=None, sin=None):
-    """[q*scale | k | v] in float64 (the bias added before the scale), with rotate-half RoPE on every 64-column group
-    of q and k: pair (c, c + 32) rotated by table column c of a [T, 32] table."""
-    y, absdot = exact(a, w, bias)
-    y = y.clone()
-    y[:, :E] *= q_scale
-    absdot = absdot.clone()
-    absdot[:, :E] *= q_scale
-    if cos is not None:
-        M = y.shape[0]
-        t = torch.arange(M, device=y.device) % T
-        c64, s64 = cos.double()[t], sin.double()[t]
-        for g0 in range(0, 2 * E, 64):
-            c, s = c64, s64
-            x1, x2 = y[:, g0:g0 + 32].clone(), y[:, g0 + 32:g0 + 64].clone()
-            y[:, g0:g0 + 32], y[:, g0 + 32:g0 + 64] = x1 * c - x2 * s, x2 * c + x1 * s
-            d1, d2 = absdot[:, g0:g0 + 32].clone(), absdot[:, g0 + 32:g0 + 64].clone()
-            absdot[:, g0:g0 + 32] = absdot[:, g0 + 32:g0 + 64] = d1 + d2  # |cos|, |sin| <= 1
-    return y, absdot
-
-
 def check_qkv(out, y, absdot, K):
-    b = acc_bound(absdot, K, y) + 4 * kr.U32 * y.abs() + f16_bound(y)
+    b = kr.qkv_bound(y, absdot, K)
     err = (out.double() - y).abs()
     assert not bool(err.isnan().any())
     ratio = float((err / b).max())

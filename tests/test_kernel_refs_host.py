@@ -755,3 +755,64 @@ def test_layer64_matches_the_oracle_layer(E, H):
     torch.testing.assert_close(gp, wp.double(), atol=2e-6, rtol=0)
     torch.testing.assert_close(got, want.double(), atol=3e-5, rtol=0)
     assert float(gp[1, :, :, 21:].abs().max()) == 0.0
+
+
+# ---- the bounds of the layer-stack stages (tests/stack_replay.py) ---------------------------------------------------
+def _fp16_operands(M, N, K, seed):
+    g = torch.Generator().manual_seed(seed)
+    a = torch.randn(M, K, generator=g).half()
+    w = (torch.randn(N, K, generator=g) * K ** -0.5).half()
+    return a, w, 0.1 * torch.randn(N, generator=g)
+
+
+@pytest.mark.parametrize("K", [1280, 5120])
+def test_residual_bound_holds_for_fp32_and_refuses_a_scaled_update(K):
+    """x + fp32(a w^T + bias) (an fp32 GEMM, then the fp32 add) stays inside residual_bound; the update scaled by
+    1 + 2^-9 leaves it"""
+    M, N = 192, 256
+    a, w, bias = _fp16_operands(M, N, K, K)
+    x = torch.randn(M, N, generator=torch.Generator().manual_seed(K + 1))
+    y32 = a.float() @ w.float().t() + bias
+    y, absdot = kr.gemm_exact(a, w, bias)
+    want = x.double() + y
+    b = kr.residual_bound(kr.gemm_acc_bound(absdot, K, y), want)
+    assert float(((x + y32).double() - want).abs().div(b).max()) <= 1.0
+    bad = x + y32 * (1 + 2.0 ** -9)
+    assert float((bad.double() - want).abs().div(b).max()) > 1.5
+
+
+def test_qkv_bound_holds_for_fp32_and_refuses_a_shifted_rotation():
+    """the QKV epilogue restated in fp32 (bias, q scale, rotate-half by the [T, 32] table, fp16 output) stays inside
+    qkv_bound around qkv_ref; the same with every row rotated by the next position's table row leaves it"""
+    from esm_b200.model import rope_tables
+    T, B, H = 64, 2, 2
+    E, M = 64 * H, 2 * 64
+    a, w, bias = _fp16_operands(M, 3 * E, E, 5)
+    inv = 1.0 / (10000 ** (torch.arange(0, 64, 2).float() / 64))
+    cos, sin = rope_tables(inv, T + 1)
+
+    def emulate(shift):
+        y = a.float() @ w.float().t() + bias
+        y[:, :E] *= 0.125
+        t = torch.arange(M) % T + shift
+        c, s = cos[t], sin[t]
+        for g0 in range(0, 2 * E, 64):
+            x1, x2 = y[:, g0:g0 + 32].clone(), y[:, g0 + 32:g0 + 64].clone()
+            y[:, g0:g0 + 32], y[:, g0 + 32:g0 + 64] = x1 * c - x2 * s, x2 * c + x1 * s
+        return y.half()
+
+    want, absdot = kr.qkv_ref(a, w, bias, 0.125, E, T, cos[:T], sin[:T])
+    b = kr.qkv_bound(want, absdot, E)
+    assert float((emulate(0).double() - want).abs().div(b).max()) <= 1.0
+    assert float((emulate(1).double() - want).abs().div(b).max()) > 10
+
+
+def test_replay_q_scales_are_the_references_fp32_values():
+    """stack_replay.q_scale rounds the reference's double to fp32, and differs by one ulp from the fp32 expression the
+    library used before at the widths and depths DESIGN.md section 4 lists"""
+    import stack_replay as sr
+    assert sr.q_scale(64) == 0.125 and sr.q_scale(24) == float(np.float32(24 ** -0.5))
+    old = [d for d in range(2, 129, 2) if sr.q_scale(d) != float(np.float32(1) / np.sqrt(np.float32(d)))]
+    assert old == [6, 18, 24, 28, 34, 58, 68, 72, 78, 82, 84, 94, 96, 102, 112, 122]
+    rows = [R for R in range(1, 1025) if sr.q_scale(64, R) != float(np.float32(0.125) / np.sqrt(np.float32(R)))]
+    assert len(rows) == 242 and rows[:3] == [6, 7, 17]
