@@ -30,6 +30,7 @@ EXPORTS = (
     "esmb200_log_softmax_rows",
     "esmb200_gemm_f16",
     "esmb200_gemm_qkv_f16",
+    "esmb200_gemm_qkv_heads",
     "esmb200_attention_scratch_bytes",
     "esmb200_attention",
     "esmb200_attention128",
@@ -167,6 +168,9 @@ def _declare(lib):
     lib.esmb200_gemm_qkv_f16.restype = c_int32
     lib.esmb200_gemm_qkv_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p,
                                          c_void_p, c_int32, c_void_p]
+    lib.esmb200_gemm_qkv_heads.restype = c_int32
+    lib.esmb200_gemm_qkv_heads.argtypes = [c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+                                           c_int32, c_int32, c_float, c_void_p, c_void_p, c_int32, c_void_p]
     lib.esmb200_attention_scratch_bytes.restype = c_size_t
     lib.esmb200_attention_scratch_bytes.argtypes = [c_int32, c_int32]
     lib.esmb200_attention.restype = c_int32

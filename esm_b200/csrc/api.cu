@@ -562,6 +562,17 @@ struct ActMaps {
   CUtensorMap qkv_o, h_o, x_o;  // GEMM outputs: qkv and h (fp16), the fp32 residual stream x
 };
 
+// The QKV projection of a layer of E = H d: N = 3 Ea columns in head slots (Ea = 64 slots H), K = E, the q columns scaled
+// by q_scale, q and k rotated per 64-wide slot by a [T, 32 slots] table when rope_cos is given, the fp32x3 lo halves
+// 3 Ea columns to the right.  attention_block and esmb200_gemm_qkv_heads launch the projection with these parameters.
+GemmParams qkv_params(int M, int E, int Ea, int slots, const float* bias, const float* rope_cos, const float* rope_sin,
+                      int T, float q_scale) {
+  GemmParams g = gemm_params(M, 3 * Ea, E, bias);
+  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.rope_ld = 32 * slots; g.T = T; g.E = Ea; g.q_scale = q_scale;
+  g.lo_col_off = 3 * Ea;
+  return g;
+}
+
 // x += out_proj(attend()) after LN1 -> fp16 and the q,k,v projection (+ bias, q scale, RoPE when rope_cos is given):
 // the self-attention half of an ESM-2 layer (multihead_attention.py:258-261,354-355,395; modules.py:124-134) and each
 // axial attention sub-layer of the MSA stack.  `attend` reads ws.qkv and writes ws.ctx.  The weights are read through
@@ -574,9 +585,7 @@ int attention_block(const esmb200_layer* L, const WeightMaps& wm, float* x, int 
   int rc = L->fp8 ? layernorm_fp8(x, L->ln1_w, L->ln1_b, ws.xn, ws.xn_s, M, L->E, L->eps, T_LN1, st)
                   : layernorm_f16(x, L->ln1_w, L->ln1_b, ws.xn, M, L->E, L->eps, split, T_LN1, st);
   if (rc) return rc;
-  GemmParams g = gemm_params(M, 3 * L->Ea, L->E, L->b_qkv);
-  g.rope_cos = rope_cos; g.rope_sin = rope_sin; g.rope_ld = 32 * L->slots; g.T = T; g.E = L->Ea; g.q_scale = q_scale;
-  g.lo_col_off = 3 * L->Ea;
+  const GemmParams g = qkv_params(M, L->E, L->Ea, L->slots, L->b_qkv, rope_cos, rope_sin, T, q_scale);
   rc = L->fp8 ? launch_gemm_fp8(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, {g, ws.xn_s, L->s_qkv, nullptr}, st, T_QKV)
               : launch_gemm(EPI_QKV_ROPE, am.xn, wm.qkv, am.qkv_o, g, st, T_QKV, split);
   if (rc) return rc;
@@ -1259,6 +1268,45 @@ int esmb200_gemm_qkv_split(const void* a, const void* w, const float* bias, void
   int rc = check_device();
   if (rc) return rc;
   return run_gemm(EPI_QKV_ROPE, a, w, bias, out, M, 3 * E, E, nullptr, nullptr, 1, E, q_scale, true, stream);
+}
+
+int esmb200_gemm_qkv_heads(int32_t precision, const void* a, const float* a_scales, const void* w,
+                           const float* w_scales, const float* bias, void* out, int32_t M, int32_t E, int32_t H,
+                           float q_scale, const float* rope_cos, const float* rope_sin, int32_t T, void* stream) {
+  if (!a || !w || !bias || !out) return fail(ESMB200_EINVAL, "null argument");
+  if (precision < 0 || precision > 2) return fail(ESMB200_EINVAL, "precision must be 0 (fp16), 1 (fp32x3) or 2 (fp8)");
+  if (precision == 2 && (!a_scales || !w_scales))
+    return fail(ESMB200_EINVAL, "fp8 precision needs a_scales and w_scales");
+  // the shapes esmb200_layer_create refuses, with its messages
+  if (M <= 0 || E <= 0 || H <= 0 || E % H != 0)
+    return fail(ESMB200_EINVAL, "embed_dim must be a positive multiple of num_heads");
+  const int d = E / H;
+  if (d > 128 || d % 2 != 0)
+    return fail(ESMB200_EINVAL, "esmb200 supports even head_dim <= 128 (every ESM-2 model, MSA Transformer)");
+  if (E % 16 != 0) return fail(ESMB200_EINVAL, "embed_dim must be a multiple of 16");
+  const int slots = head_slots(E, H);
+  if (precision == 1 && slots == 2) return fail(ESMB200_EINVAL, "fp32x3 precision is not available for head_dim > 64");
+  if (precision == 1 && E % 64 != 0)
+    return fail(ESMB200_EINVAL, "fp32x3 precision needs embed_dim % 64 == 0 (all ESM-2 models except 35M)");
+  if ((rope_cos == nullptr) != (rope_sin == nullptr) || (rope_cos && T <= 0))
+    return fail(ESMB200_EINVAL, "rope tables must be given together with T, or not at all");
+  int rc = check_device();
+  if (rc) return rc;
+  const int Ea = 64 * slots * H;
+  const GemmParams g = qkv_params(M, E, Ea, slots, bias, rope_cos, rope_sin, T > 0 ? T : 1, q_scale);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUtensorMap ta, tb, to;
+  if (precision == 2) {
+    rc = make_tmap_2d(&ta, a, 1, M, E, E, gemm_fp8_cfg::BOX_ROWS);
+    if (!rc) rc = make_tmap_2d(&tb, w, 1, 3 * (uint64_t)Ea, E, E, gemm_fp8_cfg::BOX_ROWS);
+    if (!rc) rc = make_gemm_out_map(&to, out, 2, M, 3 * (uint64_t)Ea);
+    return rc ? rc : launch_gemm_fp8(EPI_QKV_ROPE, ta, tb, to, {g, a_scales, w_scales, nullptr}, st);
+  }
+  const uint64_t pf = precision == 1 ? 2 : 1;
+  rc = make_tmap_f16(&ta, a, M, pf * E, pf * E, gemm2_cfg::BOX_M);
+  if (!rc) rc = make_tmap_f16(&tb, w, 3 * (uint64_t)Ea, pf * E, pf * E, gemm2_cfg::HALF_N);
+  if (!rc) rc = make_gemm_out_map(&to, out, 2, M, pf * 3 * Ea);
+  return rc ? rc : launch_gemm(EPI_QKV_ROPE, ta, tb, to, g, st, T_GEMM_OTHER, precision == 1);
 }
 
 int esmb200_attention(const void* qkv, const uint8_t* pad_mask, void* ctx, float* attn_probs, int32_t B, int32_t T,

@@ -249,6 +249,18 @@ int esmb200_gemm_qkv_f16(const void* a_f16, const void* w_qkv_f16, const float* 
                          int32_t E, float q_scale, const float* rope_cos, const float* rope_sin, int32_t T,
                          void* stream);
 
+/* The layer's QKV projection at any head width: qkv = [q*q_scale | k | v] in head slots, q/k rotated when tables are
+ * given. d = E / H, slots = 1 (d <= 64) or 2 (d <= 128), Ea = 64 * slots * H; w [3Ea, K] packed by head_slot (row
+ * s*Ea + slot column of projection output h*d + j, zero rows elsewhere; DESIGN.md section 1).
+ * precision 0: a fp16 [M,E], w fp16 [3Ea,E]            -> fp16 [M,3Ea]
+ *           1: a [M,2E] hi|lo, w [3Ea,2E] hi|lo         -> [M,6Ea] hi|lo
+ *           2: a e4m3 [M,E] + a_scales, w e4m3 + w_scales -> fp16 [M,3Ea]
+ * rope tables [T, 32*slots] or both NULL. The same launch as the layers' QKV projection; refuses the widths and
+ * precisions esmb200_layer_create refuses. */
+int esmb200_gemm_qkv_heads(int32_t precision, const void* a, const float* a_scales, const void* w,
+                           const float* w_scales, const float* bias, void* out, int32_t M, int32_t E, int32_t H,
+                           float q_scale, const float* rope_cos, const float* rope_sin, int32_t T, void* stream);
+
 /* ctx[B*T,E] fp16 = softmax(q k^T + key padding mask) v per head, from qkv fp16 [B*T,3E] (q pre-scaled, q/k rotated).
  * scratch: at least esmb200_attention_scratch_bytes(B,T). attn_probs as in esmb200_layer_forward. */
 size_t esmb200_attention_scratch_bytes(int32_t B, int32_t T);

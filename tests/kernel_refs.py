@@ -8,6 +8,8 @@ tests/test_kernel_refs_host.py (so that a wrong reference cannot make a GPU test
     head of model.py RobertaLMHead.forward_native, the MSA Transformer's layer in msa.py);
   * gemm_exact / gemm_acc_bound / f16_bound / residual_bound / qkv_ref / qkv_bound: the fp16 GEMM's float64 reference
     and the bounds of its epilogues (residual add, q scale and RoPE);
+  * slot_columns / slot_rows / rope_pair_sum / qkv_ref_heads: heads of any width in zero-padded 64-wide slots, mapped
+    from the reference's rotate-half pairing, and the QKV projection in the reference's layout at any head width;
   * gelu_bound: the error bound of the GEMM epilogue's erf-GELU (csrc/gemm_common.cuh gelu_erf);
   * split16 / join64 / split_rep_bound / split_acc_bound / FP32X3_MODELS: the fp32x3 precision's hi | lo operand pairs,
     the bound of their representation, the accumulation bound of the three-pass split GEMM and the models it runs;
@@ -142,6 +144,60 @@ def qkv_ref(a, w, bias, q_scale, E, T=None, cos=None, sin=None):
             y[:, g0:g0 + 32], y[:, g0 + 32:g0 + 64] = x1 * c - x2 * s, x2 * c + x1 * s
             d1, d2 = absdot[:, g0:g0 + 32].clone(), absdot[:, g0 + 32:g0 + 64].clone()
             absdot[:, g0:g0 + 32] = absdot[:, g0 + 32:g0 + 64] = d1 + d2
+    return y, absdot
+
+
+def slot_columns(d: int, H: int) -> torch.Tensor:
+    """[H d] long: the attention-side column of projection output h d + j at head width d.  rotary_embedding.py's
+    rotate_half pairs dimension j with j + d/2 under the table column p = j mod d/2; the QKV epilogue rotates columns
+    (c, c + 32) of each 64-wide slot by table column 32 (slot mod slots) + c.  So pair p of head h goes to slot p // 32
+    of the head's head_slots(H d, H) slots, at columns p % 32 and 32 + p % 32, and meets table column p."""
+    slots, half = head_slots(d * H, H), d // 2
+    cols = torch.empty(H * d, dtype=torch.long)
+    for h in range(H):
+        for p in range(half):
+            c = (h * slots + p // 32) * 64 + p % 32
+            cols[h * d + p], cols[h * d + half + p] = c, c + 32
+    return cols
+
+
+def slot_rows(d: int, H: int) -> torch.Tensor:
+    """[3 H d] long: the row of the head-slot-packed [Wq;Wk;Wv] ([3 Ea, K]) that holds each row of the reference's
+    [Wq;Wk;Wv], and the column of the kernel's [q | k | v] output ([M, 3 Ea]) that holds each reference column"""
+    Ea = 64 * head_slots(d * H, H) * H
+    cols = slot_columns(d, H)
+    return torch.cat([s * Ea + cols for s in range(3)])
+
+
+def rope_pair_sum(t: torch.Tensor, E: int, H: int) -> torch.Tensor:
+    """t [M, >= 2E] in the reference's column order: both members of every rotate-half pair (j, j + d/2) of the q and
+    k heads replaced by their sum (the bound of a rotation by |cos|, |sin| <= 1 of two bounded values)"""
+    d = E // H
+    t = t.clone()
+    qk = t[:, :2 * E].view(-1, 2, H, 2, d // 2)
+    qk[:] = qk.sum(3, keepdim=True)
+    return t
+
+
+def qkv_ref_heads(a, w, bias, q_scale, H, T=None, cos=None, sin=None):
+    """[q*scale | k | v] in float64 in the reference's layout (w [3E, K] and bias [3E] in the reference's row order,
+    unpadded), the bias added before the scale, with rotary_embedding.py's rotate-half on every q and k head of width
+    d = E / H: (x1, x2) = the head's halves, (x1 cos - x2 sin, x2 cos + x1 sin) under the [T, d/2] table (row r at
+    position r % T).  Returns (y, absdot) with absdot the matching sum of |products| (rotated pairs: both members'
+    sums).  At d = 64 this is qkv_ref."""
+    y, absdot = gemm_exact(a, w, bias)
+    E = y.shape[1] // 3
+    d = E // H
+    y[:, :E] *= q_scale
+    absdot[:, :E] *= q_scale
+    if cos is not None:
+        M = y.shape[0]
+        t = torch.arange(M, device=y.device) % T
+        c, s = cos.double()[t][:, None, None, :d // 2], sin.double()[t][:, None, None, :d // 2]
+        qk = y[:, :2 * E].view(M, 2, H, d)
+        x1, x2 = qk[..., :d // 2].clone(), qk[..., d // 2:].clone()
+        qk[..., :d // 2], qk[..., d // 2:] = x1 * c - x2 * s, x2 * c + x1 * s
+        absdot = rope_pair_sum(absdot, E, H)
     return y, absdot
 
 

@@ -2,12 +2,14 @@
 intermediate kept, and the float64 checks of each stage on its own inputs (tests/test_gpu_stack_stages.py).
 
 The replay packs the weights itself from the module parameters (`.half()`, esmb200_convert_split hi | lo, [Wq;Wk;Wv]
-quantised by esmb200_quantize_fp8) and takes every parameter from the reference's definition rather than from the
-library: the module's LayerNorm eps, the q scale fp32(d ** -0.5) (fp32(d ** -0.5 / sqrt(R)) for the MSA row attention),
-and the rotary tables of rotary_embedding.py:47-61.  A stack that packs, scales or wires one of them differently gives
-other bits than the replay.
+quantised by esmb200_quantize_fp8), heads of any width into zero-padded 64-wide slots by its own map
+(kernel_refs.slot_columns), and takes every parameter from the reference's definition rather than from the library: the
+module's LayerNorm eps, the q scale fp32(d ** -0.5) (fp32(d ** -0.5 / sqrt(R)) for the MSA row attention), and the
+rotary tables of rotary_embedding.py:47-61, padded past d/2 with other values than the library's.  A stack that packs,
+scales or wires one of them differently gives other bits than the replay.
 
-  * pack_esm / replay_esm: one ESM-2 / ESM-1b layer in precision 0 (fp16), 1 (fp32x3) or 2 (fp8), head_dim 64;
+  * pack_esm / replay_esm: one ESM-2 / ESM-1b layer in precision 0 (fp16), 1 (fp32x3) or 2 (fp8) at any head width,
+    the QKV projection through esmb200_gemm_qkv_heads (the layer's own launch);
   * check_esm_stages / check_fp8_stages: each stage of one replayed layer against float64, worst ratios per stage;
   * pack_axial / replay_axial / check_axial_stages: one MSA Transformer AxialTransformerLayer in fp16 or fp32x3, and its
     stages against float64;
@@ -64,6 +66,21 @@ def rope_ref(inv_freq: torch.Tensor, T: int):
     return emb.cos()[:, :h].contiguous(), emb.sin()[:, :h].contiguous()
 
 
+# the replay's table columns past d/2: other values than model.rope_tables' padding (cos 1, sin 0), so that a stack
+# equal to the replay bit for bit rotates only zero rows of its packed weights by them
+PAD_COS, PAD_SIN = 0.5, 0.25
+
+
+def rope_slots(cos: torch.Tensor, sin: torch.Tensor, slots: int):
+    """the reference's [T, d/2] tables widened to the QKV epilogue's [T, 32 * slots], columns past d/2 PAD_COS and
+    PAD_SIN"""
+    T, h = cos.shape
+    c = torch.full((T, 32 * slots), PAD_COS, dtype=cos.dtype, device=cos.device)
+    s = torch.full((T, 32 * slots), PAD_SIN, dtype=cos.dtype, device=cos.device)
+    c[:, :h], s[:, :h] = cos, sin
+    return c, s
+
+
 def split_dev(w: torch.Tensor) -> torch.Tensor:
     """esmb200_convert_split: fp32 [N, K] -> fp16 [N, 2K] hi | lo"""
     w = w.detach().float().contiguous()
@@ -81,11 +98,25 @@ def _pack_matrix(w: torch.Tensor, precision: int):
 
 # ---- ESM-2 / ESM-1b layer -------------------------------------------------------------------------------------------
 def pack_esm(layer, precision: int) -> Dict:
-    """The GEMM operands of one TransformerLayer (head_dim 64: the head slots are the identity)."""
+    """The GEMM operands of one TransformerLayer at any head width d = E / H: [Wq;Wk;Wv] rows, their bias and out_proj's
+    columns in zero-padded 64-wide head slots by the test's own map (kernel_refs.slot_columns; the identity at d = 64),
+    fc1 and fc2 as they are.  The slot-packed fp32 matrices are then rounded to fp16, split by esmb200_convert_split
+    (hi | lo, out_proj's pitch 2 Ea) or quantised by esmb200_quantize_fp8 in 128-row blocks over the zero rows too.
+    Also returns the maps: rows [3E] (kernel_refs.slot_rows), cols [E], and Ea, slots."""
     a = layer.self_attn
-    wqkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight]).detach().float().contiguous()
-    pk = dict(b_qkv=torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]).detach().float().contiguous(),
-              w_out=_pack_matrix(a.out_proj.weight, 1 if precision == 1 else 0))
+    E, H = layer.embed_dim, layer.attention_heads
+    slots = kr.head_slots(E, H)
+    Ea = 64 * slots * H
+    dev = a.q_proj.weight.device
+    cols, rows = kr.slot_columns(E // H, H).to(dev), kr.slot_rows(E // H, H).to(dev)
+    wqkv = torch.zeros(3 * Ea, E, device=dev)
+    wqkv[rows] = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight]).detach().float()
+    bqkv = torch.zeros(3 * Ea, device=dev)
+    bqkv[rows] = torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]).detach().float()
+    wo = torch.zeros(E, Ea, device=dev)
+    wo[:, cols] = a.out_proj.weight.detach().float()
+    pk = dict(b_qkv=bqkv, w_out=_pack_matrix(wo, 1 if precision == 1 else 0), rows=rows, cols=cols, Ea=Ea,
+              slots=slots)
     if precision == 2:
         pk["q_qkv"], pk["s_qkv"] = fp8_refs.quantize_dev(wqkv, 128)
         pk["q_fc1"], pk["s_fc1"] = fp8_refs.quantize_dev(layer.fc1.weight.detach().float().contiguous(), 128)
@@ -119,17 +150,17 @@ def _gemm8(epi, a, sa, w, sw, bias, out, out_s, M, N, K, cos=None, sin=None, T=0
 
 def replay_esm(layer, pk: Dict, x: torch.Tensor, pad8: torch.Tensor, B: int, T: int, cos, sin, precision: int,
                probs: Optional[torch.Tensor] = None) -> Dict:
-    """One layer in place on x fp32 [B*T, E], kernel by kernel as api.cu attention_block / ffn_block launch them.
-    cos = sin = None: no rotary embedding (ESM-1b).  probs: fp32 [B,H,T,T] to fill, or None.  Returns the stages:
-    x0 (input), xn1, qkv, ctx, x1 (after out_proj), xn2, h, x (output), the fp8 scales xs1 / xs2 / hs."""
+    """One layer in place on x fp32 [B*T, E], kernel by kernel as api.cu attention_block / ffn_block launch them, at
+    any head width.  cos, sin: the reference's [T, d/2] tables (rope_ref), widened by rope_slots for the QKV epilogue;
+    None: no rotary embedding (ESM-1b).  probs: fp32 [B,H,T,T] to fill, or None.  Returns the stages: x0 (input), xn1,
+    qkv, ctx (head-slot layout), x1 (after out_proj), xn2, h, x (output), the fp8 scales xs1 / xs2 / hs."""
     E, H, F = layer.embed_dim, layer.attention_heads, layer.ffn_embed_dim
+    Ea, slots = pk["Ea"], pk["slots"]
     M = B * T
-    d = E // H
     pf = 2 if precision == 1 else 1
     dev = x.device
     L = lib()
     st = dict(x0=x.clone())
-    qs = q_scale(d)
     if precision == 2:
         xn = torch.empty(M, E, dtype=torch.uint8, device=dev)
         xs = torch.empty((E + 127) // 128, M, device=dev)
@@ -137,27 +168,20 @@ def replay_esm(layer, pk: Dict, x: torch.Tensor, pad8: torch.Tensor, B: int, T: 
         xn, xs = torch.empty(M, pf * E, dtype=torch.float16, device=dev), None
     _ln(x, layer.self_attn_layer_norm, xn, precision, xs)
     st.update(xn1=xn.clone(), xs1=None if xs is None else xs.clone())
-    qkv = torch.empty(M, pf * 3 * E, dtype=torch.float16, device=dev)
-    if precision == 2:
-        # esmb200_gemm_fp8 takes rope tables only; cos = 1, sin = 0 rotates by nothing (x1 * 1 - x2 * 0 == x1)
-        assert qs == 0.125, "esmb200_gemm_fp8 scales q by 0.125"
-        c, s_ = (cos, sin) if cos is not None else (torch.ones(T, 32, device=dev), torch.zeros(T, 32, device=dev))
-        _gemm8(kr.EPI_QKV_ROPE, xn, xs, pk["q_qkv"], pk["s_qkv"], pk["b_qkv"], qkv, None, M, 3 * E, E, c, s_, T, E)
-    elif precision == 1 and cos is not None:
-        assert qs == 0.125, "esmb200_gemm_split scales q by 0.125"
-        _gemm(kr.EPI_QKV_ROPE, xn, pk["w_qkv"], pk["b_qkv"], qkv, M, 3 * E, E, 1, cos, sin, T, E)
-    elif precision == 1:
-        check(L.esmb200_gemm_qkv_split(P(xn), P(pk["w_qkv"]), P(pk["b_qkv"]), P(qkv), M, E, qs, S()))
-    else:
-        check(L.esmb200_gemm_qkv_f16(P(xn), P(pk["w_qkv"]), P(pk["b_qkv"]), P(qkv), M, E, qs, P(cos), P(sin),
-                                     T if cos is not None else 0, S()))
+    qkv = torch.empty(M, pf * 3 * Ea, dtype=torch.float16, device=dev)
+    c, s_ = rope_slots(cos, sin, slots) if cos is not None else (None, None)
+    w, ws = (pk["q_qkv"], pk["s_qkv"]) if precision == 2 else (pk["w_qkv"], None)
+    check(L.esmb200_gemm_qkv_heads(precision, P(xn), P(xs), P(w), P(ws), P(pk["b_qkv"]), P(qkv), M, E, H,
+                                   q_scale(E // H), P(c), P(s_), T if cos is not None else 0, S()))
     st["qkv"] = qkv.clone()
-    ctx = torch.empty(M, pf * E, dtype=torch.float16, device=dev)
+    ctx = torch.empty(M, pf * Ea, dtype=torch.float16, device=dev)
     scratch = torch.empty(L.esmb200_attention_scratch_bytes(B, T), dtype=torch.uint8, device=dev)
-    att = L.esmb200_attention_split if precision == 1 else L.esmb200_attention
+    att = (L.esmb200_attention_split if precision == 1 else
+           L.esmb200_attention128 if slots == 2 else L.esmb200_attention)
     check(att(P(qkv), P(pad8), P(ctx), P(probs), B, T, H, P(scratch), S()))
     st["ctx"] = ctx.clone()
-    _gemm(kr.EPI_BIAS_RESIDUAL, ctx, pk["w_out"], layer.self_attn.out_proj.bias, x, M, E, E, 1 if precision == 1 else 0)
+    _gemm(kr.EPI_BIAS_RESIDUAL, ctx, pk["w_out"], layer.self_attn.out_proj.bias, x, M, E, Ea,
+          1 if precision == 1 else 0)
     st["x1"] = x.clone()
     _ln(x, layer.final_layer_norm, xn, precision, xs)
     st.update(xn2=xn.clone(), xs2=None if xs is None else xs.clone())
@@ -221,39 +245,83 @@ def ln_stage(worst, name, x, ln, got, split):
     _worst(worst, name, _ratio(err, b))
 
 
-def _heads(t: torch.Tensor, B: int, T: int, H: int, i: int) -> torch.Tensor:
-    """section i (0 q, 1 k, 2 v) of [B*T, 3E] as [B, H, T, 64]"""
-    E = 64 * H
-    return t[:, i * E:(i + 1) * E].reshape(B, T, H, 64).transpose(1, 2)
+def _heads(t: torch.Tensor, B: int, T: int, H: int, i: int, slots: int = 1) -> torch.Tensor:
+    """section i (0 q, 1 k, 2 v) of the head-slot layout [B*T, 3 Ea] (Ea = 64 slots H) as [B, H, T, 64 slots]"""
+    D = 64 * slots
+    Ea = D * H
+    return t[:, i * Ea:(i + 1) * Ea].reshape(B, T, H, D).transpose(1, 2)
 
 
-def qkv_stage(worst, xn, w_qkv, bqkv, qkv, E, qs, T, cos, sin, split, zero_rows=None):
-    """the QKV projection (q scale, RoPE when cos is given) on the kernel's own operands; zero_rows [M] bool: rows whose
-    q the caller zeroed (the MSA row attention's padded tokens)"""
+def padding_columns(rows: torch.Tensor, width: int) -> torch.Tensor:
+    """[width] bool: the columns of a head-slot tensor that no reference column maps to"""
+    m = torch.ones(width, dtype=torch.bool, device=rows.device)
+    m[rows] = False
+    return m
+
+
+def zero_columns_stage(name, t, rows, n_halves=1):
+    """every padding column of the head-slot tensor t ([M, W] or [M, n_halves W] hi | lo) is exactly 0"""
+    W = t.shape[1] // n_halves
+    pad = padding_columns(rows, W)
+    for i in range(n_halves):
+        assert bool((t[:, i * W:(i + 1) * W][:, pad] == 0).all()), f"{name}: a padding column is not 0"
+
+
+def qkv_stage(worst, xn, w_qkv, bqkv, qkv, E, H, qs, T, cos, sin, split, zero_rows=None):
+    """the QKV projection (q scale, rotate-half RoPE when cos [T, d/2] is given) on the kernel's own operands, compared
+    in the reference's layout: w_qkv [3Ea, K] and bqkv [3Ea] in head slots, the kernel's qkv [M, 3Ea] (hi | lo
+    [M, 6Ea]) read through kernel_refs.slot_rows, against qkv_ref_heads on the unpadded rows; every padding column
+    exactly 0.  zero_rows [M] bool: rows whose q the caller zeroed (the MSA row attention's padded tokens)."""
+    rows = kr.slot_rows(E // H, H).to(qkv.device)
     if split:
-        from test_gpu_gemm_split import split_qkv_bound
-        xh, xl, wh, wl = xn[:, :E], xn[:, E:], w_qkv[:, :E], w_qkv[:, E:]
+        zero_columns_stage("qkv", qkv, rows, 2)
+        Ea3 = qkv.shape[1] // 2
+        xh, xl, wh, wl = xn[:, :E], xn[:, E:], w_qkv[rows, :E], w_qkv[rows, E:]
         aj, wj = kr.join64(xh, xl), kr.join64(wh, wl)
-        y_pre = aj @ wj.t() + bqkv.double()
+        b = bqkv[rows]
+        y_pre = aj @ wj.t() + b.double()
         y_pre[:, :E] *= qs
-        y, _ = kr.qkv_ref(aj, wj, bqkv, qs, E, T, cos, sin)
-        b = split_qkv_bound(xh, xl, wh, wl, E, y_pre, E, qs, cos) + kr.split_rep_bound(y)
-        got = kr.join64(qkv[:, :3 * E], qkv[:, 3 * E:])
+        y, _ = kr.qkv_ref_heads(aj, wj, b, qs, H, T, cos, sin)
+        bnd = split_qkv_heads_bound(xh, xl, wh, wl, y_pre, E, H, qs, cos is not None) + kr.split_rep_bound(y)
+        got = kr.join64(qkv[:, :Ea3][:, rows], qkv[:, Ea3:][:, rows])
     else:
-        y, absdot = kr.qkv_ref(xn, w_qkv, bqkv, qs, E, T, cos, sin)
-        b = kr.qkv_bound(y, absdot, E)
-        got = qkv.double()
+        zero_columns_stage("qkv", qkv, rows)
+        y, absdot = kr.qkv_ref_heads(xn, w_qkv[rows], bqkv[rows], qs, H, T, cos, sin)
+        bnd = kr.qkv_bound(y, absdot, E)
+        got = qkv[:, rows].double()
     if zero_rows is not None:
         y[zero_rows, :E] = 0.0
-    _worst(worst, "qkv", _ratio((got - y).abs(), b))
+    _worst(worst, "qkv", _ratio((got - y).abs(), bnd))
 
 
-def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,), prefix=""):
-    """fp16 attention on the kernel's q, k, v (qkv [B*T, 3E], sequences of T tokens, pad [B, T] bool): ctx element-wise
-    (attn_ctx_bound) and per (sequence, head) rel-Fro (attn_relfro_gate), probabilities and row sums of the valid query
-    rows.  blocks: the key-block sizes the kernel may walk; the bound is the largest over them."""
-    q, k, v = (_heads(qkv, B, T, H, i) for i in range(3))
-    got = _heads(ctx, B, T, H, 0).double()
+def split_qkv_heads_bound(ah, al, wh, wl, y_pre, E, H, q_scale, rotary):
+    """test_gpu_gemm_split.split_qkv_bound in the reference's layout at head width d = E / H: the split GEMM's
+    accumulation bound, times q_scale on the q columns plus one rounding (u |y_pre|), and for the rotate-half pairs
+    (j, j + d/2) of the q and k heads both members' bounds plus the rotation's two products and one add
+    (4 u (|x1| + |x2|)).  y_pre: the unrotated (a w^T + bias) * scale in float64."""
+    b = kr.split_acc_bound(ah, al, wh, wl, E, y_pre)
+    b[:, :E] *= q_scale
+    b = b + kr.U32 * y_pre.abs()
+    if rotary:
+        x = kr.rope_pair_sum(y_pre.abs(), E, H)
+        b = kr.rope_pair_sum(b, E, H)
+        b[:, :2 * E] += 4 * kr.U32 * x[:, :2 * E]
+    return b
+
+
+def key_blocks(slots: int):
+    """the key-block size of the fp16 forward kernel: 128 (attention_wg_kernel) for one slot per head, 64
+    (attention_fwd_kernel<false, 2>, esmb200_attention128) for two"""
+    return (128,) if slots == 1 else (64,)
+
+
+def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,), prefix="", slots=1):
+    """fp16 attention on the kernel's q, k, v (qkv [B*T, 3Ea] in head slots, sequences of T tokens, pad [B, T] bool):
+    ctx element-wise (attn_ctx_bound) and per (sequence, head) rel-Fro (attn_relfro_gate), probabilities and row sums
+    of the valid query rows.  The heads are taken 64 slots wide, their padding columns included (zeros add nothing to
+    q k^T or P v).  blocks: the key-block sizes the kernel may walk; the bound is the largest over them."""
+    q, k, v = (_heads(qkv, B, T, H, i, slots) for i in range(3))
+    got = _heads(ctx, B, T, H, 0, slots).double()
     terms = {bl: [0, 0, 0] for bl in blocks}
     err2 = 0
     for i0, r0 in kr.attention64_rows(q, k, v, pad, blocks[0]):
@@ -331,18 +399,20 @@ def fc1_stage(worst, xn, w, bias, h, E, F, split):
 def check_esm_stages(layer, pk: Dict, st: Dict, pad: torch.Tensor, B: int, T: int, cos, precision: int, worst: Dict,
                      probs: Optional[torch.Tensor] = None, sin=None):
     """Every stage of one replayed layer against float64 on that stage's own inputs; the largest error / bound of each
-    stage is folded into `worst`.  fp16 and fp32x3 (fp8: check_fp8_stages)."""
+    stage is folded into `worst`.  fp16 and fp32x3 (fp8: check_fp8_stages).  cos, sin: the reference's [T, d/2]
+    tables.  The QKV stage runs in the reference's layout, attention and out_proj (K = Ea) on the head slots."""
     E, H, F = layer.embed_dim, layer.attention_heads, layer.ffn_embed_dim
     split = precision == 1
     a = layer.self_attn
     ln_stage(worst, "ln1", st["x0"], layer.self_attn_layer_norm, st["xn1"], split)
     ln_stage(worst, "ln2", st["x1"], layer.final_layer_norm, st["xn2"], split)
-    qkv_stage(worst, st["xn1"], pk["w_qkv"], pk["b_qkv"], st["qkv"], E, q_scale(E // H), T, cos, sin, split)
+    qkv_stage(worst, st["xn1"], pk["w_qkv"], pk["b_qkv"], st["qkv"], E, H, q_scale(E // H), T, cos, sin, split)
+    zero_columns_stage("ctx", st["ctx"], pk["cols"], 2 if split else 1)
     if split:
         attention_stage_split(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
     else:
-        attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
-    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], E, split)
+        attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs, key_blocks(pk["slots"]), slots=pk["slots"])
+    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], pk["Ea"], split)
     fc1_stage(worst, st["xn2"], pk["w_fc1"], layer.fc1.bias, st["h"], E, F, split)
     residual_stage(worst, "fc2", st["h"], pk["w_fc2"], layer.fc2.bias, st["x1"], st["x"], F, split)
 
@@ -371,14 +441,20 @@ def check_fp8_stages(layer, pk: Dict, st: Dict, pad: torch.Tensor, B: int, T: in
                                ("ln2_codes", st["x1"], layer.final_layer_norm, st["xn2"], st["xs2"])):
         want, b = _ln_want(x, ln)
         _codes_stage(worst, name, q8, s, want, b + 2.0 ** -24 * want.abs())
+    # the QKV projection in the reference's layout (the dequantised slot rows of the reference's rows, K = E); the
+    # quantisation's zero rows must give exactly 0
+    rows = pk["rows"]
+    zero_columns_stage("qkv", st["qkv"], rows)
     A = fp8_refs.dequantize(_e4m3(st["xn1"]), st["xs1"], 1)
-    W = fp8_refs.dequantize(_e4m3(pk["q_qkv"]), pk["s_qkv"], 128)
-    y, absdot = kr.qkv_ref(A, W, pk["b_qkv"], 0.125, E, T, cos, sin)
+    W = fp8_refs.dequantize(_e4m3(pk["q_qkv"]), pk["s_qkv"], 128)[rows]
+    y, absdot = kr.qkv_ref_heads(A, W, pk["b_qkv"][rows], q_scale(E // H), H, T, cos, sin)
     acc = absdot * (2.0 ** -11 + 2.0 ** -24 * math.ceil(E / 128))
-    _worst(worst, "qkv", _ratio((st["qkv"].double() - y).abs(), acc + 6 * kr.U32 * y.abs() + kr.f16_bound(y)))
-    del A, W, y, absdot, acc
-    attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs)
-    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], E, False)
+    got = st["qkv"][:, rows].double()
+    _worst(worst, "qkv", _ratio((got - y).abs(), acc + 6 * kr.U32 * y.abs() + kr.f16_bound(y)))
+    del A, W, y, absdot, acc, got
+    zero_columns_stage("ctx", st["ctx"], pk["cols"])
+    attention_stage_f16(worst, st["qkv"], st["ctx"], pad, B, T, H, probs, key_blocks(pk["slots"]), slots=pk["slots"])
+    residual_stage(worst, "out_proj", st["ctx"], pk["w_out"], a.out_proj.bias, st["x0"], st["x1"], pk["Ea"], False)
     A = fp8_refs.dequantize(_e4m3(st["xn2"]), st["xs2"], 1)
     W = fp8_refs.dequantize(_e4m3(pk["q_fc1"]), pk["s_fc1"], 128)
     ref = A @ W.t() + layer.fc1.bias.double()
@@ -495,10 +571,10 @@ def check_axial_stages(layer, pk: Dict, st: Dict, pad: Optional[torch.Tensor], B
     ln_stage(worst, "ffn_ln", st["x_col"], layer.feed_forward_layer.layer_norm, st["ffn_xn"], split)
     zero = pad.reshape(-1) if pad is not None else None
     w_sub = {}
-    qkv_stage(w_sub, st["row_xn"], pk["row_qkv"], pk["row_b"], st["row_qkv"], E, q_scale(64, R), 1, None, None,
+    qkv_stage(w_sub, st["row_xn"], pk["row_qkv"], pk["row_b"], st["row_qkv"], E, H, q_scale(64, R), 1, None, None,
               split, zero)
     _worst(worst, "row_qkv", w_sub.pop("qkv"))
-    qkv_stage(w_sub, st["col_xn"], pk["col_qkv"], pk["col_b"], st["col_qkv"], E, q_scale(64), 1, None, None, split)
+    qkv_stage(w_sub, st["col_xn"], pk["col_qkv"], pk["col_b"], st["col_qkv"], E, H, q_scale(64), 1, None, None, split)
     _worst(worst, "col_qkv", w_sub.pop("qkv"))
     # tied row attention on its own (q-zeroed) q, k, v
     key_pad = pad[:, 0] if pad is not None else None

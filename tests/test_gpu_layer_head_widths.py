@@ -75,13 +75,16 @@ def check_layer(d, precision, T, lengths, gates=None):
     return r, pa
 
 
-@pytest.mark.parametrize("E,H,precision,message", [
+REFUSED_WIDTHS = [
     (240, 16, 0, b"even head_dim <= 128"),                 # d = 15
     (1040, 8, 0, b"even head_dim <= 128"),                 # d = 130
     (40, 5, 0, b"multiple of 16"),                         # d = 8, E % 16 = 8
     (576, 8, 1, b"not available for head_dim > 64"),       # d = 72 in fp32x3
     (480, 20, 1, b"embed_dim % 64 == 0"),                  # d = 24, E % 64 = 32 in fp32x3
-])
+]
+
+
+@pytest.mark.parametrize("E,H,precision,message", REFUSED_WIDTHS)
 def test_layer_create_refuses_unsupported_widths(E, H, precision, message):
     from esm_b200 import _lib
     lib = _lib.load()
@@ -95,3 +98,26 @@ def test_layer_create_refuses_unsupported_widths(E, H, precision, message):
     assert lib.esmb200_layer_create(ctypes.byref(w), stream, ctypes.byref(out)) == -1
     assert message in lib.esmb200_last_error(), lib.esmb200_last_error()
     assert not out.value and lib.esmb200_launch_count() == before
+
+
+@pytest.mark.parametrize("E,H,precision,message", REFUSED_WIDTHS + [
+    (320, 20, 3, b"precision must be 0"),
+    (320, 20, 2, b"needs a_scales and w_scales"),          # scales not given
+    (320, 20, 0, b"rope tables must be given together"),   # cos without sin
+])
+def test_gemm_qkv_heads_refuses_what_layer_create_refuses(E, H, precision, message):
+    """esmb200_gemm_qkv_heads refuses the widths and precisions esmb200_layer_create refuses, with its messages, before
+    any launch and without reading an operand (the pointers below are not device memory)"""
+    from esm_b200 import _lib
+    lib = _lib.load()
+    torch.cuda.init()
+    fake = ctypes.c_void_p(256)
+    scales = None if message == b"needs a_scales and w_scales" else fake
+    sin = None if message == b"rope tables must be given together" else fake
+    before = lib.esmb200_launch_count()
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    rc = lib.esmb200_gemm_qkv_heads(precision, fake, scales, fake, scales, fake, fake, 128, E, H, 0.125, fake, sin, 16,
+                                    stream)
+    assert rc == -1
+    assert message in lib.esmb200_last_error(), lib.esmb200_last_error()
+    assert lib.esmb200_launch_count() == before

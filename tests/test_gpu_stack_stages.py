@@ -78,8 +78,9 @@ def replay_stack(layers, x0, pad, T, cos, sin, precision, reprs, attn, stages, l
                  zero_pad_rows=False):
     """Replays the stack layer by layer from x0 [B,T,E]; asserts each layer's output equals reprs[i] and the
     probabilities of the layers in attn equal the stack's, bit for bit (zero_pad_rows: the stack wrote the rows of padded
-    query tokens as zeros); with stages, checks every stage against float64 and prints one PARITY line per stage with
-    the worst ratio over the layers.  Returns the replayed final stream."""
+    query tokens as zeros); with stages (True: every layer, or a collection of layer indices), checks every stage of
+    those layers against float64 and prints one PARITY line per stage with the worst ratio over the layers.  Returns the
+    replayed final stream."""
     B, _, E = x0.shape
     H = layers[0].attention_heads
     M = B * T
@@ -95,9 +96,10 @@ def replay_stack(layers, x0, pad, T, cos, sin, precision, reprs, attn, stages, l
         st = sr.replay_esm(layer, pk, x, pad8, B, T, cos, sin, precision, probs)
         if contacts is not None:
             contacts(i, probs)
-        if stages and precision == 2:
+        check_here = stages is True or (stages and i in stages)
+        if check_here and precision == 2:
             sr.check_fp8_stages(layer, pk, st, pad, B, T, cos, sin, worst, probs if i in attn else None)
-        elif stages:
+        elif check_here:
             sr.check_esm_stages(layer, pk, st, pad, B, T, cos, precision, worst, probs if i in attn else None, sin)
         assert torch.equal(x, reprs[i].view(M, E)), f"{label}: layer {i} output differs from the replay"
         if i in attn:
@@ -259,14 +261,19 @@ def test_split_stack_contacts_against_replay():
 
 # ---- ESM2.forward: the LM head and the final LayerNorm --------------------------------------------------------------
 def test_forward_lm_head_against_replay():
+    check_forward_lm_head("650M", 4, 1280, 20, seed=23)
+
+
+def check_forward_lm_head(label, L_, E, H, seed):
+    """ESM2.forward on three ragged sequences of up to 512 tokens against a replay of its layers and of the LM-head
+    chain, bit for bit, and each stage of the chain against float64"""
     from esm_b200 import ESM2
     from oracle.weights import make_state_dict, make_tokens
-    L_, E, H = 4, 1280, 20
-    sd = make_state_dict(L_, E, H, seed=23)
+    sd = make_state_dict(L_, E, H, seed=seed)
     model = ESM2(num_layers=L_, embed_dim=E, attention_heads=H)
     model.load_state_dict(sd, strict=True)
     model = model.eval().cuda()
-    tokens = make_tokens([510, 301, 77], 512, seed=24, n_mask=3).cuda()
+    tokens = make_tokens([510, 301, 77], 512, seed=seed + 1, n_mask=3).cuda()
     out = model(tokens, repr_layers=[L_])
     B, T = tokens.shape
     M = B * T
@@ -315,9 +322,9 @@ def test_forward_lm_head_against_replay():
     want, b = sr._ln_want(x_pre, ln)
     worst["final_ln"] = sr._ratio((xv.double() - want).abs(), b + kr.U32 * want.abs())
     for name, r in worst.items():
-        report(f"stack stage lm_head {name}", worst=r)
+        report(f"stack stage lm_head {label} {name}", worst=r)
     for name, r in worst.items():
-        assert r <= 1.0, (name, r)
+        assert r <= 1.0, (label, name, r)
 
 
 # ---- MSA Transformer ------------------------------------------------------------------------------------------------

@@ -15,7 +15,11 @@
   * the embedding references give the oracles' embeddings (oracle.esm2_oracle.embed, the embedding lines of
     oracle.msa_oracle.msa_transformer_forward, its representation 0), positions a hand-written example, mean_pool64 and
     log_softmax64 torch's float64 results, contact_stripes the reference contact head, and layer64 the oracle's layer;
-    torch's fp32 log-softmax stays inside log_softmax_bound and a row summed over its first 32 columns only does not."""
+    torch's fp32 log-softmax stays inside log_softmax_bound and a row summed over its first 32 columns only does not;
+  * heads in 64-wide slots at widths 8 .. 128: the replay's slot map is elementwise.cuh's head_slot and inverts; the
+    kernel's (c, c + 32) rotation on the packed heads is the reference's rotate-half; qkv_ref_heads is qkv_ref at
+    d = 64; an fp32 restatement of the QKV epilogue stays inside qkv_bound, and a neighbouring table column or a pair in
+    the head's other slot leaves it."""
 import math
 
 import numpy as np
@@ -816,3 +820,140 @@ def test_replay_q_scales_are_the_references_fp32_values():
     assert old == [6, 18, 24, 28, 34, 58, 68, 72, 78, 82, 84, 94, 96, 102, 112, 122]
     rows = [R for R in range(1, 1025) if sr.q_scale(64, R) != float(np.float32(0.125) / np.sqrt(np.float32(R)))]
     assert len(rows) == 242 and rows[:3] == [6, 7, 17]
+
+
+# ---- heads in 64-wide slots at any head width (tests/stack_replay.py pack_esm, qkv_stage) ---------------------------
+# every width tests/test_gpu_stack_head_widths.py and the stage tests run, and widths that fill a slot partly (8, 40) or
+# the second slot partly (66: one pair, 126: thirty-one)
+SLOT_WIDTHS = [16, 24, 32, 64, 128, 8, 40, 66, 126]
+SLOT_H = 3
+
+
+def _slot_tables(d, T, dtype):
+    """the reference's [T, d/2] tables (rotary_embedding.py:47-61) and the replay's [T, 32 slots] widening of them"""
+    import stack_replay as sr
+    inv = 1.0 / (10000 ** (torch.arange(0, d, 2, dtype=torch.float64) / d))
+    f = torch.arange(T, dtype=torch.float64)[:, None] * inv[None]
+    cos, sin = f.cos().to(dtype), f.sin().to(dtype)
+    return (cos, sin) + sr.rope_slots(cos, sin, kr.head_slots(d * SLOT_H, SLOT_H))
+
+
+def _slot_rotate(z, E, H, cos_s, sin_s, T):
+    """the QKV epilogue's rotation (csrc/gemm_common.cuh epi_qkv_box) on a head-slot tensor z [M, 3Ea]: columns
+    (c, c + 32) of every 64-wide group of q and k rotated by column 32 (group mod slots) + c of the [T, 32 slots] table"""
+    slots = kr.head_slots(E, H)
+    Ea = 64 * slots * H
+    t = torch.arange(z.shape[0]) % T
+    z = z.clone()
+    for g0 in range(0, 2 * Ea, 64):
+        s = (g0 // 64) % slots
+        c, sn = cos_s[t][:, 32 * s:32 * s + 32], sin_s[t][:, 32 * s:32 * s + 32]
+        x1, x2 = z[:, g0:g0 + 32].clone(), z[:, g0 + 32:g0 + 64].clone()
+        z[:, g0:g0 + 32], z[:, g0 + 32:g0 + 64] = x1 * c - x2 * sn, x2 * c + x1 * sn
+    return z
+
+
+def _pack_cols(y, rows, Ea3):
+    z = torch.zeros(y.shape[0], Ea3, dtype=y.dtype)
+    z[:, rows] = y
+    return z
+
+
+@pytest.mark.parametrize("d", SLOT_WIDTHS)
+def test_slot_map_is_the_head_slot_map_and_round_trips(d):
+    """slot_columns, derived from the rotate-half pairing, is the map fp8_refs.head_slot states (elementwise.cuh
+    head_slot); it is one to one into [0, Ea), and unpacking through slot_rows inverts packing, leaving 3 (Ea - E) padding
+    columns that hold zeros"""
+    import fp8_refs
+    import stack_replay as sr
+    H = SLOT_H
+    E = d * H
+    Ea = 64 * kr.head_slots(E, H) * H
+    cols = kr.slot_columns(d, H)
+    assert torch.equal(cols, fp8_refs.head_slot(torch.arange(E), d))
+    assert cols.unique().numel() == E and int(cols.min()) >= 0 and int(cols.max()) < Ea
+    rows = kr.slot_rows(d, H)
+    y = torch.randn(7, 3 * E, dtype=torch.float64, generator=torch.Generator().manual_seed(d))
+    z = _pack_cols(y, rows, 3 * Ea)
+    assert torch.equal(z[:, rows], y)
+    pad = sr.padding_columns(rows, 3 * Ea)
+    assert int(pad.sum()) == 3 * (Ea - E) and bool((z[:, pad] == 0).all())
+    assert torch.equal(_pack_cols(z[:, rows], rows, 3 * Ea), z)
+
+
+@pytest.mark.parametrize("d", SLOT_WIDTHS)
+def test_slot_rotation_is_the_reference_rotate_half(d):
+    """the kernel's (c, c + 32) rotation by table column 32 slot + c on the packed heads, unpacked, equals the oracle's
+    rotate-half on every q and k head bit for bit in float64 (and qkv_ref_heads' rotation); v and the padding columns
+    (rotated by the replay's padding values) stay as they were"""
+    import stack_replay as sr
+    from oracle import esm2_oracle
+    H, T = SLOT_H, 40
+    E = d * H
+    Ea = 64 * kr.head_slots(E, H) * H
+    cos, sin, cos_s, sin_s = _slot_tables(d, T, torch.float64)
+    rows = kr.slot_rows(d, H)
+    M = 2 * T
+    y = torch.randn(M, 3 * E, dtype=torch.float64, generator=torch.Generator().manual_seed(d + 1))
+    z = _slot_rotate(_pack_cols(y, rows, 3 * Ea), E, H, cos_s, sin_s, T)
+    t = torch.arange(M) % T
+    want = y.clone()
+    for sec in range(2):
+        x = y[:, sec * E:(sec + 1) * E].view(M, H, d)
+        want[:, sec * E:(sec + 1) * E] = esm2_oracle.apply_rope(x, cos[t][:, None], sin[t][:, None]).reshape(M, E)
+    assert torch.equal(z[:, rows], want)
+    assert bool((z[:, sr.padding_columns(rows, 3 * Ea)] == 0).all())
+    # qkv_ref_heads' rotation: an identity weight and zero bias pass y through the GEMM exactly
+    got, _ = kr.qkv_ref_heads(y, torch.eye(3 * E, dtype=torch.float64), torch.zeros(3 * E, dtype=torch.float64), 1.0,
+                              H, T, cos, sin)
+    assert torch.equal(got, want)
+
+
+def test_qkv_ref_heads_is_qkv_ref_at_d64():
+    from esm_b200.model import rope_tables
+    T, H = 32, 3
+    E = 64 * H
+    a, w, bias = _fp16_operands(2 * T, 3 * E, E, 8)
+    inv = 1.0 / (10000 ** (torch.arange(0, 64, 2).float() / 64))
+    cos, sin = rope_tables(inv, T)
+    y0, d0 = kr.qkv_ref(a, w, bias, 0.125, E, T, cos, sin)
+    y1, d1 = kr.qkv_ref_heads(a, w, bias, 0.125, H, T, cos, sin)
+    assert torch.equal(y0, y1) and torch.equal(d0, d1)
+
+
+def _emulate_qkv(a, w, bias, d, H, T, cos_s, sin_s, cols):
+    """the QKV GEMM and epilogue restated in fp32 on weights packed by the column map `cols` ([E] -> [0, Ea)): bias,
+    q scale fp32(d ** -0.5), the slot rotation, fp16 output; returns the output read back through the same map"""
+    import stack_replay as sr
+    E = d * H
+    Ea = 64 * kr.head_slots(E, H) * H
+    rows = torch.cat([s * Ea + cols for s in range(3)])
+    ws = torch.zeros(3 * Ea, E)
+    ws[rows] = w.float()
+    bs = torch.zeros(3 * Ea)
+    bs[rows] = bias.float()
+    y = a.float() @ ws.t() + bs
+    y[:, :Ea] *= sr.q_scale(d)
+    return _slot_rotate(y, E, H, cos_s, sin_s, T).half()[:, rows]
+
+
+@pytest.mark.parametrize("d", SLOT_WIDTHS)
+def test_qkv_heads_bound_holds_and_refuses_a_wrong_slot_or_table_column(d):
+    """the fp32 restatement stays inside qkv_bound around qkv_ref_heads (K = E); rotating every pair by the neighbouring
+    table column leaves it, and at two slots per head (d > 64) so does a map that sends each pair to the head's other
+    slot"""
+    import stack_replay as sr
+    H, T = SLOT_H, 48
+    E = d * H
+    a, w, bias = _fp16_operands(2 * T, 3 * E, E, d + 2)
+    cos, sin, cos_s, sin_s = _slot_tables(d, T, torch.float32)
+    want, absdot = kr.qkv_ref_heads(a, w, bias, sr.q_scale(d), H, T, cos, sin)
+    b = kr.qkv_bound(want, absdot, E)
+    ratio = lambda got: float((got.double() - want).abs().div(b).max())  # noqa: E731
+    cols = kr.slot_columns(d, H)
+    assert ratio(_emulate_qkv(a, w, bias, d, H, T, cos_s, sin_s, cols)) <= 1.0
+    shifted = lambda t: torch.cat([t[:, 1:], t[:, -1:]], 1)  # noqa: E731  column p reads column p + 1
+    assert ratio(_emulate_qkv(a, w, bias, d, H, T, shifted(cos_s), shifted(sin_s), cols)) > 10
+    if kr.head_slots(E, H) == 2:
+        other = cols + torch.where((cols // 64) % 2 == 0, 64, -64)  # the head's other slot, same columns
+        assert ratio(_emulate_qkv(a, w, bias, d, H, T, cos_s, sin_s, other)) > 10
