@@ -67,7 +67,7 @@ EXPORTS = (
     "esmb200_stack_contacts",
 )
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32, EPI_GELU_FP8 = range(6)
 
 
@@ -188,8 +188,8 @@ def _declare(lib):
     lib.esmb200_axial_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32]
     lib.esmb200_axial_stack_forward.restype = c_int32
     lib.esmb200_axial_stack_forward.argtypes = [POINTER(c_void_p), POINTER(c_void_p), c_int32, c_void_p, c_void_p,
-                                                c_void_p, c_int32, c_int32, c_int32, POINTER(c_void_p), c_void_p,
-                                                c_size_t, c_void_p]
+                                                c_void_p, c_int32, c_int32, c_int32, POINTER(c_void_p),
+                                                POINTER(c_void_p), c_void_p, c_size_t, c_void_p]
     lib.esmb200_msa_embed.restype = c_int32
     lib.esmb200_msa_embed.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_float,
                                       c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]

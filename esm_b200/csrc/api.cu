@@ -351,16 +351,19 @@ int run_contact_accumulate(const float* attn, long long batch_stride, const floa
 // MSA column attention (axial_attention.py:182-239) straight from the row-major qkv [B*R*C, 3E]: one "sequence" of R
 // tokens per alignment column, read with strided TMA boxes (qkv viewed as [B*R, C*3E], AttnParams::cols), no
 // regrouping copy.  s holds the key bits of the B*C column sequences.  split (fp32x3): qkv [B*R*C, 6E] (viewed as
-// [B*R, C*6E], lo halves 3E to the right), ctx [B*R*C, 2E].
+// [B*R, C*6E], lo halves 3E to the right), ctx [B*R*C, 2E].  probs: optional fp32 [B*C, H, R, R], written from the
+// same strided view with the row statistics of the forward kernel (the caller checks B*C*H <= 65535); ctx is the same
+// with and without it.
 int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B, int R, int C, int H,
-                         cudaStream_t st, bool split = false) {
+                         cudaStream_t st, bool split = false, float* probs = nullptr) {
   const int E = H * 64;
   AttnParams ap;
   ap.B = B * C; ap.T = R; ap.H = H; ap.E = E;
   ap.lo_off = split ? 3 * E : 0;
   ap.keybits = s.keybits; ap.kvlen = s.kvlen; ap.words = s.words;
   ap.ctx = static_cast<__half*>(ctx);
-  ap.row_max = nullptr; ap.row_sum = nullptr;
+  ap.row_max = probs ? s.row_max : nullptr;
+  ap.row_sum = probs ? s.row_sum : nullptr;
   ap.cols = C;
   CUtensorMap tq, tkv;
   const uint64_t wide = (uint64_t)C * (split ? 6 : 3) * E;  // token r of column c at row r, x = c*3E (split: c*6E)
@@ -373,6 +376,21 @@ int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B
     e = launch_attention_fwd(tq, tkv, ap, num_sms(), st);
   }
   if (e != cudaSuccess) return fail_cuda(e, "column attention launch");
+  if (probs) {
+    ProbsParams pp;
+    pp.B = B * C; pp.T = R; pp.H = H; pp.E = E;
+    pp.keybits = s.keybits; pp.kvlen = s.kvlen; pp.words = s.words;
+    pp.row_max = s.row_max; pp.row_sum = s.row_sum; pp.probs = probs;
+    pp.batch_stride = (long long)H * R * R;
+    pp.zero_pad_rows = 0;
+    pp.lo_off = ap.lo_off;
+    pp.cols = C;
+    {
+      ProfScope ps(T_PROBS, st);
+      e = launch_attention_probs(tq, pp, st);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "column attention probs launch");
+  }
   return ESMB200_OK;
 }
 
@@ -1423,8 +1441,8 @@ size_t esmb200_axial_workspace_bytes_split(int32_t E, int32_t F, int32_t B, int3
 // sum of the kernel times and the wall time are not host launch overhead, so the calls stay plain stream launches.)
 int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer* const* col_layers, int32_t n_layers,
                                 float* x, const uint8_t* pad_mask, const uint8_t* col_pad_mask, int32_t B, int32_t R,
-                                int32_t C, float* const* row_attn_out, void* workspace, size_t workspace_bytes,
-                                void* stream) {
+                                int32_t C, float* const* row_attn_out, float* const* col_attn_out, void* workspace,
+                                size_t workspace_bytes, void* stream) {
   if (!row_layers || !col_layers || n_layers <= 0 || !x || !workspace) return fail(ESMB200_EINVAL, "null argument");
   if (B <= 0 || R <= 0 || C <= 0) return fail(ESMB200_EINVAL, "empty alignment");
   if ((pad_mask == nullptr) != (col_pad_mask == nullptr))
@@ -1453,6 +1471,9 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C, split);
   if (workspace_bytes < aw.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   if (E != 64 * H) return fail(ESMB200_EINVAL, "the MSA axial path needs head_dim 64");
+  for (int i = 0; col_attn_out && i < n_layers; ++i)
+    if (col_attn_out[i] && (long long)B * C * H > 65535)
+      return fail(ESMB200_EINVAL, "column attention maps: B*C*H must be <= 65535");
   const int M = B * R * C;
   const Workspace& ws = aw.ws;
   ActMaps am;
@@ -1480,7 +1501,10 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
     // column attention (modules.py:208-212; axial_attention.py:182-239)
     if (!rc)
       rc = attention_block(col_layers[i], col_layers[i]->tm, x, M, 1, nullptr, nullptr, col_layers[i]->q_scale, ws, am,
-                           st, [&] { return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st, split != 0); });
+                           st, [&] {
+                             return run_column_attention(ws.qkv, ws.ctx, ws.as, B, R, C, H, st, split != 0,
+                                                         col_attn_out ? col_attn_out[i] : nullptr);
+                           });
     // feed-forward (modules.py:213-214)
     if (!rc) rc = ffn_block(col_layers[i], col_layers[i]->tm, x, M, ws, am, st);
     if (rc) return rc;

@@ -22,6 +22,7 @@ struct ProbsParams {
   int zero_pad_rows;  // 1: rows of padded query tokens are written as zeros (ESM2.forward's stacked result)
   int lo_off;         // fp32x3 precision: column offset of the lo halves in qkv [M, 6E] (0 = plain fp16 operands)
   int slots = 1;      // 2: head_dim <= 128, a head is two adjacent 64-wide column slots (E = H * 128)
+  int cols = 1;       // sequence b = (b / cols, b % cols) of a [B/cols, T, cols, 3E] qkv (fp32x3: 6E), as AttnParams::cols
 };
 
 namespace probs_cfg {
@@ -47,7 +48,8 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const Probs
   const int kb = blockIdx.x, qb = blockIdx.y;
   const int b = blockIdx.z / p.H, h = blockIdx.z % p.H;
   const int q0 = qb * BLOCK_Q, k0 = kb * BLOCK_KV;
-  const int row_base = b * p.T;
+  const int row_base = (b / p.cols) * p.T;
+  const int x0 = (b % p.cols) * (MODE == 1 ? 6 : 3) * p.E;  // MODE 1: a token's qkv is 6E wide (hi | lo)
 
   if (threadIdx.x == 0) {
     mbar_init(ld_full, 1);
@@ -64,7 +66,7 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const Probs
   if (live) {
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(ld_full, 2 * NP * TILE_BYTES);
-      const int hc = h * HEAD_DIM * (MODE == 2 ? 2 : 1), po = MODE == 2 ? HEAD_DIM : p.lo_off;
+      const int hc = x0 + h * HEAD_DIM * (MODE == 2 ? 2 : 1), po = MODE == 2 ? HEAD_DIM : p.lo_off;
 #pragma unroll
       for (int part = 0; part < NP; ++part) {
         tma_load_2d(smem_q + part * TILE_BYTES, &tmap_qkv, ld_full, hc + part * po, row_base + q0);

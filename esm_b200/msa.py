@@ -10,21 +10,20 @@ CUDA path for BASELINE.json configs[4] (SURVEY §8f #3).  All the arithmetic of 
     contraction over K = R*64 that walks the alignment rows with TMA boxes taken straight from the projection output,
     a row softmax (with the reference's -10000 fill on padded key columns), and the P.V update with V tiles as the
     MN-major operand (csrc/tied_attention.cuh);
-  * column attention: esmb200_column_attention — the flash-attention kernel with strided TMA boxes, one "sequence" of
-    R rows per alignment column, no regrouping copy (csrc/attention8.cuh, AttnParams::cols).
-PyTorch is used for the buffers, for zeroing q at padded positions (axial_attention.py:82-85, one masked_fill_) and, only
-when the column attention MAPS are requested, for regrouping qkv column-major.
+  * column attention: the flash-attention kernel with strided TMA boxes, one "sequence" of R rows per alignment column,
+    no regrouping copy (csrc/attention8.cuh, AttnParams::cols); when the maps are asked for, the probability kernel
+    writes them from the same strided view (csrc/attention_probs.cuh, ProbsParams::cols).
+The layers run in one esmb200_axial_stack_forward call, with or without attention maps; PyTorch only holds the buffers.
 
 Padding: the reference fills padded keys with -10000, this path gives them probability exactly 0 in the column
 attention — identical unless every key of a column is padded (there the reference averages v uniformly, this path
 returns 0); such positions are themselves padding.  head_dim 64, inference only.
 
 Precision: fp16 MMA operands by default; `MSATransformer.set_precision("fp32x3")` runs every GEMM and attention operand
-of the axial stack and the LM head as an fp16 hi | lo pair (the _split entry points; DESIGN.md section 4).
+of the axial stack and the LM head as an fp16 hi | lo pair (DESIGN.md section 4).
 """
 from __future__ import annotations
 
-import math
 from typing import Optional
 
 import torch
@@ -32,7 +31,7 @@ import torch.nn as nn
 
 import ctypes
 from argparse import Namespace
-from typing import Dict, List, Sequence, Union
+from typing import Dict, Sequence, Union
 
 from . import _lib
 from .alphabet import Alphabet
@@ -68,34 +67,6 @@ class _ResidualBlock(nn.Module):
         self.layer_norm = nn.LayerNorm(embed_dim)
 
 
-def _gemm(epi: int, a16: torch.Tensor, w16: torch.Tensor, bias: torch.Tensor, out: torch.Tensor,
-          split: bool = False) -> None:
-    """split (fp32x3): a16 [M,2K] and w16 [N,2K] are hi | lo halves along K (esmb200_gemm_split)."""
-    M, K = a16.shape
-    N = w16.shape[0]
-    lib = _lib.load()
-    gemm = lib.esmb200_gemm_split if split else lib.esmb200_gemm_f16
-    _lib.check(gemm(epi, _ptr(a16), _ptr(w16), _ptr(bias), _ptr(out), M, N, K // 2 if split else K, None, None, 0, 0,
-                    _stream()))
-
-
-def _ln16(x: torch.Tensor, ln: nn.LayerNorm, out16: torch.Tensor, split: bool = False) -> None:
-    """LayerNorm -> fp16 [M,E], or with split the fp32x3 hi | lo halves [M,2E]."""
-    M, E = x.shape
-    lib = _lib.load()
-    fn = lib.esmb200_layernorm_split if split else lib.esmb200_layernorm_f16
-    _lib.check(fn(_ptr(x), _ptr(ln.weight), _ptr(ln.bias), _ptr(out16), M, E, ln.eps, _stream()))
-
-
-def _split16(w: torch.Tensor) -> torch.Tensor:
-    """fp32 [N,K] -> fp16 [N,2K] hi | lo (esmb200_convert_split), the fp32x3 form of a GEMM weight."""
-    w = w.detach().float().contiguous()
-    N, K = w.shape
-    out = torch.empty((N, 2 * K), dtype=torch.float16, device=w.device)
-    _lib.check(_lib.load().esmb200_convert_split(_ptr(w), _ptr(out), N, K, _stream()))
-    return out
-
-
 class AxialTransformerLayer(nn.Module):
     """Drop-in for esm.modules.AxialTransformerLayer (modules.py:145-221) at inference."""
 
@@ -111,8 +82,6 @@ class AxialTransformerLayer(nn.Module):
         self.row_self_attention = _ResidualBlock(_AttnParams(embedding_dim, num_attention_heads), embedding_dim)
         self.column_self_attention = _ResidualBlock(_AttnParams(embedding_dim, num_attention_heads), embedding_dim)
         self.feed_forward_layer = _ResidualBlock(_FFNParams(embedding_dim, ffn_embedding_dim), embedding_dim)
-        self._packed = None
-        self._packed_key = None
         self._handles = None
         self._handles_key = None
         self.precision = 0  # 0 = fp16 MMA operands, 1 = "fp32x3" (esmb200.h: esmb200_layer_weights.precision)
@@ -171,30 +140,6 @@ class AxialTransformerLayer(nn.Module):
         except Exception:
             pass
 
-    # ---- GEMM operand copies: fp16, or fp32x3 hi | lo halves (re-made when a parameter or the precision changes) ----
-    def _pack(self):
-        ps = list(self.parameters())
-        key = (self.precision,) + tuple((p.data_ptr(), p._version) for p in ps)
-        if self._packed is None or key != self._packed_key:
-            if self.precision:
-                op = _split16
-            else:
-                def op(w):
-                    return w.detach().half().contiguous()
-
-            def qkv(a):
-                w = op(torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], 0))
-                b = torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias], 0).detach().float().contiguous()
-                return w, b
-            row, col, ffn = self.row_self_attention.layer, self.column_self_attention.layer, self.feed_forward_layer.layer
-            self._packed = {
-                "row_qkv": qkv(row), "col_qkv": qkv(col),
-                "row_out": op(row.out_proj.weight), "col_out": op(col.out_proj.weight),
-                "fc1": op(ffn.fc1.weight), "fc2": op(ffn.fc2.weight),
-            }
-            self._packed_key = key
-        return self._packed
-
     @torch.no_grad()
     def forward(self, x: torch.Tensor, self_attn_mask: Optional[torch.Tensor] = None,
                 self_attn_padding_mask: Optional[torch.Tensor] = None, need_head_weights: bool = False):
@@ -212,99 +157,27 @@ class AxialTransformerLayer(nn.Module):
             return out, col_probs, row_probs
         return out
 
-    def _qkv(self, xn: torch.Tensor, w: torch.Tensor, b: torch.Tensor, qkv: torch.Tensor, M: int, E: int,
-             q_scale: float) -> None:
-        """The q/k/v projection without rotary embedding, q columns scaled by q_scale (axial_attention.py:79-81,
-        199-202): qkv [M,3E] fp16, or [M,6E] hi | lo with fp32x3."""
-        lib = _lib.load()
-        if self.precision:
-            _lib.check(lib.esmb200_gemm_qkv_split(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, q_scale, _stream()))
-        else:
-            _lib.check(lib.esmb200_gemm_qkv_f16(_ptr(xn), _ptr(w), _ptr(b), _ptr(qkv), M, E, q_scale, None, None, 0,
-                                                _stream()))
-
     @torch.no_grad()
     def forward_batch_major(self, xb: torch.Tensor, padding_mask: Optional[torch.Tensor] = None,
                             need_probs: bool = False):
         """In-place layer on the batch-major residual stream xb [B,R,C,E] fp32 (what MSATransformer keeps between
-        layers).  padding_mask [B,R,C] bool or None.  Returns (row_attn [H,B,C,C], column_attn [H,C,B,R,R]) or
-        (None, None).  Without attention maps this is one esmb200_axial_stack_forward call; with them the sub-layers
-        are driven one C-ABI call at a time so that the column-attention maps can be produced too.  With precision 1
-        (fp32x3) every GEMM / attention operand below is an fp16 hi | lo pair, twice as wide."""
+        layers), one esmb200_axial_stack_forward call.  padding_mask [B,R,C] bool or None.  Returns (row_attn
+        [H,B,C,C], column_attn [H,C,B,R,R]), the reference's layouts (axial_attention.py:87,206), or (None, None)."""
         if not need_probs:
             run_axial_stack([self], xb, padding_mask)
             return None, None
-        lib = _lib.load()
-        B, R, C, E = xb.shape
-        H, d, Fd = self.num_heads, 64, self.ffn_embedding_dim
-        M = B * R * C
-        dev = xb.device
-        split = bool(self.precision)
-        pf = 2 if split else 1
-        pk = self._pack()
-        x2 = xb.view(M, E)
-        xn = torch.empty((M, pf * E), dtype=torch.float16, device=dev)
-        qkv = torch.empty((M, pf * 3 * E), dtype=torch.float16, device=dev)
-        ctx = torch.empty((M, pf * E), dtype=torch.float16, device=dev)
-        key_pad = col_pad = None
-        if padding_mask is not None:
-            pm = padding_mask.to(device=dev, dtype=torch.bool)
-            key_pad = pm[:, 0].contiguous().to(torch.uint8)                    # [B,C]   axial_attention.py:94-97
-            col_pad = pm.permute(0, 2, 1).contiguous().to(torch.uint8)         # [B*C,R] axial_attention.py:212-215
-        with torch.cuda.device(dev):
-            # ================= tied row attention (axial_attention.py:71-111) =================
-            blk = self.row_self_attention
-            _ln16(x2, blk.layer_norm, xn, split)
-            w, b = pk["row_qkv"]
-            self._qkv(xn, w, b, qkv, M, E, (d ** -0.5) / math.sqrt(R))
-            if padding_mask is not None:  # q (both halves with fp32x3) zeroed at padded positions (:82-85)
-                q5 = qkv.view(B, R, C, 3 * pf, E)
-                q5[:, :, :, 0].masked_fill_(pm[..., None], 0)
-                if split:
-                    q5[:, :, :, 3].masked_fill_(pm[..., None], 0)
-            row_probs = torch.empty((H, B, C, C), dtype=torch.float32, device=dev)
-            if split:
-                nbytes = lib.esmb200_tied_row_attention_split_scratch_bytes(B, C, H)
-                tied = lib.esmb200_tied_row_attention_split
-            else:
-                nbytes = lib.esmb200_tied_row_attention_scratch_bytes(B, C, H)
-                tied = lib.esmb200_tied_row_attention
-            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _lib.check(tied(_ptr(qkv), _ptr(key_pad), _ptr(ctx), _ptr(row_probs), B, R, C, H, _ptr(scratch), nbytes,
-                            _stream()))
-            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["row_out"], blk.layer.out_proj.bias, x2, split)     # :110 + residual
-
-            # ================= column attention (axial_attention.py:182-222) =================
-            blk = self.column_self_attention
-            _ln16(x2, blk.layer_norm, xn, split)
-            w, b = pk["col_qkv"]
-            self._qkv(xn, w, b, qkv, M, E, d ** -0.5)
-            scratch = torch.empty(lib.esmb200_attention_scratch_bytes(B * C, R), dtype=torch.uint8, device=dev)
-            # the maps are wanted: regroup qkv column-major and use the probability-writing path
-            qkv_t = qkv.view(B, R, C, pf * 3 * E).permute(0, 2, 1, 3).contiguous()             # [B*C, R, 3E] (6E)
-            ctx_t = torch.empty((B * C * R, pf * E), dtype=torch.float16, device=dev)
-            col_probs = torch.empty((B * C, H, R, R), dtype=torch.float32, device=dev)
-            attention = lib.esmb200_attention_split if split else lib.esmb200_attention
-            _lib.check(attention(_ptr(qkv_t), _ptr(col_pad), _ptr(ctx_t), _ptr(col_probs), B * C, R, H, _ptr(scratch),
-                                 _stream()))
-            ctx.view(B, R, C, pf * E).copy_(ctx_t.view(B, C, R, pf * E).permute(0, 2, 1, 3))
-            _gemm(_lib.EPI_BIAS_RESIDUAL, ctx, pk["col_out"], blk.layer.out_proj.bias, x2, split)
-
-            # ================= feed-forward (modules.py:413-418) =================
-            blk = self.feed_forward_layer
-            _ln16(x2, blk.layer_norm, xn, split)
-            hbuf = torch.empty((M, pf * Fd), dtype=torch.float16, device=dev)
-            _gemm(_lib.EPI_BIAS_GELU, xn, pk["fc1"], blk.layer.fc1.bias, hbuf, split)
-            _gemm(_lib.EPI_BIAS_RESIDUAL, hbuf, pk["fc2"], blk.layer.fc2.bias, x2, split)
-        # reference shapes: column_attn [H, C, B, R, R] (axial_attention.py:206), row_attn [H, B, C, C] (:87)
-        col_probs = col_probs.view(B, C, H, R, R).permute(2, 1, 0, 3, 4).contiguous()
-        return row_probs, col_probs
+        B, R, C, _ = xb.shape
+        col = torch.empty((B, C, self.num_heads, R, R), dtype=torch.float32, device=xb.device)
+        row = run_axial_stack([self], xb, padding_mask, (0,), {0: col})[0]
+        return row, col.permute(2, 1, 0, 3, 4).contiguous()
 
 
 def run_axial_stack(layers: Sequence[AxialTransformerLayer], xb: torch.Tensor,
-                    padding_mask: Optional[torch.Tensor] = None, row_attn_layers: Sequence[int] = ()):
+                    padding_mask: Optional[torch.Tensor] = None, row_attn_layers: Sequence[int] = (),
+                    col_attn: Optional[Dict[int, torch.Tensor]] = None):
     """esmb200_axial_stack_forward on xb [B,R,C,E] fp32 in place (msa_transformer.py:190-201's loop).
-    Returns {layer index: row attention [H,B,C,C] fp32} for the indices in row_attn_layers."""
+    Returns {layer index: row attention [H,B,C,C] fp32} for the indices in row_attn_layers.  col_attn: {layer index:
+    contiguous fp32 [B,C,H,R,R] buffer on xb's device}, filled with the column attention maps of those layers."""
     if not xb.is_cuda:
         raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
     assert xb.dtype == torch.float32 and xb.is_contiguous()
@@ -332,8 +205,13 @@ def run_axial_stack(layers: Sequence[AxialTransformerLayer], xb: torch.Tensor,
         for i in row_attn_layers:
             out[i] = torch.empty((H, B, C, C), dtype=torch.float32, device=dev)
             attns[i] = out[i].data_ptr()
+        col_ptrs = (ctypes.c_void_p * n)()
+        for i, t in (col_attn or {}).items():
+            assert t.shape == (B, C, H, R, R) and t.dtype == torch.float32 and t.is_contiguous() and t.device == dev
+            col_ptrs[i] = t.data_ptr()
         _lib.check(lib.esmb200_axial_stack_forward(rows, cols, n, _ptr(xb), _ptr(pm), _ptr(cm), B, R, C,
-                                                   attns if row_attn_layers else None, _ptr(ws), ws.numel(), _stream()))
+                                                   attns if row_attn_layers else None, col_ptrs if col_attn else None,
+                                                   _ptr(ws), ws.numel(), _stream()))
     return out
 
 
@@ -447,7 +325,8 @@ class MSATransformer(nn.Module):
             row_attentions = torch.stack([row_attn[i].permute(1, 0, 2, 3) for i in range(N)], 1)
             result["row_attentions"] = row_attentions
             if need_head_weights:
-                result["col_attentions"] = torch.stack(col_attn, 1)  # B,L,H,C,R,R
+                # B,C,H,R,R per layer -> B,L,H,C,R,R
+                result["col_attentions"] = torch.stack([col_attn[i].permute(0, 2, 1, 3, 4) for i in range(N)], 1)
             if return_contacts:
                 result["contacts"] = self.contact_head(tokens, row_attentions)
         return result
@@ -462,7 +341,7 @@ class MSATransformer(nn.Module):
         """The stack step of `forward` (msa_transformer.py:147-201): embedding prologue and the axial layers.
         Returns (tokens contiguous, x, hidden, row_attn, col_attn): x is the fp32 residual stream [B,R,C,E] BEFORE
         emb_layer_norm_after, hidden {i: representation} for the requested layers below num_layers, row_attn
-        {layer: [H,B,C,C]} and col_attn [B,H,C,R,R] per layer when the maps are asked for."""
+        {layer: [H,B,C,C]} and col_attn {layer: [B,C,H,R,R]} when the maps are asked for."""
         assert tokens.ndim == 3
         if not tokens.is_cuda:
             raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: pass tokens.cuda(); no CPU fallback")
@@ -493,26 +372,21 @@ class MSATransformer(nn.Module):
             if 0 in repr_layers:
                 hidden[0] = x.clone()
             row_attn: Dict[int, torch.Tensor] = {}
-            col_attn: List[torch.Tensor] = []
-            if need_head_weights:   # both kinds of attention maps: one sub-layer call at a time
-                for i, layer in enumerate(self.layers):
-                    rp, cp = layer.forward_batch_major(x, padding_mask, need_probs=True)
-                    row_attn[i] = rp
-                    col_attn.append(cp.permute(2, 0, 1, 3, 4))           # H,C,B,R,R -> B,H,C,R,R
-                    if (i + 1) in repr_layers and i + 1 < N:
-                        hidden[i + 1] = x.clone()
-            else:                   # whole segments of the stack per C-ABI call
-                stops = sorted({i for i in repr_layers if 0 < i < N} | {N})
-                start = 0
-                for stop in stops:
-                    idx = list(range(start, stop))
-                    got = run_axial_stack([self.layers[i] for i in idx], x, padding_mask,
-                                          list(range(len(idx))) if want_rows else ())
-                    for k, t in got.items():
-                        row_attn[start + k] = t
-                    if stop < N:
-                        hidden[stop] = x.clone()
-                    start = stop
+            col_attn = {i: torch.empty((B, C, H, R, R), dtype=torch.float32, device=dev)
+                        for i in range(N)} if need_head_weights else {}
+            # whole segments of the stack per C-ABI call, split at the requested representations
+            stops = sorted({i for i in repr_layers if 0 < i < N} | {N})
+            start = 0
+            for stop in stops:
+                idx = list(range(start, stop))
+                got = run_axial_stack([self.layers[i] for i in idx], x, padding_mask,
+                                      list(range(len(idx))) if want_rows else (),
+                                      {k: col_attn[i] for k, i in enumerate(idx)} if need_head_weights else None)
+                for k, t in got.items():
+                    row_attn[start + k] = t
+                if stop < N:
+                    hidden[stop] = x.clone()
+                start = stop
         return tokens, x, hidden, row_attn, col_attn
 
     def predict_contacts(self, tokens):

@@ -41,7 +41,7 @@ extern "C" {
 #define ESMB200_ENOMEM -3   /* device allocation failed ("CUDA out of memory ...") */
 #define ESMB200_EWORKSPACE -4 /* workspace too small */
 
-#define ESMB200_ABI_VERSION 2
+#define ESMB200_ABI_VERSION 3
 
 typedef struct esmb200_layer esmb200_layer; /* opaque: packed weights + TMA descriptors of one TransformerLayer */
 
@@ -298,7 +298,11 @@ int esmb200_column_attention(const void* qkv_f16, const uint8_t* pad_mask, void*
  *   the reference (axial_attention.py:82-97), the row attention zeroes q at every padded token, and its padded key
  *   columns are those of row 0 of each alignment (pad_mask[b, 0, :]).
  * row_attn_out: NULL, or n_layers pointers (NULL entries allowed) to fp32 [H,B,C,C] buffers (the reference's
- *   row-attention return layout, axial_attention.py:87,105). Column attention maps are not produced by this call.
+ *   row-attention return layout, axial_attention.py:87,105).
+ * col_attn_out: NULL, or n_layers pointers (NULL entries allowed) to fp32 [B*C,H,R,R] buffers: the column-attention
+ *   probabilities of alignment column c of alignment b at [b*C + c] (the reference returns them as [H,C,B,R,R],
+ *   axial_attention.py:206,216). B*C*H <= 65535 when any is given. x and the row maps are the same bits with and
+ *   without them.
  * workspace: esmb200_axial_workspace_bytes(E,F,B,R,C) bytes, or esmb200_axial_workspace_bytes_split(E,F,B,R,C) for
  *   layers created with precision = 1 (fp32x3: the activations, qkv, ctx and P are stored as fp16 hi | lo pairs).
  *   All 2 * n_layers layers must share one precision; mixed precision is ESMB200_EINVAL. */
@@ -306,8 +310,8 @@ size_t esmb200_axial_workspace_bytes(int32_t E, int32_t F, int32_t B, int32_t R,
 size_t esmb200_axial_workspace_bytes_split(int32_t E, int32_t F, int32_t B, int32_t R, int32_t C);
 int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer* const* col_layers, int32_t n_layers,
                                 float* x, const uint8_t* pad_mask, const uint8_t* col_pad_mask, int32_t B, int32_t R,
-                                int32_t C, float* const* row_attn_out, void* workspace, size_t workspace_bytes,
-                                void* stream);
+                                int32_t C, float* const* row_attn_out, float* const* col_attn_out, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* MSA Transformer embedding prologue, esm/model/msa_transformer.py:155-172 (+ LearnedPositionalEmbedding.forward,
  * esm/modules.py:241-257): x[B,R,C,E] fp32 = LayerNorm(embed_tokens[tok] + embed_positions[pos] +

@@ -26,7 +26,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/esmb200.h but not exported"
     assert sorted(_lib.EXPORTS) == declared
-    assert _lib.load().esmb200_abi_version() == 2
+    assert _lib.load().esmb200_abi_version() == 3
 
 
 def test_workspace_size_is_pure_host_arithmetic():

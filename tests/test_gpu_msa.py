@@ -30,6 +30,7 @@ def test_axial_layer_against_reference_golden(golden_dir):
     layer, _ = build(cfg["E"], cfg["F"], cfg["H"])
     out, col, row = layer(x.permute(1, 2, 0, 3).cuda(), need_head_weights=True)  # reference layout (R,C,B,E)
     assert out.shape == (cfg["R"], cfg["C"], cfg["B"], cfg["E"])
+    assert torch.equal(out, layer(x.permute(1, 2, 0, 3).cuda()))  # the maps change no bit of x
     assert rel_fro(out.permute(2, 0, 1, 3).cpu(), fx["out"]) <= 3e-3
     assert row.shape == fx["row_attn"].shape
     assert float((row.cpu() - fx["row_attn"]).abs().max()) <= 1e-2
@@ -57,9 +58,11 @@ def test_padded_msas_against_reference_golden(golden_dir):
     x = torch.randn(cfg["B"], cfg["R"], cfg["C"], cfg["E"], generator=g)
     layer, _ = build(cfg["E"], cfg["F"], cfg["H"])
     keep = ~mask
+    outs = []
     for need in (False, True):
         res = layer(x.permute(1, 2, 0, 3).cuda(), self_attn_padding_mask=mask.cuda(), need_head_weights=need)
         out = (res[0] if need else res).permute(2, 0, 1, 3).cpu()
+        outs.append(out)
         assert torch.isfinite(out).all()
         assert rel_fro(out[keep], fx["out"][keep]) <= 3e-3
         if need:
@@ -67,6 +70,7 @@ def test_padded_msas_against_reference_golden(golden_dir):
             col = res[1][:, :4].cpu()                       # [H, 4 columns, B, R, R]; columns 0-3 are not padding
             qkeep = keep[:, :, :4].permute(2, 0, 1)         # [4, B, R]: query rows that are not padding
             assert float((col - fx["col_attn_sample"]).abs()[:, qkeep].max()) <= 1e-2
+    assert torch.equal(outs[0], outs[1])  # the maps change no bit of x
 
 
 @pytest.mark.parametrize("B,R,C", [(1, 10, 77), (2, 5, 130), (1, 3, 300), (1, 130, 40)])
@@ -97,6 +101,20 @@ def build_model(cfg):
     return model.eval().cuda(), sd
 
 
+def assert_maps_change_no_bit(model, tokens, out, repr_layers):
+    """out = model(tokens, repr_layers, return_contacts=True), with the column maps: the same call without them, and
+    predict_contacts, give the same bits (one stack call computes every map)"""
+    model.contacts_without_col_attentions = True
+    lean = model(tokens, repr_layers=repr_layers, return_contacts=True)
+    model.contacts_without_col_attentions = False
+    assert "col_attentions" not in lean
+    for key in ("logits", "row_attentions", "contacts"):
+        assert torch.equal(lean[key], out[key]), key
+    for k in repr_layers:
+        assert torch.equal(lean["representations"][k], out["representations"][k]), k
+    assert torch.equal(model.predict_contacts(tokens), out["contacts"])
+
+
 @pytest.mark.parametrize("name", ["msa_model_L2_E128_H2", "msa_model_L3_E256_H4_nopad"])
 def test_msa_transformer_against_reference_golden(name, golden_dir):
     """esm_b200.msa.MSATransformer (embedding prologue kernel, esmb200_axial_stack_forward, LM head, contact head)
@@ -108,10 +126,7 @@ def test_msa_transformer_against_reference_golden(name, golden_dir):
     L = cfg["layers"]
     out = model(tokens.cuda(), repr_layers=[0, 1, L], return_contacts=True)
     assert "col_attentions" in out  # return_contacts implies need_head_weights (msa_transformer.py:149-150)
-    model.contacts_without_col_attentions = True
-    lean = model(tokens.cuda(), repr_layers=[L], return_contacts=True)
-    model.contacts_without_col_attentions = False
-    assert "col_attentions" not in lean and float((lean["contacts"] - out["contacts"]).abs().max()) <= 1e-4
+    assert_maps_change_no_bit(model, tokens.cuda(), out, [0, 1, L])
     for k, v in fx["representations"].items():
         assert rel_fro(out["representations"][k].cpu()[keep], v[keep]) <= (1e-5 if k == 0 else 3e-3), k
     assert rel_fro(out["logits"].cpu()[keep], fx["logits"][keep]) <= 4e-3
@@ -123,6 +138,7 @@ def test_msa_transformer_against_reference_golden(name, golden_dir):
     assert rel_fro(out2["representations"][L].cpu()[keep], fx["representations"][L][keep]) <= 3e-3
     # need_head_weights: column maps too, B x L x H x C x R x R
     out3 = model(tokens.cuda(), need_head_weights=True)
+    assert torch.equal(out3["logits"], out2["logits"])
     col = out3["col_attentions"][:, :, :, :3].cpu()
     qkeep = keep[:, :, :3].permute(0, 2, 1)                      # [B, 3, R] query rows that are not padding
     diff = (col - fx["col_attentions_sample"]).abs()             # [B, L, H, 3, R, R]
@@ -162,3 +178,22 @@ def test_axial_stack_is_deterministic():
     for o in outs[1:]:
         assert torch.equal(o, outs[0])
     assert torch.isfinite(outs[0]).all()
+
+
+def test_column_maps_over_the_grid_limit_are_refused_before_any_launch():
+    """Column maps for B*C*H > 65535 (the probability kernel's grid has one z index per map): ESMB200_EINVAL before
+    the first launch, x untouched."""
+    from esm_b200 import _lib
+    from esm_b200.msa import run_axial_stack
+    layer, _ = build(128, 512, 2)
+    layer.handles()  # the layer's weight packing launches kernels of its own
+    x = torch.randn(33, 1, 1000, 128, device="cuda")  # 33 * 1000 * 2 = 66,000 maps
+    y = x.clone()
+    lib = _lib.load()
+    torch.cuda.synchronize()
+    before = lib.esmb200_launch_count()
+    with pytest.raises(_lib.Esmb200Error, match=r"B\*C\*H must be <= 65535"):
+        run_axial_stack([layer], y, col_attn={0: torch.empty(33, 1000, 2, 1, 1, device="cuda")})
+    assert lib.esmb200_launch_count() == before
+    torch.cuda.synchronize()
+    assert torch.equal(y, x)

@@ -1,10 +1,10 @@
 """GPU (-m gpu): per-alignment key padding through the MSA Transformer's axial stack, in fp16 and fp32x3.
 
 A batch of alignments padded the way MSABatchConverter pads (each alignment's own width and depth inside one R x C)
-gives alignment b padded key columns of its own.  The tied row attention reads them at two strides: the stack
-(esmb200_axial_stack_forward, run_axial_stack) passes pad_mask [B,R,C] at stride R * C, so the keys follow row 0 of
-each alignment, and AxialTransformerLayer.forward_batch_major(..., need_probs=True) passes pad_mask[:, 0] at stride C.
-For both:
+gives alignment b padded key columns of its own.  The stack (esmb200_axial_stack_forward) passes pad_mask [B,R,C] to
+the tied row attention at stride R * C, so the keys follow row 0 of each alignment.  Two calls of it are checked,
+run_axial_stack with the row maps only and AxialTransformerLayer.forward_batch_major(..., need_probs=True), which also
+writes the column maps.  For both:
   * the row-attention probabilities are exactly 0 at each alignment's own padded key columns;
   * each alignment's outputs and row maps at valid positions are bit-identical to that alignment run alone at the
     same R and C;
@@ -122,7 +122,7 @@ def test_keys_follow_row_zero(path, precision):
 @PRECISIONS
 def test_msa_transformer_on_a_ragged_batch(precision):
     """Two MSAs of 5 x 40 and 3 x 25 tokens (<cls> included) in one padded batch, against the float64 oracle at the
-    valid tokens, with (row attention at stride C) and without (the stack, stride R * C) need_head_weights."""
+    valid tokens, with and without need_head_weights."""
     from esm_b200.msa import MSATransformer
     from oracle import msa_oracle
     L = 2
@@ -140,8 +140,10 @@ def test_msa_transformer_on_a_ragged_batch(precision):
     ref = msa_oracle.msa_transformer_forward({k: v.double() for k, v in sd.items()}, L, H, tokens, repr_layers=[L],
                                              need_head_weights=True)
     tol = (3e-3, 4e-3, 1e-2) if precision == 0 else (2e-5, 2e-5, 5e-5)  # test_gpu_msa / test_gpu_msa_precision
+    outs = []
     for need in (False, True):
         out = model(tokens.cuda(), repr_layers=[L], need_head_weights=need)
+        outs.append(out)
         rep = out["representations"][L].cpu().double()[keep]
         want = ref["representations"][L][keep]
         r = float((rep - want).norm() / want.norm())
@@ -151,3 +153,5 @@ def test_msa_transformer_on_a_ragged_batch(precision):
         report(f"msa ragged batch precision={precision} need_head_weights={need}", repr_rel_fro=r, logits_rel_fro=lr,
                row_maps_max_abs=ra)
         assert r <= tol[0] and lr <= tol[1] and ra <= tol[2]
+    assert torch.equal(outs[0]["logits"], outs[1]["logits"])  # the maps change no bit of the rest
+    assert torch.equal(outs[0]["representations"][L], outs[1]["representations"][L])

@@ -23,6 +23,7 @@ if HERE not in sys.path:
     sys.path.insert(0, HERE)  # variant_fixtures
 
 import test_gpu_tied_attention as tied  # noqa: E402
+from test_gpu_msa import assert_maps_change_no_bit  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -182,9 +183,11 @@ def test_axial_layer_fp32x3_against_reference_golden(name, golden_dir):
     layer = build_layer(cfg["E"], cfg["F"], cfg["H"])
     keep = torch.ones(x.shape[:3], dtype=torch.bool) if mask is None else ~mask
     kw = {} if mask is None else {"self_attn_padding_mask": mask.cuda()}
+    outs = []
     for need in (False, True):
         res = layer(x.permute(1, 2, 0, 3).cuda(), need_head_weights=need, **kw)
         out = (res[0] if need else res).permute(2, 0, 1, 3).cpu()
+        outs.append(out)
         r = rel_fro(out[keep], fx["out"][keep])
         line = f"PARITY msa_precision axial_layer {name} maps={need}: out rel_fro={r:.3e}"
         assert r <= 2e-5, line
@@ -196,6 +199,7 @@ def test_axial_layer_fp32x3_against_reference_golden(name, golden_dir):
             line += f" row maps max_abs={mr:.3e} column sample max_abs={mc:.3e}"
             assert mr <= 5e-5 and mc <= 5e-5, line
         print(line, flush=True)
+    assert torch.equal(outs[0], outs[1])  # the maps change no bit of x
 
 
 def build_model(cfg, seed=None):
@@ -217,11 +221,12 @@ def test_msa_transformer_fp32x3_against_reference_golden(name, golden_dir):
     keep = tokens.ne(1)
     L = cfg["layers"]
     out = model(tokens.cuda(), repr_layers=[0, 1, L], return_contacts=True)
+    assert_maps_change_no_bit(model, tokens.cuda(), out, [0, 1, L])
     reprs = {k: rel_fro(out["representations"][k].cpu()[keep], v[keep]) for k, v in fx["representations"].items()}
     lg = rel_fro(out["logits"].cpu()[keep], fx["logits"][keep])
     ra = max_abs(out["row_attentions"].cpu(), fx["row_attentions"])
     ct = max_abs(out["contacts"].cpu(), fx["contacts"])
-    pc = max_abs(model.predict_contacts(tokens.cuda()).cpu(), fx["contacts"])    # no column maps: the C stack
+    pc = max_abs(model.predict_contacts(tokens.cuda()).cpu(), fx["contacts"])    # no column maps
     out3 = model(tokens.cuda(), need_head_weights=True)
     col = out3["col_attentions"][:, :, :, :3].cpu()
     qkeep = keep[:, :, :3].permute(0, 2, 1)                                     # [B, 3, R]
@@ -360,7 +365,7 @@ def test_mixed_precision_stack_is_rejected():
     nbytes = lib.esmb200_axial_workspace_bytes_split(128, 512, 1, 4, 40)
     ws = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
     rc = lib.esmb200_axial_stack_forward((ctypes.c_void_p * 1)(row16), (ctypes.c_void_p * 1)(col32), 1, _ptr(x), None,
-                                         None, 1, 4, 40, None, _ptr(ws), nbytes, _stream())
+                                         None, 1, 4, 40, None, None, _ptr(ws), nbytes, _stream())
     assert rc == -1 and b"share one precision" in lib.esmb200_last_error()
 
 

@@ -15,7 +15,7 @@ def test_new_symbols_are_exported():
     for name in NEW_SYMBOLS:
         assert name in _lib.EXPORTS
         assert hasattr(lib, name)
-    assert _lib.load().esmb200_abi_version() == 2
+    assert _lib.load().esmb200_abi_version() == 3
 
 
 @pytest.mark.parametrize("args,nbytes", [
