@@ -65,6 +65,7 @@ EXPORTS = (
     "esmb200_gemm_fp8",
     "esmb200_stack_contacts_bytes",
     "esmb200_stack_contacts",
+    "esmb200_window_merge",
 )
 
 ABI_VERSION = 3
@@ -160,6 +161,9 @@ def _declare(lib):
     lib.esmb200_mean_pool.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]
     lib.esmb200_log_softmax_rows.restype = c_int32
     lib.esmb200_log_softmax_rows.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.esmb200_window_merge.restype = c_int32
+    lib.esmb200_window_merge.argtypes = [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                         c_int64, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -54,7 +54,7 @@ int fail_cuda(cudaError_t e, const char* what) {
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
                      T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
-                     T_COUNT };
+                     T_WINDOW_MERGE, T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1584,6 +1584,23 @@ int esmb200_log_softmax_rows(const float* logits, int64_t ld, int32_t n, int32_t
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ProfScope ps(T_LOG_SOFTMAX, st);
   log_softmax_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(logits, ld, n, V, target, out);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
+
+int esmb200_window_merge(const float* src, int64_t src_ld, const int64_t* idx, const float* w, const int64_t* seg,
+                         int32_t rows, int32_t C, float* out, int64_t out_ld, void* stream) {
+  if (rows < 0 || C <= 0 || src_ld < C || out_ld < C)
+    return fail(ESMB200_EINVAL, "window_merge needs rows >= 0, C > 0, src_ld >= C and out_ld >= C");
+  if (rows == 0) return ESMB200_OK;
+  if (!src || !idx || !w || !seg || !out) return fail(ESMB200_EINVAL, "null argument");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ProfScope ps(T_WINDOW_MERGE, st);
+  const int64_t total = (int64_t)rows * C;
+  const int64_t blocks = (total + 255) / 256;
+  window_merge_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(src, src_ld, idx, w, seg, rows, C,
+                                                                                  out, out_ld);
   CK(cudaGetLastError());
   return ESMB200_OK;
 }

@@ -9,6 +9,7 @@
 //   mean_pool         scripts/extract.py:116-119 per-sequence mean representation
 //   log_softmax_rows  examples/variant-prediction/predict.py:142,175,194,211 (torch.log_softmax over the vocabulary)
 //                     and the target gather of :114,143
+//   window_merge      weighted row sums that stitch overlapping windows of a long protein (esm_b200/windows.py)
 //   convert_f32_f16   weight packing (fp32 nn.Linear weights -> fp16 MMA operands)
 #pragma once
 
@@ -268,6 +269,29 @@ log_softmax_rows_kernel(const float* __restrict__ logits, int64_t ld, int n, int
     float* y = out + (size_t)row * V;
     if (lane < V) y[lane] = (v0 - m) - lse;
     if (lane + 32 < V) y[lane + 32] = (v1 - m) - lse;
+  }
+}
+
+// Overlapping-window merge (esm_b200/windows.py): out[r, c] = sum over j in [seg[r], seg[r+1]) of w[j] * src[idx[j], c].
+// One thread per output element (flat r * C + c, so neighbouring threads read neighbouring columns of a source row for
+// any C), grid-stride. The terms are taken in j order as one fp32 fma chain; a one-term segment is a plain copy (every
+// bit pattern, -0.0 and NaN included, passes through), an empty one writes +0. No atomics: deterministic.
+__global__ void __launch_bounds__(256)
+window_merge_kernel(const float* __restrict__ src, int64_t src_ld, const int64_t* __restrict__ idx,
+                    const float* __restrict__ w, const int64_t* __restrict__ seg, int64_t rows, int C,
+                    float* __restrict__ out, int64_t out_ld) {
+  const int64_t total = rows * C;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / C;
+    const int c = (int)(i - r * C);
+    const int64_t j0 = seg[r], j1 = seg[r + 1];
+    float acc = 0.f;
+    if (j1 - j0 == 1) {
+      acc = src[idx[j0] * src_ld + c];
+    } else {
+      for (int64_t j = j0; j < j1; ++j) acc = fmaf(w[j], src[idx[j] * src_ld + c], acc);
+    }
+    out[r * out_ld + c] = acc;
   }
 }
 

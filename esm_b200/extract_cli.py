@@ -13,6 +13,9 @@ torch.save in line, so the GPU idles during the copies and the pickling):
   * device->host copies go to pinned staging buffers on a side stream and are overlapped with the next batch's forward
     (two staging slots); slicing + `torch.save` run in writer threads;
   * the default token budget is larger (the reference's 4096 tokens leave an H100 idle);
+  * --window N writes sequences longer than N residues whole instead of truncating them: each runs as overlapping
+    windows of N residues merged with tapered weights (ProteinLanguageModel.forward_windowed); --truncation_seq_length
+    is then not applied, and --include contacts is refused;
   * under torchrun the token-budget batches are dealt round-robin to the ranks, each rank writes its own files, and no
     collective is needed because the outputs are files.
 """
@@ -51,7 +54,13 @@ def create_parser():
     p.add_argument("--cpu-offload", action="store_true",
                    help="keep the transformer layers' weights in pinned host memory and stream them to the GPU layer "
                         "by layer (ESM-2 15B on one GPU); same outputs")
+    p.add_argument("--window", type=int, default=None,
+                   help="instead of truncating, run sequences longer than this many residues as overlapping windows "
+                        "merged with tapered weights (1022 fits ESM-1b / ESM-1v); not with --include contacts")
     return p
+
+
+WINDOW_CONTACTS = "--include contacts cannot be combined with --window: contacts across windows are not predicted"
 
 
 class FileWriter:
@@ -157,6 +166,12 @@ def _finalize(p: _Pending, include, out_dir: pathlib.Path, writer: FileWriter):
 
 
 def run(args) -> int:
+    window = getattr(args, "window", None)
+    if window is not None:
+        if "contacts" in args.include:
+            raise ValueError(WINDOW_CONTACTS)
+        if window < 2:
+            raise ValueError(f"--window must be at least 2 residues, got {window}")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
@@ -177,7 +192,11 @@ def run(args) -> int:
 
     dataset = FastaBatchedDataset.from_file(args.fasta_file)
     my_batches = dataset.get_batch_indices(args.toks_per_batch, extra_toks_per_seq=1)[rank::world]
-    to_tokens = alphabet.get_batch_converter(args.truncation_seq_length)
+    if window is not None:
+        from .windows import check_window
+        check_window(model, window)
+    truncation = None if window is not None else args.truncation_seq_length
+    to_tokens = alphabet.get_batch_converter(truncation)
     args.output_dir.mkdir(parents=True, exist_ok=True)
 
     writer = FileWriter()
@@ -188,12 +207,16 @@ def run(args) -> int:
         with torch.no_grad():
             for k, idxs in enumerate(my_batches):
                 labels, strs, toks = to_tokens([dataset[i] for i in idxs])
-                lengths = [min(args.truncation_seq_length, len(s)) for s in strs]
+                lengths = [len(s) if truncation is None else min(truncation, len(s)) for s in strs]
                 toks_dev = toks.pin_memory().to(dev, non_blocking=True)
                 # contacts: the forward without the attention stack (ProteinLanguageModel._contacts_forward), so only
                 # the representations and the [B,S,S] contacts stay alive with the batch while its copies run
-                out = (model._contacts_forward(toks_dev, repr_layers=layers) if want_contacts
-                       else model(toks_dev, repr_layers=layers))
+                if window is not None:
+                    out = model.forward_windowed(toks_dev, window, repr_layers=layers)
+                elif want_contacts:
+                    out = model._contacts_forward(toks_dev, repr_layers=layers)
+                else:
+                    out = model(toks_dev, repr_layers=layers)
                 reps = out["representations"]
                 B, T, E = next(iter(reps.values())).shape
                 computed = torch.cuda.Event()

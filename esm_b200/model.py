@@ -805,6 +805,74 @@ class ProteinLanguageModel(nn.Module):
                 result["contacts"] = cast(contacts)
         return result
 
+    @torch.no_grad()
+    def forward_windowed(self, tokens, window: int, repr_layers=(), max_tokens: Optional[int] = None):
+        """forward(tokens, repr_layers) for proteins of any length: each row of tokens [B, T] (right-padded) runs as
+        overlapping windows of `window` residues, merged by the rule of esm_b200.windows. Returns {"logits": [B,T,V],
+        "representations": {layer: [B,T,E]}} (the last layer post-LN, as forward returns it; pad rows zero). The
+        windows of all rows form one batch, padded only where a protein is shorter than the window, and run through
+        the stack in chunks of at most `max_tokens` tokens (at least one window per chunk; the result does not depend
+        on it). A protein of at most `window` residues gets forward's rows bit for bit. No attention maps or
+        contacts."""
+        dtype = self.embed_tokens.weight.dtype
+        out = self._windowed(tokens, window, repr_layers, max_tokens)
+        if dtype == torch.float32:
+            return out
+        return {"logits": out["logits"].to(dtype),
+                "representations": {i: t.to(dtype) for i, t in out["representations"].items()}}
+
+    def _windowed(self, tokens, window: int, repr_layers=(), max_tokens: Optional[int] = None):
+        """forward_windowed in fp32 whatever the parameters' dtype (the variant scorers' logits)."""
+        from . import windows
+        from .variants import _copies_per_chunk
+        W = windows.check_window(self, window)
+        dev = self.embed_tokens.weight.device
+        tokens = torch.as_tensor(tokens)
+        if tokens.dim() != 2:
+            raise ValueError("tokens must be [B, T]")
+        if tokens.dtype.is_floating_point or tokens.dtype == torch.bool:
+            raise TypeError(f"tokens must be an integer tensor, got {tokens.dtype}")
+        B, T = tokens.shape
+        E, N, V = self.embed_dim, self.num_layers, self.alphabet_size
+        layers = sorted(i for i in set(repr_layers) if 0 <= i <= N)
+        bos, eos = int(self.prepend_bos), int(self.append_eos)
+        host = tokens.cpu().long()
+        Tw = min(T, W + bos + eos)
+        gather, out_rows, src_rows, weights = [], [], [], []
+        nw = 0
+        # a protein ends at its last non-pad token (a <pad> inside it stays in its window, as forward keeps it)
+        keep = host.ne(self.padding_idx)
+        extent = torch.where(keep.any(1), T - keep.flip(1).int().argmax(1), 0)
+        for b, n in enumerate((extent - bos - eos).tolist()):
+            plan = windows.Plan(max(n, 0), W, bos, eos)
+            gather.append(plan.gather(T, Tw) + b * (T + 1))
+            pos, win, row, w = plan.terms()
+            out_rows.append(b * T + pos)
+            src_rows.append((nw + win) * Tw + row)
+            weights.append(w)
+            nw += plan.K
+        ext = torch.cat([host, torch.full((B, 1), self.padding_idx, dtype=torch.int64)], 1).view(-1)
+        wtok = ext[torch.cat(gather)].to(dev)  # [nw, Tw]
+        logits = torch.empty((nw, Tw, V), dtype=torch.float32, device=dev)
+        reps = {i: torch.empty((nw, Tw, E), dtype=torch.float32, device=dev) for i in layers}
+        per = _copies_per_chunk(Tw, max_tokens)
+        ln = self.emb_layer_norm_after
+        for s in range(0, nw, per):
+            _, x, hidden, _, _ = self._stack(wtok[s:s + per], set(layers))
+            with torch.cuda.device(dev):
+                logits[s:s + per] = self._lm_head_rows(x.view(-1, E)).view(-1, Tw, V)
+                for i, t in hidden.items():
+                    reps[i][s:s + per] = t
+                if N in reps:  # esm2.py:123-128 final LayerNorm, as forward applies it
+                    ln_w, ln_b = self._mirror("ln_after.w", ln.weight), self._mirror("ln_after.b", ln.bias)
+                    _lib.check(_lib.load().esmb200_layernorm(_ptr(x), _ptr(ln_w), _ptr(ln_b), _ptr(x), x.shape[0] * Tw,
+                                                             E, ln.eps, _stream()))
+                    reps[N][s:s + per] = x
+        out_rows = torch.cat(out_rows)
+        idx, w, seg = torch.cat(src_rows), torch.cat(weights), windows.segments(out_rows, B * T)
+        merge = lambda src, C: windows.merge_rows(src.view(-1, C), idx, w, seg).view(B, T, C)
+        return {"logits": merge(logits, V), "representations": {i: merge(t, E) for i, t in reps.items()}}
+
     def predict_contacts(self, tokens):
         """forward(tokens, return_contacts=True)["contacts"], bit for bit, without the [B,L,H,T,T] attention stack:
         its peak memory is the contact partials (about 1/16 of the stack) instead of the stack."""

@@ -9,6 +9,8 @@ predict.py:45-104, plus --max-tokens) on the library's batched scorers (esm_b200
     column per --model-location named by the location string. It is written with the csv module: the input cells are
     copied unchanged, the scores written with repr. Neither pandas nor Biopython is needed.
   * --precision fp32x3 runs every model (sequence models and the MSA Transformer) with fp16 hi + lo operand pairs.
+  * --window N scores proteins longer than N residues (ESM-1b / ESM-1v cannot take more than 1022) through overlapping
+    windows of N residues (esm_b200.windows), with every strategy; sequence models only.
   * there is no CPU path: --nogpu raises.
 """
 from __future__ import annotations
@@ -26,6 +28,7 @@ from . import pretrained, variants
 STRATEGIES = ["wt-marginals", "pseudo-ppl", "masked-marginals"]
 PRECISIONS = ["fp16", "fp32x3"]
 MSA_ONLY_MASKED = "MSA Transformer only supports masked marginal strategy"  # predict.py:163-165
+MSA_NO_WINDOW = "--window applies to ESM-2, ESM-1b and ESM-1v models; MSA Transformer alignments are not windowed"
 
 
 def create_parser():
@@ -57,6 +60,10 @@ def create_parser():
                    help="keep the transformer layers' weights of ESM-2 / ESM-1b / ESM-1v models in pinned host memory "
                         "and stream them to the GPU layer by layer (ESM-2 15B on one GPU); same scores. The MSA "
                         "Transformer stays resident")
+    p.add_argument("--window", type=int, default=None,
+                   help="score through overlapping windows of this many residues, merged with tapered weights, so "
+                        "that proteins longer than the model's window (1022 residues for ESM-1b / ESM-1v) can be "
+                        "scored; sequence models only")
     return p
 
 
@@ -112,7 +119,10 @@ def write_table(path, header: List[str], rows: List[List[str]], scores: Dict[str
 
 def score_model(model, alphabet, is_msa: bool, args, mutations: List[str]) -> List[float]:
     """predict.py:159-233 for one model on the library."""
+    window = getattr(args, "window", None)
     if is_msa:
+        if window is not None:
+            raise ValueError(MSA_NO_WINDOW)
         data = [variants.read_msa(args.msa_path, args.msa_samples)]
         assert args.scoring_strategy == "masked-marginals", MSA_ONLY_MASKED
         _, _, tokens = alphabet.get_batch_converter()(data)
@@ -120,11 +130,12 @@ def score_model(model, alphabet, is_msa: bool, args, mutations: List[str]) -> Li
         return variants.label_scores(lp, alphabet, args.sequence, mutations, args.offset_idx)
     _, _, tokens = alphabet.get_batch_converter()([("protein1", args.sequence)])
     if args.scoring_strategy == "wt-marginals":
-        lp = variants.wt_marginals(model, tokens)
+        lp = variants.wt_marginals(model, tokens, window=window)
     elif args.scoring_strategy == "masked-marginals":
-        lp = variants.masked_marginals(model, tokens, max_tokens=args.max_tokens)
+        lp = variants.masked_marginals(model, tokens, max_tokens=args.max_tokens, window=window)
     else:
-        return variants.pseudo_ppl(model, alphabet, args.sequence, mutations, args.offset_idx, args.max_tokens)
+        return variants.pseudo_ppl(model, alphabet, args.sequence, mutations, args.offset_idx, args.max_tokens,
+                                   window=window)
     return variants.label_scores(lp, alphabet, args.sequence, mutations, args.offset_idx)
 
 
@@ -132,6 +143,11 @@ def run(args) -> None:
     if args.nogpu:
         raise RuntimeError("--nogpu: esm_b200 runs on CUDA (sm_90a) only and has no CPU path; run without --nogpu "
                            "on a machine with an H100")
+    if getattr(args, "window", None) is not None:
+        if args.window < 2:
+            raise ValueError(f"--window must be at least 2 residues, got {args.window}")
+        if any(is_msa_location(loc) for loc in args.model_location):
+            raise ValueError(MSA_NO_WINDOW)
     header, rows = read_table(args.dms_input)
     col = header.index(args.mutation_col)
     mutations = [r[col] for r in rows]

@@ -18,6 +18,11 @@ Reproduced as the reference has it (the command line must give predict.py's numb
     the token one to the right of the masked one; the last residue is never masked. The per-position fp32 values
     are summed as Python floats in position order.
   * label_scores reads position 1 + idx (the <cls> token comes first) and subtracts in fp32.
+
+With `window`, masked_marginals, wt_marginals and pseudo_ppl score proteins longer than the model's window through the
+overlapping windows of esm_b200.windows: a masked position gets one masked copy per window that covers it, the copies'
+logit rows are merged with the windows' weights (esmb200_window_merge) and log_softmax runs on the merged row.
+window=None is the unwindowed path, unchanged; a protein of at most `window` residues scores bit for bit as without it.
 """
 from __future__ import annotations
 
@@ -27,7 +32,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-from . import _lib
+from . import _lib, windows
 from .model import _ptr, _stream
 
 # Budget of one chunk, in tokens. Per token at E = 1280 (650M), one stack call needs its workspace
@@ -81,10 +86,13 @@ def _head_rows(model, batch: torch.Tensor, rows: torch.Tensor) -> torch.Tensor:
 
 @torch.no_grad()
 def masked_marginals(model, tokens: torch.Tensor, positions: Optional[Sequence[int]] = None,
-                     max_tokens: Optional[int] = None) -> torch.Tensor:
+                     max_tokens: Optional[int] = None, window: Optional[int] = None) -> torch.Tensor:
     """Row k: log_softmax(logits) at positions[k] of the copy of `tokens` with positions[k] masked, fp32 [n, V].
     tokens [1, T] (ESM-2, ESM-1b / ESM-1v; predict.py:205-215) or [1, R, C] (MSA Transformer, predict.py:169-178: the
-    mask goes at [0, 0, positions[k]] and the row is read from alignment row 0). positions default to all T (C)."""
+    mask goes at [0, 0, positions[k]] and the row is read from alignment row 0). positions default to all T (C).
+    window (sequence models): the logits of each position merged over the windows that cover it."""
+    if window is not None:
+        window = windows.check_window(model, window)
     dev = _device(model)
     tokens = tokens.to(dev)
     if tokens.dim() not in (2, 3) or tokens.shape[0] != 1:
@@ -99,6 +107,11 @@ def masked_marginals(model, tokens: torch.Tensor, positions: Optional[Sequence[i
     positions = positions.to("cpu", torch.int64).view(-1)
     if positions.numel() and not bool(((positions >= 0) & (positions < L)).all()):
         raise ValueError(f"positions must lie in [0, {L})")
+    if window is not None:
+        if tokens.dim() != 2:
+            raise ValueError("window applies to sequence models only: MSA windowing is not supported")
+        return log_softmax_rows(_windowed_masked_logits(model, tokens, window, torch.zeros_like(positions),
+                                                        positions, max_tokens))
     positions = positions.to(dev)
     k = _copies_per_chunk(per_copy, max_tokens)
     out = []
@@ -118,11 +131,16 @@ def masked_marginals(model, tokens: torch.Tensor, positions: Optional[Sequence[i
 
 
 @torch.no_grad()
-def wt_marginals(model, tokens: torch.Tensor) -> torch.Tensor:
-    """log_softmax(logits) of the unmasked sequence, fp32 [T, V] (predict.py:192-194). tokens [1, T]."""
+def wt_marginals(model, tokens: torch.Tensor, window: Optional[int] = None) -> torch.Tensor:
+    """log_softmax(logits) of the unmasked sequence, fp32 [T, V] (predict.py:192-194). tokens [1, T].
+    window: the logits merged over the windows (ProteinLanguageModel.forward_windowed)."""
+    if window is not None:
+        window = windows.check_window(model, window)
     tokens = tokens.to(_device(model))
     if tokens.dim() != 2 or tokens.shape[0] != 1:
         raise ValueError("tokens must be one sequence [1, T]")
+    if window is not None:
+        return log_softmax_rows(model._windowed(tokens, window)["logits"][0])
     x = model._stack(tokens)[1]
     with torch.cuda.device(x.device):
         return log_softmax_rows(model._lm_head_rows(x.view(-1, x.shape[-1])))
@@ -152,11 +170,13 @@ def label_scores(token_log_probs: torch.Tensor, alphabet, sequence: str, mutatio
 
 @torch.no_grad()
 def pseudo_ppl(model, alphabet, sequence: str, mutations: Sequence[str], offset_idx: int = 0,
-               max_tokens: Optional[int] = None) -> List[float]:
+               max_tokens: Optional[int] = None, window: Optional[int] = None) -> List[float]:
     """compute_pppl (predict.py:118-144) for each mutation, batched across mutants and positions: every mutant is a
     substitution, so all copies share one length T. For the mutated sequence s, token position i in 1 ... len(s) - 2
     is masked and scored at alphabet.get_idx(s[i]) (the reference's indexing, kept as is); the fp32 values are summed
-    as Python floats in position order."""
+    as Python floats in position order. window: each position's logits merged over the windows that cover it."""
+    if window is not None:
+        window = windows.check_window(model, window)
     seqs = []
     for row in mutations:
         wt, idx, mt = parse_mutation(row, offset_idx)
@@ -173,6 +193,11 @@ def pseudo_ppl(model, alphabet, sequence: str, mutations: Sequence[str], offset_
     toks = toks.to(dev)
     target = torch.tensor([alphabet.get_idx(s[i]) for s in seqs for i in range(1, P + 1)], dtype=torch.int64)
     target = target.to(dev)
+    if window is not None:
+        logits = _windowed_masked_logits(model, toks, window, torch.arange(M).repeat_interleave(P),
+                                         torch.arange(1, P + 1).repeat(M), max_tokens)
+        flat = log_softmax_rows(logits, target).cpu().tolist()
+        return [sum(flat[j * P:(j + 1) * P]) for j in range(M)]
     mutant = torch.arange(M, device=dev).repeat_interleave(P)
     position = torch.arange(1, P + 1, device=dev).repeat(M)
     k = _copies_per_chunk(T, max_tokens)
@@ -186,6 +211,42 @@ def pseudo_ppl(model, alphabet, sequence: str, mutations: Sequence[str], offset_
         vals.append(log_softmax_rows(_head_rows(model, batch, copy * T + pos), target[s:s + k]))
     flat = torch.cat(vals).cpu().tolist()
     return [sum(flat[j * P:(j + 1) * P]) for j in range(M)]
+
+
+def _windowed_masked_logits(model, toks: torch.Tensor, window: int, row: torch.Tensor, pos: torch.Tensor,
+                            max_tokens: Optional[int]) -> torch.Tensor:
+    """Merged logits fp32 [q, V] of queries (row[k], pos[k]): sequence row[k] of toks [M, T] (unpadded, one length)
+    with token position pos[k] masked, one masked copy per window covering pos[k] (esm_b200.windows). The copies of
+    all queries run in chunks of at most max_tokens tokens, as the unwindowed scorers run theirs."""
+    dev = _device(model)
+    M, T = toks.shape
+    bos, eos = int(model.prepend_bos), int(model.append_eos)
+    plan = windows.Plan(T - bos - eos, window, bos, eos)
+    Tw = plan.tokens
+    ext = torch.cat([toks.to(dev), torch.full((M, 1), model.padding_idx, dtype=toks.dtype, device=dev)], 1)
+    wtok = ext[:, plan.gather(T, Tw).to(dev)].reshape(M * plan.K, Tw)
+    tpos, twin, trow, tw = plan.terms()
+    first = windows.segments(tpos, T)  # terms of token position t: [first[t], first[t + 1])
+    pos, row = pos.cpu(), row.cpu()
+    counts = first[pos + 1] - first[pos]
+    seg = torch.zeros(pos.numel() + 1, dtype=torch.int64)
+    seg[1:] = counts.cumsum(0)
+    term = first[pos].repeat_interleave(counts) + torch.arange(int(seg[-1])) - seg[:-1].repeat_interleave(counts)
+    copy_win = (row.repeat_interleave(counts) * plan.K + twin[term]).to(dev)
+    copy_row = trow[term].to(dev)
+    k = _copies_per_chunk(Tw, max_tokens)
+    out = []
+    for s in range(0, copy_win.numel(), k):
+        r = copy_row[s:s + k]
+        m = r.numel()
+        batch = wtok.index_select(0, copy_win[s:s + k])
+        copy = torch.arange(m, device=dev)
+        batch[copy, r] = model.mask_idx
+        out.append(_head_rows(model, batch, copy * Tw + r))
+    if not out:
+        return torch.empty((0, model.alphabet_size), dtype=torch.float32, device=dev)
+    logits = torch.cat(out)
+    return windows.merge_rows(logits, torch.arange(logits.shape[0]), tw[term], seg)
 
 
 _INSERTION = re.compile(r"[a-z.*]")

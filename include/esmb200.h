@@ -233,6 +233,17 @@ int esmb200_mean_pool(const float* x, const int32_t* lengths, float* out, int32_
 int esmb200_log_softmax_rows(const float* logits, int64_t ld, int32_t n, int32_t V, const int64_t* target,
                              float* out, void* stream);
 
+/* Overlapping-window merge (esm_b200/windows.py: a protein longer than the window runs as overlapping crops whose
+ * rows are stitched back together): a segmented weighted row sum
+ *     out[r, c] = sum over j in [seg[r], seg[r+1]) of w[j] * src[idx[j], c],   r < rows, c < C,
+ * the terms taken in j order as one fp32 fma chain per element. A segment of one term is copied bit for bit (weight
+ * ignored; -0.0 and NaN pass through), an empty segment writes +0. src fp32 [*, src_ld], out fp32 [rows, out_ld]
+ * (must not overlap src); idx int64, w fp32 and seg int64 [rows + 1] are device arrays, seg non-decreasing and every
+ * idx[j] a valid src row (the caller builds them). Any C (33 logits, E-wide representations). Deterministic, no
+ * atomics. rows == 0 launches nothing. */
+int esmb200_window_merge(const float* src, int64_t src_ld, const int64_t* idx, const float* w, const int64_t* seg,
+                         int32_t rows, int32_t C, float* out, int64_t out_ld, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
