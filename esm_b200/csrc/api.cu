@@ -268,6 +268,22 @@ struct ContactLayer {
   int lo, S;
 };
 
+// attention_probs_kernel over the pp.B sequences: one launch (and one T_PROBS scope) per
+// probs_cfg::seqs_per_launch(H) sequences, so a single launch whenever B*H <= 65535
+int run_probs(const CUtensorMap& tq, ProbsParams pp, cudaStream_t st, const char* what) {
+  const int per = probs_cfg::seqs_per_launch(pp.H);
+  for (int b0 = 0; b0 < pp.B; b0 += per) {
+    pp.b0 = b0;
+    cudaError_t e;
+    {
+      ProfScope ps(T_PROBS, st);
+      e = launch_attention_probs(tq, pp, pp.B - b0 < per ? pp.B - b0 : per, st);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, what);
+  }
+  return ESMB200_OK;
+}
+
 int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batch_stride, int attn_flags,
                   const AttnScratch& s, int B, int T, int H, cudaStream_t st, bool split = false,
                   const ContactLayer* contact = nullptr, int slots = 1) {
@@ -314,7 +330,6 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
     return ESMB200_OK;
   }
   if (probs) {
-    if ((size_t)B * H > 65535) return fail(ESMB200_EINVAL, "need_head_weights: B*H must be <= 65535");
     ProbsParams pp;
     pp.B = B; pp.T = T; pp.H = H; pp.E = E;
     pp.keybits = s.keybits; pp.kvlen = s.kvlen; pp.words = s.words;
@@ -323,11 +338,7 @@ int run_attention(const void* qkv, void* ctx, float* probs, long long probs_batc
     pp.zero_pad_rows = attn_flags & 1;
     pp.lo_off = split ? 3 * E : 0;
     pp.slots = slots;
-    {
-      ProfScope ps(T_PROBS, st);
-      e = launch_attention_probs(tq, pp, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "attention probs launch");
+    return run_probs(tq, pp, st, "attention probs launch");
   }
   return ESMB200_OK;
 }
@@ -352,8 +363,7 @@ int run_contact_accumulate(const float* attn, long long batch_stride, const floa
 // tokens per alignment column, read with strided TMA boxes (qkv viewed as [B*R, C*3E], AttnParams::cols), no
 // regrouping copy.  s holds the key bits of the B*C column sequences.  split (fp32x3): qkv [B*R*C, 6E] (viewed as
 // [B*R, C*6E], lo halves 3E to the right), ctx [B*R*C, 2E].  probs: optional fp32 [B*C, H, R, R], written from the
-// same strided view with the row statistics of the forward kernel (the caller checks B*C*H <= 65535); ctx is the same
-// with and without it.
+// same strided view with the row statistics of the forward kernel; ctx is the same with and without it.
 int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B, int R, int C, int H,
                          cudaStream_t st, bool split = false, float* probs = nullptr) {
   const int E = H * 64;
@@ -385,11 +395,7 @@ int run_column_attention(const void* qkv, void* ctx, const AttnScratch& s, int B
     pp.zero_pad_rows = 0;
     pp.lo_off = ap.lo_off;
     pp.cols = C;
-    {
-      ProfScope ps(T_PROBS, st);
-      e = launch_attention_probs(tq, pp, st);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "column attention probs launch");
+    return run_probs(tq, pp, st, "column attention probs launch");
   }
   return ESMB200_OK;
 }
@@ -1006,7 +1012,6 @@ static int stack_forward_impl(esmb200_layer* const* layers, int32_t n_layers, fl
     if (B > 65535) return fail(ESMB200_EINVAL, "return_contacts: B must be <= 65535");
     if (split) {
       if (S > kContactMaxS) return fail(ESMB200_EINVAL, kContactMaxSMsg);
-      if ((size_t)B * H > 65535) return fail(ESMB200_EINVAL, "need_head_weights: B*H must be <= 65535");
       if (!scratch || scratch_bytes < contact_sizes(n_layers, H, B, T, S, precision).scratch)
         return fail(ESMB200_EWORKSPACE, "probability scratch smaller than esmb200_stack_contacts_bytes");
       if (reinterpret_cast<uintptr_t>(scratch) % 16 != 0)
@@ -1471,9 +1476,6 @@ int esmb200_axial_stack_forward(esmb200_layer* const* row_layers, esmb200_layer*
   const AxialWorkspace aw = axial_workspace_layout(workspace, E, F, B, R, C, split);
   if (workspace_bytes < aw.bytes) return fail(ESMB200_EWORKSPACE, "workspace too small");
   if (E != 64 * H) return fail(ESMB200_EINVAL, "the MSA axial path needs head_dim 64");
-  for (int i = 0; col_attn_out && i < n_layers; ++i)
-    if (col_attn_out[i] && (long long)B * C * H > 65535)
-      return fail(ESMB200_EINVAL, "column attention maps: B*C*H must be <= 65535");
   const int M = B * R * C;
   const Workspace& ws = aw.ws;
   ActMaps am;

@@ -7,8 +7,9 @@ namespace esmb200 {
 
 // ---------------------------------------------------------------------------------------------------------------
 // need_head_weights=True: materialise the normalised probabilities (multihead_attention.py:379,397-400).
-// One CTA per (key block, query block, sequence*head): S = Q K^T again on the tensor cores (eight warps of 16 query
-// rows x 128 keys), then p = exp(s - rowmax) / rowsum with the row statistics saved by the forward kernel, fp32 [B,H,T,T].
+// One CTA per (key block, query block, sequence*head), sequences from p.b0: S = Q K^T again on the tensor cores (eight
+// warps of 16 query rows x 128 keys), then p = exp(s - rowmax) / rowsum with the row statistics saved by the forward
+// kernel, fp32 [B,H,T,T].
 // ---------------------------------------------------------------------------------------------------------------
 struct ProbsParams {
   int B, T, H, E;
@@ -23,12 +24,16 @@ struct ProbsParams {
   int lo_off;         // fp32x3 precision: column offset of the lo halves in qkv [M, 6E] (0 = plain fp16 operands)
   int slots = 1;      // 2: head_dim <= 128, a head is two adjacent 64-wide column slots (E = H * 128)
   int cols = 1;       // sequence b = (b / cols, b % cols) of a [B/cols, T, cols, 3E] qkv (fp32x3: 6E), as AttnParams::cols
+  int b0 = 0;         // the launch's first sequence: grid z holds (sequence - b0, head) pairs (launch_attention_probs)
 };
 
 namespace probs_cfg {
 constexpr int NUM_THREADS = 256;
 constexpr int BLOCK_Q = 128, BLOCK_KV = 128;
 constexpr int smem_bytes(int np) { return 2 * np * attn_cfg::TILE_BYTES + 1024 + 64; }
+constexpr int MAX_GRID_Z = 65535;
+// sequences per launch: grid z holds one index per (sequence, head) pair
+inline int seqs_per_launch(int H) { return MAX_GRID_Z / H; }
 }  // namespace probs_cfg
 
 // MODE 0: fp16 operands, head_dim <= 64 | 1 (SPLIT): fp32x3 hi|lo operands | 2: two 64-wide slots per head
@@ -46,7 +51,7 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const Probs
 
   const uint32_t warp = threadIdx.x / 32, lane = threadIdx.x % 32, g = lane / 4, c = lane % 4;
   const int kb = blockIdx.x, qb = blockIdx.y;
-  const int b = blockIdx.z / p.H, h = blockIdx.z % p.H;
+  const int b = p.b0 + (int)(blockIdx.z / p.H), h = blockIdx.z % p.H;
   const int q0 = qb * BLOCK_Q, k0 = kb * BLOCK_KV;
   const int row_base = (b / p.cols) * p.T;
   const int x0 = (b % p.cols) * (MODE == 1 ? 6 : 3) * p.E;  // MODE 1: a token's qkv is 6E wide (hi | lo)
@@ -115,19 +120,24 @@ attention_probs_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const Probs
 }
 
 template <int MODE>
-inline cudaError_t launch_attention_probs_mode(const CUtensorMap& tmap_qkv, const ProbsParams& p, cudaStream_t stream) {
+inline cudaError_t launch_attention_probs_mode(const CUtensorMap& tmap_qkv, const ProbsParams& p, int n,
+                                               cudaStream_t stream) {
   using namespace probs_cfg;
   constexpr int smem = smem_bytes(MODE ? 2 : 1);
-  dim3 grid((p.T + BLOCK_KV - 1) / BLOCK_KV, (p.T + BLOCK_Q - 1) / BLOCK_Q, p.B * p.H);
+  dim3 grid((p.T + BLOCK_KV - 1) / BLOCK_KV, (p.T + BLOCK_Q - 1) / BLOCK_Q, n * p.H);
   cudaError_t e = cudaFuncSetAttribute(attention_probs_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   return launch_pdl(attention_probs_kernel<MODE>, grid, dim3(NUM_THREADS), smem, stream, tmap_qkv, p);
 }
 
-inline cudaError_t launch_attention_probs(const CUtensorMap& tmap_qkv, const ProbsParams& p, cudaStream_t stream) {
-  if (p.slots == 2) return launch_attention_probs_mode<2>(tmap_qkv, p, stream);
-  if (p.lo_off > 0) return launch_attention_probs_mode<1>(tmap_qkv, p, stream);
-  return launch_attention_probs_mode<0>(tmap_qkv, p, stream);
+// one launch over the n sequences p.b0 ... p.b0 + n - 1, n <= probs_cfg::seqs_per_launch(p.H): the caller splits a
+// larger batch into launches of at most that many sequences
+inline cudaError_t launch_attention_probs(const CUtensorMap& tmap_qkv, const ProbsParams& p, int n,
+                                          cudaStream_t stream) {
+  if (n <= 0 || n > probs_cfg::seqs_per_launch(p.H) || p.b0 < 0 || p.b0 + n > p.B) return cudaErrorInvalidValue;
+  if (p.slots == 2) return launch_attention_probs_mode<2>(tmap_qkv, p, n, stream);
+  if (p.lo_off > 0) return launch_attention_probs_mode<1>(tmap_qkv, p, n, stream);
+  return launch_attention_probs_mode<0>(tmap_qkv, p, n, stream);
 }
 
 }  // namespace esmb200

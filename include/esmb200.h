@@ -178,7 +178,7 @@ int esmb200_stack_forward_streamed(esmb200_layer* const* layers, int32_t n_layer
  *   fp32x3 layers: per layer, the split probability kernel writes the maps into probs_scratch (fp32 [B,H,T,T], 16-byte
  *     aligned), then esmb200_contact_accumulate's kernel reads them: row_part is row_sum [n_layers,B,H,S] and col_part
  *     is col_part [n_layers,B,H,ceil(S/16),S] of that entry, layer l at offset l*B*H*S and l*B*H*ceil(S/16)*S.
- *     a1 of layer l = row_part[l] + col_part[l] summed over its stripe axis. S <= 1024, B*H <= 65535.
+ *     a1 of layer l = row_part[l] + col_part[l] summed over its stripe axis. S <= 1024.
  *   A probs_scratch or workspace smaller than its size is ESMB200_EWORKSPACE. Every refusal comes before any launch.
  * esmb200_stack_contacts_bytes: bytes of row_part, col_part and probs_scratch for n_layers layers of num_heads heads,
  *   a [B,T] batch and S = hi - lo cropped positions in `precision` (0 fp16, 1 fp32x3, 2 fp8); scratch is 0 for 0 and 2.
@@ -312,8 +312,8 @@ int esmb200_column_attention(const void* qkv_f16, const uint8_t* pad_mask, void*
  *   row-attention return layout, axial_attention.py:87,105).
  * col_attn_out: NULL, or n_layers pointers (NULL entries allowed) to fp32 [B*C,H,R,R] buffers: the column-attention
  *   probabilities of alignment column c of alignment b at [b*C + c] (the reference returns them as [H,C,B,R,R],
- *   axial_attention.py:206,216). B*C*H <= 65535 when any is given. x and the row maps are the same bits with and
- *   without them.
+ *   axial_attention.py:206,216). Any B*C*H: the probability kernel runs one launch per 65535 / H column
+ *   sequences. x and the row maps are the same bits with and without them.
  * workspace: esmb200_axial_workspace_bytes(E,F,B,R,C) bytes, or esmb200_axial_workspace_bytes_split(E,F,B,R,C) for
  *   layers created with precision = 1 (fp32x3: the activations, qkv, ctx and P are stored as fp16 hi | lo pairs).
  *   All 2 * n_layers layers must share one precision; mixed precision is ESMB200_EINVAL. */

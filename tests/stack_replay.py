@@ -315,13 +315,16 @@ def key_blocks(slots: int):
     return (128,) if slots == 1 else (64,)
 
 
-def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,), prefix="", slots=1):
+def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,), prefix="", slots=1, qrows=None):
     """fp16 attention on the kernel's q, k, v (qkv [B*T, 3Ea] in head slots, sequences of T tokens, pad [B, T] bool):
-    ctx element-wise (attn_ctx_bound) and per (sequence, head) rel-Fro (attn_relfro_gate), probabilities and row sums
-    of the valid query rows.  The heads are taken 64 slots wide, their padding columns included (zeros add nothing to
-    q k^T or P v).  blocks: the key-block sizes the kernel may walk; the bound is the largest over them."""
+    ctx element-wise (attn_ctx_bound) and per (sequence, head) rel-Fro (attn_relfro_gate), probabilities [B, H, T, T]
+    and row sums at the query rows qrows [B, T] bool (None: the valid ones, ~pad).  The heads are taken 64 slots wide,
+    their padding columns included (zeros add nothing to q k^T or P v).  blocks: the key-block sizes the kernel may
+    walk; every bound is the largest over them."""
     q, k, v = (_heads(qkv, B, T, H, i, slots) for i in range(3))
     got = _heads(ctx, B, T, H, 0, slots).double()
+    if qrows is None:
+        qrows = ~pad.bool()
     terms = {bl: [0, 0, 0] for bl in blocks}
     err2 = 0
     for i0, r0 in kr.attention64_rows(q, k, v, pad, blocks[0]):
@@ -335,12 +338,14 @@ def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,)
             terms[bl] = [a + b for a, b in zip(terms[bl], t)]
         err2 = err2 + e.pow(2).sum((-1, -2))
         if probs is not None:
-            rows = ~pad.bool()[:, i0:i0 + n]
+            rows = qrows[:, i0:i0 + n]
             m = rows[:, None, :, None].expand_as(r0["p"])
             pr = probs[:, :, i0:i0 + n].double()
-            _worst(worst, prefix + "probs", _ratio((pr - r0["p"]).abs()[m], kr.attn_probs_bound(r0)[m]))
+            pb = torch.stack([kr.attn_probs_bound(r) for r in rs]).amax(0)
+            _worst(worst, prefix + "probs", _ratio((pr - r0["p"]).abs()[m], pb[m]))
             mr = rows[:, None, :].expand(B, H, n)
-            _worst(worst, prefix + "rowsum", _ratio((pr.sum(-1) - 1).abs()[mr], kr.attn_rowsum_bound(r0)[mr]))
+            rb = torch.stack([kr.attn_rowsum_bound(r) for r in rs]).amax(0)
+            _worst(worst, prefix + "rowsum", _ratio((pr.sum(-1) - 1).abs()[mr], rb[mr]))
         del rs, r0
     gate = torch.stack([kr.attn_relfro_combine(*terms[bl]) for bl in blocks]).amax(0)
     ctx2 = terms[blocks[0]][2]
@@ -349,9 +354,10 @@ def attention_stage_f16(worst, qkv, ctx, pad, B, T, H, probs=None, blocks=(128,)
     _worst(worst, prefix + "ctx_relfro_gate", float((fro[live] / gate[live]).max()))
 
 
-def attention_stage_split(worst, qkv, ctx, pad, B, T, H, probs=None, prefix=""):
+def attention_stage_split(worst, qkv, ctx, pad, B, T, H, probs=None, prefix="", qrows=None):
     """fp32x3 attention on the kernel's q, k, v hi | lo (qkv [B*T, 6E]): the split attention tests' element bound and
-    per-head gate, and the probabilities of the valid query rows"""
+    per-head gate, and the probabilities (test_gpu_attention_split.probs_bound) and row sums (kernel_refs
+    .attn_rowsum_bound on the split reference) at the query rows qrows [B, T] bool (None: ~pad)"""
     import test_gpu_attention_split as tas
     E = 64 * H
     r = tas.reference(qkv[:, :3 * E], qkv[:, 3 * E:], pad, B, T, H)
@@ -361,8 +367,31 @@ def attention_stage_split(worst, qkv, ctx, pad, B, T, H, probs=None, prefix=""):
     fro = (err.pow(2).sum((-1, -2)) / r["ctx"].pow(2).sum((-1, -2)).clamp_min(1e-300)).sqrt()
     _worst(worst, prefix + "ctx_relfro_gate", float((fro / tas.relfro_gate(r)).max()))
     if probs is not None:
-        m = (~pad.bool())[:, None, :, None].expand_as(r["p"])
-        _worst(worst, prefix + "probs", _ratio((probs.double() - r["p"]).abs()[m], tas.probs_bound(r)[m]))
+        if qrows is None:
+            qrows = ~pad.bool()
+        m = qrows[:, None, :, None].expand_as(r["p"])
+        pr = probs.double()
+        _worst(worst, prefix + "probs", _ratio((pr - r["p"]).abs()[m], tas.probs_bound(r)[m]))
+        mr = qrows[:, None, :].expand(B, H, T)
+        _worst(worst, prefix + "rowsum", _ratio((pr.sum(-1) - 1).abs()[mr], kr.attn_rowsum_bound(r)[mr]))
+
+
+def column_query_rows(cpad: torch.Tensor) -> torch.Tensor:
+    """[N, R] bool from the column sequences' key padding cpad [N, R]: every query row of a column with at least one
+    valid key.  The column attention masks keys only and keeps q at padded rows (axial_attention.py:211-217, no
+    zeroed rows in the stack), so a padded query row of a live column is a softmax row over the valid keys like any
+    other.  A column of padding only is written as 0 (the reference gives 1/R there) and is checked for that alone
+    (column_zero_stage)."""
+    return (~cpad.bool()).any(-1, keepdim=True).expand_as(cpad)
+
+
+def column_zero_stage(name: str, probs: torch.Tensor, cpad: torch.Tensor):
+    """the exact zeros of the column maps probs [N, H, R, R] under the key padding cpad [N, R]: every padded key of
+    every row, and every entry of a column whose keys are all padding"""
+    km = cpad.bool()[:, None, None, :].expand_as(probs)
+    assert bool((probs[km] == 0).all()), f"{name}: a padded key has probability"
+    dead = ~column_query_rows(cpad)[:, 0]
+    assert bool((probs[dead] == 0).all()), f"{name}: a column of padding only is not 0"
 
 
 def residual_stage(worst, name, a_op, w_op, bias, x_in, x_out, K, split):
@@ -557,12 +586,13 @@ def _column_major(t: torch.Tensor, B: int, R: int, C: int) -> torch.Tensor:
 
 
 def check_axial_stages(layer, pk: Dict, st: Dict, pad: Optional[torch.Tensor], B: int, R: int, C: int,
-                       precision: int, worst: Dict):
+                       precision: int, worst: Dict, col_probs: Optional[torch.Tensor] = None):
     """Every stage of one replayed AxialTransformerLayer against float64 on its own inputs: the three LayerNorms, the
     row and column QKV (row q scale fp32(d^-1/2 / sqrt(R)), q zero at padded tokens), the tied row attention end to
     end (tied_ctx_bound, tied_relfro_gate), the column attention (the fp16 or split attention bounds, per column
     sequence of R tokens, over both key-block sizes of the fp16 kernels), the two out-projections and the
-    feed-forward."""
+    feed-forward.  col_probs: the layer's column maps fp32 [B, C, H, R, R] (the stack's), checked at every query row of
+    every live column (column_query_rows) and exactly 0 where column_zero_stage says."""
     E, H, F = layer.embedding_dim, layer.num_heads, layer.ffn_embedding_dim
     split = precision == 1
     pf = 2 if split else 1
@@ -590,10 +620,15 @@ def check_axial_stages(layer, pk: Dict, st: Dict, pad: Optional[torch.Tensor], B
     cq, cc = _column_major(st["col_qkv"], B, R, C), _column_major(st["col_ctx"], B, R, C)
     cpad = pad.permute(0, 2, 1).reshape(B * C, R) if pad is not None else torch.zeros(B * C, R, dtype=torch.bool,
                                                                                          device=cq.device)
+    cp = qrows = None
+    if col_probs is not None:
+        cp = col_probs.view(B * C, H, R, R)
+        column_zero_stage("col_probs", cp, cpad)
+        qrows = column_query_rows(cpad)
     if split:
-        attention_stage_split(worst, cq, cc, cpad, B * C, R, H, prefix="col_")
+        attention_stage_split(worst, cq, cc, cpad, B * C, R, H, cp, prefix="col_", qrows=qrows)
     else:
-        attention_stage_f16(worst, cq, cc, cpad, B * C, R, H, blocks=(64, 128), prefix="col_")
+        attention_stage_f16(worst, cq, cc, cpad, B * C, R, H, cp, blocks=(64, 128), prefix="col_", qrows=qrows)
     residual_stage(worst, "row_out_proj", st["row_ctx"], pk["row_out"], layer.row_self_attention.layer.out_proj.bias,
                    st["x0"], st["x_row"], E, split)
     residual_stage(worst, "col_out_proj", st["col_ctx"], pk["col_out"],

@@ -23,7 +23,7 @@ if HERE not in sys.path:
     sys.path.insert(0, HERE)  # variant_fixtures
 
 import test_gpu_tied_attention as tied  # noqa: E402
-from test_gpu_msa import assert_maps_change_no_bit  # noqa: E402
+from test_gpu_msa import assert_maps_change_no_bit, col_maps_against_oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -216,7 +216,7 @@ def build_model(cfg, seed=None):
 def test_msa_transformer_fp32x3_against_reference_golden(name, golden_dir):
     fx = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
     cfg, tokens = fx["config"], fx["tokens"]
-    model, _ = build_model(cfg)
+    model, sd = build_model(cfg)
     model.set_precision("fp32x3")
     keep = tokens.ne(1)
     L = cfg["layers"]
@@ -232,11 +232,12 @@ def test_msa_transformer_fp32x3_against_reference_golden(name, golden_dir):
     qkeep = keep[:, :, :3].permute(0, 2, 1)                                     # [B, 3, R]
     cs = float((col - fx["col_attentions_sample"]).abs().permute(0, 3, 4, 1, 2, 5)[qkeep].max())
     ra3 = max_abs(out3["row_attentions"].cpu(), fx["row_attentions"])
+    c64 = col_maps_against_oracle(f"msa_precision model {name} fp32x3", sd, cfg, tokens, out3["col_attentions"])
     print(f"PARITY msa_precision model {name}: repr rel_fro {', '.join(f'{k}:{v:.3e}' for k, v in reprs.items())}; "
           f"logits rel_fro={lg:.3e}; row maps max_abs={ra:.3e} (need_head_weights {ra3:.3e}); column sample "
           f"max_abs={cs:.3e}; contacts max_abs={ct:.3e} (predict_contacts {pc:.3e})", flush=True)
     assert all(v <= 2e-5 for v in reprs.values()) and lg <= 2e-5
-    assert ra <= 5e-5 and ra3 <= 5e-5 and cs <= 5e-5
+    assert ra <= 5e-5 and ra3 <= 5e-5 and cs <= 5e-5 and c64 <= 5e-5
     assert ct <= 1e-4 and pc <= 1e-4
 
 

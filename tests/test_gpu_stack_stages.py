@@ -18,8 +18,8 @@ Cases (head_dim 64; random weights from oracle.weights, each stack cycling throu
     stages against float64;
   * MSA-1b (E 768, H 12), 12 layers: run_axial_stack against AxialTransformerLayer.forward_batch_major(need_probs=True)
     and the replay, layer after layer, at 2 x 32 x 256 padded, depths R = 6 and 17 (where fp32(0.125 / sqrt(R)) differs
-    from the reference's fp32(64 ** -0.5 / sqrt(R))), fp16 and fp32x3, with every stage against float64, and 128 x 512
-    in fp16;
+    from the reference's fp32(64 ** -0.5 / sqrt(R))), fp16 and fp32x3, with every stage against float64 (the column
+    maps at every query row of every live column), and 128 x 512 in fp16;
   * the pinned arena of esmb200_layer_offload against the test's own packing at head widths 16, 24, 32, 64 and 128.
 """
 import ctypes
@@ -365,8 +365,9 @@ def test_axial_stack_against_maps_path_and_replay(B, R, C, padded, precision):
     stages = C <= 256  # the float64 stages at 2 x 32 x 256 and the R = 6 / 17 depths; 128 x 512 is bit identity only
     worst = {}
     for i, layer in enumerate(layers):
-        ra = run_axial_stack([layer], xa, pad, row_attn_layers=[0])[0]
-        rb, _ = layer.forward_batch_major(xb, pad, need_probs=True)
+        ca = torch.full((B, C, H, R, R), float("nan"), device="cuda")
+        ra = run_axial_stack([layer], xa, pad, row_attn_layers=[0], col_attn={0: ca})[0]
+        rb, cb = layer.forward_batch_major(xb, pad, need_probs=True)
         rr = torch.empty(H, B, C, C, device="cuda")
         pk = sr.pack_axial(layer, precision)
         st = sr.replay_axial(layer, pk, xr.view(M, E), pad, B, R, C, precision, rr)
@@ -374,9 +375,17 @@ def test_axial_stack_against_maps_path_and_replay(B, R, C, padded, precision):
         assert torch.equal(xa, xb), f"layer {i}: run_axial_stack and forward_batch_major differ"
         assert torch.equal(xa, xr), f"layer {i}: run_axial_stack and the replay differ"
         assert torch.equal(ra, rb) and torch.equal(ra, rr), f"layer {i}: row attention maps differ"
+        # forward_batch_major returns the reference's [H,C,B,R,R]; the stack's buffer is [B,C,H,R,R]
+        assert torch.equal(cb, ca.permute(2, 1, 0, 3, 4)), f"layer {i}: column attention maps differ"
+        del cb
         if stages:
-            sr.check_axial_stages(layer, pk, st, pad, B, R, C, precision, worst)
-        del st
+            sr.check_axial_stages(layer, pk, st, pad, B, R, C, precision, worst, col_probs=ca)
+        else:
+            cpad = (pad.permute(0, 2, 1).reshape(B * C, R) if pad is not None else
+                    torch.zeros(B * C, R, dtype=torch.bool, device="cuda"))
+            assert not bool(ca.isnan().any()), f"layer {i}: a column map was not written"
+            sr.column_zero_stage("col_probs", ca.view(B * C, H, R, R), cpad)
+        del st, ca
     label = f"MSA {B}x{R}x{C} padded={padded} p{precision}"
     for name, r in worst.items():
         report(f"stack stage {label} {name}", worst_over_layers=r)

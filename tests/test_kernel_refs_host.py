@@ -957,3 +957,53 @@ def test_qkv_heads_bound_holds_and_refuses_a_wrong_slot_or_table_column(d):
     if kr.head_slots(E, H) == 2:
         other = cols + torch.where((cols // 64) % 2 == 0, 64, -64)  # the head's other slot, same columns
         assert ratio(_emulate_qkv(a, w, bias, d, H, T, cos_s, sin_s, other)) > 10
+
+
+# ---- the column attention maps (tests/stack_replay.py column_query_rows, column_zero_stage, qrows) -------------------
+def test_column_query_rows_are_every_row_of_a_live_column():
+    import stack_replay as sr
+    cpad = torch.tensor([[False, False, True], [True, True, True], [True, False, True]])
+    want = torch.tensor([[True] * 3, [False] * 3, [True] * 3])
+    assert torch.equal(sr.column_query_rows(cpad), want)
+
+
+def test_column_zero_stage_refuses_a_padded_key_or_a_dead_column_with_probability():
+    import stack_replay as sr
+    cpad = torch.tensor([[False, True], [True, True]])
+    p = torch.zeros(2, 1, 2, 2)
+    p[0, 0, :, 0] = 1.0
+    sr.column_zero_stage("maps", p, cpad)
+    for idx in ((0, 0, 1, 1), (1, 0, 0, 0)):
+        bad = p.clone()
+        bad[idx] = 2.0 ** -126
+        with pytest.raises(AssertionError):
+            sr.column_zero_stage("maps", bad, cpad)
+
+
+def test_attention_stage_f16_checks_the_padded_query_rows_it_is_given():
+    """float64 column maps rounded to fp32 pass attention_stage_f16 at every query row of the live columns; the padded
+    query rows zeroed (esm2.py's stacked-map rule, wrong for the column attention) fail it, and go unseen with the
+    default selection of the valid rows only"""
+    import stack_replay as sr
+    N, R, H = 3, 70, 2
+    g = torch.Generator().manual_seed(11)
+    qkv = torch.randn(N * R, 3 * 64 * H, generator=g)
+    qkv[:, :64 * H] *= 0.25
+    qkv = qkv.half()
+    cpad = torch.zeros(N, R, dtype=torch.bool)
+    cpad[1, 40:] = True
+    cpad[2] = True
+    q, k, v = (sr._heads(qkv, N, R, H, i) for i in range(3))
+    r = kr.attention64(q, k, v, cpad, 64)
+    ctx = r["ctx"].transpose(1, 2).reshape(N * R, 64 * H).half()
+    probs = r["p"].float()
+    qrows = sr.column_query_rows(cpad)
+    worst = {}
+    sr.attention_stage_f16(worst, qkv, ctx, cpad, N, R, H, probs, blocks=(64, 128), qrows=qrows)
+    assert worst["probs"] <= 1.0 and worst["rowsum"] <= 1.0, worst
+    bad = probs.clone()
+    bad[1, :, 40:] = 0.0
+    sr.attention_stage_f16({}, qkv, ctx, cpad, N, R, H, bad, blocks=(64, 128))  # valid rows only: unseen
+    worst = {}
+    sr.attention_stage_f16(worst, qkv, ctx, cpad, N, R, H, bad, blocks=(64, 128), qrows=qrows)
+    assert worst["probs"] > 1e3 and worst["rowsum"] > 1e3, worst
