@@ -66,6 +66,8 @@ EXPORTS = (
     "esmb200_stack_contacts_bytes",
     "esmb200_stack_contacts",
     "esmb200_window_merge",
+    "esmb200_jacobian_scratch_bytes",
+    "esmb200_jacobian_contacts",
 )
 
 ABI_VERSION = 3
@@ -164,6 +166,10 @@ def _declare(lib):
     lib.esmb200_window_merge.restype = c_int32
     lib.esmb200_window_merge.argtypes = [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
                                          c_int64, c_void_p]
+    lib.esmb200_jacobian_scratch_bytes.restype = c_size_t
+    lib.esmb200_jacobian_scratch_bytes.argtypes = [c_int32]
+    lib.esmb200_jacobian_contacts.restype = c_int32
+    lib.esmb200_jacobian_contacts.argtypes = [c_void_p, c_int32, c_void_p, c_size_t, c_void_p, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -25,6 +25,7 @@
 #include "elementwise.cuh"
 #include "gemm2.cuh"
 #include "gemm_fp8.cuh"
+#include "jacobian.cuh"
 #include "tied_attention.cuh"
 
 using namespace esmb200;
@@ -54,7 +55,7 @@ int fail_cuda(cudaError_t e, const char* what) {
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
                      T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
-                     T_WINDOW_MERGE, T_COUNT };
+                     T_WINDOW_MERGE, T_JACOBIAN, T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1604,6 +1605,51 @@ int esmb200_window_merge(const float* src, int64_t src_ld, const int64_t* idx, c
   window_merge_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(src, src_ld, idx, w, seg, rows, C,
                                                                                   out, out_ld);
   CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
+
+size_t esmb200_jacobian_scratch_bytes(int32_t L) { return L < 2 ? 0 : jacobian_scratch(nullptr, L).bytes; }
+
+int esmb200_jacobian_contacts(const float* jac, int32_t L, void* scratch, size_t scratch_bytes, float* contacts,
+                              void* stream) {
+  if (L < 2 || L > 65535) return fail(ESMB200_EINVAL, "jacobian_contacts needs 2 <= L <= 65535");
+  if (!jac || !scratch || !contacts) return fail(ESMB200_EINVAL, "null argument");
+  const JacobianScratch s = jacobian_scratch(static_cast<char*>(scratch), L);
+  if (scratch_bytes < s.bytes) return fail(ESMB200_EINVAL, "scratch smaller than esmb200_jacobian_scratch_bytes(L)");
+  if (reinterpret_cast<uintptr_t>(scratch) % 256 != 0) return fail(ESMB200_EINVAL, "scratch must be 256-byte aligned");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const unsigned tiles = (unsigned)((L + kJacTileJ - 1) / kJacTileJ);
+  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
+    ProfScope ps(T_JACOBIAN, st);
+    jacobian_marginals_kernel<<<dim3(tiles, kJacAA), 320, 0, st>>>(jac, L, s.s_i, s.part);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_JACOBIAN, st);
+    const size_t n = (size_t)L * kJacAA * kJacAA + kJacAA * kJacAA;
+    jacobian_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(s.s_i, s.part, L, s.s_j, s.s);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_JACOBIAN, st);
+    const dim3 grid((unsigned)((L + kJacNormJ - 1) / kJacNormJ), (unsigned)L);
+    jacobian_norms_kernel<<<grid, kJacNormJ * kJacAA, 0, st>>>(jac, s.s_i, s.s_j, s.s, L, s.n);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_JACOBIAN, st);
+    jacobian_apc_sums_kernel<<<(unsigned)((L + 255) / 256 + (L + 7) / 8), 256, 0, st>>>(s.n, L, s.row, s.col);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_JACOBIAN, st);
+    const size_t blocks = ((size_t)L * L + 255) / 256;
+    jacobian_apc_kernel<<<(unsigned)(blocks < 1024 ? blocks : 1024), 256, 0, st>>>(s.n, s.row, s.col, L, contacts);
+    CK(cudaGetLastError());
+  }
   return ESMB200_OK;
 }
 

@@ -244,6 +244,22 @@ int esmb200_log_softmax_rows(const float* logits, int64_t ld, int32_t n, int32_t
 int esmb200_window_merge(const float* src, int64_t src_ld, const int64_t* idx, const float* w, const int64_t* seg,
                          int32_t rows, int32_t C, float* out, int64_t out_ld, void* stream);
 
+/* Categorical Jacobian contact map (esm_b200/jacobian.py; Zhang, Wayment-Steele, Brixi, Wang, Kern & Ovchinnikov,
+ * PNAS 2024). A new operation with no reference code; its definition, for one protein of L residues:
+ *   jac [L,20,L,20] fp32: J[i,a,j,b] = how the logit of amino acid b at residue j moves when residue i is set to amino
+ *     acid a (20 amino acids "LAGVSERTIDPKQNFYMHWC"). Read only, never modified.
+ *   Jc = J centred along each of its four axes (minus the mean over that axis; the four projections commute);
+ *   N[i,j] = sqrt(sum_{a,b} Jc[i,a,j,b]^2), N[i,i] = 0;
+ *   A = N - N.sum(1, keepdim) * N.sum(0, keepdim) / N.sum() (APC, as esm/modules.py:32-41), A[i,i] = 0;
+ *   contacts [L,L] fp32 = (A + A^T) / 2. An all-zero J gives NaN off the diagonal (0 / 0), as the definition does.
+ * Two passes over J (its marginal sums, then one 20 x 20 block norm per (i,j)) and a small L x L pass; every sum is
+ * taken in fp64 in a fixed order, without atomics: the result is bit-reproducible. scratch:
+ * esmb200_jacobian_scratch_bytes(L) bytes, 256-byte aligned (fp64 marginals and N, about 58 L^2 + 6,400 L bytes:
+ * about 1/25 of J). 2 <= L <= 65535, else ESMB200_EINVAL, as is too little scratch; scratch_bytes(L < 2) is 0. */
+size_t esmb200_jacobian_scratch_bytes(int32_t L);
+int esmb200_jacobian_contacts(const float* jac, int32_t L, void* scratch, size_t scratch_bytes, float* contacts,
+                              void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -362,7 +378,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *   synchronising on the recorded events, and resets the record list.
  *   tags: 0 LN1->f16, 1 QKV+RoPE GEMM, 2 attention, 3 out-proj GEMM, 4 LN2->f16, 5 fc1+GELU GEMM, 6 fc2 GEMM,
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
- *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring) */
+ *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
+ *         18 window merge, 19 categorical Jacobian contacts (each of its kernels) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
