@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint8, c_void_p
+from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_size_t, c_uint8, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ESMB200_LIB_PATH") or os.path.join(_HERE, "libesmb200.so")  # override: developer builds
@@ -68,6 +68,8 @@ EXPORTS = (
     "esmb200_window_merge",
     "esmb200_jacobian_scratch_bytes",
     "esmb200_jacobian_contacts",
+    "esmb200_sample_order",
+    "esmb200_sample_rows",
 )
 
 ABI_VERSION = 3
@@ -170,6 +172,11 @@ def _declare(lib):
     lib.esmb200_jacobian_scratch_bytes.argtypes = [c_int32]
     lib.esmb200_jacobian_contacts.restype = c_int32
     lib.esmb200_jacobian_contacts.argtypes = [c_void_p, c_int32, c_void_p, c_size_t, c_void_p, c_void_p]
+    lib.esmb200_sample_order.restype = c_int32
+    lib.esmb200_sample_order.argtypes = [c_void_p, c_int32, c_int32, c_int64, c_int64, c_uint64, c_void_p, c_void_p]
+    lib.esmb200_sample_rows.restype = c_int32
+    lib.esmb200_sample_rows.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_float, c_uint64, c_int64, c_int64,
+                                        c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -241,11 +241,23 @@ mean_pool_kernel(const float* __restrict__ x, const int* __restrict__ lengths, f
   }
 }
 
-// log_softmax over the first V <= 64 columns of each row: one warp per row, lane l holds columns l and l + 32. The
-// arithmetic follows PyTorch's warp-per-row softmax for rows of at most 64 elements: row max, per-lane sum of
-// expf(x - max) in column order, xor-butterfly sums, then (x - max) - logf(sum). expf / logf are the accurate library
-// functions, not ex2.approx. target == nullptr: out [n, V]; otherwise out[i] = the value of column target[i] (in [0, V),
-// checked by the caller).
+// Row max m and lse = logf(sum of expf(x - m)) of a row of at most 64 columns held by one warp, lane l holding
+// columns l (v0) and l + 32 (v1), -INFINITY past the row's end. The arithmetic follows PyTorch's warp-per-row softmax:
+// row max, per-lane sum in column order, xor-butterfly sums. expf / logf are the accurate library functions, not
+// ex2.approx. Every lane gets m and lse.
+__device__ __forceinline__ void warp_row_lse(float v0, float v1, float& m, float& lse) {
+  m = fmaxf(v0, v1);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  float s = expf(v0 - m);
+  s += expf(v1 - m);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  lse = logf(s);
+}
+
+// log_softmax over the first V <= 64 columns of each row: one warp per row (warp_row_lse), then (x - max) - lse.
+// target == nullptr: out [n, V]; otherwise out[i] = the value of column target[i] (in [0, V), checked by the caller).
 __global__ void __launch_bounds__(256)
 log_softmax_rows_kernel(const float* __restrict__ logits, int64_t ld, int n, int V, const int64_t* __restrict__ target,
                         float* __restrict__ out) {
@@ -255,14 +267,8 @@ log_softmax_rows_kernel(const float* __restrict__ logits, int64_t ld, int n, int
   const float* x = logits + (size_t)row * ld;
   const float v0 = lane < V ? x[lane] : -INFINITY;
   const float v1 = lane + 32 < V ? x[lane + 32] : -INFINITY;
-  float m = fmaxf(v0, v1);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  float s = expf(v0 - m);
-  s += expf(v1 - m);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float lse = logf(s);
+  float m, lse;
+  warp_row_lse(v0, v1, m, lse);
   if (target) {
     if (lane == 0) out[row] = (x[target[row]] - m) - lse;
   } else {

@@ -79,6 +79,13 @@ def _check(model, tokens) -> torch.Tensor:
     if model.precision == "fp8":
         raise ValueError("categorical_jacobian refuses fp8 precision: its logits carry about 5 % relative error, more "
                          "than the substitution effects the Jacobian measures; use fp16 or fp32x3")
+    return _framed_protein(model, tokens, "the categorical Jacobian")
+
+
+def _framed_protein(model, tokens, what: str) -> torch.Tensor:
+    """The framing checks the categorical Jacobian and the sampler share, before any launch: tokens is one unpadded
+    protein [1, T] of integers with <cls> first, <eos> last and at least 2 residues (`what` names the caller in the
+    last message). Returns tokens as int64 [1, T] on the host."""
     tokens = torch.as_tensor(tokens)
     if tokens.dtype.is_floating_point or tokens.dtype == torch.bool:
         raise ValueError(f"tokens must be an integer tensor, got {tokens.dtype}")
@@ -91,7 +98,7 @@ def _check(model, tokens) -> torch.Tensor:
     if T < 2 or int(tokens[0, 0]) != model.cls_idx or int(tokens[0, -1]) != model.eos_idx:
         raise ValueError("tokens must start with <cls> and end with <eos>")
     if T - 2 < 2:
-        raise ValueError(f"the categorical Jacobian needs at least 2 residues, got {T - 2}")
+        raise ValueError(f"{what} needs at least 2 residues, got {T - 2}")
     return tokens
 
 

@@ -260,6 +260,35 @@ size_t esmb200_jacobian_scratch_bytes(int32_t L);
 int esmb200_jacobian_contacts(const float* jac, int32_t L, void* scratch, size_t scratch_bytes, float* contacts,
                               void* stream);
 
+/* Gibbs sampling of protein sequences (esm_b200/sampling.py). A new operation with no reference code. Random stream:
+ * R(c0, c1, c2, c3) = Philox4x32-10 (curand_Philox4x32_10) with counter (c0, c1, c2, c3) and key (seed mod 2^32,
+ * seed >> 32): four uint32 words. A word r maps to u = ((r >> 8) + 0.5) * 2^-24 rounded toward zero to fp32, which
+ * lies in (0, 1) and is exact for u < 1/2. Every draw depends only on (seed, chain, step, position), never on how the
+ * chains are batched.
+ * esmb200_sample_order: the visiting order of one sweep. keys int64 [n_chains, n]:
+ *     keys[c, j] = R(sweep, chain0 + c, p, 0).x * 65536 + p,   p = positions[j],
+ *   for the n designable residue indices positions int64 [n] (device; distinct, each in [0, 65535), checked by the
+ *   caller). Sorting each row ascending (keys are distinct) and taking key mod 65536 gives the order; the caller sorts.
+ *   n > 0, chain0 + n_chains <= 2^32, 0 <= sweep < 2^32, else ESMB200_EINVAL. n_chains == 0 launches nothing.
+ * esmb200_sample_rows: one block update of step `step` for n / per_chain chains, one warp per row, any n. Row r
+ *   belongs to chain chain0 + r / per_chain (local chain r / per_chain) and resamples residue p = positions[r]
+ *   (int64 [n], device; p in [0, T - 2), checked by the caller: a row outside writes no token and a NaN logq).
+ *   logits fp32 [n, ld]: the LM-head row of token 1 + p of that chain's masked copy. For a < 20:
+ *     z_a = logits[r, aa_offset + a] / temperature (fp32 division),
+ *     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(step, chain, p, 1 + a div 4),
+ *     a* = argmax_a (z_a + g_a), a tie to the smallest a;
+ *   tokens int64 [n / per_chain, T] (the chains' state) gets aa_offset + a* at [r / per_chain, 1 + p], in place;
+ *   logq fp32 [n] gets (z_a* - max z) - logf(sum_a expf(z_a - max z)), bit for bit esmb200_log_softmax_rows' value
+ *   with target a* on the 20 columns z. logp: NULL, or fp32 with logp[c * logp_stride] = the per_chain logq of local
+ *   chain c summed in row order (fp32, from +0). ld >= aa_offset + 20, finite temperature > 0, T >= 3, per_chain > 0
+ *   dividing n, chain0 + n / per_chain <= 2^32 and 0 <= step < 2^32, else ESMB200_EINVAL, before any launch. n == 0
+ *   launches nothing. Deterministic, no atomics. */
+int esmb200_sample_order(const int64_t* positions, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
+                         uint64_t seed, int64_t* keys, void* stream);
+int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, int32_t aa_offset, float temperature,
+                        uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain, const int64_t* positions,
+                        int64_t* tokens, int32_t T, float* logq, float* logp, int64_t logp_stride, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -379,7 +408,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *   tags: 0 LN1->f16, 1 QKV+RoPE GEMM, 2 attention, 3 out-proj GEMM, 4 LN2->f16, 5 fc1+GELU GEMM, 6 fc2 GEMM,
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
- *         18 window merge, 19 categorical Jacobian contacts (each of its kernels) */
+ *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
+ *         and each kernel of esmb200_sample_rows) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
