@@ -70,6 +70,8 @@ EXPORTS = (
     "esmb200_jacobian_contacts",
     "esmb200_sample_order",
     "esmb200_sample_rows",
+    "esmb200_msa_sample_order",
+    "esmb200_sample_rows_set",
 )
 
 ABI_VERSION = 3
@@ -177,6 +179,13 @@ def _declare(lib):
     lib.esmb200_sample_rows.restype = c_int32
     lib.esmb200_sample_rows.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_float, c_uint64, c_int64, c_int64,
                                         c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_void_p]
+    lib.esmb200_msa_sample_order.restype = c_int32
+    lib.esmb200_msa_sample_order.argtypes = [c_void_p, c_int32, c_int32, c_int64, c_int64, c_uint64, c_void_p,
+                                             c_void_p]
+    lib.esmb200_sample_rows_set.restype = c_int32
+    lib.esmb200_sample_rows_set.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_float, c_uint64, c_int64,
+                                            c_int64, c_int32, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
+                                            c_void_p, c_int64, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -389,6 +389,26 @@ class MSATransformer(nn.Module):
                 start = stop
         return tokens, x, hidden, row_attn, col_attn
 
+    def _stack_unpadded(self, tokens: torch.Tensor) -> torch.Tensor:
+        """`_stack` for contiguous tokens [B,R,C] on the device that the caller has checked hold no <pad> and fit the
+        position embeddings: the embedding prologue and one axial-stack call without a padding mask. It never reads
+        tokens back to the host, so loops over it (sampling.msa_gibbs) do not synchronise. Returns the fp32 residual
+        stream [B,R,C,E] before emb_layer_norm_after."""
+        lib = _lib.load()
+        B, R, C = tokens.shape
+        E = self.args.embed_dim
+        mp = self.msa_position_embedding
+        dev = tokens.device
+        with torch.cuda.device(dev):
+            x = torch.empty((B, R, C, E), dtype=torch.float32, device=dev)
+            ln = self.emb_layer_norm_before
+            _lib.check(lib.esmb200_msa_embed(_ptr(tokens), _ptr(self.embed_tokens.weight),
+                                             _ptr(self.embed_positions.weight), _ptr(mp),
+                                             mp.shape[-1] if mp is not None else 0, _ptr(ln.weight), _ptr(ln.bias),
+                                             ln.eps, _ptr(x), B, R, C, E, self.padding_idx, _stream()))
+            run_axial_stack(list(self.layers), x)
+        return x
+
     def predict_contacts(self, tokens):
         """msa_transformer.py:222-223; only the contacts are returned, so the column attention maps are not built."""
         prev = self.contacts_without_col_attentions

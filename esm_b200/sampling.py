@@ -39,6 +39,35 @@ every max_tokens.
 
 Cost: each step is one stack call on C copies of T tokens (in chunks); the sampler kernel and the head on C k rows
 are small beside it.
+
+Alignments from the MSA Transformer:
+
+    out = sampling.msa_gibbs(model, tokens, designable=None, chains=1, sweeps=1, block=1, temperature=1.0, seed=0,
+                             gaps=True, max_tokens=None)
+    out["tokens"]   # int64 [chains, R, C] on the model's device
+    out["logp"]     # fp32 [chains, steps]
+
+Definition. tokens [1, R, C] is one alignment in the MSA alphabet: column 0 of every row is <cls>, there is no <pad>
+and no <eos>, R <= 1024 (the MSA position embedding) and 2 <= C <= max_positions. The residue entries are (r, j),
+1 <= j < C, with the flat index p = r * (C - 1) + (j - 1) < 2^20. designable is None (every entry) or bool [R, C - 1];
+every other entry is fixed and never changes. A <mask> is allowed at a designable entry only, so <mask> rows appended
+to a real alignment generate new family members. The drawable tokens A are the 20 amino acids of
+jacobian.AMINO_ACIDS in that order and, with gaps=True, the gap "-" as A[20]. n is the number of designable entries
+and k = min(block, n). Every chain starts from tokens.
+
+For each sweep w and chain c, the designable p are sorted ascending by R(w, c, p, 0).x * 2^20 + p and cut into blocks
+of k; steps s count the blocks over all sweeps. In step s the chain's tokens with <mask> at the block's entries run
+through the axial stack, and the fp32 LM-head logits l at those entries only give, for each p and a < |A|,
+z_a = fp32(l[A_a] / temperature) and g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(s, c, p, 1 + a div 4) by the
+uniform map above. The new token is A[argmax_a (z_a + g_a)], a tie to the smaller a; the block's entries are written
+together. log q is esmb200_log_softmax_rows' value over the |A| tempered columns, and logp[c, s] the block's log q
+summed in block order (fp32). Since x dominates both order keys, an alignment of one row with gaps=False and the same
+logits draws what gibbs' kernel (esmb200_sample_rows) draws, with the same log q.
+
+Execution as for gibbs, with chains of R * C tokens in chunks of at most max_tokens (at least one chain), the order
+from esmb200_msa_sample_order and the draw from esmb200_sample_rows_set. The stack runs without a padding mask
+(MSATransformer._stack_unpadded), so nothing in the sweep loop waits for the host, and the result is the same bits for
+every max_tokens.
 """
 from __future__ import annotations
 
@@ -50,12 +79,14 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
-from .jacobian import _amino_acid_offset, _framed_protein
+from .jacobian import AMINO_ACIDS, _amino_acid_offset, _framed_protein
 from .model import ProteinLanguageModel, _ptr, _stream
 from .variants import _copies_per_chunk, _device
 
 _COUNTER = 1 << 32  # chains and steps are Philox counter words
 _MAX_RESIDUES = 65535  # the order key holds the position in 16 bits
+_MAX_MSA_ROWS = 1024  # the MSA position embedding
+_MAX_ENTRIES = 1 << 20  # the order key holds the entry index in 20 bits
 
 
 def _count(name: str, v) -> int:
@@ -95,12 +126,18 @@ def _check(model, tokens, positions, chains, sweeps, block, temperature, seed):
     fixed[pos] = False
     if bool((host[0, 1:L + 1][fixed] == model.mask_idx).any()):
         raise ValueError("a <mask> token may only sit at a designable position")
+    return (host, pos) + _check_run(pos.numel(), "positions", chains, sweeps, block, temperature, seed)
+
+
+def _check_run(n, what, chains, sweeps, block, temperature, seed):
+    """The checks gibbs and msa_gibbs share for n designable `what`: counts, the Philox counter ranges of chains and
+    steps, temperature and seed. Returns (temperature as fp32, chains, sweeps, block, seed)."""
     chains, sweeps, block = _count("chains", chains), _count("sweeps", sweeps), _count("block", block)
     if chains > _COUNTER:
         raise ValueError(f"chains must be at most 2^32, got {chains}")
-    k = min(block, pos.numel())
-    if sweeps * -(-pos.numel() // k) > _COUNTER:
-        raise ValueError("sweeps * ceil(|positions| / block) must be at most 2^32")
+    k = min(block, n)
+    if sweeps * -(-n // k) > _COUNTER:
+        raise ValueError(f"sweeps * ceil(|{what}| / block) must be at most 2^32")
     t = float(temperature)
     if not math.isfinite(t) or t <= 0:
         raise ValueError(f"temperature must be finite and > 0, got {temperature!r}")
@@ -109,7 +146,7 @@ def _check(model, tokens, positions, chains, sweeps, block, temperature, seed):
         raise ValueError(f"temperature {temperature!r} is not a finite positive fp32 value")
     if isinstance(seed, bool) or not isinstance(seed, numbers.Integral) or not 0 <= seed < 1 << 64:
         raise ValueError(f"seed must be an integer in [0, 2^64), got {seed!r}")
-    return host, pos, t32, chains, sweeps, block, int(seed)
+    return t32, chains, sweeps, block, int(seed)
 
 
 @torch.no_grad()
@@ -162,4 +199,114 @@ def gibbs(model, tokens: torch.Tensor, positions: Optional[Sequence[int]] = None
                     _lib.check(lib.esmb200_sample_rows(_ptr(logits), logits.stride(0), m * kb, aa0, tau, seed, s, c0,
                                                        kb, _ptr(blk), _ptr(state), T, _ptr(logq),
                                                        _ptr(logp[c0:, s]), steps, _stream()))
+    return {"tokens": out, "logp": logp}
+
+
+def _check_msa(model, tokens, designable, chains, sweeps, block, temperature, seed):
+    """The refusals of msa_gibbs, all before any launch. Returns (host tokens int64 [1, R, C], designable entries p
+    int64 [n] ascending on the host, temperature as fp32, chains, sweeps, block, seed)."""
+    from .msa import MSATransformer
+    if isinstance(model, ProteinLanguageModel):
+        raise ValueError("msa_gibbs samples alignments from the MSA Transformer; for ESM-2, ESM-1b and ESM-1v use "
+                         "sampling.gibbs")
+    if not isinstance(model, MSATransformer):
+        raise ValueError(f"msa_gibbs needs an MSATransformer, got {type(model).__name__}")
+    host = torch.as_tensor(tokens)
+    if host.dtype.is_floating_point or host.dtype == torch.bool:
+        raise ValueError(f"tokens must be an integer tensor, got {host.dtype}")
+    if host.dim() != 3 or host.shape[0] != 1:
+        raise ValueError(f"tokens must be one alignment [1, R, C], got shape {tuple(host.shape)}")
+    host = host.cpu().long()
+    _, R, C = host.shape
+    if C < 2:
+        raise ValueError(f"an alignment needs C >= 2 columns (<cls> and a residue), got {C}")
+    if R > _MAX_MSA_ROWS:
+        raise ValueError(f"msa_gibbs takes at most {_MAX_MSA_ROWS} rows, got {R}")
+    if C > model.embed_positions.max_positions:
+        raise ValueError(f"C = {C} is above the model's max_positions {model.embed_positions.max_positions}")
+    if R * (C - 1) > _MAX_ENTRIES:
+        raise ValueError(f"msa_gibbs takes at most 2^20 residue entries R * (C - 1), got {R * (C - 1)}")
+    if bool((host == model.padding_idx).any()) or bool((host == model.eos_idx).any()):
+        raise ValueError("tokens must be one unpadded alignment with no <pad> and no <eos>")
+    if not bool((host[0, :, 0] == model.cls_idx).all()):
+        raise ValueError("every row of the alignment must start with <cls>")
+    if designable is None:
+        des = torch.ones((R, C - 1), dtype=torch.bool)
+    else:
+        des = torch.as_tensor(designable)
+        if des.dtype != torch.bool or tuple(des.shape) != (R, C - 1):
+            raise ValueError(f"designable must be a bool tensor of shape [R, C - 1] = [{R}, {C - 1}], got "
+                             f"{des.dtype} {tuple(des.shape)}")
+        des = des.cpu()
+        if not bool(des.any()):
+            raise ValueError("designable must hold at least one True entry")
+    if bool((host[0, :, 1:][~des] == model.mask_idx).any()):
+        raise ValueError("a <mask> token may only sit at a designable entry")
+    entries = des.reshape(-1).nonzero().reshape(-1)
+    return (host, entries) + _check_run(entries.numel(), "designable", chains, sweeps, block, temperature, seed)
+
+
+def _drawable(model, gaps: bool):
+    """The token ids of A: the 20 amino acids in AMINO_ACIDS order, then "-" when gaps."""
+    ids = [model.alphabet.get_idx(c) for c in AMINO_ACIDS + ("-" if gaps else "")]
+    if len(set(ids)) != len(ids) or model.alphabet.unk_idx in ids:
+        raise ValueError("the model's alphabet does not hold the 20 amino acids and the gap as distinct tokens")
+    return ids
+
+
+@torch.no_grad()
+def msa_gibbs(model, tokens: torch.Tensor, designable: Optional[torch.Tensor] = None, chains: int = 1, sweeps: int = 1,
+              block: int = 1, temperature: float = 1.0, seed: int = 0, gaps: bool = True,
+              max_tokens: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """Gibbs sampling from an MSATransformer (fp16 or fp32x3) started at one alignment tokens [1, R, C], by the
+    definition in the module docstring. Returns {"tokens": int64 [chains, R, C], "logp": fp32 [chains, sweeps *
+    ceil(n / block)]} on the model's device, n the number of designable entries. The result does not depend on
+    max_tokens (default variants.DEFAULT_MAX_TOKENS tokens per stack call, at least one chain). Refused with ValueError
+    before any launch: a sequence model (use gibbs), tokens that are not one alignment [1, R, C] with <cls> in column 0
+    and no <pad> or <eos>, C < 2, R > 1024, C > max_positions, more than 2^20 residue entries (a model with
+    max_positions above 1025), a <mask> at a fixed entry, a designable that is not bool [R, C - 1] with a True entry,
+    chains, sweeps or block below 1, chains or steps above 2^32, a temperature that is not finite and > 0, and a seed
+    outside [0, 2^64)."""
+    host, entries, tau, chains, sweeps, block, seed = _check_msa(model, tokens, designable, chains, sweeps, block,
+                                                                 temperature, seed)
+    drawable = _drawable(model, bool(gaps))
+    _, R, C = host.shape
+    W = C - 1
+    n = entries.numel()
+    k = min(block, n)
+    blocks = -(-n // k)
+    steps = sweeps * blocks
+    lib = _lib.load()
+    dev = _device(model)
+    if dev.type != "cuda":
+        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model to the GPU; no CPU fallback")
+    tok, entries = host.to(dev), entries.to(dev)
+    token_set = torch.tensor(drawable, dtype=torch.int32, device=dev)
+    out = torch.empty((chains, R, C), dtype=torch.int64, device=dev)
+    logp = torch.empty((chains, steps), dtype=torch.float32, device=dev)
+    per = _copies_per_chunk(R * C, max_tokens)
+    with torch.cuda.device(dev):
+        for c0 in range(0, chains, per):
+            m = min(per, chains - c0)
+            state = out[c0:c0 + m]  # the chains' alignments, updated in place by esmb200_sample_rows_set
+            state.copy_(tok.expand(m, R, C))
+            base = torch.arange(m, device=dev).unsqueeze(1) * (R * C)  # flat token of each copy's (0, 0)
+            for w in range(sweeps):
+                keys = torch.empty((m, n), dtype=torch.int64, device=dev)
+                _lib.check(lib.esmb200_msa_sample_order(_ptr(entries), n, m, c0, w, seed, _ptr(keys), _stream()))
+                order = keys.sort(dim=1).values.bitwise_and_((1 << 20) - 1)  # key mod 2^20 = the entry
+                for b in range(blocks):
+                    s = w * blocks + b
+                    blk = order[:, b * k:(b + 1) * k].contiguous()
+                    kb = blk.shape[1]
+                    flat = (base + blk + blk.div(W, rounding_mode="floor") + 1).view(-1)  # (p / W) C + 1 + p % W
+                    batch = state.clone()
+                    batch.view(-1).index_fill_(0, flat, model.mask_idx)
+                    x = model._stack_unpadded(batch)
+                    logits = model._lm_head_rows(x.view(-1, x.shape[-1]).index_select(0, flat))
+                    logq = torch.empty(m * kb, dtype=torch.float32, device=dev)
+                    _lib.check(lib.esmb200_sample_rows_set(_ptr(logits), logits.stride(0), m * kb, _ptr(token_set),
+                                                           len(drawable), tau, seed, s, c0, kb, _ptr(blk),
+                                                           _ptr(state), R * C, R, C, _ptr(logq), _ptr(logp[c0:, s]),
+                                                           steps, _stream()))
     return {"tokens": out, "logp": logp}

@@ -289,6 +289,34 @@ int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, int32_t aa_o
                         uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain, const int64_t* positions,
                         int64_t* tokens, int32_t T, float* logq, float* logp, int64_t logp_stride, void* stream);
 
+/* Gibbs sampling of MSA Transformer alignments (esm_b200/sampling.py, msa_gibbs), on the random stream above. An
+ * alignment has R rows and C columns, column 0 <cls>; its residue entries (r, j), 1 <= j < C, have the flat index
+ * p = r * (C - 1) + (j - 1) < 2^20 (R <= 1024, C <= 1025).
+ * esmb200_msa_sample_order: the visiting order of one sweep. keys int64 [n_chains, n]:
+ *     keys[c, j] = R(sweep, chain0 + c, p, 0).x * 2^20 + p,   p = entries[j],
+ *   for the n designable entries entries int64 [n] (device; distinct, each in [0, 2^20), checked by the caller).
+ *   Sorting each row ascending and taking key mod 2^20 gives the order. Argument checks as esmb200_sample_order's.
+ * esmb200_sample_rows_set: one block update of step `step` for n / per_chain chains over the drawable token ids
+ *   token_set int32 [n_tokens] (device, 1 <= n_tokens <= 32, each in [0, ld), checked by the caller), one warp per row,
+ *   any n. Row r belongs to chain chain0 + r / per_chain (local chain r / per_chain) and resamples entry
+ *   p = entries[r] (int64 [n], device). logits fp32 [n, ld]: the LM-head row of that entry of the chain's masked
+ *   copy. For a < n_tokens:
+ *     z_a = logits[r, token_set[a]] / temperature (fp32 division),
+ *     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(step, chain, p, 1 + a div 4),
+ *     a* = argmax_a (z_a + g_a), a tie to the smallest a;
+ *   tokens int64 (the chains' alignments, chain c at tokens + c * chain_stride, [R, C] row-major) gets token_set[a*]
+ *   at [c * chain_stride + (p / W) * C + 1 + p % W], W = C - 1, in place; logq and logp as esmb200_sample_rows' over
+ *   the n_tokens columns z. An entry outside [0, R * W) writes no token and a NaN logq. With token_set = aa_offset
+ *   ... aa_offset + 19, R = 1 and C = T - 1 this is esmb200_sample_rows bit for bit. ld >= 1, finite temperature > 0,
+ *   R >= 1, C >= 2, chain_stride >= R * C, per_chain > 0 dividing n, chain0 + n / per_chain <= 2^32 and
+ *   0 <= step < 2^32, else ESMB200_EINVAL, before any launch. n == 0 launches nothing. Deterministic, no atomics. */
+int esmb200_msa_sample_order(const int64_t* entries, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
+                             uint64_t seed, int64_t* keys, void* stream);
+int esmb200_sample_rows_set(const float* logits, int64_t ld, int32_t n, const int32_t* token_set, int32_t n_tokens,
+                            float temperature, uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain,
+                            const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
+                            float* logq, float* logp, int64_t logp_stride, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -408,8 +436,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *   tags: 0 LN1->f16, 1 QKV+RoPE GEMM, 2 attention, 3 out-proj GEMM, 4 LN2->f16, 5 fc1+GELU GEMM, 6 fc2 GEMM,
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
- *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
- *         and each kernel of esmb200_sample_rows) */
+ *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order,
+ *         esmb200_msa_sample_order and each kernel of esmb200_sample_rows and esmb200_sample_rows_set) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
