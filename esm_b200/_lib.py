@@ -70,11 +70,9 @@ EXPORTS = (
     "esmb200_jacobian_contacts",
     "esmb200_sample_order",
     "esmb200_sample_rows",
-    "esmb200_msa_sample_order",
-    "esmb200_sample_rows_set",
 )
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32, EPI_GELU_FP8 = range(6)
 
 
@@ -177,15 +175,9 @@ def _declare(lib):
     lib.esmb200_sample_order.restype = c_int32
     lib.esmb200_sample_order.argtypes = [c_void_p, c_int32, c_int32, c_int64, c_int64, c_uint64, c_void_p, c_void_p]
     lib.esmb200_sample_rows.restype = c_int32
-    lib.esmb200_sample_rows.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_float, c_uint64, c_int64, c_int64,
-                                        c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_void_p]
-    lib.esmb200_msa_sample_order.restype = c_int32
-    lib.esmb200_msa_sample_order.argtypes = [c_void_p, c_int32, c_int32, c_int64, c_int64, c_uint64, c_void_p,
-                                             c_void_p]
-    lib.esmb200_sample_rows_set.restype = c_int32
-    lib.esmb200_sample_rows_set.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_float, c_uint64, c_int64,
-                                            c_int64, c_int32, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
-                                            c_void_p, c_int64, c_void_p]
+    lib.esmb200_sample_rows.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_float, c_uint64, c_int64,
+                                        c_int64, c_int32, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
+                                        c_void_p, c_int64, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -1655,29 +1655,11 @@ int esmb200_jacobian_contacts(const float* jac, int32_t L, void* scratch, size_t
 }
 
 
-int esmb200_sample_order(const int64_t* positions, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
+int esmb200_sample_order(const int64_t* entries, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
                          uint64_t seed, int64_t* keys, void* stream) {
   if (n <= 0 || n_chains < 0) return fail(ESMB200_EINVAL, "sample_order needs n > 0 and n_chains >= 0");
   if (chain0 < 0 || chain0 + n_chains > (int64_t(1) << 32) || sweep < 0 || sweep >= (int64_t(1) << 32))
     return fail(ESMB200_EINVAL, "sample_order needs chain0 + n_chains <= 2^32 and 0 <= sweep < 2^32");
-  if (n_chains == 0) return ESMB200_OK;
-  if (!positions || !keys) return fail(ESMB200_EINVAL, "null argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  ProfScope ps(T_SAMPLING, st);
-  const int64_t total = (int64_t)n * n_chains;
-  const int64_t blocks = (total + 255) / 256;
-  sample_order_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(positions, n, total,
-                                                                                  (uint32_t)chain0, (uint32_t)sweep,
-                                                                                  seed, 16, keys);
-  CK(cudaGetLastError());
-  return ESMB200_OK;
-}
-
-int esmb200_msa_sample_order(const int64_t* entries, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
-                             uint64_t seed, int64_t* keys, void* stream) {
-  if (n <= 0 || n_chains < 0) return fail(ESMB200_EINVAL, "msa_sample_order needs n > 0 and n_chains >= 0");
-  if (chain0 < 0 || chain0 + n_chains > (int64_t(1) << 32) || sweep < 0 || sweep >= (int64_t(1) << 32))
-    return fail(ESMB200_EINVAL, "msa_sample_order needs chain0 + n_chains <= 2^32 and 0 <= sweep < 2^32");
   if (n_chains == 0) return ESMB200_OK;
   if (!entries || !keys) return fail(ESMB200_EINVAL, "null argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1686,68 +1668,35 @@ int esmb200_msa_sample_order(const int64_t* entries, int32_t n, int32_t n_chains
   const int64_t blocks = (total + 255) / 256;
   sample_order_kernel<<<(unsigned)(blocks < 65536 ? blocks : 65536), 256, 0, st>>>(entries, n, total,
                                                                                   (uint32_t)chain0, (uint32_t)sweep,
-                                                                                  seed, 20, keys);
+                                                                                  seed, keys);
   CK(cudaGetLastError());
   return ESMB200_OK;
 }
 
-int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, int32_t aa_offset, float temperature,
-                        uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain, const int64_t* positions,
-                        int64_t* tokens, int32_t T, float* logq, float* logp, int64_t logp_stride, void* stream) {
+int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, const int32_t* token_set, int32_t n_tokens,
+                        float temperature, uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain,
+                        const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
+                        float* logq, float* logp, int64_t logp_stride, void* stream) {
   if (n < 0 || per_chain <= 0 || n % per_chain != 0)
     return fail(ESMB200_EINVAL, "sample_rows needs n >= 0 and per_chain > 0 dividing n");
-  if (aa_offset < 0 || ld < (int64_t)aa_offset + kSampleAA)
-    return fail(ESMB200_EINVAL, "sample_rows needs aa_offset >= 0 and ld >= aa_offset + 20");
+  if (n_tokens < 1 || n_tokens > 32 || ld < 1)
+    return fail(ESMB200_EINVAL, "sample_rows needs 1 <= n_tokens <= 32 and ld >= 1");
   if (!(temperature > 0.f) || !(temperature < INFINITY))
     return fail(ESMB200_EINVAL, "sample_rows needs a finite temperature > 0");
-  if (T < 3) return fail(ESMB200_EINVAL, "sample_rows needs T >= 3");
+  if (R < 1 || C < 2 || chain_stride < (int64_t)R * C)
+    return fail(ESMB200_EINVAL, "sample_rows needs R >= 1, C >= 2 and chain_stride >= R * C");
   const int64_t n_chains = n / per_chain;
   if (chain0 < 0 || chain0 + n_chains > (int64_t(1) << 32) || step < 0 || step >= (int64_t(1) << 32))
     return fail(ESMB200_EINVAL, "sample_rows needs chain0 + n / per_chain <= 2^32 and 0 <= step < 2^32");
   if (logp && logp_stride < 1) return fail(ESMB200_EINVAL, "sample_rows needs logp_stride >= 1");
   if (n == 0) return ESMB200_OK;
-  if (!logits || !positions || !tokens || !logq) return fail(ESMB200_EINVAL, "null argument");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
-    ProfScope ps(T_SAMPLING, st);
-    sample_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(logits, ld, n, aa_offset, temperature, seed,
-                                                                (uint32_t)step, (uint32_t)chain0, per_chain, positions,
-                                                                tokens, T, logq);
-    CK(cudaGetLastError());
-  }
-  if (logp) {
-    ProfScope ps(T_SAMPLING, st);
-    sample_logp_kernel<<<(unsigned)((n_chains + 255) / 256), 256, 0, st>>>(logq, n_chains, per_chain, logp,
-                                                                           logp_stride);
-    CK(cudaGetLastError());
-  }
-  return ESMB200_OK;
-}
-
-int esmb200_sample_rows_set(const float* logits, int64_t ld, int32_t n, const int32_t* token_set, int32_t n_tokens,
-                            float temperature, uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain,
-                            const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
-                            float* logq, float* logp, int64_t logp_stride, void* stream) {
-  if (n < 0 || per_chain <= 0 || n % per_chain != 0)
-    return fail(ESMB200_EINVAL, "sample_rows_set needs n >= 0 and per_chain > 0 dividing n");
-  if (n_tokens < 1 || n_tokens > 32 || ld < 1)
-    return fail(ESMB200_EINVAL, "sample_rows_set needs 1 <= n_tokens <= 32 and ld >= 1");
-  if (!(temperature > 0.f) || !(temperature < INFINITY))
-    return fail(ESMB200_EINVAL, "sample_rows_set needs a finite temperature > 0");
-  if (R < 1 || C < 2 || chain_stride < (int64_t)R * C)
-    return fail(ESMB200_EINVAL, "sample_rows_set needs R >= 1, C >= 2 and chain_stride >= R * C");
-  const int64_t n_chains = n / per_chain;
-  if (chain0 < 0 || chain0 + n_chains > (int64_t(1) << 32) || step < 0 || step >= (int64_t(1) << 32))
-    return fail(ESMB200_EINVAL, "sample_rows_set needs chain0 + n / per_chain <= 2^32 and 0 <= step < 2^32");
-  if (logp && logp_stride < 1) return fail(ESMB200_EINVAL, "sample_rows_set needs logp_stride >= 1");
-  if (n == 0) return ESMB200_OK;
   if (!logits || !token_set || !entries || !tokens || !logq) return fail(ESMB200_EINVAL, "null argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   {  // one ProfScope per kernel: esmb200_launch_count counts kernels
     ProfScope ps(T_SAMPLING, st);
-    sample_rows_set_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(logits, ld, n, token_set, n_tokens, temperature,
-                                                                    seed, (uint32_t)step, (uint32_t)chain0, per_chain,
-                                                                    entries, tokens, chain_stride, R, C, logq);
+    sample_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(logits, ld, n, token_set, n_tokens, temperature, seed,
+                                                                (uint32_t)step, (uint32_t)chain0, per_chain, entries,
+                                                                tokens, chain_stride, R, C, logq);
     CK(cudaGetLastError());
   }
   if (logp) {

@@ -1,73 +1,58 @@
-"""Sequence generation from a masked protein language model (ESM-2, ESM-1b, ESM-1v) by Gibbs sampling: batched chains,
-block updates of the designable positions in a random order per sweep, and a counter-based random stream, so that a
-sample depends only on (seed, chain, step, position).
+"""Gibbs sampling from a masked protein language model: sequences from ESM-2, ESM-1b and ESM-1v, alignments from the
+MSA Transformer. Batched chains, block updates of the designable entries in a random order per sweep, and a
+counter-based random stream, so that a sample depends only on (seed, chain, step, entry).
 
     from esm_b200 import sampling
     out = sampling.gibbs(model, tokens, positions=None, chains=1, sweeps=1, block=1, temperature=1.0, seed=0,
                          max_tokens=None)
-    out["tokens"]   # int64 [C, T] on the model's device
-    out["logp"]     # fp32 [C, steps]
-
-Definition. tokens [1, T] is one protein with <cls> first, <eos> last and no padding; residues sit at token positions
-1 ... L. positions D (residue indices in [0, L), distinct; default all) are designable, every other residue is fixed
-and never changes, whatever token it holds. A <mask> is allowed at a designable position only, so `<cls> <mask>*L
-<eos>` starts de novo generation. Only the 20 amino acids AA = jacobian.AMINO_ACIDS are sampled. Every chain starts
-from tokens. k = min(block, |D|).
-
-R(c0, c1, c2, c3) is Philox4x32-10 with counter (c0, c1, c2, c3) and key (seed mod 2^32, seed >> 32); a word r gives
-the uniform u = ((r >> 8) + 0.5) * 2^-24, rounded toward zero to fp32 (exact for u < 1/2, always in (0, 1)).
-
-For each sweep w (0-based) and chain c (global index 0 ... C-1):
-  1. Order: D sorted ascending by R(w, c, p, 0).x * 65536 + p, cut into consecutive blocks of k (the last one may be
-     shorter, equally for every chain). Steps are the blocks, counted over all sweeps as s; there are
-     W * ceil(|D| / k) of them.
-  2. Step s: the chain's current tokens with <mask> at the block's positions run through the stack; the fp32 LM-head
-     logits l at rows 1 + p of the block give, for each p and a < 20, z_a = fp32(l[AA_a] / temperature) and
-     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(s, c, p, 1 + a div 4). The new token is AA[a*],
-     a* = argmax_a (z_a + g_a), a tie to the smallest a. All positions of the block are written together (a block
-     update). log q = log_softmax(z)[a*], by esmb200_log_softmax_rows' formula: (z - max) - logf(sum expf(z - max)).
-  3. In sweep 0 of a de novo start, positions not yet visited are still <mask> when their neighbours are drawn
-     (iterative decoding in random order); after sweep 0 no designable position holds <mask>.
-logp[c, s] is the sum of step s's log q in block order (fp32).
-
-The chains run in chunks of at most `max_tokens` tokens (variants._copies_per_chunk, at least one chain); each chunk
-runs all its sweeps. A step is one stack call on the chunk's masked copies, the LM head on the block rows only, then
-esmb200_sample_rows, which draws the tokens and writes them into the chains' device state in place. The order of a
-sweep is esmb200_sample_order's keys sorted on the device. Nothing in the sweep loop waits for the host. The stack is
-batch-invariant and every draw depends only on (seed, chain, step, position), so the result is the same bits for
-every max_tokens.
-
-Cost: each step is one stack call on C copies of T tokens (in chunks); the sampler kernel and the head on C k rows
-are small beside it.
-
-Alignments from the MSA Transformer:
-
+    out["tokens"]   # int64 [chains, T] on the model's device
+    out["logp"]     # fp32 [chains, steps]
     out = sampling.msa_gibbs(model, tokens, designable=None, chains=1, sweeps=1, block=1, temperature=1.0, seed=0,
                              gaps=True, max_tokens=None)
     out["tokens"]   # int64 [chains, R, C] on the model's device
     out["logp"]     # fp32 [chains, steps]
 
-Definition. tokens [1, R, C] is one alignment in the MSA alphabet: column 0 of every row is <cls>, there is no <pad>
-and no <eos>, R <= 1024 (the MSA position embedding) and 2 <= C <= max_positions. The residue entries are (r, j),
-1 <= j < C, with the flat index p = r * (C - 1) + (j - 1) < 2^20. designable is None (every entry) or bool [R, C - 1];
-every other entry is fixed and never changes. A <mask> is allowed at a designable entry only, so <mask> rows appended
-to a real alignment generate new family members. The drawable tokens A are the 20 amino acids of
-jacobian.AMINO_ACIDS in that order and, with gaps=True, the gap "-" as A[20]. n is the number of designable entries
-and k = min(block, n). Every chain starts from tokens.
+Definition. A chain is an alignment of R rows and C columns whose column 0 is <cls>. Its residue entries (r, j),
+1 <= j < C, have the flat index p = r * (C - 1) + (j - 1) < 2^20. The designable entries D are resampled, every other
+entry is fixed and never changes, whatever token it holds; a <mask> is allowed at a designable entry only. The drawable
+tokens A are a list of token ids. Every chain starts from tokens. k = min(block, |D|).
 
-For each sweep w and chain c, the designable p are sorted ascending by R(w, c, p, 0).x * 2^20 + p and cut into blocks
-of k; steps s count the blocks over all sweeps. In step s the chain's tokens with <mask> at the block's entries run
-through the axial stack, and the fp32 LM-head logits l at those entries only give, for each p and a < |A|,
-z_a = fp32(l[A_a] / temperature) and g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(s, c, p, 1 + a div 4) by the
-uniform map above. The new token is A[argmax_a (z_a + g_a)], a tie to the smaller a; the block's entries are written
-together. log q is esmb200_log_softmax_rows' value over the |A| tempered columns, and logp[c, s] the block's log q
-summed in block order (fp32). Since x dominates both order keys, an alignment of one row with gaps=False and the same
-logits draws what gibbs' kernel (esmb200_sample_rows) draws, with the same log q.
+R(c0, c1, c2, c3) is Philox4x32-10 with counter (c0, c1, c2, c3) and key (seed mod 2^32, seed >> 32); a word r gives
+the uniform u = ((r >> 8) + 0.5) * 2^-24, rounded toward zero to fp32 (exact for u < 1/2, always in (0, 1)).
 
-Execution as for gibbs, with chains of R * C tokens in chunks of at most max_tokens (at least one chain), the order
-from esmb200_msa_sample_order and the draw from esmb200_sample_rows_set. The stack runs without a padding mask
-(MSATransformer._stack_unpadded), so nothing in the sweep loop waits for the host, and the result is the same bits for
-every max_tokens.
+For each sweep w (0-based) and chain c (global index 0 ... chains-1):
+  1. Order: D sorted ascending by R(w, c, p, 0).x * 2^20 + p, cut into consecutive blocks of k (the last one may be
+     shorter, equally for every chain). Steps are the blocks, counted over all sweeps as s; there are
+     sweeps * ceil(|D| / k) of them.
+  2. Step s: the chain's current tokens with <mask> at the block's entries run through the stack; the fp32 LM-head
+     logits l at those entries give, for each p and a < |A|, z_a = fp32(l[A_a] / temperature) and
+     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(s, c, p, 1 + a div 4). The new token is A[a*],
+     a* = argmax_a (z_a + g_a), a tie to the smallest a. All entries of the block are written together (a block
+     update). log q = log_softmax(z)[a*], by esmb200_log_softmax_rows' formula: (z - max) - logf(sum expf(z - max)).
+  3. In sweep 0 of a de novo start, entries not yet visited are still <mask> when their neighbours are drawn
+     (iterative decoding in random order); after sweep 0 no designable entry holds <mask>.
+logp[c, s] is the sum of step s's log q in block order (fp32).
+
+Sequences (gibbs). tokens [1, T] is one protein with <cls> first, <eos> last and no padding, 2 ... 65535 residues at
+token positions 1 ... L: the layout R = 1, C = T - 1, so entry p is residue p, token 1 + p, and <eos> is no entry.
+positions D (residue indices in [0, L), distinct; default all) are designable, so `<cls> <mask>*L <eos>` starts de
+novo generation. A is the 20 amino acids of jacobian.AMINO_ACIDS in that order.
+
+Alignments (msa_gibbs). tokens [1, R, C] is one alignment in the MSA alphabet: column 0 of every row is <cls>, there is
+no <pad> and no <eos>, R <= 1024 (the MSA position embedding) and 2 <= C <= max_positions. designable is None (every
+entry) or bool [R, C - 1], so <mask> rows appended to a real alignment generate new family members. A is the 20 amino
+acids of jacobian.AMINO_ACIDS in that order and, with gaps=True, the gap "-" as A[20].
+
+Execution. The chains run in chunks of at most `max_tokens` tokens (variants._copies_per_chunk, at least one chain);
+each chunk runs all its sweeps. The order of a sweep is esmb200_sample_order's keys sorted on the device. A step is one
+stack call on the chunk's masked copies, the LM head on the block's entries only, then esmb200_sample_rows, which
+draws the tokens and writes them into the chains' device state in place. Nothing in the sweep loop waits for the host:
+the MSA Transformer's stack runs without a padding mask (MSATransformer._stack_unpadded). The stacks are
+batch-invariant and every draw depends only on (seed, chain, step, entry), so the result is the same bits for every
+max_tokens.
+
+Cost: each step is one stack call on the chains' copies (in chunks); the sampler kernels and the head on the block's
+entries are small beside it.
 """
 from __future__ import annotations
 
@@ -84,7 +69,7 @@ from .model import ProteinLanguageModel, _ptr, _stream
 from .variants import _copies_per_chunk, _device
 
 _COUNTER = 1 << 32  # chains and steps are Philox counter words
-_MAX_RESIDUES = 65535  # the order key holds the position in 16 bits
+_MAX_RESIDUES = 65535  # gibbs' documented limit (its docstring, DESIGN.md section 1)
 _MAX_MSA_ROWS = 1024  # the MSA position embedding
 _MAX_ENTRIES = 1 << 20  # the order key holds the entry index in 20 bits
 
@@ -165,41 +150,9 @@ def gibbs(model, tokens: torch.Tensor, positions: Optional[Sequence[int]] = None
                                                          seed)
     aa0 = _amino_acid_offset(model)
     T = host.shape[1]
-    n = pos.numel()
-    k = min(block, n)
-    blocks = -(-n // k)
-    steps = sweeps * blocks
-    lib = _lib.load()
-    dev = _device(model)
-    if dev.type != "cuda":
-        raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model to the GPU; no CPU fallback")
-    tok, pos = host.to(dev), pos.to(dev)
-    out = torch.empty((chains, T), dtype=torch.int64, device=dev)
-    logp = torch.empty((chains, steps), dtype=torch.float32, device=dev)
-    per = _copies_per_chunk(T, max_tokens)
-    with torch.cuda.device(dev):
-        for c0 in range(0, chains, per):
-            m = min(per, chains - c0)
-            state = out[c0:c0 + m]  # the chains' tokens, updated in place by esmb200_sample_rows
-            state.copy_(tok.expand(m, T))
-            row1 = torch.arange(m, device=dev).unsqueeze(1) * T + 1  # flat row of each copy's first residue
-            for w in range(sweeps):
-                keys = torch.empty((m, n), dtype=torch.int64, device=dev)
-                _lib.check(lib.esmb200_sample_order(_ptr(pos), n, m, c0, w, seed, _ptr(keys), _stream()))
-                order = keys.sort(dim=1).values.bitwise_and_(0xFFFF)  # key mod 65536 = the position
-                for b in range(blocks):
-                    s = w * blocks + b
-                    blk = order[:, b * k:(b + 1) * k].contiguous()
-                    kb = blk.shape[1]
-                    batch = state.clone()
-                    batch.scatter_(1, blk + 1, model.mask_idx)
-                    x = model._stack(batch)[1]
-                    logits = model._lm_head_rows(x.view(-1, x.shape[-1]).index_select(0, (row1 + blk).view(-1)))
-                    logq = torch.empty(m * kb, dtype=torch.float32, device=dev)
-                    _lib.check(lib.esmb200_sample_rows(_ptr(logits), logits.stride(0), m * kb, aa0, tau, seed, s, c0,
-                                                       kb, _ptr(blk), _ptr(state), T, _ptr(logq),
-                                                       _ptr(logp[c0:, s]), steps, _stream()))
-    return {"tokens": out, "logp": logp}
+    amino_acids = list(range(aa0, aa0 + len(AMINO_ACIDS)))
+    return _sweep(model, host, pos, amino_acids, (1, T - 1, T), lambda b: model._stack(b)[1], tau, chains, sweeps,
+                  block, seed, max_tokens)
 
 
 def _check_msa(model, tokens, designable, chains, sweeps, block, temperature, seed):
@@ -269,9 +222,17 @@ def msa_gibbs(model, tokens: torch.Tensor, designable: Optional[torch.Tensor] = 
     outside [0, 2^64)."""
     host, entries, tau, chains, sweeps, block, seed = _check_msa(model, tokens, designable, chains, sweeps, block,
                                                                  temperature, seed)
-    drawable = _drawable(model, bool(gaps))
     _, R, C = host.shape
-    W = C - 1
+    return _sweep(model, host, entries, _drawable(model, bool(gaps)), (R, C, R * C), model._stack_unpadded, tau,
+                  chains, sweeps, block, seed, max_tokens)
+
+
+def _sweep(model, host, entries, drawable, layout, stack, tau, chains, sweeps, block, seed, max_tokens):
+    """The sweep loop of gibbs and msa_gibbs after their checks, by the definition in the module docstring. host: the
+    start tokens [1, ...] of one chain; entries: the designable entries p int64 [n] on the host; drawable: the token ids
+    of A; layout: (R, C, chain_stride), chain_stride the number of tokens of a chain; stack: the masked batch
+    [m, ...] -> its pre-LN residual stream."""
+    R, C, chain_stride = layout
     n = entries.numel()
     k = min(block, n)
     blocks = -(-n // k)
@@ -282,31 +243,32 @@ def msa_gibbs(model, tokens: torch.Tensor, designable: Optional[torch.Tensor] = 
         raise _lib.Esmb200Error("esm_b200 runs on CUDA (sm_90a) only: move the model to the GPU; no CPU fallback")
     tok, entries = host.to(dev), entries.to(dev)
     token_set = torch.tensor(drawable, dtype=torch.int32, device=dev)
-    out = torch.empty((chains, R, C), dtype=torch.int64, device=dev)
+    out = torch.empty((chains,) + tuple(host.shape[1:]), dtype=torch.int64, device=dev)
     logp = torch.empty((chains, steps), dtype=torch.float32, device=dev)
-    per = _copies_per_chunk(R * C, max_tokens)
+    per = _copies_per_chunk(chain_stride, max_tokens)
     with torch.cuda.device(dev):
         for c0 in range(0, chains, per):
             m = min(per, chains - c0)
-            state = out[c0:c0 + m]  # the chains' alignments, updated in place by esmb200_sample_rows_set
-            state.copy_(tok.expand(m, R, C))
-            base = torch.arange(m, device=dev).unsqueeze(1) * (R * C)  # flat token of each copy's (0, 0)
+            state = out[c0:c0 + m]  # the chains' tokens, updated in place by esmb200_sample_rows
+            state.copy_(tok.expand_as(state))
+            base = torch.arange(m, device=dev).unsqueeze(1) * chain_stride  # flat token of each copy's (0, 0)
             for w in range(sweeps):
                 keys = torch.empty((m, n), dtype=torch.int64, device=dev)
-                _lib.check(lib.esmb200_msa_sample_order(_ptr(entries), n, m, c0, w, seed, _ptr(keys), _stream()))
+                _lib.check(lib.esmb200_sample_order(_ptr(entries), n, m, c0, w, seed, _ptr(keys), _stream()))
                 order = keys.sort(dim=1).values.bitwise_and_((1 << 20) - 1)  # key mod 2^20 = the entry
                 for b in range(blocks):
                     s = w * blocks + b
                     blk = order[:, b * k:(b + 1) * k].contiguous()
                     kb = blk.shape[1]
-                    flat = (base + blk + blk.div(W, rounding_mode="floor") + 1).view(-1)  # (p / W) C + 1 + p % W
+                    # token (p / W) C + 1 + p % W of each copy, W = C - 1
+                    flat = (base + blk + blk.div(C - 1, rounding_mode="floor") + 1).view(-1)
                     batch = state.clone()
                     batch.view(-1).index_fill_(0, flat, model.mask_idx)
-                    x = model._stack_unpadded(batch)
+                    x = stack(batch)
                     logits = model._lm_head_rows(x.view(-1, x.shape[-1]).index_select(0, flat))
                     logq = torch.empty(m * kb, dtype=torch.float32, device=dev)
-                    _lib.check(lib.esmb200_sample_rows_set(_ptr(logits), logits.stride(0), m * kb, _ptr(token_set),
-                                                           len(drawable), tau, seed, s, c0, kb, _ptr(blk),
-                                                           _ptr(state), R * C, R, C, _ptr(logq), _ptr(logp[c0:, s]),
-                                                           steps, _stream()))
+                    _lib.check(lib.esmb200_sample_rows(_ptr(logits), logits.stride(0), m * kb, _ptr(token_set),
+                                                       len(drawable), tau, seed, s, c0, kb, _ptr(blk), _ptr(state),
+                                                       chain_stride, R, C, _ptr(logq), _ptr(logp[c0:, s]), steps,
+                                                       _stream()))
     return {"tokens": out, "logp": logp}

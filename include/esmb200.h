@@ -41,7 +41,7 @@ extern "C" {
 #define ESMB200_ENOMEM -3   /* device allocation failed ("CUDA out of memory ...") */
 #define ESMB200_EWORKSPACE -4 /* workspace too small */
 
-#define ESMB200_ABI_VERSION 3
+#define ESMB200_ABI_VERSION 4
 
 typedef struct esmb200_layer esmb200_layer; /* opaque: packed weights + TMA descriptors of one TransformerLayer */
 
@@ -260,43 +260,20 @@ size_t esmb200_jacobian_scratch_bytes(int32_t L);
 int esmb200_jacobian_contacts(const float* jac, int32_t L, void* scratch, size_t scratch_bytes, float* contacts,
                               void* stream);
 
-/* Gibbs sampling of protein sequences (esm_b200/sampling.py). A new operation with no reference code. Random stream:
- * R(c0, c1, c2, c3) = Philox4x32-10 (curand_Philox4x32_10) with counter (c0, c1, c2, c3) and key (seed mod 2^32,
- * seed >> 32): four uint32 words. A word r maps to u = ((r >> 8) + 0.5) * 2^-24 rounded toward zero to fp32, which
- * lies in (0, 1) and is exact for u < 1/2. Every draw depends only on (seed, chain, step, position), never on how the
- * chains are batched.
+/* Gibbs sampling of protein sequences and MSA Transformer alignments (esm_b200/sampling.py). A new operation with no
+ * reference code. Random stream: R(c0, c1, c2, c3) = Philox4x32-10 (curand_Philox4x32_10) with counter
+ * (c0, c1, c2, c3) and key (seed mod 2^32, seed >> 32): four uint32 words. A word r maps to
+ * u = ((r >> 8) + 0.5) * 2^-24 rounded toward zero to fp32, which lies in (0, 1) and is exact for u < 1/2. Every draw
+ * depends only on (seed, chain, step, entry), never on how the chains are batched.
+ * Layout: a chain is an alignment of R rows and C columns, column 0 <cls>, row-major; its residue entries (r, j),
+ * 1 <= j < C, have the flat index p = r * W + (j - 1), W = C - 1, and p < 2^20. A protein of T tokens is R = 1,
+ * C = T - 1: residue p is token 1 + p, and the <eos> column is never an entry.
  * esmb200_sample_order: the visiting order of one sweep. keys int64 [n_chains, n]:
- *     keys[c, j] = R(sweep, chain0 + c, p, 0).x * 65536 + p,   p = positions[j],
- *   for the n designable residue indices positions int64 [n] (device; distinct, each in [0, 65535), checked by the
- *   caller). Sorting each row ascending (keys are distinct) and taking key mod 65536 gives the order; the caller sorts.
- *   n > 0, chain0 + n_chains <= 2^32, 0 <= sweep < 2^32, else ESMB200_EINVAL. n_chains == 0 launches nothing.
- * esmb200_sample_rows: one block update of step `step` for n / per_chain chains, one warp per row, any n. Row r
- *   belongs to chain chain0 + r / per_chain (local chain r / per_chain) and resamples residue p = positions[r]
- *   (int64 [n], device; p in [0, T - 2), checked by the caller: a row outside writes no token and a NaN logq).
- *   logits fp32 [n, ld]: the LM-head row of token 1 + p of that chain's masked copy. For a < 20:
- *     z_a = logits[r, aa_offset + a] / temperature (fp32 division),
- *     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(step, chain, p, 1 + a div 4),
- *     a* = argmax_a (z_a + g_a), a tie to the smallest a;
- *   tokens int64 [n / per_chain, T] (the chains' state) gets aa_offset + a* at [r / per_chain, 1 + p], in place;
- *   logq fp32 [n] gets (z_a* - max z) - logf(sum_a expf(z_a - max z)), bit for bit esmb200_log_softmax_rows' value
- *   with target a* on the 20 columns z. logp: NULL, or fp32 with logp[c * logp_stride] = the per_chain logq of local
- *   chain c summed in row order (fp32, from +0). ld >= aa_offset + 20, finite temperature > 0, T >= 3, per_chain > 0
- *   dividing n, chain0 + n / per_chain <= 2^32 and 0 <= step < 2^32, else ESMB200_EINVAL, before any launch. n == 0
- *   launches nothing. Deterministic, no atomics. */
-int esmb200_sample_order(const int64_t* positions, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
-                         uint64_t seed, int64_t* keys, void* stream);
-int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, int32_t aa_offset, float temperature,
-                        uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain, const int64_t* positions,
-                        int64_t* tokens, int32_t T, float* logq, float* logp, int64_t logp_stride, void* stream);
-
-/* Gibbs sampling of MSA Transformer alignments (esm_b200/sampling.py, msa_gibbs), on the random stream above. An
- * alignment has R rows and C columns, column 0 <cls>; its residue entries (r, j), 1 <= j < C, have the flat index
- * p = r * (C - 1) + (j - 1) < 2^20 (R <= 1024, C <= 1025).
- * esmb200_msa_sample_order: the visiting order of one sweep. keys int64 [n_chains, n]:
  *     keys[c, j] = R(sweep, chain0 + c, p, 0).x * 2^20 + p,   p = entries[j],
  *   for the n designable entries entries int64 [n] (device; distinct, each in [0, 2^20), checked by the caller).
- *   Sorting each row ascending and taking key mod 2^20 gives the order. Argument checks as esmb200_sample_order's.
- * esmb200_sample_rows_set: one block update of step `step` for n / per_chain chains over the drawable token ids
+ *   Sorting each row ascending (keys are distinct) and taking key mod 2^20 gives the order; the caller sorts.
+ *   n > 0, chain0 + n_chains <= 2^32, 0 <= sweep < 2^32, else ESMB200_EINVAL. n_chains == 0 launches nothing.
+ * esmb200_sample_rows: one block update of step `step` for n / per_chain chains over the drawable token ids
  *   token_set int32 [n_tokens] (device, 1 <= n_tokens <= 32, each in [0, ld), checked by the caller), one warp per row,
  *   any n. Row r belongs to chain chain0 + r / per_chain (local chain r / per_chain) and resamples entry
  *   p = entries[r] (int64 [n], device). logits fp32 [n, ld]: the LM-head row of that entry of the chain's masked
@@ -304,18 +281,19 @@ int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, int32_t aa_o
  *     z_a = logits[r, token_set[a]] / temperature (fp32 division),
  *     g_a = -logf(-logf(u_a)), u_a from word a mod 4 of R(step, chain, p, 1 + a div 4),
  *     a* = argmax_a (z_a + g_a), a tie to the smallest a;
- *   tokens int64 (the chains' alignments, chain c at tokens + c * chain_stride, [R, C] row-major) gets token_set[a*]
- *   at [c * chain_stride + (p / W) * C + 1 + p % W], W = C - 1, in place; logq and logp as esmb200_sample_rows' over
- *   the n_tokens columns z. An entry outside [0, R * W) writes no token and a NaN logq. With token_set = aa_offset
- *   ... aa_offset + 19, R = 1 and C = T - 1 this is esmb200_sample_rows bit for bit. ld >= 1, finite temperature > 0,
- *   R >= 1, C >= 2, chain_stride >= R * C, per_chain > 0 dividing n, chain0 + n / per_chain <= 2^32 and
- *   0 <= step < 2^32, else ESMB200_EINVAL, before any launch. n == 0 launches nothing. Deterministic, no atomics. */
-int esmb200_msa_sample_order(const int64_t* entries, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
-                             uint64_t seed, int64_t* keys, void* stream);
-int esmb200_sample_rows_set(const float* logits, int64_t ld, int32_t n, const int32_t* token_set, int32_t n_tokens,
-                            float temperature, uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain,
-                            const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
-                            float* logq, float* logp, int64_t logp_stride, void* stream);
+ *   tokens int64 (the chains' state, chain c at tokens + c * chain_stride) gets token_set[a*] at
+ *   [c * chain_stride + (p / W) * C + 1 + p % W], in place; logq fp32 [n] gets (z_a* - max z) - logf(sum_a expf(z_a -
+ *   max z)), bit for bit esmb200_log_softmax_rows' value with target a* on the n_tokens columns z. An entry outside
+ *   [0, R * W) writes no token and a NaN logq. logp: NULL, or fp32 with logp[c * logp_stride] = the per_chain logq of
+ *   local chain c summed in row order (fp32, from +0). ld >= 1, finite temperature > 0, R >= 1, C >= 2,
+ *   chain_stride >= R * C, per_chain > 0 dividing n, chain0 + n / per_chain <= 2^32 and 0 <= step < 2^32, else
+ *   ESMB200_EINVAL, before any launch. n == 0 launches nothing. Deterministic, no atomics. */
+int esmb200_sample_order(const int64_t* entries, int32_t n, int32_t n_chains, int64_t chain0, int64_t sweep,
+                         uint64_t seed, int64_t* keys, void* stream);
+int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, const int32_t* token_set, int32_t n_tokens,
+                        float temperature, uint64_t seed, int64_t step, int64_t chain0, int32_t per_chain,
+                        const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
+                        float* logq, float* logp, int64_t logp_stride, void* stream);
 
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
@@ -436,8 +414,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *   tags: 0 LN1->f16, 1 QKV+RoPE GEMM, 2 attention, 3 out-proj GEMM, 4 LN2->f16, 5 fc1+GELU GEMM, 6 fc2 GEMM,
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
- *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order,
- *         esmb200_msa_sample_order and each kernel of esmb200_sample_rows and esmb200_sample_rows_set) */
+ *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
+ *         and each kernel of esmb200_sample_rows) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);

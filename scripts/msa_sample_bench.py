@@ -8,7 +8,7 @@ Prints one JSON line: the card and its power limit (a read-only nvidia-smi query
   * the same number of esmb200_axial_stack_forward calls on a batch of the same shape ([8, R, C, 768]), timed in the
     same run, alternating with msa_gibbs, and the step-to-stack ratio (best of --repeats for each);
   * the sampler kernels' time per step from the library's profiler (tag 20: the order kernel and both kernels of
-    esmb200_sample_rows_set), in a separate profiled run, and their share of a step.
+    esmb200_sample_rows), in a separate profiled run, and their share of a step.
 
     python scripts/msa_sample_bench.py [--sweeps 1] [--repeats 3] [--precision fp16] [--out results.jsonl]
 """

@@ -5,8 +5,8 @@ One JSON line per repeat with:
   * seconds per step and stack tokens/s: gibbs over --sweeps sweeps, CUDA events around synchronised work;
   * the plain stack model._stack on the same [256, 258] batch, timed over the same number of calls in the same run,
     alternating with gibbs, and the step-to-stack time ratio;
-  * the sampler kernels' time per step from the library's profiler (tag 20: the order kernel and the two sampler
-    kernels), in a separate profiled sweep, and their share of a step.
+  * the sampler kernels' time per step from the library's profiler (tag 20: the order kernel and both kernels of
+    esmb200_sample_rows), in a separate profiled sweep, and their share of a step.
 The first line names the card and its power limit (a read-only nvidia-smi query).
 
     python scripts/sample_bench.py [--sweeps 1] [--repeats 3] [--precision fp16] [--out results.jsonl]

@@ -1,6 +1,7 @@
-"""Numpy restatement of the sampler's definition (esm_b200/sampling.py): Philox4x32-10, the uniform map, the visiting
-order and block partition of a sweep, and the Gumbel-max draw in float64. The CPU tests pin it against the toolkit's
-Philox known answers and the definition's properties; the GPU tests gate the kernels and gibbs against it."""
+"""Numpy restatement of the sampler's definition (esm_b200/sampling.py): Philox4x32-10, the uniform map, the entry
+index of a layout, the visiting order and block partition of a sweep, the uniforms of a token set of up to 32 ids, and
+the Gumbel-max draw in float64. The CPU tests pin it against the toolkit's Philox known answers and the definition's
+properties; the GPU tests gate the kernels, gibbs and msa_gibbs against it."""
 from __future__ import annotations
 
 import numpy as np
@@ -34,31 +35,44 @@ def uniform(r):
     return np.where(j < (1 << 23), exact, j.astype(np.float64) * 2.0 ** -24).astype(np.float32)
 
 
-def order_keys(positions, chains, sweep, seed):
-    """keys [len(chains), n] int64 = R(sweep, c, p, 0).x * 65536 + p."""
-    p = np.asarray(positions, dtype=np.int64)[None, :]
+def entry_token(p, C):
+    """(row, column) of entry p in an alignment of C columns whose column 0 is <cls>."""
+    p = np.asarray(p, dtype=np.int64)
+    return p // (C - 1), 1 + p % (C - 1)
+
+
+def order_keys(entries, chains, sweep, seed):
+    """keys [len(chains), n] int64 = R(sweep, c, p, 0).x * 2^20 + p."""
+    p = np.asarray(entries, dtype=np.int64)[None, :]
     c = np.asarray(chains, dtype=np.int64)[:, None]
     x = philox4x32_10(sweep, c, p, 0, seed)[0]
-    return x.astype(np.int64) * 65536 + p
+    return x.astype(np.int64) * (1 << 20) + p
 
 
-def sweep_blocks(positions, chain, sweep, seed, block):
-    """The blocks of one sweep of one chain: the designable positions sorted by their keys, cut into runs of
+def sweep_blocks(entries, chain, sweep, seed, block):
+    """The blocks of one sweep of one chain: the designable entries sorted by their keys, cut into runs of
     min(block, n)."""
-    keys = order_keys(positions, [chain], sweep, seed)[0]
-    order = np.sort(keys) % 65536
+    keys = order_keys(entries, [chain], sweep, seed)[0]
+    order = np.sort(keys) % (1 << 20)
     k = min(block, len(order))
     return [order[i:i + k] for i in range(0, len(order), k)]
 
 
-def gumbel_uniforms(step, chain, p, seed):
-    """u [20] fp32 of one row: u_a = word a mod 4 of R(step, chain, p, 1 + a div 4)."""
-    words = philox4x32_10(step, chain, p, np.arange(1, 6), seed)  # 4 arrays of 5
-    return uniform(np.stack(words, 1).reshape(-1))
+def uniforms(step, chains, entries, seed, n_set):
+    """u [n, n_set] fp32 of n rows (chain, entry): u_a = word a mod 4 of R(step, chain, p, 1 + a div 4)."""
+    chains = np.asarray(chains, dtype=np.int64)[:, None]
+    entries = np.asarray(entries, dtype=np.int64)[:, None]
+    words = philox4x32_10(step, chains, entries, np.arange(1, 9)[None, :], seed)  # 4 arrays of [n, 8]
+    return uniform(np.stack(words, -1).reshape(len(entries), 32)[:, :n_set])
+
+
+def draw_f64(z, step, chains, entries, seed):
+    """Float64 Gumbel-max scores and a* of fp32 tempered logits z [n, n_set] for rows (chain, entry)."""
+    return gumbel_max_f64(z, uniforms(step, chains, entries, seed, np.shape(z)[-1]))
 
 
 def gumbel_max_f64(z, u):
-    """Float64 Gumbel-max scores z + g, g = -log(-log(u)), and a* (the first maximum). z [..., 20], u [..., 20]."""
+    """Float64 Gumbel-max scores z + g, g = -log(-log(u)), and a* (the first maximum). z [..., n_set], u likewise."""
     score = np.asarray(z, dtype=np.float64) - np.log(-np.log(np.asarray(u, dtype=np.float64)))
     return score, np.argmax(score, axis=-1)
 

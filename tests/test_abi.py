@@ -16,7 +16,7 @@ def header_symbols():
     return sorted(set(re.findall(r"\b(esmb200_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_builds_and_exports_every_declared_symbol():
+def test_library_builds_and_exports_every_declared_symbol_at_abi_version_4():
     from esm_b200 import _lib, build
     path = build.build()
     assert os.path.exists(path)
@@ -26,7 +26,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/esmb200.h but not exported"
     assert sorted(_lib.EXPORTS) == declared
-    assert _lib.load().esmb200_abi_version() == 3
+    assert _lib.load().esmb200_abi_version() == 4
 
 
 def test_workspace_size_is_pure_host_arithmetic():

@@ -1,16 +1,15 @@
-"""GPU: alignment sampling from the MSA Transformer (esm_b200.sampling.msa_gibbs, esmb200_msa_sample_order,
-esmb200_sample_rows_set).
+"""GPU: alignment sampling from the MSA Transformer (esm_b200.sampling.msa_gibbs, esmb200_sample_order,
+esmb200_sample_rows).
 
   1. the order kernel against the numpy restatement, bit for bit, up to entry 2^20 - 1 and chain0 near 2^32;
   2. the token-set sampler against float64 for 1, 20, 21 and 32 tokens: draws away from near-ties, log q bit for bit
      against esmb200_log_softmax_rows, ties to the smaller a, an out-of-range entry, the block sums;
-  3. with the 20 amino acids on a one-row layout, bit for bit esmb200_sample_rows;
-  4. a chi-square test of 200,000 draws over the 21-token set;
-  5. msa_gibbs on the tiny MSA fixture in fp16 and fp32x3: fixed entries, drawable tokens, chunking, seeds, and every
+  3. a chi-square test of 200,000 draws over the 21-token set;
+  4. msa_gibbs on the tiny MSA fixture in fp16 and fp32x3: fixed entries, drawable tokens, chunking, seeds, and every
      step replayed through the public forward and the float64 Gumbel restatement;
-  6. one step's logits against the float64 oracle, and the draws wherever the Gumbel gap exceeds that error;
-  7. no host synchronisation after the first step;
-  8. the command line end to end.
+  5. one step's logits against the float64 oracle, and the draws wherever the Gumbel gap exceeds that error;
+  6. no host synchronisation after the first step;
+  7. the command line end to end.
 Every gated comparison prints a PARITY line.
 """
 import json
@@ -24,9 +23,8 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 if HERE not in sys.path:
-    sys.path.insert(0, HERE)  # sampling_refs, msa_sampling_refs, variant_fixtures
+    sys.path.insert(0, HERE)  # sampling_refs, variant_fixtures
 
-import msa_sampling_refs as mr  # noqa: E402
 import sampling_refs as sr  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -45,12 +43,12 @@ def _tempered(logits, tau):
     return logits / torch.full_like(logits, tau)
 
 
-def _rows_set(logits, token_set, tau, seed, step, chain0, per, entries, tokens, R, C, logp=None, stride=0):
+def _rows(logits, token_set, tau, seed, step, chain0, per, entries, tokens, R, C, logp=None, stride=0):
     from esm_b200 import _lib
     n = logits.shape[0]
     ts = torch.tensor(token_set, dtype=torch.int32, device="cuda")
     logq = torch.full((n,), float("nan"), device="cuda")
-    _lib.check(_lib.load().esmb200_sample_rows_set(
+    _lib.check(_lib.load().esmb200_sample_rows(
         logits.data_ptr(), logits.stride(0), n, ts.data_ptr(), len(token_set), tau, seed, step, chain0, per,
         entries.data_ptr(), tokens.data_ptr(), tokens[0].numel(), R, C, logq.data_ptr(),
         logp.data_ptr() if logp is not None else None, stride, _stream()))
@@ -59,18 +57,18 @@ def _rows_set(logits, token_set, tau, seed, step, chain0, per, entries, tokens, 
 
 # ---- 1. the order kernel --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("n,chains,chain0", [(1, 1, 0), (37, 5, 2 ** 32 - 5), (4093, 9, 3)])
-def test_msa_sample_order_matches_the_restatement(n, chains, chain0):
+def test_sample_order_of_alignment_entries_matches_the_restatement(n, chains, chain0):
     from esm_b200 import _lib
     entries = np.random.default_rng(n).choice(1 << 20, n, replace=False)
     entries[0] = (1 << 20) - 1
     ent = torch.as_tensor(entries, device="cuda")
     keys = torch.empty((chains, n), dtype=torch.int64, device="cuda")
     for sweep, seed in [(0, 0), (9, 2 ** 64 - 1), (2 ** 32 - 1, 77)]:
-        _lib.check(_lib.load().esmb200_msa_sample_order(ent.data_ptr(), n, chains, chain0, sweep, seed,
-                                                        keys.data_ptr(), _stream()))
-        want = mr.msa_order_keys(entries, chain0 + np.arange(chains), sweep, seed)
+        _lib.check(_lib.load().esmb200_sample_order(ent.data_ptr(), n, chains, chain0, sweep, seed, keys.data_ptr(),
+                                                    _stream()))
+        want = sr.order_keys(entries, chain0 + np.arange(chains), sweep, seed)
         assert np.array_equal(keys.cpu().numpy(), want), (sweep, seed)
-    print(f"PARITY msa_sample_order n={n} chains={chains} chain0={chain0}: bit-identical to the numpy restatement")
+    print(f"PARITY sample_order n={n} chains={chains} chain0={chain0}: bit-identical to the numpy restatement")
 
 
 # ---- 2. the token-set sampler ---------------------------------------------------------------------------------------
@@ -80,7 +78,7 @@ SETS = {1: [7], 20: AA, 21: AA + [GAP], 32: [int(v) for v in np.random.default_r
 @pytest.mark.parametrize("tau", [0.05, 1.0, 20.0])
 @pytest.mark.parametrize("n_set", sorted(SETS))
 @pytest.mark.parametrize("per", [1, 7, 40])
-def test_sample_rows_set_against_float64(per, n_set, tau):
+def test_sample_rows_over_token_sets_against_float64(per, n_set, tau):
     from esm_b200 import variants
     token_set = SETS[n_set]
     R, C, chains = 5, 9, 6  # 40 entries per alignment
@@ -93,19 +91,19 @@ def test_sample_rows_set_against_float64(per, n_set, tau):
     before = tokens.clone()
     seed, step, chain0 = 2 ** 64 - 5, 11, 2 ** 32 - chains
     logp = torch.full((chains, 3), float("nan"), device="cuda")
-    logq = _rows_set(logits, token_set, tau, seed, step, chain0, per, ent, tokens, R, C, logp[:, 1], 3)
+    logq = _rows(logits, token_set, tau, seed, step, chain0, per, ent, tokens, R, C, logp[:, 1], 3)
     z = _tempered(logits[:, token_set], tau)
     chain = chain0 + np.arange(n) // per
     entries = ent.cpu().numpy()
-    score, want = mr.draw_f64(z.cpu().numpy(), step, chain, entries, seed)
-    r, j = mr.entry_token(entries, C)
+    score, want = sr.draw_f64(z.cpu().numpy(), step, chain, entries, seed)
+    r, j = sr.entry_token(entries, C)
     local = np.arange(n) // per
     got_tok = tokens.cpu().numpy()[local, r, j]
     lookup = {t: a for a, t in enumerate(token_set)}
     got = np.array([lookup.get(int(t), -1) for t in got_tok])
     close = sr.top_two_gap(score) <= NEAR_TIE if n_set > 1 else np.zeros(n, dtype=bool)
     mism = int((got != want)[~close].sum())
-    print(f"PARITY sample_rows_set |A|={n_set} per={per} tau={tau}: {mism} draws differ from float64 away from "
+    print(f"PARITY sample_rows |A|={n_set} per={per} tau={tau}: {mism} draws differ from float64 away from "
           f"near-ties, {int(close.sum())} near-ties")
     assert mism == 0 and bool((got >= 0).all())
     ref = variants.log_softmax_rows(z.contiguous(), torch.as_tensor(got, device="cuda"))
@@ -123,7 +121,7 @@ def test_sample_rows_set_against_float64(per, n_set, tau):
 
 
 @pytest.mark.parametrize("n_set", [20, 21, 32])
-def test_ties_go_to_the_smaller_index_and_out_of_range_entries_write_nothing(n_set):
+def test_sample_rows_ties_go_to_the_smaller_index_and_out_of_range_entries_write_nothing(n_set):
     """Two set members at 1e30 and the rest at -1e30: every Gumbel score rounds to 1e30 exactly, a tie, so the
     smaller index wins with log q = -log 2. Entries -1 and R (C - 1) write nothing and give a NaN log q."""
     token_set = SETS[n_set]
@@ -134,41 +132,18 @@ def test_ties_go_to_the_smaller_index_and_out_of_range_entries_write_nothing(n_s
         logits[i, token_set[a]] = logits[i, token_set[b]] = 1e30
     ent = torch.tensor([0, 4, 9, 14, -1, R * (C - 1)], device="cuda")
     tokens = torch.zeros((6, R, C), dtype=torch.int64, device="cuda")
-    logq = _rows_set(logits, token_set, 1.0, 3, 0, 0, 1, ent, tokens, R, C)
+    logq = _rows(logits, token_set, 1.0, 3, 0, 0, 1, ent, tokens, R, C)
     for i, (a, _) in enumerate(pairs):
-        r, j = mr.entry_token(int(ent[i]), C)
+        r, j = sr.entry_token(int(ent[i]), C)
         assert int(tokens[i, r, j]) == token_set[a], (i, a)
         assert float(logq[i]) == pytest.approx(-np.log(2), abs=1e-6)
     assert bool(logq[-2:].isnan().all()) and int(tokens[-2:].abs().sum()) == 0
     assert int((tokens != 0).sum()) == len(pairs)
-    print(f"PARITY sample_rows_set |A|={n_set}: ties to the smaller index, out-of-range entries write nothing")
+    print(f"PARITY sample_rows |A|={n_set}: ties to the smaller index, out-of-range entries write nothing")
 
 
-# ---- 3. the sequence sampler is the one-row case ------------------------------------------------------------------
-@pytest.mark.parametrize("tau", [0.3, 1.0])
-def test_one_row_with_the_amino_acids_is_sample_rows(tau):
-    from esm_b200 import _lib
-    lib = _lib.load()
-    T, chains, per = 60, 50, 9
-    n = chains * per
-    g = torch.Generator(device="cuda").manual_seed(5)
-    logits = torch.randn((n, 33), device="cuda", generator=g) * 2
-    pos = torch.stack([torch.randperm(T - 2, device="cuda", generator=g)[:per] for _ in range(chains)]).view(-1)
-    a = torch.randint(0, 33, (chains, T), device="cuda", generator=g)
-    b = a.clone()
-    seed, step, chain0 = 991, 3, 17
-    logq_a = torch.empty(n, device="cuda")
-    logp_a = torch.empty((chains, 2), device="cuda")
-    logp_b = torch.empty((chains, 2), device="cuda")
-    _lib.check(lib.esmb200_sample_rows(logits.data_ptr(), 33, n, 4, tau, seed, step, chain0, per, pos.data_ptr(),
-                                       a.data_ptr(), T, logq_a.data_ptr(), logp_a[:, 1].data_ptr(), 2, _stream()))
-    logq_b = _rows_set(logits, AA, tau, seed, step, chain0, per, pos, b.view(chains, 1, T), 1, T - 1, logp_b[:, 1], 2)
-    print(f"PARITY sample_rows_set one row, 20 amino acids, tau={tau}: tokens, log q and logp against sample_rows")
-    assert torch.equal(a, b) and torch.equal(logq_a, logq_b) and torch.equal(logp_a[:, 1], logp_b[:, 1])
-
-
-# ---- 4. statistics ----------------------------------------------------------------------------------------------------
-def test_two_hundred_thousand_draws_follow_the_tempered_softmax():
+# ---- 3. statistics ----------------------------------------------------------------------------------------------------
+def test_two_hundred_thousand_draws_over_21_tokens_follow_the_tempered_softmax():
     from scipy.stats import chisquare
     token_set = AA + [GAP]
     z = torch.linspace(-3.0, 1.0, 21)
@@ -179,16 +154,16 @@ def test_two_hundred_thousand_draws_follow_the_tempered_softmax():
     counts = torch.zeros(33, dtype=torch.int64)
     for step in range(8):  # 8 steps x 25,000 chains
         tokens = torch.zeros((25000, 1, 2), dtype=torch.int64, device="cuda")
-        _rows_set(logits, token_set, tau, 31337, step, 0, 1, ent, tokens, 1, 2)
+        _rows(logits, token_set, tau, 31337, step, 0, 1, ent, tokens, 1, 2)
         counts += torch.bincount(tokens[:, 0, 1].cpu(), minlength=33)
     assert int(counts.sum()) == 200000 and int(counts[token_set].sum()) == 200000
     p = torch.softmax(_tempered(z, tau).double(), 0).numpy()
     stat, pval = chisquare(counts[token_set].numpy(), p * 200000)
-    print(f"PARITY sample_rows_set chi-square of 200,000 draws over 21 tokens: {stat:.2f} on 20 dof, p = {pval:.3g}")
+    print(f"PARITY sample_rows chi-square of 200,000 draws over 21 tokens: {stat:.2f} on 20 dof, p = {pval:.3g}")
     assert pval > 1e-3
 
 
-# ---- 5. msa_gibbs on the tiny MSA fixture ---------------------------------------------------------------------------
+# ---- 4. msa_gibbs on the tiny MSA fixture ---------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def msa_fixture(golden_dir):
     import variant_fixtures as vf
@@ -281,13 +256,13 @@ def test_every_step_replayed_through_the_public_forward(msa_fixture, precision, 
             s = 0
             logp = []
             for w in range(sweeps):
-                for blk in mr.msa_sweep_blocks(entries, c, w, seed, block):
-                    r, j = mr.entry_token(blk, C)
+                for blk in sr.sweep_blocks(entries, c, w, seed, block):
+                    r, j = sr.entry_token(blk, C)
                     masked = state.clone()
                     masked[0, r, j] = model.mask_idx
                     logits = model(masked)["logits"][0, r, j][:, token_set].float()
                     z = _tempered(logits, tau)
-                    score, a = mr.draw_f64(z.cpu().numpy(), s, np.full(len(blk), c), blk, seed)
+                    score, a = sr.draw_f64(z.cpu().numpy(), s, np.full(len(blk), c), blk, seed)
                     min_gap = min(min_gap, float(sr.top_two_gap(score).min()))
                     logq = variants.log_softmax_rows(z.contiguous(), torch.as_tensor(a, device="cuda")).cpu().numpy()
                     acc = np.float32(0)
@@ -305,7 +280,7 @@ def test_every_step_replayed_through_the_public_forward(msa_fixture, precision, 
         model.set_precision("fp16")
 
 
-# ---- 6. against the float64 oracle ------------------------------------------------------------------------------------
+# ---- 5. against the float64 oracle ------------------------------------------------------------------------------------
 @pytest.mark.parametrize("precision,tol", [("fp16", 2e-2), ("fp32x3", 1e-3)])
 def test_one_step_against_the_float64_oracle(msa_fixture, precision, tol):
     """One step (block = every designable entry): the logits at the block's entries against msa_transformer_forward
@@ -326,8 +301,8 @@ def test_one_step_against_the_float64_oracle(msa_fixture, precision, tol):
         tau, seed, chains = 0.9, 55, 3
         out = sampling.msa_gibbs(model, x, designable=des, chains=chains, block=len(entries), temperature=tau,
                                  seed=seed)
-        blk = mr.msa_sweep_blocks(entries, 0, 0, seed, len(entries))[0]
-        r, j = mr.entry_token(blk, C)
+        blk = sr.sweep_blocks(entries, 0, 0, seed, len(entries))[0]
+        r, j = sr.entry_token(blk, C)
         masked = x.clone()
         masked[0, r, j] = model.mask_idx
         got = model(masked)["logits"][0, r, j].double().cpu()
@@ -339,7 +314,7 @@ def test_one_step_against_the_float64_oracle(msa_fixture, precision, tol):
         err = np.abs(_tempered(got[:, token_set].float().cuda(), tau).double().cpu().numpy() - z_ref).max(-1)
         agree, decided = 0, 0
         for c in range(chains):
-            score, a = mr.draw_f64(z_ref, 0, np.full(len(blk), c), blk, seed)
+            score, a = sr.draw_f64(z_ref, 0, np.full(len(blk), c), blk, seed)
             sure = sr.top_two_gap(score) > 2 * err
             drawn = out["tokens"][c, r, j].cpu().numpy()
             decided += int(sure.sum())
@@ -352,7 +327,7 @@ def test_one_step_against_the_float64_oracle(msa_fixture, precision, tol):
         model.set_precision("fp16")
 
 
-# ---- 7. host synchronisation ------------------------------------------------------------------------------------------
+# ---- 6. host synchronisation ------------------------------------------------------------------------------------------
 def test_no_host_synchronisation_after_the_first_step(msa_fixture):
     from esm_b200 import sampling
     model, _, tokens, _, _ = msa_fixture
@@ -381,7 +356,7 @@ def test_no_host_synchronisation_after_the_first_step(msa_fixture):
     assert not bool((out["tokens"] == model.mask_idx).any())
 
 
-# ---- 8. the command line ----------------------------------------------------------------------------------------------
+# ---- 7. the command line ----------------------------------------------------------------------------------------------
 def test_cli_end_to_end(msa_fixture, tmp_path):
     import variant_fixtures as vf
     from esm_b200 import sample_msa_cli, sampling, variants

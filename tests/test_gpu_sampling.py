@@ -1,9 +1,10 @@
-"""GPU: Gibbs sampling (esm_b200.sampling, esmb200_sample_order, esmb200_sample_rows).
+"""GPU: Gibbs sampling of sequences (esm_b200.sampling.gibbs, esmb200_sample_order, esmb200_sample_rows).
 
-  1. the sampler kernel against the float64/numpy oracle at several temperatures and row counts: a* on every row
+  1. the sampler kernel in the sequence layout (the 20 amino acids, R = 1, C = T - 1, stride T) against the
+     float64/numpy oracle at several temperatures and row counts: a* on every row
      whose top two scores are more than 1e-5 apart, log q bit for bit against esmb200_log_softmax_rows, only the
      targeted token entries written, the block sums of log q;
-  2. the order kernel against the numpy restatement, bit for bit;
+  2. the order kernel on residue indices against the numpy restatement, bit for bit;
   3. a chi-square test of 200,000 draws of one row against softmax(z);
   4. tiny ESM-2 and ESM-1b models in fp16 and fp32x3: fixed positions, amino acids only after sweep 0 of a de novo
      start, reproducibility, chunking, log q against the public forward, the tokens against the oracle's draw;
@@ -28,6 +29,7 @@ import sampling_refs as sr  # noqa: E402
 pytestmark = pytest.mark.gpu
 
 AA0 = 4  # AMINO_ACIDS are tokens 4 ... 23 of the ESM-1b / ESM-2 alphabet
+AA = list(range(AA0, AA0 + 20))
 NEAR_TIE = 1e-5
 
 
@@ -36,12 +38,16 @@ def _stream():
 
 
 def _rows(logits, tau, seed, step, chain0, per, pos, tokens, logp=None, stride=0):
+    """esmb200_sample_rows in the sequence layout: the 20 amino acids, tokens [chains, T] as R = 1, C = T - 1."""
     from esm_b200 import _lib
     n = logits.shape[0]
+    T = tokens.shape[1]
+    ts = torch.tensor(AA, dtype=torch.int32, device="cuda")
     logq = torch.full((n,), float("nan"), device="cuda")
-    rc = _lib.load().esmb200_sample_rows(logits.data_ptr(), logits.stride(0), n, AA0, tau, seed, step, chain0, per,
-                                         pos.data_ptr(), tokens.data_ptr(), tokens.shape[1], logq.data_ptr(),
-                                         logp.data_ptr() if logp is not None else None, stride, _stream())
+    rc = _lib.load().esmb200_sample_rows(logits.data_ptr(), logits.stride(0), n, ts.data_ptr(), len(AA), tau, seed,
+                                         step, chain0, per, pos.data_ptr(), tokens.data_ptr(), T, 1, T - 1,
+                                         logq.data_ptr(), logp.data_ptr() if logp is not None else None, stride,
+                                         _stream())
     _lib.check(rc)
     return logq
 
@@ -52,17 +58,10 @@ def _tempered(logits, tau):
     return logits / torch.full_like(logits, tau)
 
 
-def _oracle_draw(z, tau_rows_chain, pos, step, seed):
-    """float64 Gumbel-max on fp32 z [n, 20] with the numpy Philox uniforms of each row (chain, p)."""
-    words = sr.philox4x32_10(step, tau_rows_chain[:, None], pos[:, None], np.arange(1, 6)[None, :], seed)
-    u = sr.uniform(np.stack(words, -1).reshape(len(pos), 20))
-    return sr.gumbel_max_f64(z, u)
-
-
 # ---- 1. the sampler kernel ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("tau", [0.3, 1.0, 2.5])
 @pytest.mark.parametrize("n,per", [(1, 1), (31, 31), (32, 4), (65537, 1)])
-def test_sample_rows_against_float64(n, per, tau):
+def test_sample_rows_in_the_sequence_layout_against_float64(n, per, tau):
     from esm_b200 import variants
     g = torch.Generator(device="cuda").manual_seed(n * 7 + int(tau * 10))
     T = 300
@@ -76,7 +75,7 @@ def test_sample_rows_against_float64(n, per, tau):
     logq = _rows(logits, tau, seed, step, chain0, per, pos, tokens, logp[:, 1], 3)
     z = _tempered(logits[:, AA0:AA0 + 20], tau)
     chain = chain0 + np.arange(n) // per
-    score, want = _oracle_draw(z.cpu().numpy(), chain, pos.cpu().numpy(), step, seed)
+    score, want = sr.draw_f64(z.cpu().numpy(), step, chain, pos.cpu().numpy(), seed)
     rows = torch.arange(n, device="cuda") // per
     got = (tokens[rows, pos + 1] - AA0).cpu().numpy()
     close = sr.top_two_gap(score) <= NEAR_TIE
@@ -98,7 +97,7 @@ def test_sample_rows_against_float64(n, per, tau):
     assert bool(logp[:, 0].isnan().all()) and bool(logp[:, 2].isnan().all())
 
 
-def test_sample_rows_argument_checks_and_an_out_of_range_position():
+def test_sequence_layout_argument_checks_and_an_out_of_range_position():
     from esm_b200 import _lib
     logits = torch.zeros((2, 33), device="cuda")
     tokens = torch.zeros((2, 6), dtype=torch.int64, device="cuda")
@@ -106,14 +105,14 @@ def test_sample_rows_argument_checks_and_an_out_of_range_position():
     logq = _rows(logits, 1.0, 0, 0, 0, 1, pos, tokens)
     assert bool(logq[1].isnan()) and int(tokens[1].abs().sum()) == 0
     assert AA0 <= int(tokens[0, 4]) < AA0 + 20 and float(logq[0]) == pytest.approx(-np.log(20), abs=1e-6)
-    lib = _lib.load()
-    assert lib.esmb200_sample_rows(logits.data_ptr(), 33, 2, AA0, 0.0, 0, 0, 0, 1, pos.data_ptr(), tokens.data_ptr(),
-                                   6, logq.data_ptr(), None, 0, _stream()) == -1
+    ts = torch.tensor(AA, dtype=torch.int32, device="cuda")
+    assert _lib.load().esmb200_sample_rows(logits.data_ptr(), 33, 2, ts.data_ptr(), 20, 0.0, 0, 0, 0, 1, pos.data_ptr(),
+                                           tokens.data_ptr(), 6, 1, 5, logq.data_ptr(), None, 0, _stream()) == -1
 
 
 # ---- 2. the order kernel --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("n,chains,chain0", [(1, 1, 0), (37, 5, 2 ** 32 - 5), (1022, 64, 3)])
-def test_sample_order_matches_the_restatement(n, chains, chain0):
+def test_sample_order_of_residue_indices_matches_the_restatement(n, chains, chain0):
     from esm_b200 import _lib
     g = np.random.default_rng(n)
     positions = g.choice(65535, n, replace=False)
@@ -129,7 +128,7 @@ def test_sample_order_matches_the_restatement(n, chains, chain0):
 
 
 # ---- 3. statistics ----------------------------------------------------------------------------------------------------
-def test_two_hundred_thousand_draws_follow_softmax():
+def test_two_hundred_thousand_sequence_layout_draws_follow_softmax():
     from scipy.stats import chisquare
     z = torch.linspace(-3.0, 1.0, 20)
     logits = torch.zeros((25000, 33), device="cuda")
@@ -233,7 +232,7 @@ def test_one_step_against_the_public_forward_and_the_oracle(fixtures, name, prec
         zn = z.float().cpu().numpy()
         mism, ties = 0, 0
         for c in range(C):
-            score, want = _oracle_draw(zn, np.full(len(D), c), np.array(D), 0, seed)
+            score, want = sr.draw_f64(zn, 0, np.full(len(D), c), np.array(D), seed)
             close = sr.top_two_gap(score) <= NEAR_TIE
             ties += int(close.sum())
             mism += int((drawn[c].cpu().numpy() != want)[~close].sum())

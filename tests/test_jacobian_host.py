@@ -147,15 +147,15 @@ def test_cli_refuses_a_random_init_model(tmp_path, monkeypatch):
 
 
 # ---- the C ABI --------------------------------------------------------------------------------------------------
-def test_new_symbols_are_declared_and_exported_at_abi_version_3():
+def test_jacobian_symbols_are_declared_and_exported_at_abi_version_4():
     from esm_b200 import _lib
     text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "esmb200.h")).read(), flags=re.S)
     for name in ("esmb200_jacobian_scratch_bytes", "esmb200_jacobian_contacts"):
         assert re.search(rf"\b{name}\s*\(", text), name
         assert name in _lib.EXPORTS
-    assert re.search(r"#define ESMB200_ABI_VERSION 3\b", text)
-    assert _lib.ABI_VERSION == 3
-    assert _lib.load().esmb200_abi_version() == 3
+    assert re.search(r"#define ESMB200_ABI_VERSION 4\b", text)
+    assert _lib.ABI_VERSION == 4
+    assert _lib.load().esmb200_abi_version() == 4
 
 
 @pytest.mark.parametrize("L,nbytes", [(0, 0), (1, 0), (2, 23296), (3, 33280), (17, 169984), (64, 651520),

@@ -1,8 +1,7 @@
 """CPU: alignment sampling from the MSA Transformer (esm_b200.sampling.msa_gibbs) without a GPU. The restatement of the
 20-bit visiting order and block partition, every refusal of msa_gibbs raised before any launch, a valid call reaching
-the launch, the command line's parser and designable entries, and the new C ABI symbols and their argument checks."""
+the launch, and the command line's parser and designable entries."""
 import os
-import re
 import sys
 
 import numpy as np
@@ -11,12 +10,9 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 if HERE not in sys.path:
-    sys.path.insert(0, HERE)  # sampling_refs, msa_sampling_refs
+    sys.path.insert(0, HERE)  # sampling_refs
 
-import msa_sampling_refs as mr  # noqa: E402
 import sampling_refs as sr  # noqa: E402
-
-ROOT = os.path.dirname(HERE)
 
 
 # ---- order and partition ----------------------------------------------------------------------------------------
@@ -29,7 +25,7 @@ def test_every_entry_once_per_sweep_and_the_block_sizes(n, block):
     n = len(entries)
     k = min(block, n)
     for chain, sweep, seed in [(0, 0, 0), (5, 3, 2 ** 64 - 1), (2 ** 32 - 1, 7, 12345)]:
-        blocks = mr.msa_sweep_blocks(entries, chain, sweep, seed, block)
+        blocks = sr.sweep_blocks(entries, chain, sweep, seed, block)
         assert len(blocks) == -(-n // k)
         assert [len(b) for b in blocks[:-1]] == [k] * (len(blocks) - 1)
         assert len(blocks[-1]) == n - k * (len(blocks) - 1)
@@ -37,20 +33,23 @@ def test_every_entry_once_per_sweep_and_the_block_sizes(n, block):
 
 
 def test_the_order_is_the_sequence_order_when_both_keys_apply():
-    """x dominates both keys, so for entries below 2^16 the 20-bit order equals the sequence sampler's 16-bit one."""
+    """x dominates the key, so the order is x ascending with ties to the smaller entry: for the residue indices of a
+    protein (below 2^16) it is the order of any key x * 2^b + p with 2^b above them."""
     positions = np.random.default_rng(3).choice(65535, 300, replace=False)
     for chain, sweep, seed in [(0, 0, 0), (9, 4, 2 ** 63 + 11)]:
-        a = np.concatenate(mr.msa_sweep_blocks(positions, chain, sweep, seed, 7))
-        b = np.concatenate(sr.sweep_blocks(positions, chain, sweep, seed, 7))
-        assert np.array_equal(a, b)
+        a = np.concatenate(sr.sweep_blocks(positions, chain, sweep, seed, 7))
+        x = sr.philox4x32_10(sweep, chain, positions, 0, seed)[0].astype(np.int64)
+        assert np.array_equal(a, positions[np.lexsort((positions, x))])
+        assert np.array_equal(a, np.sort(x * 65536 + positions) % 65536)
 
 
 def test_entry_index_and_uniforms():
-    r, j = mr.entry_token([0, 5, 6, 13], 7)
+    r, j = sr.entry_token([0, 5, 6, 13], 7)
     assert r.tolist() == [0, 0, 1, 2] and j.tolist() == [1, 6, 1, 2]
-    u = mr.set_uniforms(4, [3], [17], 4242, 20)
-    assert np.array_equal(u[0], sr.gumbel_uniforms(4, 3, 17, 4242))  # the first 20 are the sequence sampler's
-    u32 = mr.set_uniforms(4, [3, 3], [17, 18], 4242, 32)
+    u = sr.uniforms(4, [3], [17], 4242, 20)
+    words = sr.philox4x32_10(4, 3, 17, np.arange(1, 6), 4242)  # 4 arrays of 5: the 20 uniforms of one row
+    assert np.array_equal(u[0], sr.uniform(np.stack(words, 1).reshape(-1)))
+    u32 = sr.uniforms(4, [3, 3], [17, 18], 4242, 32)
     assert u32.shape == (2, 32) and np.array_equal(u32[0, :20], u[0]) and not np.array_equal(u32[0], u32[1])
 
 
@@ -247,38 +246,3 @@ def test_cli_refuses_a_random_init_model(tmp_path, monkeypatch):
         with pytest.raises(RuntimeError, match="random-init"):
             sample_msa_cli.run(args)
     assert not out.exists()
-
-
-# ---- the C ABI --------------------------------------------------------------------------------------------------
-def test_new_symbols_are_declared_and_exported_at_abi_version_3():
-    from esm_b200 import _lib
-    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "esmb200.h")).read(), flags=re.S)
-    for name in ("esmb200_msa_sample_order", "esmb200_sample_rows_set"):
-        assert re.search(rf"\b{name}\s*\(", text), name
-        assert name in _lib.EXPORTS
-    assert _lib.load().esmb200_abi_version() == 3
-
-
-def test_entry_points_check_their_arguments_before_any_launch():
-    """Every refusal returns ESMB200_EINVAL with no device: argument checks come before any CUDA call."""
-    from esm_b200 import _lib
-    lib = _lib.load()
-    p = 16  # any non-null address: never dereferenced on a refusal
-    order = lambda *a: lib.esmb200_msa_sample_order(*a)
-    assert order(p, 0, 1, 0, 0, 0, p, None) == -1                 # n == 0
-    assert order(p, 4, -1, 0, 0, 0, p, None) == -1                # n_chains < 0
-    assert order(p, 4, 1, 2 ** 32, 0, 0, p, None) == -1           # chain0 + n_chains > 2^32
-    assert order(p, 4, 1, -1, 0, 0, p, None) == -1
-    assert order(p, 4, 1, 0, 2 ** 32, 0, p, None) == -1           # sweep >= 2^32
-    assert order(p, 4, 1, 0, -1, 0, p, None) == -1
-    assert order(p, 4, 0, 0, 0, 0, p, None) == 0                  # no chains: nothing launched
-    rows = lambda **kw: lib.esmb200_sample_rows_set(*{**dict(
-        logits=p, ld=33, n=8, set=p, n_set=21, tau=1.0, seed=0, step=0, chain0=0, per=2, ent=p, tok=p, stride=40,
-        R=4, C=10, logq=p, logp=None, lstride=0, stream=None), **kw}.values())
-    for kw in [dict(n=-1), dict(per=0), dict(n=7), dict(n_set=0), dict(n_set=33), dict(ld=0), dict(tau=0.0),
-               dict(tau=-1.0), dict(tau=float("inf")), dict(tau=float("nan")), dict(R=0), dict(C=1),
-               dict(stride=39), dict(step=2 ** 32), dict(step=-1), dict(chain0=2 ** 32 - 3), dict(chain0=-1),
-               dict(logp=p, lstride=0), dict(logits=None), dict(set=None), dict(ent=None), dict(tok=None),
-               dict(logq=None)]:
-        assert rows(**kw) == -1, kw
-    assert rows(n=0) == 0

@@ -9,13 +9,13 @@ import torch
 NEW_SYMBOLS = ("esmb200_layer_packed_bytes", "esmb200_layer_offload", "esmb200_stack_forward_streamed")
 
 
-def test_new_symbols_are_exported():
+def test_offload_symbols_are_exported_at_abi_version_4():
     from esm_b200 import _lib
     lib = ctypes.CDLL(_lib.LIB_PATH)
     for name in NEW_SYMBOLS:
         assert name in _lib.EXPORTS
         assert hasattr(lib, name)
-    assert _lib.load().esmb200_abi_version() == 3
+    assert _lib.load().esmb200_abi_version() == 4
 
 
 @pytest.mark.parametrize("args,nbytes", [

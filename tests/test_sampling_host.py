@@ -74,7 +74,7 @@ def test_orders_differ_between_chains_sweeps_and_seeds():
     for chain, sweep, seed in [(1, 0, 0), (0, 1, 0), (0, 0, 1)]:
         assert not np.array_equal(np.concatenate(sr.sweep_blocks(positions, chain, sweep, seed, 1)), base)
     keys = sr.order_keys(positions, np.arange(4), 0, 9)
-    assert keys.shape == (4, 40) and np.array_equal(keys % 65536, np.broadcast_to(positions, (4, 40)))
+    assert keys.shape == (4, 40) and np.array_equal(keys % (1 << 20), np.broadcast_to(positions, (4, 40)))
 
 
 def test_gumbel_max_frequencies_of_the_restatement():
@@ -90,7 +90,7 @@ def test_gumbel_max_frequencies_of_the_restatement():
     stat, pval = chisquare(counts, p * n)
     print(f"restated Gumbel-max chi-square {stat:.2f}, p = {pval:.3g}")
     assert pval > 1e-3
-    assert np.array_equal(sr.gumbel_uniforms(5, 3, 17, 4242), u[5])
+    assert np.array_equal(sr.uniforms(5, [3], [17], 4242, 20)[0], u[5])
 
 
 # ---- refusals, before any launch: CPU-resident models would raise Esmb200Error at the first launch ---------------
@@ -222,30 +222,35 @@ def test_cli_refuses_a_random_init_model(tmp_path, monkeypatch):
 
 
 # ---- the C ABI --------------------------------------------------------------------------------------------------
-def test_new_symbols_are_declared_and_exported_at_abi_version_3():
+def test_symbols_are_declared_and_exported_at_abi_version_4():
     from esm_b200 import _lib
     text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "esmb200.h")).read(), flags=re.S)
     for name in ("esmb200_sample_order", "esmb200_sample_rows"):
         assert re.search(rf"\b{name}\s*\(", text), name
         assert name in _lib.EXPORTS
-    assert _lib.load().esmb200_abi_version() == 3
+    assert _lib.load().esmb200_abi_version() == 4
 
 
-def test_entry_points_check_their_arguments_before_any_launch():
+def test_sampler_entry_points_check_their_arguments_before_any_launch():
     """Every refusal returns ESMB200_EINVAL with no device: argument checks come before any CUDA call."""
     from esm_b200 import _lib
     lib = _lib.load()
     p = 16  # any non-null address: never dereferenced on a refusal
     order = lambda *a: lib.esmb200_sample_order(*a)
     assert order(p, 0, 1, 0, 0, 0, p, None) == -1                 # n == 0
+    assert order(p, 4, -1, 0, 0, 0, p, None) == -1                # n_chains < 0
     assert order(p, 4, 1, 2 ** 32, 0, 0, p, None) == -1           # chain0 + n_chains > 2^32
+    assert order(p, 4, 1, -1, 0, 0, p, None) == -1
     assert order(p, 4, 1, 0, 2 ** 32, 0, p, None) == -1           # sweep >= 2^32
+    assert order(p, 4, 1, 0, -1, 0, p, None) == -1
     assert order(p, 4, 0, 0, 0, 0, p, None) == 0                  # no chains: nothing launched
-    rows = lambda **kw: lib.esmb200_sample_rows(*{**dict(logits=p, ld=33, n=8, aa=4, tau=1.0, seed=0, step=0,
-                                                        chain0=0, per=2, pos=p, tok=p, T=10, logq=p, logp=None,
-                                                        stride=0, stream=None), **kw}.values())
-    for kw in [dict(n=-1), dict(per=0), dict(n=7), dict(aa=-1), dict(ld=23), dict(tau=0.0), dict(tau=-1.0),
-               dict(tau=float("inf")), dict(tau=float("nan")), dict(T=2), dict(step=2 ** 32), dict(step=-1),
-               dict(chain0=2 ** 32 - 3), dict(logp=p, stride=0), dict(logits=None)]:
+    rows = lambda **kw: lib.esmb200_sample_rows(*{**dict(
+        logits=p, ld=33, n=8, set=p, n_set=21, tau=1.0, seed=0, step=0, chain0=0, per=2, ent=p, tok=p, stride=40,
+        R=4, C=10, logq=p, logp=None, lstride=0, stream=None), **kw}.values())
+    for kw in [dict(n=-1), dict(per=0), dict(n=7), dict(n_set=0), dict(n_set=33), dict(ld=0), dict(tau=0.0),
+               dict(tau=-1.0), dict(tau=float("inf")), dict(tau=float("nan")), dict(R=0), dict(C=1),
+               dict(stride=39), dict(step=2 ** 32), dict(step=-1), dict(chain0=2 ** 32 - 3), dict(chain0=-1),
+               dict(logp=p, lstride=0), dict(logits=None), dict(set=None), dict(ent=None), dict(tok=None),
+               dict(logq=None)]:
         assert rows(**kw) == -1, kw
     assert rows(n=0) == 0

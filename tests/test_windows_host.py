@@ -147,10 +147,10 @@ def test_extract_cli_window_flag(tmp_path):
     assert not (tmp_path / "out").exists()
 
 
-def test_merge_entry_point_is_exported_at_abi_version_3():
+def test_merge_entry_point_is_exported_at_abi_version_4():
     from esm_b200 import _lib
     header = open(os.path.join(ROOT, "include", "esmb200.h")).read()
     assert re.search(r"\bint esmb200_window_merge\(", header)
     assert "esmb200_window_merge" in _lib.EXPORTS
-    assert re.search(r"#define ESMB200_ABI_VERSION 3\b", header)
-    assert _lib.ABI_VERSION == 3
+    assert re.search(r"#define ESMB200_ABI_VERSION 4\b", header)
+    assert _lib.ABI_VERSION == 4
