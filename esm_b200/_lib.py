@@ -70,9 +70,12 @@ EXPORTS = (
     "esmb200_jacobian_contacts",
     "esmb200_sample_order",
     "esmb200_sample_rows",
+    "esmb200_msa_select_scratch_bytes",
+    "esmb200_msa_greedy_select",
 )
 
 ABI_VERSION = 4
+SELECT_MAX, SELECT_MIN = 0, 1  # ESMB200_SELECT_MAX / ESMB200_SELECT_MIN
 EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32, EPI_GELU_FP8 = range(6)
 
 
@@ -178,6 +181,11 @@ def _declare(lib):
     lib.esmb200_sample_rows.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_float, c_uint64, c_int64,
                                         c_int64, c_int32, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
                                         c_void_p, c_int64, c_void_p]
+    lib.esmb200_msa_select_scratch_bytes.restype = c_size_t
+    lib.esmb200_msa_select_scratch_bytes.argtypes = [c_int32, c_int32, c_int32]
+    lib.esmb200_msa_greedy_select.restype = c_int32
+    lib.esmb200_msa_greedy_select.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                                              c_void_p, c_size_t, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -26,6 +26,7 @@
 #include "gemm2.cuh"
 #include "gemm_fp8.cuh"
 #include "jacobian.cuh"
+#include "msa_select.cuh"
 #include "sampling.cuh"
 #include "tied_attention.cuh"
 
@@ -56,7 +57,7 @@ int fail_cuda(cudaError_t e, const char* what) {
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
                      T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
-                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_COUNT };
+                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_MSA_SELECT, T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1703,6 +1704,52 @@ int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, const int32_
     ProfScope ps(T_SAMPLING, st);
     sample_logp_kernel<<<(unsigned)((n_chains + 255) / 256), 256, 0, st>>>(logq, n_chains, per_chain, logp,
                                                                            logp_stride);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+
+size_t esmb200_msa_select_scratch_bytes(int32_t N, int32_t C, int32_t k) {
+  if (N < 0 || C < 0 || k < 0) return 0;
+  return msa_select_scratch(nullptr, N, C, k).bytes;
+}
+
+int esmb200_msa_greedy_select(const uint8_t* rows, int64_t ld, int32_t N, int32_t C, int32_t k, int32_t mode,
+                              int64_t* selected, void* scratch, size_t scratch_bytes, void* stream) {
+  if (C < 1 || C > 65535) return fail(ESMB200_EINVAL, "msa_greedy_select needs 1 <= C <= 65535");
+  if (N < 0 || k < 0 || k > N) return fail(ESMB200_EINVAL, "msa_greedy_select needs 0 <= k <= N");
+  if (mode != ESMB200_SELECT_MAX && mode != ESMB200_SELECT_MIN)
+    return fail(ESMB200_EINVAL, "msa_greedy_select mode must be ESMB200_SELECT_MAX or ESMB200_SELECT_MIN");
+  if (ld < C || ld % 16 != 0) return fail(ESMB200_EINVAL, "msa_greedy_select needs ld >= C and ld % 16 == 0");
+  if (k == 0) return ESMB200_OK;
+  if (!rows || !selected || !scratch) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(rows) % 16 != 0) return fail(ESMB200_EINVAL, "rows must be 16-byte aligned");
+  const MsaSelectScratch s = msa_select_scratch(static_cast<char*>(scratch), N, C, k);
+  if (scratch_bytes < s.bytes) return fail(ESMB200_EINVAL, "scratch smaller than esmb200_msa_select_scratch_bytes");
+  if (reinterpret_cast<uintptr_t>(scratch) % 256 != 0) return fail(ESMB200_EINVAL, "scratch must be 256-byte aligned");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t smem = (size_t)ld;
+  if (smem > 48 * 1024) {  // the picked row: C <= 65535, so at most 64 KiB
+    CK(cudaFuncSetAttribute(msa_select_step_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaFuncSetAttribute(msa_select_step_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
+    ProfScope ps(T_MSA_SELECT, st);
+    const int n = N > C + 1 ? N : C + 1;
+    msa_select_init_kernel<<<(unsigned)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024), 256, 0, st>>>(
+        N, C, s.dist, s.picked, s.ticket, selected);
+    CK(cudaGetLastError());
+  }
+  const unsigned blocks = (unsigned)(((int64_t)N + kSelThreads - 1) / kSelThreads);
+  for (int t = 1; t < k; ++t) {  // the picked index stays on the device: no host synchronisation in this loop
+    ProfScope ps(T_MSA_SELECT, st);
+    if (mode == ESMB200_SELECT_MAX)
+      msa_select_step_kernel<true><<<blocks, kSelThreads, smem, st>>>(rows, ld, N, t, selected, s);
+    else
+      msa_select_step_kernel<false><<<blocks, kSelThreads, smem, st>>>(rows, ld, N, t, selected, s);
     CK(cudaGetLastError());
   }
   return ESMB200_OK;

@@ -11,6 +11,8 @@ predict.py:45-104, plus --max-tokens) on the library's batched scorers (esm_b200
   * --precision fp32x3 runs every model (sequence models and the MSA Transformer) with fp16 hi + lo operand pairs.
   * --window N scores proteins longer than N residues (ESM-1b / ESM-1v cannot take more than 1022) through overlapping
     windows of N residues (esm_b200.windows), with every strategy; sequence models only.
+  * --msa-select max / min reads the whole a3m file and keeps --msa-samples rows picked by the greedy Hamming
+    selection of the reference's contact notebook (esm_b200.msa_select.greedy_select) instead of the first ones.
   * there is no CPU path: --nogpu raises.
 """
 from __future__ import annotations
@@ -23,10 +25,11 @@ from typing import Dict, List
 
 import torch
 
-from . import pretrained, variants
+from . import msa_select, pretrained, variants
 
 STRATEGIES = ["wt-marginals", "pseudo-ppl", "masked-marginals"]
 PRECISIONS = ["fp16", "fp32x3"]
+MSA_SELECT = ["first", "max", "min"]
 MSA_ONLY_MASKED = "MSA Transformer only supports masked marginal strategy"  # predict.py:163-165
 MSA_NO_WINDOW = "--window applies to ESM-2, ESM-1b and ESM-1v models; MSA Transformer alignments are not windowed"
 
@@ -50,6 +53,10 @@ def create_parser():
                         "pseudo-ppl: pseudo-log-likelihood of each mutated sequence")
     p.add_argument("--msa-path", type=pathlib.Path, help="a3m alignment whose first row is --sequence (MSA Transformer)")
     p.add_argument("--msa-samples", type=int, default=400, help="how many alignment rows to read, from the top")
+    p.add_argument("--msa-select", choices=MSA_SELECT, default="first",
+                   help="which --msa-samples rows to keep: first: the first ones in the file; max / min: the whole file "
+                        "is read and rows are picked greedily for the largest / smallest mean Hamming distance to "
+                        "those already picked, starting from the query (the contact notebook's greedy_select)")
     p.add_argument("--nogpu", action="store_true", help="accepted for compatibility; raises, as there is no CPU path")
     p.add_argument("--max-tokens", type=int, default=variants.DEFAULT_MAX_TOKENS,
                    help="tokens per batched forward of masked copies (at least one copy per forward)")
@@ -117,13 +124,21 @@ def write_table(path, header: List[str], rows: List[List[str]], scores: Dict[str
             w.writerow([str(i)] + r)
 
 
+def read_alignment(path, samples, select: str = "first"):
+    """The alignment rows to run: the first `samples` records of the a3m file (all for None), or with select "max" /
+    "min" `samples` rows of the whole file picked by msa_select.greedy_select."""
+    if select == "first":
+        return variants.read_msa(path, samples)
+    return msa_select.greedy_select(variants.read_msa(path, None), samples, select)
+
+
 def score_model(model, alphabet, is_msa: bool, args, mutations: List[str]) -> List[float]:
     """predict.py:159-233 for one model on the library."""
     window = getattr(args, "window", None)
     if is_msa:
         if window is not None:
             raise ValueError(MSA_NO_WINDOW)
-        data = [variants.read_msa(args.msa_path, args.msa_samples)]
+        data = [read_alignment(args.msa_path, args.msa_samples, getattr(args, "msa_select", "first"))]
         assert args.scoring_strategy == "masked-marginals", MSA_ONLY_MASKED
         _, _, tokens = alphabet.get_batch_converter()(data)
         lp = variants.masked_marginals(model, tokens, max_tokens=args.max_tokens)

@@ -9,7 +9,8 @@ entries: with neither --rows nor --columns, every entry, or only the appended ro
 --columns (1-based numbers and inclusive ranges; rows count the input rows first, then the appended ones; columns
 count alignment columns, not <cls>) make the entries in those rows and columns designable, each defaulting to all;
 appended rows stay designable in full. MODEL is an MSA Transformer name or .pt file, loaded as predict_cli loads it,
-and a random-init model is refused.
+and a random-init model is refused. --msa-select max / min reads the whole file and keeps --msa-samples rows picked by
+esm_b200.msa_select.greedy_select; it needs --msa-samples.
 
 Writes DIR/sample_{c}.a3m per chain (the input descriptions, then generated_{i} for the appended rows, 0-based) and
 DIR/samples.tsv with the columns chain, seed and logp, the summed log q of the chain's last sweep.
@@ -21,8 +22,8 @@ import pathlib
 
 import torch
 
-from . import sampling, variants
-from .predict_cli import load_model
+from . import sampling
+from .predict_cli import MSA_SELECT, load_model, read_alignment
 from .sample_cli import _positive, parse_positions
 from .variants import DEFAULT_MAX_TOKENS
 
@@ -41,6 +42,9 @@ def create_parser():
     p.add_argument("--msa", type=pathlib.Path, required=True, help="a3m alignment to start every chain from")
     p.add_argument("--msa-samples", type=_positive, default=None,
                    help="how many alignment rows to read, from the top (default: all)")
+    p.add_argument("--msa-select", choices=MSA_SELECT, default="first",
+                   help="which --msa-samples rows to keep: first (default) or max / min, picked from the whole file "
+                        "for the largest / smallest mean Hamming distance, as the contact notebook's greedy_select")
     p.add_argument("--rows", type=parse_positions, default=None,
                    help="designable rows, 1-based numbers and inclusive ranges such as 1-3 (default: see above)")
     p.add_argument("--columns", type=parse_positions, default=None,
@@ -83,7 +87,9 @@ def designable_mask(R: int, W: int, appended: int, rows, columns) -> torch.Tenso
 
 def run(args) -> int:
     """Returns the number of chains written."""
-    msa = variants.read_msa(args.msa, args.msa_samples)
+    if args.msa_select != "first" and args.msa_samples is None:
+        raise ValueError(f"--msa-select {args.msa_select} picks --msa-samples rows from the file: give --msa-samples")
+    msa = read_alignment(args.msa, args.msa_samples, args.msa_select)
     if not msa:
         raise ValueError(f"{args.msa} holds no alignment records")
     model, alphabet, _ = load_model(args.model_location)

@@ -295,6 +295,32 @@ int esmb200_sample_rows(const float* logits, int64_t ld, int32_t n, const int32_
                         const int64_t* entries, int64_t* tokens, int64_t chain_stride, int32_t R, int32_t C,
                         float* logq, float* logp, int64_t logp_stride, void* stream);
 
+/* Greedy row selection of a deep alignment for the MSA Transformer (esm_b200/msa_select.py): greedy_select of the
+ * reference's examples/contact_prediction.ipynb ("MSA Transformer" section), which picks the rows fed to
+ * predict_contacts, with the same rows for every input. rows uint8 [N, ld] (device, 16-byte aligned; ld % 16 == 0,
+ * ld >= C, and the bytes in columns [C, ld) equal in every row, so they never differ); bytes are compared as bytes.
+ * selected int64 [k] (device) receives the picked row indices in selection order:
+ *   selected[0] = 0 (the query); for t = 1 ... k - 1:
+ *     d_t[j]   = fp64(count_j / C), count_j = the columns in which row j differs from row selected[t - 1]
+ *                (scipy's cdist(..., "hamming"));
+ *     score[j] = pairwise_sum(d_1[j], ..., d_t[j]) / t in fp64, pairwise_sum numpy's: below 8 terms a sequential sum
+ *                from +0; up to 128 eight strided accumulators r[i % 8] over the first n - n % 8 terms, combined as
+ *                ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)), then the tail added in order; above 128 the sums
+ *                of the halves split at n / 2 - (n / 2) % 8 (the notebook's np.delete(..., axis=1).mean(0) reduces
+ *                an F-contiguous array along its contiguous axis);
+ *     selected[t] = the argmax (ESMB200_SELECT_MAX) or argmin (ESMB200_SELECT_MIN) of score over the rows not yet
+ *                picked, a tie to the smallest index.
+ *   The caller returns the rows unchanged when N <= k, and sorts the indices for the notebook's order.
+ * One init launch and one launch per step; the picked index stays on the device, nothing synchronises with the host.
+ * Deterministic. scratch: esmb200_msa_select_scratch_bytes(N, C, k) bytes, 256-byte aligned (uint16 counts
+ * [k - 1, N] and O(N + C) more). 1 <= C <= 65535, 0 <= k <= N, a known mode, ld as above and enough scratch, else
+ * ESMB200_EINVAL before any launch. k == 0 launches nothing. scratch_bytes of a negative argument is 0. */
+#define ESMB200_SELECT_MAX 0
+#define ESMB200_SELECT_MIN 1
+size_t esmb200_msa_select_scratch_bytes(int32_t N, int32_t C, int32_t k);
+int esmb200_msa_greedy_select(const uint8_t* rows, int64_t ld, int32_t N, int32_t C, int32_t k, int32_t mode,
+                              int64_t* selected, void* scratch, size_t scratch_bytes, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -415,7 +441,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *         7 key bits, 8 embed, 9 LayerNorm fp32, 10 attention probs, 11 convert, 12 other GEMM, 13 mean pool,
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
  *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
- *         and each kernel of esmb200_sample_rows) */
+ *         and each kernel of esmb200_sample_rows), 21 greedy MSA row selection (each kernel of
+ *         esmb200_msa_greedy_select) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
