@@ -1,6 +1,7 @@
 """Float64 references of the categorical Jacobian contact map (esm_b200/jacobian.py, steps 3-6 of its definition):
-`contacts_f64`, the vectorised definition the GPU tests gate against, and `contacts_brute_force`, the same map with
-every mean, norm and sum written out as loops, which pins the definition itself (tests/test_jacobian_host.py)."""
+`contacts_f64`, the vectorised definition the GPU tests gate against; `contacts_f64_chunked`, the same map one slab of
+i at a time, for a J whose float64 copies would not fit; and `contacts_brute_force`, the same map with every mean, norm
+and sum written out as loops, which pins the definition itself (tests/test_jacobian_host.py)."""
 from __future__ import annotations
 
 import itertools
@@ -19,6 +20,42 @@ def contacts_f64(jac: torch.Tensor) -> torch.Tensor:
     a = n - n.sum(1, keepdim=True) * n.sum(0, keepdim=True) / n.sum()
     a.fill_diagonal_(0)
     return (a + a.T) / 2
+
+
+def contacts_f64_chunked(jac: torch.Tensor, rows: int):
+    """contacts_f64 for a J too large for a float64 copy: returns (C [L,L] float64, max N, max|J|) on jac's device,
+    where max N is taken over every block, the diagonal included, before it is zeroed. Float64 slabs of `rows` values
+    of i are formed one at a time:
+      1. the marginal sums over i (S_i [20,L,20]) and over j (S_j [L,20,20]), and max|J|;
+      2. per slab, the centring along i and j, X = J - S_i/L - S_j/L + S/L^2 with S = sum_j S_i, then each 20 x 20
+         block (i, j) centred along a and along b and its Frobenius norm. The four centrings are commuting projections,
+         so this equals centring the whole J along each axis in turn.
+    APC and the symmetrisation then run on N [L,L] as in contacts_f64."""
+    L = jac.shape[0]
+    s_i = torch.zeros((20, L, 20), dtype=torch.float64, device=jac.device)
+    s_j = torch.empty((L, 20, 20), dtype=torch.float64, device=jac.device)
+    jmax = 0.0
+    for i0 in range(0, L, rows):
+        x = jac[i0:i0 + rows].double()
+        s_i += x.sum(0)
+        s_j[i0:i0 + rows] = x.sum(2)
+        jmax = max(jmax, float(x.abs().max()))
+    s = s_i.sum(1)
+    n = torch.empty((L, L), dtype=torch.float64, device=jac.device)
+    for i0 in range(0, L, rows):
+        x = jac[i0:i0 + rows].double()
+        x -= s_i[None] / L
+        x -= s_j[i0:i0 + rows, :, None, :] / L
+        x += s[None, :, None, :] / (L * L)
+        x -= x.mean(1, keepdim=True)
+        x -= x.mean(3, keepdim=True)
+        n[i0:i0 + rows] = x.pow(2).sum((1, 3)).sqrt()
+    del x
+    nmax = float(n.max())
+    n.fill_diagonal_(0)
+    a = n - n.sum(1, keepdim=True) * n.sum(0, keepdim=True) / n.sum()
+    a.fill_diagonal_(0)
+    return (a + a.T) / 2, nmax, jmax
 
 
 def contacts_brute_force(jac: torch.Tensor) -> torch.Tensor:

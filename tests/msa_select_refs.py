@@ -64,14 +64,16 @@ def as_rows(msa):
     return np.array([list(seq) for _, seq in msa], dtype=np.bytes_).view(np.uint8)
 
 
-def greedy_order(rows, k, mode="max"):
+def greedy_order(rows, k, mode="max", shortcut=True):
     """The notebook's picks for uint8 rows [N, C], in selection order (the notebook returns them sorted). N <= k
-    returns every row."""
+    returns every row, as the notebook (and esm_b200.msa_select) does without a selection; shortcut=False instead runs
+    the loop up to k = N, whose last step has a single candidate, as the C ABI does when called with k = N."""
     assert mode in ("max", "min")
     rows = np.asarray(rows, dtype=np.uint8)
     N, C = rows.shape
-    if N <= k:
+    if shortcut and N <= k:
         return list(range(N))
+    assert k <= N
     sel = [0]
     picked = np.zeros(N, dtype=bool)
     picked[0] = True

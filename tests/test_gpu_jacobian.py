@@ -1,7 +1,8 @@
 """GPU: the categorical Jacobian (esm_b200.jacobian, esmb200_jacobian_contacts).
 
   1. the contact kernel against the float64 definition on the same fp32 J, element-wise within a bound derived from
-     the summation lengths; an all-zero J; bit-reproducibility;
+     the summation lengths, at every tile and grid edge of its kernels, with a large term constant along each centred
+     axis, and past 2^31 elements of J, the output and scratch poisoned first; an all-zero J; bit-reproducibility;
   2. batching is exact: J equals a loop of the public forward, for every max_tokens, and identity copies give f_wt;
   3. against the unmodified reference (oracle/_ref) in float64 on the CPU;
   4. cpu_offload() and model.half();
@@ -22,7 +23,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 if HERE not in sys.path:
     sys.path.insert(0, HERE)  # jacobian_refs, variant_fixtures, esm1b_weights
 
-from jacobian_refs import contacts_f64  # noqa: E402
+from jacobian_refs import contacts_f64, contacts_f64_chunked  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -34,29 +35,52 @@ U64 = 2.0 ** -53  # fp64 unit roundoff: every sum of the kernel
 
 
 # ---- 1. the kernel against float64 --------------------------------------------------------------------------------
-def _random_jac(L, seed, offset=0.0):
+# A term constant along the named axes, 100x the substitution effects: the centring along them must cancel it.
+OFFSET_SHAPES = {"i,a": lambda L: (1, 1, L, 20), "i": lambda L: (1, 20, L, 20), "a": lambda L: (L, 1, L, 20),
+                 "j": lambda L: (L, 20, 1, 20), "b": lambda L: (L, 20, L, 1)}
+
+
+def _random_jac(L, seed, offset=0.0, axes="i,a"):
     g = torch.Generator(device="cuda").manual_seed(seed)
-    jac = torch.randn((L, 20, L, 20), device="cuda", generator=g) * 8
+    jac = torch.randn((L, 20, L, 20), device="cuda", generator=g).mul_(8)
     if offset:
-        jac += torch.randn((1, 1, L, 20), device="cuda", generator=g) * offset
+        jac += torch.randn(OFFSET_SHAPES[axes](L), device="cuda", generator=g) * offset
     return jac
 
 
-def _gate(C, jac, label):
-    """C [L,L] from the kernel against contacts_f64 on the same fp32 J. The kernel reads J exactly into fp64 and takes
-    every sum there: S_i and S_j over L terms, S over L^2, a block's centring and norm over 20 and 400, the APC sums
-    over L and L^2. A sequential sum of n terms is off by at most n U64 times the sum of their magnitudes, so relative
-    to max|J| (the marginals and the centred block) and max N (the APC terms) every step stays within (L^2 + 400) U64,
-    a few such steps compose, hence 64 (L^2 + 400) U64 (max|J| + max N). The output rounding adds U32 |C|. The bound
-    must be no looser than 1e-5 max N."""
+def _poisoned_contacts(jac):
+    """esmb200_jacobian_contacts through the C ABI with the output filled with NaN and the scratch with 0xFF bytes
+    (NaN as fp64), so that an entry no kernel writes, or a scratch value read before it is written, shows."""
+    from esm_b200 import _lib
+    lib = _lib.load()
     L = jac.shape[0]
-    want = contacts_f64(jac)
-    jmax = float(jac.abs().max())
-    jc = jac.double()
-    for axis in range(4):
-        jc = jc - jc.mean(axis, keepdim=True)
-    nmax = float(jc.pow(2).sum((1, 3)).sqrt().max())
-    del jc
+    n = lib.esmb200_jacobian_scratch_bytes(L)
+    scratch = torch.full((n,), 0xFF, dtype=torch.uint8, device="cuda")
+    out = torch.full((L, L), float("nan"), device="cuda")
+    _lib.check(lib.esmb200_jacobian_contacts(jac.data_ptr(), L, scratch.data_ptr(), n, out.data_ptr(),
+                                             torch.cuda.current_stream().cuda_stream))
+    return out
+
+
+def _gate(C, jac, label, rows=None):
+    """C [L,L] from the kernel against contacts_f64 on the same fp32 J (contacts_f64_chunked in slabs of `rows` values
+    of i, when given). The kernel reads J exactly into fp64 and takes every sum there: S_i and S_j over L terms, S over
+    L^2, a block's centring and norm over 20 and 400, the APC sums over L and L^2. A sequential sum of n terms is off by
+    at most n U64 times the sum of their magnitudes, so relative to max|J| (the marginals and the centred block) and
+    max N (the APC terms) every step stays within (L^2 + 400) U64, a few such steps compose, hence
+    64 (L^2 + 400) U64 (max|J| + max N). The output rounding adds U32 |C|. The bound must be no looser than
+    1e-5 max N."""
+    L = jac.shape[0]
+    if rows is None:
+        want = contacts_f64(jac)
+        jmax = float(jac.abs().max())
+        jc = jac.double()
+        for axis in range(4):
+            jc = jc - jc.mean(axis, keepdim=True)
+        nmax = float(jc.pow(2).sum((1, 3)).sqrt().max())
+        del jc
+    else:
+        want, nmax, jmax = contacts_f64_chunked(jac, rows)
     f64 = 64 * (L * L + 400) * U64 * (jmax + nmax)
     bound = U32 * want.abs() + f64
     err = (C.double() - want).abs()
@@ -64,27 +88,51 @@ def _gate(C, jac, label):
     print(f"PARITY jacobian_contacts {label} L={L}: max_abs_err={float(err.max()):.3e} max N={nmax:.4g} "
           f"max|C|={float(want.abs().max()):.4g} err/bound={worst:.3e} bound/maxN={float(bound.max()) / nmax:.3e}")
     assert float(bound.max()) <= 1e-5 * nmax
-    assert worst <= 1.0
+    assert worst <= 1.0  # also false for a NaN
 
 
-@pytest.mark.parametrize("L", [2, 3, 17, 64, 300, 1022])
+# 15, 16: pass 1's 16-row staging; 63, 65, 129: its 64-wide j tiles; 255, 256, 257: the 256-column blocks of the APC
+# sums; 512, 513: exactly the APC kernel's 1024 blocks, and one row past them (its grid-stride loop)
+@pytest.mark.parametrize("L", [2, 3, 15, 16, 17, 63, 64, 65, 129, 255, 256, 257, 300, 512, 513, 1022])
 def test_contact_kernel_matches_float64(L):
     from esm_b200 import jacobian
     jac = _random_jac(L, seed=L)
     before = jac.clone()
-    C = jacobian.jacobian_contacts(jac)
-    assert C.dtype == torch.float32 and C.shape == (L, L)
+    C = _poisoned_contacts(jac)
     assert torch.equal(jac, before), "J must be read only"
     _gate(C, jac, "random")
-    assert torch.equal(jacobian.jacobian_contacts(jac), C), "two runs must be bit-identical"
+    got = jacobian.jacobian_contacts(jac)
+    assert got.dtype == torch.float32 and got.shape == (L, L)
+    assert torch.equal(got, C), "two runs must be bit-identical"
 
 
+@pytest.mark.parametrize("axes", list(OFFSET_SHAPES))
 @pytest.mark.parametrize("L", [17, 300])
-def test_contact_kernel_cancels_a_large_common_offset(L):
-    """A wild-type-like term per (j, b), 100x the substitution effects: centring along i must cancel it."""
-    from esm_b200 import jacobian
-    jac = _random_jac(L, seed=100 + L, offset=800.0)
-    _gate(jacobian.jacobian_contacts(jac), jac, "offset")
+def test_contact_kernel_cancels_a_large_common_offset(L, axes):
+    """A term constant along `axes` only (a wild-type-like term per (j, b) for "i,a"), 100x the substitution effects:
+    the fp64 centring along those axes must cancel it."""
+    jac = _random_jac(L, seed=100 + L + 1000 * list(OFFSET_SHAPES).index(axes), offset=800.0, axes=axes)
+    _gate(_poisoned_contacts(jac), jac, f"offset along {axes}")
+
+
+def test_contact_kernel_past_2_31_jacobian_elements():
+    """L = 2400: J holds 2.30e9 elements (9.2 GB), so an index formed in 32 bits anywhere would go wrong. The float64
+    reference is taken one 64-row slab of i at a time; the peak is J, the scratch and one slab's float64 copies."""
+    import time
+    L = 2400
+    assert L * 20 * L * 20 > 2 ** 31
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    torch.cuda.reset_peak_memory_stats()
+    base = torch.cuda.memory_allocated()
+    jac = _random_jac(L, seed=L)
+    C = _poisoned_contacts(jac)
+    _gate(C, jac, "random past 2^31 elements", rows=64)
+    torch.cuda.synchronize()
+    peak = (torch.cuda.max_memory_allocated() - base) / 1e9
+    print(f"PARITY jacobian_contacts L={L}: J {jac.numel() / 1e9:.2f}e9 elements, peak {peak:.1f} GB, "
+          f"wall {time.perf_counter() - t0:.1f} s")
+    assert peak <= jac.numel() * 4 / 1e9 + 4
 
 
 def test_contact_kernel_all_zero_jacobian_is_nan_where_the_definition_is():

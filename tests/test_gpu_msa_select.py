@@ -3,13 +3,15 @@
   1. the rows of every case of tests/golden/msa_select.json (the reference notebook's greedy_select), both modes;
   2. the selection order against the numpy restatement (tests/msa_select_refs.py), bit for bit, up to 50,000 rows,
      columns that are not a multiple of 16 (padded on the device), one column, a row wider than 48 KiB and picks past
-     128, 256 and 512;
+     128, 256 and 512; past the step kernel's 256 partials and the init kernel's grid (N = 70,000 and 300,000) with
+     poisoned scratch, scratch reused by a second call, a count of 65,535 and k = N, through the C ABI;
   3. the tensor API under torch.cuda.set_sync_debug_mode("error");
   4. every argument refusal of the C ABI, before any launch;
   5. predict_cli and sample_msa_cli with --msa-select against the same commands on an a3m file that holds exactly the
      picked rows.
 """
 import ctypes
+import functools
 import json
 import os
 import sys
@@ -65,6 +67,117 @@ def test_the_selection_order_matches_the_restatement(N, C, k, symbols, mode):
     got = msa_select._order(torch.from_numpy(rows).cuda(), k, mode).tolist()
     assert got == want
     print(f"PARITY msa_select order N={N} C={C} k={k} {mode}: equal to the restatement", flush=True)
+
+
+# ---- 2b. past the grid caps, through the C ABI with poisoned scratch ------------------------------------------------
+def _select_abi(rows, C, k, mode, scratch=None):
+    """esmb200_msa_greedy_select on rows uint8 [N, ld] (contiguous on the GPU, ld a multiple of 16). The scratch, when
+    not given, is filled with 0xFF bytes first: every row then reads as picked and every table entry as NaN until the
+    init kernel rewrites it. Returns (the picks, the scratch)."""
+    from esm_b200 import _lib
+    lib = _lib.load()
+    N, ld = rows.shape
+    n = lib.esmb200_msa_select_scratch_bytes(N, C, k)
+    if scratch is None:
+        scratch = torch.full((n,), 0xFF, dtype=torch.uint8, device="cuda")
+    assert scratch.numel() >= n
+    sel = torch.full((k,), -1, dtype=torch.int64, device="cuda")
+    code = _lib.SELECT_MAX if mode == "max" else _lib.SELECT_MIN
+    _lib.check(lib.esmb200_msa_greedy_select(rows.data_ptr(), ld, N, C, k, code, sel.data_ptr(), scratch.data_ptr(),
+                                             scratch.numel(), torch.cuda.current_stream().cuda_stream))
+    return sel.tolist(), scratch
+
+
+FAR = (65536, 262144)  # the step kernel's 256 partials per last-block pass, and the init kernel's 1024 x 256 grid
+SCALE_C, SCALE_K = 48, 48
+
+
+@functools.lru_cache(maxsize=None)
+def _scale_case(N, mode):
+    """Random rows over four letters, and 8 planted rows in each of [65536, 262144) and [262144, N) that win the first
+    picks: in max mode rows over sixteen other letters (they differ from every other row in every column), in min
+    mode near-copies of the query (1 to 4 columns changed). Random rows tie often and ties go to the smallest index,
+    so without them the picks could all come from the first blocks. Returns (rows, the restatement's picks)."""
+    rows = _random_rows(N, SCALE_C, 4, seed=N + (mode == "min"))
+    g = np.random.default_rng(N + 7)
+    planted = np.concatenate([g.choice(np.arange(lo, min(hi, N)), 8, replace=False)
+                              for lo, hi in zip(FAR, FAR[1:] + (N,)) if lo < N])
+    other = np.frombuffer(b"FGHIKLMNPQRSTVWY", dtype=np.uint8)
+    for m, r in enumerate(planted):
+        if mode == "max":
+            rows[r] = other[g.integers(0, 16, SCALE_C)]
+        else:
+            rows[r] = rows[0]
+            cols = g.choice(SCALE_C, 1 + m % 4, replace=False)
+            rows[r, cols] = np.where(rows[0, cols] == ord("A"), ord("C"), ord("A"))
+    return rows, ref.greedy_order(rows, SCALE_K, mode)
+
+
+def _far_picks(want, N):
+    """The restatement's picks in [65536, 262144) and past 262144: each range that N reaches must hold some."""
+    far = [sum(FAR[0] <= i < FAR[1] for i in want), sum(i >= FAR[1] for i in want)]
+    assert far[0] > 0 and (N <= FAR[1] or far[1] > 0), want
+    return far
+
+
+@pytest.mark.parametrize("mode", ["max", "min"])
+@pytest.mark.parametrize("N", [70000, 300000])
+def test_the_selection_order_past_the_grid_caps(N, mode):
+    """N = 70,000 has 274 blocks, so the last block's loop over the partials runs twice; N = 300,000 also needs the
+    init kernel's grid-stride loop (1172 blocks of rows against its 1024)."""
+    rows, want = _scale_case(N, mode)
+    far = _far_picks(want, N)
+    got, _ = _select_abi(torch.from_numpy(rows).cuda(), SCALE_C, SCALE_K, mode)
+    print(f"PARITY msa_select order N={N} C={SCALE_C} k={SCALE_K} {mode}, poisoned scratch: "
+          f"{'equal to' if got == want else 'DIFFERENT from'} the restatement; picks past 65,536 / 262,144: "
+          f"{far[0]} / {far[1]}", flush=True)
+    assert got == want
+
+
+def test_scratch_reused_for_a_smaller_alignment_and_the_other_mode():
+    """The init kernel rewrites picked, the distance table and the ticket: a second call on the first call's scratch,
+    with fewer rows (so every array sits at another offset) and the other mode, picks the restatement's rows too."""
+    (big, want_big), (small, want_small) = _scale_case(300000, "max"), _scale_case(70000, "min")
+    got_big, scratch = _select_abi(torch.from_numpy(big).cuda(), SCALE_C, SCALE_K, "max")
+    got_small, _ = _select_abi(torch.from_numpy(small).cuda(), SCALE_C, SCALE_K, "min", scratch=scratch)
+    print(f"PARITY msa_select scratch reuse: N=300000 max then N=70000 min on one scratch, "
+          f"{'both equal' if (got_big, got_small) == (want_big, want_small) else 'NOT equal'} to the restatement",
+          flush=True)
+    assert got_big == want_big and got_small == want_small
+
+
+def test_the_count_at_its_maximum():
+    """C = 65,535 and a row that differs from the query in every column: its uint16 count is 65,535, its distance
+    exactly 1.0, so max mode picks it first."""
+    N, C, k, far = 200, 65535, 12, 137
+    rows = _random_rows(N, C, 4, seed=C)
+    rows[far] = ord("W")
+    ld = C + 1
+    dev = torch.zeros((N, ld), dtype=torch.uint8, device="cuda")
+    dev[:, :C] = torch.from_numpy(rows).cuda()
+    for mode in ("max", "min"):
+        got, scratch = _select_abi(dev, C, k, mode)
+        counts = scratch[:2 * N].view(torch.int16).cpu().numpy().view(np.uint16)  # counts[0, :]: against the query
+        assert counts[far] == 65535 and np.array_equal(counts, (rows != rows[0]).sum(1))
+        want = ref.greedy_order(rows, k, mode)
+        assert got == want
+        if mode == "max":
+            assert want[1] == far
+    print(f"PARITY msa_select C={C} N={N} k={k}: count {int(counts[far])} (d = 1.0) picked second in max mode; both "
+          f"modes equal to the restatement", flush=True)
+
+
+@pytest.mark.parametrize("mode", ["max", "min"])
+def test_k_equal_to_n_runs_to_a_single_candidate(mode):
+    """The C ABI at k = N: the last step has one unpicked row left. The Python API returns every row without a launch
+    there, so this compares with the restatement's loop run to k = N."""
+    N, C = 600, 32
+    rows = _random_rows(N, C, 3, seed=N + C)
+    got, _ = _select_abi(torch.from_numpy(rows).cuda(), C, N, mode)
+    want = ref.greedy_order(rows, N, mode, shortcut=False)
+    print(f"PARITY msa_select k=N={N} C={C} {mode}: {'equal to' if got == want else 'DIFFERENT from'} the "
+          f"restatement's loop without the N <= k shortcut", flush=True)
+    assert got == want and sorted(got) == list(range(N))
 
 
 # ---- 3. host synchronisation ---------------------------------------------------------------------------------------

@@ -6,7 +6,7 @@
      targeted token entries written, the block sums of log q;
   2. the order kernel on residue indices against the numpy restatement, bit for bit;
   3. a chi-square test of 200,000 draws of one row against softmax(z);
-  4. tiny ESM-2 and ESM-1b models in fp16 and fp32x3: fixed positions, amino acids only after sweep 0 of a de novo
+  4. tiny ESM-2 and ESM-1b models in fp16, fp32x3 and fp8: fixed positions, amino acids only after sweep 0 of a de novo
      start, reproducibility, chunking, log q against the public forward, the tokens against the oracle's draw;
   5. cpu_offload() bit-identical; no host synchronisation after the first step;
   6. the command line end to end.
@@ -167,7 +167,7 @@ def _de_novo(model, L):
     return torch.tensor([[model.cls_idx] + [model.mask_idx] * L + [model.eos_idx]], device="cuda")
 
 
-@pytest.mark.parametrize("precision", ["fp16", "fp32x3"])
+@pytest.mark.parametrize("precision", ["fp16", "fp32x3", "fp8"])
 @pytest.mark.parametrize("name", ["esm2_t2_tiny", "esm1b_t2_tiny"])
 def test_gibbs_on_a_tiny_model(fixtures, name, precision):
     from esm_b200 import sampling
@@ -206,7 +206,7 @@ def test_gibbs_on_a_tiny_model(fixtures, name, precision):
         model.set_precision("fp16")
 
 
-@pytest.mark.parametrize("precision", ["fp16", "fp32x3"])
+@pytest.mark.parametrize("precision", ["fp16", "fp32x3", "fp8"])
 @pytest.mark.parametrize("name", ["esm2_t2_tiny", "esm1b_t2_tiny"])
 def test_one_step_against_the_public_forward_and_the_oracle(fixtures, name, precision):
     """block = |D|, one sweep: one step. Its logp equals log_softmax(model(x_masked)["logits"][rows][:, AA] / tau) at

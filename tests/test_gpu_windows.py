@@ -1,7 +1,8 @@
 """GPU (-m gpu): overlapping windows for long proteins (esm_b200.windows, ProteinLanguageModel.forward_windowed, the
 windowed variant scorers and the --window flag of both command lines).
 
-  * esmb200_window_merge against a float64 restatement; bit-reproducible; one-term rows copied bit for bit;
+  * esmb200_window_merge against a float64 restatement, past its launch's grid cap, into a poisoned output wider
+    than C; bit-reproducible; one-term rows copied bit for bit;
   * proteins within the window: forward_windowed and the three scorers bit-identical to the unwindowed path;
   * longer proteins (an ESM-1b-shaped model with 64 learned positions, and ESM-2): every merged row against a float64
     merge of what forward gives on each window alone; bit-identical for any max_tokens;
@@ -67,22 +68,26 @@ def protein(n, seed):
 
 # ---- the kernel -------------------------------------------------------------------------------------------------
 def merge_f64(src, idx, w, seg):
+    """The float64 merge and the sum of its terms' magnitudes, [rows, C] each: every term w[j] * src[idx[j]] added into
+    its row r (seg[r] <= j < seg[r + 1]) by index_add_."""
     s, i, ww, sg = src.double().cpu(), idx.cpu(), w.double().cpu(), seg.cpu()
     rows = sg.numel() - 1
-    out = torch.zeros((rows, s.shape[1]), dtype=torch.float64)
-    mag = torch.zeros_like(out)
-    for r in range(rows):
-        for j in range(int(sg[r]), int(sg[r + 1])):
-            out[r] += ww[j] * s[i[j]]
-            mag[r] += (ww[j] * s[i[j]]).abs()
+    row_of = torch.repeat_interleave(torch.arange(rows), sg.diff())
+    terms = ww[:, None] * s[i]
+    out = torch.zeros((rows, s.shape[1]), dtype=torch.float64).index_add_(0, row_of, terms)
+    mag = torch.zeros_like(out).index_add_(0, row_of, terms.abs_())
     return out, mag
 
 
-@pytest.mark.parametrize("C", [1, 33, 64, 1280])
-def test_merge_matches_float64_and_copies_single_terms(C):
-    from esm_b200 import windows
+POISON = 0x7FA5A5A5  # a NaN no fp32 operation produces: it marks output elements the kernel must not touch or skipped
+
+
+# 5120 x 3500: 17.9 M elements, past the launch's 65,536 blocks of 256 threads, so the grid-stride loop runs (a 15B
+# representation merged over a protein of about 3,300 residues)
+@pytest.mark.parametrize("C,rows", [(1, 400), (33, 400), (64, 400), (1280, 120), (5120, 3500)])
+def test_merge_matches_float64_and_copies_single_terms(C, rows):
+    from esm_b200 import _lib, windows
     g = torch.Generator().manual_seed(C)
-    rows = 400 if C < 1280 else 120
     R = 3 * rows
     ld = C + 7                                                                 # a row stride wider than C
     buf = torch.randn((R, ld), generator=g) * 10
@@ -104,6 +109,17 @@ def test_merge_matches_float64_and_copies_single_terms(C):
     again = windows.merge_rows(src, idx, w, seg)
     assert got.shape == (rows, C)
     assert torch.equal(got.view(torch.int32), again.view(torch.int32))        # bit-reproducible
+    # through the C ABI into a poisoned output 5 columns wider than C: every element written, no padding column touched
+    out_ld = C + 5
+    poisoned = torch.full((rows, out_ld), POISON, dtype=torch.int32, device="cuda").view(torch.float32)
+    dev = lambda t, dt: t.to("cuda", dt).contiguous()  # noqa: E731
+    idx_d, w_d, seg_d = dev(idx, torch.int64), dev(w, torch.float32), dev(seg, torch.int64)
+    _lib.check(_lib.load().esmb200_window_merge(src.data_ptr(), ld, idx_d.data_ptr(), w_d.data_ptr(), seg_d.data_ptr(),
+                                                rows, C, poisoned.data_ptr(), out_ld,
+                                                torch.cuda.current_stream().cuda_stream))
+    bits = poisoned.view(torch.int32)
+    assert bool((bits[:, C:] == POISON).all()), "a padding column was written"
+    assert torch.equal(bits[:, :C], got.view(torch.int32)), "an element was not written, or differs between calls"
     s = src.cpu()
     copied = got.cpu()[single]
     assert torch.equal(copied.view(torch.int32), s[srows].contiguous().view(torch.int32))
@@ -116,7 +132,9 @@ def test_merge_matches_float64_and_copies_single_terms(C):
     err = (g64 - want)[fin].abs()
     bound = 6 * U * mag[fin] + 1e-30
     assert bool((err <= bound).all()), float((err / bound).max())
-    print(f"PARITY window_merge C={C}: max err/bound {float((err / bound).max()):.3f} (bound 6u sum|w x|)")
+    print(f"PARITY window_merge C={C} rows={rows} ({rows * C / 1e6:.2f} M elements): max err/bound "
+          f"{float((err / bound).max()):.3f} (bound 6u sum|w x|); poisoned output with out_ld = C + 5: every element "
+          f"written, no padding column touched")
 
 
 def test_merge_argument_checks():

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 if HERE not in sys.path:
     sys.path.insert(0, HERE)  # jacobian_refs
 
-from jacobian_refs import contacts_brute_force, contacts_f64  # noqa: E402
+from jacobian_refs import contacts_brute_force, contacts_f64, contacts_f64_chunked  # noqa: E402
 
 ROOT = os.path.dirname(HERE)
 
@@ -28,6 +28,27 @@ def test_definition_matches_brute_force(L):
     assert got.shape == (L, L)
     assert torch.allclose(got, want, rtol=1e-12, atol=1e-12 * float(want.abs().max()))
     assert torch.equal(got, got.T) and bool((got.diagonal() == 0).all())
+
+
+@pytest.mark.parametrize("L", [2, 5, 17])
+def test_chunked_reference_matches_the_definition(L):
+    """contacts_f64_chunked, which the GPU test past 2^31 elements gates against, equals contacts_f64 for any slab size,
+    with a large term constant along each axis in turn; its max N and max|J| are those of the whole J."""
+    g = torch.Generator().manual_seed(50 + L)
+    jac = torch.randn((L, 20, L, 20), generator=g) * 8
+    for shape in ([1, 1, L, 20], [1, 20, L, 20], [L, 1, L, 20], [L, 20, 1, 20], [L, 20, L, 1]):
+        jac += torch.randn(shape, generator=g) * 800
+    want = contacts_f64(jac)
+    jc = jac.double()
+    for axis in range(4):
+        jc = jc - jc.mean(axis, keepdim=True)
+    nmax = float(jc.pow(2).sum((1, 3)).sqrt().max())
+    for rows in (1, 8, L):
+        got, n, j = contacts_f64_chunked(jac, rows)
+        assert got.dtype == torch.float64 and got.shape == (L, L)
+        assert float((got - want).abs().max()) <= 1e-12 * float(want.abs().max()), rows
+        assert abs(n - nmax) <= 1e-12 * nmax and j == float(jac.abs().max())
+        assert torch.equal(got, got.T) and bool((got.diagonal() == 0).all())
 
 
 def test_definition_of_an_all_zero_jacobian_is_nan_off_the_diagonal():

@@ -35,6 +35,20 @@ def test_the_restatement_picks_the_notebook_rows(i):
     assert sorted(order) == selected
 
 
+@pytest.mark.parametrize("mode", ["max", "min"])
+def test_the_loop_without_the_shortcut_runs_to_k_equal_n(mode):
+    """shortcut=False at k = N picks every row once, starting at the query, and its first k' picks are the picks at
+    k' < N: the last step, with one candidate left, takes it."""
+    rows = np.random.default_rng(4).integers(0, 3, (140, 9)).astype(np.uint8)
+    order = ref.greedy_order(rows, 140, mode, shortcut=False)
+    assert ref.greedy_order(rows, 140, mode) == list(range(140))
+    assert order[0] == 0 and sorted(order) == list(range(140))
+    for k in (1, 2, 9, 130, 139):
+        assert order[:k] == ref.greedy_order(rows, k, mode)
+    with pytest.raises(AssertionError):
+        ref.greedy_order(rows, 141, mode, shortcut=False)
+
+
 def test_a_running_sum_is_not_the_rule():
     """On at least one fixture case past 8 picks, a running mean in selection order picks other rows."""
     def running(rows, k, mode):
