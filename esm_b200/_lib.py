@@ -72,6 +72,8 @@ EXPORTS = (
     "esmb200_sample_rows",
     "esmb200_msa_select_scratch_bytes",
     "esmb200_msa_greedy_select",
+    "esmb200_knn_scratch_bytes",
+    "esmb200_knn_search",
 )
 
 ABI_VERSION = 4
@@ -186,6 +188,12 @@ def _declare(lib):
     lib.esmb200_msa_greedy_select.restype = c_int32
     lib.esmb200_msa_greedy_select.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_void_p,
                                               c_void_p, c_size_t, c_void_p]
+    lib.esmb200_knn_scratch_bytes.restype = c_int32
+    lib.esmb200_knn_scratch_bytes.argtypes = [c_int32, c_int32, c_int32, POINTER(c_size_t)]
+    lib.esmb200_knn_search.restype = c_int32
+    lib.esmb200_knn_search.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_int32, c_void_p,
+                                       c_float, c_int64, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p,
+                                       c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

@@ -26,6 +26,7 @@
 #include "gemm2.cuh"
 #include "gemm_fp8.cuh"
 #include "jacobian.cuh"
+#include "knn.cuh"
 #include "msa_select.cuh"
 #include "sampling.cuh"
 #include "tied_attention.cuh"
@@ -57,7 +58,7 @@ int fail_cuda(cudaError_t e, const char* what) {
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
                      T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
-                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_MSA_SELECT, T_COUNT };
+                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_MSA_SELECT, T_KNN, T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1750,6 +1751,67 @@ int esmb200_msa_greedy_select(const uint8_t* rows, int64_t ld, int32_t N, int32_
       msa_select_step_kernel<true><<<blocks, kSelThreads, smem, st>>>(rows, ld, N, t, selected, s);
     else
       msa_select_step_kernel<false><<<blocks, kSelThreads, smem, st>>>(rows, ld, N, t, selected, s);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+
+int esmb200_knn_scratch_bytes(int32_t Q, int32_t k, int32_t splits, size_t* out) {
+  if (!out) return fail(ESMB200_EINVAL, "null argument");
+  if (Q < 0 || k < 1 || k > knn_cfg::MAX_K || splits < 1 || splits > knn_cfg::MAX_SPLITS)
+    return fail(ESMB200_EINVAL, "knn_scratch_bytes needs Q >= 0, 1 <= k <= 128 and 1 <= splits <= 1024");
+  *out = (size_t)splits * (size_t)Q * (size_t)k * 8;
+  return ESMB200_OK;
+}
+
+int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld, int64_t N,
+                       int32_t D, const float* beta, float alpha, int64_t self_offset, int32_t k, int32_t splits,
+                       void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream) {
+  if (k < 1 || k > knn_cfg::MAX_K) return fail(ESMB200_EINVAL, "knn_search needs 1 <= k <= 128");
+  if (Q < 0 || N < 1 || N > INT32_MAX) return fail(ESMB200_EINVAL, "knn_search needs Q >= 0 and 1 <= N < 2^31");
+  if (k > (self_offset >= 0 ? N - 1 : N))
+    return fail(ESMB200_EINVAL, "knn_search needs k <= N candidates (N - 1 with self_offset >= 0)");
+  if (D < 64 || D % 64 != 0) return fail(ESMB200_EINVAL, "knn_search needs D % 64 == 0");
+  if (q_ld < D || b_ld < D || q_ld % 8 != 0 || b_ld % 8 != 0)
+    return fail(ESMB200_EINVAL, "knn_search needs q_ld, b_ld >= D and multiples of 8 (16-byte rows for TMA)");
+  if (splits < 1 || splits > knn_cfg::MAX_SPLITS) return fail(ESMB200_EINVAL, "knn_search needs 1 <= splits <= 1024");
+  if (!queries || !base || !scratch || !out_scores || !out_idx) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(queries) % 16 != 0 || reinterpret_cast<uintptr_t>(base) % 16 != 0)
+    return fail(ESMB200_EINVAL, "knn_search needs 16-byte aligned queries and base (TMA)");
+  if (reinterpret_cast<uintptr_t>(scratch) % 16 != 0) return fail(ESMB200_EINVAL, "scratch must be 16-byte aligned");
+  if (scratch_bytes < (size_t)splits * (size_t)Q * (size_t)k * 8)
+    return fail(ESMB200_EINVAL, "scratch smaller than esmb200_knn_scratch_bytes");
+  if (Q == 0) return ESMB200_OK;
+  int rc = check_device();
+  if (rc) return rc;
+  CUtensorMap tq, tx;
+  if ((rc = make_tmap_f16(&tq, queries, (uint64_t)Q, (uint64_t)D, (uint64_t)q_ld, knn_cfg::BLOCK_M))) return rc;
+  if ((rc = make_tmap_f16(&tx, base, (uint64_t)N, (uint64_t)D, (uint64_t)b_ld, knn_cfg::BLOCK_N))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KnnParams p;
+  p.Q = Q;
+  p.D = D;
+  p.k = k;
+  p.N = N;
+  const int64_t tiles = (N + knn_cfg::BLOCK_N - 1) / knn_cfg::BLOCK_N;
+  p.tiles_per_stripe = (int)((tiles + splits - 1) / splits);
+  p.query_blocks = (Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  p.beta = beta;
+  p.alpha = alpha;
+  p.self_offset = self_offset;
+  p.keys = static_cast<unsigned long long*>(scratch);
+  CK(cudaFuncSetAttribute(knn_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, knn_cfg::SMEM_BYTES));
+  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
+    ProfScope ps(T_KNN, st);
+    const int64_t grid = (int64_t)p.query_blocks * splits;
+    knn_topk_kernel<<<(unsigned)grid, knn_cfg::NUM_THREADS, knn_cfg::SMEM_BYTES, st>>>(tq, tx, p);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_KNN, st);
+    const int threads = splits >= 256 ? 256 : (splits + 31) / 32 * 32;
+    knn_merge_kernel<<<(unsigned)Q, threads, 0, st>>>(p.keys, Q, k, splits, out_scores, out_idx);
     CK(cudaGetLastError());
   }
   return ESMB200_OK;

@@ -1,0 +1,387 @@
+// esm_b200 — exact k-nearest-neighbour search over embeddings (esm_b200/search.py): a wgmma similarity GEMM whose
+// epilogue keeps each query's top k, so the [Q, N] score matrix never reaches HBM.  Definition in include/esmb200.h at
+// esmb200_knn_search.
+//
+//   s(i, j) = alpha * (A_i . X_j) + beta_j   (fp16 operands, fp32 accumulation), j in [0, N), j != i + self_offset
+//
+// Ranking key.  A candidate is the 64-bit key (ord(s) << 32) | (2^32 - 1 - j), ord the order-preserving map of fp32
+// bits to uint32.  Keys are distinct for distinct j and order candidates by (score descending, index ascending), so the
+// top k of a set of keys is one well-defined set whatever order the candidates arrive in.  Key 0 is below every finite
+// score and marks an empty slot.
+//
+// knn_topk_kernel: one CTA per (64-query block, database stripe); blockIdx.x = stripe * query_blocks + block, so the
+// CTAs resident at one time share a stripe and read its tiles from the L2.
+//   * warpgroup 0: one thread streams 64-wide K slabs of the query block (64 rows, 8 KB) and of a 256-row database
+//     tile (32 KB) through a 3-stage TMA ring (128B swizzle); TMA zero-fills rows >= Q and >= N;
+//   * warpgroup 1: wgmma m64n256k16 into 128 fp32 accumulators per thread, then the epilogue: s = alpha acc + beta_j
+//     in registers, key > the row's k-th best key (a warpgroup-wide OR first, so a tile without a survivor costs one
+//     barrier); survivors go to the row's 64-entry queue in shared memory, 32 columns at a time; when a row's queue
+//     could overflow with the next 32, every row's queue is sorted (warp bitonic sort) and merged into its k-list by
+//     rank.  Rows >= Q, columns >= N and j == i + self_offset never produce a candidate.  The threshold only rises,
+//     and queued candidates are never lost, so the list is the exact top k of the stripe.
+//   * the k-list of each valid row is written to scratch keys[stripe, q, 0..k) (descending, 0 past the stripe's
+//     candidates).
+// knn_merge_kernel: one block per query merges the S stripe lists (k rounds of a block-wide maximum over the list
+// heads) and decodes the keys to fp32 scores and int64 indices.
+//
+// Shared memory of knn_topk_kernel (k <= 128): ring 3 x (8 + 32) KB = 120 KB, k-lists 64 x 128 x 8 B = 64 KB, queues
+// 64 x 64 x 8 B = 32 KB, thresholds 512 B, queue counts 256 B, barriers, 1 KB alignment slack: 223,232 B of 232,448.
+// 64 query rows per CTA: 128 rows would need 128 KB of k-lists at k = 128, leaving no room for a 3-stage ring.
+#pragma once
+
+#include "common.cuh"
+
+namespace esmb200 {
+
+namespace knn_cfg {
+constexpr int BLOCK_M = 64;    // query rows per CTA
+constexpr int BLOCK_N = 256;   // database rows per tile
+constexpr int BLOCK_K = 64;
+constexpr int STAGES = 3;
+constexpr int MAX_K = 128;
+constexpr int QCAP = 64;       // queue entries per row
+constexpr int CHUNK = 32;      // columns pushed between overflow checks
+constexpr int MAX_SPLITS = 1024;
+constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 8 KB
+constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KB
+constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+constexpr int LIST_BYTES = BLOCK_M * MAX_K * 8;
+constexpr int QUEUE_BYTES = BLOCK_M * QCAP * 8;
+constexpr int NUM_THREADS = 256;  // warpgroup 0: TMA producer, warpgroup 1: MMA + top-k epilogue
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + LIST_BYTES + QUEUE_BYTES + BLOCK_M * 8 + BLOCK_M * 4 + 256 + 1024;
+static_assert(SMEM_BYTES <= 232448, "knn_topk_kernel shared memory");
+}  // namespace knn_cfg
+
+struct KnnParams {
+  int Q, D, k;
+  int64_t N;
+  int tiles_per_stripe;  // 256-row tiles per stripe
+  int query_blocks;
+  const float* beta;     // [N] or nullptr
+  float alpha;
+  int64_t self_offset;   // < 0: none
+  unsigned long long* keys;  // scratch [splits, Q, k]
+};
+
+__device__ __forceinline__ unsigned long long knn_key(float s, int64_t j) {
+  const uint32_t u = __float_as_uint(s);
+  const uint32_t o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)o << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)j);
+}
+
+// warpgroup-wide OR (bar.red on a named barrier: also a barrier with bar.sync's memory ordering)
+__device__ __forceinline__ bool knn_bar_or(uint32_t id, bool v) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.or.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(r)
+      : "r"((uint32_t)v), "r"(id)
+      : "memory");
+  return r != 0;
+}
+
+// Merge one row's queue (cnt > 0 entries) into its k-list; one warp, called with a warp-uniform row.
+__device__ __forceinline__ void knn_merge_row(unsigned long long* list, unsigned long long* queue, int* cnt,
+                                              unsigned long long* th, int k, uint32_t lane) {
+  const int n = *cnt < knn_cfg::QCAP ? *cnt : knn_cfg::QCAP;
+  unsigned long long v[2];
+#pragma unroll
+  for (int sl = 0; sl < 2; ++sl) v[sl] = (int)(32 * sl + lane) < n ? queue[32 * sl + lane] : 0ull;
+  // bitonic sort of the 64 keys, descending; element x = 32 slot + lane
+#pragma unroll
+  for (int size = 2; size <= 64; size <<= 1) {
+#pragma unroll
+    for (int d = size / 2; d > 0; d >>= 1) {
+      if (d == 32) {  // size == 64: the two slots of one lane
+        const unsigned long long hi = v[0] > v[1] ? v[0] : v[1], lo = v[0] > v[1] ? v[1] : v[0];
+        v[0] = hi;
+        v[1] = lo;
+      } else {
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+          const uint32_t x = 32 * sl + lane;
+          const unsigned long long p = __shfl_xor_sync(0xffffffffu, v[sl], d);
+          const bool want_max = ((x & d) == 0) == ((x & size) == 0);
+          v[sl] = want_max ? (v[sl] > p ? v[sl] : p) : (v[sl] < p ? v[sl] : p);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int sl = 0; sl < 2; ++sl) queue[32 * sl + lane] = v[sl];
+  __syncwarp();
+  // merge by rank: a list entry goes to i + #(queue > it), a queue entry to j + #(list >= it); ranks < k are kept
+  unsigned long long lv[knn_cfg::MAX_K / 32];
+  int lr[knn_cfg::MAX_K / 32], qr[2];
+#pragma unroll
+  for (int t = 0; t < knn_cfg::MAX_K / 32; ++t) {
+    const int i = 32 * t + (int)lane;
+    lr[t] = knn_cfg::MAX_K;
+    if (i < k) {
+      const unsigned long long x = list[i];
+      int lo = 0, hi = knn_cfg::QCAP;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (queue[mid] > x) lo = mid + 1; else hi = mid;
+      }
+      lv[t] = x;
+      lr[t] = i + lo;
+    }
+  }
+#pragma unroll
+  for (int sl = 0; sl < 2; ++sl) {
+    int lo = 0, hi = k;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (list[mid] >= v[sl]) lo = mid + 1; else hi = mid;
+    }
+    qr[sl] = 32 * sl + (int)lane + lo;
+  }
+  __syncwarp();
+#pragma unroll
+  for (int t = 0; t < knn_cfg::MAX_K / 32; ++t)
+    if (lr[t] < k) list[lr[t]] = lv[t];
+#pragma unroll
+  for (int sl = 0; sl < 2; ++sl)
+    if (qr[sl] < k) list[qr[sl]] = v[sl];
+  __syncwarp();
+  if (lane == 0) {
+    *th = list[k - 1];
+    *cnt = 0;
+  }
+  __syncwarp();
+}
+
+__global__ void __launch_bounds__(knn_cfg::NUM_THREADS, 1)
+knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                const KnnParams p) {
+  using namespace knn_cfg;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
+  unsigned long long* s_list = reinterpret_cast<unsigned long long*>(smem + STAGES * STAGE_BYTES);  // [64][k]
+  unsigned long long* s_queue = s_list + BLOCK_M * MAX_K;                                           // [64][QCAP]
+  unsigned long long* s_th = s_queue + BLOCK_M * QCAP;                                              // [64]
+  int* s_cnt = reinterpret_cast<int*>(s_th + BLOCK_M);                                              // [64]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_cnt + BLOCK_M);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + STAGES;
+
+  const int k = p.k;
+  const int qb = blockIdx.x % p.query_blocks, stripe = blockIdx.x / p.query_blocks;
+  const int q0 = qb * BLOCK_M;
+  const int tiles = (int)((p.N + BLOCK_N - 1) / BLOCK_N);
+  const int t_begin = stripe * p.tiles_per_stripe;
+  const int t_end = min(tiles, t_begin + p.tiles_per_stripe);
+  const int num_kb = p.D / BLOCK_K;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_q);
+    tma_prefetch_desc(&tmap_x);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 1);
+    }
+    fence_barrier_init();
+  }
+  for (int i = threadIdx.x; i < BLOCK_M * MAX_K; i += NUM_THREADS) s_list[i] = 0ull;
+  for (int i = threadIdx.x; i < BLOCK_M; i += NUM_THREADS) {
+    s_th[i] = 0ull;
+    s_cnt[i] = 0;
+  }
+  __syncthreads();
+
+  const uint32_t wg = __shfl_sync(0xffffffffu, threadIdx.x / 128, 0);
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    if (threadIdx.x == 0) {
+      uint32_t it = 0;
+      for (int t = t_begin; t < t_end; ++t) {
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const uint32_t s = it % STAGES;
+          while (!mbar_try_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1)) __nanosleep(64);
+          mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
+          tma_load_2d(smem_a + s * A_STAGE_BYTES, &tmap_q, &full_bar[s], kb * BLOCK_K, q0);
+          tma_load_2d(smem_b + s * B_STAGE_BYTES, &tmap_x, &full_bar[s], kb * BLOCK_K, t * BLOCK_N);
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== MMA + top-k warpgroup =====================
+  const uint32_t warp = (threadIdx.x / 32) % 4;  // rows [16 warp, +16) of the block
+  const uint32_t lane = threadIdx.x % 32;
+  const uint32_t g = lane / 4, c = lane % 4;
+  const bool signal = (threadIdx.x % 128) == 0;
+  const uint32_t a_base = smem_u32(smem_a);
+  const uint32_t b_base = smem_u32(smem_b);
+  uint32_t it = 0;
+  float acc[128];
+
+  int rl[2];           // the thread's rows of the block
+  bool rvalid[2];
+  int64_t excl[2];     // the excluded column of each row (-1: none)
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    rl[hr] = (int)(warp * 16 + g + 8 * hr);
+    const int q = q0 + rl[hr];
+    rvalid[hr] = q < p.Q;
+    excl[hr] = p.self_offset >= 0 ? (int64_t)q + p.self_offset : -1;
+  }
+
+  // every row's queue into its list: warp w takes rows 16 w .. 16 w + 15
+  auto merge_all = [&]() {
+    for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r)
+      if (s_cnt[r] > 0) knn_merge_row(s_list + r * MAX_K, s_queue + r * QCAP, s_cnt + r, s_th + r, k, lane);
+  };
+
+  for (int t = t_begin; t < t_end; ++t) {
+    const int64_t n0 = (int64_t)t * BLOCK_N;
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const uint32_t s = it % STAGES;
+      // plain try_wait loop: any call in a wgmma kernel makes ptxas serialise every wgmma (C7510)
+      while (!mbar_try_wait(&full_bar[s], (it / STAGES) & 1)) {
+      }
+      wgmma_fence();
+      const uint64_t da = wgmma_desc_sw128(a_base + s * A_STAGE_BYTES);
+      const uint64_t db = wgmma_desc_sw128(b_base + s * B_STAGE_BYTES);
+#pragma unroll
+      for (int kk = 0; kk < BLOCK_K / 16; ++kk) wgmma_m64n256k16(acc, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (kb > 0 && signal) mbar_arrive(&empty_bar[(it + STAGES - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    reg_fence_f(acc);
+    if (signal) mbar_arrive(&empty_bar[(it + STAGES - 1) % STAGES]);
+
+    // ---- epilogue: acc[4 i + 2 hr + e] is row rl[hr], column n0 + 8 i + 2 c + e.  Thresholds change only in merges,
+    // which are bracketed by warpgroup barriers, so each pass reads them fresh.
+    // s + 0: a score of -0 becomes +0, so equal scores have equal keys
+    bool any = false;
+    {
+      const unsigned long long th0 = s_th[rl[0]], th1 = s_th[rl[1]];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int64_t j = n0 + 8 * i + 2 * (int)c + e;
+          const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
+          const bool in = j < p.N;
+          any |= in && rvalid[0] && j != excl[0] && knn_key(fmaf(p.alpha, acc[4 * i + e], b) + 0.0f, j) > th0;
+          any |= in && rvalid[1] && j != excl[1] && knn_key(fmaf(p.alpha, acc[4 * i + 2 + e], b) + 0.0f, j) > th1;
+        }
+      }
+    }
+    if (!knn_bar_or(1, any)) continue;
+#pragma unroll
+    for (int ch = 0; ch < BLOCK_N / CHUNK; ++ch) {
+      const unsigned long long th0 = s_th[rl[0]], th1 = s_th[rl[1]];
+      bool full = false;
+#pragma unroll
+      for (int ii = 0; ii < CHUNK / 8; ++ii) {
+        const int i = ch * (CHUNK / 8) + ii;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int64_t j = n0 + 8 * i + 2 * (int)c + e;
+          const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const unsigned long long key = knn_key(fmaf(p.alpha, acc[4 * i + 2 * hr + e], b) + 0.0f, j);
+            if (j < p.N && rvalid[hr] && j != excl[hr] && key > (hr ? th1 : th0)) {
+              const int pos = atomicAdd(s_cnt + rl[hr], 1);  // < QCAP: at most QCAP - CHUNK queued before a chunk
+              s_queue[rl[hr] * QCAP + pos] = key;
+              full |= pos >= QCAP - CHUNK;
+            }
+          }
+        }
+      }
+      if (knn_bar_or(1, full)) {
+        merge_all();
+        named_bar_sync(1, 128);
+      }
+    }
+  }
+  named_bar_sync(1, 128);
+  merge_all();
+  __syncwarp();
+  // ---- the stripe's lists: warp w writes rows 16 w ..
+  for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r) {
+    const int q = q0 + r;
+    if (q >= p.Q) break;
+    unsigned long long* dst = p.keys + ((size_t)stripe * p.Q + q) * k;
+    for (int i = (int)lane; i < k; i += 32) dst[i] = s_list[r * MAX_K + i];
+  }
+}
+
+// One block per query: k rounds, each taking the largest head of the S stripe lists (keys are distinct, so the
+// winner is unique) and advancing that list.  Thread t owns stripes t, t + blockDim, ... (at most 4).
+__global__ void __launch_bounds__(256)
+knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int S, float* __restrict__ out_scores,
+                 int64_t* __restrict__ out_idx) {
+  __shared__ unsigned long long red_key[2][8];
+  __shared__ int red_s[2][8];
+  const int q = blockIdx.x;
+  const int nt = blockDim.x, warp = threadIdx.x / 32, nw = nt / 32;
+  unsigned long long head[4];
+  int pos[4];
+#pragma unroll
+  for (int m = 0; m < 4; ++m) {
+    const int s = threadIdx.x + m * nt;
+    pos[m] = 0;
+    head[m] = s < S ? keys[((size_t)s * Q + q) * k] : 0ull;
+  }
+  for (int r = 0; r < k; ++r) {
+    unsigned long long best = 0ull;
+    int bs = -1;
+#pragma unroll
+    for (int m = 0; m < 4; ++m)
+      if (head[m] > best || bs < 0) {
+        best = head[m];
+        bs = threadIdx.x + m * nt;
+      }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long b2 = __shfl_xor_sync(0xffffffffu, best, o);
+      const int s2 = __shfl_xor_sync(0xffffffffu, bs, o);
+      if (b2 > best || (b2 == best && s2 < bs)) {
+        best = b2;
+        bs = s2;
+      }
+    }
+    if (threadIdx.x % 32 == 0) {
+      red_key[r & 1][warp] = best;
+      red_s[r & 1][warp] = bs;
+    }
+    __syncthreads();
+    best = red_key[r & 1][0];
+    bs = red_s[r & 1][0];
+    for (int w = 1; w < nw; ++w) {
+      const unsigned long long b2 = red_key[r & 1][w];
+      const int s2 = red_s[r & 1][w];
+      if (b2 > best || (b2 == best && s2 < bs)) {
+        best = b2;
+        bs = s2;
+      }
+    }
+#pragma unroll
+    for (int m = 0; m < 4; ++m)
+      if (bs == (int)threadIdx.x + m * nt && bs < S) {
+        ++pos[m];
+        head[m] = pos[m] < k ? keys[((size_t)bs * Q + q) * k + pos[m]] : 0ull;
+      }
+    if (threadIdx.x == 0) {
+      const uint32_t o = (uint32_t)(best >> 32);
+      const uint32_t u = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
+      out_scores[(size_t)q * k + r] = __uint_as_float(u);
+      out_idx[(size_t)q * k + r] = (int64_t)(0xFFFFFFFFu - (uint32_t)(best & 0xFFFFFFFFull));
+    }
+  }
+}
+
+}  // namespace esmb200

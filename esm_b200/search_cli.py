@@ -1,0 +1,86 @@
+"""Nearest-neighbour search over extract_cli embeddings (esm_b200.search):
+
+    python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out db.pt
+    python -m esm_b200.search_cli query db.pt (--queries EXTRACT_DIR | --all) --k 10 --out hits.tsv
+
+`build` reads the mean representation at --layer of every `<label>.pt` under EXTRACT_DIR (extract_cli --include mean)
+and saves an index. `query` searches it with the mean representations of a second extract_cli directory, which must
+hold the index's layer at the index's width, or with every indexed protein against the others (--all). hits.tsv has
+one line per hit: query, rank (1-based), target, score (cosine similarity, or Euclidean distance for l2).
+Embedding the queries stays in extract_cli, with its model loading and checkpoint checks.
+"""
+from __future__ import annotations
+
+import argparse
+import pathlib
+import sys
+
+import torch
+
+from . import search
+
+
+def create_parser():
+    p = argparse.ArgumentParser(description="Exact k-nearest-neighbour search over extract_cli embeddings")
+    sub = p.add_subparsers(dest="command", required=True)
+    b = sub.add_parser("build", help="build an index from an extract_cli output directory")
+    b.add_argument("extract_dir", type=pathlib.Path)
+    b.add_argument("--layer", type=int, required=True, help="the representation layer to index")
+    b.add_argument("--metric", choices=list(search.METRICS), default="cosine")
+    b.add_argument("--out", type=pathlib.Path, required=True)
+    q = sub.add_parser("query", help="search an index")
+    q.add_argument("index", type=pathlib.Path)
+    src = q.add_mutually_exclusive_group(required=True)
+    src.add_argument("--queries", type=pathlib.Path, help="an extract_cli output directory of query proteins")
+    src.add_argument("--all", action="store_true", help="every indexed protein against the others")
+    q.add_argument("--k", type=int, default=10, help=f"hits per query, 1 to {search.MAX_K}")
+    q.add_argument("--out", type=pathlib.Path, required=True)
+    return p
+
+
+def write_hits(path, query_labels, target_labels, scores: torch.Tensor, idx: torch.Tensor) -> int:
+    """hits.tsv; returns the number of hit lines."""
+    scores, idx = scores.cpu().tolist(), idx.cpu().tolist()
+    n = 0
+    with open(path, "w") as f:
+        f.write("query\trank\ttarget\tscore\n")
+        for q, row_s, row_i in zip(query_labels, scores, idx):
+            for r, (s, i) in enumerate(zip(row_s, row_i)):
+                f.write(f"{q}\t{r + 1}\t{target_labels[i]}\t{s:.6g}\n")
+                n += 1
+    return n
+
+
+def run(args) -> int:
+    """Returns the number of rows indexed (build) or hit lines written (query)."""
+    if args.command == "build":
+        index = search.EmbeddingIndex.from_extract_dir(args.extract_dir, args.layer, args.metric)
+        args.out.parent.mkdir(parents=True, exist_ok=True)
+        index.save(args.out)
+        return len(index)
+    index = search.EmbeddingIndex.load(args.index, device="cpu")
+    candidates = len(index) - 1 if args.all else len(index)
+    index._check_k(args.k, candidates)
+    if args.all:
+        qlabels, queries = index.labels, None
+    else:
+        if index.layer is None:
+            raise ValueError(f"{args.index} records no layer: query it through esm_b200.search")
+        qlabels, queries = search._read_extract_dir(args.queries, index.layer)
+        if queries.shape[1] != index.dim:
+            raise ValueError(f"the queries have width {queries.shape[1]}, the index {index.dim}")
+        search.prepare_rows(queries, index.metric, "queries")
+    index = index.to(torch.device("cuda", torch.cuda.current_device()))
+    scores, idx = index.search_all(args.k) if args.all else index.search(queries, args.k)
+    args.out.parent.mkdir(parents=True, exist_ok=True)
+    return write_hits(args.out, qlabels, index.labels, scores, idx)
+
+
+def main():
+    args = create_parser().parse_args()
+    n = run(args)
+    print(f"indexed {n} rows" if args.command == "build" else f"wrote {n} hits to {args.out}", file=sys.stderr)
+
+
+if __name__ == "__main__":
+    main()

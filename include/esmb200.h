@@ -321,6 +321,27 @@ size_t esmb200_msa_select_scratch_bytes(int32_t N, int32_t C, int32_t k);
 int esmb200_msa_greedy_select(const uint8_t* rows, int64_t ld, int32_t N, int32_t C, int32_t k, int32_t mode,
                               int64_t* selected, void* scratch, size_t scratch_bytes, void* stream);
 
+/* Exact k-nearest-neighbour search over embeddings (esm_b200/search.py). queries fp16 [Q, q_ld] and base fp16 [N, b_ld]
+ * (device, 16-byte aligned, row-major, the first D columns used). For each query row i, the k largest of
+ *     s(i, j) = alpha * (queries_i . base_j) + beta[j]      (fp32 accumulation of the fp16 products; beta NULL = 0)
+ * over j in [0, N), leaving out j == i + self_offset when self_offset >= 0 (an all-against-all search passes 0),
+ * ordered by (score descending, index ascending): out_scores fp32 [Q, k] and out_idx int64 [Q, k] (device, dense).
+ * Cosine similarity: alpha 1, no beta, rows normalised before rounding to fp16. Squared Euclidean distance:
+ * alpha 2, beta[j] = -|base_j|^2, so ranking by s descending ranks by distance ascending.
+ * A query's results are bit-identical whatever the other queries, Q, its row or `splits`: a score depends only on its
+ * two rows, and the top k under a total order does not depend on the order candidates are seen in.
+ * Two launches: the fused wgmma GEMM + top-k over `splits` contiguous stripes of the database, one partial top k per
+ * (query, stripe) into scratch, then a merge of the stripes' lists per query. The score matrix is never stored.
+ * scratch: esmb200_knn_scratch_bytes(Q, k, splits) bytes, 16-byte aligned. 1 <= k <= 128, k <= N (k <= N - 1 with
+ * self_offset >= 0), 1 <= N < 2^31, Q >= 0, D % 64 == 0, q_ld and b_ld >= D and multiples of 8, 1 <= splits <= 1024,
+ * non-NULL pointers and enough scratch, else ESMB200_EINVAL before any launch. Q == 0 launches nothing.
+ * esmb200_knn_scratch_bytes writes the size to *out; it refuses (ESMB200_EINVAL) k or splits out of range, Q < 0 and
+ * a NULL out. */
+int esmb200_knn_scratch_bytes(int32_t Q, int32_t k, int32_t splits, size_t* out);
+int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld, int64_t N,
+                       int32_t D, const float* beta, float alpha, int64_t self_offset, int32_t k, int32_t splits,
+                       void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -442,7 +463,7 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
  *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
  *         and each kernel of esmb200_sample_rows), 21 greedy MSA row selection (each kernel of
- *         esmb200_msa_greedy_select) */
+ *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
