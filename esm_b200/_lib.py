@@ -74,10 +74,14 @@ EXPORTS = (
     "esmb200_msa_greedy_select",
     "esmb200_knn_scratch_bytes",
     "esmb200_knn_search",
+    "esmb200_align_scratch_bytes",
+    "esmb200_align_similarity",
+    "esmb200_align",
 )
 
 ABI_VERSION = 4
 SELECT_MAX, SELECT_MIN = 0, 1  # ESMB200_SELECT_MAX / ESMB200_SELECT_MIN
+ALIGN_LOCAL, ALIGN_GLOBAL = 0, 1  # ESMB200_ALIGN_LOCAL / ESMB200_ALIGN_GLOBAL
 EPI_QKV_ROPE, EPI_BIAS_RESIDUAL, EPI_BIAS_GELU, EPI_BIAS_F32, EPI_BIAS_GELU_F32, EPI_GELU_FP8 = range(6)
 
 
@@ -194,6 +198,14 @@ def _declare(lib):
     lib.esmb200_knn_search.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_int32, c_void_p,
                                        c_float, c_int64, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p,
                                        c_void_p]
+    lib.esmb200_align_scratch_bytes.restype = c_size_t
+    lib.esmb200_align_scratch_bytes.argtypes = [c_int32, c_int64, c_int64, c_int64]
+    lib.esmb200_align_similarity.restype = c_int32
+    lib.esmb200_align_similarity.argtypes = [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int64,
+                                             c_int64, c_int64, c_int32, c_void_p, c_void_p, c_size_t, c_void_p]
+    lib.esmb200_align.restype = c_int32
+    lib.esmb200_align.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_int64, c_int64, c_int32,
+                                  c_float, c_float, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.esmb200_layernorm_f16.restype = c_int32
     lib.esmb200_layernorm_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p]
     lib.esmb200_gemm_f16.restype = c_int32

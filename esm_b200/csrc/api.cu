@@ -18,6 +18,7 @@
 
 #include <mutex>
 
+#include "align.cuh"
 #include "attention8.cuh"
 #include "attention_contact.cuh"
 #include "attention_probs.cuh"
@@ -58,7 +59,7 @@ int fail_cuda(cudaError_t e, const char* what) {
 // ---- launch accounting + optional per-launch CUDA-event timing (bench.py's roofline numbers) --------------------
 enum ProfTag : int { T_LN1 = 0, T_QKV, T_ATTN, T_OUT, T_LN2, T_FC1, T_FC2, T_KEYBITS, T_EMBED, T_LN_F32, T_PROBS,
                      T_CONVERT, T_GEMM_OTHER, T_MEANPOOL, T_TIED_SCORES, T_TIED_SOFTMAX, T_TIED_PV, T_LOG_SOFTMAX,
-                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_MSA_SELECT, T_KNN, T_COUNT };
+                     T_WINDOW_MERGE, T_JACOBIAN, T_SAMPLING, T_MSA_SELECT, T_KNN, T_ALIGN, T_COUNT };
 struct Profiler {  // process-wide, guarded by `mu`: launches may come from several host threads / streams
   std::mutex mu;
   bool on = false;
@@ -1812,6 +1813,101 @@ int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void*
     ProfScope ps(T_KNN, st);
     const int threads = splits >= 256 ? 256 : (splits + 31) / 32 * 32;
     knn_merge_kernel<<<(unsigned)Q, threads, 0, st>>>(p.keys, Q, k, splits, out_scores, out_idx);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+
+size_t esmb200_align_scratch_bytes(int32_t P, int64_t n_q, int64_t n_t, int64_t n_cells) {
+  if (P < 0 || n_q < 0 || n_t < 0 || n_cells < 0) return 0;
+  return align_scratch(P, n_q, n_t, n_cells).bytes;
+}
+
+namespace {
+// the refusals both alignment calls share; the per-pair offsets are the caller's (esm_b200/align.py builds them)
+int align_check(const int64_t* q_off, const int64_t* t_off, const int64_t* s_off, int32_t P, int64_t n_q, int64_t n_t,
+                int64_t n_cells, const void* scratch, size_t scratch_bytes) {
+  if (P < 0) return fail(ESMB200_EINVAL, "align needs P >= 0");
+  if (n_q < P || n_t < P || n_cells < P || n_q > INT32_MAX * (int64_t)P || n_t > INT32_MAX * (int64_t)P)
+    return fail(ESMB200_EINVAL, "align needs La, Lb >= 1 for every pair: n_q, n_t and n_cells >= P");
+  if (n_cells > (int64_t(1) << 40)) return fail(ESMB200_EINVAL, "align needs n_cells <= 2^40");
+  if (P == 0) return ESMB200_OK;
+  if (!q_off || !t_off || !s_off || !scratch) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(scratch) % 256 != 0) return fail(ESMB200_EINVAL, "scratch must be 256-byte aligned");
+  if (scratch_bytes < align_scratch(P, n_q, n_t, n_cells).bytes)
+    return fail(ESMB200_EINVAL, "more cells than the scratch: scratch smaller than esmb200_align_scratch_bytes");
+  return ESMB200_OK;
+}
+
+unsigned align_splits(int32_t P, int per_sm) {  // CTAs per pair: fill the GPU about per_sm times over
+  const int64_t want = ((int64_t)per_sm * num_sms() + P - 1) / P;
+  return (unsigned)(want < 1 ? 1 : want > 64 ? 64 : want);
+}
+}  // namespace
+
+int esmb200_align_similarity(const void* q_rows, const void* t_rows, int32_t D, const int64_t* q_off,
+                             const int64_t* t_off, const int64_t* s_off, int32_t P, int64_t n_q, int64_t n_t,
+                             int64_t n_cells, int32_t zscore, float* out, void* scratch, size_t scratch_bytes,
+                             void* stream) {
+  if (D < 64 || D % 64 != 0) return fail(ESMB200_EINVAL, "align_similarity needs D % 64 == 0");
+  if (zscore != 0 && zscore != 1) return fail(ESMB200_EINVAL, "align_similarity zscore must be 0 or 1");
+  int rc = align_check(q_off, t_off, s_off, P, n_q, n_t, n_cells, scratch, scratch_bytes);
+  if (rc || P == 0) return rc;
+  if (!q_rows || !t_rows || !out) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(q_rows) % 16 != 0 || reinterpret_cast<uintptr_t>(t_rows) % 16 != 0)
+    return fail(ESMB200_EINVAL, "align_similarity needs 16-byte aligned rows");
+  if ((rc = check_device())) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const AlignScratch sc = align_scratch(P, n_q, n_t, n_cells);
+  float2* stats = reinterpret_cast<float2*>(static_cast<char*>(scratch) + sc.stats_off);
+  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
+    ProfScope ps(T_ALIGN, st);
+    align_sim_kernel<<<dim3((unsigned)P, align_splits(P, 8)), kAlignSimThreads, 0, st>>>(
+        static_cast<const __half*>(q_rows), static_cast<const __half*>(t_rows), D, q_off, t_off, s_off, out);
+    CK(cudaGetLastError());
+  }
+  if (zscore) {
+    {
+      ProfScope ps(T_ALIGN, st);
+      align_stats_kernel<<<dim3((unsigned)P, align_splits(P, 8)), kAlignStatThreads, 0, st>>>(out, q_off, t_off, s_off,
+                                                                                               n_q, stats);
+      CK(cudaGetLastError());
+    }
+    ProfScope ps(T_ALIGN, st);
+    align_zscore_kernel<<<dim3((unsigned)P, align_splits(P, 8)), kAlignStatThreads, 0, st>>>(out, q_off, t_off, s_off,
+                                                                                              n_q, stats);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+int esmb200_align(const float* s, const int64_t* q_off, const int64_t* t_off, const int64_t* s_off, int32_t P,
+                  int64_t n_q, int64_t n_t, int64_t n_cells, int32_t mode, float gap_open, float gap_extend,
+                  void* scratch, size_t scratch_bytes, float* scores, int32_t* spans, uint8_t* ops, int32_t* n_ops,
+                  void* stream) {
+  if (mode != ESMB200_ALIGN_LOCAL && mode != ESMB200_ALIGN_GLOBAL)
+    return fail(ESMB200_EINVAL, "align mode must be ESMB200_ALIGN_LOCAL or ESMB200_ALIGN_GLOBAL");
+  if (!(gap_open >= 0.f) || !(gap_extend >= 0.f) || !isfinite(gap_open) || !isfinite(gap_extend))
+    return fail(ESMB200_EINVAL, "align needs finite gap penalties >= 0");
+  int rc = align_check(q_off, t_off, s_off, P, n_q, n_t, n_cells, scratch, scratch_bytes);
+  if (rc || P == 0) return rc;
+  if (!s || !scores || !spans || !ops || !n_ops) return fail(ESMB200_EINVAL, "null argument");
+  if ((rc = check_device())) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const AlignScratch sc = align_scratch(P, n_q, n_t, n_cells);
+  uint8_t* base = static_cast<uint8_t*>(scratch);
+  const int local = mode == ESMB200_ALIGN_LOCAL;
+  {
+    ProfScope ps(T_ALIGN, st);
+    align_dp_kernel<<<(unsigned)P, 32, 0, st>>>(s, q_off, t_off, s_off, local, gap_open, gap_extend, base,
+                                                sc.border_off, scores, spans);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_ALIGN, st);
+    align_trace_kernel<<<(unsigned)((P + 127) / 128), 128, 0, st>>>(q_off, t_off, s_off, P, local, base, spans, ops,
+                                                                    n_ops);
     CK(cudaGetLastError());
   }
   return ESMB200_OK;

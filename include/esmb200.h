@@ -342,6 +342,50 @@ int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void*
                        int32_t D, const float* beta, float alpha, int64_t self_offset, int32_t k, int32_t splits,
                        void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream);
 
+/* Pairwise alignment of proteins by their per-residue embeddings (esm_b200/align.py; the EBA / pLM-BLAST family of
+ * methods). A new operation with no reference code. Pair p (of P) has La query rows and Lb target rows, La, Lb >= 1:
+ * query rows [q_off[p], q_off[p+1]) and target rows [t_off[p], t_off[p+1]), its similarity S' as [La, Lb] fp32
+ * row-major at s_off[p] (offsets: int64 [P+1] device arrays from 0, non-decreasing; n_q = q_off[P] query rows,
+ * n_t = t_off[P] target rows and n_cells = s_off[P] are passed from the host as well; the per-pair offsets are
+ * checked by the caller). Results depend only on the pair: not on the other pairs, their order or the device.
+ * esmb200_align_similarity: q_rows, t_rows fp16 [*, D] (16-byte aligned, D % 64 == 0, rows normalised and
+ *   zero-padded by the caller), S[i,j] = q_i . t_j with fp32 accumulation of the fp16 products (mma.sync).
+ *   zscore 1: S'[i,j] = 0.5 * ((S - mu_r_i) / sd_r_i + (S - mu_c_j) / sd_c_j), mean and population standard
+ *   deviation of row i and column j taken in fp64 in a fixed order and rounded to fp32, a term 0 where its sd is 0;
+ *   zscore 0: S' = S. Written to out at s_off. The z-score statistics use the scratch.
+ * esmb200_align: the affine-gap dynamic programme on S' in fp32, gap_open o >= 0 and gap_extend e >= 0 finite:
+ *     E[i][j] = max(H[i][j-1] - o, E[i][j-1] - e)   target residue j against a gap, op 'T'
+ *     F[i][j] = max(H[i-1][j] - o, F[i-1][j] - e)   query residue i against a gap,  op 'Q'
+ *     H[i][j] = max(H[i-1][j-1] + S'[i-1][j-1], E[i][j], F[i][j] [, 0 local])       diagonal,  op 'M'
+ *   one fp32 add or subtract per candidate, no fused operations. ESMB200_ALIGN_LOCAL: H = 0 on row 0 and column 0,
+ *   E = F = -inf there; the end cell is the largest H, a tie to the smallest i, then j (a score of 0 ends at (0, 0)).
+ *   ESMB200_ALIGN_GLOBAL: H[0][0] = 0, row 0 and column 0 follow the same recurrences without the diagonal and with
+ *   -inf outside the matrix; the end cell is (La, Lb). The source of a value is the first candidate equal to the
+ *   maximum in the order diagonal, E, F, zero (H) and open, extend (E, F). Traceback from the end cell in state H:
+ *   diagonal emits M to (i-1, j-1); E or F switches state at the same cell; E emits T to (i, j-1) and F emits Q to
+ *   (i-1, j), into state H if it opened and its own state if it extended. Local stops at a cell whose H came from
+ *   zero or at row or column 0; global at (0, 0).
+ *   Outputs (device): scores fp32 [P]; spans int32 [P, 4] = q0, q1, t0, t1 (0-based, end exclusive); the op string
+ *   of pair p in query->target order at ops + q_off[p] + t_off[p] (La + Lb bytes per pair, n_q + n_t in all);
+ *   n_ops int32 [P]. Two kernels: one warp per pair runs the wavefront and stores one direction byte per cell, then one
+ *   thread per pair walks the traceback.
+ * scratch: esmb200_align_scratch_bytes(P, n_q, n_t, n_cells) bytes, 256-byte aligned, for either call: about one byte
+ *   per cell plus 32 per row and column and 8 per row and column (border rows of the programme, z-score statistics);
+ *   0 for a negative argument. Refused with ESMB200_EINVAL before any launch: P < 0, n_q, n_t or n_cells < P,
+ *   n_cells > 2^40, D, an unknown mode or zscore, non-finite or negative penalties, NULL pointers, unaligned or too
+ *   little scratch ("more cells than the scratch"). P == 0 launches nothing. No atomics. */
+#define ESMB200_ALIGN_LOCAL 0
+#define ESMB200_ALIGN_GLOBAL 1
+size_t esmb200_align_scratch_bytes(int32_t P, int64_t n_q, int64_t n_t, int64_t n_cells);
+int esmb200_align_similarity(const void* q_rows, const void* t_rows, int32_t D, const int64_t* q_off,
+                             const int64_t* t_off, const int64_t* s_off, int32_t P, int64_t n_q, int64_t n_t,
+                             int64_t n_cells, int32_t zscore, float* out, void* scratch, size_t scratch_bytes,
+                             void* stream);
+int esmb200_align(const float* s, const int64_t* q_off, const int64_t* t_off, const int64_t* s_off, int32_t P,
+                  int64_t n_q, int64_t n_t, int64_t n_cells, int32_t mode, float gap_open, float gap_extend,
+                  void* scratch, size_t scratch_bytes, float* scores, int32_t* spans, uint8_t* ops, int32_t* n_ops,
+                  void* stream);
+
 /* ---- single-kernel entry points (used by the parity tests and profiles; same kernels as above) ---- */
 
 /* out = epilogue(A[M,K] fp16 x W[N,K]^T fp16 + bias[N]);  epilogue: 0 qkv+rope -> fp16, 1 residual-add into fp32 out,
@@ -463,7 +507,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
  *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
  *         and each kernel of esmb200_sample_rows), 21 greedy MSA row selection (each kernel of
- *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search) */
+ *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search),
+ *         23 embedding alignment (each kernel of esmb200_align_similarity and esmb200_align) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
 int esmb200_profile_read(int32_t* tags, float* ms, int32_t max_records);
