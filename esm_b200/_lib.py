@@ -74,6 +74,8 @@ EXPORTS = (
     "esmb200_msa_greedy_select",
     "esmb200_knn_scratch_bytes",
     "esmb200_knn_search",
+    "esmb200_knn_search_accumulate",
+    "esmb200_knn_decode",
     "esmb200_align_scratch_bytes",
     "esmb200_align_similarity",
     "esmb200_align",
@@ -198,6 +200,12 @@ def _declare(lib):
     lib.esmb200_knn_search.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_int32, c_void_p,
                                        c_float, c_int64, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p,
                                        c_void_p]
+    lib.esmb200_knn_search_accumulate.restype = c_int32
+    lib.esmb200_knn_search_accumulate.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_int64,
+                                                  c_int32, c_void_p, c_float, c_int64, c_int32, c_int32, c_void_p,
+                                                  c_size_t, c_void_p, c_void_p]
+    lib.esmb200_knn_decode.restype = c_int32
+    lib.esmb200_knn_decode.argtypes = [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
     lib.esmb200_align_scratch_bytes.restype = c_size_t
     lib.esmb200_align_scratch_bytes.argtypes = [c_int32, c_int64, c_int64, c_int64]
     lib.esmb200_align_similarity.restype = c_int32

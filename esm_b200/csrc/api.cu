@@ -1758,6 +1758,21 @@ int esmb200_msa_greedy_select(const uint8_t* rows, int64_t ld, int32_t N, int32_
 }
 
 
+extern "C++" {
+namespace {
+// the fused GEMM + top-k launch both search calls share
+template <bool STREAM>
+int knn_launch_topk(const CUtensorMap& tq, const CUtensorMap& tx, const KnnParams& p, int splits, cudaStream_t st) {
+  CK(cudaFuncSetAttribute(knn_topk_kernel<STREAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, knn_cfg::SMEM_BYTES));
+  ProfScope ps(T_KNN, st);  // one ProfScope per kernel: esmb200_launch_count counts kernels
+  const int64_t grid = (int64_t)p.query_blocks * splits;
+  knn_topk_kernel<STREAM><<<(unsigned)grid, knn_cfg::NUM_THREADS, knn_cfg::SMEM_BYTES, st>>>(tq, tx, p);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+}  // namespace
+}  // extern "C++"
+
 int esmb200_knn_scratch_bytes(int32_t Q, int32_t k, int32_t splits, size_t* out) {
   if (!out) return fail(ESMB200_EINVAL, "null argument");
   if (Q < 0 || k < 1 || k > knn_cfg::MAX_K || splits < 1 || splits > knn_cfg::MAX_SPLITS)
@@ -1801,20 +1816,89 @@ int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void*
   p.beta = beta;
   p.alpha = alpha;
   p.self_offset = self_offset;
+  p.row0 = 0;
+  p.seed = nullptr;
   p.keys = static_cast<unsigned long long*>(scratch);
-  CK(cudaFuncSetAttribute(knn_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, knn_cfg::SMEM_BYTES));
-  {  // one ProfScope per kernel: esmb200_launch_count counts kernels
-    ProfScope ps(T_KNN, st);
-    const int64_t grid = (int64_t)p.query_blocks * splits;
-    knn_topk_kernel<<<(unsigned)grid, knn_cfg::NUM_THREADS, knn_cfg::SMEM_BYTES, st>>>(tq, tx, p);
-    CK(cudaGetLastError());
-  }
+  if ((rc = knn_launch_topk<false>(tq, tx, p, splits, st))) return rc;
   {
     ProfScope ps(T_KNN, st);
     const int threads = splits >= 256 ? 256 : (splits + 31) / 32 * 32;
-    knn_merge_kernel<<<(unsigned)Q, threads, 0, st>>>(p.keys, Q, k, splits, out_scores, out_idx);
+    knn_merge_kernel<4, false><<<(unsigned)Q, threads, 0, st>>>(p.keys, Q, k, splits, nullptr, out_scores, out_idx);
     CK(cudaGetLastError());
   }
+  return ESMB200_OK;
+}
+
+int esmb200_knn_search_accumulate(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld,
+                                  int64_t n, int64_t row0, int32_t D, const float* beta, float alpha,
+                                  int64_t self_offset, int32_t k, int32_t splits, void* scratch, size_t scratch_bytes,
+                                  uint64_t* keys, void* stream) {
+  if (k < 1 || k > knn_cfg::MAX_K) return fail(ESMB200_EINVAL, "knn_search_accumulate needs 1 <= k <= 128");
+  if (Q < 0 || n < 1 || row0 < 0 || row0 > INT32_MAX || n > INT32_MAX - row0)
+    return fail(ESMB200_EINVAL, "knn_search_accumulate needs Q >= 0, n >= 1, row0 >= 0 and row0 + n < 2^31");
+  if (D < 64 || D % 64 != 0) return fail(ESMB200_EINVAL, "knn_search_accumulate needs D % 64 == 0");
+  if (q_ld < D || b_ld < D || q_ld % 8 != 0 || b_ld % 8 != 0)
+    return fail(ESMB200_EINVAL,
+                "knn_search_accumulate needs q_ld, b_ld >= D and multiples of 8 (16-byte rows for TMA)");
+  if (splits < 1 || splits > knn_cfg::MAX_SPLITS)
+    return fail(ESMB200_EINVAL, "knn_search_accumulate needs 1 <= splits <= 1024");
+  if (!queries || !base || !scratch || !keys) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(queries) % 16 != 0 || reinterpret_cast<uintptr_t>(base) % 16 != 0)
+    return fail(ESMB200_EINVAL, "knn_search_accumulate needs 16-byte aligned queries and base (TMA)");
+  if (reinterpret_cast<uintptr_t>(scratch) % 16 != 0) return fail(ESMB200_EINVAL, "scratch must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(keys) % 8 != 0) return fail(ESMB200_EINVAL, "keys must be 8-byte aligned");
+  if (scratch_bytes < (size_t)splits * (size_t)Q * (size_t)k * 8)
+    return fail(ESMB200_EINVAL, "scratch smaller than esmb200_knn_scratch_bytes");
+  if (Q == 0) return ESMB200_OK;
+  int rc = check_device();
+  if (rc) return rc;
+  CUtensorMap tq, tx;
+  if ((rc = make_tmap_f16(&tq, queries, (uint64_t)Q, (uint64_t)D, (uint64_t)q_ld, knn_cfg::BLOCK_M))) return rc;
+  if ((rc = make_tmap_f16(&tx, base, (uint64_t)n, (uint64_t)D, (uint64_t)b_ld, knn_cfg::BLOCK_N))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KnnParams p;
+  p.Q = Q;
+  p.D = D;
+  p.k = k;
+  p.N = n;
+  const int64_t tiles = (n + knn_cfg::BLOCK_N - 1) / knn_cfg::BLOCK_N;
+  p.tiles_per_stripe = (int)((tiles + splits - 1) / splits);
+  p.query_blocks = (Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  p.beta = beta;
+  p.alpha = alpha;
+  p.self_offset = self_offset;
+  p.row0 = row0;
+  p.seed = reinterpret_cast<const unsigned long long*>(keys);
+  p.keys = static_cast<unsigned long long*>(scratch);
+  if ((rc = knn_launch_topk<true>(tq, tx, p, splits, st))) return rc;
+  {
+    ProfScope ps(T_KNN, st);
+    const int lists = splits + 1;  // the stripes and the running list
+    const int threads = lists >= 256 ? 256 : (lists + 31) / 32 * 32;
+    knn_merge_kernel<5, true><<<(unsigned)Q, threads, 0, st>>>(p.keys, Q, k, splits,
+                                                               reinterpret_cast<unsigned long long*>(keys), nullptr,
+                                                               nullptr);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_scores, int64_t* out_idx, void* stream) {
+  if (Q < 0 || k < 1 || k > knn_cfg::MAX_K) return fail(ESMB200_EINVAL, "knn_decode needs Q >= 0 and 1 <= k <= 128");
+  if (!keys || !out_scores || !out_idx) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(keys) % 8 != 0) return fail(ESMB200_EINVAL, "keys must be 8-byte aligned");
+  if (reinterpret_cast<uintptr_t>(out_scores) % 4 != 0 || reinterpret_cast<uintptr_t>(out_idx) % 8 != 0)
+    return fail(ESMB200_EINVAL, "knn_decode needs 4-byte aligned out_scores and 8-byte aligned out_idx");
+  if (Q == 0) return ESMB200_OK;
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t total = (int64_t)Q * k;
+  ProfScope ps(T_KNN, st);
+  const int64_t blocks = (total + 255) / 256;
+  knn_decode_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), total, out_scores, out_idx);
+  CK(cudaGetLastError());
   return ESMB200_OK;
 }
 

@@ -24,6 +24,14 @@
 // knn_merge_kernel: one block per query merges the S stripe lists (k rounds of a block-wide maximum over the list
 // heads) and decodes the keys to fp32 scores and int64 indices.
 //
+// Streamed search (esmb200_knn_search_accumulate): the database arrives in chunks; a chunk of n rows holds global rows
+// [row0, row0 + n), and candidate keys carry the global index, so a key means the same thing in every chunk.  A running
+// list keys [Q, k] (0 = empty slot) holds the top k of the chunks seen so far.  knn_topk_kernel seeds each row's
+// threshold with the running k-th key: a candidate at or below it cannot enter the final top k, so seeding changes no
+// result, and once the list has filled most tiles end at the warpgroup OR.  knn_merge_kernel<ACC> then merges the
+// stripe lists and the running list (copied to shared memory first, since it is overwritten in place) and writes keys
+// back undecoded; knn_decode_kernel decodes the final list once.
+//
 // Shared memory of knn_topk_kernel (k <= 128): ring 3 x (8 + 32) KB = 120 KB, k-lists 64 x 128 x 8 B = 64 KB, queues
 // 64 x 64 x 8 B = 32 KB, thresholds 512 B, queue counts 256 B, barriers, 1 KB alignment slack: 223,232 B of 232,448.
 // 64 query rows per CTA: 128 rows would need 128 KB of k-lists at k = 128, leaving no room for a 3-stage ring.
@@ -59,7 +67,9 @@ struct KnnParams {
   int query_blocks;
   const float* beta;     // [N] or nullptr
   float alpha;
-  int64_t self_offset;   // < 0: none
+  int64_t self_offset;   // < 0: none; in global rows
+  int64_t row0;          // global index of the chunk's row 0 (0 for esmb200_knn_search)
+  const unsigned long long* seed;  // running list [Q, k] whose k-th key seeds the thresholds, or nullptr
   unsigned long long* keys;  // scratch [splits, Q, k]
 };
 
@@ -67,6 +77,14 @@ __device__ __forceinline__ unsigned long long knn_key(float s, int64_t j) {
   const uint32_t u = __float_as_uint(s);
   const uint32_t o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
   return ((unsigned long long)o << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)j);
+}
+
+// the inverse of knn_key: the fp32 score and the index
+__device__ __forceinline__ void knn_decode_key(unsigned long long key, float* score, int64_t* idx) {
+  const uint32_t o = (uint32_t)(key >> 32);
+  const uint32_t u = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
+  *score = __uint_as_float(u);
+  *idx = (int64_t)(0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull));
 }
 
 // warpgroup-wide OR (bar.red on a named barrier: also a barrier with bar.sync's memory ordering)
@@ -83,7 +101,9 @@ __device__ __forceinline__ bool knn_bar_or(uint32_t id, bool v) {
   return r != 0;
 }
 
-// Merge one row's queue (cnt > 0 entries) into its k-list; one warp, called with a warp-uniform row.
+// Merge one row's queue (cnt > 0 entries) into its k-list; one warp, called with a warp-uniform row.  SEEDED: the
+// threshold may start above the list's k-th key (streamed search), so a merge keeps the larger of the two.
+template <bool SEEDED>
 __device__ __forceinline__ void knn_merge_row(unsigned long long* list, unsigned long long* queue, int* cnt,
                                               unsigned long long* th, int k, uint32_t lane) {
   const int n = *cnt < knn_cfg::QCAP ? *cnt : knn_cfg::QCAP;
@@ -149,12 +169,15 @@ __device__ __forceinline__ void knn_merge_row(unsigned long long* list, unsigned
     if (qr[sl] < k) list[qr[sl]] = v[sl];
   __syncwarp();
   if (lane == 0) {
-    *th = list[k - 1];
+    *th = (SEEDED && *th > list[k - 1]) ? *th : list[k - 1];
     *cnt = 0;
   }
   __syncwarp();
 }
 
+// STREAM: a chunk of a streamed search (row0 and the seeded thresholds); without it the kernel is the resident one,
+// with no code for either.
+template <bool STREAM>
 __global__ void __launch_bounds__(knn_cfg::NUM_THREADS, 1)
 knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                 const KnnParams p) {
@@ -172,6 +195,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   uint64_t* empty_bar = bars + STAGES;
 
   const int k = p.k;
+  const int64_t row0 = STREAM ? p.row0 : 0;
   const int qb = blockIdx.x % p.query_blocks, stripe = blockIdx.x / p.query_blocks;
   const int q0 = qb * BLOCK_M;
   const int tiles = (int)((p.N + BLOCK_N - 1) / BLOCK_N);
@@ -190,7 +214,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   for (int i = threadIdx.x; i < BLOCK_M * MAX_K; i += NUM_THREADS) s_list[i] = 0ull;
   for (int i = threadIdx.x; i < BLOCK_M; i += NUM_THREADS) {
-    s_th[i] = 0ull;
+    s_th[i] = (STREAM && p.seed != nullptr && q0 + i < p.Q) ? p.seed[(size_t)(q0 + i) * k + k - 1] : 0ull;
     s_cnt[i] = 0;
   }
   __syncthreads();
@@ -225,19 +249,19 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
   int rl[2];           // the thread's rows of the block
   bool rvalid[2];
-  int64_t excl[2];     // the excluded column of each row (-1: none)
+  int64_t excl[2];     // the excluded column of each row, chunk-local (negative: none)
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     rl[hr] = (int)(warp * 16 + g + 8 * hr);
     const int q = q0 + rl[hr];
     rvalid[hr] = q < p.Q;
-    excl[hr] = p.self_offset >= 0 ? (int64_t)q + p.self_offset : -1;
+    excl[hr] = p.self_offset >= 0 ? (int64_t)q + p.self_offset - row0 : -1;
   }
 
   // every row's queue into its list: warp w takes rows 16 w .. 16 w + 15
   auto merge_all = [&]() {
     for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r)
-      if (s_cnt[r] > 0) knn_merge_row(s_list + r * MAX_K, s_queue + r * QCAP, s_cnt + r, s_th + r, k, lane);
+      if (s_cnt[r] > 0) knn_merge_row<STREAM>(s_list + r * MAX_K, s_queue + r * QCAP, s_cnt + r, s_th + r, k, lane);
   };
 
   for (int t = t_begin; t < t_end; ++t) {
@@ -273,8 +297,9 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           const int64_t j = n0 + 8 * i + 2 * (int)c + e;
           const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
           const bool in = j < p.N;
-          any |= in && rvalid[0] && j != excl[0] && knn_key(fmaf(p.alpha, acc[4 * i + e], b) + 0.0f, j) > th0;
-          any |= in && rvalid[1] && j != excl[1] && knn_key(fmaf(p.alpha, acc[4 * i + 2 + e], b) + 0.0f, j) > th1;
+          any |= in && rvalid[0] && j != excl[0] && knn_key(fmaf(p.alpha, acc[4 * i + e], b) + 0.0f, j + row0) > th0;
+          any |= in && rvalid[1] && j != excl[1] &&
+                 knn_key(fmaf(p.alpha, acc[4 * i + 2 + e], b) + 0.0f, j + row0) > th1;
         }
       }
     }
@@ -292,7 +317,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
 #pragma unroll
           for (int hr = 0; hr < 2; ++hr) {
-            const unsigned long long key = knn_key(fmaf(p.alpha, acc[4 * i + 2 * hr + e], b) + 0.0f, j);
+            const unsigned long long key = knn_key(fmaf(p.alpha, acc[4 * i + 2 * hr + e], b) + 0.0f, j + row0);
             if (j < p.N && rvalid[hr] && j != excl[hr] && key > (hr ? th1 : th0)) {
               const int pos = atomicAdd(s_cnt + rl[hr], 1);  // < QCAP: at most QCAP - CHUNK queued before a chunk
               s_queue[rl[hr] * QCAP + pos] = key;
@@ -319,28 +344,41 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
 }
 
-// One block per query: k rounds, each taking the largest head of the S stripe lists (keys are distinct, so the
-// winner is unique) and advancing that list.  Thread t owns stripes t, t + blockDim, ... (at most 4).
+// One block per query: k rounds, each taking the largest head of the lists (keys are distinct, so the winner is unique
+// unless it is an empty slot) and advancing that list.  The lists are the S stripe lists and, with ACC, the running
+// list run[q] as list S; thread t owns lists t, t + blockDim, ... (at most M).  Without ACC the winners are decoded to
+// out_scores / out_idx; with ACC they are written back to run[q] as keys.
+template <int M, bool ACC>
 __global__ void __launch_bounds__(256)
-knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int S, float* __restrict__ out_scores,
-                 int64_t* __restrict__ out_idx) {
+knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int S, unsigned long long* run,
+                 float* __restrict__ out_scores, int64_t* __restrict__ out_idx) {
   __shared__ unsigned long long red_key[2][8];
   __shared__ int red_s[2][8];
+  __shared__ unsigned long long s_run[ACC ? knn_cfg::MAX_K : 1];
   const int q = blockIdx.x;
   const int nt = blockDim.x, warp = threadIdx.x / 32, nw = nt / 32;
-  unsigned long long head[4];
-  int pos[4];
+  const int L = ACC ? S + 1 : S;
+  if (ACC) {
+    for (int i = threadIdx.x; i < k; i += nt) s_run[i] = run[(size_t)q * k + i];
+    __syncthreads();
+  }
+  auto fetch = [&](int s, int pos) -> unsigned long long {
+    if (ACC && s == S) return s_run[pos];
+    return keys[((size_t)s * Q + q) * k + pos];
+  };
+  unsigned long long head[M];
+  int pos[M];
 #pragma unroll
-  for (int m = 0; m < 4; ++m) {
+  for (int m = 0; m < M; ++m) {
     const int s = threadIdx.x + m * nt;
     pos[m] = 0;
-    head[m] = s < S ? keys[((size_t)s * Q + q) * k] : 0ull;
+    head[m] = s < L ? fetch(s, 0) : 0ull;
   }
   for (int r = 0; r < k; ++r) {
     unsigned long long best = 0ull;
     int bs = -1;
 #pragma unroll
-    for (int m = 0; m < 4; ++m)
+    for (int m = 0; m < M; ++m)
       if (head[m] > best || bs < 0) {
         best = head[m];
         bs = threadIdx.x + m * nt;
@@ -370,18 +408,26 @@ knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int 
       }
     }
 #pragma unroll
-    for (int m = 0; m < 4; ++m)
-      if (bs == (int)threadIdx.x + m * nt && bs < S) {
+    for (int m = 0; m < M; ++m)
+      if (bs == (int)threadIdx.x + m * nt && bs < L) {
         ++pos[m];
-        head[m] = pos[m] < k ? keys[((size_t)bs * Q + q) * k + pos[m]] : 0ull;
+        head[m] = pos[m] < k ? fetch(bs, pos[m]) : 0ull;
       }
     if (threadIdx.x == 0) {
-      const uint32_t o = (uint32_t)(best >> 32);
-      const uint32_t u = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
-      out_scores[(size_t)q * k + r] = __uint_as_float(u);
-      out_idx[(size_t)q * k + r] = (int64_t)(0xFFFFFFFFu - (uint32_t)(best & 0xFFFFFFFFull));
+      if (ACC)
+        run[(size_t)q * k + r] = best;
+      else
+        knn_decode_key(best, out_scores + (size_t)q * k + r, out_idx + (size_t)q * k + r);
     }
   }
+}
+
+// keys [n] to fp32 scores and int64 indices, as knn_merge_kernel<M, false> writes them
+__global__ void __launch_bounds__(256)
+knn_decode_kernel(const unsigned long long* __restrict__ keys, int64_t n, float* __restrict__ out_scores,
+                  int64_t* __restrict__ out_idx) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    knn_decode_key(keys[i], out_scores + i, out_idx + i);
 }
 
 }  // namespace esmb200

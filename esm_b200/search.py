@@ -14,17 +14,25 @@ descending. "l2": rows are rounded to fp16 as given; scores are Euclidean distan
 sqrt(max(|q|^2 - s, 0)) from the kernel's s = 2 q.x - |x|^2 (|x|^2 in fp32 from the fp16 rows). Ties go to the
 smaller index. Rows are zero-padded to a multiple of 64 columns, which changes no dot product.
 
+Databases larger than the GPU: IndexWriter writes a sharded index directory, and ShardedIndex memory-maps it and
+streams it through the GPU with the same results (see ShardedIndex).
+
 One search is two kernel launches per batch of queries (esmb200_knn_search, include/esmb200.h): a wgmma GEMM whose
 epilogue keeps each query's top k, and a merge of the database stripes' lists. The [Q, N] score matrix is never
 stored, and a query's result does not depend on the other queries or on how the database is split.
 """
 from __future__ import annotations
 
+import bisect
 import ctypes
+import json
 import math
 import os
+import pathlib
+from concurrent.futures import ThreadPoolExecutor
 from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -113,9 +121,26 @@ def knn(queries: torch.Tensor, base: torch.Tensor, k: int, beta: Optional[torch.
     return scores, idx
 
 
+def _check_k(k, candidates: int) -> int:
+    if isinstance(k, bool) or not isinstance(k, int):
+        raise TypeError(f"k must be an int, got {type(k).__name__}")
+    hi = min(MAX_K, candidates)
+    if not 1 <= k <= hi:
+        raise ValueError(f"k must be in [1, {hi}] for this index, got {k}")
+    return k
+
+
 def _read_extract_dir(path, layer: int) -> Tuple[List[str], torch.Tensor]:
     """(labels, fp32 [n, E]) from extract_cli's <label>.pt files under path (recursive: labels may contain '/'),
     ordered by the stored label. ValueError for a file without mean_representations[layer] or mixed widths."""
+    items = _scan_extract_dir(path, layer, keep_vectors=True)
+    return [l for l, _ in items], torch.stack([v for _, v in items])
+
+
+def _scan_extract_dir(path, layer: int, keep_vectors: bool):
+    """[(label, fp32 [E] vector or file path)] of every extract_cli file under path in label order, after the checks
+    _read_extract_dir makes; with keep_vectors False only the paths are kept, so memory does not grow with the
+    directory."""
     files = []
     for root, _, names in os.walk(path):
         files += [os.path.join(root, f) for f in names if f.endswith(".pt")]
@@ -133,9 +158,9 @@ def _read_extract_dir(path, layer: int) -> Tuple[List[str], torch.Tensor]:
             width = (v.numel(), f)
         elif v.numel() != width[0]:
             raise ValueError(f"{f} has width {v.numel()}, {width[1]} has {width[0]}: one index holds one width")
-        items.append((str(obj.get("label", os.path.splitext(os.path.relpath(f, path))[0])), v))
+        items.append((str(obj.get("label", os.path.splitext(os.path.relpath(f, path))[0])), v if keep_vectors else f))
     items.sort(key=lambda t: t[0])
-    return [l for l, _ in items], torch.stack([v for _, v in items])
+    return items
 
 
 class EmbeddingIndex:
@@ -198,12 +223,7 @@ class EmbeddingIndex:
 
     # ---- search ------------------------------------------------------------------------------------------------------
     def _check_k(self, k, candidates: int) -> int:
-        if isinstance(k, bool) or not isinstance(k, int):
-            raise TypeError(f"k must be an int, got {type(k).__name__}")
-        hi = min(MAX_K, candidates)
-        if not 1 <= k <= hi:
-            raise ValueError(f"k must be in [1, {hi}] for this index, got {k}")
-        return k
+        return _check_k(k, candidates)
 
     def _check_device(self) -> None:
         if not self.rows.is_cuda:
@@ -239,4 +259,519 @@ class EmbeddingIndex:
                 s = (squared_norms(q[b0:b1])[:, None] - s).clamp_min(0).sqrt()
             scores[b0:b1] = s
             idx[b0:b1] = i
+        return scores, idx
+
+
+# ---- sharded indexes on disk ------------------------------------------------------------------------------------------
+SHARD_FORMAT = "esm_b200.search-shards/1"
+MANIFEST = "manifest.json"
+SHARD_ROWS = 1 << 20          # rows per shard file the writer aims for
+TILE = 256                    # database rows per kernel tile: chunks are whole tiles
+RING_SLOTS = 2                # pinned host slots, and as many device slots
+MAX_SLOT_BYTES = 256 << 20    # the most database bytes one ring slot holds
+REFILL_THREADS = 16           # host threads copying one slot's rows out of the memory maps
+DEVICE_SHARE = 0.5            # default max_device_bytes: this share of the device's free memory
+
+
+def _read_manifest(path) -> dict:
+    f = pathlib.Path(path) / MANIFEST
+    try:
+        man = json.loads(f.read_text())
+    except (OSError, ValueError) as e:
+        raise ValueError(f"{path} is not a sharded index: {e}") from None
+    if not isinstance(man, dict) or man.get("format") != SHARD_FORMAT:
+        raise ValueError(f"{f} is not a {SHARD_FORMAT} manifest")
+    _check_metric(man["metric"])
+    return man
+
+
+def _write_durable(path: pathlib.Path, data) -> None:
+    """Writes bytes (or a numpy array's raw bytes) to path and fsyncs the file."""
+    with open(path, "wb") as f:
+        f.write(data if isinstance(data, bytes) else memoryview(np.ascontiguousarray(data)).cast("B"))
+        f.flush()
+        os.fsync(f.fileno())
+
+
+def _fsync_dir(path: pathlib.Path) -> None:
+    fd = os.open(path, os.O_RDONLY)
+    try:
+        os.fsync(fd)
+    finally:
+        os.close(fd)
+
+
+def _write_atomic(path: pathlib.Path, text: str) -> None:
+    """Replaces path with text: written and fsynced under a temporary name, the directory fsynced (so the files the
+    text names are durable first), renamed, and the directory fsynced again."""
+    tmp = path.with_name(f".{path.name}.tmp{os.getpid()}")
+    _write_durable(tmp, text.encode())
+    _fsync_dir(path.parent)
+    os.replace(tmp, path)
+    _fsync_dir(path.parent)
+
+
+class IndexWriter:
+    """Writes a sharded index directory, or appends shards to an existing one.
+
+        with search.IndexWriter("db/", dim=1280, metric="cosine", layer=33) as w:
+            w.add(vectors, labels)       # any number of times; fp32/fp16 [n, dim], labels default to the row numbers
+        index = search.ShardedIndex.open("db/")
+
+    The directory holds manifest.json (format, metric, dim, padded_dim, layer and the ordered shards with their row
+    counts) and per shard `<name>.f16` (raw little-endian fp16 rows [n, padded_dim], prepare_rows's rows),
+    `<name>.labels.json` and, for l2, `<name>.norms` (little-endian fp32 |x|^2, squared_norms's values). add()
+    prepares a batch at most one shard's rows at a time and buffers them until a shard is full, so memory stays
+    within one shard whatever the batch size (the caller's batch aside). A batch that is refused leaves the writer as
+    it was before the call. Shard files are fsynced as they are written; the manifest is written last, by close(),
+    fsynced under a temporary name and renamed over the old one, so a writer that stops before close(), or a power
+    loss at any point, leaves the previous index intact."""
+
+    def __init__(self, path, dim: int, metric: str = "cosine", layer: Optional[int] = None,
+                 shard_rows: int = SHARD_ROWS):
+        _check_metric(metric)
+        if isinstance(dim, bool) or not isinstance(dim, int) or dim < 1:
+            raise ValueError(f"dim must be a positive int, got {dim!r}")
+        if isinstance(shard_rows, bool) or not isinstance(shard_rows, int) or shard_rows < 1:
+            raise ValueError(f"shard_rows must be a positive int, got {shard_rows!r}")
+        self.path = pathlib.Path(path)
+        self.dim, self.metric, self.layer, self.shard_rows = dim, metric, layer, shard_rows
+        self._shards = []
+        if (self.path / MANIFEST).exists():
+            man = _read_manifest(self.path)
+            for key, want in (("metric", metric), ("dim", dim), ("layer", layer)):
+                if man[key] != want:
+                    raise ValueError(f"{path} holds an index of {key} {man[key]!r}: cannot append {key} {want!r}")
+            self._shards = list(man["shards"])
+        self.path.mkdir(parents=True, exist_ok=True)
+        self._pieces: List[Tuple[torch.Tensor, List[str]]] = []  # prepared rows and labels of the open shard
+        self._buffered = 0
+        self._closed = False
+
+    def __len__(self) -> int:
+        """Rows in the index once closed: the existing shards' and every row added."""
+        return sum(s["rows"] for s in self._shards) + self._buffered
+
+    def add(self, vectors: torch.Tensor, labels: Optional[Sequence[str]] = None) -> None:
+        if self._closed:
+            raise ValueError("the writer is closed")
+        if not (isinstance(vectors, torch.Tensor) and vectors.dim() == 2):
+            prepare_rows(vectors, self.metric)  # raises the TypeError
+        if vectors.shape[1] != self.dim:
+            raise ValueError(f"vectors have width {vectors.shape[1]}, the index {self.dim}")
+        n, n0 = vectors.shape[0], len(self)
+        labels = [str(n0 + i) for i in range(n)] if labels is None else [str(l) for l in labels]
+        if len(labels) != n:
+            raise ValueError(f"{len(labels)} labels for {n} rows")
+        state = (list(self._pieces), self._buffered, len(self._shards))
+        try:
+            r0 = 0
+            while r0 < n:  # fill the open shard, one slice at a time
+                r1 = min(n, r0 + self.shard_rows - self._buffered)
+                self._pieces.append((prepare_rows(vectors[r0:r1], self.metric).cpu(), labels[r0:r1]))
+                self._buffered += r1 - r0
+                if self._buffered == self.shard_rows:
+                    self._flush()
+                r0 = r1
+        except BaseException:
+            # the shards this call wrote are left out of the manifest; a later shard of the same name replaces them
+            self._pieces, self._buffered = state[0], state[1]
+            del self._shards[state[2]:]
+            raise
+
+    def _flush(self) -> None:
+        rows = torch.cat([r for r, _ in self._pieces])
+        labels = [l for _, ls in self._pieces for l in ls]
+        name = f"shard-{len(self._shards):05d}"
+        _write_durable(self.path / f"{name}.f16", rows.numpy().astype("<f2", copy=False))
+        if self.metric == "l2":
+            _write_durable(self.path / f"{name}.norms", squared_norms(rows).numpy().astype("<f4", copy=False))
+        _write_durable(self.path / f"{name}.labels.json", json.dumps(labels).encode())
+        self._shards.append({"name": name, "rows": rows.shape[0]})
+        self._pieces, self._buffered = [], 0
+
+    def close(self) -> None:
+        """Writes the last shard and then the manifest."""
+        if self._closed:
+            return
+        if len(self) < 1:
+            raise ValueError("an index needs at least one row")
+        if self._buffered:
+            self._flush()
+        man = {"format": SHARD_FORMAT, "metric": self.metric, "dim": self.dim, "padded_dim": padded_dim(self.dim),
+               "layer": self.layer, "shards": self._shards}
+        _write_atomic(self.path / MANIFEST, json.dumps(man, indent=1))
+        self._closed = True
+
+    def __enter__(self) -> "IndexWriter":
+        return self
+
+    def __exit__(self, exc_type, exc, tb) -> None:
+        if exc_type is None:
+            self.close()
+
+
+class _ShardLabels(Sequence):
+    """The labels of a sharded index by global row, each shard's file read the first time one of its rows is named."""
+
+    def __init__(self, path: pathlib.Path, shards, starts):
+        self._path, self._shards, self._starts = path, shards, starts
+        self._cache = {}
+
+    def __len__(self) -> int:
+        return self._starts[-1]
+
+    def __getitem__(self, i):
+        if isinstance(i, slice):
+            return [self[j] for j in range(*i.indices(len(self)))]
+        i = int(i)
+        if not 0 <= i < len(self):
+            raise IndexError(i)
+        s = bisect.bisect_right(self._starts, i) - 1
+        if s not in self._cache:
+            self._cache[s] = json.loads((self._path / f"{self._shards[s]['name']}.labels.json").read_text())
+        return self._cache[s][i - self._starts[s]]
+
+
+def _batch_sizes(q_rows: int, q_out: int) -> set:
+    """The query-batch sizes a streamed search launches: q_out queries in blocks of q_rows (the last block shorter),
+    each block in batches of QUERY_BATCH (the last batch shorter)."""
+    sizes = set()
+    for block in {min(q_rows, q_out), q_out % q_rows if q_rows else 0}:
+        if block > 0:
+            sizes.add(min(block, QUERY_BATCH))
+            if block > QUERY_BATCH and block % QUERY_BATCH:
+                sizes.add(block % QUERY_BATCH)
+    return sizes
+
+
+def scratch_bytes(q_rows: int, q_out: int, k: int, num_sms: int) -> int:
+    """Scratch for every accumulate call of a streamed search (q_rows, q_out as _batch_sizes): the largest
+    esmb200_knn_scratch_bytes over its batch sizes b at the most stripes choose_splits gives b (a short chunk only
+    lowers that). Splits times b is not monotone in b, so a short last batch can need more than a full one."""
+    most = lambda b: choose_splits(b, MAX_SPLITS * TILE, num_sms)  # noqa: E731  (no tile cap)
+    return max([most(b) * b * k * 8 for b in _batch_sizes(q_rows, q_out)] + [16])
+
+
+def _fixed_device_bytes(q_rows: int, q_out: int, k: int, D: int, metric: str, num_sms: int) -> int:
+    """Device bytes of a streamed search besides the ring: q_rows resident query rows (and l2 norms) with their
+    running lists, q_out rows of results, and the scratch (scratch_bytes)."""
+    per_tensor = 512  # the caching allocator's rounding, for each of the call's tensors
+    return (q_rows * D * 2 + (q_rows * 4 if metric == "l2" else 0) + q_rows * k * 8 + q_out * k * 12
+            + scratch_bytes(q_rows, q_out, k, num_sms) + 16 * per_tensor)
+
+
+def _row_bytes(D: int, metric: str) -> int:
+    return D * 2 + (4 if metric == "l2" else 0)
+
+
+def plan_chunk_rows(q_rows: int, q_out: int, k: int, D: int, metric: str, max_device_bytes: int,
+                    num_sms: int) -> int:
+    """Database rows per chunk of a streamed search: whole 256-row tiles, as many as let the ring's device slots and
+    the fixed buffers (_fixed_device_bytes) fit in max_device_bytes, and at most MAX_SLOT_BYTES per slot.
+    ValueError when not even one tile fits."""
+    fixed = _fixed_device_bytes(q_rows, q_out, k, D, metric, num_sms)
+    tile_bytes = RING_SLOTS * TILE * _row_bytes(D, metric)
+    tiles = (max_device_bytes - fixed) // tile_bytes
+    if tiles < 1:
+        raise ValueError(f"max_device_bytes = {max_device_bytes} leaves no room for a {TILE}-row chunk beside "
+                         f"{fixed} bytes of queries, lists, results and scratch: pass fewer queries or more bytes")
+    return int(min(tiles, max(1, MAX_SLOT_BYTES // (TILE * _row_bytes(D, metric))))) * TILE
+
+
+def device_bytes(q_rows: int, q_out: int, k: int, D: int, metric: str, chunk_rows: int, num_sms: int) -> int:
+    """The device bytes plan_chunk_rows budgets for a chunk of chunk_rows rows."""
+    return _fixed_device_bytes(q_rows, q_out, k, D, metric, num_sms) + RING_SLOTS * chunk_rows * _row_bytes(D, metric)
+
+
+def knn_accumulate(queries: torch.Tensor, base: torch.Tensor, row0: int, k: int, keys: torch.Tensor, scratch,
+                   beta: Optional[torch.Tensor] = None, alpha: float = 1.0, self_offset: int = -1,
+                   splits: Optional[int] = None) -> None:
+    """esmb200_knn_search_accumulate: fold the chunk base fp16 [n, D] (global rows row0 ..) into the running keys
+    [Q, k] (int64 storage of the uint64 keys, zeros before the first chunk). scratch: a contiguous CUDA uint8 tensor
+    of at least esmb200_knn_scratch_bytes(Q, k, splits) bytes, or None to allocate one."""
+    for name, t in (("queries", queries), ("base", base)):
+        if t.dtype != torch.float16 or t.dim() != 2 or not t.is_cuda or t.stride(1) != 1:
+            raise ValueError(f"{name} must be a CUDA fp16 tensor [n, D] with contiguous rows")
+    Q, n = queries.shape[0], base.shape[0]
+    dev = base.device
+    if queries.device != dev or queries.shape[1] != base.shape[1]:
+        raise ValueError("queries and base must be on one device with one width")
+    _check_keys(keys, Q, k, dev)
+    if beta is not None and (beta.dtype != torch.float32 or not beta.is_contiguous() or beta.numel() != n
+                             or beta.device != dev):
+        raise ValueError("beta must be a contiguous fp32 tensor [n] on the base's device")
+    if scratch is not None and (scratch.dtype != torch.uint8 or not scratch.is_contiguous() or scratch.device != dev):
+        raise ValueError("scratch must be a contiguous uint8 tensor on the base's device")
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        if splits is None:
+            splits = choose_splits(Q, n, torch.cuda.get_device_properties(base.device).multi_processor_count)
+        nbytes = ctypes.c_size_t(0)
+        _lib.check(lib.esmb200_knn_scratch_bytes(Q, k, splits, ctypes.byref(nbytes)))
+        if scratch is None:
+            scratch = torch.empty(max(nbytes.value, 16), dtype=torch.uint8, device=base.device)
+        _lib.check(lib.esmb200_knn_search_accumulate(
+            _ptr(queries), queries.stride(0), Q, _ptr(base), base.stride(0), n, row0, base.shape[1], _ptr(beta),
+            float(alpha), self_offset, k, splits, _ptr(scratch), scratch.numel(), _ptr(keys), _stream()))
+
+
+def _check_keys(keys: torch.Tensor, Q: int, k: int, dev: torch.device) -> None:
+    if not (isinstance(keys, torch.Tensor) and keys.dtype == torch.int64 and keys.is_contiguous()
+            and tuple(keys.shape) == (Q, k) and keys.device == dev):
+        raise ValueError(f"keys must be a contiguous int64 tensor [{Q}, {k}] on {dev}")
+
+
+def knn_decode(keys: torch.Tensor, scores: torch.Tensor, idx: torch.Tensor) -> None:
+    """esmb200_knn_decode: running keys [Q, k] to scores fp32 [Q, k] and idx int64 [Q, k] (dense, on keys' device)."""
+    if not (isinstance(keys, torch.Tensor) and keys.dim() == 2 and keys.is_cuda):
+        raise ValueError("keys must be a CUDA tensor [Q, k]")
+    Q, k = keys.shape
+    _check_keys(keys, Q, k, keys.device)
+    for name, t, dtype in (("scores", scores, torch.float32), ("idx", idx, torch.int64)):
+        if not (t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == (Q, k) and t.device == keys.device):
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor [{Q}, {k}] on the keys' device")
+    with torch.cuda.device(keys.device):
+        _lib.check(_lib.load().esmb200_knn_decode(_ptr(keys), Q, k, _ptr(scores), _ptr(idx), _stream()))
+
+
+def _cuda_device(device) -> torch.device:
+    if not torch.cuda.is_available():
+        raise ValueError("searching a sharded index needs a CUDA device")
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise ValueError(f"results go to a CUDA device, got {dev}")
+    return torch.device("cuda", dev.index if dev.index is not None else torch.cuda.current_device())
+
+
+class _HostRing:
+    """RING_SLOTS page-locked host slots of `rows` database rows (and l2 betas): plain host memory registered with
+    CUDA, the only host memory a streamed search pins (never the database)."""
+
+    def __init__(self, rows: int, D: int, l2: bool):
+        self.rows = [torch.empty((rows, D), dtype=torch.float16) for _ in range(RING_SLOTS)]
+        self.beta = [torch.empty(rows, dtype=torch.float32) for _ in range(RING_SLOTS)] if l2 else None
+        self._registered = []
+        cudart = torch.cuda.cudart()
+        for t in self.rows + (self.beta or []):
+            rc = cudart.cudaHostRegister(t.data_ptr(), t.numel() * t.element_size(), 0)
+            if int(rc) != 0:
+                self.release()
+                raise RuntimeError(f"cudaHostRegister failed ({int(rc)}) for a {t.nbytes}-byte ring slot")
+            self._registered.append(t)
+
+    def fits(self, rows: int, D: int, l2: bool) -> bool:
+        return self.rows[0].shape[0] >= rows and self.rows[0].shape[1] == D and (self.beta is not None or not l2)
+
+    def release(self) -> None:
+        cudart = torch.cuda.cudart()
+        for t in self._registered:
+            cudart.cudaHostUnregister(t.data_ptr())
+        self._registered = []
+
+
+_host_rings: dict = {}
+
+
+def _host_ring(rows: int, D: int, l2: bool, device: torch.device) -> _HostRing:
+    """The page-locked ring of the streamed searches on (device, current CUDA stream), kept registered between calls:
+    allocating and registering 2 x 268 MB costs about half a second, as much as streaming several GB. A larger or
+    different ring replaces it (the calls before it have synchronised). release_host_memory() unregisters them."""
+    key = (device, torch.cuda.current_stream(device).cuda_stream)
+    ring = _host_rings.get(key)
+    if ring is None or not ring.fits(rows, D, l2):
+        if ring is not None:
+            ring.release()
+            del _host_rings[key]
+        ring = _host_rings[key] = _HostRing(rows, D, l2)
+    return ring
+
+
+def release_host_memory() -> None:
+    """Unregisters and frees the page-locked rings ShardedIndex searches keep between calls."""
+    for ring in _host_rings.values():
+        ring.release()
+    _host_rings.clear()
+
+
+class ShardedIndex:
+    """A sharded index directory (IndexWriter), memory-mapped and searched by streaming its rows through the GPU, so
+    the database may be larger than the device. Same rows, labels, metric conventions and results as an EmbeddingIndex
+    of the same vectors:
+
+        index = search.ShardedIndex.open("db/")
+        scores, idx = index.search(queries, k=10)      # fp32 / int64 [Q, k] on the current CUDA device
+        scores, idx = index.search_all(k=10)           # every row against the index, its own row left out
+        index.labels[idx[0, 0]]                        # labels are read per shard, when a hit is named
+
+    Each call streams the database through a ring of RING_SLOTS page-locked host slots and as many device slots, one
+    chunk of whole 256-row tiles per slot: host threads refill a slot from the memory maps, a copy stream moves it to
+    the device, and the fused top-k kernel folds it into each query's running top-k list on the compute stream. The
+    database crosses the host link once per call (once per query block for search_all when its queries do not fit
+    beside the ring). max_device_bytes caps the device memory of the call and sets the chunk size; it does not change
+    the results. The page-locked host slots (at most 2 x 256 MB) stay registered for the next call, since registering
+    them costs about half a second; search.release_host_memory() frees them."""
+
+    def __init__(self, path, man: dict):
+        self.path = pathlib.Path(path)
+        self.metric, self.dim, self.layer = man["metric"], int(man["dim"]), man["layer"]
+        self.padded_dim = int(man["padded_dim"])
+        if self.padded_dim != padded_dim(self.dim):
+            raise ValueError(f"{path}: padded_dim {self.padded_dim} does not match dim {self.dim}")
+        self.shards = list(man["shards"])
+        self._starts = [0]
+        for s in self.shards:
+            self._starts.append(self._starts[-1] + int(s["rows"]))
+        if self._starts[-1] >= 1 << 31:
+            raise ValueError(f"{path} holds {self._starts[-1]} rows: a search takes fewer than 2^31")
+        self._rows, self._norms = [], []
+        for s in self.shards:
+            n = int(s["rows"])
+            self._rows.append(np.memmap(self.path / f"{s['name']}.f16", dtype="<f2", mode="r",
+                                        shape=(n, self.padded_dim)))
+            if self.metric == "l2":
+                self._norms.append(np.memmap(self.path / f"{s['name']}.norms", dtype="<f4", mode="r", shape=(n,)))
+        self.labels = _ShardLabels(self.path, self.shards, self._starts)
+
+    @classmethod
+    def open(cls, path) -> "ShardedIndex":
+        return cls(path, _read_manifest(path))
+
+    def __len__(self) -> int:
+        return self._starts[-1]
+
+    def read_rows(self, g0: int, g1: int, rows_out: np.ndarray, beta_out: Optional[np.ndarray] = None) -> None:
+        """Global rows [g0, g1) into rows_out fp16 [g1 - g0, padded_dim] and, for l2, -|x|^2 into beta_out."""
+        s, o = bisect.bisect_right(self._starts, g0) - 1, 0
+        while g0 + o < g1:
+            a = g0 + o - self._starts[s]
+            b = min(g1, self._starts[s + 1]) - self._starts[s]
+            np.copyto(rows_out[o:o + b - a], self._rows[s][a:b])
+            if beta_out is not None:
+                np.negative(self._norms[s][a:b], out=beta_out[o:o + b - a])
+            o += b - a
+            s += 1
+
+    def _read_parallel(self, pool, g0: int, g1: int, rows_out: np.ndarray, beta_out: Optional[np.ndarray]) -> None:
+        """read_rows split into REFILL_THREADS pieces run on the pool's threads (numpy copies release the GIL)."""
+        step = -(-(g1 - g0) // REFILL_THREADS)
+        jobs = [pool.submit(self.read_rows, p, min(g1, p + step), rows_out[p - g0:min(g1, p + step) - g0],
+                            None if beta_out is None else beta_out[p - g0:min(g1, p + step) - g0])
+                for p in range(g0, g1, step)]
+        for j in jobs:
+            j.result()
+
+    # ---- search ------------------------------------------------------------------------------------------------------
+    def search(self, queries: torch.Tensor, k: int = 10, device=None,
+               max_device_bytes: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The k nearest rows of each query (fp32/fp16 [Q, E] or [E], any device): (scores fp32 [Q, k], idx int64
+        [Q, k]) on `device` (default: the current CUDA device), as EmbeddingIndex.search returns them."""
+        _check_k(k, len(self))
+        if isinstance(queries, torch.Tensor) and queries.dim() == 1:
+            queries = queries[None]
+        if isinstance(queries, torch.Tensor) and queries.dim() == 2 and queries.shape[1] != self.dim:
+            raise ValueError(f"queries have width {queries.shape[1]}, the index {self.dim}")
+        q = prepare_rows(queries, self.metric, "queries")
+        dev = _cuda_device(device)
+        qn = squared_norms(q) if self.metric == "l2" else None
+        return self._stream(q, qn, k, dev, max_device_bytes)
+
+    def search_all(self, k: int = 10, device=None,
+                   max_device_bytes: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Every row against the index with its own row left out: (scores, idx) [N, k] as search()."""
+        _check_k(k, len(self) - 1)
+        dev = _cuda_device(device)
+        return self._stream(None, None, k, dev, max_device_bytes)
+
+    def _query_block(self, k: int, cap: int, num_sms: int) -> int:
+        """Rows of the database held on the device as queries at once by search_all: all of them if they fit beside
+        a ring of one-tile slots (the database then crosses the host link once), else the largest multiple of 64
+        that fits in half the cap."""
+        N, D = len(self), self.padded_dim
+        if _fixed_device_bytes(N, N, k, D, self.metric, num_sms) + RING_SLOTS * TILE * _row_bytes(D, self.metric) <= cap:
+            return N
+        fits = lambda b: _fixed_device_bytes(b, N, k, D, self.metric, num_sms) <= cap // 2  # noqa: E731
+        lo, hi = 0, N // 64
+        while lo < hi:
+            mid = (lo + hi + 1) // 2
+            lo, hi = (mid, hi) if fits(64 * mid) else (lo, mid - 1)
+        if lo == 0:
+            raise ValueError(f"max_device_bytes = {cap} holds no block of 64 query rows beside the results of "
+                             f"{N} queries: pass more bytes")
+        return 64 * lo
+
+    def _stream(self, q: Optional[torch.Tensor], qn: Optional[torch.Tensor], k: int, dev: torch.device,
+                max_device_bytes: Optional[int]):
+        N, D, l2 = len(self), self.padded_dim, self.metric == "l2"
+        self_rows = q is None
+        Q = N if self_rows else q.shape[0]
+        alpha = 2.0 if l2 else 1.0
+        with torch.cuda.device(dev):
+            num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            cap = int(DEVICE_SHARE * torch.cuda.mem_get_info(dev)[0]) if max_device_bytes is None \
+                else int(max_device_bytes)
+            block = self._query_block(k, cap, num_sms) if self_rows else Q
+            chunk = plan_chunk_rows(block, Q, k, D, self.metric, cap, num_sms)
+            chunk = min(chunk, -(-N // TILE) * TILE)
+            scores = torch.empty((Q, k), dtype=torch.float32, device=dev)
+            idx = torch.empty((Q, k), dtype=torch.int64, device=dev)
+            if Q == 0:
+                return scores, idx
+            scratch = torch.empty(scratch_bytes(block, Q, k, num_sms), dtype=torch.uint8, device=dev)
+            dev_rows = [torch.empty((chunk, D), dtype=torch.float16, device=dev) for _ in range(RING_SLOTS)]
+            dev_beta = [torch.empty(chunk, dtype=torch.float32, device=dev) for _ in range(RING_SLOTS)] if l2 else None
+            host = _host_ring(chunk, D, l2, dev)
+            compute, copy = torch.cuda.current_stream(dev), torch.cuda.Stream(device=dev)
+            copied = [torch.cuda.Event() for _ in range(RING_SLOTS)]
+            consumed = [torch.cuda.Event() for _ in range(RING_SLOTS)]
+            bounds = [(g, min(N, g + chunk)) for g in range(0, N, chunk)]
+            try:
+                with ThreadPoolExecutor(REFILL_THREADS) as pool:
+                    for a0 in range(0, Q, block):
+                        a1 = min(Q, a0 + block)
+                        if self_rows:  # the block's rows and, for l2, |x|^2 (read as -|x|^2, negated exactly)
+                            buf = torch.empty((a1 - a0, D), dtype=torch.float16)
+                            nbuf = torch.empty(a1 - a0, dtype=torch.float32) if l2 else None
+                            self._read_parallel(pool, a0, a1, buf.numpy(), nbuf.numpy() if l2 else None)
+                            qrows, qnorm = buf.to(dev), ((-nbuf).to(dev) if l2 else None)
+                        else:
+                            qrows, qnorm = q.to(dev), (qn.to(dev) if l2 else None)
+                        keys = torch.zeros((a1 - a0, k), dtype=torch.int64, device=dev)
+
+                        def fill(c):  # host slot c % RING_SLOTS <- chunk c, once the slot's last copy has finished
+                            s, (g0, g1) = c % RING_SLOTS, bounds[c]
+                            copied[s].synchronize()
+                            self._read_parallel(pool, g0, g1, host.rows[s].numpy(),
+                                                host.beta[s].numpy() if l2 else None)
+                            with torch.cuda.stream(copy):  # device slot s is free once chunk c - RING_SLOTS is done
+                                copy.wait_event(consumed[s])
+                                n = g1 - g0
+                                dev_rows[s][:n].copy_(host.rows[s][:n], non_blocking=True)
+                                if l2:
+                                    dev_beta[s][:n].copy_(host.beta[s][:n], non_blocking=True)
+                                copied[s].record(copy)
+
+                        fill(0)
+                        for c, (g0, g1) in enumerate(bounds):
+                            s = c % RING_SLOTS
+                            compute.wait_event(copied[s])
+                            for b0 in range(0, a1 - a0, QUERY_BATCH):
+                                b1 = min(a1 - a0, b0 + QUERY_BATCH)
+                                splits = choose_splits(b1 - b0, g1 - g0, num_sms)
+                                knn_accumulate(qrows[b0:b1], dev_rows[s][:g1 - g0], g0, k, keys[b0:b1], scratch,
+                                               dev_beta[s][:g1 - g0] if l2 else None, alpha,
+                                               a0 + b0 if self_rows else -1,
+                                               splits)
+                            consumed[s].record(compute)
+                            if c + 1 < len(bounds):
+                                fill(c + 1)  # the host refills the next slot while the GPU works on this one
+                        knn_decode(keys, scores[a0:a1], idx[a0:a1])
+                        if l2:
+                            sc = scores[a0:a1]
+                            torch.sub(qnorm[:, None], sc, out=sc)
+                            sc.clamp_min_(0).sqrt_()
+                        del keys, qrows
+            finally:  # the host ring is reused by the next call: nothing may still read it
+                compute.synchronize()
+                copy.synchronize()
         return scores, idx

@@ -1,13 +1,18 @@
 """Nearest-neighbour search over extract_cli embeddings (esm_b200.search):
 
     python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out db.pt
-    python -m esm_b200.search_cli query db.pt (--queries EXTRACT_DIR | --all) --k 10 --out hits.tsv
+    python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out db/ [--append]
+    python -m esm_b200.search_cli query db.pt|db/ (--queries EXTRACT_DIR | --all) --k 10 --out hits.tsv
 
 `build` reads the mean representation at --layer of every `<label>.pt` under EXTRACT_DIR (extract_cli --include mean)
-and saves an index. `query` searches it with the mean representations of a second extract_cli directory, which must
-hold the index's layer at the index's width, or with every indexed protein against the others (--all). hits.tsv has
-one line per hit: query, rank (1-based), target, score (cosine similarity, or Euclidean distance for l2).
-Embedding the queries stays in extract_cli, with its model loading and checkpoint checks.
+and saves an index: one file (EmbeddingIndex) when --out ends in .pt, else a sharded index directory (IndexWriter),
+written one shard at a time so that memory stays bounded; --append adds EXTRACT_DIR's proteins to an existing
+directory index as new shards. Both formats hold the rows in label order, so they give the same hits. `query`
+searches an index with the mean representations of a second extract_cli directory, which must hold the index's layer
+at the index's width, or with every indexed protein against the others (--all); a directory index is streamed through
+the GPU (ShardedIndex), so it may be larger than the device's memory. hits.tsv has one line per hit: query, rank
+(1-based), target, score (cosine similarity, or Euclidean distance for l2). Embedding the queries stays in
+extract_cli, with its model loading and checkpoint checks.
 """
 from __future__ import annotations
 
@@ -27,7 +32,10 @@ def create_parser():
     b.add_argument("extract_dir", type=pathlib.Path)
     b.add_argument("--layer", type=int, required=True, help="the representation layer to index")
     b.add_argument("--metric", choices=list(search.METRICS), default="cosine")
-    b.add_argument("--out", type=pathlib.Path, required=True)
+    b.add_argument("--out", type=pathlib.Path, required=True,
+                   help="db.pt: one file; any other path: a sharded index directory")
+    b.add_argument("--append", action="store_true", help="add shards to an existing directory index")
+    b.add_argument("--shard-rows", type=int, default=search.SHARD_ROWS, help="rows per shard of a directory index")
     q = sub.add_parser("query", help="search an index")
     q.add_argument("index", type=pathlib.Path)
     src = q.add_mutually_exclusive_group(required=True)
@@ -51,16 +59,51 @@ def write_hits(path, query_labels, target_labels, scores: torch.Tensor, idx: tor
     return n
 
 
+BUILD_BATCH = 4096  # extract_cli files read per IndexWriter.add
+
+
+def _is_file_index(path: pathlib.Path) -> bool:
+    return path.suffix == ".pt"
+
+
+def build_shards(extract_dir, layer: int, metric: str, out, append: bool, shard_rows: int = search.SHARD_ROWS) -> int:
+    """A sharded index of extract_dir's mean representations in label order, or new shards after an existing index's
+    (append). Files are read twice, once for the labels and once in label order, so memory holds one batch and one
+    shard. Returns the rows added."""
+    out = pathlib.Path(out)
+    exists = (out / search.MANIFEST).exists()
+    if exists and not append:
+        raise ValueError(f"{out} already holds an index: pass --append to add to it")
+    if append and not exists:
+        raise ValueError(f"--append needs an existing directory index at {out}")
+    search._check_metric(metric)
+    items = search._scan_extract_dir(extract_dir, layer, keep_vectors=False)
+    dim = torch.load(items[0][1], map_location="cpu", weights_only=True)["mean_representations"][layer].numel()
+    writer = search.IndexWriter(out, dim, metric, layer, shard_rows)
+    for b0 in range(0, len(items), BUILD_BATCH):
+        batch = items[b0:b0 + BUILD_BATCH]
+        vecs = [torch.load(f, map_location="cpu", weights_only=True)["mean_representations"][layer].reshape(-1).float()
+                for _, f in batch]
+        writer.add(torch.stack(vecs), [l for l, _ in batch])
+    writer.close()
+    return len(items)
+
+
 def run(args) -> int:
     """Returns the number of rows indexed (build) or hit lines written (query)."""
     if args.command == "build":
+        if not _is_file_index(args.out):
+            return build_shards(args.extract_dir, args.layer, args.metric, args.out, args.append, args.shard_rows)
+        if args.append:
+            raise ValueError("--append adds shards to a directory index, not to a .pt file")
         index = search.EmbeddingIndex.from_extract_dir(args.extract_dir, args.layer, args.metric)
         args.out.parent.mkdir(parents=True, exist_ok=True)
         index.save(args.out)
         return len(index)
-    index = search.EmbeddingIndex.load(args.index, device="cpu")
+    sharded = args.index.is_dir()
+    index = search.ShardedIndex.open(args.index) if sharded else search.EmbeddingIndex.load(args.index, device="cpu")
     candidates = len(index) - 1 if args.all else len(index)
-    index._check_k(args.k, candidates)
+    search._check_k(args.k, candidates)
     if args.all:
         qlabels, queries = index.labels, None
     else:
@@ -70,7 +113,8 @@ def run(args) -> int:
         if queries.shape[1] != index.dim:
             raise ValueError(f"the queries have width {queries.shape[1]}, the index {index.dim}")
         search.prepare_rows(queries, index.metric, "queries")
-    index = index.to(torch.device("cuda", torch.cuda.current_device()))
+    if not sharded:
+        index = index.to(torch.device("cuda", torch.cuda.current_device()))
     scores, idx = index.search_all(args.k) if args.all else index.search(queries, args.k)
     args.out.parent.mkdir(parents=True, exist_ok=True)
     return write_hits(args.out, qlabels, index.labels, scores, idx)

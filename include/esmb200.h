@@ -342,6 +342,28 @@ int esmb200_knn_search(const void* queries, int64_t q_ld, int32_t Q, const void*
                        int32_t D, const float* beta, float alpha, int64_t self_offset, int32_t k, int32_t splits,
                        void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream);
 
+/* Streamed k-nearest-neighbour search over a database that arrives in chunks (esm_b200/search.py ShardedIndex).
+ * esmb200_knn_search_accumulate: base fp16 [n, b_ld] holds the database's global rows [row0, row0 + n); everything else
+ * is as for esmb200_knn_search, with j the global index and self_offset in global rows (query i leaves out global row
+ * i + self_offset). keys uint64 [Q, k] (device, dense) is the running list of each query: the top k so far as ranking
+ * keys (ord(s) << 32) | (2^32 - 1 - j), descending, 0 for an empty slot (all zeros before the first chunk). The call
+ * folds the chunk's candidates into it in place, so after every chunk has been passed once, in any order and any
+ * split into chunks, keys hold the same top k esmb200_knn_search returns over the whole database. The chunk may hold
+ * fewer than k candidates. Two launches: the fused GEMM + top-k over `splits` stripes, its thresholds seeded with
+ * each query's running k-th key, then a merge of the stripe lists with the running list. scratch as
+ * esmb200_knn_scratch_bytes(Q, k, splits). 1 <= k <= 128, Q >= 0, n >= 1, row0 >= 0 and row0 + n < 2^31, D, q_ld,
+ * b_ld, splits and the alignments as for esmb200_knn_search, keys non-NULL and 8-byte aligned, else ESMB200_EINVAL
+ * before any launch. Q == 0 launches nothing.
+ * esmb200_knn_decode: keys [Q, k] to out_scores fp32 [Q, k] and out_idx int64 [Q, k] (device, dense), exactly as
+ * esmb200_knn_search writes them (an empty slot decodes to NaN and index 2^32 - 1). Q >= 0, 1 <= k <= 128, non-NULL
+ * pointers, keys and out_idx 8-byte aligned and out_scores 4-byte aligned, else ESMB200_EINVAL before any launch;
+ * Q == 0 launches nothing. One launch. */
+int esmb200_knn_search_accumulate(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld,
+                                  int64_t n, int64_t row0, int32_t D, const float* beta, float alpha,
+                                  int64_t self_offset, int32_t k, int32_t splits, void* scratch, size_t scratch_bytes,
+                                  uint64_t* keys, void* stream);
+int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_scores, int64_t* out_idx, void* stream);
+
 /* Pairwise alignment of proteins by their per-residue embeddings (esm_b200/align.py; the EBA / pLM-BLAST family of
  * methods). A new operation with no reference code. Pair p (of P) has La query rows and Lb target rows, La, Lb >= 1:
  * query rows [q_off[p], q_off[p+1]) and target rows [t_off[p], t_off[p+1]), its similarity S' as [La, Lb] fp32
@@ -507,7 +529,8 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *         14 tied row logits, 15 tied row softmax, 16 tied row update, 17 log_softmax rows (variant scoring),
  *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
  *         and each kernel of esmb200_sample_rows), 21 greedy MSA row selection (each kernel of
- *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search),
+ *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search,
+ *         esmb200_knn_search_accumulate and esmb200_knn_decode),
  *         23 embedding alignment (each kernel of esmb200_align_similarity and esmb200_align) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
