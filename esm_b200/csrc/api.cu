@@ -1903,6 +1903,251 @@ int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_sc
 }
 
 
+extern "C++" {
+namespace {
+// Constants of the inverted-file search (esmb200_ivf_search); include/esmb200.h states them.
+constexpr int kIvfExtraStripes = 64;  // probed lists: sum over the lists of their stripes beyond one is at most this
+constexpr int kIvfAllCtas = 264;      // every list: stripes so that about two waves of a 132-SM H100 run
+constexpr int kIvfMaxLists = 1 << 24;
+
+// The scratch of one esmb200_ivf_search call: every region's byte offset, from the arguments alone.
+struct IvfLayout {
+  bool all;
+  int T, R;          // tiles per stripe; partial lists per query (stride)
+  int64_t P;         // gathered query rows (probed) or Q (all)
+  int64_t max_items;
+  size_t cnt, gstart, istart, slot, pbase, gq, gself, counts, items, qg, keys, bytes;
+};
+
+IvfLayout ivf_layout(int Q, int nprobe, int nlist, int64_t N, int D, int k) {
+  IvfLayout L{};
+  L.all = nprobe == nlist;
+  const int64_t tiles = (N + knn_cfg::BLOCK_N - 1) / knn_cfg::BLOCK_N;
+  const int64_t blocks = ((int64_t)Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  if (L.all) {
+    int64_t S = blocks > 0 ? (kIvfAllCtas + blocks - 1) / blocks : 1;
+    S = S < tiles ? S : tiles;
+    L.T = (int)((tiles + S - 1) / S);
+    L.R = (int)((tiles + L.T - 1) / L.T);  // the stripes of T tiles
+    L.P = Q;
+    L.max_items = blocks * L.R;
+  } else {
+    const int64_t total = tiles + nlist;  // at least the sum over the lists of their tiles
+    L.T = (int)((total + kIvfExtraStripes - 1) / kIvfExtraStripes);
+    L.R = nprobe + kIvfExtraStripes;
+    L.P = (int64_t)Q * nprobe;
+    L.max_items = L.P / knn_cfg::BLOCK_M + (nlist < L.P ? nlist : L.P) + blocks * kIvfExtraStripes;
+  }
+  size_t o = 0;
+  auto take = [&](size_t bytes) {
+    const size_t at = o;
+    o += (bytes + 255) / 256 * 256;
+    return at;
+  };
+  const size_t P = (size_t)L.P, nl = L.all ? 0 : (size_t)nlist + 1;
+  L.cnt = take(nl * 4);
+  L.gstart = take(nl * 4);
+  L.istart = take(nl * 4);
+  L.slot = take(L.all ? 0 : P * 4);
+  L.pbase = take(P * 4);
+  L.gq = take(L.all ? 0 : P * 4);
+  L.gself = take(L.all ? 0 : P * 8);
+  L.counts = take((size_t)Q * 4);
+  L.items = take((size_t)L.max_items * sizeof(IvfItem));
+  L.qg = take(L.all ? 0 : P * (size_t)D * 2);
+  L.keys = take((size_t)Q * L.R * (size_t)k * 8);
+  L.bytes = o < 256 ? 256 : o;
+  return L;
+}
+
+// the refusals the scratch size and the search share
+int ivf_check(int32_t Q, int32_t nprobe, int32_t nlist, int64_t N, int32_t D, int32_t k, const char* what) {
+  const std::string w(what);
+  if (k < 1 || k > knn_cfg::MAX_K) return fail(ESMB200_EINVAL, w + " needs 1 <= k <= 128");
+  if (Q < 0 || N < 1 || N > INT32_MAX) return fail(ESMB200_EINVAL, w + " needs Q >= 0 and 1 <= N < 2^31");
+  if (nlist < 1 || nlist > kIvfMaxLists || nlist > N) return fail(ESMB200_EINVAL, w + " needs 1 <= nlist <= min(N, 2^24)");
+  if (nprobe != nlist && (nprobe < 1 || nprobe > knn_cfg::MAX_K))
+    return fail(ESMB200_EINVAL, w + " needs 1 <= nprobe <= min(nlist, 128) or nprobe == nlist");
+  if (nprobe > nlist) return fail(ESMB200_EINVAL, w + " needs 1 <= nprobe <= min(nlist, 128) or nprobe == nlist");
+  if (D < 64 || D % 64 != 0) return fail(ESMB200_EINVAL, w + " needs D % 64 == 0");
+  if (nprobe != nlist && (int64_t)Q * nprobe > INT32_MAX / 2)
+    return fail(ESMB200_EINVAL, w + " needs Q * nprobe < 2^30");
+  // partial lists are indexed in int32: q * R + s for every query q and s < R
+  if ((int64_t)Q * ivf_layout(Q, nprobe, nlist, N, D, k).R > INT32_MAX)
+    return fail(ESMB200_EINVAL, w + " needs Q * R < 2^31 partial lists (R = nprobe + 64, or the stripes of every list)");
+  return ESMB200_OK;
+}
+}  // namespace
+}  // extern "C++"
+
+int esmb200_ivf_scratch_bytes(int32_t Q, int32_t nprobe, int32_t nlist, int64_t N, int32_t D, int32_t k, size_t* out) {
+  if (!out) return fail(ESMB200_EINVAL, "null argument");
+  int rc = ivf_check(Q, nprobe, nlist, N, D, k, "ivf_scratch_bytes");
+  if (rc) return rc;
+  *out = ivf_layout(Q, nprobe, nlist, N, D, k).bytes;
+  return ESMB200_OK;
+}
+
+int esmb200_ivf_search(const void* queries, int64_t q_ld, int32_t Q, const void* rows, int64_t b_ld, int64_t N,
+                       const int64_t* ids, const int64_t* offsets, int32_t nlist, int32_t D, const float* beta,
+                       float alpha, const int32_t* probes, int32_t nprobe, const int64_t* self_ids, int32_t k,
+                       void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream) {
+  int rc = ivf_check(Q, nprobe, nlist, N, D, k, "ivf_search");
+  if (rc) return rc;
+  const bool all = nprobe == nlist;
+  if (q_ld < D || b_ld < D || q_ld % 8 != 0 || b_ld % 8 != 0)
+    return fail(ESMB200_EINVAL, "ivf_search needs q_ld, b_ld >= D and multiples of 8 (16-byte rows for TMA)");
+  if (!queries || !rows || !ids || !offsets || !scratch || !out_scores || !out_idx)
+    return fail(ESMB200_EINVAL, "null argument");
+  if (all != (probes == nullptr))
+    return fail(ESMB200_EINVAL, "ivf_search needs probes NULL exactly when nprobe == nlist (every list)");
+  if (reinterpret_cast<uintptr_t>(queries) % 16 != 0 || reinterpret_cast<uintptr_t>(rows) % 16 != 0)
+    return fail(ESMB200_EINVAL, "ivf_search needs 16-byte aligned queries and rows (TMA)");
+  if (reinterpret_cast<uintptr_t>(ids) % 8 != 0 || reinterpret_cast<uintptr_t>(offsets) % 8 != 0 ||
+      reinterpret_cast<uintptr_t>(self_ids) % 8 != 0 || reinterpret_cast<uintptr_t>(probes) % 4 != 0 ||
+      reinterpret_cast<uintptr_t>(beta) % 4 != 0)
+    return fail(ESMB200_EINVAL, "ivf_search needs 8-byte aligned ids, offsets and self_ids, 4-byte aligned probes and beta");
+  if (reinterpret_cast<uintptr_t>(out_scores) % 4 != 0 || reinterpret_cast<uintptr_t>(out_idx) % 8 != 0)
+    return fail(ESMB200_EINVAL, "ivf_search needs 4-byte aligned out_scores and 8-byte aligned out_idx");
+  if (reinterpret_cast<uintptr_t>(scratch) % 256 != 0) return fail(ESMB200_EINVAL, "scratch must be 256-byte aligned");
+  const IvfLayout L = ivf_layout(Q, nprobe, nlist, N, D, k);
+  if (scratch_bytes < L.bytes) return fail(ESMB200_EINVAL, "scratch smaller than esmb200_ivf_scratch_bytes");
+  if (Q == 0) return ESMB200_OK;
+  if ((rc = check_device())) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* sc = static_cast<uint8_t*>(scratch);
+  int* cnt = reinterpret_cast<int*>(sc + L.cnt);
+  int* gstart = reinterpret_cast<int*>(sc + L.gstart);
+  int* istart = reinterpret_cast<int*>(sc + L.istart);
+  int* slot = reinterpret_cast<int*>(sc + L.slot);
+  int* pbase = reinterpret_cast<int*>(sc + L.pbase);
+  int* gq = reinterpret_cast<int*>(sc + L.gq);
+  int64_t* gself = reinterpret_cast<int64_t*>(sc + L.gself);
+  int* counts = reinterpret_cast<int*>(sc + L.counts);
+  IvfItem* items = reinterpret_cast<IvfItem*>(sc + L.items);
+  __half* qg = reinterpret_cast<__half*>(sc + L.qg);
+  int64_t n_items;
+  const void* a_rows = queries;  // the query rows the list scan reads, and their leading dimension
+  int64_t a_ld = q_ld;
+  if (all) {
+    n_items = ((int64_t)Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M * L.R;
+    ProfScope ps(T_KNN, st);
+    const int64_t b = (n_items > Q ? n_items : Q) / 256 + 1;
+    ivf_all_items_kernel<<<(unsigned)(b < 1024 ? b : 1024), 256, 0, st>>>(Q, N, L.R, L.T, items, pbase, counts);
+    CK(cudaGetLastError());
+  } else {
+    CK(cudaMemsetAsync(cnt, 0, (size_t)nlist * 4, st));
+    const int64_t P = L.P;
+    {
+      ProfScope ps(T_KNN, st);
+      const int64_t b = (P + 255) / 256;
+      ivf_count_kernel<<<(unsigned)(b < 4096 ? b : 4096), 256, 0, st>>>(probes, P, nprobe, nlist, cnt, slot);
+      CK(cudaGetLastError());
+    }
+    {
+      ProfScope ps(T_KNN, st);
+      ivf_scan_kernel<<<1, 512, 0, st>>>(cnt, offsets, nlist, N, L.T, gstart, istart);
+      CK(cudaGetLastError());
+    }
+    int host_items = 0;  // the one host synchronisation: the grid of the list scan
+    CK(cudaMemcpyAsync(&host_items, istart + nlist, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    n_items = host_items;
+    if (n_items > L.max_items) return fail(ESMB200_EINVAL, "ivf_search: offsets that do not partition [0, N)");
+    {
+      ProfScope ps(T_KNN, st);
+      ivf_place_kernel<<<(unsigned)((Q + 255) / 256), 256, 0, st>>>(probes, slot, gstart, offsets, Q, nprobe, nlist, N,
+                                                                    L.T, L.R, self_ids, gq, gself, pbase, counts);
+      CK(cudaGetLastError());
+    }
+    {
+      ProfScope ps(T_KNN, st);
+      ivf_items_kernel<<<(unsigned)((nlist + 255) / 256), 256, 0, st>>>(cnt, gstart, istart, offsets, nlist, N, L.T,
+                                                                        items);
+      CK(cudaGetLastError());
+    }
+    {
+      ProfScope ps(T_KNN, st);
+      const int64_t b = (P * (D / 8) + 255) / 256;
+      ivf_gather_kernel<<<(unsigned)(b < 8192 ? b : 8192), 256, 0, st>>>(static_cast<const __half*>(queries), q_ld,
+                                                                         gq, gstart + nlist, D, qg);
+      CK(cudaGetLastError());
+    }
+    a_rows = qg;
+    a_ld = D;
+  }
+  if (n_items > 0) {
+    CUtensorMap tq, tx;
+    if ((rc = make_tmap_f16(&tq, a_rows, (uint64_t)L.P, (uint64_t)D, (uint64_t)a_ld, knn_cfg::BLOCK_M))) return rc;
+    if ((rc = make_tmap_f16(&tx, rows, (uint64_t)N, (uint64_t)D, (uint64_t)b_ld, knn_cfg::BLOCK_N))) return rc;
+    KnnParams p{};
+    p.Q = (int)L.P;
+    p.D = D;
+    p.k = k;
+    p.N = N;
+    p.tiles_per_stripe = L.T;
+    p.query_blocks = 1;
+    p.beta = beta;
+    p.alpha = alpha;
+    p.self_offset = -1;
+    p.row0 = 0;
+    p.seed = nullptr;
+    p.keys = reinterpret_cast<unsigned long long*>(sc + L.keys);
+    p.items = items;
+    p.ids = ids;
+    p.gself = all ? self_ids : gself;
+    p.pbase = pbase;
+    CK(cudaFuncSetAttribute(knn_topk_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            knn_cfg::SMEM_BYTES));
+    ProfScope ps(T_KNN, st);
+    knn_topk_kernel<false, true><<<(unsigned)n_items, knn_cfg::NUM_THREADS, knn_cfg::SMEM_BYTES, st>>>(tq, tx, p);
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_KNN, st);
+    knn_merge_kernel<2, false, true><<<(unsigned)Q, 256, 0, st>>>(
+        reinterpret_cast<const unsigned long long*>(sc + L.keys), Q, k, L.R, nullptr, out_scores, out_idx, counts);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
+int esmb200_kmeans_means(const void* rows, int64_t ld, int64_t n, int32_t D, const int64_t* assign, int32_t nlist,
+                         int64_t* sums, float* means_out, int64_t* counts_out, void* stream) {
+  if (n < 0 || n > (int64_t(1) << 23))
+    return fail(ESMB200_EINVAL, "kmeans_means needs 0 <= n <= 2^23 (so no int64 column sum can overflow)");
+  if (D < 8 || D % 8 != 0 || ld < D || ld % 8 != 0)
+    return fail(ESMB200_EINVAL, "kmeans_means needs D % 8 == 0 and ld >= D, a multiple of 8");
+  if (nlist < 1 || nlist > kIvfMaxLists) return fail(ESMB200_EINVAL, "kmeans_means needs 1 <= nlist <= 2^24");
+  if (!rows || !assign || !sums || !means_out || !counts_out) return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(rows) % 16 != 0 || reinterpret_cast<uintptr_t>(assign) % 8 != 0 ||
+      reinterpret_cast<uintptr_t>(sums) % 8 != 0 || reinterpret_cast<uintptr_t>(counts_out) % 8 != 0 ||
+      reinterpret_cast<uintptr_t>(means_out) % 4 != 0)
+    return fail(ESMB200_EINVAL, "kmeans_means needs 16-byte aligned rows, 8-byte aligned assign, sums and counts");
+  if ((int64_t)nlist * D > (int64_t(1) << 40)) return fail(ESMB200_EINVAL, "kmeans_means needs nlist * D <= 2^40");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CK(cudaMemsetAsync(sums, 0, (size_t)nlist * D * 8, st));
+  CK(cudaMemsetAsync(counts_out, 0, (size_t)nlist * 8, st));
+  if (n > 0) {
+    ProfScope ps(T_KNN, st);
+    const int64_t b = (n + 7) / 8;
+    kmeans_sum_kernel<<<(unsigned)(b < 8192 ? b : 8192), 256, 0, st>>>(
+        static_cast<const __half*>(rows), ld, n, D, assign, nlist, reinterpret_cast<unsigned long long*>(sums),
+        reinterpret_cast<unsigned long long*>(counts_out));
+    CK(cudaGetLastError());
+  }
+  {
+    ProfScope ps(T_KNN, st);
+    const int64_t b = ((int64_t)nlist * D + 255) / 256;
+    kmeans_mean_kernel<<<(unsigned)(b < 8192 ? b : 8192), 256, 0, st>>>(
+        reinterpret_cast<const long long*>(sums), reinterpret_cast<const long long*>(counts_out), nlist, D, means_out);
+    CK(cudaGetLastError());
+  }
+  return ESMB200_OK;
+}
+
 size_t esmb200_align_scratch_bytes(int32_t P, int64_t n_q, int64_t n_t, int64_t n_cells) {
   if (P < 0 || n_q < 0 || n_t < 0 || n_cells < 0) return 0;
   return align_scratch(P, n_q, n_t, n_cells).bytes;

@@ -60,6 +60,12 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + LIST_BYTES + QUEUE_BYTES + BLO
 static_assert(SMEM_BYTES <= 232448, "knn_topk_kernel shared memory");
 }  // namespace knn_cfg
 
+// A list-scan work item: query rows [g0, g1) (at most BLOCK_M, all probing one list) against stored rows [r0, r1) (a
+// stripe of that list, tiles starting at r0); the rows' partial lists go to keys[pbase[g] + stripe].
+struct IvfItem {
+  int32_t g0, g1, r0, r1, stripe;
+};
+
 struct KnnParams {
   int Q, D, k;
   int64_t N;
@@ -70,7 +76,12 @@ struct KnnParams {
   int64_t self_offset;   // < 0: none; in global rows
   int64_t row0;          // global index of the chunk's row 0 (0 for esmb200_knn_search)
   const unsigned long long* seed;  // running list [Q, k] whose k-th key seeds the thresholds, or nullptr
-  unsigned long long* keys;  // scratch [splits, Q, k]
+  unsigned long long* keys;  // scratch [splits, Q, k]; list scan: [Q, R, k] (the query's partial lists, ragged)
+  // list scan (LISTS) only
+  const IvfItem* items;  // one work item per CTA
+  const int64_t* ids;           // [N] original row of each stored row: the key's index
+  const int64_t* gself;         // [query rows] the original row each query row leaves out (< 0: none), or nullptr
+  const int* pbase;             // [query rows] partial-list index of the row's stripe 0 (< 0: the row writes nothing)
 };
 
 __device__ __forceinline__ unsigned long long knn_key(float s, int64_t j) {
@@ -176,8 +187,10 @@ __device__ __forceinline__ void knn_merge_row(unsigned long long* list, unsigned
 }
 
 // STREAM: a chunk of a streamed search (row0 and the seeded thresholds); without it the kernel is the resident one,
-// with no code for either.
-template <bool STREAM>
+// with no code for either.  LISTS: the inverted-file list scan (esmb200_ivf_search): CTA b runs work item items[b],
+// columns outside [r0, r1) and query rows outside [g0, g1) produce no candidate, a key's index is ids[j] and a row
+// leaves out the column whose id is gself[row]; without it none of this is compiled.
+template <bool STREAM, bool LISTS = false>
 __global__ void __launch_bounds__(knn_cfg::NUM_THREADS, 1)
 knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                 const KnnParams p) {
@@ -196,11 +209,16 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
   const int k = p.k;
   const int64_t row0 = STREAM ? p.row0 : 0;
-  const int qb = blockIdx.x % p.query_blocks, stripe = blockIdx.x / p.query_blocks;
-  const int q0 = qb * BLOCK_M;
-  const int tiles = (int)((p.N + BLOCK_N - 1) / BLOCK_N);
-  const int t_begin = stripe * p.tiles_per_stripe;
-  const int t_end = min(tiles, t_begin + p.tiles_per_stripe);
+  IvfItem item = {0, 0, 0, 0, 0};
+  if (LISTS) item = p.items[blockIdx.x];
+  const int qb = blockIdx.x % p.query_blocks, stripe = LISTS ? item.stripe : blockIdx.x / p.query_blocks;
+  const int q0 = LISTS ? item.g0 : qb * BLOCK_M;
+  const int q_end = LISTS ? item.g1 : p.Q;
+  const int64_t c0 = LISTS ? item.r0 : 0;       // the column of tile 0
+  const int64_t c_end = LISTS ? item.r1 : p.N;  // columns >= c_end are no candidates
+  const int tiles = LISTS ? (item.r1 - item.r0 + BLOCK_N - 1) / BLOCK_N : (int)((p.N + BLOCK_N - 1) / BLOCK_N);
+  const int t_begin = LISTS ? 0 : stripe * p.tiles_per_stripe;
+  const int t_end = LISTS ? tiles : min(tiles, t_begin + p.tiles_per_stripe);
   const int num_kb = p.D / BLOCK_K;
 
   if (threadIdx.x == 0) {
@@ -230,7 +248,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           while (!mbar_try_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1)) __nanosleep(64);
           mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
           tma_load_2d(smem_a + s * A_STAGE_BYTES, &tmap_q, &full_bar[s], kb * BLOCK_K, q0);
-          tma_load_2d(smem_b + s * B_STAGE_BYTES, &tmap_x, &full_bar[s], kb * BLOCK_K, t * BLOCK_N);
+          tma_load_2d(smem_b + s * B_STAGE_BYTES, &tmap_x, &full_bar[s], kb * BLOCK_K, (int)c0 + t * BLOCK_N);
         }
       }
     }
@@ -249,13 +267,16 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
   int rl[2];           // the thread's rows of the block
   bool rvalid[2];
-  int64_t excl[2];     // the excluded column of each row, chunk-local (negative: none)
+  int64_t excl[2];     // the excluded column of each row, chunk-local (negative: none); LISTS: the excluded id
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     rl[hr] = (int)(warp * 16 + g + 8 * hr);
     const int q = q0 + rl[hr];
-    rvalid[hr] = q < p.Q;
-    excl[hr] = p.self_offset >= 0 ? (int64_t)q + p.self_offset - row0 : -1;
+    rvalid[hr] = q < q_end;
+    if (LISTS)
+      excl[hr] = (p.gself != nullptr && rvalid[hr]) ? p.gself[q] : -1;
+    else
+      excl[hr] = p.self_offset >= 0 ? (int64_t)q + p.self_offset - row0 : -1;
   }
 
   // every row's queue into its list: warp w takes rows 16 w .. 16 w + 15
@@ -265,7 +286,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   };
 
   for (int t = t_begin; t < t_end; ++t) {
-    const int64_t n0 = (int64_t)t * BLOCK_N;
+    const int64_t n0 = c0 + (int64_t)t * BLOCK_N;
     for (int kb = 0; kb < num_kb; ++kb, ++it) {
       const uint32_t s = it % STAGES;
       // plain try_wait loop: any call in a wgmma kernel makes ptxas serialise every wgmma (C7510)
@@ -295,6 +316,13 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int64_t j = n0 + 8 * i + 2 * (int)c + e;
+          if (LISTS) {  // index 0 gives a score's largest key: a superset of the survivors, without reading ids
+            const float b = (p.beta != nullptr && j < c_end) ? __ldg(p.beta + j) : 0.f;
+            const bool in = j < c_end;
+            any |= in && rvalid[0] && knn_key(fmaf(p.alpha, acc[4 * i + e], b) + 0.0f, 0) > th0;
+            any |= in && rvalid[1] && knn_key(fmaf(p.alpha, acc[4 * i + 2 + e], b) + 0.0f, 0) > th1;
+            continue;
+          }
           const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
           const bool in = j < p.N;
           any |= in && rvalid[0] && j != excl[0] && knn_key(fmaf(p.alpha, acc[4 * i + e], b) + 0.0f, j + row0) > th0;
@@ -314,6 +342,24 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int64_t j = n0 + 8 * i + 2 * (int)c + e;
+          if (LISTS) {  // ids[j] is read only for a score that can pass the threshold
+            const float b = (p.beta != nullptr && j < c_end) ? __ldg(p.beta + j) : 0.f;
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const float sc = fmaf(p.alpha, acc[4 * i + 2 * hr + e], b) + 0.0f;
+              const unsigned long long th = hr ? th1 : th0;
+              if (j < c_end && rvalid[hr] && knn_key(sc, 0) > th) {
+                const int64_t id = __ldg(reinterpret_cast<const long long*>(p.ids) + j);
+                const unsigned long long key = knn_key(sc, id);
+                if (id != excl[hr] && key > th) {
+                  const int pos = atomicAdd(s_cnt + rl[hr], 1);
+                  s_queue[rl[hr] * QCAP + pos] = key;
+                  full |= pos >= QCAP - CHUNK;
+                }
+              }
+            }
+            continue;
+          }
           const float b = (p.beta != nullptr && j < p.N) ? __ldg(p.beta + j) : 0.f;
 #pragma unroll
           for (int hr = 0; hr < 2; ++hr) {
@@ -338,8 +384,9 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   // ---- the stripe's lists: warp w writes rows 16 w ..
   for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r) {
     const int q = q0 + r;
-    if (q >= p.Q) break;
-    unsigned long long* dst = p.keys + ((size_t)stripe * p.Q + q) * k;
+    if (q >= q_end) break;
+    if (LISTS && p.pbase[q] < 0) continue;
+    unsigned long long* dst = LISTS ? p.keys + ((size_t)p.pbase[q] + stripe) * k : p.keys + ((size_t)stripe * p.Q + q) * k;
     for (int i = (int)lane; i < k; i += 32) dst[i] = s_list[r * MAX_K + i];
   }
 }
@@ -347,23 +394,25 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 // One block per query: k rounds, each taking the largest head of the lists (keys are distinct, so the winner is unique
 // unless it is an empty slot) and advancing that list.  The lists are the S stripe lists and, with ACC, the running
 // list run[q] as list S; thread t owns lists t, t + blockDim, ... (at most M).  Without ACC the winners are decoded to
-// out_scores / out_idx; with ACC they are written back to run[q] as keys.
-template <int M, bool ACC>
+// out_scores / out_idx; with ACC they are written back to run[q] as keys.  RAGGED (esmb200_ivf_search): query q has
+// counts[q] lists, at keys[q * S + s] (S the per-query stride), and an empty slot decodes to NaN and index -1.
+template <int M, bool ACC, bool RAGGED = false>
 __global__ void __launch_bounds__(256)
 knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int S, unsigned long long* run,
-                 float* __restrict__ out_scores, int64_t* __restrict__ out_idx) {
+                 float* __restrict__ out_scores, int64_t* __restrict__ out_idx, const int* counts = nullptr) {
   __shared__ unsigned long long red_key[2][8];
   __shared__ int red_s[2][8];
   __shared__ unsigned long long s_run[ACC ? knn_cfg::MAX_K : 1];
   const int q = blockIdx.x;
   const int nt = blockDim.x, warp = threadIdx.x / 32, nw = nt / 32;
-  const int L = ACC ? S + 1 : S;
+  const int L = RAGGED ? counts[q] : ACC ? S + 1 : S;
   if (ACC) {
     for (int i = threadIdx.x; i < k; i += nt) s_run[i] = run[(size_t)q * k + i];
     __syncthreads();
   }
   auto fetch = [&](int s, int pos) -> unsigned long long {
     if (ACC && s == S) return s_run[pos];
+    if (RAGGED) return keys[((size_t)q * S + s) * k + pos];
     return keys[((size_t)s * Q + q) * k + pos];
   };
   unsigned long long head[M];
@@ -418,6 +467,7 @@ knn_merge_kernel(const unsigned long long* __restrict__ keys, int Q, int k, int 
         run[(size_t)q * k + r] = best;
       else
         knn_decode_key(best, out_scores + (size_t)q * k + r, out_idx + (size_t)q * k + r);
+      if (RAGGED && best == 0ull) out_idx[(size_t)q * k + r] = -1;
     }
   }
 }
@@ -428,6 +478,183 @@ knn_decode_kernel(const unsigned long long* __restrict__ keys, int64_t n, float*
                   int64_t* __restrict__ out_idx) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     knn_decode_key(keys[i], out_scores + i, out_idx + i);
+}
+
+// ---- inverted-file search (esmb200_ivf_search): the grouping of (query, probe) pairs into list-scan work items --------
+// A list's stripes: T 256-row tiles each, so S_l = ceil(ceil(len_l / 256) / T).
+__device__ __forceinline__ int ivf_stripes(const int64_t* offsets, int l, int64_t N, int T) {
+  const int64_t a = min(max(offsets[l], (int64_t)0), N), b = min(max(offsets[l + 1], a), N);
+  const int64_t tiles = (b - a + knn_cfg::BLOCK_N - 1) / knn_cfg::BLOCK_N;
+  return (int)((tiles + T - 1) / T);
+}
+
+// each pair (query, probe) takes the next position in its list's group; an entry outside [0, nlist), or one that
+// repeats an earlier entry of its row, probes nothing (slot -1), so a list is scanned at most once per query.  The
+// positions depend on the order the atomics land in, which changes no result: the top k under the key order does not
+// depend on the order candidates are seen in.
+__global__ void __launch_bounds__(256)
+ivf_count_kernel(const int32_t* __restrict__ probes, int64_t P, int nprobe, int nlist, int* __restrict__ cnt,
+                 int* __restrict__ slot) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < P; i += (int64_t)gridDim.x * blockDim.x) {
+    const int l = probes[i];
+    bool ok = l >= 0 && l < nlist;
+    for (int64_t j = i - i % nprobe; ok && j < i; ++j) ok = probes[j] != l;
+    slot[i] = ok ? atomicAdd(cnt + l, 1) : -1;
+  }
+}
+
+// one block of 512 threads: gstart = exclusive scan of the group sizes, istart = exclusive scan of the work items per list
+// (ceil(cnt / 64) query blocks times the list's stripes); both [nlist + 1]
+__global__ void __launch_bounds__(512)
+ivf_scan_kernel(const int* __restrict__ cnt, const int64_t* __restrict__ offsets, int nlist, int64_t N, int T,
+                int* __restrict__ gstart, int* __restrict__ istart) {
+  __shared__ int s_g[512], s_i[512];
+  const int per = (nlist + 511) / 512, l0 = threadIdx.x * per, l1 = min(nlist, l0 + per);
+  int sg = 0, si = 0;
+  for (int l = l0; l < l1; ++l) {
+    sg += cnt[l];
+    si += (cnt[l] + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M * ivf_stripes(offsets, l, N, T);
+  }
+  s_g[threadIdx.x] = sg;
+  s_i[threadIdx.x] = si;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int ag = 0, ai = 0;
+    for (int t = 0; t < 512; ++t) {
+      const int g = s_g[t], i = s_i[t];
+      s_g[t] = ag;
+      s_i[t] = ai;
+      ag += g;
+      ai += i;
+    }
+    gstart[nlist] = ag;
+    istart[nlist] = ai;
+  }
+  __syncthreads();
+  sg = s_g[threadIdx.x];
+  si = s_i[threadIdx.x];
+  for (int l = l0; l < l1; ++l) {
+    gstart[l] = sg;
+    istart[l] = si;
+    sg += cnt[l];
+    si += (cnt[l] + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M * ivf_stripes(offsets, l, N, T);
+  }
+}
+
+// one thread per query: its gathered rows (query index, excluded id) and their partial lists, R per query, in probe
+// order; counts[q] = the query's partial lists.  A pair whose stripes would pass R (only with offsets that do not
+// partition [0, N)) writes nothing.
+__global__ void __launch_bounds__(256)
+ivf_place_kernel(const int32_t* __restrict__ probes, const int* __restrict__ slot, const int* __restrict__ gstart,
+                 const int64_t* __restrict__ offsets, int Q, int nprobe, int nlist, int64_t N, int T, int R,
+                 const int64_t* __restrict__ self_ids, int* __restrict__ gq, int64_t* __restrict__ gself,
+                 int* __restrict__ pbase, int* __restrict__ counts) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= Q) return;
+  int run = 0;
+  for (int i = 0; i < nprobe; ++i) {
+    const int64_t pr = (int64_t)q * nprobe + i;
+    const int l = probes[pr];
+    if (slot[pr] < 0) continue;
+    const int g = gstart[l] + slot[pr], S = ivf_stripes(offsets, l, N, T);
+    gq[g] = q;
+    gself[g] = self_ids != nullptr ? self_ids[q] : -1;
+    pbase[g] = run + S <= R ? q * R + run : -1;
+    run += run + S <= R ? S : 0;
+  }
+  counts[q] = run;
+}
+
+// one thread per list: its work items, query block major, at istart[l]
+__global__ void __launch_bounds__(256)
+ivf_items_kernel(const int* __restrict__ cnt, const int* __restrict__ gstart, const int* __restrict__ istart,
+                 const int64_t* __restrict__ offsets, int nlist, int64_t N, int T, IvfItem* __restrict__ items) {
+  const int l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l >= nlist) return;
+  const int S = ivf_stripes(offsets, l, N, T), nb = (cnt[l] + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  const int64_t a = min(max(offsets[l], (int64_t)0), N), b = min(max(offsets[l + 1], a), N);
+  const int64_t span = (int64_t)T * knn_cfg::BLOCK_N;
+  for (int qb = 0; qb < nb; ++qb)
+    for (int s = 0; s < S; ++s) {
+      IvfItem it;
+      it.g0 = gstart[l] + qb * knn_cfg::BLOCK_M;
+      it.g1 = min(gstart[l] + cnt[l], it.g0 + knn_cfg::BLOCK_M);
+      it.r0 = (int)(a + s * span);
+      it.r1 = (int)min(b, a + (s + 1) * span);
+      it.stripe = s;
+      items[istart[l] + qb * S + s] = it;
+    }
+}
+
+// every list at once (nprobe == nlist): the stored rows in S stripes of T tiles, stripe major as knn_topk_kernel's
+// grid, and each query's S partial lists at q * S
+__global__ void __launch_bounds__(256)
+ivf_all_items_kernel(int Q, int64_t N, int S, int T, IvfItem* __restrict__ items, int* __restrict__ pbase,
+                     int* __restrict__ counts) {
+  const int blocks = (Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  const int64_t span = (int64_t)T * knn_cfg::BLOCK_N;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < blocks * S; i += gridDim.x * blockDim.x) {
+    const int qb = i % blocks, s = i / blocks;
+    IvfItem it;
+    it.g0 = qb * knn_cfg::BLOCK_M;
+    it.g1 = min(Q, it.g0 + knn_cfg::BLOCK_M);
+    it.r0 = (int)min(N, s * span);
+    it.r1 = (int)min(N, (s + 1) * span);
+    it.stripe = s;
+    items[i] = it;
+  }
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < Q; q += gridDim.x * blockDim.x) {
+    pbase[q] = q * S;
+    counts[q] = S;
+  }
+}
+
+// gathered query rows: dst [P, D] (dense) row g = src row gq[g] for the *placed rows (pairs with a list); 16-byte copies
+__global__ void __launch_bounds__(256)
+ivf_gather_kernel(const __half* __restrict__ src, int64_t ld, const int* __restrict__ gq, const int* __restrict__ placed,
+                  int D, __half* __restrict__ dst) {
+  const int per = D / 8;
+  const int64_t P = *placed;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < P * per; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t g = i / per;
+    const int c = (int)(i % per);
+    reinterpret_cast<uint4*>(dst + g * D)[c] = reinterpret_cast<const uint4*>(src + (int64_t)gq[g] * ld)[c];
+  }
+}
+
+// ---- k-means means (esmb200_kmeans_means) ---------------------------------------------------------------------------
+// Every fp16 value is an integer multiple of 2^-24, so x * 2^24 is an exact integer and the member sum per column is
+// an exact int64 whatever order the atomics land in.  One warp per row.
+__global__ void __launch_bounds__(256)
+kmeans_sum_kernel(const __half* __restrict__ rows, int64_t ld, int64_t n, int D, const int64_t* __restrict__ assign,
+                  int nlist, unsigned long long* __restrict__ sums, unsigned long long* __restrict__ counts) {
+  const int lane = threadIdx.x % 32;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x / 32);
+  for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < n; r += warps) {
+    const int64_t c = assign[r];
+    if (c < 0 || c >= nlist) continue;
+    if (lane == 0) atomicAdd(counts + c, 1ull);
+    for (int v = lane; v < D / 8; v += 32) {
+      const uint4 u = reinterpret_cast<const uint4*>(rows + r * ld)[v];
+      const __half* h = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const long long x = __float2ll_rn(__half2float(h[e]) * 16777216.0f);
+        if (x != 0) atomicAdd(sums + c * D + 8 * v + e, (unsigned long long)x);
+      }
+    }
+  }
+}
+
+// means[c, j] = fp32(((double)S / count) * 2^-24), 0 for an empty cluster
+__global__ void __launch_bounds__(256)
+kmeans_mean_kernel(const long long* __restrict__ sums, const long long* __restrict__ counts, int nlist, int D,
+                   float* __restrict__ means) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (int64_t)nlist * D;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const long long cnt = counts[i / D];
+    means[i] = cnt > 0 ? __double2float_rn(__ddiv_rn((double)sums[i], (double)cnt) * 0x1p-24) : 0.f;
+  }
 }
 
 }  // namespace esmb200

@@ -17,6 +17,10 @@ smaller index. Rows are zero-padded to a multiple of 64 columns, which changes n
 Databases larger than the GPU: IndexWriter writes a sharded index directory, and ShardedIndex memory-maps it and
 streams it through the GPU with the same results (see ShardedIndex).
 
+Faster, approximate search: IVFIndex clusters the rows around nlist k-means centroids and scans only the nprobe lists
+nearest each query, exactly over those lists, with the same scores and tie rule; nprobe == nlist gives EmbeddingIndex's
+results bit for bit (see IVFIndex).
+
 One search is two kernel launches per batch of queries (esmb200_knn_search, include/esmb200.h): a wgmma GEMM whose
 epilogue keeps each query's top k, and a merge of the database stripes' lists. The [Q, N] score matrix is never
 stored, and a query's result does not depend on the other queries or on how the database is split.
@@ -213,7 +217,10 @@ class EmbeddingIndex:
     @classmethod
     def load(cls, path, device=None) -> "EmbeddingIndex":
         """An index saved by save(), on `device` (default: the current CUDA device if there is one, else the CPU)."""
-        obj = torch.load(path, map_location="cpu", weights_only=True)
+        return cls._from_saved(torch.load(path, map_location="cpu", weights_only=True), path, device)
+
+    @classmethod
+    def _from_saved(cls, obj, path, device) -> "EmbeddingIndex":
         if not isinstance(obj, dict) or obj.get("format") != FORMAT:
             raise ValueError(f"{path} is not a saved EmbeddingIndex")
         if device is None:
@@ -775,3 +782,372 @@ class ShardedIndex:
                 compute.synchronize()
                 copy.synchronize()
         return scores, idx
+
+
+# ---- inverted-file index ----------------------------------------------------------------------------------------------
+IVF_FORMAT = "esm_b200.search-ivf/1"
+MAX_NPROBE = 128
+DEFAULT_NPROBE = 8
+IVF_SCRATCH_CAP = 1 << 30   # device bytes of one esmb200_ivf_search call's scratch: query batches are sized to it
+ASSIGN_BATCH = 1 << 20      # rows assigned to their lists per knn launch pair
+MEAN_ROWS = 1 << 23         # rows per esmb200_kmeans_means call, its limit: no column sum of one call can overflow
+
+
+def ivf_scratch_bytes(Q: int, nprobe: int, nlist: int, N: int, D: int, k: int) -> int:
+    """esmb200_ivf_scratch_bytes: pure host arithmetic; ValueError (the library's message) for arguments it refuses."""
+    nbytes = ctypes.c_size_t(0)
+    _lib.check(_lib.load().esmb200_ivf_scratch_bytes(Q, nprobe, nlist, N, D, k, ctypes.byref(nbytes)))
+    return nbytes.value
+
+
+def ivf_query_batch(nprobe: int, nlist: int, N: int, D: int, k: int, cap: Optional[int] = None) -> int:
+    """Queries per esmb200_ivf_search call: the most (up to QUERY_BATCH) whose scratch stays within cap (default
+    IVF_SCRATCH_CAP), at least 1."""
+    cap = IVF_SCRATCH_CAP if cap is None else cap
+    lo, hi = 1, QUERY_BATCH
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        lo, hi = (mid, hi) if ivf_scratch_bytes(mid, nprobe, nlist, N, D, k) <= cap else (lo, mid - 1)
+    return lo
+
+
+def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, offsets: torch.Tensor, k: int,
+               beta: Optional[torch.Tensor] = None, alpha: float = 1.0, probes: Optional[torch.Tensor] = None,
+               self_ids: Optional[torch.Tensor] = None, scratch: Optional[torch.Tensor] = None
+               ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """esmb200_ivf_search on prepared operands, all on one CUDA device: queries fp16 [Q, D], rows fp16 [N, D] in list
+    order, ids int64 [N], offsets int64 [nlist + 1], beta fp32 [N] or None, probes int32 [Q, nprobe] (None: every
+    list), self_ids int64 [Q] or None. Returns (s fp32 [Q, k], idx int64 [Q, k]), NaN / -1 past the candidates."""
+    for name, t in (("queries", queries), ("rows", rows)):
+        if t.dtype != torch.float16 or t.dim() != 2 or not t.is_cuda or t.stride(1) != 1:
+            raise ValueError(f"{name} must be a CUDA fp16 tensor [n, D] with contiguous rows")
+    dev = rows.device
+    Q, N, D = queries.shape[0], rows.shape[0], rows.shape[1]
+    nlist = offsets.numel() - 1
+    want = [("ids", ids, torch.int64, (N,)), ("offsets", offsets, torch.int64, (nlist + 1,))]
+    if beta is not None:
+        want.append(("beta", beta, torch.float32, (N,)))
+    if probes is not None:
+        want.append(("probes", probes, torch.int32, (Q, probes.shape[-1] if probes.dim() == 2 else -1)))
+    if self_ids is not None:
+        want.append(("self_ids", self_ids, torch.int64, (Q,)))
+    for name, t, dtype, shape in want:
+        if not (t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == shape and t.device == dev):
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor {list(shape)} on the rows' device")
+    if queries.device != dev or queries.shape[1] != D:
+        raise ValueError("queries and rows must be on one device with one width")
+    nprobe = nlist if probes is None else probes.shape[1]
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        nbytes = ivf_scratch_bytes(Q, nprobe, nlist, N, D, k)
+        if scratch is None or scratch.numel() < nbytes:
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        scores = torch.empty((Q, k), dtype=torch.float32, device=dev)
+        idx = torch.empty((Q, k), dtype=torch.int64, device=dev)
+        _lib.check(lib.esmb200_ivf_search(_ptr(queries), queries.stride(0), Q, _ptr(rows), rows.stride(0), N,
+                                          _ptr(ids), _ptr(offsets), nlist, D, _ptr(beta), float(alpha), _ptr(probes),
+                                          nprobe, _ptr(self_ids), k, _ptr(scratch), scratch.numel(), _ptr(scores),
+                                          _ptr(idx), _stream()))
+    return scores, idx
+
+
+def kmeans_means(rows: torch.Tensor, assign: torch.Tensor, nlist: int
+                 ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """esmb200_kmeans_means: (sums int64 [nlist, D], means fp32 [nlist, D], counts int64 [nlist]) of rows fp16 [n, D]
+    under assign int64 [n], on the rows' CUDA device; means = fp32((sums / counts) * 2^-24), exactly."""
+    if rows.dtype != torch.float16 or rows.dim() != 2 or not rows.is_cuda or rows.stride(1) != 1:
+        raise ValueError("rows must be a CUDA fp16 tensor [n, D] with contiguous rows")
+    n, D = rows.shape
+    if not (assign.dtype == torch.int64 and assign.is_contiguous() and tuple(assign.shape) == (n,)
+            and assign.device == rows.device):
+        raise ValueError(f"assign must be a contiguous int64 tensor [{n}] on the rows' device")
+    dev = rows.device
+    sums = torch.empty((nlist, D), dtype=torch.int64, device=dev)
+    means = torch.empty((nlist, D), dtype=torch.float32, device=dev)
+    counts = torch.empty(nlist, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().esmb200_kmeans_means(_ptr(rows), rows.stride(0), n, D, _ptr(assign), nlist,
+                                                    _ptr(sums), _ptr(means), _ptr(counts), _stream()))
+    return sums, means, counts
+
+
+def check_sum_bound(counts: torch.Tensor, max_abs: float) -> None:
+    """ValueError when a cluster's exact column sum could pass int64: count * max|x| * 2^24 >= 2^63 (cosine rows,
+    |x| <= 1, never can; l2 rows up to 65504 can past 2^23 members)."""
+    most = int(counts.max()) if counts.numel() else 0
+    if most * int(max_abs * 2 ** 24) >= 2 ** 63:
+        raise ValueError(f"a cluster of {most} rows with values up to {max_abs:g} could overflow its int64 column sums: "
+                         f"train on fewer rows")
+
+
+def exact_means(rows: torch.Tensor, assign: torch.Tensor, nlist: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(means fp32 [nlist, D], counts int64 [nlist]) as kmeans_means defines them, for any number of rows: more than
+    MEAN_ROWS rows go through kmeans_means in slices whose int64 sums are added exactly, and the means are formed as
+    the kernel forms them, fp32(((double)S / count) * 2^-24), bit for bit; check_sum_bound refuses a cluster whose sum
+    could overflow."""
+    n = rows.shape[0]
+    if n <= MEAN_ROWS:
+        _, means, counts = kmeans_means(rows, assign, nlist)
+        return means, counts
+    sums = counts = None
+    for r0 in range(0, n, MEAN_ROWS):
+        s, _, c = kmeans_means(rows[r0:r0 + MEAN_ROWS], assign[r0:r0 + MEAN_ROWS], nlist)
+        sums, counts = (s, c) if sums is None else (sums + s, counts + c)
+    # each slice's sums and the total are bounded by count * max|x| * 2^24, so no addition wrapped if this holds
+    check_sum_bound(counts, float(rows.abs().max()))
+    means = ((sums.double() / counts[:, None].double()) * 2.0 ** -24).float()
+    means[counts == 0] = 0
+    return means, counts
+
+
+def training_sample(N: int, train_rows: int, seed: int) -> torch.Tensor:
+    """The k-means training sample: the first train_rows entries of a seeded permutation of the N rows, drawn on the CPU
+    so that every device trains on the same rows. Its first nlist rows are the initial centroids."""
+    return torch.randperm(N, generator=torch.Generator().manual_seed(seed))[:train_rows]
+
+
+def worst_served(s: torch.Tensor, x_sqnorm: Optional[torch.Tensor], metric: str) -> torch.Tensor:
+    """Sample positions from worst to best served by their centroid: the lowest cosine similarity s, or the largest
+    l2 distance |x|^2 - s (fp32, s = 2 x.c - |c|^2), ties to the smaller position."""
+    bad = -s if metric == "cosine" else x_sqnorm - s
+    return torch.sort(-bad, stable=True).indices
+
+
+def fill_empty(centroids: torch.Tensor, empty: torch.Tensor, x: torch.Tensor, s: torch.Tensor,
+               x_sqnorm: Optional[torch.Tensor], metric: str) -> torch.Tensor:
+    """The empty-cluster rule: the empty centroids (bool [nlist]), in ascending index order, each take the next
+    worst-served sample row (worst_served); the row becomes the centroid as it is. Returns the new centroid rows."""
+    e = empty.nonzero().flatten()
+    if e.numel() == 0:
+        return centroids
+    out = centroids.clone()
+    out[e] = x[worst_served(s, x_sqnorm, metric)[:e.numel()]]
+    return out
+
+
+def _check_int(name, v, lo, hi=None):
+    if isinstance(v, bool) or not isinstance(v, int) or v < lo or (hi is not None and v > hi):
+        raise ValueError(f"{name} must be an int in [{lo}, {hi if hi is not None else 'inf'}], got {v!r}")
+    return v
+
+
+def _assign(rows: torch.Tensor, centroids: torch.Tensor, metric: str) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(s fp32 [n], list int64 [n]): each row's best centroid under the search score, ties to the smaller index."""
+    l2 = metric == "l2"
+    beta = -squared_norms(centroids) if l2 else None
+    s_out, a_out = [], []
+    for r0 in range(0, rows.shape[0], ASSIGN_BATCH):
+        s, a = knn(rows[r0:r0 + ASSIGN_BATCH], centroids, 1, beta, 2.0 if l2 else 1.0)
+        s_out.append(s[:, 0])
+        a_out.append(a[:, 0])
+    return torch.cat(s_out), torch.cat(a_out)
+
+
+def train_kmeans(rows: torch.Tensor, dim: int, metric: str, nlist: int, train_rows: int, iters: int,
+                 seed: int) -> torch.Tensor:
+    """Lloyd's k-means on the prepared rows (fp16 [N, D], CUDA): the centroid rows fp16 [nlist, D] (IVFIndex)."""
+    x = rows[training_sample(rows.shape[0], train_rows, seed).to(rows.device)]
+    x_sqnorm = squared_norms(x) if metric == "l2" else None
+    cent = x[:nlist].clone()
+    for _ in range(iters):
+        s, a = _assign(x, cent, metric)
+        means, counts = exact_means(x, a, nlist)
+        empty = counts == 0
+        if metric == "cosine":  # a mean of zero has no direction: the cluster is refilled as an empty one
+            empty |= (means != 0).sum(1) == 0
+        new = torch.empty_like(cent)
+        keep = (~empty).nonzero().flatten()
+        new[keep] = prepare_rows(means[keep][:, :dim], metric, "centroids")
+        cent = fill_empty(new, empty, x, s, x_sqnorm, metric)
+    return cent
+
+
+class IVFIndex:
+    """An inverted-file index: the rows of an EmbeddingIndex grouped into nlist lists around k-means centroids.
+
+        index = search.IVFIndex.from_extract_dir("out/", layer=33, nlist=1024)   # or IVFIndex(vectors, nlist=...)
+        index = search.IVFIndex.from_index(embedding_index, nlist=1024)
+        scores, idx = index.search(queries, k=10, nprobe=8)    # idx: original row numbers, -1 for a missing hit
+        scores, idx = index.search_all(k=10, nprobe=8)         # every row against the index, its own row left out
+
+    Rows, metrics and scores are EmbeddingIndex's. A query's result is the exact top k, by (score descending, original
+    index ascending), over the rows of the nprobe lists whose centroids score highest for it (the same score, ties to
+    the smaller list); with fewer than k rows in them the missing slots are NaN and -1. nprobe == nlist scans every
+    list and gives EmbeddingIndex's results bit for bit.
+
+    Training (Lloyd's k-means on the GPU, deterministic for given rows and seed): the sample is training_sample(N,
+    train_rows, seed) (train_rows defaults to min(N, 256 nlist)) and its first nlist rows are the initial centroids.
+    Each of `iters` iterations assigns every sample row to its best centroid (esmb200_knn_search with k = 1), takes each
+    centroid's exact mean (exact_means) and prepares it as a row (prepare_rows: cosine centroids are unit fp16 rows);
+    a cluster left empty (or, for cosine, with a zero mean) takes the worst-served sample row instead (fill_empty).
+    Every row then goes to its best centroid's list; a list holds its rows in ascending original index."""
+
+    def __init__(self, vectors: torch.Tensor, labels: Optional[Sequence[str]] = None, metric: str = "cosine",
+                 layer: Optional[int] = None, *, nlist: int, train_rows: Optional[int] = None, iters: int = 20,
+                 seed: int = 0):
+        _check_metric(metric)
+        if isinstance(vectors, torch.Tensor) and vectors.dim() == 2 and vectors.shape[0] < 1:
+            raise ValueError("an index needs at least one row")
+        rows = prepare_rows(vectors, metric)
+        self._build(rows, vectors.shape[1], labels, metric, layer, nlist, train_rows, iters, seed)
+
+    def _build(self, rows, dim, labels, metric, layer, nlist, train_rows, iters, seed):
+        N = rows.shape[0]
+        _check_int("nlist", nlist, 1, N)
+        train_rows = min(N, 256 * nlist) if train_rows is None else train_rows
+        _check_int("train_rows", train_rows, nlist, N)
+        _check_int("iters", iters, 0)
+        _check_int("seed", seed, 0)
+        labels = [str(i) for i in range(N)] if labels is None else [str(l) for l in labels]
+        if len(labels) != N:
+            raise ValueError(f"{len(labels)} labels for {N} rows")
+        if not rows.is_cuda:
+            if not torch.cuda.is_available():
+                raise ValueError("training an IVFIndex needs a CUDA device")
+            rows = rows.to(torch.device("cuda", torch.cuda.current_device()))
+        cent = train_kmeans(rows, dim, metric, nlist, train_rows, iters, seed)
+        _, a = _assign(rows, cent, metric)
+        ids = torch.sort(a, stable=True).indices
+        offsets = torch.zeros(nlist + 1, dtype=torch.int64, device=rows.device)
+        offsets[1:] = torch.cumsum(torch.bincount(a, minlength=nlist), 0)
+        params = {"nlist": nlist, "train_rows": train_rows, "iters": iters, "seed": seed}
+        self._set(rows[ids], ids, offsets, cent, dim, labels, metric, layer, params)
+
+    def _set(self, rows, ids, offsets, centroids, dim, labels, metric, layer, params):
+        self.rows, self.ids, self.offsets, self.centroids = rows, ids, offsets, centroids
+        self.dim, self.labels, self.metric, self.layer, self.params = int(dim), list(labels), metric, layer, dict(params)
+        self.nlist = offsets.numel() - 1
+        self.sqnorm = squared_norms(rows) if metric == "l2" else None
+        self._beta = -self.sqnorm if metric == "l2" else None
+        self._cbeta = -squared_norms(centroids) if metric == "l2" else None
+        self._pos = torch.empty_like(ids)  # the stored position of each original row
+        self._pos[ids] = torch.arange(ids.numel(), device=ids.device)
+
+    @classmethod
+    def _from_parts(cls, rows, ids, offsets, centroids, dim, labels, metric, layer, params) -> "IVFIndex":
+        self = cls.__new__(cls)
+        self._set(rows, ids, offsets, centroids, dim, labels, metric, layer, params)
+        return self
+
+    @classmethod
+    def from_index(cls, index: EmbeddingIndex, *, nlist: int, train_rows: Optional[int] = None, iters: int = 20,
+                   seed: int = 0) -> "IVFIndex":
+        """An IVF index of an EmbeddingIndex's rows, labels, metric and layer (its rows are used as they are)."""
+        self = cls.__new__(cls)
+        self._build(index.rows, index.dim, index.labels, index.metric, index.layer, nlist, train_rows, iters, seed)
+        return self
+
+    @classmethod
+    def from_extract_dir(cls, path, layer: int, metric: str = "cosine", *, nlist: int, train_rows: Optional[int] = None,
+                         iters: int = 20, seed: int = 0, device=None) -> "IVFIndex":
+        """An IVF index of the mean representations at `layer` of every extract_cli file under path (label order)."""
+        _check_metric(metric)
+        labels, x = _read_extract_dir(path, layer)
+        return cls(x.to(device) if device is not None else x, labels, metric, layer, nlist=nlist,
+                   train_rows=train_rows, iters=iters, seed=seed)
+
+    def __len__(self) -> int:
+        return self.rows.shape[0]
+
+    @property
+    def device(self) -> torch.device:
+        return self.rows.device
+
+    def to(self, device) -> "IVFIndex":
+        return IVFIndex._from_parts(self.rows.to(device), self.ids.to(device), self.offsets.to(device),
+                                    self.centroids.to(device), self.dim, self.labels, self.metric, self.layer,
+                                    self.params)
+
+    def save(self, path) -> None:
+        torch.save({"format": IVF_FORMAT, "rows": self.rows.cpu(), "ids": self.ids.cpu(),
+                    "offsets": self.offsets.cpu(), "centroids": self.centroids.cpu(), "labels": self.labels,
+                    "metric": self.metric, "layer": self.layer, "dim": self.dim, "params": self.params}, path)
+
+    @classmethod
+    def _from_saved(cls, obj, path, device) -> "IVFIndex":
+        if not isinstance(obj, dict) or obj.get("format") != IVF_FORMAT:
+            raise ValueError(f"{path} is not a saved IVFIndex")
+        if device is None:
+            device = "cuda" if torch.cuda.is_available() else "cpu"
+        _check_metric(obj["metric"])
+        return cls._from_parts(obj["rows"].to(device), obj["ids"].to(device), obj["offsets"].to(device),
+                               obj["centroids"].to(device), obj["dim"], obj["labels"], obj["metric"], obj["layer"],
+                               obj["params"])
+
+    @classmethod
+    def load(cls, path, device=None) -> "IVFIndex":
+        """An index saved by save(), on `device` (default: the current CUDA device if there is one, else the CPU)."""
+        return cls._from_saved(torch.load(path, map_location="cpu", weights_only=True), path, device)
+
+    # ---- search ------------------------------------------------------------------------------------------------------
+    def check_nprobe(self, nprobe) -> int:
+        """nprobe, or the default min(DEFAULT_NPROBE, nlist) for None; ValueError outside [1, min(nlist, 128)] unless
+        it is nlist."""
+        if nprobe is None:
+            return min(DEFAULT_NPROBE, self.nlist)
+        if isinstance(nprobe, bool) or not isinstance(nprobe, int) or not (
+                nprobe == self.nlist or 1 <= nprobe <= min(self.nlist, MAX_NPROBE)):
+            raise ValueError(f"nprobe must be in [1, {min(self.nlist, MAX_NPROBE)}] or nlist = {self.nlist}, "
+                             f"got {nprobe!r}")
+        return nprobe
+
+    def probes(self, q: torch.Tensor, nprobe: int) -> torch.Tensor:
+        """The coarse step on prepared query rows: int32 [Q, nprobe], each query's top-nprobe lists by the search
+        score against the centroid rows, ties to the smaller list."""
+        _, lists = knn(q, self.centroids, nprobe, self._cbeta, 2.0 if self.metric == "l2" else 1.0)
+        return lists.int()
+
+    def search(self, queries: torch.Tensor, k: int = 10, nprobe: Optional[int] = None
+               ) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The k nearest rows of each query among its nprobe lists (default min(8, nlist)), as EmbeddingIndex.search
+        returns them, with original row numbers; NaN / -1 past the probed lists' rows."""
+        _check_k(k, len(self))
+        nprobe = self.check_nprobe(nprobe)
+        if isinstance(queries, torch.Tensor) and queries.dim() == 1:
+            queries = queries[None]
+        if isinstance(queries, torch.Tensor) and queries.dim() == 2 and queries.shape[1] != self.dim:
+            raise ValueError(f"queries have width {queries.shape[1]}, the index {self.dim}")
+        q = prepare_rows(queries, self.metric, "queries")
+        self._check_device()
+        return self._search_rows(q.to(self.device), k, nprobe, self_rows=False)
+
+    def search_all(self, k: int = 10, nprobe: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Every row (in original order) against the index with its own row left out: (scores, idx) [N, k]."""
+        _check_k(k, len(self) - 1)
+        nprobe = self.check_nprobe(nprobe)
+        self._check_device()
+        return self._search_rows(None, k, nprobe, self_rows=True)
+
+    def _check_device(self) -> None:
+        if not self.rows.is_cuda:
+            raise ValueError("the index is on the CPU: move it to a GPU with index.to('cuda') to search")
+
+    def _search_rows(self, q: Optional[torch.Tensor], k: int, nprobe: int, self_rows: bool):
+        Q = len(self) if self_rows else q.shape[0]
+        N, D, l2 = len(self), self.rows.shape[1], self.metric == "l2"
+        scores = torch.empty((Q, k), dtype=torch.float32, device=self.device)
+        idx = torch.empty((Q, k), dtype=torch.int64, device=self.device)
+        batch = ivf_query_batch(nprobe, self.nlist, N, D, k)
+        scratch = None
+        for b0 in range(0, Q, batch):
+            b1 = min(Q, b0 + batch)
+            qb = self.rows[self._pos[b0:b1]] if self_rows else q[b0:b1]
+            probes = None if nprobe == self.nlist else self.probes(qb, nprobe)
+            self_ids = torch.arange(b0, b1, device=self.device) if self_rows else None
+            if scratch is None:
+                scratch = torch.empty(ivf_scratch_bytes(b1 - b0, nprobe, self.nlist, N, D, k), dtype=torch.uint8,
+                                      device=self.device)
+            s, i = ivf_search(qb, self.rows, self.ids, self.offsets, k, self._beta, 2.0 if l2 else 1.0, probes,
+                              self_ids, scratch)
+            if l2:
+                s = (squared_norms(qb)[:, None] - s).clamp_min(0).sqrt()
+            scores[b0:b1] = s
+            idx[b0:b1] = i
+        return scores, idx
+
+
+def load_file_index(path, device=None):
+    """The EmbeddingIndex or IVFIndex saved in one .pt file, by its format (read once)."""
+    obj = torch.load(path, map_location="cpu", weights_only=True)
+    ivf = isinstance(obj, dict) and obj.get("format") == IVF_FORMAT
+    return (IVFIndex if ivf else EmbeddingIndex)._from_saved(obj, path, device)

@@ -2,7 +2,10 @@
 
     python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out db.pt
     python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out db/ [--append]
-    python -m esm_b200.search_cli query db.pt|db/ (--queries EXTRACT_DIR | --all) --k 10 --out hits.tsv
+    python -m esm_b200.search_cli build EXTRACT_DIR --layer 33 [--metric cosine|l2] --out ivf.pt --nlist 4096
+                                        [--train-rows N] [--iters 20] [--seed 0]
+    python -m esm_b200.search_cli query db.pt|db/|ivf.pt (--queries EXTRACT_DIR | --all) --k 10 [--nprobe P]
+                                        --out hits.tsv
 
 `build` reads the mean representation at --layer of every `<label>.pt` under EXTRACT_DIR (extract_cli --include mean)
 and saves an index: one file (EmbeddingIndex) when --out ends in .pt, else a sharded index directory (IndexWriter),
@@ -13,6 +16,12 @@ at the index's width, or with every indexed protein against the others (--all); 
 the GPU (ShardedIndex), so it may be larger than the device's memory. hits.tsv has one line per hit: query, rank
 (1-based), target, score (cosine similarity, or Euclidean distance for l2). Embedding the queries stays in
 extract_cli, with its model loading and checkpoint checks.
+
+`build --nlist` trains an inverted-file index (IVFIndex: k-means lists on the GPU) and saves it to a .pt file; it
+cannot go to a directory or be appended to. `query` reads the index type from the file, and --nprobe (default
+min(8, nlist); nlist scans every list and gives the exact hits) sets how many lists each query scans. An IVF query
+can find fewer than k hits when its lists hold fewer rows; hits.tsv then has fewer lines for it. --nprobe on an exact
+or sharded index is refused.
 """
 from __future__ import annotations
 
@@ -36,12 +45,17 @@ def create_parser():
                    help="db.pt: one file; any other path: a sharded index directory")
     b.add_argument("--append", action="store_true", help="add shards to an existing directory index")
     b.add_argument("--shard-rows", type=int, default=search.SHARD_ROWS, help="rows per shard of a directory index")
+    b.add_argument("--nlist", type=int, help="train an inverted-file index of this many k-means lists (.pt only)")
+    b.add_argument("--train-rows", type=int, help="k-means training sample (default min(N, 256 nlist))")
+    b.add_argument("--iters", type=int, default=20, help="k-means iterations")
+    b.add_argument("--seed", type=int, default=0, help="k-means training sample seed")
     q = sub.add_parser("query", help="search an index")
     q.add_argument("index", type=pathlib.Path)
     src = q.add_mutually_exclusive_group(required=True)
     src.add_argument("--queries", type=pathlib.Path, help="an extract_cli output directory of query proteins")
     src.add_argument("--all", action="store_true", help="every indexed protein against the others")
     q.add_argument("--k", type=int, default=10, help=f"hits per query, 1 to {search.MAX_K}")
+    q.add_argument("--nprobe", type=int, help="lists scanned per query (IVF index only)")
     q.add_argument("--out", type=pathlib.Path, required=True)
     return p
 
@@ -54,6 +68,8 @@ def write_hits(path, query_labels, target_labels, scores: torch.Tensor, idx: tor
         f.write("query\trank\ttarget\tscore\n")
         for q, row_s, row_i in zip(query_labels, scores, idx):
             for r, (s, i) in enumerate(zip(row_s, row_i)):
+                if i < 0:  # an IVF query with fewer hits than k
+                    continue
                 f.write(f"{q}\t{r + 1}\t{target_labels[i]}\t{s:.6g}\n")
                 n += 1
     return n
@@ -92,16 +108,33 @@ def build_shards(extract_dir, layer: int, metric: str, out, append: bool, shard_
 def run(args) -> int:
     """Returns the number of rows indexed (build) or hit lines written (query)."""
     if args.command == "build":
+        if args.nlist is not None and not _is_file_index(args.out):
+            raise ValueError("--nlist builds an IVF index into one .pt file, not a directory")
+        if args.nlist is not None and args.append:
+            raise ValueError("--nlist builds a new IVF index: it cannot --append")
+        if args.nlist is None and (args.train_rows is not None or args.iters != 20 or args.seed != 0):
+            raise ValueError("--train-rows, --iters and --seed train an IVF index: pass --nlist")
         if not _is_file_index(args.out):
             return build_shards(args.extract_dir, args.layer, args.metric, args.out, args.append, args.shard_rows)
         if args.append:
             raise ValueError("--append adds shards to a directory index, not to a .pt file")
-        index = search.EmbeddingIndex.from_extract_dir(args.extract_dir, args.layer, args.metric)
+        if args.nlist is not None:
+            index = search.IVFIndex.from_extract_dir(args.extract_dir, args.layer, args.metric, nlist=args.nlist,
+                                                     train_rows=args.train_rows, iters=args.iters, seed=args.seed)
+        else:
+            index = search.EmbeddingIndex.from_extract_dir(args.extract_dir, args.layer, args.metric)
         args.out.parent.mkdir(parents=True, exist_ok=True)
         index.save(args.out)
         return len(index)
     sharded = args.index.is_dir()
-    index = search.ShardedIndex.open(args.index) if sharded else search.EmbeddingIndex.load(args.index, device="cpu")
+    if sharded and args.nprobe is not None:
+        raise ValueError("--nprobe applies to an IVF index; a directory index is searched exactly")
+    index = search.ShardedIndex.open(args.index) if sharded else search.load_file_index(args.index, device="cpu")
+    ivf = isinstance(index, search.IVFIndex)
+    if args.nprobe is not None and not ivf:
+        raise ValueError(f"--nprobe applies to an IVF index; {args.index} is an exact index")
+    if ivf:
+        index.check_nprobe(args.nprobe)
     candidates = len(index) - 1 if args.all else len(index)
     search._check_k(args.k, candidates)
     if args.all:
@@ -115,7 +148,8 @@ def run(args) -> int:
         search.prepare_rows(queries, index.metric, "queries")
     if not sharded:
         index = index.to(torch.device("cuda", torch.cuda.current_device()))
-    scores, idx = index.search_all(args.k) if args.all else index.search(queries, args.k)
+    extra = {"nprobe": args.nprobe} if ivf else {}
+    scores, idx = index.search_all(args.k, **extra) if args.all else index.search(queries, args.k, **extra)
     args.out.parent.mkdir(parents=True, exist_ok=True)
     return write_hits(args.out, qlabels, index.labels, scores, idx)
 

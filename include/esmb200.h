@@ -364,6 +364,55 @@ int esmb200_knn_search_accumulate(const void* queries, int64_t q_ld, int32_t Q, 
                                   uint64_t* keys, void* stream);
 int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_scores, int64_t* out_idx, void* stream);
 
+/* Inverted-file (IVF) search (esm_b200/search.py IVFIndex). The stored rows fp16 [N, b_ld] (device, 16-byte aligned) are
+ * grouped into nlist lists: list l is rows [offsets[l], offsets[l+1]) (offsets int64 [nlist + 1], 0 = offsets[0] <=
+ * ... <= offsets[nlist] = N), and ids int64 [N] holds each stored row's original index (distinct, in [0, 2^31)). beta
+ * fp32 [N] (or NULL) is in stored order. For each query row i (queries fp16 [Q, q_ld]) the result is the exact top k of
+ *     s(i, j) = alpha * (queries_i . rows_j) + beta[j]      (fp32 accumulation of the fp16 products)
+ * over the stored rows j of the lists query i probes, leaving out the row with ids[j] == self_ids[i] (self_ids int64
+ * [Q], or NULL for none), ranked by (score descending, ids[j] ascending): out_scores fp32 [Q, k] and out_idx int64
+ * [Q, k] (= ids[j]), dense. Slots past the probed lists' candidates are score NaN and index -1.
+ *   nprobe < nlist: probes int32 [Q, nprobe] (device) names the lists of each query, 1 <= nprobe <= 128; an entry
+ *     outside [0, nlist), or one that repeats an earlier entry of its row, probes nothing, so each list is scanned
+ *     at most once per query.
+ *   nprobe == nlist: every list, probes NULL; the result is then esmb200_knn_search's over the rows in original order,
+ *     bit for bit.
+ * The scores are esmb200_knn_search's, so a query's result depends only on the query, the rows and its probed lists:
+ * not on the other queries, Q or the launch configuration.
+ * Work: the (query, probe) pairs are grouped by list (probed only: a count, a scan, the placement, the work items and a
+ * gather of the query rows into scratch, then one device-to-host read of the work-item count, the call's only host
+ * synchronisation); one knn_topk_kernel<false, true> CTA per work item (a list, a block of <= 64 queries probing it,
+ * a stripe of T of its 256-row tiles), so each list is read once per query block; then a merge of each query's
+ * partial lists. Stripes: probed, T = ceil((ceil(N / 256) + nlist) / 64), so a query has at most nprobe + 64 partial
+ * lists; every list, the rows split into min(ceil(N / 256), ceil(264 / ceil(Q / 64))) stripes (about two waves of a
+ * 132-SM H100).
+ * scratch: esmb200_ivf_scratch_bytes(Q, nprobe, nlist, N, D, k) bytes, 256-byte aligned; it grows with Q: about
+ * Q * nprobe * D * 2 bytes of gathered query rows and Q * (nprobe + 64) * k * 8 of partial lists (probed). 1 <= k <= 128,
+ * 1 <= N < 2^31, Q >= 0, 1 <= nlist <= min(N, 2^24), nprobe as above with Q * nprobe < 2^30 and Q * R < 2^31 (R the
+ * partial lists per query: nprobe + 64, or the stripe count when every list is probed), D % 64 == 0, q_ld and b_ld
+ * >= D and multiples of 8, probes NULL exactly when nprobe == nlist, non-NULL queries, rows, ids, offsets, scratch and
+ * outputs with their alignments and enough scratch, else ESMB200_EINVAL before any launch. Q == 0 launches nothing.
+ * A work-item count past the bound (offsets that do not partition [0, N); offsets are not otherwise checked) is
+ * refused after the grouping launches, before the scan. esmb200_ivf_scratch_bytes writes the size to *out, with the same refusals. */
+int esmb200_ivf_scratch_bytes(int32_t Q, int32_t nprobe, int32_t nlist, int64_t N, int32_t D, int32_t k, size_t* out);
+int esmb200_ivf_search(const void* queries, int64_t q_ld, int32_t Q, const void* rows, int64_t b_ld, int64_t N,
+                       const int64_t* ids, const int64_t* offsets, int32_t nlist, int32_t D, const float* beta,
+                       float alpha, const int32_t* probes, int32_t nprobe, const int64_t* self_ids, int32_t k,
+                       void* scratch, size_t scratch_bytes, float* out_scores, int64_t* out_idx, void* stream);
+
+/* k-means centroid means, exactly (esm_b200/search.py IVFIndex training). rows fp16 [n, ld] (device, 16-byte aligned,
+ * first D columns), assign int64 [n] (a row with assign outside [0, nlist) is left out). Every fp16 value is an integer
+ * multiple of 2^-24, so
+ *     sums[c, j]  = sum over rows r with assign[r] == c of rows[r, j] * 2^24      (int64, exact)
+ *     counts[c]   = the rows with assign == c                                     (int64)
+ *     means[c, j] = fp32(((double)sums[c, j] / counts[c]) * 2^-24), 0 for an empty cluster
+ * are IEEE-defined and do not depend on the order of the additions (atomics). sums int64 [nlist, D], means_out fp32
+ * [nlist, D] and counts_out int64 [nlist] (device, dense) are outputs. n <= 2^23 (|x| <= 65504, so |sums| < 2^63),
+ * D % 8 == 0, ld >= D a multiple of 8, 1 <= nlist <= 2^24, non-NULL and aligned pointers, else ESMB200_EINVAL before
+ * any launch. Two memsets and two launches. */
+int esmb200_kmeans_means(const void* rows, int64_t ld, int64_t n, int32_t D, const int64_t* assign, int32_t nlist,
+                         int64_t* sums, float* means_out, int64_t* counts_out, void* stream);
+
 /* Pairwise alignment of proteins by their per-residue embeddings (esm_b200/align.py; the EBA / pLM-BLAST family of
  * methods). A new operation with no reference code. Pair p (of P) has La query rows and Lb target rows, La, Lb >= 1:
  * query rows [q_off[p], q_off[p+1]) and target rows [t_off[p], t_off[p+1]), its similarity S' as [La, Lb] fp32
@@ -530,7 +579,7 @@ int esmb200_layernorm_f16(const float* x, const float* weight, const float* bias
  *         18 window merge, 19 categorical Jacobian contacts (each of its kernels), 20 sampling (esmb200_sample_order
  *         and each kernel of esmb200_sample_rows), 21 greedy MSA row selection (each kernel of
  *         esmb200_msa_greedy_select), 22 nearest-neighbour search (each kernel of esmb200_knn_search,
- *         esmb200_knn_search_accumulate and esmb200_knn_decode),
+ *         esmb200_knn_search_accumulate, esmb200_knn_decode, esmb200_ivf_search and esmb200_kmeans_means),
  *         23 embedding alignment (each kernel of esmb200_align_similarity and esmb200_align) */
 long long esmb200_launch_count(void);
 int esmb200_profile_enable(int32_t max_launches);
