@@ -76,6 +76,9 @@ EXPORTS = (
     "esmb200_knn_search",
     "esmb200_knn_search_accumulate",
     "esmb200_knn_decode",
+    "esmb200_knn_range",
+    "esmb200_knn_range_finish_scratch_bytes",
+    "esmb200_knn_range_finish",
     "esmb200_ivf_scratch_bytes",
     "esmb200_ivf_search",
     "esmb200_kmeans_means",
@@ -209,6 +212,15 @@ def _declare(lib):
                                                   c_size_t, c_void_p, c_void_p]
     lib.esmb200_knn_decode.restype = c_int32
     lib.esmb200_knn_decode.argtypes = [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.esmb200_knn_range.restype = c_int32
+    lib.esmb200_knn_range.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int64, c_int64, c_int32,
+                                      c_void_p, c_float, c_int64, c_void_p, c_int32, c_void_p, c_void_p, c_int64,
+                                      c_void_p, c_void_p, c_void_p]
+    lib.esmb200_knn_range_finish_scratch_bytes.restype = c_int32
+    lib.esmb200_knn_range_finish_scratch_bytes.argtypes = [c_int32, POINTER(c_size_t)]
+    lib.esmb200_knn_range_finish.restype = c_int32
+    lib.esmb200_knn_range_finish.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_int64, c_void_p,
+                                             c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.esmb200_ivf_scratch_bytes.restype = c_int32
     lib.esmb200_ivf_scratch_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, POINTER(c_size_t)]
     lib.esmb200_ivf_search.restype = c_int32

@@ -1902,6 +1902,103 @@ int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_sc
   return ESMB200_OK;
 }
 
+int esmb200_knn_range(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld, int64_t n,
+                      int64_t row0, int32_t D, const float* beta, float alpha, int64_t self_offset, const float* tau,
+                      int32_t splits, uint64_t* hit_keys, int32_t* hit_rows, int64_t hit_cap, uint64_t* hit_counts,
+                      uint64_t* hit_total, void* stream) {
+  if (Q < 0 || n < 1 || row0 < 0 || row0 > INT32_MAX || n > INT32_MAX - row0)
+    return fail(ESMB200_EINVAL, "knn_range needs Q >= 0, n >= 1, row0 >= 0 and row0 + n < 2^31");
+  if (D < 64 || D % 64 != 0) return fail(ESMB200_EINVAL, "knn_range needs D % 64 == 0");
+  if (q_ld < D || b_ld < D || q_ld % 8 != 0 || b_ld % 8 != 0)
+    return fail(ESMB200_EINVAL, "knn_range needs q_ld, b_ld >= D and multiples of 8 (16-byte rows for TMA)");
+  if (splits < 1 || splits > knn_cfg::MAX_SPLITS) return fail(ESMB200_EINVAL, "knn_range needs 1 <= splits <= 1024");
+  if (hit_cap < 0 || hit_cap > INT32_MAX) return fail(ESMB200_EINVAL, "knn_range needs 0 <= hit_cap < 2^31");
+  if (!queries || !base || !tau || !hit_counts || !hit_total || (hit_cap > 0 && (!hit_keys || !hit_rows)))
+    return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(queries) % 16 != 0 || reinterpret_cast<uintptr_t>(base) % 16 != 0)
+    return fail(ESMB200_EINVAL, "knn_range needs 16-byte aligned queries and base (TMA)");
+  if (reinterpret_cast<uintptr_t>(beta) % 4 != 0 || reinterpret_cast<uintptr_t>(tau) % 4 != 0 ||
+      reinterpret_cast<uintptr_t>(hit_rows) % 4 != 0 || reinterpret_cast<uintptr_t>(hit_keys) % 8 != 0 ||
+      reinterpret_cast<uintptr_t>(hit_counts) % 8 != 0 || reinterpret_cast<uintptr_t>(hit_total) % 8 != 0)
+    return fail(ESMB200_EINVAL, "knn_range needs 4-byte aligned beta, tau and hit_rows, 8-byte aligned hit_keys, "
+                                "hit_counts and hit_total");
+  if (Q == 0) return ESMB200_OK;
+  int rc = check_device();
+  if (rc) return rc;
+  CUtensorMap tq, tx;
+  if ((rc = make_tmap_f16(&tq, queries, (uint64_t)Q, (uint64_t)D, (uint64_t)q_ld, knn_cfg::BLOCK_M))) return rc;
+  if ((rc = make_tmap_f16(&tx, base, (uint64_t)n, (uint64_t)D, (uint64_t)b_ld, knn_cfg::BLOCK_N))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  KnnParams p = {};
+  p.Q = Q;
+  p.D = D;
+  p.k = 1;
+  p.N = n;
+  const int64_t tiles = (n + knn_cfg::BLOCK_N - 1) / knn_cfg::BLOCK_N;
+  p.tiles_per_stripe = (int)((tiles + splits - 1) / splits);
+  p.query_blocks = (Q + knn_cfg::BLOCK_M - 1) / knn_cfg::BLOCK_M;
+  p.beta = beta;
+  p.alpha = alpha;
+  p.self_offset = self_offset;
+  p.row0 = row0;
+  p.tau = tau;
+  p.hit_keys = reinterpret_cast<unsigned long long*>(hit_keys);
+  p.hit_rows = hit_rows;
+  p.hit_counts = reinterpret_cast<unsigned long long*>(hit_counts);
+  p.hit_total = reinterpret_cast<unsigned long long*>(hit_total);
+  p.hit_cap = hit_cap;
+  CK(cudaFuncSetAttribute(knn_topk_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                          knn_cfg::SMEM_BYTES));
+  ProfScope ps(T_KNN, st);
+  const int64_t grid = (int64_t)p.query_blocks * splits;
+  knn_topk_kernel<false, false, true><<<(unsigned)grid, knn_cfg::NUM_THREADS, knn_cfg::SMEM_BYTES, st>>>(tq, tx, p);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
+int esmb200_knn_range_finish_scratch_bytes(int32_t Q, size_t* out) {
+  if (!out) return fail(ESMB200_EINVAL, "null argument");
+  if (Q < 0) return fail(ESMB200_EINVAL, "knn_range_finish_scratch_bytes needs Q >= 0");
+  *out = ((size_t)Q + 1) * 8;
+  return ESMB200_OK;
+}
+
+int esmb200_knn_range_finish(const uint64_t* keys, const int32_t* rows, int64_t nnz, const uint64_t* counts, int32_t Q,
+                             int64_t max_hits, void* scratch, size_t scratch_bytes, int64_t* lims, float* scores,
+                             int64_t* idx, void* stream) {
+  if (Q < 0 || nnz < 0 || nnz > INT32_MAX)
+    return fail(ESMB200_EINVAL, "knn_range_finish needs Q >= 0 and 0 <= nnz < 2^31");
+  if (max_hits < 1 && max_hits != -1) return fail(ESMB200_EINVAL, "knn_range_finish needs max_hits >= 1, or -1");
+  if (!counts || !scratch || !lims || (nnz > 0 && (!keys || !rows || !scores || !idx)))
+    return fail(ESMB200_EINVAL, "null argument");
+  if (reinterpret_cast<uintptr_t>(keys) % 8 != 0 || reinterpret_cast<uintptr_t>(rows) % 4 != 0 ||
+      reinterpret_cast<uintptr_t>(counts) % 8 != 0 || reinterpret_cast<uintptr_t>(scratch) % 8 != 0 ||
+      reinterpret_cast<uintptr_t>(lims) % 8 != 0 || reinterpret_cast<uintptr_t>(scores) % 4 != 0 ||
+      reinterpret_cast<uintptr_t>(idx) % 8 != 0)
+    return fail(ESMB200_EINVAL, "knn_range_finish needs 8-byte aligned keys, counts, scratch, lims and idx, 4-byte "
+                                "aligned rows and scores");
+  if (scratch_bytes < ((size_t)Q + 1) * 8)
+    return fail(ESMB200_EINVAL, "scratch smaller than esmb200_knn_range_finish_scratch_bytes");
+  int rc = check_device();
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  long long* off = static_cast<long long*>(scratch);
+  {
+    ProfScope ps(T_KNN, st);
+    knn_range_scan_kernel<<<1, 1024, 0, st>>>(reinterpret_cast<const long long*>(counts), Q, max_hits, off,
+                                              reinterpret_cast<long long*>(lims));
+    CK(cudaGetLastError());
+  }
+  if (nnz == 0) return ESMB200_OK;
+  ProfScope ps(T_KNN, st);
+  const int64_t blocks = (nnz + 255) / 256;
+  knn_range_decode_kernel<<<(unsigned)(blocks < 8192 ? blocks : 8192), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), rows, nnz, Q, off, reinterpret_cast<const long long*>(lims),
+      scores, idx);
+  CK(cudaGetLastError());
+  return ESMB200_OK;
+}
+
 
 extern "C++" {
 namespace {

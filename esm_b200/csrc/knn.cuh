@@ -75,13 +75,25 @@ struct KnnParams {
   float alpha;
   int64_t self_offset;   // < 0: none; in global rows
   int64_t row0;          // global index of the chunk's row 0 (0 for esmb200_knn_search)
-  const unsigned long long* seed;  // running list [Q, k] whose k-th key seeds the thresholds, or nullptr
-  unsigned long long* keys;  // scratch [splits, Q, k]; list scan: [Q, R, k] (the query's partial lists, ragged)
-  // list scan (LISTS) only
-  const IvfItem* items;  // one work item per CTA
-  const int64_t* ids;           // [N] original row of each stored row: the key's index
-  const int64_t* gself;         // [query rows] the original row each query row leaves out (< 0: none), or nullptr
-  const int* pbase;             // [query rows] partial-list index of the row's stripe 0 (< 0: the row writes nothing)
+  union {  // one mode's pointers: the range fields overlay the top-k ones, so the parameter block keeps its size
+    struct {
+      const unsigned long long* seed;  // running list [Q, k] whose k-th key seeds the thresholds, or nullptr
+      unsigned long long* keys;  // scratch [splits, Q, k]; list scan: [Q, R, k] (the query's partial lists, ragged)
+      // list scan (LISTS) only
+      const IvfItem* items;  // one work item per CTA
+      const int64_t* ids;           // [N] original row of each stored row: the key's index
+      const int64_t* gself;         // [query rows] the original row each query row leaves out (< 0: none), or nullptr
+      const int* pbase;             // [query rows] partial-list index of the row's stripe 0 (< 0: the row writes nothing)
+    };
+    struct {  // range search (RANGE) only
+      const float* tau;                  // [Q] each query's threshold: its hits are the candidates with s >= tau
+      unsigned long long* hit_keys;      // [hit_cap] appended hit keys
+      int* hit_rows;                     // [hit_cap] the query row of each appended hit
+      unsigned long long* hit_counts;    // [Q] hits per query, counted past hit_cap
+      unsigned long long* hit_total;     // hits appended in all, counted past hit_cap
+      int64_t hit_cap;
+    };
+  };
 };
 
 __device__ __forceinline__ unsigned long long knn_key(float s, int64_t j) {
@@ -189,8 +201,11 @@ __device__ __forceinline__ void knn_merge_row(unsigned long long* list, unsigned
 // STREAM: a chunk of a streamed search (row0 and the seeded thresholds); without it the kernel is the resident one,
 // with no code for either.  LISTS: the inverted-file list scan (esmb200_ivf_search): CTA b runs work item items[b],
 // columns outside [r0, r1) and query rows outside [g0, g1) produce no candidate, a key's index is ids[j] and a row
-// leaves out the column whose id is gself[row]; without it none of this is compiled.
-template <bool STREAM, bool LISTS = false>
+// leaves out the column whose id is gself[row]; without it none of this is compiled.  RANGE: the range search
+// (esmb200_knn_range): global indices from row0, each row's threshold fixed at (ord(tau) << 32) - 1, so key > th
+// exactly when s >= tau, and a queue that could overflow is flushed to the global hit buffer instead of merged into a
+// k-list; no k-list is kept or written.
+template <bool STREAM, bool LISTS = false, bool RANGE = false>
 __global__ void __launch_bounds__(knn_cfg::NUM_THREADS, 1)
 knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                 const KnnParams p) {
@@ -208,7 +223,7 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   uint64_t* empty_bar = bars + STAGES;
 
   const int k = p.k;
-  const int64_t row0 = STREAM ? p.row0 : 0;
+  const int64_t row0 = STREAM ? p.row0 : RANGE ? p.row0 : 0;
   IvfItem item = {0, 0, 0, 0, 0};
   if (LISTS) item = p.items[blockIdx.x];
   const int qb = blockIdx.x % p.query_blocks, stripe = LISTS ? item.stripe : blockIdx.x / p.query_blocks;
@@ -230,10 +245,17 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < BLOCK_M * MAX_K; i += NUM_THREADS) s_list[i] = 0ull;
-  for (int i = threadIdx.x; i < BLOCK_M; i += NUM_THREADS) {
-    s_th[i] = (STREAM && p.seed != nullptr && q0 + i < p.Q) ? p.seed[(size_t)(q0 + i) * k + k - 1] : 0ull;
-    s_cnt[i] = 0;
+  if constexpr (RANGE) {
+    for (int i = threadIdx.x; i < BLOCK_M; i += NUM_THREADS) {  // tau is never NaN: ord(tau) > 0, th does not wrap
+      s_th[i] = q0 + i < p.Q ? knn_key(__ldg(p.tau + q0 + i) + 0.0f, 0xFFFFFFFFll) - 1ull : 0ull;
+      s_cnt[i] = 0;
+    }
+  } else {
+    for (int i = threadIdx.x; i < BLOCK_M * MAX_K; i += NUM_THREADS) s_list[i] = 0ull;
+    for (int i = threadIdx.x; i < BLOCK_M; i += NUM_THREADS) {
+      s_th[i] = (STREAM && p.seed != nullptr && q0 + i < p.Q) ? p.seed[(size_t)(q0 + i) * k + k - 1] : 0ull;
+      s_cnt[i] = 0;
+    }
   }
   __syncthreads();
 
@@ -283,6 +305,27 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   auto merge_all = [&]() {
     for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r)
       if (s_cnt[r] > 0) knn_merge_row<STREAM>(s_list + r * MAX_K, s_queue + r * QCAP, s_cnt + r, s_th + r, k, lane);
+  };
+  // RANGE: every row's queue appended to the global hit buffer, with one atomicAdd per row for its space
+  auto flush_all = [&]() {
+    for (int r = (int)warp * 16; r < (int)warp * 16 + 16; ++r) {
+      const int n = s_cnt[r];  // warp-uniform, at most QCAP
+      if (n == 0) continue;
+      unsigned long long at = 0;
+      if (lane == 0) {
+        at = atomicAdd(p.hit_total, (unsigned long long)n);
+        atomicAdd(p.hit_counts + q0 + r, (unsigned long long)n);
+      }
+      at = __shfl_sync(0xffffffffu, at, 0);
+      for (int i = (int)lane; i < n; i += 32)
+        if (at + i < (unsigned long long)p.hit_cap) {  // past the capacity the hits are counted, not written
+          p.hit_keys[at + i] = s_queue[r * QCAP + i];
+          p.hit_rows[at + i] = q0 + r;
+        }
+      __syncwarp();
+      if (lane == 0) s_cnt[r] = 0;
+      __syncwarp();
+    }
   };
 
   for (int t = t_begin; t < t_end; ++t) {
@@ -373,12 +416,16 @@ knn_topk_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         }
       }
       if (knn_bar_or(1, full)) {
-        merge_all();
+        if constexpr (RANGE) flush_all(); else merge_all();
         named_bar_sync(1, 128);
       }
     }
   }
   named_bar_sync(1, 128);
+  if constexpr (RANGE) {
+    flush_all();
+    return;
+  }
   merge_all();
   __syncwarp();
   // ---- the stripe's lists: warp w writes rows 16 w ..
@@ -478,6 +525,61 @@ knn_decode_kernel(const unsigned long long* __restrict__ keys, int64_t n, float*
                   int64_t* __restrict__ out_idx) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     knn_decode_key(keys[i], out_scores + i, out_idx + i);
+}
+
+// ---- range search (esmb200_knn_range_finish): the appended hits, sorted by (query row, key descending), to CSR -------
+// One block of 1024 threads: off = exclusive scan of counts (where each query's hits start), lims = exclusive scan of
+// min(counts, max_hits) (max_hits < 0: no cap); both [Q + 1].
+__global__ void __launch_bounds__(1024)
+knn_range_scan_kernel(const long long* __restrict__ counts, int Q, long long max_hits, long long* __restrict__ off,
+                      long long* __restrict__ lims) {
+  __shared__ long long s_o[1024], s_l[1024];
+  const int per = (Q + 1023) / 1024, l0 = min(Q, (int)threadIdx.x * per), l1 = min(Q, l0 + per);
+  auto kept = [&](long long c) { return max_hits >= 0 && c > max_hits ? max_hits : c; };
+  long long so = 0, sl = 0;
+  for (int q = l0; q < l1; ++q) {
+    so += counts[q];
+    sl += kept(counts[q]);
+  }
+  s_o[threadIdx.x] = so;
+  s_l[threadIdx.x] = sl;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long ao = 0, al = 0;
+    for (int t = 0; t < 1024; ++t) {
+      const long long o = s_o[t], l = s_l[t];
+      s_o[t] = ao;
+      s_l[t] = al;
+      ao += o;
+      al += l;
+    }
+    off[Q] = ao;
+    lims[Q] = al;
+  }
+  __syncthreads();
+  so = s_o[threadIdx.x];
+  sl = s_l[threadIdx.x];
+  for (int q = l0; q < l1; ++q) {
+    off[q] = so;
+    lims[q] = sl;
+    so += counts[q];
+    sl += kept(counts[q]);
+  }
+}
+
+// hit p (query rows[p], rank p - off[q] within its query) goes to lims[q] + rank when the rank is below the query's
+// kept count, decoded to a score and an index
+__global__ void __launch_bounds__(256)
+knn_range_decode_kernel(const unsigned long long* __restrict__ keys, const int* __restrict__ rows, int64_t nnz, int Q,
+                        const long long* __restrict__ off, const long long* __restrict__ lims,
+                        float* __restrict__ out_scores, int64_t* __restrict__ out_idx) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz; i += (int64_t)gridDim.x * blockDim.x) {
+    const int q = rows[i];
+    if (q < 0 || q >= Q) continue;
+    const long long r = i - off[q];
+    if (r < 0 || r >= lims[q + 1] - lims[q]) continue;
+    knn_decode_key(keys[i], out_scores + lims[q] + r, out_idx + lims[q] + r);
+  }
 }
 
 // ---- inverted-file search (esmb200_ivf_search): the grouping of (query, probe) pairs into list-scan work items --------

@@ -31,6 +31,7 @@ import bisect
 import ctypes
 import json
 import math
+import numbers
 import os
 import pathlib
 from concurrent.futures import ThreadPoolExecutor
@@ -267,6 +268,308 @@ class EmbeddingIndex:
             scores[b0:b1] = s
             idx[b0:b1] = i
         return scores, idx
+
+    # ---- range search ------------------------------------------------------------------------------------------------
+    def range_search(self, queries: torch.Tensor, *, min_score: Optional[float] = None,
+                     max_distance: Optional[float] = None, max_hits: Optional[int] = None
+                     ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every row within a threshold of each query (fp32/fp16 [Q, E] or [E], any device): cosine rows with
+        similarity >= min_score, or l2 rows at distance <= max_distance (the threshold must match the metric). Returns
+        CSR on the index's device: lims int64 [Q + 1], scores fp32 [nnz] and idx int64 [nnz]; query i's hits are
+        scores[lims[i]:lims[i + 1]], ordered as search() orders them (its first k are search(k)'s, bit for bit).
+        max_hits keeps each query's first max_hits hits. A query with more hits than the hit buffer holds
+        (RANGE_HIT_BYTES / 12) is refused."""
+        check_range_args(self.metric, min_score, max_distance, max_hits)
+        if isinstance(queries, torch.Tensor) and queries.dim() == 1:
+            queries = queries[None]
+        if isinstance(queries, torch.Tensor) and queries.dim() == 2 and queries.shape[1] != self.dim:
+            raise ValueError(f"queries have width {queries.shape[1]}, the index {self.dim}")
+        q = prepare_rows(queries, self.metric, "queries")
+        self._check_device()
+        return self._range_rows(q.to(self.device), False, min_score, max_distance, max_hits)
+
+    def range_search_all(self, *, min_score: Optional[float] = None, max_distance: Optional[float] = None,
+                         max_hits: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every row against the index with its own row left out: (lims, scores, idx) as range_search()."""
+        check_range_args(self.metric, min_score, max_distance, max_hits)
+        self._check_device()
+        return self._range_rows(self.rows, True, min_score, max_distance, max_hits)
+
+    def _range_rows(self, q: torch.Tensor, self_rows: bool, min_score, max_distance, max_hits):
+        Q, N, l2 = q.shape[0], len(self), self.metric == "l2"
+        alpha = 2.0 if l2 else 1.0
+        qn = squared_norms(q) if l2 else None
+        tau = range_thresholds(self.metric, qn, Q, min_score, max_distance, self.device)
+        parts = []
+        for b0 in range(0, Q, QUERY_BATCH):
+            b1 = min(Q, b0 + QUERY_BATCH)
+
+            def run(c0, c1, cap_rows):  # queries [b0 + c0, b0 + c1) into a hit buffer of cap_rows hits
+                hits = _HitBuffer(c1 - c0, cap_rows, self.device)
+                knn_range(q[b0 + c0:b0 + c1], self.rows, 0, tau[b0 + c0:b0 + c1], *hits.tensors(), self._beta,
+                          alpha, b0 + c0 if self_rows else -1)
+                return hits
+
+            for hits, c0, c1 in _range_passes(run, b1 - b0, min(range_hit_cap(), (b1 - b0) * N),
+                                              _threshold_text(min_score, max_distance), b0):
+                parts.append(_range_part(hits, max_hits, qn[b0 + c0:b0 + c1] if l2 else None))
+        return _concat_csr(parts, self.device)
+
+
+# ---- range search -----------------------------------------------------------------------------------------------------
+RANGE_HIT_BYTES = 1 << 30  # device bytes of one range search's hit buffer (HIT_BYTES a hit): batches are sized to it
+HIT_BYTES = 12             # a uint64 key and an int32 query row
+
+
+def range_hit_cap() -> int:
+    """Hits one hit buffer holds."""
+    return RANGE_HIT_BYTES // HIT_BYTES
+
+
+def check_range_args(metric: str, min_score, max_distance, max_hits) -> None:
+    """ValueError unless exactly the metric's threshold is given (cosine: min_score, l2: max_distance >= 0), it is not
+    NaN, and max_hits is None or an int >= 1."""
+    if (min_score is None) == (max_distance is None):
+        raise ValueError("pass exactly one threshold: min_score (cosine index) or max_distance (l2 index)")
+    name, v = ("min_score", min_score) if min_score is not None else ("max_distance", max_distance)
+    want = "min_score" if metric == "cosine" else "max_distance"
+    if name != want:
+        raise ValueError(f"a {metric} index takes {want}, not {name}")
+    if isinstance(v, bool) or not isinstance(v, numbers.Real):
+        raise ValueError(f"{name} must be a real number, got {v!r}")
+    if math.isnan(float(v)):
+        raise ValueError(f"{name} must not be NaN")
+    if name == "max_distance" and float(v) < 0:
+        raise ValueError(f"max_distance must be >= 0, got {v!r}")
+    if max_hits is not None and (isinstance(max_hits, bool) or not isinstance(max_hits, int) or max_hits < 1):
+        raise ValueError(f"max_hits must be None or an int >= 1, got {max_hits!r}")
+
+
+def _threshold_text(min_score, max_distance) -> str:
+    return f"min_score {min_score!r}" if min_score is not None else f"max_distance {max_distance!r}"
+
+
+def fp32_at_or_above(x: float) -> float:
+    """The smallest fp32 >= x (a real number): s >= x exactly when s >= it, for every fp32 s."""
+    with np.errstate(over="ignore"):
+        f = np.float32(x)
+        if float(f) < x:
+            f = np.nextafter(f, np.float32(np.inf))
+    return float(f)
+
+
+def fp32_at_or_below(x: float) -> float:
+    """The largest fp32 <= x: d <= x exactly when d <= it, for every fp32 d."""
+    with np.errstate(over="ignore"):
+        f = np.float32(x)
+        if float(f) > x:
+            f = np.nextafter(f, np.float32(-np.inf))
+    return float(f)
+
+
+_ORD_NEG_INF = -0x7F800000 - 1  # ordinal of -inf: fp32 bits b >= 0 map to b, negative ones to -(b & 0x7FFFFFFF) - 1
+_ORD_POS_INF = 0x7F800000
+
+
+def _f32_of_ordinal(o: torch.Tensor) -> torch.Tensor:
+    bits = torch.where(o >= 0, o, (-(o + 1)) - (1 << 31))  # int32 value of 0x80000000 | m is m - 2^31
+    return bits.to(torch.int32).view(torch.float32)
+
+
+def l2_distance(qn: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """The reported l2 distance of kernel scores s: sqrt(max(|q|^2 - s, 0)) in fp32, as search() computes it."""
+    return (qn - s).clamp_min(0).sqrt()
+
+
+def l2_thresholds(qn: torch.Tensor, max_distance: float) -> torch.Tensor:
+    """tau fp32 [Q]: per query (|q|^2 fp32 [Q]), the smallest fp32 s with l2_distance(|q|^2, s) <= max_distance.
+    The distance is a chain of correctly rounded monotone operations, so it does not increase with s and the hits
+    are exactly the candidates with s >= tau. Found by bisection over the ordered fp32 bit patterns, with the same
+    operations on qn's device: 33 halvings cover [-inf, +inf], and +inf always qualifies (distance 0)."""
+    r = fp32_at_or_below(float(max_distance))
+    lo = torch.full(qn.shape, _ORD_NEG_INF, dtype=torch.int64, device=qn.device)
+    hi = torch.full(qn.shape, _ORD_POS_INF, dtype=torch.int64, device=qn.device)
+    for _ in range(33):
+        mid = torch.div(lo + hi, 2, rounding_mode="floor")
+        ok = l2_distance(qn, _f32_of_ordinal(mid)) <= r
+        hi = torch.where(ok, mid, hi)
+        lo = torch.where(ok, lo, mid + 1)
+    return _f32_of_ordinal(hi) + 0.0  # -0 as +0, as the scores are
+
+
+def range_thresholds(metric: str, qn: Optional[torch.Tensor], Q: int, min_score, max_distance,
+                     device) -> torch.Tensor:
+    """Each query's tau fp32 [Q] on device: its hits are the candidates with kernel score s >= tau."""
+    if metric == "cosine":
+        return torch.full((Q,), fp32_at_or_above(float(min_score)) + 0.0, dtype=torch.float32, device=device)
+    return l2_thresholds(qn.to(device), max_distance)
+
+
+def knn_range(queries: torch.Tensor, base: torch.Tensor, row0: int, tau: torch.Tensor, hit_keys: torch.Tensor,
+              hit_rows: torch.Tensor, counts: torch.Tensor, total: torch.Tensor, beta: Optional[torch.Tensor] = None,
+              alpha: float = 1.0, self_offset: int = -1, splits: Optional[int] = None) -> None:
+    """esmb200_knn_range: append the hits of chunk base fp16 [n, D] (global rows row0 ..) for queries fp16 [Q, D]
+    with thresholds tau fp32 [Q] to hit_keys int64 [cap] (uint64 keys) and hit_rows int32 [cap], adding to counts
+    int64 [Q] and total int64 [1] (zeros before the first chunk), which count past cap."""
+    for name, t in (("queries", queries), ("base", base)):
+        if t.dtype != torch.float16 or t.dim() != 2 or not t.is_cuda or t.stride(1) != 1:
+            raise ValueError(f"{name} must be a CUDA fp16 tensor [n, D] with contiguous rows")
+    Q, n = queries.shape[0], base.shape[0]
+    dev = base.device
+    if queries.device != dev or queries.shape[1] != base.shape[1]:
+        raise ValueError("queries and base must be on one device with one width")
+    cap = hit_keys.numel() if isinstance(hit_keys, torch.Tensor) else -1
+    want = [("tau", tau, torch.float32, (Q,)), ("hit_keys", hit_keys, torch.int64, (cap,)),
+            ("hit_rows", hit_rows, torch.int32, (cap,)), ("counts", counts, torch.int64, (Q,)),
+            ("total", total, torch.int64, (1,))]
+    if beta is not None:
+        want.append(("beta", beta, torch.float32, (n,)))
+    for name, t, dtype, shape in want:
+        if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.is_contiguous() and tuple(t.shape) == shape
+                and t.device == dev):
+            raise ValueError(f"{name} must be a contiguous {dtype} tensor {list(shape)} on the base's device")
+    with torch.cuda.device(dev):
+        if splits is None:
+            splits = choose_splits(Q, n, torch.cuda.get_device_properties(dev).multi_processor_count)
+        _lib.check(_lib.load().esmb200_knn_range(
+            _ptr(queries), queries.stride(0), Q, _ptr(base), base.stride(0), n, row0, base.shape[1], _ptr(beta),
+            float(alpha), self_offset, _ptr(tau), splits, _ptr(hit_keys) if cap else None,
+            _ptr(hit_rows) if cap else None, cap, _ptr(counts), _ptr(total), _stream()))
+
+
+_SIGN = -(1 << 63)
+
+
+def knn_range_finish(hit_keys: torch.Tensor, hit_rows: torch.Tensor, counts: torch.Tensor,
+                     max_hits: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """esmb200_knn_range_finish on the nnz = sum(counts) appended hits (hit_keys int64 [nnz], hit_rows int32 [nnz],
+    counts int64 [Q], one CUDA device, in any order): (lims int64 [Q + 1], scores fp32, idx int64), each query's hits
+    by key descending (score descending, index ascending), the first max_hits of each kept. The hits are sorted here
+    with two stable torch sorts (keys are uint64: flipping the sign bit makes torch's signed order theirs)."""
+    if not (isinstance(counts, torch.Tensor) and counts.dtype == torch.int64 and counts.dim() == 1
+            and counts.is_contiguous() and counts.is_cuda):
+        raise ValueError("counts must be a contiguous CUDA int64 tensor [Q]")
+    dev, Q = counts.device, counts.numel()
+    nnz = hit_keys.numel() if isinstance(hit_keys, torch.Tensor) else -1
+    for name, t, dtype in (("hit_keys", hit_keys, torch.int64), ("hit_rows", hit_rows, torch.int32)):
+        if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.dim() == 1 and t.numel() == nnz
+                and t.device == dev):
+            raise ValueError(f"{name} must be a {dtype} tensor [nnz] on the counts' device")
+    if max_hits is not None and (isinstance(max_hits, bool) or not isinstance(max_hits, int) or max_hits < 1):
+        raise ValueError(f"max_hits must be None or an int >= 1, got {max_hits!r}")
+    order = torch.sort(hit_keys ^ _SIGN, descending=True, stable=True).indices
+    order = order[torch.sort(hit_rows[order], stable=True).indices]
+    keys, rows = hit_keys[order].contiguous(), hit_rows[order].contiguous()
+    kept = counts if max_hits is None else counts.clamp(max=max_hits)
+    n_out = int(kept.sum()) if Q else 0
+    lims = torch.empty(Q + 1, dtype=torch.int64, device=dev)
+    scores = torch.empty(n_out, dtype=torch.float32, device=dev)
+    idx = torch.empty(n_out, dtype=torch.int64, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        nbytes = ctypes.c_size_t(0)
+        _lib.check(lib.esmb200_knn_range_finish_scratch_bytes(Q, ctypes.byref(nbytes)))
+        scratch = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        _lib.check(lib.esmb200_knn_range_finish(_ptr(keys), _ptr(rows), nnz, _ptr(counts), Q,
+                                                -1 if max_hits is None else max_hits, _ptr(scratch), nbytes.value,
+                                                _ptr(lims), _ptr(scores), _ptr(idx), _stream()))
+    return lims, scores, idx
+
+
+class _HitBuffer:
+    """A range search pass's buffers: hit keys and rows [cap], counts [Q] and the total, counters zeroed."""
+
+    def __init__(self, Q: int, cap: int, dev: torch.device):
+        self.keys = torch.empty(cap, dtype=torch.int64, device=dev)
+        self.rows = torch.empty(cap, dtype=torch.int32, device=dev)
+        self.counts = torch.zeros(Q, dtype=torch.int64, device=dev)
+        self.total = torch.zeros(1, dtype=torch.int64, device=dev)
+
+    def tensors(self):
+        return self.keys, self.rows, self.counts, self.total
+
+
+def plan_range_reruns(counts: Sequence[int], cap: int, threshold: str, q_base: int = 0) -> List[Tuple[int, int]]:
+    """After a pass overflowed a hit buffer of cap hits: consecutive query groups [c0, c1) whose exact counts sum to at
+    most cap, each re-run with a buffer of exactly that many. ValueError naming the threshold and the count for a query
+    whose hits alone exceed cap (q_base: the first query's number in the call)."""
+    groups, c0, acc = [], 0, 0
+    for i, c in enumerate(counts):
+        if c > cap:
+            raise ValueError(f"query {q_base + i} has {c} hits at {threshold}, more than the {cap} one hit buffer holds "
+                             f"(search.RANGE_HIT_BYTES): use a tighter threshold")
+        if acc + c > cap:
+            groups.append((c0, i))
+            c0, acc = i, 0
+        acc += c
+    if c0 < len(counts):
+        groups.append((c0, len(counts)))
+    return groups
+
+
+def _range_passes(run, n: int, cap: int, threshold: str, q_base: int):
+    """(hits, c0, c1) covering queries [0, n): one pass run(0, n, cap) into a buffer of cap hits, whose total is read
+    once; after an overflow, the groups plan_range_reruns makes from its exact counts, each re-run into a buffer of
+    exactly its hits."""
+    hits = run(0, n, cap)
+    total = int(hits.total.item())
+    if total <= cap:
+        yield hits, 0, n
+        return
+    counts = hits.counts.tolist()
+    del hits
+    for c0, c1 in plan_range_reruns(counts, cap, threshold, q_base):
+        want = sum(counts[c0:c1])
+        hits = run(c0, c1, want)
+        if int(hits.total.item()) != want:
+            raise RuntimeError(f"a range search re-run found {int(hits.total.item())} hits, its first pass {want}")
+        yield hits, c0, c1
+
+
+def _range_part(hits: _HitBuffer, max_hits, qn: Optional[torch.Tensor]):
+    """The CSR of one pass; l2 scores become distances (l2_distance of each hit's query norm)."""
+    nnz = min(int(hits.total.item()), hits.keys.numel())
+    lims, s, i = knn_range_finish(hits.keys[:nnz], hits.rows[:nnz], hits.counts, max_hits)
+    if qn is not None:
+        s = l2_distance(qn.repeat_interleave(lims.diff(), output_size=s.numel()), s)
+    return lims, s, i
+
+
+def _concat_csr(parts, dev):
+    lims, scores, idx, off = [torch.zeros(1, dtype=torch.int64, device=dev)], [], [], 0
+    for l, s, i in parts:
+        lims.append(l[1:] + off)
+        scores.append(s)
+        idx.append(i)
+        off += s.numel()
+    if not parts:
+        return lims[0], torch.empty(0, dtype=torch.float32, device=dev), torch.empty(0, dtype=torch.int64, device=dev)
+    return torch.cat(lims), torch.cat(scores), torch.cat(idx)
+
+
+def plan_range_stream(N: int, Q: int, D: int, metric: str, cap: int) -> Tuple[int, int, int]:
+    """(query block, chunk rows, hit buffer) of a streamed range search within cap device bytes: the hit buffer takes
+    at most a quarter of cap (and RANGE_HIT_BYTES), the query block all Q rows if they fit beside a ring of one-tile
+    slots, else the largest multiple of 64 within half of cap, and the ring's chunks the rest (whole tiles, at most
+    MAX_SLOT_BYTES a slot). The results, whose size is the hit count, are not part of cap. ValueError when no block of
+    64 queries or no one-tile chunk fits."""
+    hit_cap = min(RANGE_HIT_BYTES, cap // 4) // HIT_BYTES
+    if hit_cap < 1:
+        raise ValueError(f"max_device_bytes = {cap} holds no hit buffer: pass more bytes")
+    per_query = D * 2 + 4 + 8 + (4 if metric == "l2" else 0)  # rows, tau, counts, |q|^2
+    fixed = lambda b: b * per_query + hit_cap * HIT_BYTES + 16 * 512  # noqa: E731  (512: the allocator's rounding)
+    ring_tile = RING_SLOTS * TILE * _row_bytes(D, metric)
+    block = Q
+    if fixed(Q) + ring_tile > cap:
+        block = max(0, cap // 2 - fixed(0)) // per_query // 64 * 64
+        if block < 64:
+            raise ValueError(f"max_device_bytes = {cap} holds no block of 64 query rows beside the hit buffer: "
+                             f"pass more bytes")
+    tiles = (cap - fixed(block)) // ring_tile
+    if tiles < 1:
+        raise ValueError(f"max_device_bytes = {cap} leaves no room for a {TILE}-row chunk: pass more bytes")
+    chunk = int(min(tiles, max(1, MAX_SLOT_BYTES // (TILE * _row_bytes(D, metric))))) * TILE
+    return max(block, 1), min(chunk, -(-N // TILE) * TILE), hit_cap
 
 
 # ---- sharded indexes on disk ------------------------------------------------------------------------------------------
@@ -707,6 +1010,17 @@ class ShardedIndex:
                              f"{N} queries: pass more bytes")
         return 64 * lo
 
+    def _block_queries(self, pool, q, qn, a0: int, a1: int, dev: torch.device):
+        """The query rows [a0, a1) on the device and, for l2, their |x|^2: q's, or the database's own rows (q None,
+        read from the maps; |x|^2 read as -|x|^2 and negated exactly)."""
+        l2 = self.metric == "l2"
+        if q is not None:
+            return q[a0:a1].to(dev), (qn[a0:a1].to(dev) if l2 else None)
+        buf = torch.empty((a1 - a0, self.padded_dim), dtype=torch.float16)
+        nbuf = torch.empty(a1 - a0, dtype=torch.float32) if l2 else None
+        self._read_parallel(pool, a0, a1, buf.numpy(), nbuf.numpy() if l2 else None)
+        return buf.to(dev), ((-nbuf).to(dev) if l2 else None)
+
     def _stream(self, q: Optional[torch.Tensor], qn: Optional[torch.Tensor], k: int, dev: torch.device,
                 max_device_bytes: Optional[int]):
         N, D, l2 = len(self), self.padded_dim, self.metric == "l2"
@@ -725,53 +1039,22 @@ class ShardedIndex:
             if Q == 0:
                 return scores, idx
             scratch = torch.empty(scratch_bytes(block, Q, k, num_sms), dtype=torch.uint8, device=dev)
-            dev_rows = [torch.empty((chunk, D), dtype=torch.float16, device=dev) for _ in range(RING_SLOTS)]
-            dev_beta = [torch.empty(chunk, dtype=torch.float32, device=dev) for _ in range(RING_SLOTS)] if l2 else None
-            host = _host_ring(chunk, D, l2, dev)
-            compute, copy = torch.cuda.current_stream(dev), torch.cuda.Stream(device=dev)
-            copied = [torch.cuda.Event() for _ in range(RING_SLOTS)]
-            consumed = [torch.cuda.Event() for _ in range(RING_SLOTS)]
-            bounds = [(g, min(N, g + chunk)) for g in range(0, N, chunk)]
+            ring = _ChunkRing(self, chunk, dev)
             try:
                 with ThreadPoolExecutor(REFILL_THREADS) as pool:
                     for a0 in range(0, Q, block):
                         a1 = min(Q, a0 + block)
-                        if self_rows:  # the block's rows and, for l2, |x|^2 (read as -|x|^2, negated exactly)
-                            buf = torch.empty((a1 - a0, D), dtype=torch.float16)
-                            nbuf = torch.empty(a1 - a0, dtype=torch.float32) if l2 else None
-                            self._read_parallel(pool, a0, a1, buf.numpy(), nbuf.numpy() if l2 else None)
-                            qrows, qnorm = buf.to(dev), ((-nbuf).to(dev) if l2 else None)
-                        else:
-                            qrows, qnorm = q.to(dev), (qn.to(dev) if l2 else None)
+                        qrows, qnorm = self._block_queries(pool, q, qn, a0, a1, dev)
                         keys = torch.zeros((a1 - a0, k), dtype=torch.int64, device=dev)
 
-                        def fill(c):  # host slot c % RING_SLOTS <- chunk c, once the slot's last copy has finished
-                            s, (g0, g1) = c % RING_SLOTS, bounds[c]
-                            copied[s].synchronize()
-                            self._read_parallel(pool, g0, g1, host.rows[s].numpy(),
-                                                host.beta[s].numpy() if l2 else None)
-                            with torch.cuda.stream(copy):  # device slot s is free once chunk c - RING_SLOTS is done
-                                copy.wait_event(consumed[s])
-                                n = g1 - g0
-                                dev_rows[s][:n].copy_(host.rows[s][:n], non_blocking=True)
-                                if l2:
-                                    dev_beta[s][:n].copy_(host.beta[s][:n], non_blocking=True)
-                                copied[s].record(copy)
-
-                        fill(0)
-                        for c, (g0, g1) in enumerate(bounds):
-                            s = c % RING_SLOTS
-                            compute.wait_event(copied[s])
+                        def consume(rows, beta, g0, g1):
                             for b0 in range(0, a1 - a0, QUERY_BATCH):
                                 b1 = min(a1 - a0, b0 + QUERY_BATCH)
                                 splits = choose_splits(b1 - b0, g1 - g0, num_sms)
-                                knn_accumulate(qrows[b0:b1], dev_rows[s][:g1 - g0], g0, k, keys[b0:b1], scratch,
-                                               dev_beta[s][:g1 - g0] if l2 else None, alpha,
-                                               a0 + b0 if self_rows else -1,
-                                               splits)
-                            consumed[s].record(compute)
-                            if c + 1 < len(bounds):
-                                fill(c + 1)  # the host refills the next slot while the GPU works on this one
+                                knn_accumulate(qrows[b0:b1], rows, g0, k, keys[b0:b1], scratch, beta, alpha,
+                                               a0 + b0 if self_rows else -1, splits)
+
+                        ring.run(pool, consume)
                         knn_decode(keys, scores[a0:a1], idx[a0:a1])
                         if l2:
                             sc = scores[a0:a1]
@@ -779,9 +1062,116 @@ class ShardedIndex:
                             sc.clamp_min_(0).sqrt_()
                         del keys, qrows
             finally:  # the host ring is reused by the next call: nothing may still read it
-                compute.synchronize()
-                copy.synchronize()
+                ring.synchronize()
         return scores, idx
+
+    # ---- range search ------------------------------------------------------------------------------------------------
+    def range_search(self, queries: torch.Tensor, *, min_score: Optional[float] = None,
+                     max_distance: Optional[float] = None, max_hits: Optional[int] = None, device=None,
+                     max_device_bytes: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every row within the threshold of each query, as EmbeddingIndex.range_search returns them (lims, scores,
+        idx on `device`, default the current CUDA device), streamed through the GPU as search() streams it."""
+        check_range_args(self.metric, min_score, max_distance, max_hits)
+        if isinstance(queries, torch.Tensor) and queries.dim() == 1:
+            queries = queries[None]
+        if isinstance(queries, torch.Tensor) and queries.dim() == 2 and queries.shape[1] != self.dim:
+            raise ValueError(f"queries have width {queries.shape[1]}, the index {self.dim}")
+        q = prepare_rows(queries, self.metric, "queries")
+        dev = _cuda_device(device)
+        qn = squared_norms(q) if self.metric == "l2" else None
+        return self._range_stream(q, qn, min_score, max_distance, max_hits, dev, max_device_bytes)
+
+    def range_search_all(self, *, min_score: Optional[float] = None, max_distance: Optional[float] = None,
+                         max_hits: Optional[int] = None, device=None,
+                         max_device_bytes: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every row against the index with its own row left out: (lims, scores, idx) as range_search()."""
+        check_range_args(self.metric, min_score, max_distance, max_hits)
+        dev = _cuda_device(device)
+        return self._range_stream(None, None, min_score, max_distance, max_hits, dev, max_device_bytes)
+
+    def _range_stream(self, q, qn, min_score, max_distance, max_hits, dev, max_device_bytes):
+        N, D, l2 = len(self), self.padded_dim, self.metric == "l2"
+        self_rows = q is None
+        Q = N if self_rows else q.shape[0]
+        alpha = 2.0 if l2 else 1.0
+        with torch.cuda.device(dev):
+            num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            cap = int(DEVICE_SHARE * torch.cuda.mem_get_info(dev)[0]) if max_device_bytes is None \
+                else int(max_device_bytes)
+            block, chunk, hit_cap = plan_range_stream(N, Q, D, self.metric, cap)
+            parts = []
+            ring = _ChunkRing(self, chunk, dev)
+            try:
+                with ThreadPoolExecutor(REFILL_THREADS) as pool:
+                    for a0 in range(0, Q, block):
+                        a1 = min(Q, a0 + block)
+                        qrows, qnorm = self._block_queries(pool, q, qn, a0, a1, dev)
+                        tau = range_thresholds(self.metric, qnorm, a1 - a0, min_score, max_distance, dev)
+
+                        def run(c0, c1, cap_rows):  # query rows [c0, c1) of the block: one pass over the database
+                            hits = _HitBuffer(c1 - c0, cap_rows, dev)
+
+                            def consume(rows, beta, g0, g1):
+                                knn_range(qrows[c0:c1], rows, g0, tau[c0:c1], *hits.tensors(), beta, alpha,
+                                          a0 + c0 if self_rows else -1, choose_splits(c1 - c0, g1 - g0, num_sms))
+
+                            ring.run(pool, consume)
+                            return hits
+
+                        for hits, c0, c1 in _range_passes(run, a1 - a0, min(hit_cap, (a1 - a0) * N),
+                                                          _threshold_text(min_score, max_distance), a0):
+                            parts.append(_range_part(hits, max_hits, qnorm[c0:c1] if l2 else None))
+                        del qrows
+            finally:
+                ring.synchronize()
+        return _concat_csr(parts, dev)
+
+
+class _ChunkRing:
+    """One streamed call's ring: RING_SLOTS device slots of `chunk` rows (and l2 betas), the page-locked host ring,
+    a copy stream and the events that order them. run() passes the whole database through it once."""
+
+    def __init__(self, index: "ShardedIndex", chunk: int, dev: torch.device):
+        self.index, self.l2 = index, index.metric == "l2"
+        N, D = len(index), index.padded_dim
+        self.rows = [torch.empty((chunk, D), dtype=torch.float16, device=dev) for _ in range(RING_SLOTS)]
+        self.beta = [torch.empty(chunk, dtype=torch.float32, device=dev) for _ in range(RING_SLOTS)] if self.l2 \
+            else None
+        self.host = _host_ring(chunk, D, self.l2, dev)
+        self.compute, self.copy = torch.cuda.current_stream(dev), torch.cuda.Stream(device=dev)
+        self.copied = [torch.cuda.Event() for _ in range(RING_SLOTS)]
+        self.consumed = [torch.cuda.Event() for _ in range(RING_SLOTS)]
+        self.bounds = [(g, min(N, g + chunk)) for g in range(0, N, chunk)]
+
+    def _fill(self, pool, c: int) -> None:
+        """host slot c % RING_SLOTS <- chunk c, once the slot's last copy has finished"""
+        s, (g0, g1) = c % RING_SLOTS, self.bounds[c]
+        host = self.host
+        self.copied[s].synchronize()
+        self.index._read_parallel(pool, g0, g1, host.rows[s].numpy(), host.beta[s].numpy() if self.l2 else None)
+        with torch.cuda.stream(self.copy):  # device slot s is free once chunk c - RING_SLOTS is done
+            self.copy.wait_event(self.consumed[s])
+            n = g1 - g0
+            self.rows[s][:n].copy_(host.rows[s][:n], non_blocking=True)
+            if self.l2:
+                self.beta[s][:n].copy_(host.beta[s][:n], non_blocking=True)
+            self.copied[s].record(self.copy)
+
+    def run(self, pool, consume) -> None:
+        """consume(rows fp16 [n, D], beta fp32 [n] or None, g0, g1) enqueues the work on chunk [g0, g1) on the
+        compute stream; chunks come in order."""
+        self._fill(pool, 0)
+        for c, (g0, g1) in enumerate(self.bounds):
+            s = c % RING_SLOTS
+            self.compute.wait_event(self.copied[s])
+            consume(self.rows[s][:g1 - g0], self.beta[s][:g1 - g0] if self.l2 else None, g0, g1)
+            self.consumed[s].record(self.compute)
+            if c + 1 < len(self.bounds):
+                self._fill(pool, c + 1)  # the host refills the next slot while the GPU works on this one
+
+    def synchronize(self) -> None:
+        self.compute.synchronize()
+        self.copy.synchronize()
 
 
 # ---- inverted-file index ----------------------------------------------------------------------------------------------

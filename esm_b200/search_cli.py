@@ -6,6 +6,8 @@
                                         [--train-rows N] [--iters 20] [--seed 0]
     python -m esm_b200.search_cli query db.pt|db/|ivf.pt (--queries EXTRACT_DIR | --all) --k 10 [--nprobe P]
                                         --out hits.tsv
+    python -m esm_b200.search_cli range db.pt|db/ (--queries EXTRACT_DIR | --all)
+                                        (--min-score S | --max-distance R) [--max-hits M] --out hits.tsv
 
 `build` reads the mean representation at --layer of every `<label>.pt` under EXTRACT_DIR (extract_cli --include mean)
 and saves an index: one file (EmbeddingIndex) when --out ends in .pt, else a sharded index directory (IndexWriter),
@@ -22,6 +24,11 @@ cannot go to a directory or be appended to. `query` reads the index type from th
 min(8, nlist); nlist scans every list and gives the exact hits) sets how many lists each query scans. An IVF query
 can find fewer than k hits when its lists hold fewer rows; hits.tsv then has fewer lines for it. --nprobe on an exact
 or sharded index is refused.
+
+`range` finds every indexed protein within a threshold instead of the top k: --min-score for a cosine index (every
+hit with similarity >= S), --max-distance for an l2 index (distance <= R); --max-hits keeps each query's best M. It
+writes the same hits.tsv as `query`, ranks in the same order, so align_cli reads it unchanged. A threshold flag that
+does not match the index's metric, NaN, or an IVF index (its range over the probed lists is not defined) is refused.
 """
 from __future__ import annotations
 
@@ -57,12 +64,29 @@ def create_parser():
     q.add_argument("--k", type=int, default=10, help=f"hits per query, 1 to {search.MAX_K}")
     q.add_argument("--nprobe", type=int, help="lists scanned per query (IVF index only)")
     q.add_argument("--out", type=pathlib.Path, required=True)
+    r = sub.add_parser("range", help="every indexed protein within a threshold of each query")
+    r.add_argument("index", type=pathlib.Path)
+    src = r.add_mutually_exclusive_group(required=True)
+    src.add_argument("--queries", type=pathlib.Path, help="an extract_cli output directory of query proteins")
+    src.add_argument("--all", action="store_true", help="every indexed protein against the others")
+    thr = r.add_mutually_exclusive_group(required=True)
+    thr.add_argument("--min-score", type=float, help="cosine index: hits with similarity >= this")
+    thr.add_argument("--max-distance", type=float, help="l2 index: hits at Euclidean distance <= this")
+    r.add_argument("--max-hits", type=int, help="keep each query's best M hits")
+    r.add_argument("--out", type=pathlib.Path, required=True)
     return p
 
 
-def write_hits(path, query_labels, target_labels, scores: torch.Tensor, idx: torch.Tensor) -> int:
-    """hits.tsv; returns the number of hit lines."""
-    scores, idx = scores.cpu().tolist(), idx.cpu().tolist()
+def csr_rows(lims: torch.Tensor, values: torch.Tensor) -> list:
+    """A CSR array (lims [Q + 1]) as one Python list per query."""
+    lims, values = lims.cpu().tolist(), values.cpu().tolist()
+    return [values[lims[i]:lims[i + 1]] for i in range(len(lims) - 1)]
+
+
+def write_hits(path, query_labels, target_labels, scores, idx) -> int:
+    """hits.tsv from [Q, k] tensors or per-query lists; returns the number of hit lines."""
+    if isinstance(scores, torch.Tensor):
+        scores, idx = scores.cpu().tolist(), idx.cpu().tolist()
     n = 0
     with open(path, "w") as f:
         f.write("query\trank\ttarget\tscore\n")
@@ -126,6 +150,8 @@ def run(args) -> int:
         args.out.parent.mkdir(parents=True, exist_ok=True)
         index.save(args.out)
         return len(index)
+    if args.command == "range":
+        return run_range(args)
     sharded = args.index.is_dir()
     if sharded and args.nprobe is not None:
         raise ValueError("--nprobe applies to an IVF index; a directory index is searched exactly")
@@ -137,21 +163,42 @@ def run(args) -> int:
         index.check_nprobe(args.nprobe)
     candidates = len(index) - 1 if args.all else len(index)
     search._check_k(args.k, candidates)
-    if args.all:
-        qlabels, queries = index.labels, None
-    else:
-        if index.layer is None:
-            raise ValueError(f"{args.index} records no layer: query it through esm_b200.search")
-        qlabels, queries = search._read_extract_dir(args.queries, index.layer)
-        if queries.shape[1] != index.dim:
-            raise ValueError(f"the queries have width {queries.shape[1]}, the index {index.dim}")
-        search.prepare_rows(queries, index.metric, "queries")
+    qlabels, queries = _queries(args, index)
     if not sharded:
         index = index.to(torch.device("cuda", torch.cuda.current_device()))
     extra = {"nprobe": args.nprobe} if ivf else {}
     scores, idx = index.search_all(args.k, **extra) if args.all else index.search(queries, args.k, **extra)
     args.out.parent.mkdir(parents=True, exist_ok=True)
     return write_hits(args.out, qlabels, index.labels, scores, idx)
+
+
+def _queries(args, index):
+    """(query labels, fp32 queries or None for --all) of a query or range command, checked against the index."""
+    if args.all:
+        return index.labels, None
+    if index.layer is None:
+        raise ValueError(f"{args.index} records no layer: query it through esm_b200.search")
+    qlabels, queries = search._read_extract_dir(args.queries, index.layer)
+    if queries.shape[1] != index.dim:
+        raise ValueError(f"the queries have width {queries.shape[1]}, the index {index.dim}")
+    search.prepare_rows(queries, index.metric, "queries")
+    return qlabels, queries
+
+
+def run_range(args) -> int:
+    sharded = args.index.is_dir()
+    index = search.ShardedIndex.open(args.index) if sharded else search.load_file_index(args.index, device="cpu")
+    if isinstance(index, search.IVFIndex):
+        raise ValueError(f"{args.index} is an IVF index: a range search over its probed lists is not defined; "
+                         f"range-search the exact index it was built from")
+    thr = {"min_score": args.min_score, "max_distance": args.max_distance, "max_hits": args.max_hits}
+    search.check_range_args(index.metric, **thr)
+    qlabels, queries = _queries(args, index)
+    if not sharded:
+        index = index.to(torch.device("cuda", torch.cuda.current_device()))
+    lims, scores, idx = index.range_search_all(**thr) if args.all else index.range_search(queries, **thr)
+    args.out.parent.mkdir(parents=True, exist_ok=True)
+    return write_hits(args.out, qlabels, index.labels, csr_rows(lims, scores), csr_rows(lims, idx))
 
 
 def main():

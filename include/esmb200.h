@@ -364,6 +364,42 @@ int esmb200_knn_search_accumulate(const void* queries, int64_t q_ld, int32_t Q, 
                                   uint64_t* keys, void* stream);
 int esmb200_knn_decode(const uint64_t* keys, int32_t Q, int32_t k, float* out_scores, int64_t* out_idx, void* stream);
 
+/* Range search over embeddings (esm_b200/search.py EmbeddingIndex.range_search, ShardedIndex.range_search): every
+ * candidate at or above a threshold instead of the top k. The score s(i, j) and the candidates are
+ * esmb200_knn_search_accumulate's (global index j = row0 + the chunk row, query i leaves out global row i + self_offset
+ * when self_offset >= 0, -0 taken as +0). Candidate j is a hit of query i iff s(i, j) >= tau[i] (tau fp32 [Q], device,
+ * never NaN; -0 is taken as +0; -inf makes every candidate a hit). A cosine search passes the smallest fp32 at or
+ * above its min_score; an l2 search passes, per query, the smallest fp32 s whose distance sqrt(max(|q|^2 - s, 0))
+ * (fp32, correctly rounded) is at most max_distance: the distance does not increase with s, so that is the hit set.
+ * esmb200_knn_range: appends the chunk's hits, unordered, to hit_keys uint64 [hit_cap] (the ranking keys
+ *   (ord(s) << 32) | (2^32 - 1 - j)) and hit_rows int32 [hit_cap] (the query row), at positions taken from *hit_total
+ *   (uint64, device), and adds each query's hits to hit_counts uint64 [Q] (device). Both counters count every hit,
+ *   but a hit is written only below hit_cap, so after an overflow they give each query's exact count and the exact
+ *   total (set them to 0 before the first chunk; hit_cap 0 with NULL buffers only counts). Chunks are appended one
+ *   after another into the same buffers, in any order. One launch: knn_topk_kernel in range mode (fixed thresholds,
+ *   a full queue flushed with one global atomicAdd per row), 12 bytes of buffer per hit. No scratch. Q >= 0, n >= 1,
+ *   row0 >= 0 and row0 + n < 2^31, D, q_ld, b_ld, splits and the query and base alignments as for
+ *   esmb200_knn_search, 0 <= hit_cap < 2^31, non-NULL tau, hit_counts and hit_total (hit_keys and hit_rows too when
+ *   hit_cap > 0), 4-byte aligned beta, tau and hit_rows and 8-byte aligned hit_keys, hit_counts and hit_total, else
+ *   ESMB200_EINVAL before any launch. Q == 0 launches nothing.
+ * esmb200_knn_range_finish: the hits of one range search to CSR. keys and rows hold all nnz = sum(counts) hits, sorted
+ *   by query row ascending and, within a query, by key descending (a stable sort by key descending, then a stable sort
+ *   by row, leaves them so; keys are distinct within a query, so any correct sort gives the same bits). Writes lims
+ *   int64 [Q + 1] (lims[q + 1] - lims[q] = min(counts[q], max_hits), max_hits = -1 for no cap), and each query's
+ *   first hits, decoded, to scores fp32 [lims[Q]] and idx int64 [lims[Q]]. scratch:
+ *   esmb200_knn_range_finish_scratch_bytes(Q) bytes, 8-byte aligned. Q >= 0, 0 <= nnz < 2^31, max_hits >= 1 or -1,
+ *   non-NULL counts, scratch and lims (keys, rows, scores and idx too when nnz > 0), the alignments of their types
+ *   and enough scratch, else ESMB200_EINVAL before any launch. Two launches (one when nnz == 0).
+ * esmb200_knn_range_finish_scratch_bytes writes (Q + 1) * 8 to *out; it refuses Q < 0 and a NULL out. */
+int esmb200_knn_range(const void* queries, int64_t q_ld, int32_t Q, const void* base, int64_t b_ld, int64_t n,
+                      int64_t row0, int32_t D, const float* beta, float alpha, int64_t self_offset, const float* tau,
+                      int32_t splits, uint64_t* hit_keys, int32_t* hit_rows, int64_t hit_cap, uint64_t* hit_counts,
+                      uint64_t* hit_total, void* stream);
+int esmb200_knn_range_finish_scratch_bytes(int32_t Q, size_t* out);
+int esmb200_knn_range_finish(const uint64_t* keys, const int32_t* rows, int64_t nnz, const uint64_t* counts, int32_t Q,
+                             int64_t max_hits, void* scratch, size_t scratch_bytes, int64_t* lims, float* scores,
+                             int64_t* idx, void* stream);
+
 /* Inverted-file (IVF) search (esm_b200/search.py IVFIndex). The stored rows fp16 [N, b_ld] (device, 16-byte aligned) are
  * grouped into nlist lists: list l is rows [offsets[l], offsets[l+1]) (offsets int64 [nlist + 1], 0 = offsets[0] <=
  * ... <= offsets[nlist] = N), and ids int64 [N] holds each stored row's original index (distinct, in [0, 2^31)). beta
